@@ -52,7 +52,8 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_test_attention", "gam_launch_count", "gam_profile_begin", "gam_profile_end", "gam_profile_class_count",
            "gam_profile_class_name", "gam_logmel_workspace_bytes", "gam_logmel_tc", "gam_test_attention_relpos",
            "gam_decode_workspace_bytes", "gam_group_words", "gam_comm_unique_id", "gam_comm_init",
-           "gam_comm_nccl_version", "gam_gather_hyps", "gam_test_attention_varlen")
+           "gam_comm_nccl_version", "gam_gather_hyps", "gam_test_attention_varlen", "gam_ctc_log_probs",
+           "gam_rnnt_joint_workspace_bytes", "gam_rnnt_joint", "gam_rnnt_predict")
 
 
 def lib_path() -> Path:
@@ -104,6 +105,14 @@ def load() -> C.CDLL:
     for fn in (lib.gam_ctc_greedy, lib.gam_rnnt_greedy):
         fn.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, i64, c_vp, c_vp, c_vp, i32, c_vp]
         fn.restype = C.c_int
+    lib.gam_ctc_log_probs.argtypes = [H, c_vp, i32, i32, c_vp, c_vp]
+    lib.gam_ctc_log_probs.restype = C.c_int
+    lib.gam_rnnt_joint_workspace_bytes.argtypes = [H, i32, i32, i32]
+    lib.gam_rnnt_joint_workspace_bytes.restype = i64
+    lib.gam_rnnt_joint.argtypes = [H, c_vp, c_vp, i32, i32, i32, c_vp, i64, c_vp, c_vp]
+    lib.gam_rnnt_joint.restype = C.c_int
+    lib.gam_rnnt_predict.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, c_vp, c_vp, c_vp, c_vp]
+    lib.gam_rnnt_predict.restype = C.c_int
     lib.gam_test_gemm.argtypes = [H, i32, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, C.c_float, c_vp]
     lib.gam_test_gemm.restype = C.c_int
     lib.gam_test_attention.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, c_vp]

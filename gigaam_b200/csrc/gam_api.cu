@@ -132,7 +132,7 @@ struct gam_handle {
 enum ProfClass : int {
   PC_LOGMEL = 0, PC_SUB_CONV1, PC_GEMM_CONV2, PC_GEMM_SUBOUT, PC_GEMM_FFN_UP, PC_GEMM_FFN_DOWN, PC_GEMM_QKV, PC_GEMM_PROJ,
   PC_GEMM_GLU, PC_LAYERNORM, PC_ATTENTION, PC_DWCONV, PC_CTC_ARGMAX, PC_CTC_COLLAPSE, PC_RNNT_ENCPROJ, PC_RNNT_GREEDY,
-  PC_MISC, PC_COUNT
+  PC_MISC, PC_CTC_LOG_PROBS, PC_RNNT_JOINT, PC_RNNT_PREDICT, PC_COUNT
 };
 
 struct ProfScope {
@@ -629,6 +629,78 @@ int gam_rnnt_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int
   return 0;
 }
 
+int gam_ctc_log_probs(gam_handle* h, const float* enc, int32_t B, int32_t T, float* log_probs, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 1) return fail(h, -1, "ctc_log_probs: model has no CTC head");
+  if (B <= 0 || T <= 0) return fail(h, -1, "ctc_log_probs: bad sizes (B=%d, T=%d)", B, T);
+  const int64_t R = static_cast<int64_t>(B) * T;
+  if (R > INT32_MAX) return fail(h, -1, "ctc_log_probs: B*T = %lld exceeds 2^31 - 1 frames", (long long)R);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  { PROF(PC_CTC_LOG_PROBS);
+    launch_ctc_log_probs(enc, h->w.ctc_w, h->w.ctc_b, log_probs, static_cast<int>(R), c.d_model, c.num_classes, s); }
+  GAM_CHECK_LAUNCH(h, "ctc_log_probs");
+  return 0;
+}
+
+int64_t gam_rnnt_joint_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || U <= 0) return -1;
+  const int64_t J = h->cfg.joint_hidden;
+  return align_up(static_cast<int64_t>(B) * T * J * 4, 1024) + align_up(static_cast<int64_t>(B) * U * J * 4, 1024) + 1024;
+}
+
+int gam_rnnt_joint(gam_handle* h, const float* enc, const float* dec, int32_t B, int32_t T, int32_t U, void* workspace,
+                   int64_t workspace_bytes, float* out, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 2) return fail(h, -1, "rnnt_joint: model has no RNN-T head");
+  if (B <= 0 || T <= 0 || U <= 0) return fail(h, -1, "rnnt_joint: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
+  constexpr int64_t kMaxProjRows = 65535LL * 64;   // grid.y limit of the projection GEMMs (64 rows per block)
+  if (static_cast<int64_t>(B) * T > kMaxProjRows || static_cast<int64_t>(B) * U > kMaxProjRows)
+    return fail(h, -1, "rnnt_joint: B*T and B*U must be <= %lld (B=%d, T=%d, U=%d)", (long long)kMaxProjRows, B, T, U);
+  const int J = c.joint_hidden;
+  if (J % 4 != 0 || J > rnnt_joint_max_hidden() || c.pred_hidden % 16 != 0 || c.d_model % 16 != 0)
+    return fail(h, -1, "rnnt_joint: needs joint_hidden %% 4 == 0 and <= %d, pred_hidden %% 16 == 0 (joint_hidden %d, pred_hidden %d)",
+                rnnt_joint_max_hidden(), J, c.pred_hidden);
+  const int64_t need = gam_rnnt_joint_workspace_bytes(h, B, T, U);
+  if (workspace_bytes < need)
+    return fail(h, -1, "rnnt_joint: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  uint8_t* ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
+  float* E = reinterpret_cast<float*>(ws);
+  float* P = reinterpret_cast<float*>(ws + align_up(static_cast<int64_t>(B) * T * J * 4, 1024));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc = 0;
+  { PROF(PC_RNNT_JOINT);
+    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, E, B * T, J, c.d_model, s); }
+  { PROF(PC_RNNT_JOINT);
+    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, P, B * U, J, c.pred_hidden, s); }
+  { PROF(PC_RNNT_JOINT);
+    rc = launch_rnnt_joint(E, P, h->w.rnnt_wo, h->w.rnnt_bo, out, B, T, U, J, c.num_classes, s); }
+  if (rc != 0) return fail(h, -4, "rnnt_joint: lattice launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, "rnnt_joint");
+  return 0;
+}
+
+int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g, float* h1,
+                     float* c1, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 2) return fail(h, -1, "rnnt_predict: model has no RNN-T head");
+  if (B <= 0 || U <= 0) return fail(h, -1, "rnnt_predict: bad sizes (B=%d, U=%d)", B, U);
+  if (x == nullptr && U != 1) return fail(h, -1, "rnnt_predict: without labels the step count U must be 1 (got %d)", U);
+  if (c.pred_hidden > 1024) return fail(h, -1, "rnnt_predict: pred_hidden %d exceeds 1024", c.pred_hidden);
+  const int H = c.pred_hidden;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  for (int u = 0; u < U; ++u) {
+    // step u reads h from g[:, u-1] (steps are separate launches, so every block of step u sees all of step u-1) and
+    // updates c1 in place
+    const float* h_in = u == 0 ? h0 : g + static_cast<int64_t>(u - 1) * H;
+    const int64_t pitch = u == 0 ? H : static_cast<int64_t>(U) * H;
+    PROF(PC_RNNT_PREDICT);
+    launch_lstm_step(x, U, u, c.num_classes, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h_in, pitch, u == 0 ? c0 : c1, g,
+                     u == U - 1 ? h1 : nullptr, c1, B, H, s);
+  }
+  GAM_CHECK_LAUNCH(h, "rnnt_predict");
+  return 0;
+}
+
 int gam_group_words(gam_handle* h, const int32_t* ids, const int32_t* frames, const int32_t* counts, int32_t B, int32_t max_out,
                     const uint8_t* token_flags, int32_t V, int32_t max_words, int32_t* word_start, int32_t* word_end,
                     int32_t* word_first_token, int32_t* word_tokens, int32_t* n_words, void* stream) {
@@ -698,7 +770,8 @@ int gam_profile_class_count(void) { return PC_COUNT; }
 const char* gam_profile_class_name(int32_t cls) {
   static const char* names[PC_COUNT] = {"logmel", "subsample_conv1", "gemm_conv2_implicit", "gemm_subsample_out", "gemm_ffn_up_silu",
                                         "gemm_ffn_down_res", "gemm_qkv", "gemm_proj_res", "gemm_pw1_glu", "layernorm", "attention",
-                                        "dwconv_bn_silu", "ctc_head_argmax", "ctc_collapse", "rnnt_enc_proj", "rnnt_greedy", "misc"};
+                                        "dwconv_bn_silu", "ctc_head_argmax", "ctc_collapse", "rnnt_enc_proj", "rnnt_greedy", "misc",
+                                        "ctc_log_probs", "rnnt_joint", "rnnt_predict"};
   return (cls >= 0 && cls < PC_COUNT) ? names[cls] : "?";
 }
 

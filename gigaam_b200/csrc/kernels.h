@@ -62,7 +62,22 @@ void launch_group_words(const int* ids, const int* frames, const int* counts, co
                         int max_words, int* w_start, int* w_end, int* w_first, int* w_ntok, int* n_words, cudaStream_t s);
 
 // rnnt.cu
+// C[M,N] = A[M,K] W[N,K]^T + bias (bias may be null); K % 16 == 0
 void launch_sgemm_tn_bias(const float* A, const float* W, const float* bias, float* C, int M, int N, int K, cudaStream_t s);
+// the same with W given transposed: Wt[K,N] row-major, N % 4 == 0
+void launch_sgemm_nn_bias(const float* A, const float* Wt, const float* bias, float* C, int M, int N, int K, cudaStream_t s);
+
+// heads.cu: the heads' forward passes (fp32).  ctc: enc [R, D] -> log_probs [R, V1]
+void launch_ctc_log_probs(const float* enc, const float* W, const float* bias, float* out, int R, int D, int V1, cudaStream_t s);
+// E [B*T, J], P [B*U, J] -> out [B, T, U, V1] = log_softmax(Wo relu(E[b,t] + P[b,u]) + bo); 64-bit offsets.
+// Returns 0 ok, 1 = unsupported J (J % 4 != 0 or J > rnnt_joint_max_hidden()) or grid, <0 = attribute error
+constexpr size_t kJointMaxSmem = 200 * 1024;
+int rnnt_joint_max_hidden();
+int launch_rnnt_joint(const float* E, const float* P, const float* Wo, const float* bo, float* out, int B, int T, int U, int J,
+                      int V1, cudaStream_t s);
+// one step u of the 1-layer prediction LSTM (heads.cu: lstm_step_kernel documents the operands); H <= 1024
+void launch_lstm_step(const int64_t* x, int U, int u, int V1, const float* emb_gates, const float* whh_t, const float* h_in,
+                      int64_t h_pitch, const float* c_in, float* g, float* h_out, float* c_out, int B, int H, cudaStream_t s);
 
 // rnnt_cluster.cu: returns 0 ok, 1 = 16-CTA clusters unavailable / unsupported shape, <0 error
 int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float* emb_gates, const float* whhT, const float* wpT,

@@ -1,18 +1,29 @@
-"""CTC / RNN-T heads with the reference's interface and state_dict keys (gigaam/decoder.py).  The heads are
-parameter holders: their arithmetic (fp32, as in the reference, gigaam/__init__.py:188-189) runs inside the
-greedy-decode kernels (`gam_ctc_greedy`, `gam_rnnt_greedy`)."""
+"""CTC / RNN-T heads with the reference's interface and state_dict keys (gigaam/decoder.py).  The greedy decoders use
+the heads' parameters inside their own fused kernels (`gam_ctc_greedy`, `gam_rnnt_greedy`); the heads' public
+methods -- `CTCHead.forward`, `RNNTDecoder.predict` / `forward`, `RNNTJoint.joint` / `forward` -- run the head
+kernels of csrc/heads.cu (`gam_ctc_log_probs`, `gam_rnnt_predict`, `gam_rnnt_joint`) for callers that do their own
+search.  All head arithmetic is fp32, as in the reference (gigaam/__init__.py:188-189)."""
 from __future__ import annotations
 
-from typing import Dict
+from typing import Dict, Optional, Tuple
 
 import torch
+from torch import Tensor
 
 from . import synthetic
 from ._params import Bound, build_tree
+from .decoding import _as_btd
 
 
 def _zeros(entries):
     return [(k, torch.zeros(shape, dtype=torch.float32)) for k, shape, kind, _ in entries]
+
+
+def _on_device(t: Tensor, eng, dtype: torch.dtype) -> Tensor:
+    if not t.is_cuda:
+        raise RuntimeError("gigaam_b200 has no CPU path: pass CUDA tensors to the head (the model runs on "
+                           f"{eng.device})")
+    return t.to(device=eng.device, dtype=dtype)
 
 
 class CTCHead(Bound):
@@ -23,13 +34,76 @@ class CTCHead(Bound):
         self.feat_in, self.num_classes = feat_in, num_classes
         build_tree(self, _zeros(synthetic.head_param_list(dict(type="ctc", feat_in=feat_in, num_classes=num_classes))), "head.")
 
+    def forward(self, encoder_output: Tensor) -> Tensor:
+        """[B, feat_in, T] -> log-probs [B, T, num_classes] (gigaam/decoder.py:18-21).  The encoder's output is a
+        transposed view of a [B, T, d] buffer, which the kernel reads as it is."""
+        eng = self._engine()
+        return eng.ctc_log_probs(_as_btd(_on_device(encoder_output, eng, torch.float32)))
+
+
+class RNNTJoint(Bound):
+    """gigaam/decoder.py:24-69 -- `enc` / `pred` / `joint_net.1` parameters; the lattice runs in `gam_rnnt_joint`."""
+
+    def __init__(self, enc_hidden: int, pred_hidden: int, joint_hidden: int, num_classes: int):
+        super().__init__()
+        self.enc_hidden = enc_hidden
+        self.pred_hidden = pred_hidden
+
+    def joint(self, encoder_out: Tensor, decoder_out: Tensor) -> Tensor:
+        """[B, T, enc_hidden], [B, U, pred_hidden] -> log-probs [B, T, U, num_classes] (gigaam/decoder.py:41-47)"""
+        eng = self._engine()
+        enc = _on_device(encoder_out, eng, torch.float32).contiguous()
+        dec = _on_device(decoder_out, eng, torch.float32).contiguous()
+        return eng.rnnt_joint(enc, dec)
+
+    def forward(self, enc: Tensor, dec: Tensor) -> Tensor:
+        """[B, enc_hidden, T], [B, pred_hidden, U] -> [B, T, U, num_classes] (gigaam/decoder.py:68-69)"""
+        return self.joint(enc.transpose(1, 2), dec.transpose(1, 2))
+
+
+class RNNTDecoder(Bound):
+    """gigaam/decoder.py:72-137 -- `embed` + 1-layer `lstm` parameters; the steps run in `gam_rnnt_predict`."""
+
+    def __init__(self, pred_hidden: int, pred_rnn_layers: int, num_classes: int):
+        super().__init__()
+        self.blank_id = num_classes - 1
+        self.pred_hidden = pred_hidden
+
+    def predict(self, x: Optional[Tensor], state: Optional[Tuple[Tensor, Tensor]], batch_size: int = 1
+                ) -> Tuple[Tensor, Tuple[Tensor, Tensor]]:
+        """x [B, U] label ids or None (one step from the zero embedding, `batch_size` rows); state (h, c), each
+        [1, B, pred_hidden] (strided views are fine), or None (zeros) -> (g [B, U, pred_hidden], (h, c) [1, B, pred_hidden])
+        (gigaam/decoder.py:85-102).  A row with an id outside [0, num_classes) comes back as NaN."""
+        eng = self._engine()
+        if x is not None:
+            x = _on_device(x, eng, torch.int64).contiguous()
+        h = c = None
+        if state is not None:
+            h, c = (_on_device(s, eng, torch.float32) for s in state)
+            if h.dim() != 3 or h.shape[0] != 1 or c.shape != h.shape:
+                raise ValueError(f"predict: state must be two [1, B, {self.pred_hidden}] tensors (one LSTM layer), got "
+                                 f"{tuple(h.shape)} and {tuple(c.shape)}")
+            h, c = h[0].contiguous(), c[0].contiguous()
+        g, h1, c1 = eng.rnnt_predict(x, h, c, batch_size)
+        return g, (h1.unsqueeze(0), c1.unsqueeze(0))
+
+    def forward(self, x: Tensor, h: Tensor, c: Tensor) -> Tuple[Tensor, Tensor, Tensor]:
+        """ONNX form of predict: (x, h, c) -> (g, h, c) (gigaam/decoder.py:131-137)"""
+        g, (h, c) = self.predict(x, (h, c))
+        return g, h, c
+
 
 class RNNTHead(Bound):
-    """gigaam/decoder.py:140-149 -- `decoder` (Embedding + LSTM) and `joint` (enc / pred / joint_net) holders."""
+    """gigaam/decoder.py:140-149 -- `decoder` (RNNTDecoder) and `joint` (RNNTJoint)."""
 
     def __init__(self, decoder: Dict[str, int], joint: Dict[str, int]):
         super().__init__()
         self.decoder_cfg, self.joint_cfg = dict(decoder), dict(joint)
+        self.decoder = RNNTDecoder(**self.decoder_cfg)
+        self.joint = RNNTJoint(**self.joint_cfg)
         build_tree(self, _zeros(synthetic.head_param_list(dict(type="rnnt", decoder=self.decoder_cfg, joint=self.joint_cfg))), "head.")
-        self.decoder.blank_id = decoder["num_classes"] - 1
-        self.decoder.pred_hidden = decoder["pred_hidden"]
+
+    def _bind(self, owner) -> None:
+        super()._bind(owner)
+        self.decoder._bind(owner)
+        self.joint._bind(owner)

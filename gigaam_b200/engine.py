@@ -160,6 +160,7 @@ class Engine:
         self._ws_enc = _WorkspaceCache(self.WS_CACHE)
         self._ws_mel = _WorkspaceCache(self.WS_CACHE)
         self._ws_dec = _WorkspaceCache(self.WS_CACHE)
+        self._ws_joint = _WorkspaceCache(self.WS_CACHE)
         self.handle = C.c_void_p()
         pre, enc = cfg["preprocessor"], cfg["encoder"]
         head = cfg.get("head") if isinstance(cfg, dict) else None
@@ -360,6 +361,7 @@ class Engine:
         if dc["pred_rnn_layers"] != 1:
             raise NotImplementedError("multi-layer prediction LSTM")
         self.head_type, self.num_classes = 2, jt["num_classes"]
+        self.pred_hidden = dc["pred_hidden"]
         gc.pred_hidden, gc.joint_hidden = dc["pred_hidden"], jt["joint_hidden"]
         emb = sd["head.decoder.embed.weight"].double().clone()
         # predict(None, None) starts from an all-zero embedding (gigaam/decoder.py:92-95) and nn.Embedding's padding_idx
@@ -466,6 +468,69 @@ class Engine:
                     frames.data_ptr(), counts.data_ptr(), max_out, self._stream())
         _lib.check(self.lib, self.handle, rc, "gam_greedy")
         return ids, frames, counts
+
+    def ctc_log_probs(self, enc_btd: Tensor) -> Tensor:
+        """enc [B, T, d] f32 contiguous -> log_probs [B, T, V+1] f32 (CTCHead.forward, gigaam/decoder.py:18-21)."""
+        assert enc_btd.is_cuda and enc_btd.dtype == torch.float32 and enc_btd.is_contiguous() and enc_btd.dim() == 3
+        if self.head_type != 1:
+            raise RuntimeError("model has no CTC head")
+        B, T, _ = enc_btd.shape
+        out = torch.empty((B, T, self.num_classes), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_ctc_log_probs(self.handle, enc_btd.data_ptr(), B, T, out.data_ptr(), self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_ctc_log_probs")
+        return out
+
+    def rnnt_joint(self, enc: Tensor, dec: Tensor) -> Tensor:
+        """enc [B, T, d], dec [B, U, pred_hidden] f32 contiguous -> [B, T, U, V+1] log-probs (RNNTJoint.joint,
+        gigaam/decoder.py:41-47).  The projection workspace is cached per (B, T, U) like the decode workspace."""
+        assert enc.is_cuda and dec.is_cuda and enc.dtype == dec.dtype == torch.float32
+        assert enc.is_contiguous() and dec.is_contiguous() and enc.dim() == dec.dim() == 3
+        if self.head_type != 2:
+            raise RuntimeError("model has no RNN-T head")
+        B, T, _ = enc.shape
+        U = dec.shape[1]
+        if dec.shape[0] != B:
+            raise ValueError(f"joint: encoder batch {B} != decoder batch {dec.shape[0]}")
+        out = torch.empty((B, T, U, self.num_classes), dtype=torch.float32, device=self.device)
+        nbytes = int(self.lib.gam_rnnt_joint_workspace_bytes(self.handle, B, T, U))
+        if nbytes < 0:
+            raise ValueError(f"joint: bad sizes B={B}, T={T}, U={U}")
+        ws = self._ws_joint.get((B, T, U), nbytes, self.device)
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_rnnt_joint(self.handle, enc.data_ptr(), dec.data_ptr(), B, T, U, ws.data_ptr(), ws.numel(),
+                                         out.data_ptr(), self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_rnnt_joint")
+        return out
+
+    def rnnt_predict(self, x: Optional[Tensor], h: Optional[Tensor], c: Optional[Tensor], batch_size: int = 1
+                     ) -> Tuple[Tensor, Tensor, Tensor]:
+        """x [B, U] i64 or None (one step from the zero embedding), h / c [B, H] f32 contiguous or None (zeros)
+        -> (g [B, U, H], h1 [B, H], c1 [B, H]) (RNNTDecoder.predict, gigaam/decoder.py:85-102)."""
+        if self.head_type != 2:
+            raise RuntimeError("model has no RNN-T head")
+        H = self.pred_hidden
+        if x is not None:
+            assert x.is_cuda and x.dtype == torch.int64 and x.is_contiguous() and x.dim() == 2
+            B, U = x.shape
+        else:
+            B, U = int(batch_size), 1
+        for name, t in (("h", h), ("c", c)):
+            if t is not None:
+                assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
+                if tuple(t.shape) != (B, H):
+                    raise ValueError(f"predict: state {name} has shape {tuple(t.shape)}, expected ({B}, {H})")
+        g = torch.empty((B, U, H), dtype=torch.float32, device=self.device)
+        h1 = torch.empty((B, H), dtype=torch.float32, device=self.device)
+        c1 = torch.empty((B, H), dtype=torch.float32, device=self.device)
+
+        def ptr(t):
+            return None if t is None else t.data_ptr()
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_rnnt_predict(self.handle, ptr(x), ptr(h), ptr(c), B, U, g.data_ptr(), h1.data_ptr(), c1.data_ptr(),
+                                           self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_rnnt_predict")
+        return g, h1, c1
 
     def group_words(self, ids: Tensor, frames: Tensor, counts: Tensor, token_flags: Tensor):
         """Device word grouping (gam_group_words): -> (word_start, word_end, word_first, word_ntok [B, max_out] i32, n_words [B] i32)."""

@@ -187,6 +187,12 @@ class GigaAMASR(GigaAM):
             out.append((tok.decode(row), words))
         return out
 
+    def forward_for_export(self, features: Tensor, feature_lengths: Tensor) -> Tuple[Tensor, Tensor]:
+        """log-mel [B, F, M], lengths [B] -> (head(encoded), encoded_len) (gigaam/model.py:142-149): CTC log-probs
+        [B, T', V+1].  An RNN-T head has no forward, so this raises for RNN-T models, as in the reference."""
+        encoded, encoded_len = self.encoder(features, feature_lengths)
+        return self.head(encoded), encoded_len
+
     @torch.inference_mode()
     def transcribe(self, wav_file, word_timestamps: bool = False) -> TranscriptionResult:
         """gigaam/model.py:126-140"""

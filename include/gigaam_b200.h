@@ -10,6 +10,9 @@
  *   gam_encode        <- gigaam/encoder.py:605-647    ConformerEncoder.forward (subsampling + N layers)
  *   gam_ctc_greedy    <- gigaam/decoder.py:18-21 + gigaam/decoding.py:56-96  CTCHead + CTCGreedyDecoding
  *   gam_rnnt_greedy   <- gigaam/decoder.py:41-47,85-102 + gigaam/decoding.py:128-207
+ *   gam_ctc_log_probs <- gigaam/decoder.py:18-21      CTCHead.forward
+ *   gam_rnnt_joint    <- gigaam/decoder.py:41-47      RNNTJoint.joint
+ *   gam_rnnt_predict  <- gigaam/decoder.py:85-102     RNNTDecoder.predict (1-layer LSTM)
  *
  * Conventions: every pointer marked "device" is a CUDA device pointer on the handle's device; the
  * library never allocates or frees caller memory in the hot calls (the caller passes a workspace of
@@ -169,6 +172,32 @@ int gam_ctc_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int3
 int gam_rnnt_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
                     int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
                     void* stream);
+
+/* ---- the heads' forward passes, for callers that run their own search (LM beam search, N-best rescoring, forced
+ * alignment, lattice scoring).  fp32 CUDA-core arithmetic like the reference's heads; no workspace except for the joint.
+ *
+ * CTC posteriors: enc: device f32 [B, T, d_model] (gam_encode's layout)
+ *   -> log_probs: device f32 [B, T, V+1] = log_softmax(W enc + b) over the last axis.  Every frame is computed; frames at or
+ *   past enc_len hold zeros in gam_encode's output and so give log_softmax(b). */
+int gam_ctc_log_probs(gam_handle* h, const float* enc, int32_t B, int32_t T, float* log_probs, void* stream);
+
+/* RNN-T joint lattice: enc: device f32 [B, T, d_model]; dec: device f32 [B, U, pred_hidden] (prediction-network outputs)
+ *   -> out: device f32 [B, T, U, V+1] = log_softmax(W_o relu(W_e enc[b,t] + b_e + W_p dec[b,u] + b_p) + b_o).
+ * workspace: device scratch of at least gam_rnnt_joint_workspace_bytes(B, T, U) bytes (the two projections); the
+ * [B, T, U, joint_hidden] hidden tensor is never stored.  Offsets are 64-bit: out may exceed 2^31 elements.
+ * gam_rnnt_joint_workspace_bytes returns -1 for a handle without an RNN-T head or non-positive sizes. */
+int64_t gam_rnnt_joint_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_rnnt_joint(gam_handle* h, const float* enc, const float* dec, int32_t B, int32_t T, int32_t U, void* workspace,
+                   int64_t workspace_bytes, float* out, void* stream);
+
+/* RNN-T prediction network, U sequential LSTM steps (gate order i, f, g, o):
+ *   x: device i64 [B, U] label ids, or NULL = one step (U must be 1) from the all-zero embedding;
+ *   h0, c0: device f32 [B, pred_hidden] each, or NULL = zeros;
+ *   -> g: device f32 [B, U, pred_hidden] (hidden state after every step), h1, c1: device f32 [B, pred_hidden] (final state).
+ * An utterance with an id outside [0, V] gets NaN in all of its g, h1 and c1; the others are unaffected and the call
+ * succeeds.  One launch per step. */
+int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g, float* h1,
+                     float* c1, void* stream);
 
 /* ---- the one multi-GPU exchange of the path (SURVEY 8e): utterances are sharded over ranks, one process per GPU, and the
  * device-resident hypotheses are all-gathered ONCE over NCCL (NVLink / NVSwitch) when the batch was actually split.
