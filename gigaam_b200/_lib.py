@@ -53,7 +53,9 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_profile_class_name", "gam_logmel_workspace_bytes", "gam_logmel_tc", "gam_test_attention_relpos",
            "gam_decode_workspace_bytes", "gam_group_words", "gam_comm_unique_id", "gam_comm_init",
            "gam_comm_nccl_version", "gam_gather_hyps", "gam_test_attention_varlen", "gam_ctc_log_probs",
-           "gam_rnnt_joint_workspace_bytes", "gam_rnnt_joint", "gam_rnnt_predict")
+           "gam_rnnt_joint_workspace_bytes", "gam_rnnt_joint", "gam_rnnt_predict", "gam_test_gemm_conv",
+           "gam_test_layernorm", "gam_test_ln_rope", "gam_test_ln_out_ln", "gam_test_unpack_rows", "gam_test_dwconv",
+           "gam_test_pack_plan", "gam_test_subsample_conv1", "gam_test_mel_to_tmajor")
 
 
 def lib_path() -> Path:
@@ -113,8 +115,22 @@ def load() -> C.CDLL:
     lib.gam_rnnt_joint.restype = C.c_int
     lib.gam_rnnt_predict.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, c_vp, c_vp, c_vp, c_vp]
     lib.gam_rnnt_predict.restype = C.c_int
-    lib.gam_test_gemm.argtypes = [H, i32, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, C.c_float, c_vp]
-    lib.gam_test_gemm.restype = C.c_int
+    lib.gam_test_gemm.argtypes = [H, i32, c_vp, c_vp, i32, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, i32, C.c_float, i32, c_vp,
+                                  c_vp]
+    lib.gam_test_gemm_conv.argtypes = [H, i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, i32, i32, i32, i32, c_vp]
+    lib.gam_test_layernorm.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, c_vp, i32, c_vp]
+    lib.gam_test_ln_rope.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, c_vp, c_vp, i32, i32, c_vp]
+    lib.gam_test_ln_out_ln.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, c_vp, i32, c_vp]
+    lib.gam_test_unpack_rows.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, c_vp]
+    lib.gam_test_dwconv.argtypes = [H, i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32,
+                                    c_vp]
+    lib.gam_test_pack_plan.argtypes = [H, c_vp, i32, i32, i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    lib.gam_test_subsample_conv1.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i64, i32, c_vp]
+    lib.gam_test_mel_to_tmajor.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, i64, c_vp]
+    for fn in (lib.gam_test_gemm, lib.gam_test_gemm_conv, lib.gam_test_layernorm, lib.gam_test_ln_rope, lib.gam_test_ln_out_ln,
+               lib.gam_test_unpack_rows, lib.gam_test_dwconv, lib.gam_test_pack_plan, lib.gam_test_subsample_conv1,
+               lib.gam_test_mel_to_tmajor):
+        fn.restype = C.c_int
     lib.gam_test_attention.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, c_vp]
     lib.gam_test_attention.restype = C.c_int
     lib.gam_test_attention_relpos.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, i32, c_vp]

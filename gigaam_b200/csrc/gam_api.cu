@@ -1,6 +1,7 @@
 // C-ABI + host engine of libgigaam_b200.so: weight/plan bookkeeping, TMA descriptor construction,
 // and the kernel sequence of the path.  No compute lives here and nothing here falls back to a CPU
 // or library implementation: every stage is one of the hand-written kernels in this directory.
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -268,7 +269,19 @@ Plan* get_plan(gam_handle* h, int B, int64_t M, void* ws, int64_t ws_bytes) {
   return p;
 }
 
-#define GAM_CHECK_LAUNCH(h, what)                                                             \
+// gam_test_gemm's kind for the DFT power epilogue (launch_gemm_power); kinds 0-4 are GemmKind
+constexpr int kTestGemmPower = 7;
+
+// Unit-test entry points only: copies n device ints to the host (synchronising the stream) so that a hook can refuse row
+// maps that would send its kernel outside the caller's buffers.  Returns 0 on success.
+int dev_ints(const int32_t* p, int n, std::vector<int>& v, cudaStream_t s) {
+  v.assign(n > 0 ? n : 0, 0);
+  if (n <= 0) return 0;
+  if (cudaMemcpyAsync(v.data(), p, static_cast<size_t>(n) * sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess) return -1;
+  return cudaStreamSynchronize(s) == cudaSuccess ? 0 : -1;
+}
+
+#define GAM_CHECK_LAUNCH(h, what)                                                           \
   do {                                                                                        \
     cudaError_t e__ = cudaGetLastError(); /* reads AND clears: one failed launch must not poison later calls */ \
     if (e__ != cudaSuccess) return fail(h, -3, "%s: %s", what, cudaGetErrorString(e__));      \
@@ -775,19 +788,233 @@ const char* gam_profile_class_name(int32_t cls) {
   return (cls >= 0 && cls < PC_COUNT) ? names[cls] : "?";
 }
 
-int gam_test_gemm(gam_handle* h, int32_t kind, const void* A, const void* W, const float* bias, const float* res, void* out,
-                  int32_t M, int32_t N, int32_t K, int32_t ldo, float scale, void* stream) {
-  CUtensorMap ta, tw;
+int gam_test_gemm(gam_handle* h, int32_t kind, const void* A, const void* A2, int32_t n1, const void* W, const float* bias,
+                  const float* res, void* out, int32_t M, int32_t N, int32_t K, int32_t ldo, int32_t col0, float scale,
+                  int32_t reverse, const int32_t* m_dev, void* stream) {
+  if (kind < GEMM_BIAS_F16 || (kind > GEMM_BIAS_F32 && kind != kTestGemmPower))
+    return fail(h, -1, "test_gemm: unknown kind %d", kind);
+  if (!A || !W || !out || (kind != kTestGemmPower && !bias) || (kind == GEMM_BIAS_RES_F32 && !res))
+    return fail(h, -1, "test_gemm: A, W, out, bias (and res for kind 3) are required");
+  if (M <= 0 || N <= 0 || N % 256 != 0 || K <= 0 || K % 64 != 0) return fail(h, -1, "test_gemm: bad sizes M=%d N=%d K=%d", M, N, K);
+  // GLU and power write one column per pair of accumulator columns; f32 epilogues store float2, f16 ones half2
+  const int ncol = (kind == GEMM_BIAS_GLU_F16 || kind == kTestGemmPower) ? N / 2 : N;
+  if (col0 < 0 || col0 % 2 != 0 || ldo % 2 != 0 || ldo < col0 + ncol)
+    return fail(h, -1, "test_gemm: columns [%d, %d) do not fit an even row pitch %d", col0, col0 + ncol, ldo);
+  if (A2 && (kind != GEMM_BIAS_F16 || n1 <= 0 || n1 >= N || n1 % 256 != 0))
+    return fail(h, -1, "test_gemm: a second A operand needs kind 0 and 0 < n1 < N, n1 %% 256 == 0 (n1=%d)", n1);
+  CUtensorMap ta, ta2, tw;
   int rc = make_tmap_2d_f16(&ta, A, M, K, K, 128, 64);
+  if (A2) rc |= make_tmap_2d_f16(&ta2, A2, M, K, K, 128, 64);
   rc |= make_tmap_2d_f16(&tw, W, N, K, K, 128, 64);
   if (rc) return fail(h, -2, "tensor map encode failed (rc=%d)", rc);
+  const size_t esz = (kind == GEMM_BIAS_RES_F32 || kind == GEMM_BIAS_F32 || kind == kTestGemmPower) ? 4 : 2;
+  void* o = static_cast<char*>(out) + col0 * esz;
+  const float* r = res ? reinterpret_cast<const float*>(reinterpret_cast<const char*>(res) + col0 * esz) : nullptr;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   {
     PROF(PC_MISC);
-    rc = launch_gemm(kind, &ta, &tw, M, N, K, bias, res, out, ldo, scale, h->num_sms, s);
+    if (kind == kTestGemmPower)
+      rc = launch_gemm_power(&ta, &tw, M, N, K, static_cast<float*>(o), ldo, h->num_sms, s);
+    else if (A2)
+      rc = launch_gemm_dual_a(&ta, &ta2, n1, &tw, M, N, K, bias, o, ldo, h->num_sms, s, reverse, m_dev);
+    else
+      rc = launch_gemm(kind, &ta, &tw, M, N, K, bias, r, o, ldo, scale, h->num_sms, s, reverse, m_dev);
   }
   if (rc) return fail(h, -4, "gemm launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "test_gemm");
+  return 0;
+}
+
+int gam_test_gemm_conv(gam_handle* h, int32_t conv1d, const void* A, const void* W, const float* bias, const int32_t* len_out,
+                       const int32_t* cu, const int32_t* plen, void* out, int32_t out_frames, int32_t B, int32_t T_in, int32_t F1,
+                       int32_t C, int32_t taps, int32_t N, int32_t f32_out, void* stream) {
+  if (!A || !W || !bias || !len_out || !out) return fail(h, -1, "test_gemm_conv: A, W, bias, len_out and out are required");
+  if ((cu != nullptr) != (plen != nullptr)) return fail(h, -1, "test_gemm_conv: cu and plen go together");
+  if (B <= 0 || T_in <= 0 || C <= 0 || C % 64 != 0 || N <= 0 || N % 256 != 0)
+    return fail(h, -1, "test_gemm_conv: bad sizes B=%d T_in=%d C=%d N=%d (C %% 64 == 0, N %% 256 == 0)", B, T_in, C, N);
+  if (!conv1d && F1 != 32)
+    return fail(h, -1, "test_gemm_conv: the 3x3 conv maps 16 output bins per frame (F1 = 32), got F1=%d", F1);
+  if (!conv1d && (taps != 9 || f32_out)) return fail(h, -1, "test_gemm_conv: the 3x3 conv has 9 taps and fp16 output");
+  if (conv1d && (taps < 1 || taps % 2 == 0)) return fail(h, -1, "test_gemm_conv: conv1d needs an odd tap count (got %d)", taps);
+  const int k = conv1d ? taps : 3;
+  const int T_out = sub_out_len(T_in, k, (k - 1) / 2);
+  if (T_out <= 0) return fail(h, -1, "test_gemm_conv: T_in=%d gives no output frame", T_in);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (cu) {
+    std::vector<int> c, p;
+    if (dev_ints(cu, B, c, s) || dev_ints(plen, B, p, s)) return fail(h, -3, "test_gemm_conv: cannot read cu / plen");
+    for (int b = 0; b < B; ++b)
+      if (c[b] < 0 || static_cast<int64_t>(c[b]) + std::min(std::max(p[b], 0), T_out) > out_frames)
+        return fail(h, -1, "test_gemm_conv: utterance %d (cu %d, plen %d) runs past %d output frames", b, c[b], p[b], out_frames);
+  } else if (static_cast<int64_t>(B) * T_out > out_frames) {
+    return fail(h, -1, "test_gemm_conv: %d x %d output frames do not fit %d", B, T_out, out_frames);
+  }
+  CUtensorMap ta, tw;
+  int rc = conv1d ? make_tmap_conv3d(&ta, A, B, T_in, C) : make_tmap_conv4d(&ta, A, B, T_in, F1, C);
+  rc |= make_tmap_2d_f16(&tw, W, N, static_cast<uint64_t>(taps) * C, static_cast<uint64_t>(taps) * C, 128, 64);
+  if (rc) return fail(h, -2, "tensor map encode failed (rc=%d)", rc);
+  {
+    PROF(PC_MISC);
+    rc = conv1d ? launch_gemm_conv1d(&ta, &tw, B, T_out, C, taps, N, bias, len_out, cu, plen, out, N, f32_out, h->num_sms, s)
+                : launch_gemm_conv(&ta, &tw, B, T_out, C, N, bias, len_out, cu, plen, out, N, h->num_sms, s);
+  }
+  if (rc) return fail(h, -4, "conv gemm launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, "test_gemm_conv");
+  return 0;
+}
+
+int gam_test_layernorm(gam_handle* h, const float* x, const float* g, const float* b, void* out, int32_t rows, const int32_t* rows_dev,
+                       int32_t reverse, void* stream) {
+  if (!x || !g || !b || !out || rows <= 0) return fail(h, -1, "test_layernorm: x, g, b, out and rows > 0 are required");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  { PROF(PC_LAYERNORM);
+    launch_ln_f16(x, g, b, static_cast<__half*>(out), rows, rows_dev, reverse, s); }
+  GAM_CHECK_LAUNCH(h, "test_layernorm");
+  return 0;
+}
+
+int gam_test_ln_rope(gam_handle* h, const float* x, const float* g, const float* b, const float* rope_cos, const float* rope_sin,
+                     int32_t table_rows, int32_t half_dim, void* out_u, void* out_r, int32_t rows, const int32_t* rows_dev,
+                     const int32_t* row_t, int32_t T, int32_t reverse, void* stream) {
+  if (!x || !g || !b || !rope_cos || !rope_sin || !out_u || !out_r || rows <= 0)
+    return fail(h, -1, "test_ln_rope: every buffer and rows > 0 are required");
+  if (half_dim <= 0 || half_dim % 4 != 0 || 768 % (2 * half_dim) != 0)
+    return fail(h, -1, "test_ln_rope: half_dim %d must be a multiple of 4 and 2*half_dim divide 768", half_dim);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (row_t) {
+    std::vector<int> n, t;
+    int live = rows;
+    if (rows_dev) {
+      if (dev_ints(rows_dev, 1, n, s)) return fail(h, -3, "test_ln_rope: cannot read rows_dev");
+      live = std::min(std::max(n[0], 0), rows);
+    }
+    if (live > 0 && dev_ints(row_t, live, t, s)) return fail(h, -3, "test_ln_rope: cannot read row_t");
+    for (int r = 0; r < live; ++r)
+      if (t[r] < 0 || t[r] >= table_rows) return fail(h, -1, "test_ln_rope: row %d has position %d outside the %d-row table", r, t[r], table_rows);
+  } else if (T <= 0 || T > table_rows) {
+    return fail(h, -1, "test_ln_rope: T=%d must be in [1, %d] without row_t", T, table_rows);
+  }
+  { PROF(PC_LAYERNORM);
+    launch_ln_rope_f16(x, g, b, rope_cos, rope_sin, static_cast<__half*>(out_u), static_cast<__half*>(out_r), rows, rows_dev, row_t,
+                       T > 0 ? T : 1, half_dim, reverse, s); }
+  GAM_CHECK_LAUNCH(h, "test_ln_rope");
+  return 0;
+}
+
+int gam_test_ln_out_ln(gam_handle* h, const float* r, const float* g_out, const float* b_out, const float* g_next, const float* b_next,
+                       float* x_out, void* y_out, int32_t rows, const int32_t* rows_dev, int32_t reverse, void* stream) {
+  if (!r || !g_out || !b_out || !x_out || rows <= 0 || (y_out && (!g_next || !b_next)))
+    return fail(h, -1, "test_ln_out_ln: r, g_out, b_out, x_out, rows > 0 (and g_next, b_next with y_out) are required");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  { PROF(PC_LAYERNORM);
+    launch_ln_out_ln(r, g_out, b_out, g_next, b_next, x_out, static_cast<__half*>(y_out), rows, rows_dev, reverse, s); }
+  GAM_CHECK_LAUNCH(h, "test_ln_out_ln");
+  return 0;
+}
+
+int gam_test_unpack_rows(gam_handle* h, const float* x, const float* gamma, const float* beta, const int32_t* cu, const int32_t* plen,
+                         float* out, int32_t B, int32_t T, int32_t rows, int32_t reverse, void* stream) {
+  if (!x || !cu || !plen || !out || (gamma != nullptr) != (beta != nullptr) || B <= 0 || T <= 0)
+    return fail(h, -1, "test_unpack_rows: x, cu, plen, out, B > 0, T > 0 (and gamma with beta) are required");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<int> c, p;
+  if (dev_ints(cu, B, c, s) || dev_ints(plen, B, p, s)) return fail(h, -3, "test_unpack_rows: cannot read cu / plen");
+  for (int b = 0; b < B; ++b) {
+    const int n = std::min(p[b], T);
+    if (n > 0 && (c[b] < 0 || static_cast<int64_t>(c[b]) + n > rows))
+      return fail(h, -1, "test_unpack_rows: utterance %d (cu %d, plen %d) reads past %d rows", b, c[b], p[b], rows);
+  }
+  { PROF(PC_MISC);
+    launch_unpack_rows(x, gamma, beta, cu, plen, out, B, T, reverse, s); }
+  GAM_CHECK_LAUNCH(h, "test_unpack_rows");
+  return 0;
+}
+
+int gam_test_dwconv(gam_handle* h, int32_t layer_norm, const void* g, const float* w, const float* bias, const float* gamma,
+                    const float* beta, const int32_t* len, const int32_t* cu, const int32_t* plen, const int32_t* row_b,
+                    const int32_t* row_t, const int32_t* rows_dev, void* out, int32_t B, int32_t T, int32_t rows, int32_t kw,
+                    void* stream) {
+  if (!g || !w || !bias || !len || !out || B <= 0 || T <= 0) return fail(h, -1, "test_dwconv: g, w, bias, len, out, B, T are required");
+  if (kw != 5 && kw != 31) return fail(h, -1, "test_dwconv: kernel size %d (5 or 31 are compiled)", kw);
+  if ((cu != nullptr) != (plen != nullptr)) return fail(h, -1, "test_dwconv: cu and plen go together");
+  if (layer_norm && (!gamma || !beta || (cu && (!row_b || !row_t))))
+    return fail(h, -1, "test_dwconv: the LayerNorm variant needs gamma, beta (and row_b, row_t when packed)");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<int> l, c, p;
+  if (dev_ints(len, B, l, s)) return fail(h, -3, "test_dwconv: cannot read len");
+  if (cu && (dev_ints(cu, B, c, s) || dev_ints(plen, B, p, s))) return fail(h, -3, "test_dwconv: cannot read cu / plen");
+  for (int b = 0; b < B; ++b) {
+    // rows of utterance b the kernel touches: reads frames < min(len, T), writes frames < min(plen, T) (padded: T)
+    const int n = std::max(std::min(l[b], T), cu ? std::min(p[b], T) : T);
+    const int64_t base = cu ? c[b] : static_cast<int64_t>(b) * T;
+    if (n > 0 && (base < 0 || base + n > rows))
+      return fail(h, -1, "test_dwconv: utterance %d (rows %lld + %d) runs past %d rows", b, (long long)base, n, rows);
+  }
+  if (layer_norm) {   // one warp per row < live rows; a packed row finds its (utterance, frame) in row_b / row_t
+    int live = B * T;
+    std::vector<int> n, rb, rt;
+    if (rows_dev) {
+      if (dev_ints(rows_dev, 1, n, s)) return fail(h, -3, "test_dwconv: cannot read rows_dev");
+      live = std::min(std::max(n[0], 0), B * T);
+    }
+    if (live > rows) return fail(h, -1, "test_dwconv: %d live rows exceed the %d-row buffers", live, rows);
+    if (cu && live > 0) {
+      if (dev_ints(row_b, live, rb, s) || dev_ints(row_t, live, rt, s)) return fail(h, -3, "test_dwconv: cannot read row_b / row_t");
+      for (int r = 0; r < live; ++r)
+        if (rb[r] < 0 || rb[r] >= B || rt[r] < 0 || rt[r] >= T)
+          return fail(h, -1, "test_dwconv: row %d maps to (utterance %d, frame %d) outside [%d, %d)", r, rb[r], rt[r], B, T);
+    }
+  }
+  int rc;
+  { PROF(PC_DWCONV);
+    rc = layer_norm ? launch_dwconv_ln_silu(static_cast<const __half*>(g), w, bias, gamma, beta, len, cu, row_b, row_t, rows_dev,
+                                            static_cast<__half*>(out), B, T, kw, s)
+                    : launch_dwconv_bn_silu(static_cast<const __half*>(g), w, bias, len, cu, plen, static_cast<__half*>(out), B, T, kw, s); }
+  if (rc) return fail(h, -4, "test_dwconv: launch rejected (kw=%d)", kw);
+  GAM_CHECK_LAUNCH(h, "test_dwconv");
+  return 0;
+}
+
+int gam_test_pack_plan(gam_handle* h, const int64_t* mel_len, int32_t B, int32_t k, int64_t M, int32_t* len0, int32_t* len1,
+                       int32_t* len2, int32_t* plen, int32_t* run1, int32_t* cu, int32_t* rows_dev, int32_t* row_b, int32_t* row_t,
+                       void* stream) {
+  if (!mel_len || !len0 || !len1 || !len2 || !plen || !run1 || !cu || !rows_dev || !row_b || !row_t)
+    return fail(h, -1, "test_pack_plan: every buffer is required");
+  if (B <= 0 || B > 65535 || k < 1 || M <= 0 || M > INT32_MAX) return fail(h, -1, "test_pack_plan: bad sizes B=%d k=%d M=%lld", B, k, (long long)M);
+  const int pad = (k - 1) / 2;
+  const int T1 = sub_out_len(static_cast<int>(M), k, pad), T2 = sub_out_len(T1, k, pad);
+  if (T2 <= 0) return fail(h, -1, "test_pack_plan: M=%lld gives no encoder frame", (long long)M);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  { PROF(PC_MISC);
+    launch_pack_plan(reinterpret_cast<const long long*>(mel_len), B, 2 * pad - k, static_cast<int>(M), T1, T2, len0, len1, len2, plen,
+                     run1, cu, rows_dev, row_b, row_t, s); }
+  GAM_CHECK_LAUNCH(h, "test_pack_plan");
+  return 0;
+}
+
+int gam_test_subsample_conv1(gam_handle* h, const float* mel, const int32_t* len0, const int32_t* len1, const int32_t* run1,
+                             const float* w, const float* bias, void* out, int32_t B, int32_t F, int64_t M, int32_t C, void* stream) {
+  if (!mel || !len0 || !len1 || !w || !bias || !out || B <= 0 || M <= 0 || M > INT32_MAX)
+    return fail(h, -1, "test_subsample_conv1: mel, len0, len1, w, bias, out, B > 0, M > 0 are required");
+  if (F <= 0 || F > 70 || C <= 0 || C % 8 != 0 || C / 8 > 128)
+    return fail(h, -1, "test_subsample_conv1: F=%d (<= 70) or C=%d (multiple of 8, <= 1024) unsupported", F, C);
+  const int T1 = sub_out_len(static_cast<int>(M), 3, 1), F1 = sub_out_len(F, 3, 1);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  { PROF(PC_SUB_CONV1);
+    rc = launch_subsample_conv1(mel, len0, len1, run1, w, bias, static_cast<__half*>(out), B, static_cast<int>(M), F, T1, F1, C, s); }
+  if (rc) return fail(h, -4, "test_subsample_conv1: launch rejected");
+  GAM_CHECK_LAUNCH(h, "test_subsample_conv1");
+  return 0;
+}
+
+int gam_test_mel_to_tmajor(gam_handle* h, const float* mel, const int32_t* len0, void* out, int32_t B, int32_t F, int64_t M, void* stream) {
+  if (!mel || !len0 || !out || B <= 0 || B > 65535 || F <= 0 || M <= 0 || M > INT32_MAX)
+    return fail(h, -1, "test_mel_to_tmajor: mel, len0, out and sizes B in [1, 65535], F > 0, M > 0 are required");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  { PROF(PC_SUB_CONV1);
+    launch_mel_to_tmajor_f16(mel, len0, static_cast<__half*>(out), B, F, static_cast<int>(M), s); }
+  GAM_CHECK_LAUNCH(h, "test_mel_to_tmajor");
   return 0;
 }
 

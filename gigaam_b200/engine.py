@@ -44,6 +44,11 @@ def pack_conv2_weight(w2: Tensor) -> Tensor:
     return w2.permute(0, 2, 3, 1).reshape(w2.shape[0], -1)
 
 
+def pack_conv1d_weight(w: Tensor) -> Tensor:
+    """Conv1d weight [C_out, C_in, k] -> [C_out, (k, C_in)]: K order (tap, channel) of the implicit conv1d GEMM."""
+    return w.permute(0, 2, 1).reshape(w.shape[0], -1)
+
+
 def pack_sub_out_weight(wo: Tensor, channels: int) -> Tensor:
     """pre_encode.out.weight [d, C*F2] with K index c*F2+f (gigaam/encoder.py:125-127) -> K index f*C+c, the order in
     which the stage-2 conv epilogue writes its [B, T', F2, C] output."""
@@ -282,8 +287,7 @@ class Engine:
         if enc["subsampling"] == "conv1d":
             # Conv1d weights [out, in, k] -> (out, k, in): K order (tap, channel) of the implicit GEMM
             for i, name in ((0, "c1d_w1"), (2, "c1d_w2")):
-                w = sd[f"{p}conv.{i}.weight"].float()
-                setattr(gw, name, self._dev(w.permute(0, 2, 1).reshape(w.shape[0], -1), torch.float16))
+                setattr(gw, name, self._dev(pack_conv1d_weight(sd[f"{p}conv.{i}.weight"].float()), torch.float16))
             gw.c1d_b1 = self._dev(sd[p + "conv.0.bias"].float())
             gw.c1d_b2 = self._dev(sd[p + "conv.2.bias"].float())
             return

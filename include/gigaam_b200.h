@@ -222,11 +222,64 @@ int gam_group_words(gam_handle* h, const int32_t* ids, const int32_t* frames, co
                     const uint8_t* token_flags, int32_t V, int32_t max_words, int32_t* word_start, int32_t* word_end,
                     int32_t* word_first_token, int32_t* word_tokens, int32_t* n_words, void* stream);
 
-/* ---- unit entry points (parity tests of the individual kernels) ---- */
+/* ---- unit entry points (parity tests of the individual kernels).  Operands come from the caller, not from the handle; every
+ * size the kernel does not support is refused, and device-side row maps are read back and checked against the buffers
+ * (these calls synchronise the stream to do so: they are for tests, not for the hot path). ---- */
 /* D[M,N] = A[M,K] W[N,K]^T with epilogue `kind` (0 bias->f16, 1 bias+silu->f16, 2 bias+glu->f16 [N/2 cols],
- * 3 res + scale*(acc+bias) -> f32, 4 bias -> f32).  A, W fp16 device; N % 256 == 0; K % 64 == 0. */
-int gam_test_gemm(gam_handle* h, int32_t kind, const void* A, const void* W, const float* bias, const float* res, void* out,
-                  int32_t M, int32_t N, int32_t K, int32_t ldo, float scale, void* stream);
+ * 3 res + scale*(acc+bias) -> f32, 4 bias -> f32, 7 DFT power (re^2 + im^2) * 2^-28 -> f32 [N/2 cols], no bias), written to
+ * columns [col0, col0 + cols) of out (and read from the same columns of res; res == out is allowed) with row pitch ldo.
+ * A2 != NULL (kind 0 only): columns [0, n1) read A, [n1, N) read A2 (one launch, as gam_encode's q/k/v projection).
+ * reverse: walk the tiles from the last; m_dev: device i32 row count (clamped to [0, M]; rows at or past it are not written)
+ * or NULL = M.  A, A2, W fp16 device [M or N, K]; N % 256 == 0; K % 64 == 0. */
+int gam_test_gemm(gam_handle* h, int32_t kind, const void* A, const void* A2, int32_t n1, const void* W, const float* bias,
+                  const float* res, void* out, int32_t M, int32_t N, int32_t K, int32_t ldo, int32_t col0, float scale,
+                  int32_t reverse, const int32_t* m_dev, void* stream);
+/* Implicit-GEMM stride-2 convolutions of the subsampling, out[frame, N] = relu(conv + bias) for frames t < len_out[b], 0 for the
+ * others (fp16, or fp32 when f32_out):
+ *   conv1d == 0: 3x3 / pad 1 over channels-last A f16 [B, T_in, F1 = 32, C], W = [N, (kt, kf, c)] f16; frame row = 16 rows
+ *                (one per output bin) of out [out_frames * 16, N];
+ *   conv1d == 1: `taps` / pad (taps-1)/2 over time-major A f16 [B, T_in, C], W = [N, (tap, c)] f16; out [out_frames, N].
+ * T_out = floor((T_in + 2 pad - k) / 2 + 1).  cu / plen (device i32 [B], both or neither): frame (b, t < plen[b]) -> row cu[b] + t
+ * and nothing else is written; NULL: frame (b, t) -> row b * T_out + t for every t < T_out. */
+int gam_test_gemm_conv(gam_handle* h, int32_t conv1d, const void* A, const void* W, const float* bias, const int32_t* len_out,
+                       const int32_t* cu, const int32_t* plen, void* out, int32_t out_frames, int32_t B, int32_t T_in, int32_t F1,
+                       int32_t C, int32_t taps, int32_t N, int32_t f32_out, void* stream);
+/* LayerNorm(768, eps 1e-5) of fp32 rows -> fp16, rows at or past *rows_dev (NULL: rows) untouched; reverse walks them from the last */
+int gam_test_layernorm(gam_handle* h, const float* x, const float* g, const float* b, void* out, int32_t rows, const int32_t* rows_dev,
+                       int32_t reverse, void* stream);
+/* LayerNorm + rotary embedding: out_u = LN(x) f16, out_r = rope(LN(x)) f16 per head of 2*half_dim with the [table_rows, half_dim]
+ * fp32 cos / sin tables at position row_t[row] (device i32, or NULL: row % T) */
+int gam_test_ln_rope(gam_handle* h, const float* x, const float* g, const float* b, const float* rope_cos, const float* rope_sin,
+                     int32_t table_rows, int32_t half_dim, void* out_u, void* out_r, int32_t rows, const int32_t* rows_dev,
+                     const int32_t* row_t, int32_t T, int32_t reverse, void* stream);
+/* x_out = LN_out(r) fp32 (x_out may be r), y_out = LN_next(x_out) f16 (y_out NULL: not computed) */
+int gam_test_ln_out_ln(gam_handle* h, const float* r, const float* g_out, const float* b_out, const float* g_next, const float* b_next,
+                       float* x_out, void* y_out, int32_t rows, const int32_t* rows_dev, int32_t reverse, void* stream);
+/* packed fp32 rows x [rows, 768] -> out f32 [B, T, 768]: out[b, t] = x[cu[b] + t] (LayerNorm'd when gamma != NULL) for
+ * t < plen[b], zeros elsewhere */
+int gam_test_unpack_rows(gam_handle* h, const float* x, const float* gamma, const float* beta, const int32_t* cu, const int32_t* plen,
+                         float* out, int32_t B, int32_t T, int32_t rows, int32_t reverse, void* stream);
+/* depthwise conv (kw = 5 or 31 taps, w f32 [kw, 768], frames t >= len[b] read as zero) + SiLU, layer_norm == 0: bias carries the
+ * folded BatchNorm; layer_norm == 1: LayerNorm over channels (gamma, beta) before the SiLU.  g, out f16 [rows, 768]: utterance
+ * b at row cu[b] with plen[b] frames (cu / plen NULL: row b * T, T frames); the LayerNorm variant walks rows < *rows_dev (NULL:
+ * B * T) and finds their (utterance, frame) in row_b / row_t when packed. */
+int gam_test_dwconv(gam_handle* h, int32_t layer_norm, const void* g, const float* w, const float* bias, const float* gamma,
+                    const float* beta, const int32_t* len, const int32_t* cu, const int32_t* plen, const int32_t* row_b,
+                    const int32_t* row_t, const int32_t* rows_dev, void* out, int32_t B, int32_t T, int32_t rows, int32_t kw,
+                    void* stream);
+/* gam_encode's first kernels: stage lengths of the subsampling (kernel size k) for mel lengths mel_len (device i64 [B]) and
+ * M mel frames, and the packed-row plan: len0..len2, plen, run1 i32 [B], cu i32 [B + 1], rows_dev i32 [1], row_b / row_t
+ * i32 [B * T'] (rows < cu[B] written) */
+int gam_test_pack_plan(gam_handle* h, const int64_t* mel_len, int32_t B, int32_t k, int64_t M, int32_t* len0, int32_t* len1,
+                       int32_t* len2, int32_t* plen, int32_t* run1, int32_t* cu, int32_t* rows_dev, int32_t* row_b, int32_t* row_t,
+                       void* stream);
+/* conv2d subsampling stage 1: mel f32 [B, F, M] -> out f16 [B, T1, F1, C] (3x3 / stride 2 / pad 1, one input channel, w f32
+ * [C, 9]); mel frames >= len0 read as zero, frames >= len1 written as zero, 8-frame blocks from run1[b] on (run1 may be NULL)
+ * not written */
+int gam_test_subsample_conv1(gam_handle* h, const float* mel, const int32_t* len0, const int32_t* len1, const int32_t* run1,
+                             const float* w, const float* bias, void* out, int32_t B, int32_t F, int64_t M, int32_t C, void* stream);
+/* mel f32 [B, F, M] -> time-major f16 [B, M, F], frames >= len0[b] zeroed (conv1d subsampling input) */
+int gam_test_mel_to_tmajor(gam_handle* h, const float* mel, const int32_t* len0, void* out, int32_t B, int32_t F, int64_t M, void* stream);
 /* qkv: f16 [B*T, 3*d_model]; klen i32 [B] or NULL -> out f16 [B*T, d_model] */
 int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void* out, int32_t B, int32_t T, void* stream);
 /* rel_pos variant: qkv f16 [B*T, 4*d_model] = [q+u | q+v | k | v]; pos f16 [2*GAM_REL_POS_MAX_T-1, d_model] */

@@ -48,25 +48,7 @@ def _stream():
 
 
 # ------------------------------------------------------------------------------------------ kernels in isolation
-@pytest.mark.parametrize("M,N,K", [(128, 256, 64), (1000, 768, 768), (777, 768, 3072), (300, 1536, 768), (1, 256, 128)])
-def test_gemm_epilogues(eng_ctc, dev, M, N, K):
-    g = torch.Generator().manual_seed(M + N + K)
-    A = (torch.randn(M, K, generator=g) * 0.5).half().to(dev)
-    W = (torch.randn(N, K, generator=g) / K ** 0.5).half().to(dev)
-    bias = torch.randn(N, generator=g).to(dev)
-    res = torch.randn(M, N, generator=g).to(dev)
-    ref = A.float() @ W.float().t() + bias                       # torch fp32 reference of the same op
-    r4 = ref.view(M, N // 256, 2, 128)
-    wants = {0: ref, 1: F.silu(ref), 2: (r4[:, :, 0] * torch.sigmoid(r4[:, :, 1])).reshape(M, N // 2), 3: res + 0.5 * ref, 4: ref}
-    for kind, want in wants.items():
-        out = torch.zeros(want.shape, dtype=torch.float16 if kind < 3 else torch.float32, device=dev)
-        rc = eng_ctc.lib.gam_test_gemm(eng_ctc.handle, kind, A.data_ptr(), W.data_ptr(), bias.data_ptr(),
-                                       res.data_ptr() if kind == 3 else None, out.data_ptr(), M, N, K, want.shape[1], 0.5, _stream())
-        torch.cuda.synchronize()
-        assert rc == 0
-        assert rel(out.float(), want) < (1e-3 if kind < 3 else 1e-5), f"kind {kind}"
-
-
+# (the GEMM, row, subsampling and packing kernels have float64 unit tests of their own in test_kernel_units.py)
 @pytest.mark.parametrize("B,T,lens", [(1, 128, None), (2, 51, [51, 30]), (3, 251, [251, 200, 97]), (2, 376, [376, 129]),
                                       (1, 626, None), (2, 5, [5, 1]), (2, 129, [129, 128]), (2, 751, [751, 640]), (1, 768, None)])
 def test_attention_matches_masked_softmax(eng_ctc, dev, B, T, lens):

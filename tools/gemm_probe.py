@@ -30,8 +30,8 @@ for (N, K, kinds) in ((768, 768, (3,)), (768, 3072, (3,)), (3072, 768, (1,)), (2
             flush.fill_(it)
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            rc = eng.lib.gam_test_gemm(eng.handle, kind, A.data_ptr(), W.data_ptr(), bias.data_ptr(), out.data_ptr() if kind == 3 else None,
-                                       out.data_ptr(), M, N, K, ncol, 0.5, st)
+            rc = eng.lib.gam_test_gemm(eng.handle, kind, A.data_ptr(), None, 0, W.data_ptr(), bias.data_ptr(),
+                                       out.data_ptr() if kind == 3 else None, out.data_ptr(), M, N, K, ncol, 0, 0.5, 0, None, st)
             e1.record()
             torch.cuda.synchronize()
             assert rc == 0
