@@ -117,7 +117,7 @@ struct gam_handle {
   const void* lm_A = nullptr;
   int64_t lm_F = 0;
   int device = 0;
-  int num_sms = 132;
+  int gemm_clusters = 0;   // co-resident clusters of the GEMM kernel (gemm_init)
   int64_t launches = 0;
   void* comm = nullptr;      // ncclComm_t of gam_comm_init
   int comm_rank = 0, comm_nranks = 1;
@@ -320,9 +320,8 @@ int gam_create(const gam_config* cfg, const gam_weights* w, int device, gam_hand
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(h, -11, "cudaGetDeviceProperties failed");
   if (prop.major != 9 || prop.minor != 0)
     return fail(h, -12, "sm_90a kernels need a Hopper (cc 9.0) device, found cc %d.%d", prop.major, prop.minor);
-  h->num_sms = prop.multiProcessorCount;
   if (init_encode() != 0) return fail(h, -13, "cuTensorMapEncodeTiled entry point not available");
-  if (gemm_init() != 0) return fail(h, -14, "cudaFuncSetAttribute failed for the GEMM kernels: %s", cudaGetErrorString(cudaGetLastError()));
+  if (gemm_init(&h->gemm_clusters) != 0) return fail(h, -14, "GEMM kernel set-up (shared memory opt-in, cluster occupancy) failed: %s", cudaGetErrorString(cudaGetLastError()));
   h->layers.assign(w->layers, w->layers + c.n_layers);
   h->w.layers = h->layers.data();
   h->lmaps.resize(c.n_layers);
@@ -446,7 +445,7 @@ int gam_logmel_tc(gam_handle* h, const float* wav, int32_t B, int64_t n_samples,
   }
   {
     PROF(PC_LOGMEL);
-    if (launch_gemm_power(&h->m_lm_a, &h->m_dft_w, static_cast<int>(F), 512, 3 * Kp, P, 256, h->num_sms, s) != 0)
+    if (launch_gemm_power(&h->m_lm_a, &h->m_dft_w, static_cast<int>(F), 512, 3 * Kp, P, 256, h->gemm_clusters, s) != 0)
       return fail(h, -4, "logmel_tc: DFT GEMM launch rejected");
   }
   {
@@ -468,7 +467,7 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
   if (p->T2 > GAM_REL_POS_MAX_T)
     return fail(h, -1, "T'=%d exceeds the attention kernels' %d-frame limit (%.1f s of audio); cut the recording into segments "
                 "(transcribe_longform does)", p->T2, GAM_REL_POS_MAX_T, GAM_REL_POS_MAX_T * 0.04);
-  const int d = c.d_model, R = p->R, nsm = h->num_sms;
+  const int d = c.d_model, R = p->R, ncl = h->gemm_clusters;
   const int L = (n_layers_run < 0 || n_layers_run > c.n_layers) ? c.n_layers : n_layers_run;
   int rc = 0;
 
@@ -491,13 +490,13 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
     }
     {
       PROF(PC_GEMM_CONV2);
-      rc |= launch_gemm_conv(&p->m_s1, &h->m_sub2_w, B, p->T2, d, d, h->w.sub2_b, p->len2, p->cu, p->plen, p->s2, d, nsm, s);
+      rc |= launch_gemm_conv(&p->m_s1, &h->m_sub2_w, B, p->T2, d, d, h->w.sub2_b, p->len2, p->cu, p->plen, p->s2, d, ncl, s);
     }
     GAM_CHECK_LAUNCH(h, "subsampling");
     if (rc) return fail(h, -4, "subsampling launch rejected (rc=%d)", rc);
     {
       PROF(PC_GEMM_SUBOUT);
-      rc |= launch_gemm(GEMM_BIAS_F32, &p->m_s2, &h->m_sub_out_w, R, d, p->F2 * d, h->w.sub_out_b, nullptr, p->x, d, 1.f, nsm, s, 0, rdev);
+      rc |= launch_gemm(GEMM_BIAS_F32, &p->m_s2, &h->m_sub_out_w, R, d, p->F2 * d, h->w.sub_out_b, nullptr, p->x, d, 1.f, ncl, s, 0, rdev);
     }
   } else {
     // conv1d subsampling (gigaam/encoder.py:59-70 with Conv1d): two k-tap / stride-2 implicit GEMMs over time-major data
@@ -508,12 +507,12 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
     {
       PROF(PC_GEMM_CONV2);
       rc |= launch_gemm_conv1d(&p->m_melT, &h->m_sub2_w, B, p->T1, c.feat_in, c.subs_kernel_size, d, h->w.c1d_b1, p->len1, nullptr,
-                               nullptr, p->s1, d, 0, nsm, s);   // stage 1 stays [B, T1]: stage 2 fetches it with 3-D TMA boxes
+                               nullptr, p->s1, d, 0, ncl, s);   // stage 1 stays [B, T1]: stage 2 fetches it with 3-D TMA boxes
     }
     {
       PROF(PC_GEMM_SUBOUT);
       rc |= launch_gemm_conv1d(&p->m_s1_3d, &h->m_sub_out_w, B, p->T2, d, c.subs_kernel_size, d, h->w.c1d_b2, p->len2, p->cu,
-                               p->plen, p->x, d, 1, nsm, s);
+                               p->plen, p->x, d, 1, ncl, s);
     }
     GAM_CHECK_LAUNCH(h, "subsampling");
     if (rc) return fail(h, -4, "conv1d subsampling launch rejected (rc=%d)", rc);
@@ -536,9 +535,9 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
     const LayerMaps& m = h->lmaps[l];
     // x += 0.5 * FF1(LN(x))                                     (encoder.py:480-483)
     { PROF(PC_GEMM_FFN_UP);
-      rc |= launch_gemm(GEMM_BIAS_SILU_F16, &p->m_a16, &m.ff1_w1, R, c.d_ff, d, w.ff1_b1, nullptr, p->big16, c.d_ff, 1.f, nsm, s, 0, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_SILU_F16, &p->m_a16, &m.ff1_w1, R, c.d_ff, d, w.ff1_b1, nullptr, p->big16, c.d_ff, 1.f, ncl, s, 0, rdev); }
     { PROF(PC_GEMM_FFN_DOWN);
-      rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_hid, &m.ff1_w2, R, d, c.d_ff, w.ff1_b2, p->x, p->x, d, 0.5f, nsm, s, zz, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_hid, &m.ff1_w2, R, d, c.d_ff, w.ff1_b2, p->x, p->x, d, 0.5f, ncl, s, zz, rdev); }
     // x += W_o attn(q = W_q rope(u), k = W_k rope(u), v = W_v u), u = LN(x)   (encoder.py:485-487, 236-277)
     if (c.self_attention == 0) {
       { PROF(PC_LAYERNORM);
@@ -547,13 +546,13 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
       bool merged = false;
       if (m.qkv_merged) {
         PROF(PC_GEMM_QKV);
-        merged = launch_gemm_dual_a(&p->m_r16, &p->m_a16, 2 * d, &m.w_qkv, R, 3 * d, d, w.b_qk, p->big16, 3 * d, nsm, s, zz, rdev) == 0;
+        merged = launch_gemm_dual_a(&p->m_r16, &p->m_a16, 2 * d, &m.w_qkv, R, 3 * d, d, w.b_qk, p->big16, 3 * d, ncl, s, zz, rdev) == 0;
       }
       if (!merged) {
         { PROF(PC_GEMM_QKV);
-          rc |= launch_gemm(GEMM_BIAS_F16, &p->m_r16, &m.w_qk, R, 2 * d, d, w.b_qk, nullptr, p->big16, 3 * d, 1.f, nsm, s, zz, rdev); }
+          rc |= launch_gemm(GEMM_BIAS_F16, &p->m_r16, &m.w_qk, R, 2 * d, d, w.b_qk, nullptr, p->big16, 3 * d, 1.f, ncl, s, zz, rdev); }
         { PROF(PC_GEMM_QKV);
-          rc |= launch_gemm(GEMM_BIAS_F16, &p->m_a16, &m.w_v, R, d, d, w.b_v, nullptr, p->big16 + 2 * d, 3 * d, 1.f, nsm, s, zz, rdev); }
+          rc |= launch_gemm(GEMM_BIAS_F16, &p->m_a16, &m.w_v, R, d, d, w.b_v, nullptr, p->big16 + 2 * d, 3 * d, 1.f, ncl, s, zz, rdev); }
       }
       { PROF(PC_ATTENTION);
         rc |= launch_attention(&p->m_qkv, p->plen, p->cu, p->o16, B, p->T2, c.n_heads, dk, d, s); }
@@ -562,17 +561,17 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
       { PROF(PC_LAYERNORM);
         launch_ln_f16(p->x, w.ln_att_g, w.ln_att_b, p->a16, R, rdev, 0, s); }
       { PROF(PC_GEMM_QKV);
-        rc |= launch_gemm(GEMM_BIAS_F16, &p->m_a16, &m.w_qkv_rel, R, 4 * d, d, w.b_qkv_rel, nullptr, p->big16, 4 * d, 1.f, nsm, s, zz, rdev); }
+        rc |= launch_gemm(GEMM_BIAS_F16, &p->m_a16, &m.w_qkv_rel, R, 4 * d, d, w.b_qkv_rel, nullptr, p->big16, 4 * d, 1.f, ncl, s, zz, rdev); }
       { PROF(PC_ATTENTION);
         rc |= launch_attention_relpos(&p->m_qkv4, &m.pos_proj, p->plen, p->cu, p->o16, B, p->T2, c.n_heads, dk, d, s); }
     }
     { PROF(PC_GEMM_PROJ);
-      rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_o16, &m.w_o, R, d, d, w.b_o, p->x, p->x, d, 1.f, nsm, s, zz, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_o16, &m.w_o, R, d, d, w.b_o, p->x, p->x, d, 1.f, ncl, s, zz, rdev); }
     // x += Conv(LN(x))                                           (encoder.py:489-491, 396-409)
     { PROF(PC_LAYERNORM);
       launch_ln_f16(p->x, w.ln_conv_g, w.ln_conv_b, p->a16, R, rdev, 0, s); }
     { PROF(PC_GEMM_GLU);
-      rc |= launch_gemm(GEMM_BIAS_GLU_F16, &p->m_a16, &m.pw1, R, 2 * d, d, w.pw1_b, nullptr, p->g16, d, 1.f, nsm, s, zz, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_GLU_F16, &p->m_a16, &m.pw1, R, 2 * d, d, w.pw1_b, nullptr, p->g16, d, 1.f, ncl, s, zz, rdev); }
     { PROF(PC_DWCONV);
       if (c.conv_norm == 0)
         rc |= launch_dwconv_bn_silu(p->g16, w.dw_w, w.dw_b, p->len2, p->cu, p->plen, p->o16, B, p->T2, c.conv_kernel_size, s);
@@ -580,14 +579,14 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
         rc |= launch_dwconv_ln_silu(p->g16, w.dw_w, w.dw_b, w.cn_g, w.cn_b, p->len2, p->cu, p->row_b, p->row_t, rdev, p->o16, B, p->T2,
                                     c.conv_kernel_size, s); }
     { PROF(PC_GEMM_PROJ);
-      rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_o16, &m.pw2, R, d, d, w.pw2_b, p->x, p->x, d, 1.f, nsm, s, zz, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_o16, &m.pw2, R, d, d, w.pw2_b, p->x, p->x, d, 1.f, ncl, s, zz, rdev); }
     // x += 0.5 * FF2(LN(x))                                      (encoder.py:493-495)
     { PROF(PC_LAYERNORM);
       launch_ln_f16(p->x, w.ln_ff2_g, w.ln_ff2_b, p->a16, R, rdev, 0, s); }
     { PROF(PC_GEMM_FFN_UP);
-      rc |= launch_gemm(GEMM_BIAS_SILU_F16, &p->m_a16, &m.ff2_w1, R, c.d_ff, d, w.ff2_b1, nullptr, p->big16, c.d_ff, 1.f, nsm, s, zz, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_SILU_F16, &p->m_a16, &m.ff2_w1, R, c.d_ff, d, w.ff2_b1, nullptr, p->big16, c.d_ff, 1.f, ncl, s, zz, rdev); }
     { PROF(PC_GEMM_FFN_DOWN);
-      rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_hid, &m.ff2_w2, R, d, c.d_ff, w.ff2_b2, p->x, p->x, d, 0.5f, nsm, s, 0, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_hid, &m.ff2_w2, R, d, c.d_ff, w.ff2_b2, p->x, p->x, d, 0.5f, ncl, s, 0, rdev); }
     // x = LN_out(x) (+ next layer's first LN fused)                (encoder.py:497)
     { PROF(PC_LAYERNORM);
       if (l + 1 < L)
@@ -814,11 +813,11 @@ int gam_test_gemm(gam_handle* h, int32_t kind, const void* A, const void* A2, in
   {
     PROF(PC_MISC);
     if (kind == kTestGemmPower)
-      rc = launch_gemm_power(&ta, &tw, M, N, K, static_cast<float*>(o), ldo, h->num_sms, s);
+      rc = launch_gemm_power(&ta, &tw, M, N, K, static_cast<float*>(o), ldo, h->gemm_clusters, s);
     else if (A2)
-      rc = launch_gemm_dual_a(&ta, &ta2, n1, &tw, M, N, K, bias, o, ldo, h->num_sms, s, reverse, m_dev);
+      rc = launch_gemm_dual_a(&ta, &ta2, n1, &tw, M, N, K, bias, o, ldo, h->gemm_clusters, s, reverse, m_dev);
     else
-      rc = launch_gemm(kind, &ta, &tw, M, N, K, bias, r, o, ldo, scale, h->num_sms, s, reverse, m_dev);
+      rc = launch_gemm(kind, &ta, &tw, M, N, K, bias, r, o, ldo, scale, h->gemm_clusters, s, reverse, m_dev);
   }
   if (rc) return fail(h, -4, "gemm launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "test_gemm");
@@ -855,8 +854,8 @@ int gam_test_gemm_conv(gam_handle* h, int32_t conv1d, const void* A, const void*
   if (rc) return fail(h, -2, "tensor map encode failed (rc=%d)", rc);
   {
     PROF(PC_MISC);
-    rc = conv1d ? launch_gemm_conv1d(&ta, &tw, B, T_out, C, taps, N, bias, len_out, cu, plen, out, N, f32_out, h->num_sms, s)
-                : launch_gemm_conv(&ta, &tw, B, T_out, C, N, bias, len_out, cu, plen, out, N, h->num_sms, s);
+    rc = conv1d ? launch_gemm_conv1d(&ta, &tw, B, T_out, C, taps, N, bias, len_out, cu, plen, out, N, f32_out, h->gemm_clusters, s)
+                : launch_gemm_conv(&ta, &tw, B, T_out, C, N, bias, len_out, cu, plen, out, N, h->gemm_clusters, s);
   }
   if (rc) return fail(h, -4, "conv gemm launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "test_gemm_conv");

@@ -1,4 +1,5 @@
-// Instantiations and host launchers of the wgmma GEMM (gemm_sm90.cuh: 128 x 256 tiles, one persistent CTA per SM).
+// Instantiations and host launchers of the wgmma GEMM (gemm_sm90.cuh: 128 x 256 tiles, persistent clusters of two CTAs).
+#include <climits>
 #include <cstdlib>
 
 #include "gemm_sm90.cuh"
@@ -10,40 +11,55 @@ namespace {
 
 constexpr int kBN = kG2BN;
 
-// p.num_m_tiles counts 128-row blocks = the kernel's m tiles
+// p.num_m_tiles counts 128-row blocks; the grid is one cluster of kG2Cluster CTAs per co-resident pair of m-blocks
+// (max_clusters: gemm_init's count), each walking the list of tile pairs
 template <int EPI, int AMODE>
-int launch_v2(const CUtensorMap* ta, const CUtensorMap* tw, GemmParams p, int num_sms, cudaStream_t s,
+int launch_v2(const CUtensorMap* ta, const CUtensorMap* tw, GemmParams p, int max_clusters, cudaStream_t s,
               const CUtensorMap* ta2 = nullptr) {
   auto kern = gemm_f16_tn_kernel<EPI, AMODE>;
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
-  const int nctas = tiles < num_sms ? tiles : num_sms;
-  if (nctas <= 0) return 0;
-  return launch_k(kern, dim3(nctas), dim3(kG2Threads), kG2Smem, s, *ta, ta2 ? *ta2 : *ta, *tw, p) == cudaSuccess ? 0 : -2;
+  const int pairs = (p.num_m_tiles + kG2Cluster - 1) / kG2Cluster * p.num_n_tiles;
+  const int nclusters = pairs < max_clusters ? pairs : max_clusters;
+  if (nclusters <= 0) return 0;
+  return launch_k(kern, dim3(nclusters * kG2Cluster), dim3(kG2Threads), kG2Smem, s, *ta, ta2 ? *ta2 : *ta, *tw, p) == cudaSuccess
+             ? 0
+             : -2;
 }
 
+// opt in to the dynamic shared memory and lower *clusters to the number of this instantiation's clusters that fit
+// on the current device at once
 template <int EPI, int AMODE>
-int set_attr() {
-  return cudaFuncSetAttribute(gemm_f16_tn_kernel<EPI, AMODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kG2Smem) == cudaSuccess ? 0 : -1;
+int init_one(int* clusters) {
+  auto kern = gemm_f16_tn_kernel<EPI, AMODE>;
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kG2Smem) != cudaSuccess) return -1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(kG2Cluster);
+  cfg.blockDim = dim3(kG2Threads);
+  cfg.dynamicSmemBytes = kG2Smem;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) return -1;
+  if (n < *clusters) *clusters = n;
+  return 0;
 }
 
 }  // namespace
 
-int gemm_init() {
-  int rc = 0;
-  rc |= set_attr<EPI_BIAS_F16, A_2D>();
-  rc |= set_attr<EPI_BIAS_SILU_F16, A_2D>();
-  rc |= set_attr<EPI_BIAS_GLU_F16, A_2D>();
-  rc |= set_attr<EPI_BIAS_RES_F32, A_2D>();
-  rc |= set_attr<EPI_BIAS_F32, A_2D>();
-  rc |= set_attr<EPI_CONV_RELU_MASK_F16, A_CONV>();
-  rc |= set_attr<EPI_POWER_F32, A_2D>();
-  rc |= set_attr<EPI_CONV_RELU_MASK_F16, A_CONV1D>();
-  rc |= set_attr<EPI_CONV_RELU_MASK_F32, A_CONV1D>();
+int gemm_init(int* max_clusters) {
+  int n = INT_MAX, rc = 0;
+  rc |= init_one<EPI_BIAS_F16, A_2D>(&n);
+  rc |= init_one<EPI_BIAS_SILU_F16, A_2D>(&n);
+  rc |= init_one<EPI_BIAS_GLU_F16, A_2D>(&n);
+  rc |= init_one<EPI_BIAS_RES_F32, A_2D>(&n);
+  rc |= init_one<EPI_BIAS_F32, A_2D>(&n);
+  rc |= init_one<EPI_CONV_RELU_MASK_F16, A_CONV>(&n);
+  rc |= init_one<EPI_POWER_F32, A_2D>(&n);
+  rc |= init_one<EPI_CONV_RELU_MASK_F16, A_CONV1D>(&n);
+  rc |= init_one<EPI_CONV_RELU_MASK_F32, A_CONV1D>(&n);
+  *max_clusters = n;
   return rc;
 }
 
 int launch_gemm(int kind, const CUtensorMap* ta, const CUtensorMap* tw, int M, int N, int K, const float* bias,
-                const float* res, void* out, int ldo, float scale, int num_sms, cudaStream_t s, int reverse, const int* m_dev) {
+                const float* res, void* out, int ldo, float scale, int max_clusters, cudaStream_t s, int reverse, const int* m_dev) {
   if (N % kBN != 0 || K % kGemmBK != 0 || M <= 0) return -1;
   GemmParams p{};
   p.M = M;
@@ -59,11 +75,11 @@ int launch_gemm(int kind, const CUtensorMap* ta, const CUtensorMap* tw, int M, i
   p.scale = scale;
   p.reverse = reverse;
   switch (kind) {
-    case GEMM_BIAS_F16: return launch_v2<EPI_BIAS_F16, A_2D>(ta, tw, p, num_sms, s);
-    case GEMM_BIAS_SILU_F16: return launch_v2<EPI_BIAS_SILU_F16, A_2D>(ta, tw, p, num_sms, s);
-    case GEMM_BIAS_GLU_F16: return launch_v2<EPI_BIAS_GLU_F16, A_2D>(ta, tw, p, num_sms, s);
-    case GEMM_BIAS_RES_F32: return launch_v2<EPI_BIAS_RES_F32, A_2D>(ta, tw, p, num_sms, s);
-    case GEMM_BIAS_F32: return launch_v2<EPI_BIAS_F32, A_2D>(ta, tw, p, num_sms, s);
+    case GEMM_BIAS_F16: return launch_v2<EPI_BIAS_F16, A_2D>(ta, tw, p, max_clusters, s);
+    case GEMM_BIAS_SILU_F16: return launch_v2<EPI_BIAS_SILU_F16, A_2D>(ta, tw, p, max_clusters, s);
+    case GEMM_BIAS_GLU_F16: return launch_v2<EPI_BIAS_GLU_F16, A_2D>(ta, tw, p, max_clusters, s);
+    case GEMM_BIAS_RES_F32: return launch_v2<EPI_BIAS_RES_F32, A_2D>(ta, tw, p, max_clusters, s);
+    case GEMM_BIAS_F32: return launch_v2<EPI_BIAS_F32, A_2D>(ta, tw, p, max_clusters, s);
     default: return -1;
   }
 }
@@ -71,7 +87,7 @@ int launch_gemm(int kind, const CUtensorMap* ta, const CUtensorMap* tw, int M, i
 // D[:, :n1] = A1 W[:n1]^T + b, D[:, n1:] = A2 W[n1:]^T + b  (fp16 out) in ONE launch of the persistent kernel: more tiles
 // per launch = less wave quantisation and one launch less.
 int launch_gemm_dual_a(const CUtensorMap* ta1, const CUtensorMap* ta2, int n1, const CUtensorMap* tw, int M, int N, int K,
-                       const float* bias, void* out, int ldo, int num_sms, cudaStream_t s, int reverse, const int* m_dev) {
+                       const float* bias, void* out, int ldo, int max_clusters, cudaStream_t s, int reverse, const int* m_dev) {
   if (N % kBN != 0 || n1 % kBN != 0 || n1 <= 0 || n1 >= N || K % kGemmBK != 0 || M <= 0) return -1;
   GemmParams p{};
   p.M = M;
@@ -86,11 +102,11 @@ int launch_gemm_dual_a(const CUtensorMap* ta1, const CUtensorMap* ta2, int n1, c
   p.scale = 1.f;
   p.a1_nblks = n1 / kBN;
   p.reverse = reverse;
-  return launch_v2<EPI_BIAS_F16, A_2D>(ta1, tw, p, num_sms, s, ta2);
+  return launch_v2<EPI_BIAS_F16, A_2D>(ta1, tw, p, max_clusters, s, ta2);
 }
 
 int launch_gemm_conv(const CUtensorMap* ta4, const CUtensorMap* tw, int B, int T2, int C, int N, const float* bias,
-                     const int* len2, const int* cu, const int* plen, void* out, int ldo, int num_sms, cudaStream_t s) {
+                     const int* len2, const int* cu, const int* plen, void* out, int ldo, int max_clusters, cudaStream_t s) {
   if (N % kBN != 0 || C % kGemmBK != 0 || (cu != nullptr) != (plen != nullptr)) return -1;
   GemmParams p{};
   p.M = 0;
@@ -110,11 +126,11 @@ int launch_gemm_conv(const CUtensorMap* ta4, const CUtensorMap* tw, int B, int T
   p.out = out;
   p.ldo = ldo;
   p.scale = 1.f;
-  return launch_v2<EPI_CONV_RELU_MASK_F16, A_CONV>(ta4, tw, p, num_sms, s);
+  return launch_v2<EPI_CONV_RELU_MASK_F16, A_CONV>(ta4, tw, p, max_clusters, s);
 }
 
 // power spectrum of a split-precision DFT: D = A W^T with W tiles [128 cos | 128 sin]; out[:, N/2] = re^2 + im^2
-int launch_gemm_power(const CUtensorMap* ta, const CUtensorMap* tw, int M, int N, int K, float* out, int ldo, int num_sms,
+int launch_gemm_power(const CUtensorMap* ta, const CUtensorMap* tw, int M, int N, int K, float* out, int ldo, int max_clusters,
                       cudaStream_t s) {
   if (N % kBN != 0 || K % kGemmBK != 0 || M <= 0) return -1;
   GemmParams p{};
@@ -126,14 +142,14 @@ int launch_gemm_power(const CUtensorMap* ta, const CUtensorMap* tw, int M, int N
   p.out = out;
   p.ldo = ldo;
   p.scale = 1.0f / (2048.0f * 2048.0f * 8.0f * 8.0f);   // frames x 2^11, basis x 2^3 (engine.py DFT_*_SCALE), squared
-  return launch_v2<EPI_POWER_F32, A_2D>(ta, tw, p, num_sms, s);
+  return launch_v2<EPI_POWER_F32, A_2D>(ta, tw, p, max_clusters, s);
 }
 
 // k-tap / stride-2 conv1d over time-major [B, T_in, C_in] as an implicit GEMM (3-D strided TMA), K order (tap, c).
 // out rows = (b, t_out); fp16 (intermediate stage) or fp32 (last stage = encoder input) with ReLU + time mask.
 int launch_gemm_conv1d(const CUtensorMap* ta3, const CUtensorMap* tw, int B, int T_out, int C_in, int taps, int N,
                        const float* bias, const int* len_out, const int* cu, const int* plen, void* out, int ldo, int f32_out,
-                       int num_sms, cudaStream_t s) {
+                       int max_clusters, cudaStream_t s) {
   if (N % kBN != 0 || C_in % kGemmBK != 0 || taps < 1 || (cu != nullptr) != (plen != nullptr)) return -1;
   GemmParams p{};
   p.conv_cu = cu;
@@ -152,8 +168,8 @@ int launch_gemm_conv1d(const CUtensorMap* ta3, const CUtensorMap* tw, int B, int
   p.out = out;
   p.ldo = ldo;
   p.scale = 1.f;
-  return f32_out ? launch_v2<EPI_CONV_RELU_MASK_F32, A_CONV1D>(ta3, tw, p, num_sms, s)
-                 : launch_v2<EPI_CONV_RELU_MASK_F16, A_CONV1D>(ta3, tw, p, num_sms, s);
+  return f32_out ? launch_v2<EPI_CONV_RELU_MASK_F32, A_CONV1D>(ta3, tw, p, max_clusters, s)
+                 : launch_v2<EPI_CONV_RELU_MASK_F16, A_CONV1D>(ta3, tw, p, max_clusters, s);
 }
 
 }  // namespace gam

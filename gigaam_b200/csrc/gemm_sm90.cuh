@@ -1,21 +1,34 @@
 // Warp-specialised wgmma GEMM for sm_90a:  D[M,N] = A[M,K] * W[N,K]^T  (+ fused epilogue)
 //
-// One persistent CTA per SM walks 128 x 256 output tiles.  Warp 0 of the producer warpgroup streams 64-wide k-blocks of
-// A (128 rows) and W (256 rows, two 128-row TMA boxes) into a 4-stage shared-memory ring; the two consumer warpgroups
-// each own 64 rows of the tile and issue wgmma.m64n256k16 with both operands read from shared memory (K-major,
-// SWIZZLE_128B, exactly as TMA wrote them).  A stage goes back to the producer as soon as the wgmma group that read it
-// has retired (one group stays in flight), so the loads of the next tile run under this tile's epilogue.
+// Persistent CTAs, one per SM and paired into clusters (below), walk 128 x 256 output tiles.  Warp 0 of the producer
+// warpgroup streams 64-wide k-blocks of A (128 rows) and W (256 rows, two 128-row TMA boxes) into a 4-stage shared-memory
+// ring; the two consumer warpgroups each own 64 rows of the tile and issue wgmma.m64n256k16 with both operands read from
+// shared memory (K-major, SWIZZLE_128B, exactly as TMA wrote them).  A stage goes back to the producer as soon as the
+// wgmma group that read it has retired (one group stays in flight), so the loads of the next tile run under this tile's
+// epilogue.
 //
 // Accumulators stay in registers (128 fp32 per consumer thread): the epilogue applies bias / residual / activation
 // straight from the wgmma fragment (a thread holds two adjacent columns of two rows per 8-column block; four threads
 // cover 32 contiguous bytes of a row, so every access fills whole 32-byte sectors).
 //
-// Barriers: full[s] (one producer arrival + the TMA bytes), empty[s] (one arrival per consumer warpgroup).
+// Clusters of two CTAs share the weight tile.  The persistent grid walks pairs of tiles, m-blocks 2i and 2i + 1 of one
+// n-block; the CTA of cluster rank r computes m-block 2i + r and loads W rows 128 r .. 128 r + 127 of the n-block with a
+// TMA multicast into the same stage of both CTAs.  Each CTA so fetches 16 KB of A and 16 KB of W per k-block instead of
+// 16 + 32 KB: the L2 -> shared-memory feed, which all SMs share, carries a third less per FLOP.  A pair is skipped only
+// when both its blocks are dead; the phantom second block of an odd block count (and a dead block whose partner is
+// live) still loads (TMA zero-fills rows past the tensor) and still arrives on every barrier, but stores nothing.
+//
+// Barriers: full[s] (one local producer arrival + 48 KB, of which 16 KB come from the peer's multicast and may land
+// before the local expect_tx), empty[s] (one arrival per consumer warpgroup of BOTH CTAs: a stage is reloaded only when
+// neither CTA still reads it, because either producer's multicast writes it in both).  A cluster barrier follows the
+// barrier init and ends the kernel, so no CTA exits while its peer can still write into its shared memory or arrive
+// on its barriers.
 #pragma once
 #include "gemm_params.cuh"
 
 namespace gam {
 
+constexpr int kG2Cluster = 2;   // CTAs per cluster, along M
 constexpr int kG2Threads = 384;
 constexpr int kG2Stages = 4;
 constexpr int kG2BN = 256;
@@ -57,7 +70,7 @@ __device__ __forceinline__ GemmRow gemm_row(const GemmParams& p, int m_rows, int
 }
 
 template <int EPI, int AMODE>
-__global__ void __launch_bounds__(kG2Threads, 1)
+__global__ void __cluster_dims__(kG2Cluster, 1, 1) __launch_bounds__(kG2Threads, 1)
 gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
                    const __grid_constant__ CUtensorMap tmap_w, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -77,18 +90,24 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       num_m_tiles = (m_rows + 127) >> 7;
     }
   }
-  const int num_tiles = num_m_tiles * p.num_n_tiles;
-  // conv modes with packed output: a 128-row block whose first frame lies past the utterance's length produces nothing
-  // and is skipped by both roles (same predicate, same tile list)
+  // both CTAs of a cluster walk the same list of tile pairs; rank r takes m-block 2 * m_pair + r
+  const int crank = static_cast<int>(ptx::cluster_ctarank());
+  const int num_pairs = ((num_m_tiles + 1) >> 1) * p.num_n_tiles;
+  const int cluster_id = blockIdx.x / kG2Cluster, num_clusters = gridDim.x / kG2Cluster;
+  // conv modes with packed output: a 128-row block whose first frame lies past the utterance's length produces nothing;
+  // a pair of two such blocks (or of one and the phantom block past the last) is skipped by every role of both CTAs
+  // (same predicate, same pair list)
   [[maybe_unused]] auto conv_tile_dead = [&](int m_blk) -> bool {
     if constexpr (AMODE == A_2D) {
       return false;
     } else {
       if (p.conv_cu == nullptr) return false;
+      if (m_blk >= num_m_tiles) return true;
       constexpr int kFramesPerBlock = (AMODE == A_CONV) ? 8 : 128;
       return (m_blk % p.conv_tiles_per_utt) * kFramesPerBlock >= __ldg(p.conv_plen + m_blk / p.conv_tiles_per_utt);
     }
   };
+  auto pair_dead = [&](int m_pair) -> bool { return conv_tile_dead(2 * m_pair) && conv_tile_dead(2 * m_pair + 1); };
 
   if (warp_idx == 0 && ptx::elect_one()) {
     ptx::prefetch_tmap(&tmap_a);
@@ -96,11 +115,12 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     ptx::prefetch_tmap(&tmap_w);
     for (int s = 0; s < kG2Stages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 2);   // one arrival per consumer warpgroup
+      ptx::mbar_init(&empty_bar[s], 2 * kG2Cluster);   // one arrival per consumer warpgroup of every CTA in the cluster
     }
     ptx::fence_mbar_init();
   }
-  __syncthreads();
+  __syncwarp();
+  ptx::cluster_sync();   // the peer's barriers are initialised before the first multicast or remote arrival reaches them
 
   if (warp_idx < 4) {
     // ===================================================== TMA producer (warp 0 of warpgroup 0)
@@ -108,11 +128,12 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     if (warp_idx == 0 && ptx::elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int tl = p.reverse ? num_tiles - 1 - tile : tile;
-        const int m_blk = tl / p.num_n_tiles;
-        const int n_blk = tl % p.num_n_tiles;
-        if (conv_tile_dead(m_blk)) continue;
+      for (int pr = cluster_id; pr < num_pairs; pr += num_clusters) {
+        const int pl = p.reverse ? num_pairs - 1 - pr : pr;
+        const int m_pair = pl / p.num_n_tiles;
+        const int n_blk = pl % p.num_n_tiles;
+        if (pair_dead(m_pair)) continue;
+        const int m_blk = 2 * m_pair + crank;
         const CUtensorMap* ta = (p.a1_nblks > 0 && n_blk >= p.a1_nblks) ? &tmap_a2 : &tmap_a;
         [[maybe_unused]] int conv_b = 0, conv_t0 = 0;
         if constexpr (AMODE == A_CONV) {
@@ -140,9 +161,9 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
             const int kt = tap / 3, kf = tap % 3;
             ptx::tma_load_4d(sa, &tmap_a, &full_bar[stage], c0, kf - 1, 2 * conv_t0 + kt - 1, conv_b);
           }
-          uint8_t* sb = smem_b + stage * kG2BBytes;
-          ptx::tma_load_2d(sb, &tmap_w, &full_bar[stage], kb * kGemmBK, n_blk * kG2BN);
-          ptx::tma_load_2d(sb + kG2BBytes / 2, &tmap_w, &full_bar[stage], kb * kGemmBK, n_blk * kG2BN + 128);
+          // this CTA's 128-row half of the W tile, into the same stage of both CTAs
+          ptx::tma_load_2d_multicast(smem_b + stage * kG2BBytes + crank * (kG2BBytes / kG2Cluster), &tmap_w, &full_bar[stage],
+                                     kb * kGemmBK, n_blk * kG2BN + crank * (kG2BN / kG2Cluster), (1u << kG2Cluster) - 1);
           if (++stage == kG2Stages) { stage = 0; phase ^= 1; }
         }
       }
@@ -157,11 +178,17 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     const int cq = 2 * (lane & 3);                                 // column of d[4i] inside 8-column block i
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int tl = p.reverse ? num_tiles - 1 - tile : tile;
-      const int m_blk = tl / p.num_n_tiles;
-      const int n_blk = tl % p.num_n_tiles;
-      if (conv_tile_dead(m_blk)) continue;
+    // a stage is released to the producers of both CTAs: either one's multicast writes it here
+    auto release = [&](int s) {
+      if (wg_leader)
+        for (int c = 0; c < kG2Cluster; ++c) ptx::mbar_arrive_cluster(&empty_bar[s], c);
+    };
+    for (int pr = cluster_id; pr < num_pairs; pr += num_clusters) {
+      const int pl = p.reverse ? num_pairs - 1 - pr : pr;
+      const int m_pair = pl / p.num_n_tiles;
+      const int n_blk = pl % p.num_n_tiles;
+      if (pair_dead(m_pair)) continue;
+      const int m_blk = 2 * m_pair + crank;
 
       float acc[128];
       int prev = -1;
@@ -176,7 +203,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                                     (kb | k) != 0 ? 1u : 0u);
         ptx::wgmma_commit();
         ptx::wgmma_wait<1>();   // the group of the previous k-block has retired: its stage is free
-        if (prev >= 0 && wg_leader) ptx::mbar_arrive(&empty_bar[prev]);
+        if (prev >= 0) release(prev);
         prev = stage;
         if (++stage == kG2Stages) { stage = 0; phase ^= 1; }
       }
@@ -184,7 +211,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       // the accumulators are final only now: keep the compiler from reading them ahead of the wait
 #pragma unroll
       for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(acc[i])::"memory");
-      if (prev >= 0 && wg_leader) ptx::mbar_arrive(&empty_bar[prev]);
+      if (prev >= 0) release(prev);
 
       // ---- epilogue straight from the fragment
 #pragma unroll
@@ -219,31 +246,44 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         } else {
           const float* bsrc = p.bias + n_blk * kG2BN;
           const size_t base = static_cast<size_t>(gr.row) * p.ldo + static_cast<size_t>(n_blk) * kG2BN;
+          // residual loads go out 16 at a time, each batch before its first store: the output may alias the residual
+          // (in place), so the compiler keeps a load that follows a store behind it, and one load per store made every
+          // load of the row wait out a full memory latency of its own
+          constexpr int kBatch = 16;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int c = 8 * i + cq;
-            const float2 bv = __ldg(reinterpret_cast<const float2*>(bsrc + c));
-            float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
+          for (int i0 = 0; i0 < 32; i0 += kBatch) {
+            [[maybe_unused]] float2 res[kBatch];
             if constexpr (EPI == EPI_BIAS_RES_F32) {
-              const float2 r = *reinterpret_cast<const float2*>(p.res + base + c);
-              x0 = fmaf(p.scale, x0, r.x);
-              x1 = fmaf(p.scale, x1, r.y);
+#pragma unroll
+              for (int j = 0; j < kBatch; ++j) res[j] = *reinterpret_cast<const float2*>(p.res + base + 8 * (i0 + j) + cq);
             }
-            if constexpr (EPI == EPI_BIAS_SILU_F16) { x0 = silu_f(x0); x1 = silu_f(x1); }
-            if constexpr (EPI == EPI_CONV_RELU_MASK_F16 || EPI == EPI_CONV_RELU_MASK_F32) {
-              x0 = gr.live ? fmaxf(x0, 0.f) : 0.f;
-              x1 = gr.live ? fmaxf(x1, 0.f) : 0.f;
-            }
-            if constexpr (EPI == EPI_BIAS_RES_F32 || EPI == EPI_BIAS_F32 || EPI == EPI_CONV_RELU_MASK_F32) {
-              *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + base + c) = make_float2(x0, x1);
-            } else {
-              *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(p.out) + base + c) = pack_half2(x0, x1);
+#pragma unroll
+            for (int i = i0; i < i0 + kBatch; ++i) {
+              const int c = 8 * i + cq;
+              const float2 bv = __ldg(reinterpret_cast<const float2*>(bsrc + c));
+              float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
+              if constexpr (EPI == EPI_BIAS_RES_F32) {
+                x0 = fmaf(p.scale, x0, res[i - i0].x);
+                x1 = fmaf(p.scale, x1, res[i - i0].y);
+              }
+              if constexpr (EPI == EPI_BIAS_SILU_F16) { x0 = silu_f(x0); x1 = silu_f(x1); }
+              if constexpr (EPI == EPI_CONV_RELU_MASK_F16 || EPI == EPI_CONV_RELU_MASK_F32) {
+                x0 = gr.live ? fmaxf(x0, 0.f) : 0.f;
+                x1 = gr.live ? fmaxf(x1, 0.f) : 0.f;
+              }
+              if constexpr (EPI == EPI_BIAS_RES_F32 || EPI == EPI_BIAS_F32 || EPI == EPI_CONV_RELU_MASK_F32) {
+                *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + base + c) = make_float2(x0, x1);
+              } else {
+                *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(p.out) + base + c) = pack_half2(x0, x1);
+              }
             }
           }
         }
       }
     }
   }
+  __syncwarp();
+  ptx::cluster_sync();   // the peer may still multicast into this CTA's stages and arrive on its barriers until here
 }
 
 }  // namespace gam

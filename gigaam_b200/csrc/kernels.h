@@ -96,29 +96,29 @@ enum GemmKind : int {
 };
 // 2-D operand GEMM  D[M,N] = A[M,K] W[N,K]^T with fused epilogue `kind`; N % 256 == 0, K % 64 == 0.
 int launch_gemm(int kind, const CUtensorMap* tmap_a, const CUtensorMap* tmap_w, int M, int N, int K, const float* bias,
-                const float* res, void* out, int ldo, float scale, int num_sms, cudaStream_t s, int reverse = 0,
+                const float* res, void* out, int ldo, float scale, int max_clusters, cudaStream_t s, int reverse = 0,
                 const int* m_dev = nullptr);   // m_dev: row count on the device (<= M), see GemmParams::m_dev
 // one launch for two GEMMs that share M, K, W's row space and the output buffer but read different A operands:
 // columns [0, n1) from tmap_a1, [n1, N) from tmap_a2 (bias -> fp16).  
 int launch_gemm_dual_a(const CUtensorMap* tmap_a1, const CUtensorMap* tmap_a2, int n1, const CUtensorMap* tmap_w, int M, int N,
-                       int K, const float* bias, void* out, int ldo, int num_sms, cudaStream_t s, int reverse = 0,
+                       int K, const float* bias, void* out, int ldo, int max_clusters, cudaStream_t s, int reverse = 0,
                        const int* m_dev = nullptr);
 // implicit-GEMM 3x3/s2 conv over channels-last [B,T1,F1,C] (tmap_a 4-D strided), output [rows*16, N] fp16.
 // cu / plen (both or neither): packed output rows, frame (b, t < plen[b]) -> row cu[b] + t; null: row b*T2 + t, all frames
 int launch_gemm_conv(const CUtensorMap* tmap_a4d, const CUtensorMap* tmap_w, int B, int T2, int C, int N, const float* bias,
-                     const int* len2, const int* cu, const int* plen, void* out, int ldo, int num_sms, cudaStream_t s);
+                     const int* len2, const int* cu, const int* plen, void* out, int ldo, int max_clusters, cudaStream_t s);
 // implicit-GEMM k-tap/s2 conv1d over time-major [B,T_in,C_in] (tmap_a 3-D strided); out [B*T_out, N] fp16 or fp32
 int launch_gemm_conv1d(const CUtensorMap* tmap_a3d, const CUtensorMap* tmap_w, int B, int T_out, int C_in, int taps, int N,
                        const float* bias, const int* len_out, const int* cu, const int* plen, void* out, int ldo, int f32_out,
-                       int num_sms, cudaStream_t s);
-int launch_gemm_power(const CUtensorMap* tmap_a, const CUtensorMap* tmap_w, int M, int N, int K, float* out, int ldo, int num_sms,
+                       int max_clusters, cudaStream_t s);
+int launch_gemm_power(const CUtensorMap* tmap_a, const CUtensorMap* tmap_w, int M, int N, int K, float* out, int ldo, int max_clusters,
                       cudaStream_t s);
 // tensor-core front end helpers (frontend.cu)
 void launch_frames_split(const float* wav, int B, int n_samples, int n_frames, const float* window, __half* A, int n_fft, int Kp,
                          int hop, int center, cudaStream_t s);
 void launch_mel_log(const float* P, int ldp, int B, int n_frames, int nbins, const float* fb, const int* mel_lo, const int* mel_hi,
                     float* mel, int n_mels, cudaStream_t s);
-int gemm_init();
+int gemm_init(int* max_clusters);   // per device: also the number of GEMM clusters that fit at once
 // mel [B, F, M] f32 -> time-major fp16 [B, M, F] with frames >= len zeroed (conv1d subsampling input)
 void launch_mel_to_tmajor_f16(const float* mel, const int* len0, __half* out, int B, int F, int M, cudaStream_t s);
 

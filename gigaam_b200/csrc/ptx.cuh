@@ -81,6 +81,16 @@ __device__ __forceinline__ void tma_load_2d(void* smem, const CUtensorMap* m, ui
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+// the same box into the same shared-memory offset of every CTA in `cta_mask`, each completing on its own mbarrier at
+// `bar`'s offset
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
+      "%4}], [%2], %5;" ::"r"(smem_u32(smem)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
@@ -133,6 +143,22 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t cta) {
   uint32_t r;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(cta));
   return r;
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA in the cluster; orders each thread's earlier shared-memory accesses and remote arrivals
+// before what any thread of the cluster does after it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// arrive on the mbarrier at `bar`'s offset in CTA `cta` of the cluster (this CTA included).  Default (.release.cta)
+// semantics: it releases a stage whose wgmma reads have retired (wgmma.wait_group), which needs no fence; the
+// .release.cluster form would add a MEMBAR.GPU that waits for the epilogue's global stores.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(mapa_u32(smem_u32(bar), cta)) : "memory");
 }
 // 16-byte store into another CTA's shared memory whose arrival is counted (complete_tx, 16 bytes) on an mbarrier of
 // that same CTA: the receiver waits on its own barrier, no cluster-wide barrier / fence is involved
