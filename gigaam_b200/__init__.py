@@ -16,6 +16,7 @@ from typing import Dict, Optional, Union
 
 import torch
 
+from .engine import max_encoded_frames_config
 from .model import GigaAM, GigaAMASR
 from .preprocess import load_audio
 from .synthetic import synthetic_audio, synthetic_checkpoint
@@ -45,14 +46,20 @@ def _torch_load_ckpt(path: str) -> Dict:
 
 def load_model(model_name: str, fp16_encoder: bool = True, use_flash: Optional[bool] = False,
                device: Optional[Union[str, torch.device]] = None, download_root: Optional[str] = None, *,
-               checkpoint: Optional[Dict] = None, synthetic: Optional[bool] = None, seed: int = 0
-               ) -> Union[GigaAM, GigaAMASR]:
+               checkpoint: Optional[Dict] = None, synthetic: Optional[bool] = None, seed: int = 0,
+               max_encoded_frames: Optional[int] = None) -> Union[GigaAM, GigaAMASR]:
     """Same positional signature and semantics as gigaam.load_model (gigaam/__init__.py:110-192).
 
     `use_flash` is accepted for compatibility: attention always runs on the project's tensor-core kernel.
     Keyword-only extensions (the boxes this runs on have no network): `checkpoint` = an in-memory
     `{"cfg", "state_dict"}`; `synthetic=True` (or env GIGAAM_B200_SYNTHETIC=1) builds the seeded synthetic
-    checkpoint of that model shape when `<download_root>/<name>.ckpt` does not exist."""
+    checkpoint of that model shape when `<download_root>/<name>.ckpt` does not exist.
+
+    `max_encoded_frames`: longest utterance the model encodes, in encoder frames of 40 ms (like the max shape of a
+    TensorRT profile).  None keeps 768 frames (30.7 s); up to the encoder's `pos_emb_max_len` (5000 frames, up to
+    3 199 999 samples at 16 kHz, for the shipped checkpoints) may be requested.  Longer input is refused with the limit in the
+    message.  A v1 (rel_pos) model's projected position tables take 16 x (2 * max - 1) x 768 fp16 of device memory
+    (38 MB at 768, 246 MB at 5000)."""
     device_obj = _normalize_device(device)
     pack_cache_base = None
     if download_root is None:
@@ -62,7 +69,7 @@ def load_model(model_name: str, fp16_encoder: bool = True, use_flash: Optional[b
         if os.path.isfile(local_path):  # fine-tuned Lightning checkpoint (gigaam/__init__.py:139-156)
             finetuned = _torch_load_ckpt(local_path)
             base = load_model(finetuned["hyper_parameters"]["model_name"], fp16_encoder, use_flash, device_obj,
-                              download_root, synthetic=synthetic, seed=seed)
+                              download_root, synthetic=synthetic, seed=seed, max_encoded_frames=max_encoded_frames)
             sd = {k: v for k, v in finetuned["state_dict"].items() if k.startswith(("preprocessor.", "encoder.", "head."))}
             base.load_state_dict(sd)
             return base
@@ -88,9 +95,11 @@ def load_model(model_name: str, fp16_encoder: bool = True, use_flash: Optional[b
     if "emo" in model_name:
         raise NotImplementedError("GigaAMEmo is outside the accelerated path (SURVEY 2.1 row 6)")
     model = GigaAM(cfg) if "ssl" in model_name else GigaAMASR(cfg)
+    max_encoded_frames_config(max_encoded_frames, model.encoder.cfg["pos_emb_max_len"])   # ValueError before any device work
     model.load_state_dict(checkpoint["state_dict"])
     model = model.eval()
     model.__dict__["_pack_cache_base"] = pack_cache_base    # packed-weight cache next to the checkpoint (model.py)
+    model.__dict__["_max_encoded_frames"] = max_encoded_frames   # kept across the engine rebuilds of .to() / load_state_dict
     if device_obj.type == "cpu":
         logging.warning("gigaam_b200 has no CPU compute path; the model is constructed but forward() needs CUDA")
     if fp16_encoder and device_obj.type != "cpu":

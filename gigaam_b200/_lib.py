@@ -19,7 +19,7 @@ class GamConfig(C.Structure):
         "sample_rate", "n_mels", "n_fft", "win_length", "hop_length", "center",
         "feat_in", "n_layers", "d_model", "n_heads", "d_ff",
         "subsampling", "subs_kernel_size", "conv_kernel_size", "conv_norm", "self_attention", "pos_emb_max_len",
-        "head", "num_classes", "pred_hidden", "joint_hidden", "max_symbols")]
+        "head", "num_classes", "pred_hidden", "joint_hidden", "max_symbols", "max_encoded_frames")]
 
 
 LAYER_FIELDS = (
@@ -29,7 +29,7 @@ LAYER_FIELDS = (
     "ln_ff2_g", "ln_ff2_b", "ff2_w1", "ff2_b1", "ff2_w2", "ff2_b2", "ln_out_g", "ln_out_b",
     "w_qkv_rel", "b_qkv_rel", "pos_proj")
 
-REL_POS_MAX_T = 768   # GAM_REL_POS_MAX_T in include/gigaam_b200.h
+REL_POS_MAX_T = 768   # GAM_REL_POS_MAX_T in include/gigaam_b200.h: the default longest T' (GamConfig.max_encoded_frames = 0)
 
 
 class GamLayerWeights(C.Structure):

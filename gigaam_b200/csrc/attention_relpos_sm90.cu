@@ -4,7 +4,8 @@
 //
 //   qkv : [rows, 4*768] fp16 = [q+u | q+v | k | v], head h at columns h*48 .. h*48+47 of each part; rows are packed
 //         (utterance b = rows cu[b] .. cu[b] + klen[b]; cu == null: the padded [B, T] layout of the unit tests)
-//   pos : [2*kRelPosMaxT-1, 768] fp16 = W_pos pe(r) for r = kRelPosMaxT-1 ... -(kRelPosMaxT-1)   (row = kRelPosMaxT-1-r)
+//   pos : [2*max_t-1, 768] fp16 = W_pos pe(r) for r = max_t-1 ... -(max_t-1)   (row = max_t-1-r); max_t >= T is the
+//         handle's max_encoded_frames (GAM_REL_POS_MAX_T = 768 unless the model asked for more)
 //   out : [rows, 768] fp16
 //
 //   s[i, j] = ((q_i+u) . k_j + (q_i+v) . p_{i-j}) / sqrt(d_k)          p_r = pos row for relative position r
@@ -19,6 +20,11 @@
 // One CTA per (128-query tile, head, utterance), eight warps; single sweep with a running maximum (O rescaled in
 // registers).  One thread issues TMA loads of Q(u), Q(v) and a 2-stage ring of {K, V, 256 window rows} per key block;
 // a stage is refilled once every warp is done with it.
+//
+// Window rows outside the table are zero-filled by TMA.  Past its end (row > 2*max_t-2: r < -(max_t-1)) they only meet
+// keys j > i + max_t - 1 >= T, which are masked.  Before its start (row < 0: r > max_t-1, which happens in the last query
+// tile when max_t is not a multiple of 128, e.g. 5000 = 39*128 + 8) they only meet queries i > j + max_t - 1 >= T, whose
+// rows are never stored.
 #include "kernels.h"
 #include "launch.cuh"
 #include "ptx.cuh"
@@ -27,7 +33,6 @@ namespace gam {
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kMaxKB = 6;                // up to 768 keys
 constexpr int kTile = 128 * 128;         // bytes of a 128-row x 64-column fp16 tile
 constexpr int kStageBytes = 4 * kTile;   // K, V, 2 position tiles
 constexpr int kBdPitch = 33;             // floats per row of a warp's 16 x 32 bounce tile
@@ -41,7 +46,7 @@ struct RelParams {
   __half* out;
   int ld_out;        // d_model
   int dk;
-  int pos_center;    // table row of relative position 0 (= kRelPosMaxT - 1)
+  int pos_center;    // table row of relative position 0 (= max_t - 1)
   float scale_log2;
 };
 
@@ -271,10 +276,10 @@ int launch_ks(const CUtensorMap* tmap_qkv, const CUtensorMap* tmap_pos, const Re
 
 }  // namespace
 
-int launch_attention_relpos(const CUtensorMap* tmap_qkv, const CUtensorMap* tmap_pos, const int* klen, const int* cu, __half* out,
-                            int B, int T, int H, int dk, int d_model, cudaStream_t s) {
+int launch_attention_relpos(const CUtensorMap* tmap_qkv, const CUtensorMap* tmap_pos, int max_t, const int* klen, const int* cu,
+                            __half* out, int B, int T, int H, int dk, int d_model, cudaStream_t s) {
   const int nkb = (T + 127) / 128;
-  if (nkb > kMaxKB || nkb <= 0 || T > kRelPosMaxT || dk % 16 != 0 || dk > 64 || (cu != nullptr && klen == nullptr)) return -1;
+  if (nkb <= 0 || T > max_t || dk % 16 != 0 || dk > 64 || (cu != nullptr && klen == nullptr)) return -1;
   RelParams p;
   p.T = T;
   p.klen = klen;
@@ -282,7 +287,7 @@ int launch_attention_relpos(const CUtensorMap* tmap_qkv, const CUtensorMap* tmap
   p.out = out;
   p.ld_out = d_model;
   p.dk = dk;
-  p.pos_center = kRelPosMaxT - 1;
+  p.pos_center = max_t - 1;
   p.scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(dk));
   switch (dk / 16) {
     case 1: return launch_ks<1>(tmap_qkv, tmap_pos, p, nkb, B, H, s);

@@ -1,4 +1,4 @@
-// Tensor-core attention for the Conformer block (head_dim <= 48, T' <= 768, key-padding mask by length).
+// Tensor-core attention for the Conformer block (head_dim <= 48, any T', key-padding mask by length).
 // Replaces F.scaled_dot_product_attention / flash_attn_varlen in
 // gigaam/encoder.py:258-277 (RotaryPositionMultiHeadAttention) on the q/k/v produced by the fused
 // LN+RoPE -> GEMM kernels.
@@ -13,8 +13,11 @@
 // klen are zeroed in shared memory before P.V: their P is 0, but 0 x (stale inf / NaN bits) would not be.
 //
 // One CTA per (128-query tile, head, utterance), eight warps of 16 query rows each.  A single thread issues TMA loads of
-// the Q tile and of EVERY K / V block of the utterance (at most 6 x 32 KB, each block on its own mbarrier), so the
-// first block's math starts while the rest are still in flight and nothing is ever reloaded.  Per key block of 128:
+// the Q tile and of the first min(nk, 6) K / V blocks of the utterance (32 KB each, every stage on its own mbarrier), so
+// the first block's math starts while the rest are still in flight.  Up to T' = 768 that is every block and nothing is
+// ever reloaded.  Longer utterances run the stages as a ring: key block kb lives in stage kb % 6, and once all eight
+// warps are done with block kb (a __syncthreads after its P.V) thread 0 refills the stage with block kb + 6, which
+// therefore has five blocks of math to land in.  Per key block of 128:
 // S = Q K^T with mma.sync m16n8k16 (operands by ldmatrix from the SWIZZLE_128B tiles TMA wrote), an online softmax on
 // the S fragment in registers, and O += P V with P re-packed from the S fragment as the A operand (no shared-memory
 // round trip).  The softmax:
@@ -28,7 +31,7 @@
 namespace gam {
 namespace {
 
-constexpr int kMaxKB = 6;              // up to 768 keys (30 s segments of the reference's VAD, gigaam/vad_utils.py:85)
+constexpr int kMaxKB = 6;              // K / V stages: 768 keys resident (30 s segments of the reference's VAD, gigaam/vad_utils.py:85)
 constexpr int kTileBytes = 128 * 128;  // 128 rows x 64 fp16
 constexpr int kThreads = 256;
 constexpr float kLazyLog2 = 8.0f;      // the softmax reference point trails the running maximum by at most 2^8
@@ -54,11 +57,11 @@ template <int KS>
 __global__ void __launch_bounds__(kThreads) attention_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int nkb = p.nkb;
+  const int nst = min(p.nkb, kMaxKB);              // stages in shared memory
   uint8_t* sQ = smem;
-  uint8_t* sK = smem + kTileBytes;                  // [nkb]
-  uint8_t* sV = sK + nkb * kTileBytes;              // [nkb]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + nkb * kTileBytes);
+  uint8_t* sK = smem + kTileBytes;                  // [nst]
+  uint8_t* sV = sK + nst * kTileBytes;              // [nst]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + nst * kTileBytes);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;                     // [kMaxKB]
 
@@ -72,18 +75,25 @@ __global__ void __launch_bounds__(kThreads) attention_kernel(const __grid_consta
   const int nk = max(1, kb_valid);                 // key blocks that are multiplied
   const int dmodel = p.ld_out;
 
+  // key block kb -> stage kb % kMaxKB (its completion kb / kMaxKB of kv_full[stage])
+  auto issue_block = [&](int kb, int st) {
+    ptx::mbar_arrive_expect_tx(&kv_full[st], 2 * kTileBytes);
+    ptx::tma_load_2d(sK + st * kTileBytes, &tmap_qkv, &kv_full[st], dmodel + h * p.dk, row0 + kb * 128);
+    ptx::tma_load_2d(sV + st * kTileBytes, &tmap_qkv, &kv_full[st], 2 * dmodel + h * p.dk, row0 + kb * 128);
+  };
   if (threadIdx.x == 0) {
+    const int npre = nk < kMaxKB ? nk : kMaxKB;    // blocks issued up front, one per stage
     ptx::prefetch_tmap(&tmap_qkv);
     ptx::mbar_init(q_full, 1);
-    for (int i = 0; i < nk; ++i) ptx::mbar_init(&kv_full[i], 1);
+#pragma unroll
+    for (int i = 0; i < kMaxKB; ++i)
+      if (i < npre) ptx::mbar_init(&kv_full[i], 1);
     ptx::fence_mbar_init();
     ptx::mbar_arrive_expect_tx(q_full, kTileBytes);
     ptx::tma_load_2d(sQ, &tmap_qkv, q_full, h * p.dk, row0 + qt * 128);
-    for (int kb = 0; kb < nk; ++kb) {
-      ptx::mbar_arrive_expect_tx(&kv_full[kb], 2 * kTileBytes);
-      ptx::tma_load_2d(sK + kb * kTileBytes, &tmap_qkv, &kv_full[kb], dmodel + h * p.dk, row0 + kb * 128);
-      ptx::tma_load_2d(sV + kb * kTileBytes, &tmap_qkv, &kv_full[kb], 2 * dmodel + h * p.dk, row0 + kb * 128);
-    }
+#pragma unroll
+    for (int kb = 0; kb < kMaxKB; ++kb)
+      if (kb < npre) issue_block(kb, kb);
   }
   __syncthreads();
 
@@ -105,10 +115,11 @@ __global__ void __launch_bounds__(kThreads) attention_kernel(const __grid_consta
 
   for (int kb = 0; kb < nk; ++kb) {
     const int nvalid = max(min(klen - kb * 128, 128), 0);
-    ptx::mbar_wait(&kv_full[kb], 0);
-    uint8_t* kt = sK + kb * kTileBytes;
-    uint8_t* vt = sV + kb * kTileBytes;
-    if (nvalid < 128) {   // only the last block (uniform for the CTA): V rows past klen -> 0
+    const int st = kb % kMaxKB;
+    ptx::mbar_wait(&kv_full[st], (kb / kMaxKB) & 1);
+    uint8_t* kt = sK + st * kTileBytes;
+    uint8_t* vt = sV + st * kTileBytes;
+    if (nvalid < 128) {   // only the last block (uniform for the CTA; its stage is never refilled): V rows past klen -> 0
       __syncthreads();
       for (int i = threadIdx.x; i < (128 - nvalid) * 8; i += kThreads)
         reinterpret_cast<uint4*>(vt + nvalid * 128)[i] = make_uint4(0u, 0u, 0u, 0u);
@@ -190,6 +201,11 @@ __global__ void __launch_bounds__(kThreads) attention_kernel(const __grid_consta
         }
       }
     }
+    // every warp is done with this stage (K in S = QK^T, V in P.V): refill it with block kb + kMaxKB
+    if (kb + kMaxKB < nk) {
+      __syncthreads();
+      if (threadIdx.x == 0) issue_block(kb + kMaxKB, st);
+    }
   }
 
   // ---- O / row sum -> fp16 (a row without a valid key: sum 0 -> zeros)
@@ -212,7 +228,7 @@ __global__ void __launch_bounds__(kThreads) attention_kernel(const __grid_consta
 
 template <int KS>
 int launch_ks(const CUtensorMap* tmap_qkv, const AttnParams& p, int B, int H, cudaStream_t s) {
-  const int smem = (1 + 2 * p.nkb) * kTileBytes + kBarBytes + 1024;
+  const int smem = (1 + 2 * (p.nkb < kMaxKB ? p.nkb : kMaxKB)) * kTileBytes + kBarBytes + 1024;
   static PerDeviceOnce attr_once;
   if (attr_once.first() &&
       cudaFuncSetAttribute(attention_kernel<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (1 + 2 * kMaxKB) * kTileBytes + kBarBytes + 1024) !=
@@ -226,7 +242,7 @@ int launch_ks(const CUtensorMap* tmap_qkv, const AttnParams& p, int B, int H, cu
 int launch_attention(const CUtensorMap* tmap_qkv, const int* klen, const int* cu, __half* out, int B, int T, int H, int dk,
                      int d_model, cudaStream_t s) {
   const int nkb = (T + 127) / 128;
-  if (nkb > kMaxKB || nkb <= 0 || dk % 16 != 0 || dk > 48 || (cu != nullptr && klen == nullptr)) return -1;
+  if (nkb <= 0 || dk % 16 != 0 || dk > 48 || (cu != nullptr && klen == nullptr)) return -1;
   AttnParams p;
   p.T = T;
   p.nkb = nkb;

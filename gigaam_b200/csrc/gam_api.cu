@@ -118,6 +118,7 @@ struct gam_handle {
   int64_t lm_F = 0;
   int device = 0;
   int gemm_clusters = 0;   // co-resident clusters of the GEMM kernel (gemm_init)
+  int max_t = GAM_REL_POS_MAX_T;   // longest T' (cfg.max_encoded_frames, 0 = default); rel_pos tables have 2*max_t-1 rows
   int64_t launches = 0;
   void* comm = nullptr;      // ncclComm_t of gam_comm_init
   int comm_rank = 0, comm_nranks = 1;
@@ -315,6 +316,12 @@ int gam_create(const gam_config* cfg, const gam_weights* w, int device, gam_hand
                 c.d_model, c.n_heads);
   if (c.d_ff % 256 != 0 || (c.subsampling == 0 && c.subs_kernel_size != 3)) return fail(h, -10, "unsupported d_ff / subs_kernel_size");
   if (c.win_length != c.n_fft) return fail(h, -10, "win_length != n_fft is not supported");
+  if (c.max_encoded_frames != 0) {
+    if (c.max_encoded_frames < GAM_REL_POS_MAX_T || c.max_encoded_frames > c.pos_emb_max_len)
+      return fail(h, -10, "max_encoded_frames %d outside [%d, pos_emb_max_len = %d]: the rotary and relative-position tables "
+                  "have pos_emb_max_len rows", c.max_encoded_frames, GAM_REL_POS_MAX_T, c.pos_emb_max_len);
+    h->max_t = c.max_encoded_frames;
+  }
   if (cudaSetDevice(device) != cudaSuccess) return fail(h, -11, "cudaSetDevice(%d) failed", device);
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(h, -11, "cudaGetDeviceProperties failed");
@@ -341,7 +348,7 @@ int gam_create(const gam_config* cfg, const gam_weights* w, int device, gam_hand
     } else {
       if (!lw.w_qkv_rel || !lw.b_qkv_rel || !lw.pos_proj) return fail(h, -10, "layer %d: rel_pos weights missing", l);
       rc |= make_tmap_2d_f16(&lm.w_qkv_rel, lw.w_qkv_rel, 4 * d, d, d, 128, 64);
-      rc |= make_tmap_2d_f16(&lm.pos_proj, lw.pos_proj, 2 * kRelPosMaxT - 1, d, d, 128, 64);
+      rc |= make_tmap_2d_f16(&lm.pos_proj, lw.pos_proj, 2 * static_cast<uint64_t>(h->max_t) - 1, d, d, 128, 64);
     }
     rc |= make_tmap_2d_f16(&lm.w_o, lw.w_o, d, d, d, 128, 64);
     rc |= make_tmap_2d_f16(&lm.pw1, lw.pw1_w, 2 * d, d, d, 128, 64);
@@ -464,9 +471,9 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
   Plan* p = get_plan(h, B, M, workspace, workspace_bytes);
   if (!p) return -1;
   if (p->T2 <= 0) return fail(h, -1, "input too short for the subsampling (M=%lld)", (long long)M);
-  if (p->T2 > GAM_REL_POS_MAX_T)
+  if (p->T2 > h->max_t)
     return fail(h, -1, "T'=%d exceeds the attention kernels' %d-frame limit (%.1f s of audio); cut the recording into segments "
-                "(transcribe_longform does)", p->T2, GAM_REL_POS_MAX_T, GAM_REL_POS_MAX_T * 0.04);
+                "(transcribe_longform does)", p->T2, h->max_t, h->max_t * 0.04);
   const int d = c.d_model, R = p->R, ncl = h->gemm_clusters;
   const int L = (n_layers_run < 0 || n_layers_run > c.n_layers) ? c.n_layers : n_layers_run;
   int rc = 0;
@@ -563,7 +570,7 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
       { PROF(PC_GEMM_QKV);
         rc |= launch_gemm(GEMM_BIAS_F16, &p->m_a16, &m.w_qkv_rel, R, 4 * d, d, w.b_qkv_rel, nullptr, p->big16, 4 * d, 1.f, ncl, s, zz, rdev); }
       { PROF(PC_ATTENTION);
-        rc |= launch_attention_relpos(&p->m_qkv4, &m.pos_proj, p->plen, p->cu, p->o16, B, p->T2, c.n_heads, dk, d, s); }
+        rc |= launch_attention_relpos(&p->m_qkv4, &m.pos_proj, h->max_t, p->plen, p->cu, p->o16, B, p->T2, c.n_heads, dk, d, s); }
     }
     { PROF(PC_GEMM_PROJ);
       rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_o16, &m.w_o, R, d, d, w.b_o, p->x, p->x, d, 1.f, ncl, s, zz, rdev); }
@@ -1019,6 +1026,7 @@ int gam_test_mel_to_tmajor(gam_handle* h, const float* mel, const int32_t* len0,
 
 int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void* out, int32_t B, int32_t T, void* stream) {
   const gam_config& c = h->cfg;
+  if (T > h->max_t) return fail(h, -1, "test_attention: T=%d exceeds the handle's %d-frame limit", T, h->max_t);
   CUtensorMap tq;
   const uint64_t d = c.d_model;
   int rc = make_tmap_2d_f16(&tq, qkv, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, 128, 64);
@@ -1036,15 +1044,17 @@ int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void
 int gam_test_attention_relpos(gam_handle* h, const void* qkv, const void* pos, const int32_t* klen, void* out, int32_t B,
                               int32_t T, void* stream) {
   const gam_config& c = h->cfg;
+  if (T > h->max_t) return fail(h, -1, "test_attention_relpos: T=%d exceeds the handle's %d-frame limit", T, h->max_t);
   CUtensorMap tq, tp;
   const uint64_t d = c.d_model;
   int rc = make_tmap_2d_f16(&tq, qkv, static_cast<uint64_t>(B) * T, 4 * d, 4 * d, 128, 64);
-  rc |= make_tmap_2d_f16(&tp, pos, 2 * kRelPosMaxT - 1, d, d, 128, 64);
+  rc |= make_tmap_2d_f16(&tp, pos, 2 * static_cast<uint64_t>(h->max_t) - 1, d, d, 128, 64);
   if (rc) return fail(h, -2, "tensor map encode failed (rc=%d)", rc);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   {
     PROF(PC_ATTENTION);
-    rc = launch_attention_relpos(&tq, &tp, klen, nullptr, static_cast<__half*>(out), B, T, c.n_heads, c.d_model / c.n_heads, c.d_model, s);
+    rc = launch_attention_relpos(&tq, &tp, h->max_t, klen, nullptr, static_cast<__half*>(out), B, T, c.n_heads, c.d_model / c.n_heads,
+                                 c.d_model, s);
   }
   if (rc) return fail(h, -4, "rel_pos attention launch rejected (T=%d, rc=%d)", T, rc);
   GAM_CHECK_LAUNCH(h, "test_attention_relpos");
@@ -1055,15 +1065,17 @@ int gam_test_attention_varlen(gam_handle* h, const void* qkv, const void* pos, c
                               int32_t B, int32_t T, int32_t rows, void* stream) {
   const gam_config& c = h->cfg;
   if (!klen || !cu || rows <= 0) return fail(h, -1, "attention_varlen: klen, cu and rows are required");
+  if (T > h->max_t) return fail(h, -1, "attention_varlen: T=%d exceeds the handle's %d-frame limit", T, h->max_t);
   CUtensorMap tq, tp;
   const uint64_t d = c.d_model, parts = pos ? 4 : 3;
   int rc = make_tmap_2d_f16(&tq, qkv, static_cast<uint64_t>(rows), parts * d, parts * d, 128, 64);
-  if (pos) rc |= make_tmap_2d_f16(&tp, pos, 2 * kRelPosMaxT - 1, d, d, 128, 64);
+  if (pos) rc |= make_tmap_2d_f16(&tp, pos, 2 * static_cast<uint64_t>(h->max_t) - 1, d, d, 128, 64);
   if (rc) return fail(h, -2, "tensor map encode failed (rc=%d)", rc);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   {
     PROF(PC_ATTENTION);
-    rc = pos ? launch_attention_relpos(&tq, &tp, klen, cu, static_cast<__half*>(out), B, T, c.n_heads, c.d_model / c.n_heads, c.d_model, s)
+    rc = pos ? launch_attention_relpos(&tq, &tp, h->max_t, klen, cu, static_cast<__half*>(out), B, T, c.n_heads, c.d_model / c.n_heads,
+                                       c.d_model, s)
              : launch_attention(&tq, klen, cu, static_cast<__half*>(out), B, T, c.n_heads, c.d_model / c.n_heads, c.d_model, s);
   }
   if (rc) return fail(h, -4, "varlen attention launch rejected (T=%d, rc=%d)", T, rc);

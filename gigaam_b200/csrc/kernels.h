@@ -45,11 +45,10 @@ int launch_subsample_conv1(const float* mel, const int* len0, const int* len1, c
 int launch_attention(const CUtensorMap* tmap_qkv, const int* klen, const int* cu, __half* out, int B, int T, int H, int dk,
                      int d_model, cudaStream_t s);
 
-// attention_relpos_sm90.cu: qkv [B*T, 4*d_model] = [q+u | q+v | k | v]; pos = projected position table of
-// 2*kRelPosMaxT-1 rows (GAM_REL_POS_MAX_T in the public header)
-constexpr int kRelPosMaxT = 768;
-int launch_attention_relpos(const CUtensorMap* tmap_qkv, const CUtensorMap* tmap_pos, const int* klen, const int* cu, __half* out,
-                            int B, int T, int H, int dk, int d_model, cudaStream_t s);
+// attention_relpos_sm90.cu: qkv [B*T, 4*d_model] = [q+u | q+v | k | v]; pos = projected position table of 2*max_t-1 rows,
+// row max_t-1-r for relative position r; T <= max_t
+int launch_attention_relpos(const CUtensorMap* tmap_qkv, const CUtensorMap* tmap_pos, int max_t, const int* klen, const int* cu,
+                            __half* out, int B, int T, int H, int dk, int d_model, cudaStream_t s);
 
 // ctc.cu
 void launch_ctc_argmax(const float* enc, const float* W, const float* bias, int* labels, int R, int D, int V1,

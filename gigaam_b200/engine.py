@@ -99,6 +99,20 @@ def pack_rel_pos_qkv(wq: Tensor, bq: Tensor, wk: Tensor, bk: Tensor, wv: Tensor,
     return w, b
 
 
+def max_encoded_frames_config(max_encoded_frames: Optional[int], pos_emb_max_len: int) -> int:
+    """gam_config.max_encoded_frames for a requested limit on T': 0 (the library's default of _lib.REL_POS_MAX_T frames)
+    for None, else the value, which must lie in [REL_POS_MAX_T, pos_emb_max_len] -- the rotary and relative-position
+    tables of the reference have pos_emb_max_len rows (gigaam/encoder.py:312-361)."""
+    if max_encoded_frames is None:
+        return 0
+    if isinstance(max_encoded_frames, bool) or int(max_encoded_frames) != max_encoded_frames:
+        raise ValueError(f"max_encoded_frames must be an integer, got {max_encoded_frames!r}")
+    if not _lib.REL_POS_MAX_T <= max_encoded_frames <= pos_emb_max_len:
+        raise ValueError(f"max_encoded_frames={max_encoded_frames} outside [{_lib.REL_POS_MAX_T}, {pos_emb_max_len}] "
+                         f"(pos_emb_max_len of this encoder)")
+    return int(max_encoded_frames)
+
+
 def rotary_half_tables(dk: int, base: float, max_len: int):
     """cos/sin [max_len, dk/2] of t * base^(-2i/dk) (gigaam/encoder.py:342-355; base = pos_emb_max_len)."""
     inv_freq = 1.0 / (base ** (torch.arange(0, dk, 2).float() / dk))
@@ -142,11 +156,16 @@ class Engine:
 
     PACK_FORMAT = 3   # bump when the packing order / layouts below change
 
-    def __init__(self, cfg: Dict, state_dict: Dict[str, Tensor], device: torch.device, pack_cache: Optional[str] = None):
+    def __init__(self, cfg: Dict, state_dict: Dict[str, Tensor], device: torch.device, pack_cache: Optional[str] = None, *,
+                 max_encoded_frames: Optional[int] = None):
         """`pack_cache`: path of an on-disk cache of the re-laid-out weights (SURVEY 8f-4).  When it exists and matches
         this cfg the load-time re-layout (BN folding, concatenations, permutations, fp16 casts, tables) is skipped and the
         packed tensors are uploaded as stored; otherwise it is written after packing.  Callers key the path by the
-        checkpoint's md5 (load_model does)."""
+        checkpoint's md5 (load_model does).
+
+        `max_encoded_frames`: longest T' (encoder frames, 40 ms each) this engine encodes; None = _lib.REL_POS_MAX_T (768,
+        30.7 s), at most the encoder's pos_emb_max_len (5000 for the shipped checkpoints, just under 200 s).  A rel_pos
+        (v1) model's projected position tables grow with it: 16 x (2 * max - 1) x 768 fp16."""
         if device.type != "cuda":
             raise RuntimeError("gigaam_b200 runs on CUDA (sm_90a, H100) devices only; there is no CPU path")
         if device.index is None:      # an index-less "cuda" means the CURRENT device, not GPU 0
@@ -155,7 +174,13 @@ class Engine:
         self.device = device
         self.cfg = cfg
         self._keep: List[Tensor] = []
-        self._pack_sig = hashlib.sha256(json.dumps([self.PACK_FORMAT, cfg], sort_keys=True, default=str).encode()).hexdigest()
+        enc = cfg["encoder"]
+        gc_max = max_encoded_frames_config(max_encoded_frames, enc["pos_emb_max_len"])
+        self.max_encoded_frames = gc_max or _lib.REL_POS_MAX_T
+        # the limit sizes the rel_pos position tables that go through _dev(): a cache written for one limit must not be
+        # replayed for another
+        self._pack_sig = hashlib.sha256(json.dumps([self.PACK_FORMAT, cfg, self.max_encoded_frames], sort_keys=True,
+                                                   default=str).encode()).hexdigest()
         self._pack_in: Optional[List[Tensor]] = None      # tensors replayed from the cache, in _dev() call order
         self._pack_out: Optional[List[Tensor]] = None     # tensors recorded for the cache
         if pack_cache is not None:
@@ -167,7 +192,7 @@ class Engine:
         self._ws_dec = _WorkspaceCache(self.WS_CACHE)
         self._ws_joint = _WorkspaceCache(self.WS_CACHE)
         self.handle = C.c_void_p()
-        pre, enc = cfg["preprocessor"], cfg["encoder"]
+        pre = cfg["preprocessor"]
         head = cfg.get("head") if isinstance(cfg, dict) else None
         sr = _cfg_get(pre, "sample_rate")
         self.n_fft = _cfg_get(pre, "n_fft", sr // 40)
@@ -182,7 +207,7 @@ class Engine:
         if enc["self_attention_model"] not in ("rotary", "rel_pos"):
             raise ValueError(f"unknown self_attention_model {enc['self_attention_model']!r}")
         self.rel_pos = enc["self_attention_model"] == "rel_pos"
-        self._pos_emb = rel_pos_embedding(_lib.REL_POS_MAX_T, self.d_model).to(device) if self.rel_pos else None
+        self._pos_emb = rel_pos_embedding(self.max_encoded_frames, self.d_model).to(device) if self.rel_pos else None
         self.head_type = 0
         self.num_classes = 0
         self.max_symbols = 10
@@ -195,6 +220,7 @@ class Engine:
         gc.conv_norm = 0 if enc["conv_norm_type"] == "batch_norm" else 1
         gc.self_attention = 1 if self.rel_pos else 0
         gc.pos_emb_max_len = enc["pos_emb_max_len"]
+        gc.max_encoded_frames = gc_max
         gw = _lib.GamWeights()
         sd = state_dict
         self._pack_frontend(gw, sd)
@@ -213,6 +239,7 @@ class Engine:
                 self._pack_rnnt(gw, gc, sd, head)
                 self.max_symbols = int(_cfg_get(cfg.get("decoding", {}), "max_symbols_per_step", 10))
         gc.head, gc.num_classes, gc.max_symbols = self.head_type, self.num_classes, self.max_symbols
+        self.gam_config = gc
         with torch.cuda.device(device):
             rc = self.lib.gam_create(C.byref(gc), C.byref(gw), device.index, C.byref(self.handle))
         _lib.check(self.lib, self.handle, rc, "gam_create")

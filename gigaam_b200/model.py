@@ -82,7 +82,8 @@ class GigaAM(nn.Module):
             if dev.type != "cuda":
                 raise RuntimeError("gigaam_b200 has no CPU path: move the model to a CUDA (sm_90a, H100) device first")
             sd = {k: v for k, v in self.state_dict().items()}
-            eng = Engine(self._engine_cfg(), sd, dev, pack_cache=self._pack_cache_path())
+            eng = Engine(self._engine_cfg(), sd, dev, pack_cache=self._pack_cache_path(),
+                         max_encoded_frames=self.__dict__.get("_max_encoded_frames"))
             self.__dict__["_engine_obj"] = eng
         return eng
 

@@ -46,6 +46,9 @@ typedef struct gam_config {
   int32_t head;        /* 0 = none (ssl), 1 = ctc, 2 = rnnt */
   int32_t num_classes; /* V + 1, blank id = V */
   int32_t pred_hidden, joint_hidden, max_symbols;
+  /* longest T' the handle encodes; 0 = GAM_REL_POS_MAX_T.  Larger values (up to pos_emb_max_len) need a rel_pos model's
+   * pos_proj tables of 2*max_encoded_frames-1 rows */
+  int32_t max_encoded_frames;
 } gam_config;
 
 /* One Conformer layer; all pointers device.  "h" = fp16 row-major [out, in]; "f" = fp32. */
@@ -80,11 +83,11 @@ typedef struct gam_layer_weights {
   /* self_attention == 1 (rel_pos, gigaam/encoder.py:191-228) only, else NULL; w_qk / w_v are then unused */
   const void* w_qkv_rel;  /* h [4d, d] = [linear_q ; linear_q ; linear_k ; linear_v] */
   const float* b_qkv_rel; /* f [4d]    = [b_q + pos_bias_u ; b_q + pos_bias_v ; b_k ; b_v] */
-  const void* pos_proj;   /* h [2*GAM_REL_POS_MAX_T-1, d]: linear_pos(pe(r)), row GAM_REL_POS_MAX_T-1-r for relative
-                           * position r (pe = gigaam/encoder.py:318-326) */
+  const void* pos_proj;   /* h [2*max-1, d]: linear_pos(pe(r)), row max-1-r for relative position r (pe =
+                           * gigaam/encoder.py:318-326), max = gam_config.max_encoded_frames (0: GAM_REL_POS_MAX_T) */
 } gam_layer_weights;
 
-#define GAM_REL_POS_MAX_T 768 /* longest T' the attention kernels serve (6 key blocks of 128 = 30.7 s of audio) */
+#define GAM_REL_POS_MAX_T 768 /* default longest T' (6 key blocks of 128 = 30.7 s of audio); see max_encoded_frames */
 
 typedef struct gam_weights {
   /* front end */
@@ -280,9 +283,10 @@ int gam_test_subsample_conv1(gam_handle* h, const float* mel, const int32_t* len
                              const float* w, const float* bias, void* out, int32_t B, int32_t F, int64_t M, int32_t C, void* stream);
 /* mel f32 [B, F, M] -> time-major f16 [B, M, F], frames >= len0[b] zeroed (conv1d subsampling input) */
 int gam_test_mel_to_tmajor(gam_handle* h, const float* mel, const int32_t* len0, void* out, int32_t B, int32_t F, int64_t M, void* stream);
-/* qkv: f16 [B*T, 3*d_model]; klen i32 [B] or NULL -> out f16 [B*T, d_model] */
+/* qkv: f16 [B*T, 3*d_model]; klen i32 [B] or NULL -> out f16 [B*T, d_model].  T up to the handle's max_encoded_frames */
 int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void* out, int32_t B, int32_t T, void* stream);
-/* rel_pos variant: qkv f16 [B*T, 4*d_model] = [q+u | q+v | k | v]; pos f16 [2*GAM_REL_POS_MAX_T-1, d_model] */
+/* rel_pos variant: qkv f16 [B*T, 4*d_model] = [q+u | q+v | k | v]; pos f16 [2*max-1, d_model] laid out like pos_proj
+ * (max = the handle's max_encoded_frames, GAM_REL_POS_MAX_T by default) */
 int gam_test_attention_relpos(gam_handle* h, const void* qkv, const void* pos, const int32_t* klen, void* out, int32_t B,
                               int32_t T, void* stream);
 /* packed-row (varlen) form of the two calls above, the one gam_encode uses: qkv f16 [rows, 3*d_model] (pos == NULL, rotary)
