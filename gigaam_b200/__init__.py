@@ -4,6 +4,7 @@
     import gigaam_b200 as gigaam
     model = gigaam.load_model("v2_ctc")            # same signature as gigaam.load_model (gigaam/__init__.py:110-116)
     model.transcribe("example.wav")                # -> TranscriptionResult
+    gigaam.load_model("emo").get_probs("example.wav")  # -> {"angry": p, "sad": p, "neutral": p, "positive": p}
     enc, enc_len = model(wav, lengths)              # batched forward
     model.decoding.decode(model.head, enc, enc_len) # -> [(text, ids, frames)]
 """
@@ -17,12 +18,12 @@ from typing import Dict, Optional, Union
 import torch
 
 from .engine import max_encoded_frames_config
-from .model import GigaAM, GigaAMASR
+from .model import GigaAM, GigaAMASR, GigaAMEmo, check_emo_head
 from .preprocess import load_audio
 from .synthetic import synthetic_audio, synthetic_checkpoint
 from .types import LongformTranscriptionResult, Segment, TranscriptionResult, Word
 
-__all__ = ["GigaAM", "GigaAMASR", "load_audio", "load_model", "synthetic_checkpoint", "synthetic_audio",
+__all__ = ["GigaAM", "GigaAMASR", "GigaAMEmo", "load_audio", "load_model", "synthetic_checkpoint", "synthetic_audio",
            "TranscriptionResult", "Word", "Segment", "LongformTranscriptionResult"]
 
 _CACHE_DIR = os.path.expanduser("~/.cache/gigaam")
@@ -47,7 +48,7 @@ def _torch_load_ckpt(path: str) -> Dict:
 def load_model(model_name: str, fp16_encoder: bool = True, use_flash: Optional[bool] = False,
                device: Optional[Union[str, torch.device]] = None, download_root: Optional[str] = None, *,
                checkpoint: Optional[Dict] = None, synthetic: Optional[bool] = None, seed: int = 0,
-               max_encoded_frames: Optional[int] = None) -> Union[GigaAM, GigaAMASR]:
+               max_encoded_frames: Optional[int] = None) -> Union[GigaAM, GigaAMASR, GigaAMEmo]:
     """Same positional signature and semantics as gigaam.load_model (gigaam/__init__.py:110-192).
 
     `use_flash` is accepted for compatibility: attention always runs on the project's tensor-core kernel.
@@ -93,8 +94,10 @@ def load_model(model_name: str, fp16_encoder: bool = True, use_flash: Optional[b
             checkpoint = synthetic_checkpoint(model_name, seed=seed)
     cfg = checkpoint["cfg"]
     if "emo" in model_name:
-        raise NotImplementedError("GigaAMEmo is outside the accelerated path (SURVEY 2.1 row 6)")
-    model = GigaAM(cfg) if "ssl" in model_name else GigaAMASR(cfg)
+        check_emo_head(cfg, checkpoint["state_dict"])     # NotImplementedError before any device work
+        model = GigaAMEmo(cfg)
+    else:
+        model = GigaAM(cfg) if "ssl" in model_name else GigaAMASR(cfg)
     max_encoded_frames_config(max_encoded_frames, model.encoder.cfg["pos_emb_max_len"])   # ValueError before any device work
     model.load_state_dict(checkpoint["state_dict"])
     model = model.eval()

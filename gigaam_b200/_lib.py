@@ -39,7 +39,8 @@ class GamLayerWeights(C.Structure):
 WEIGHT_FIELDS_HEAD = ("window", "dft_cos", "dft_sin", "mel_fb", "sub1_w", "sub1_b", "sub2_w", "sub2_b",
                       "sub_out_w", "sub_out_b", "rope_cos", "rope_sin")
 WEIGHT_FIELDS_TAIL = ("ctc_w", "ctc_b", "rnnt_enc_w", "rnnt_enc_b", "rnnt_emb_gates", "rnnt_whh_t", "rnnt_wp_t",
-                      "rnnt_bp", "rnnt_wo", "rnnt_bo", "c1d_w1", "c1d_b1", "c1d_w2", "c1d_b2", "dft_w", "mel_lo", "mel_hi")
+                      "rnnt_bp", "rnnt_wo", "rnnt_bo", "c1d_w1", "c1d_b1", "c1d_w2", "c1d_b2", "dft_w", "mel_lo", "mel_hi",
+                      "emo_w", "emo_b")
 
 
 class GamWeights(C.Structure):
@@ -55,7 +56,8 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_comm_nccl_version", "gam_gather_hyps", "gam_test_attention_varlen", "gam_ctc_log_probs",
            "gam_rnnt_joint_workspace_bytes", "gam_rnnt_joint", "gam_rnnt_predict", "gam_test_gemm_conv",
            "gam_test_layernorm", "gam_test_ln_rope", "gam_test_ln_out_ln", "gam_test_unpack_rows", "gam_test_dwconv",
-           "gam_test_pack_plan", "gam_test_subsample_conv1", "gam_test_mel_to_tmajor")
+           "gam_test_pack_plan", "gam_test_subsample_conv1", "gam_test_mel_to_tmajor", "gam_emo_workspace_bytes",
+           "gam_emo_head")
 
 
 def lib_path() -> Path:
@@ -115,6 +117,10 @@ def load() -> C.CDLL:
     lib.gam_rnnt_joint.restype = C.c_int
     lib.gam_rnnt_predict.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, c_vp, c_vp, c_vp, c_vp]
     lib.gam_rnnt_predict.restype = C.c_int
+    lib.gam_emo_workspace_bytes.argtypes = [H, i32, i32]
+    lib.gam_emo_workspace_bytes.restype = i64
+    lib.gam_emo_head.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, i64, c_vp, c_vp, c_vp, c_vp]
+    lib.gam_emo_head.restype = C.c_int
     lib.gam_test_gemm.argtypes = [H, i32, c_vp, c_vp, i32, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, i32, C.c_float, i32, c_vp,
                                   c_vp]
     lib.gam_test_gemm_conv.argtypes = [H, i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, i32, i32, i32, i32, c_vp]

@@ -134,7 +134,7 @@ struct gam_handle {
 enum ProfClass : int {
   PC_LOGMEL = 0, PC_SUB_CONV1, PC_GEMM_CONV2, PC_GEMM_SUBOUT, PC_GEMM_FFN_UP, PC_GEMM_FFN_DOWN, PC_GEMM_QKV, PC_GEMM_PROJ,
   PC_GEMM_GLU, PC_LAYERNORM, PC_ATTENTION, PC_DWCONV, PC_CTC_ARGMAX, PC_CTC_COLLAPSE, PC_RNNT_ENCPROJ, PC_RNNT_GREEDY,
-  PC_MISC, PC_CTC_LOG_PROBS, PC_RNNT_JOINT, PC_RNNT_PREDICT, PC_COUNT
+  PC_MISC, PC_CTC_LOG_PROBS, PC_RNNT_JOINT, PC_RNNT_PREDICT, PC_EMO_HEAD, PC_COUNT
 };
 
 struct ProfScope {
@@ -321,6 +321,11 @@ int gam_create(const gam_config* cfg, const gam_weights* w, int device, gam_hand
       return fail(h, -10, "max_encoded_frames %d outside [%d, pos_emb_max_len = %d]: the rotary and relative-position tables "
                   "have pos_emb_max_len rows", c.max_encoded_frames, GAM_REL_POS_MAX_T, c.pos_emb_max_len);
     h->max_t = c.max_encoded_frames;
+  }
+  if (c.head == 3) {
+    if (c.num_classes < 1 || c.num_classes > kPoolMaxClasses)
+      return fail(h, -10, "emo head: %d classes outside [1, %d]", c.num_classes, kPoolMaxClasses);
+    if (!w->emo_w || !w->emo_b) return fail(h, -10, "emo head: emo_w / emo_b missing");
   }
   if (cudaSetDevice(device) != cudaSuccess) return fail(h, -11, "cudaSetDevice(%d) failed", device);
   cudaDeviceProp prop;
@@ -720,6 +725,30 @@ int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const flo
   return 0;
 }
 
+int64_t gam_emo_workspace_bytes(const gam_handle* h, int32_t B, int32_t T) {
+  if (!h || h->cfg.head != 3 || B < 1 || T < 1 || T > 65535 * kPoolChunk) return -1;
+  return static_cast<int64_t>(B) * pool_chunk_count(T) * h->cfg.d_model * 4;
+}
+
+int gam_emo_head(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
+                 int64_t workspace_bytes, float* pooled, float* logits, float* probs, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 3) return fail(h, -1, "emo_head: model has no emo head");
+  if (B < 1 || T < 1 || T > 65535 * kPoolChunk)
+    return fail(h, -1, "emo_head: bad sizes (B=%d, T=%d; 1 <= T <= %d)", B, T, 65535 * kPoolChunk);
+  const int64_t need = gam_emo_workspace_bytes(h, B, T);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "emo_head: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  float* part = static_cast<float*>(workspace);
+  { PROF(PC_EMO_HEAD);
+    launch_pool_chunks(enc, enc_len, B, T, part, s); }
+  { PROF(PC_EMO_HEAD);
+    launch_pooled_head(part, enc_len, B, T, h->w.emo_w, h->w.emo_b, c.num_classes, pooled, logits, probs, s); }
+  GAM_CHECK_LAUNCH(h, "emo_head");
+  return 0;
+}
+
 int gam_group_words(gam_handle* h, const int32_t* ids, const int32_t* frames, const int32_t* counts, int32_t B, int32_t max_out,
                     const uint8_t* token_flags, int32_t V, int32_t max_words, int32_t* word_start, int32_t* word_end,
                     int32_t* word_first_token, int32_t* word_tokens, int32_t* n_words, void* stream) {
@@ -790,7 +819,7 @@ const char* gam_profile_class_name(int32_t cls) {
   static const char* names[PC_COUNT] = {"logmel", "subsample_conv1", "gemm_conv2_implicit", "gemm_subsample_out", "gemm_ffn_up_silu",
                                         "gemm_ffn_down_res", "gemm_qkv", "gemm_proj_res", "gemm_pw1_glu", "layernorm", "attention",
                                         "dwconv_bn_silu", "ctc_head_argmax", "ctc_collapse", "rnnt_enc_proj", "rnnt_greedy", "misc",
-                                        "ctc_log_probs", "rnnt_joint", "rnnt_predict"};
+                                        "ctc_log_probs", "rnnt_joint", "rnnt_predict", "emo_head"};
   return (cls >= 0 && cls < PC_COUNT) ? names[cls] : "?";
 }
 

@@ -66,6 +66,18 @@ void launch_sgemm_tn_bias(const float* A, const float* W, const float* bias, flo
 // the same with W given transposed: Wt[K,N] row-major, N % 4 == 0
 void launch_sgemm_nn_bias(const float* A, const float* Wt, const float* bias, float* C, int M, int N, int K, cudaStream_t s);
 
+// pooled_head.cu: GigaAMEmo's head.  enc f32 [B, T, 768], enc_len i32 [B] or null -> part f32 [B, pool_chunk_count(T), 768]
+// (sums of kPoolChunk frames; chunks past an utterance's length are not written), then pooled [B, 768] = mean over the
+// utterance's frames, logits [B, C] = W pooled + b, probs [B, C] = softmax(logits); any of the three may be null.  Frames pooled
+// for utterance b: enc_len[b] clamped to [0, T], or all T for B == 1 or enc_len == null.  1 <= C <= kPoolMaxClasses,
+// 1 <= B, 1 <= T, pool_chunk_count(T) <= 65535.
+constexpr int kPoolChunk = 32;
+constexpr int kPoolMaxClasses = 256;
+inline int pool_chunk_count(int T) { return (T + kPoolChunk - 1) / kPoolChunk; }
+void launch_pool_chunks(const float* enc, const int* enc_len, int B, int T, float* part, cudaStream_t s);
+void launch_pooled_head(const float* part, const int* enc_len, int B, int T, const float* W, const float* bias, int C, float* pooled,
+                        float* logits, float* probs, cudaStream_t s);
+
 // heads.cu: the heads' forward passes (fp32).  ctc: enc [R, D] -> log_probs [R, V1]
 void launch_ctc_log_probs(const float* enc, const float* W, const float* bias, float* out, int R, int D, int V1, cudaStream_t s);
 // E [B*T, J], P [B*U, J] -> out [B, T, U, V1] = log_softmax(Wo relu(E[b,t] + P[b,u]) + bo); 64-bit offsets.

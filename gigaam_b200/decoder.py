@@ -2,7 +2,8 @@
 the heads' parameters inside their own fused kernels (`gam_ctc_greedy`, `gam_rnnt_greedy`); the heads' public
 methods -- `CTCHead.forward`, `RNNTDecoder.predict` / `forward`, `RNNTJoint.joint` / `forward` -- run the head
 kernels of csrc/heads.cu (`gam_ctc_log_probs`, `gam_rnnt_predict`, `gam_rnnt_joint`) for callers that do their own
-search.  All head arithmetic is fp32, as in the reference (gigaam/__init__.py:188-189)."""
+search.  `Linear` is the emo model's head (a torch.nn.Linear in the reference's checkpoint); it runs `gam_emo_head`.  All
+head arithmetic is fp32, as in the reference (gigaam/__init__.py:188-189)."""
 from __future__ import annotations
 
 from typing import Dict, Optional, Tuple
@@ -107,3 +108,28 @@ class RNNTHead(Bound):
         super()._bind(owner)
         self.decoder._bind(owner)
         self.joint._bind(owner)
+
+
+class Linear(Bound):
+    """The emo model's head: torch.nn.Linear(in_features, out_features) with keys `head.weight` [C, d] and `head.bias` [C]
+    (gigaam/model.py:269, instantiated from the checkpoint's `head._target_`).  Only in_features = d_model with a bias is
+    supported; the model refuses other heads at load time."""
+
+    def __init__(self, in_features: int, out_features: int, bias: bool = True):
+        super().__init__()
+        self.in_features, self.out_features = in_features, out_features
+        build_tree(self, _zeros(synthetic.head_param_list(dict(type="emo", in_features=in_features, out_features=out_features,
+                                                               bias=bias))), "head.")
+
+    def forward(self, x: Tensor) -> Tensor:
+        """x [..., in_features] -> logits [..., out_features] (x W^T + b, fp32).  Runs the pooled-head kernel with one frame
+        per row, whose mean is the row itself."""
+        eng = self._engine()
+        x = _on_device(x, eng, torch.float32)
+        if x.shape[-1] != self.in_features:
+            raise ValueError(f"Linear: last dimension {x.shape[-1]} != in_features {self.in_features}")
+        rows = x.reshape(-1, 1, self.in_features).contiguous()
+        if rows.shape[0] == 0:
+            return torch.empty((*x.shape[:-1], self.out_features), dtype=torch.float32, device=eng.device)
+        _, logits, _ = eng.emo_head(rows, None)
+        return logits.reshape(*x.shape[:-1], self.out_features)

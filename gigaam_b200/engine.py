@@ -191,6 +191,7 @@ class Engine:
         self._ws_mel = _WorkspaceCache(self.WS_CACHE)
         self._ws_dec = _WorkspaceCache(self.WS_CACHE)
         self._ws_joint = _WorkspaceCache(self.WS_CACHE)
+        self._ws_emo = _WorkspaceCache(self.WS_CACHE)
         self.handle = C.c_void_p()
         pre = cfg["preprocessor"]
         head = cfg.get("head") if isinstance(cfg, dict) else None
@@ -235,6 +236,11 @@ class Engine:
                 self.head_type, self.num_classes = 1, head["num_classes"]
                 gw.ctc_w = self._dev(sd["head.decoder_layers.0.weight"].reshape(self.num_classes, -1).float())
                 gw.ctc_b = self._dev(sd["head.decoder_layers.0.bias"].float())
+            elif head["type"] == "emo":
+                # Linear(d, C) over the mean of the encoder frames (gigaam/model.py:272-293), fp32 like the reference's head
+                self.head_type, self.num_classes = 3, head["out_features"]
+                gw.emo_w = self._dev(sd["head.weight"].float())
+                gw.emo_b = self._dev(sd["head.bias"].float())
             else:
                 self._pack_rnnt(gw, gc, sd, head)
                 self.max_symbols = int(_cfg_get(cfg.get("decoding", {}), "max_symbols_per_step", 10))
@@ -427,7 +433,7 @@ class Engine:
         pointers it baked stay valid however many other shapes pass through the engine afterwards."""
         M = self.logmel_frames(N)
         T = self.encoded_frames(M)
-        held = [self._ws_mel.peek((B, N)), self._ws_enc.peek((B, M)), self._ws_dec.peek((B, T))]
+        held = [self._ws_mel.peek((B, N)), self._ws_enc.peek((B, M)), self._ws_dec.peek((B, T)), self._ws_emo.peek((B, T))]
         return [t for t in held if t is not None]
 
     def logmel(self, wav: Tensor, fused: bool = False) -> Tensor:
@@ -562,6 +568,30 @@ class Engine:
                                            self._stream())
         _lib.check(self.lib, self.handle, rc, "gam_rnnt_predict")
         return g, h1, c1
+
+    def emo_head(self, enc_btd: Tensor, enc_len: Optional[Tensor]) -> Tuple[Tensor, Tensor, Tensor]:
+        """enc [B, T, d] f32 contiguous, len [B] or None (all T frames) -> (pooled [B, d], logits [B, C], probs [B, C]) f32
+        (gam_emo_head: GigaAMEmo's mean + head + softmax, gigaam/model.py:272-293).  Utterance b pools len[b] frames, except
+        that a batch of ONE pools all T.  The workspace is cached per (B, T) like the decode workspace."""
+        assert enc_btd.is_cuda and enc_btd.dtype == torch.float32 and enc_btd.is_contiguous() and enc_btd.dim() == 3
+        if self.head_type != 3:
+            raise RuntimeError("model has no emo head")
+        B, T, _ = enc_btd.shape
+        nbytes = int(self.lib.gam_emo_workspace_bytes(self.handle, B, T))
+        if nbytes < 0:
+            raise ValueError(f"emo_head: bad sizes B={B}, T={T}")
+        if enc_len is not None:
+            enc_len = enc_len.to(device=self.device, dtype=torch.int32).contiguous()
+        pooled = torch.empty((B, self.d_model), dtype=torch.float32, device=self.device)
+        logits = torch.empty((B, self.num_classes), dtype=torch.float32, device=self.device)
+        probs = torch.empty((B, self.num_classes), dtype=torch.float32, device=self.device)
+        ws = self._ws_emo.get((B, T), nbytes, self.device)
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_emo_head(self.handle, enc_btd.data_ptr(), None if enc_len is None else enc_len.data_ptr(), B, T,
+                                       ws.data_ptr(), ws.numel(), pooled.data_ptr(), logits.data_ptr(), probs.data_ptr(),
+                                       self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_emo_head")
+        return pooled, logits, probs
 
     def group_words(self, ids: Tensor, frames: Tensor, counts: Tensor, token_flags: Tensor):
         """Device word grouping (gam_group_words): -> (word_start, word_end, word_first, word_ntok [B, max_out] i32, n_words [B] i32)."""

@@ -1,6 +1,7 @@
 """Model wrappers with the reference's surface (gigaam/model.py:16-140): GigaAM.forward / embed_audio /
-prepare_wav, GigaAMASR.transcribe / _decode, `_device`, `_dtype`, `cfg`, `preprocessor`, `encoder`, `head`,
-`decoding`.  Hydra `_target_` instantiation is replaced by a small registry keyed on the same class names."""
+prepare_wav, GigaAMASR.transcribe / _decode, GigaAMEmo.get_probs / forward_for_export (:262-293), `_device`, `_dtype`,
+`cfg`, `preprocessor`, `encoder`, `head`, `decoding`, `id2name`.  Hydra `_target_` instantiation is replaced by a small
+registry keyed on the same class names."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Tuple, Union
@@ -9,8 +10,8 @@ import numpy as np
 import torch
 from torch import Tensor, nn
 
-from .decoder import CTCHead, RNNTHead
-from .decoding import CTCGreedyDecoding, RNNTGreedyDecoding
+from .decoder import CTCHead, Linear, RNNTHead
+from .decoding import CTCGreedyDecoding, RNNTGreedyDecoding, _as_btd
 from .encoder import ConformerEncoder
 from .engine import Engine
 from .preprocess import SAMPLE_RATE, FeatureExtractor, load_audio
@@ -21,7 +22,10 @@ LONGFORM_THRESHOLD = 25 * SAMPLE_RATE
 _REGISTRY = {
     "FeatureExtractor": FeatureExtractor, "ConformerEncoder": ConformerEncoder, "CTCHead": CTCHead,
     "RNNTHead": RNNTHead, "CTCGreedyDecoding": CTCGreedyDecoding, "RNNTGreedyDecoding": RNNTGreedyDecoding,
+    "Linear": Linear,
 }
+
+EMO_MAX_CLASSES = 256   # kPoolMaxClasses of csrc/kernels.h: one class per thread of the softmax
 
 
 def _plain(obj):
@@ -46,16 +50,46 @@ def instantiate(section: Dict, default_cls: str):
 
 def normalize_cfg(cfg) -> Dict:
     """Bring a checkpoint cfg (Hydra-style, with `_target_`s) or a synthetic cfg to one plain-dict shape:
-    sections `preprocessor`, `encoder`, optional `head` (with `type`) and `decoding`."""
+    sections `preprocessor`, `encoder`, optional `head` (with `type`) and `decoding`.  A cfg with `id2name` is an emo model
+    (gigaam/model.py:270): its head's type is "emo"."""
     c = _plain(cfg)
     out = dict(c)
     head = c.get("head")
     if head is not None and "type" not in head:
         tgt = str(head.get("_target_", ""))
         head = dict(head)
-        head["type"] = "rnnt" if "RNNT" in tgt or "decoder" in head else "ctc"
+        if "id2name" in c:
+            head["type"] = "emo"
+        else:
+            head["type"] = "rnnt" if "RNNT" in tgt or "decoder" in head else "ctc"
         out["head"] = head
     return out
+
+
+def check_emo_head(cfg, state_dict: Optional[Dict[str, Tensor]] = None) -> None:
+    """Refuse an emo head this build cannot run, before any device work.  The supported head is a `_target_` whose last
+    component is `Linear`, with in_features = d_model, a bias and out_features = len(id2name) in [1, 256] (the reference's
+    checkpoint names a class outside `gigaam` that maps [B, 768] -> [B, C]).  Nothing else is approximated: the
+    NotImplementedError names the target and the checkpoint's `head.*` keys, so that the head to add is known."""
+    c = _plain(cfg)
+    head, names = dict(c.get("head") or {}), list(c.get("id2name") or [])
+    target = head.get("_target_")
+    d_model = c["encoder"]["d_model"]
+    keys = sorted(k for k in (state_dict or {}) if k.startswith("head."))
+    why = None
+    if target is None or str(target).rsplit(".", 1)[-1] != "Linear":
+        why = "only a Linear head (torch.nn.Linear) is supported"
+    elif head.get("in_features") != d_model:
+        why = f"in_features {head.get('in_features')} != d_model {d_model}"
+    elif not head.get("bias", True):
+        why = "a Linear head without bias is not supported"
+    elif head.get("out_features") != len(names):
+        why = f"out_features {head.get('out_features')} != len(id2name) {len(names)}"
+    elif not 1 <= len(names) <= EMO_MAX_CLASSES:
+        why = f"{len(names)} classes outside [1, {EMO_MAX_CLASSES}]"
+    if why is not None:
+        raise NotImplementedError(f"emo head {target!r} is not supported: {why}"
+                                  + (f" (checkpoint head keys: {keys})" if state_dict is not None else ""))
 
 
 class GigaAM(nn.Module):
@@ -225,3 +259,39 @@ class GigaAMASR(GigaAM):
         """Batched entry (the path eval.py / transcribe_longform drive: model(wav, len) -> decoding.decode)."""
         encoded, encoded_len = self.forward(wav, lengths)
         return [t for t, _, _ in self.decoding.decode(self.head, encoded, encoded_len)]
+
+
+class GigaAMEmo(GigaAM):
+    """Giga Acoustic Model for Emotion Recognition -- drop-in for gigaam.model.GigaAMEmo (gigaam/model.py:262-293).
+
+    Frames pooled for utterance b: n_b = encoded_len[b], except that a batch of ONE pools all T' frames (the rule of the
+    encoder's packed rows, DESIGN §3.1).  `get_probs` is thus exactly the reference's (it pools every frame of its one
+    utterance), and every utterance's probabilities are independent of the batch it is in.  The reference's
+    `forward_for_export` averages over the padded T' instead; on ragged batches of more than one utterance its answer
+    depends on the padding, and this build's padded frames are zeros, so that answer is not reproduced.  An utterance with
+    n_b = 0 gives a NaN row (the mean of an empty set)."""
+
+    def __init__(self, cfg):
+        super().__init__(cfg)
+        check_emo_head(cfg)
+        self.head = instantiate(self._ncfg["head"], "Linear")
+        self.head._bind(self)
+        self.id2name = self._ncfg["id2name"]
+
+    def _pooled_probs(self, encoded: Tensor, encoded_len: Optional[Tensor]) -> Tensor:
+        _, _, probs = self._get_engine().emo_head(_as_btd(encoded), encoded_len)
+        return probs
+
+    @torch.inference_mode()
+    def get_probs(self, wav_file) -> Dict[str, float]:
+        """gigaam/model.py:272-285: {class name: probability} of one recording (a path or an in-memory waveform)."""
+        wav, length = self.prepare_wav(wav_file)
+        encoded, encoded_len = self.forward(wav, length)
+        probs = self._pooled_probs(encoded, encoded_len)[0].tolist()
+        return {self.id2name[i]: probs[i] for i in range(len(self.id2name))}
+
+    def forward_for_export(self, features: Tensor, feature_lengths: Tensor) -> Tensor:
+        """log-mel [B, F, M], lengths [B] -> probs [B, C] (gigaam/model.py:287-293), pooling each utterance over its own
+        encoded_len frames (all T' for a batch of one; see the class docstring)."""
+        encoded, encoded_len = self.encoder(features, feature_lengths)
+        return self._pooled_probs(encoded, encoded_len)

@@ -49,6 +49,8 @@ def _encoder_cfg(version: str) -> Dict:
 
 def model_cfg(model_name: str, n_layers: int | None = None) -> Dict:
     """Plain-dict cfg for a model name of the reference's registry (gigaam/__init__.py:28-41)."""
+    if model_name == "emo":
+        return emo_cfg(n_layers)
     version = model_name.split("_")[0]
     if version not in ("v1", "v2", "v3"):
         raise ValueError(f"unknown synthetic model {model_name!r}")
@@ -78,6 +80,32 @@ def model_cfg(model_name: str, n_layers: int | None = None) -> Dict:
     return cfg
 
 
+EMO_CLASSES = ["angry", "sad", "neutral", "positive"]   # order of the reference's expected values (tests/test_loading.py:13-18)
+
+
+def emo_cfg(n_layers: int | None = None, num_classes: int | None = None) -> Dict:
+    """GigaAM-Emo: a v1 encoder (README.md:56) and a Linear(768, C) head over the mean of the encoder frames
+    (gigaam/model.py:262-293).  The head's `_target_` is RECALLED to be torch.nn.Linear: the reference instantiates a class
+    outside `gigaam` that maps [B, 768] -> [B, C].  `num_classes` (default 4) replaces the class list by C generic names."""
+    enc = _encoder_cfg("v1")
+    if n_layers is not None:
+        enc["n_layers"] = n_layers
+    names = list(EMO_CLASSES) if num_classes is None else [f"class_{i}" for i in range(num_classes)]
+    return dict(model_name="emo", sample_rate=SAMPLE_RATE, preprocessor=dict(sample_rate=SAMPLE_RATE, features=64), encoder=enc,
+                head={"_target_": "torch.nn.Linear", "in_features": enc["d_model"], "out_features": len(names), "bias": True},
+                id2name=names)
+
+
+def head_kind(head) -> Optional[str]:
+    """"ctc" | "rnnt" | "emo" for a head section (a normalized cfg carries `type`; the emo head is named by its
+    `_target_`), None without a head."""
+    if not head:
+        return None
+    if "type" in head:
+        return head["type"]
+    return "emo" if str(head.get("_target_", "")).rsplit(".", 1)[-1] == "Linear" else None
+
+
 # ------------------------------------------------------------------------------------------ front-end buffers
 def hann_window(n: int) -> torch.Tensor:
     """Periodic Hann window (torch.hann_window default, used by torchaudio Spectrogram)."""
@@ -104,7 +132,7 @@ def mel_filterbank(n_freqs: int, n_mels: int, sample_rate: int) -> torch.Tensor:
 # network's logits depend on the frame and on the prediction-network state so that greedy decoding is not a
 # degenerate all-or-nothing function of the blank bias.
 _GAIN = {"head.joint.joint_net.1.weight": 6.0, "head.joint.enc.weight": 20.0, "head.joint.pred.weight": 10.0,
-         "head.decoder_layers.0.weight": 4.0}
+         "head.decoder_layers.0.weight": 4.0, "head.weight": 4.0}
 
 def _param_list(cfg: Dict) -> List[Tuple[str, Tuple[int, ...], str, float]]:
     """(key, shape, kind, fan_in) in a fixed order.  kind: w|b|ln_w|ln_b|bn_mean|bn_var|int|emb"""
@@ -179,17 +207,23 @@ def encoder_param_list(enc: Dict) -> List[Tuple[str, Tuple[int, ...], str, float
 
 
 def head_param_list(head) -> List[Tuple[str, Tuple[int, ...], str, float]]:
-    """state_dict entries of gigaam.decoder.CTCHead / RNNTHead (keys carry the "head." prefix)."""
+    """state_dict entries of gigaam.decoder.CTCHead / RNNTHead and of the emo model's torch.nn.Linear head (keys carry
+    the "head." prefix)."""
     out: List[Tuple[str, Tuple[int, ...], str, float]] = []
 
     def lin(prefix: str, o: int, i: int):
         out.append((prefix + ".weight", (o, i), "w", i))
         out.append((prefix + ".bias", (o,), "b", i))
 
-    if head and head["type"] == "ctc":
+    kind = head_kind(head)
+    if kind == "emo":
+        out.append(("head.weight", (head["out_features"], head["in_features"]), "w", head["in_features"]))
+        if head.get("bias", True):
+            out.append(("head.bias", (head["out_features"],), "b", head["in_features"]))
+    elif kind == "ctc":
         out.append(("head.decoder_layers.0.weight", (head["num_classes"], head["feat_in"], 1), "w", head["feat_in"]))
         out.append(("head.decoder_layers.0.bias", (head["num_classes"],), "b", head["feat_in"]))
-    elif head and head["type"] == "rnnt":
+    elif kind == "rnnt":
         dc, jt = head["decoder"], head["joint"]
         H = dc["pred_hidden"]
         out.append(("head.decoder.embed.weight", (dc["num_classes"], H), "emb", 0))
@@ -238,7 +272,7 @@ def synthetic_state_dict(cfg: Dict, seed: int = 0, rnnt_calibration: Optional[Di
             raise AssertionError(kind)
         sd[key] = t * _GAIN.get(key, 1.0)
     head = cfg.get("head")
-    if head and head["type"] == "rnnt":
+    if head_kind(head) == "rnnt":
         cal = _rnnt_calibration(cfg["model_name"]) if rnnt_calibration is None else rnnt_calibration
         if "enc_null" in cal:       # rows orthogonal to the directions in which utterance means differ (oracle/calibrate_rnnt.py)
             null = torch.as_tensor(cal["enc_null"])

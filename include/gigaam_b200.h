@@ -13,6 +13,7 @@
  *   gam_ctc_log_probs <- gigaam/decoder.py:18-21      CTCHead.forward
  *   gam_rnnt_joint    <- gigaam/decoder.py:41-47      RNNTJoint.joint
  *   gam_rnnt_predict  <- gigaam/decoder.py:85-102     RNNTDecoder.predict (1-layer LSTM)
+ *   gam_emo_head      <- gigaam/model.py:272-293      GigaAMEmo pooling + head + softmax
  *
  * Conventions: every pointer marked "device" is a CUDA device pointer on the handle's device; the
  * library never allocates or frees caller memory in the hot calls (the caller passes a workspace of
@@ -43,8 +44,8 @@ typedef struct gam_config {
   int32_t self_attention;   /* 0 = rotary, 1 = rel_pos (v1 checkpoints) */
   int32_t pos_emb_max_len;
   /* head (gigaam/decoder.py) */
-  int32_t head;        /* 0 = none (ssl), 1 = ctc, 2 = rnnt */
-  int32_t num_classes; /* V + 1, blank id = V */
+  int32_t head;        /* 0 = none (ssl), 1 = ctc, 2 = rnnt, 3 = emo (pooled Linear head, gam_emo_head) */
+  int32_t num_classes; /* V + 1, blank id = V; emo: the C classes, 1 <= C <= 256 */
   int32_t pred_hidden, joint_hidden, max_symbols;
   /* longest T' the handle encodes; 0 = GAM_REL_POS_MAX_T.  Larger values (up to pos_emb_max_len) need a rel_pos model's
    * pos_proj tables of 2*max_encoded_frames-1 rows */
@@ -128,6 +129,9 @@ typedef struct gam_weights {
   const void* dft_w;
   const int32_t* mel_lo; /* i32 [n_mels] first bin with a non-zero weight */
   const int32_t* mel_hi; /* i32 [n_mels] one past the last */
+  /* emotion head (head == 3), fp32: Linear(d_model, C) applied to the mean of the encoder frames */
+  const float* emo_w; /* f [C, d]  head.weight */
+  const float* emo_b; /* f [C]     head.bias */
 } gam_weights;
 
 int gam_create(const gam_config* cfg, const gam_weights* w, int device, gam_handle** out);
@@ -201,6 +205,20 @@ int gam_rnnt_joint(gam_handle* h, const float* enc, const float* dec, int32_t B,
  * succeeds.  One launch per step. */
 int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g, float* h1,
                      float* c1, void* stream);
+
+/* Emotion head  <- gigaam/model.py:272-293 (GigaAMEmo.get_probs / forward_for_export): the mean of utterance b's encoder
+ * frames, logits = W mean + b, probs = softmax(logits), fp32.
+ *   enc: device f32 [B, T, d_model] (gam_encode's layout); enc_len: device i32 [B], or NULL = all T frames.
+ *   Frames pooled for utterance b: n_b = enc_len[b] clamped to [0, T], except that a batch of ONE pools all T frames (the
+ *   rule of gam_encode's packed rows, and what the reference's get_probs does).  Frames t >= n_b are never read; n_b = 0
+ *   gives a NaN row.  Utterance b's summation order depends on n_b alone, so its outputs are bit-identical in any batch.
+ *   -> pooled: device f32 [B, d_model], logits / probs: device f32 [B, C]; each may be NULL (not written).
+ * workspace: device scratch of at least gam_emo_workspace_bytes(B, T) bytes.  Two launches, no host synchronisation:
+ * capturable in a CUDA graph.  gam_emo_workspace_bytes returns -1 for a handle without an emo head or bad sizes
+ * (B < 1, T < 1 or T > 2 097 120). */
+int64_t gam_emo_workspace_bytes(const gam_handle* h, int32_t B, int32_t T);
+int gam_emo_head(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
+                 int64_t workspace_bytes, float* pooled, float* logits, float* probs, void* stream);
 
 /* ---- the one multi-GPU exchange of the path (SURVEY 8e): utterances are sharded over ranks, one process per GPU, and the
  * device-resident hypotheses are all-gathered ONCE over NCCL (NVLink / NVSwitch) when the batch was actually split.
