@@ -27,6 +27,9 @@ struct LogmelSmem {
   // phase 2: power [kFr][kBinsPad] (aliases s/d) ; out tile [64 mel][kFr+1]
 };
 
+// mel.clamp_(1e-9, 1e9) of gigaam/preprocess.py:50: NaN stays NaN (fmaxf alone would turn it into 1e-9, i.e. silence)
+__device__ __forceinline__ float clamp_power(float v) { return v != v ? v : fminf(fmaxf(v, 1e-9f), 1e9f); }
+
 __global__ void __launch_bounds__(256) logmel_kernel(const float* __restrict__ wav, int n_samples, int n_frames,
                                                      const float* __restrict__ window, const float* __restrict__ tcos,
                                                      const float* __restrict__ tsin, const float* __restrict__ fb,
@@ -136,7 +139,7 @@ __global__ void __launch_bounds__(256) logmel_kernel(const float* __restrict__ w
       for (int i = 0; i < 16; ++i) acc[i] = fmaf(pw[(fg * 16 + i) * PP + k], w, acc[i]);
     }
 #pragma unroll
-    for (int i = 0; i < 16; ++i) ot[m * (kFr + 1) + fg * 16 + i] = logf(fminf(fmaxf(acc[i], 1e-9f), 1e9f));
+    for (int i = 0; i < 16; ++i) ot[m * (kFr + 1) + fg * 16 + i] = logf(clamp_power(acc[i]));
   }
   __syncthreads();
   for (int i = threadIdx.x; i < n_mels * kFr; i += blockDim.x) {
@@ -233,21 +236,28 @@ __global__ void __launch_bounds__(256) mel_to_tmajor_f16_kernel(const float* __r
 // fp16 (hi, lo) pairs and the three significant products are folded into ONE GEMM by concatenating along K:
 //   A' = [ f_hi | f_lo | f_hi ],   W' = [ d_hi | d_hi | d_lo ]     (K = 3 * Kp, ~22-bit effective mantissas)
 // run on the wgmma GEMM kernel with the power epilogue (re^2 + im^2).  This kernel builds A'.
+// Frame f is stored as x.w.2^e_f: e_f = 11 moves the fp16 `lo` halves of quiet samples out of the subnormal range, and
+// is lowered for a frame whose max |x.w| (NaN ignored) would round a `hi` to inf, so that max |x.w.2^e_f| < 2^15.
+// e_f goes to fexp[f]; the GEMM epilogue undoes 2^22 and mel_log_kernel the remaining 2^(2 e_f - 22).
+constexpr int kSplitIters = 8;   // Kp / 64: gam_logmel_tc admits n_fft / 2 + 1 <= 256 bins, so Kp <= 512
 __global__ void __launch_bounds__(256) frames_split_kernel(const float* __restrict__ wav, int n_samples, int n_frames,
-                                                           const float* __restrict__ window, __half* __restrict__ A, int n_fft,
-                                                           int Kp, int hop, int center) {
+                                                           const float* __restrict__ window, __half* __restrict__ A,
+                                                           int* __restrict__ fexp, int n_fft, int Kp, int hop, int center) {
   const int b = blockIdx.y;
   const int frame = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (frame >= n_frames) return;
   const int lane = threadIdx.x & 31;
   const float* x = wav + static_cast<size_t>(b) * n_samples;
-  __half* row = A + (static_cast<size_t>(b) * n_frames + frame) * (3 * Kp);
+  const size_t f = static_cast<size_t>(b) * n_frames + frame;
+  __half* row = A + f * (3 * Kp);
   const int half = n_fft / 2;
-  for (int i2 = lane; i2 < Kp / 2; i2 += 32) {
-    float v[2];
+  float v[kSplitIters][2];
+  float amax = 0.f;
+#pragma unroll
+  for (int it = 0; it < kSplitIters; ++it) {
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      const int j = 2 * i2 + e;
+      const int j = 2 * (lane + 32 * it) + e;
       float s = 0.f;
       if (j < n_fft) {
         int idx = frame * hop + j - (center ? half : 0);
@@ -255,14 +265,26 @@ __global__ void __launch_bounds__(256) frames_split_kernel(const float* __restri
           if (idx < 0) idx = -idx;
           if (idx >= n_samples) idx = 2 * (n_samples - 1) - idx;
         }
-        // x 2^11: moves the fp16 `lo` halves of quiet samples out of the subnormal range (undone in the power epilogue)
-        if (idx >= 0 && idx < n_samples) s = x[idx] * __ldg(window + j) * 2048.0f;
+        if (idx >= 0 && idx < n_samples) s = x[idx] * __ldg(window + j);
       }
-      v[e] = s;
+      v[it][e] = s;
+      amax = fmaxf(amax, fabsf(s));
     }
-    const __half2 hi = __floats2half2_rn(v[0], v[1]);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  // fp16 rounds [65520, inf) to inf; 2^11 is kept whenever it fits, so frames with |x| <= 1 are stored as before
+  const int ef = amax * 2048.0f < 65520.0f ? 11 : max(14 - ilogbf(amax), -126);
+  const float scale = __int_as_float((127 + ef) << 23);
+  if (lane == 0) fexp[f] = ef;
+#pragma unroll
+  for (int it = 0; it < kSplitIters; ++it) {
+    const int i2 = lane + 32 * it;
+    if (i2 >= Kp / 2) break;
+    const float v0 = v[it][0] * scale, v1 = v[it][1] * scale;
+    const __half2 hi = __floats2half2_rn(v0, v1);
     const float2 hf = __half22float2(hi);
-    const __half2 lo = __floats2half2_rn(v[0] - hf.x, v[1] - hf.y);
+    const __half2 lo = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
     reinterpret_cast<__half2*>(row)[i2] = hi;
     reinterpret_cast<__half2*>(row + Kp)[i2] = lo;
     reinterpret_cast<__half2*>(row + 2 * Kp)[i2] = hi;
@@ -271,9 +293,10 @@ __global__ void __launch_bounds__(256) frames_split_kernel(const float* __restri
 
 // power spectrum [F, ldp] f32 -> log(clamp(P . fb)) written as [B, n_mels, M] (gigaam/preprocess.py:49-50, MelScale).
 // block = 32 frames of one utterance; thread = (mel m, 8 frames); the HTK triangles are sparse, so each mel filter only
-// walks its own bin range [lo_m, hi_m).
-__global__ void __launch_bounds__(256) mel_log_kernel(const float* __restrict__ P, int ldp, int n_frames, int nbins,
-                                                      const float* __restrict__ fb, const int* __restrict__ mel_lo,
+// walks its own bin range [lo_m, hi_m).  Frame f's power rows carry 2^(2 fexp[f] - 22) (frames_split_kernel), undone exactly
+// before the clamp.
+__global__ void __launch_bounds__(256) mel_log_kernel(const float* __restrict__ P, const int* __restrict__ fexp, int ldp, int n_frames,
+                                                      int nbins, const float* __restrict__ fb, const int* __restrict__ mel_lo,
                                                       const int* __restrict__ mel_hi, float* __restrict__ mel, int n_mels) {
   __shared__ float ps[32][257];
   __shared__ float ot[64][33];
@@ -298,7 +321,10 @@ __global__ void __launch_bounds__(256) mel_log_kernel(const float* __restrict__ 
       for (int i = 0; i < 8; ++i) acc[i] = fmaf(ps[fg * 8 + i][k], w, acc[i]);
     }
 #pragma unroll
-    for (int i = 0; i < 8; ++i) ot[m][fg * 8 + i] = logf(fminf(fmaxf(acc[i], 1e-9f), 1e9f));
+    for (int i = 0; i < 8; ++i) {
+      const int fr = min(f0 + fg * 8 + i, n_frames - 1);   // rows past the last frame are zero and never stored
+      ot[m][fg * 8 + i] = logf(clamp_power(ldexpf(acc[i], 22 - 2 * __ldg(fexp + static_cast<size_t>(b) * n_frames + fr))));
+    }
   }
   __syncthreads();
   for (int i = threadIdx.x; i < n_mels * 32; i += 256) {
@@ -309,16 +335,20 @@ __global__ void __launch_bounds__(256) mel_log_kernel(const float* __restrict__ 
 
 }  // namespace
 
-void launch_frames_split(const float* wav, int B, int n_samples, int n_frames, const float* window, __half* A, int n_fft, int Kp,
-                         int hop, int center, cudaStream_t s) {
+int launch_frames_split(const float* wav, int B, int n_samples, int n_frames, const float* window, __half* A, int* fexp, int n_fft,
+                        int Kp, int hop, int center, cudaStream_t s) {
+  if (Kp > 64 * kSplitIters || n_fft > Kp) return -1;
   dim3 grid((n_frames + 7) / 8, B);
-  frames_split_kernel<<<grid, 256, 0, s>>>(wav, n_samples, n_frames, window, A, n_fft, Kp, hop, center);
+  frames_split_kernel<<<grid, 256, 0, s>>>(wav, n_samples, n_frames, window, A, fexp, n_fft, Kp, hop, center);
+  return 0;
 }
 
-void launch_mel_log(const float* P, int ldp, int B, int n_frames, int nbins, const float* fb, const int* mel_lo, const int* mel_hi,
-                    float* mel, int n_mels, cudaStream_t s) {
+int launch_mel_log(const float* P, const int* fexp, int ldp, int B, int n_frames, int nbins, const float* fb, const int* mel_lo,
+                   const int* mel_hi, float* mel, int n_mels, cudaStream_t s) {
+  if (n_mels > 64 || nbins > 256 || ldp != 256) return -1;   // ot[64][33], ps[32][257] and its float4 row loads
   dim3 grid((n_frames + 31) / 32, B);
-  mel_log_kernel<<<grid, 256, 0, s>>>(P, ldp, n_frames, nbins, fb, mel_lo, mel_hi, mel, n_mels);
+  mel_log_kernel<<<grid, 256, 0, s>>>(P, fexp, ldp, n_frames, nbins, fb, mel_lo, mel_hi, mel, n_mels);
+  return 0;
 }
 
 void launch_mel_to_tmajor_f16(const float* mel, const int* len0, __half* out, int B, int F, int M, cudaStream_t s) {

@@ -316,6 +316,7 @@ int gam_create(const gam_config* cfg, const gam_weights* w, int device, gam_hand
                 c.d_model, c.n_heads);
   if (c.d_ff % 256 != 0 || (c.subsampling == 0 && c.subs_kernel_size != 3)) return fail(h, -10, "unsupported d_ff / subs_kernel_size");
   if (c.win_length != c.n_fft) return fail(h, -10, "win_length != n_fft is not supported");
+  if (c.n_mels < 1 || c.n_mels > 64) return fail(h, -10, "n_mels %d outside [1, 64]: the log-mel kernels hold 64 mel rows", c.n_mels);
   if (c.max_encoded_frames != 0) {
     if (c.max_encoded_frames < GAM_REL_POS_MAX_T || c.max_encoded_frames > c.pos_emb_max_len)
       return fail(h, -10, "max_encoded_frames %d outside [%d, pos_emb_max_len = %d]: the rotary and relative-position tables "
@@ -425,9 +426,10 @@ int gam_logmel(gam_handle* h, const float* wav, int32_t B, int64_t n_samples, fl
 
 static inline int logmel_kp(const gam_config& c) { return (c.n_fft + 63) / 64 * 64; }
 
+// workspace of gam_logmel_tc: A' f16 [F, 3 Kp] | power f32 [F, 256] | per-frame exponent i32 [F] (frames_split_kernel)
 int64_t gam_logmel_workspace_bytes(const gam_handle* h, int32_t B, int64_t n_samples) {
   const int64_t F = static_cast<int64_t>(B) * gam_logmel_frames(h, n_samples);
-  return align_up(F * 3 * logmel_kp(h->cfg) * 2, 1024) + align_up(F * 256 * 4, 1024) + 2048;
+  return align_up(F * 3 * logmel_kp(h->cfg) * 2, 1024) + align_up(F * 256 * 4, 1024) + align_up(F * 4, 1024) + 2048;
 }
 
 int gam_logmel_tc(gam_handle* h, const float* wav, int32_t B, int64_t n_samples, float* mel, void* workspace,
@@ -446,6 +448,7 @@ int gam_logmel_tc(gam_handle* h, const float* wav, int32_t B, int64_t n_samples,
   ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws) + 1023) & ~uintptr_t(1023));
   __half* A = reinterpret_cast<__half*>(ws);
   float* P = reinterpret_cast<float*>(ws + align_up(F * 3 * Kp * 2, 1024));
+  int* fexp = reinterpret_cast<int*>(ws + align_up(F * 3 * Kp * 2, 1024) + align_up(F * 256 * 4, 1024));
   if (h->lm_A != A || h->lm_F != F) {
     if (make_tmap_2d_f16(&h->m_lm_a, A, F, 3 * Kp, 3 * Kp, 128, 64) != 0) return fail(h, -2, "logmel_tc: tensor map encode failed");
     h->lm_A = A;
@@ -453,7 +456,9 @@ int gam_logmel_tc(gam_handle* h, const float* wav, int32_t B, int64_t n_samples,
   }
   {
     PROF(PC_LOGMEL);
-    launch_frames_split(wav, B, static_cast<int>(n_samples), static_cast<int>(M), h->w.window, A, c.n_fft, Kp, c.hop_length, c.center, s);
+    if (launch_frames_split(wav, B, static_cast<int>(n_samples), static_cast<int>(M), h->w.window, A, fexp, c.n_fft, Kp, c.hop_length,
+                            c.center, s) != 0)
+      return fail(h, -4, "logmel_tc: frame split launch rejected (n_fft %d)", c.n_fft);
   }
   {
     PROF(PC_LOGMEL);
@@ -462,7 +467,9 @@ int gam_logmel_tc(gam_handle* h, const float* wav, int32_t B, int64_t n_samples,
   }
   {
     PROF(PC_LOGMEL);
-    launch_mel_log(P, 256, B, static_cast<int>(M), c.n_fft / 2 + 1, h->w.mel_fb, h->w.mel_lo, h->w.mel_hi, mel, c.n_mels, s);
+    if (launch_mel_log(P, fexp, 256, B, static_cast<int>(M), c.n_fft / 2 + 1, h->w.mel_fb, h->w.mel_lo, h->w.mel_hi, mel, c.n_mels,
+                       s) != 0)
+      return fail(h, -4, "logmel_tc: mel projection launch rejected (n_mels %d)", c.n_mels);
   }
   GAM_CHECK_LAUNCH(h, "logmel_tc");
   return 0;
@@ -1050,6 +1057,42 @@ int gam_test_mel_to_tmajor(gam_handle* h, const float* mel, const int32_t* len0,
   { PROF(PC_SUB_CONV1);
     launch_mel_to_tmajor_f16(mel, len0, static_cast<__half*>(out), B, F, static_cast<int>(M), s); }
   GAM_CHECK_LAUNCH(h, "test_mel_to_tmajor");
+  return 0;
+}
+
+int gam_test_frames_split(gam_handle* h, const float* wav, int32_t B, int64_t n_samples, void* A, int32_t* fexp, void* stream) {
+  const gam_config& c = h->cfg;
+  if (!wav || !A || !fexp || B <= 0 || B > 65535 || n_samples > INT32_MAX)
+    return fail(h, -1, "test_frames_split: wav, A, fexp and B in [1, 65535] are required");
+  const int64_t M = gam_logmel_frames(h, n_samples);
+  if (M <= 0) return fail(h, -1, "waveform too short: %lld samples", (long long)n_samples);
+  if (c.center && n_samples <= c.n_fft / 2) return fail(h, -1, "reflect padding needs more than n_fft/2 samples");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  { PROF(PC_LOGMEL);
+    rc = launch_frames_split(wav, B, static_cast<int>(n_samples), static_cast<int>(M), h->w.window, static_cast<__half*>(A), fexp,
+                             c.n_fft, logmel_kp(c), c.hop_length, c.center, s); }
+  if (rc) return fail(h, -4, "test_frames_split: launch rejected (n_fft %d)", c.n_fft);
+  GAM_CHECK_LAUNCH(h, "test_frames_split");
+  return 0;
+}
+
+int gam_test_mel_log(gam_handle* h, const float* P, const int32_t* fexp, int32_t B, int32_t M, int32_t nbins, const float* fb,
+                     const int32_t* mel_lo, const int32_t* mel_hi, int32_t n_mels, float* mel, void* stream) {
+  if (!P || !fexp || !fb || !mel_lo || !mel_hi || !mel || B <= 0 || B > 65535 || M <= 0)
+    return fail(h, -1, "test_mel_log: P, fexp, fb, mel_lo, mel_hi, mel and B in [1, 65535], M > 0 are required");
+  if (nbins <= 0 || nbins > 256 || n_mels <= 0 || n_mels > 64)
+    return fail(h, -1, "test_mel_log: nbins %d (<= 256) or n_mels %d (<= 64) unsupported", nbins, n_mels);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<int> lo, hi;
+  if (dev_ints(mel_lo, n_mels, lo, s) || dev_ints(mel_hi, n_mels, hi, s)) return fail(h, -3, "test_mel_log: cannot read mel_lo / mel_hi");
+  for (int m = 0; m < n_mels; ++m)
+    if (lo[m] < 0 || hi[m] > nbins) return fail(h, -1, "test_mel_log: mel %d bin range [%d, %d) outside [0, %d)", m, lo[m], hi[m], nbins);
+  int rc;
+  { PROF(PC_LOGMEL);
+    rc = launch_mel_log(P, fexp, 256, B, M, nbins, fb, mel_lo, mel_hi, mel, n_mels, s); }
+  if (rc) return fail(h, -4, "test_mel_log: launch rejected");
+  GAM_CHECK_LAUNCH(h, "test_mel_log");
   return 0;
 }
 

@@ -125,10 +125,11 @@ int launch_gemm_conv1d(const CUtensorMap* tmap_a3d, const CUtensorMap* tmap_w, i
 int launch_gemm_power(const CUtensorMap* tmap_a, const CUtensorMap* tmap_w, int M, int N, int K, float* out, int ldo, int max_clusters,
                       cudaStream_t s);
 // tensor-core front end helpers (frontend.cu)
-void launch_frames_split(const float* wav, int B, int n_samples, int n_frames, const float* window, __half* A, int n_fft, int Kp,
-                         int hop, int center, cudaStream_t s);
-void launch_mel_log(const float* P, int ldp, int B, int n_frames, int nbins, const float* fb, const int* mel_lo, const int* mel_hi,
-                    float* mel, int n_mels, cudaStream_t s);
+// tensor-core log-mel stages; fexp: i32 per frame, the power of two frame f is stored at (see frames_split_kernel)
+int launch_frames_split(const float* wav, int B, int n_samples, int n_frames, const float* window, __half* A, int* fexp, int n_fft,
+                        int Kp, int hop, int center, cudaStream_t s);
+int launch_mel_log(const float* P, const int* fexp, int ldp, int B, int n_frames, int nbins, const float* fb, const int* mel_lo,
+                   const int* mel_hi, float* mel, int n_mels, cudaStream_t s);
 int gemm_init(int* max_clusters);   // per device: also the number of GEMM clusters that fit at once
 // mel [B, F, M] f32 -> time-major fp16 [B, M, F] with frames >= len zeroed (conv1d subsampling input)
 void launch_mel_to_tmajor_f16(const float* mel, const int* len0, __half* out, int B, int F, int M, cudaStream_t s);

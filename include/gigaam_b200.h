@@ -301,6 +301,14 @@ int gam_test_subsample_conv1(gam_handle* h, const float* mel, const int32_t* len
                              const float* w, const float* bias, void* out, int32_t B, int32_t F, int64_t M, int32_t C, void* stream);
 /* mel f32 [B, F, M] -> time-major f16 [B, M, F], frames >= len0[b] zeroed (conv1d subsampling input) */
 int gam_test_mel_to_tmajor(gam_handle* h, const float* mel, const int32_t* len0, void* out, int32_t B, int32_t F, int64_t M, void* stream);
+/* gam_logmel_tc's first stage: wav f32 [B, n_samples] -> A' f16 [B * M, 3 Kp] = [hi | lo | hi] of the windowed frames x 2^e_f
+ * (Kp = n_fft rounded up to 64, columns [n_fft, Kp) zero) and fexp i32 [B * M] = e_f (11 unless a hi would overflow) */
+int gam_test_frames_split(gam_handle* h, const float* wav, int32_t B, int64_t n_samples, void* A, int32_t* fexp, void* stream);
+/* gam_logmel_tc's last stage: power rows P f32 [B * M, 256] of frames stored at 2^fexp (device i32 [B * M]) -> mel f32
+ * [B, n_mels, M] = log(clamp(2^(22 - 2 fexp) P[:, :nbins] . fb, 1e-9, 1e9)), NaN kept; fb f32 [nbins, n_mels], mel m summed over
+ * bins [mel_lo[m], mel_hi[m]) only (device i32 [n_mels]) */
+int gam_test_mel_log(gam_handle* h, const float* P, const int32_t* fexp, int32_t B, int32_t M, int32_t nbins, const float* fb,
+                     const int32_t* mel_lo, const int32_t* mel_hi, int32_t n_mels, float* mel, void* stream);
 /* qkv: f16 [B*T, 3*d_model]; klen i32 [B] or NULL -> out f16 [B*T, d_model].  T up to the handle's max_encoded_frames */
 int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void* out, int32_t B, int32_t T, void* stream);
 /* rel_pos variant: qkv f16 [B*T, 4*d_model] = [q+u | q+v | k | v]; pos f16 [2*max-1, d_model] laid out like pos_proj
