@@ -57,7 +57,7 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_rnnt_joint_workspace_bytes", "gam_rnnt_joint", "gam_rnnt_predict", "gam_test_gemm_conv",
            "gam_test_layernorm", "gam_test_ln_rope", "gam_test_ln_out_ln", "gam_test_unpack_rows", "gam_test_dwconv",
            "gam_test_pack_plan", "gam_test_subsample_conv1", "gam_test_mel_to_tmajor", "gam_emo_workspace_bytes",
-           "gam_emo_head", "gam_test_frames_split", "gam_test_mel_log")
+           "gam_emo_head", "gam_test_frames_split", "gam_test_mel_log", "gam_test_rnnt_greedy")
 
 
 def lib_path() -> Path:
@@ -135,9 +135,11 @@ def load() -> C.CDLL:
     lib.gam_test_mel_to_tmajor.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, i64, c_vp]
     lib.gam_test_frames_split.argtypes = [H, c_vp, i32, i64, c_vp, c_vp, c_vp]
     lib.gam_test_mel_log.argtypes = [H, c_vp, c_vp, i32, i32, i32, c_vp, c_vp, c_vp, i32, c_vp, c_vp]
+    lib.gam_test_rnnt_greedy.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, i32, c_vp, c_vp, c_vp,
+                                         c_vp, c_vp]
     for fn in (lib.gam_test_gemm, lib.gam_test_gemm_conv, lib.gam_test_layernorm, lib.gam_test_ln_rope, lib.gam_test_ln_out_ln,
                lib.gam_test_unpack_rows, lib.gam_test_dwconv, lib.gam_test_pack_plan, lib.gam_test_subsample_conv1,
-               lib.gam_test_mel_to_tmajor, lib.gam_test_frames_split, lib.gam_test_mel_log):
+               lib.gam_test_mel_to_tmajor, lib.gam_test_frames_split, lib.gam_test_mel_log, lib.gam_test_rnnt_greedy):
         fn.restype = C.c_int
     lib.gam_test_attention.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, c_vp]
     lib.gam_test_attention.restype = C.c_int

@@ -1,6 +1,8 @@
 // CTC head + greedy decode (gigaam/decoder.py:7-21, gigaam/decoding.py:56-96).
 //   (1) head + argmax: labels[b,t] = argmax_c (W[c,:] . enc[b,t,:] + bias[c]) in fp32 - log_softmax is
-//       argmax-invariant so it is never computed.  First maximal index wins (torch.argmax).
+//       argmax-invariant on finite rows so it is never computed.  The label is torch's log_softmax(row).argmax(-1):
+//       on a row whose maximum is finite the first maximal index (torch.argmax); if any logit is NaN or +inf, or none
+//       exceeds -inf, 0 (log_softmax makes such a row all NaN).  Always in [0, V1).
 //   (2) collapse: keep (l != blank) && (t == 0 || l != l_{t-1}) && (t < len); one warp per utterance,
 //       ballot + popc prefix compaction, results resident on device:
 //       ids[B,T], frames[B,T], counts[B] (int32).
@@ -63,7 +65,13 @@ __global__ void __launch_bounds__(kRows * kGroups) ctc_argmax_kernel(const float
       const int cls = c0 + cg * kCG + c;
       if (cls < V1) {
         const float v = acc[c] + __ldg(bias + cls);
-        if (v > best) { best = v; best_i = cls; }       // ascending classes, strict >: first maximal index wins
+        // ascending classes, strict >: first maximal index wins; a NaN or +inf logit becomes (+inf, -1), the
+        // "non-finite seen" mark that no later logit replaces and that wins the merge below
+        if (!(v <= best)) {
+          const bool bad = !(v < INFINITY);
+          best = bad ? INFINITY : v;
+          best_i = bad ? -1 : cls;
+        }
       }
     }
   }
@@ -79,7 +87,7 @@ __global__ void __launch_bounds__(kRows * kGroups) ctc_argmax_kernel(const float
       const int i = best_c[g][r];
       if (v > best || (v == best && i < best_i)) { best = v; best_i = i; }
     }
-    labels[row0 + r] = best_i;
+    labels[row0 + r] = best_i < 0 ? 0 : best_i;   // NaN or +inf in any group -> 0
   }
 }
 

@@ -651,7 +651,7 @@ int gam_rnnt_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int
   PROF(PC_RNNT_GREEDY);
   const int rc = launch_rnnt_greedy_cluster(encproj, enc_len, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h->w.rnnt_wp_t, h->w.rnnt_bp,
                                             h->w.rnnt_wo, h->w.rnnt_bo, B, T, c.pred_hidden, c.num_classes, c.num_classes - 1,
-                                            c.max_symbols, max_out, ids, frames, counts, s);
+                                            c.max_symbols, max_out, ids, frames, counts, nullptr, s);
   if (rc > 0)
     return fail(h, -1, "rnnt: the greedy kernel is specialised for pred_hidden = joint_hidden = 320 and needs 16-CTA clusters "
                 "(pred_hidden %d)", c.pred_hidden);
@@ -1093,6 +1093,25 @@ int gam_test_mel_log(gam_handle* h, const float* P, const int32_t* fexp, int32_t
     rc = launch_mel_log(P, fexp, 256, B, M, nbins, fb, mel_lo, mel_hi, mel, n_mels, s); }
   if (rc) return fail(h, -4, "test_mel_log: launch rejected");
   GAM_CHECK_LAUNCH(h, "test_mel_log");
+  return 0;
+}
+
+int gam_test_rnnt_greedy(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,
+                         const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
+                         int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts, int32_t* plan,
+                         void* stream) {
+  if (!encproj || !len || !emb_gates || !whhT || !wpT || !bp || !wo || !bo || !ids || !frames || !counts)
+    return fail(h, -1, "test_rnnt_greedy: every operand is required");
+  if (B <= 0 || T <= 0 || V1 < 2 || max_symbols <= 0 || max_out <= 0)
+    return fail(h, -1, "test_rnnt_greedy: bad sizes (B=%d, T=%d, V1=%d, max_symbols=%d, max_out=%d)", B, T, V1, max_symbols, max_out);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  { PROF(PC_RNNT_GREEDY);
+    rc = launch_rnnt_greedy_cluster(encproj, len, emb_gates, whhT, wpT, bp, wo, bo, B, T, 320, V1, V1 - 1, max_symbols, max_out, ids,
+                                    frames, counts, plan, s); }
+  if (rc > 0) return fail(h, -1, "test_rnnt_greedy: 16-CTA clusters cannot be scheduled on this device");
+  if (rc < 0) return fail(h, -4, "test_rnnt_greedy: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, "test_rnnt_greedy");
   return 0;
 }
 

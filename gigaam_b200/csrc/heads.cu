@@ -140,7 +140,9 @@ __global__ void __launch_bounds__(kJThreads) rnnt_joint_kernel(const float* __re
       const int64_t bu = bt / T * U + row % U;
       const float4 e = *reinterpret_cast<const float4*>(E + bt * J + k4);
       const float4 p = *reinterpret_cast<const float4*>(P + bu * J + k4);
-      z = make_float4(fmaxf(e.x + p.x, 0.f), fmaxf(e.y + p.y, 0.f), fmaxf(e.z + p.z, 0.f), fmaxf(e.w + p.w, 0.f));
+      // relu that keeps NaN, as torch.relu (fmaxf(NaN, 0) = 0 would give finite log-probs where the reference has NaN)
+      const float z0 = e.x + p.x, z1 = e.y + p.y, z2 = e.z + p.z, z3 = e.w + p.w;
+      z = make_float4(z0 < 0.f ? 0.f : z0, z1 < 0.f ? 0.f : z1, z2 < 0.f ? 0.f : z2, z3 < 0.f ? 0.f : z3);
     }
     A_s[(k4 + 0) * kJLd + m] = z.x;
     A_s[(k4 + 1) * kJLd + m] = z.y;

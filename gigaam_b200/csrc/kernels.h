@@ -90,10 +90,11 @@ int launch_rnnt_joint(const float* E, const float* P, const float* Wo, const flo
 void launch_lstm_step(const int64_t* x, int U, int u, int V1, const float* emb_gates, const float* whh_t, const float* h_in,
                       int64_t h_pitch, const float* c_in, float* g, float* h_out, float* c_out, int B, int H, cudaStream_t s);
 
-// rnnt_cluster.cu: returns 0 ok, 1 = 16-CTA clusters unavailable / unsupported shape, <0 error
+// rnnt_cluster.cu: returns 0 ok, 1 = 16-CTA clusters unavailable / unsupported shape, <0 error.  plan: host int[7] that
+// receives the chosen launch (NH, GLOB, rows_smem, cls_per, nu, groups, clusters), or NULL
 int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float* emb_gates, const float* whhT, const float* wpT,
                                const float* bp, const float* wo, const float* bo, int B, int T, int H, int V1, int blank,
-                               int max_symbols, int max_out, int* ids, int* frames, int* counts, cudaStream_t s);
+                               int max_symbols, int max_out, int* ids, int* frames, int* counts, int* plan, cudaStream_t s);
 
 // gemm.cu
 struct GemmParams;

@@ -24,9 +24,15 @@
 //  * the prediction-network state is double-buffered by a cluster-wide parity that flips on every LSTM round;
 //    utterances that do not step in that round carry their state over inside the same float4.
 // All arithmetic is fp32 as in the reference head.
+//
+// Decision contract: the label of a joint row is what torch gives for log_softmax(row).argmax(-1) (gigaam/decoder.py:47,
+// gigaam/decoding.py:162): on a row whose maximum is finite, the first maximal index; if any logit is NaN or +inf, or
+// no logit exceeds -inf, label 0 (torch's log_softmax turns such a row all-NaN, and argmax of all-NaN is 0).  The label
+// is therefore always in [0, V1).  A NaN or +inf logit enters the argmax as (+inf, index -1), which wins every later
+// compare and every merge (equal values: lower index); warp 0 maps index -1 ("non-finite seen") and the empty index
+// 0x7fffffff ("no winner") to 0.  hid keeps NaN as relu(NaN) = NaN does.
 #include <cooperative_groups.h>
 
-#include <cstdio>
 #include <cstdlib>
 
 #include "kernels.h"
@@ -112,6 +118,19 @@ __device__ __forceinline__ float reduce4(const float4 v, int lane) {
   k += __shfl_xor_sync(0xffffffffu, k, 2);
   k += __shfl_xor_sync(0xffffffffu, k, 1);
   return k;
+}
+
+// relu that keeps NaN (torch.relu); fmaxf(x, 0) would turn NaN into 0
+__device__ __forceinline__ float relu_nan(float x) { return x < 0.f ? 0.f : x; }
+
+// running argmax over ascending classes: strict > keeps the first maximum; a NaN or +inf logit becomes (+inf, -1), the
+// "non-finite seen" mark that no later logit replaces and that wins every merge
+__device__ __forceinline__ void arg_update(float a, int cls, float& bv, int& bi) {
+  if (!(a <= bv)) {
+    const bool bad = !(a < INFINITY);
+    bv = bad ? INFINITY : a;
+    bi = bad ? -1 : cls;
+  }
 }
 
 __device__ __forceinline__ void fma4(float4& a, float w, const float4& h) {
@@ -356,8 +375,8 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         for (int hh = 0; hh < NH; ++hh) {
           const float4 g4 = s.pg4[hh][tid];
           const int am = act_m >> (4 * hh);
-          s.hid4[hh][tid] = make_float4((am & 1) ? fmaxf(ep[hh].x + g4.x, 0.f) : 0.f, (am & 2) ? fmaxf(ep[hh].y + g4.y, 0.f) : 0.f,
-                                        (am & 4) ? fmaxf(ep[hh].z + g4.z, 0.f) : 0.f, (am & 8) ? fmaxf(ep[hh].w + g4.w, 0.f) : 0.f);
+          s.hid4[hh][tid] = make_float4((am & 1) ? relu_nan(ep[hh].x + g4.x) : 0.f, (am & 2) ? relu_nan(ep[hh].y + g4.y) : 0.f,
+                                        (am & 4) ? relu_nan(ep[hh].z + g4.z) : 0.f, (am & 8) ? relu_nan(ep[hh].w + g4.w) : 0.f);
         }
       }
       __syncthreads();
@@ -394,8 +413,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
           if (lr < nsm) {
 #pragma unroll
             for (int hh = 0; hh < NH; ++hh) {
-              const float a = reduce4(acc[c][hh], lane) + s_bo[lr];
-              if (a > bv[hh]) { bv[hh] = a; bi[hh] = cls0 + lr; }
+              arg_update(reduce4(acc[c][hh], lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh]);
             }
           }
         }
@@ -410,8 +428,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int kk = 0; kk < kH / 32; ++kk) fma4(acc, wg[gi][kk], s.hid4[hh][lane + 32 * kk]);
-            const float a = reduce4(acc, lane) + s_bo[gcls[gi]];
-            if (a > bv[hh]) { bv[hh] = a; bi[hh] = cls0 + gcls[gi]; }
+            arg_update(reduce4(acc, lane) + s_bo[gcls[gi]], cls0 + gcls[gi], bv[hh], bi[hh]);
           }
         }
       }
@@ -421,8 +438,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         for (int hh = 0; hh < NH; ++hh) {
           float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
           for (int kk = 0; kk < kH / 32; ++kk) fma4(acc, __ldg(w + lane + 32 * kk), s.hid4[hh][lane + 32 * kk]);
-          const float a = reduce4(acc, lane) + s_bo[lr];
-          if (a > bv[hh]) { bv[hh] = a; bi[hh] = cls0 + lr; }
+          arg_update(reduce4(acc, lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh]);
         }
       }
       }
@@ -480,6 +496,9 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
           if (v > v0 || (v == v0 && i < i0)) { v0 = v; i0 = i; }
         }
         DBG_T(10);
+        // "non-finite seen" (-1) and "no winner" (0x7fffffff: every logit -inf) give label 0, as torch's argmax of an
+        // all-NaN log_softmax row; the label that indexes emb_gates below is in [0, V1) by construction
+        const int lab = (i0 < 0 || i0 >= p.V1) ? 0 : i0;
         // lane u < NU decides for utterance u (gigaam/decoding.py:176-205)
         bool act_new = false, run_new = false, moved = false, emitted = false;
         if (lane < NU) {
@@ -487,7 +506,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
           const int Lu = s.ctl.L[u];
           int need = s.ctl.need[u];
           if (t < Lu) {
-            if (i0 == p.blank) {
+            if (lab == p.blank) {
               t += 1;
               s.ctl.nsym[u] = 0;
               need = 0;
@@ -496,11 +515,11 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
               const int cnt = s.ctl.cnt[u];
               if (rank == 0 && cnt < p.max_out) {
                 const size_t o = static_cast<size_t>(group * p.nu + u) * p.max_out + cnt;
-                p.ids[o] = i0;
+                p.ids[o] = lab;
                 p.frames[o] = t;
               }
               s.ctl.cnt[u] = cnt + 1;
-              s.ctl.label[u] = i0;
+              s.ctl.label[u] = lab;
               need = 1;   // the state that produced this token becomes the input of the next LSTM step
               emitted = true;
               int ns = s.ctl.nsym[u] + 1;
@@ -567,7 +586,7 @@ struct LaunchState {
 };
 
 template <int NH, bool GLOB>
-int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, bool info, cudaStream_t s) {
+int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, int* plan, cudaStream_t s) {
   static LaunchState per_device[64];   // function attributes and cluster occupancy are per device
   int dev_index = 0;
   cudaGetDevice(&dev_index);
@@ -614,10 +633,10 @@ int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, bool info, cudaStrea
   p.cls_pad = cls_pad;
   const int nclusters = p.num_groups < st.max_clusters ? p.num_groups : st.max_clusters;
   cfg.gridDim = dim3(nclusters * kCl);
-  if (info)
-    fprintf(stderr, "[gam] rnnt cluster kernel<%d,%d>: at most %d clusters of %d CTAs resident; %d groups of %d utterances on %d clusters; "
-                    "%d of %d class rows per CTA in shared memory (%d B)\n", NH, GLOB ? 1 : 0, st.max_clusters, kCl, p.num_groups, nu, nclusters,
-            rows_smem, cls_per, smem);
+  if (plan) {
+    const int v[7] = {NH, GLOB ? 1 : 0, rows_smem, cls_per, nu, p.num_groups, nclusters};
+    for (int i = 0; i < 7; ++i) plan[i] = v[i];
+  }
   if (cudaLaunchKernelEx(&cfg, rnnt_cluster_kernel<NH, GLOB>, p) != cudaSuccess) return -2;
   return 0;
 }
@@ -631,13 +650,13 @@ extern "C" int gam_rnnt_debug_read(long long* out16) {
 #endif
 
 // returns 0 on success, 1 if the shape is unsupported (pred_hidden != 320) or a 16-CTA cluster cannot be scheduled on
-// this device, negative on a launch error
+// this device, negative on a launch error.  plan (host, 7 ints, or NULL) receives the launch that was chosen:
+// NH, GLOB, class rows per CTA in shared memory, classes per CTA, utterances per group, groups, clusters launched.
 int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float* emb_gates, const float* whhT, const float* wpT,
                                const float* bp, const float* wo, const float* bo, int B, int T, int H, int V1, int blank,
-                               int max_symbols, int max_out, int* ids, int* frames, int* counts, cudaStream_t s) {
+                               int max_symbols, int max_out, int* ids, int* frames, int* counts, int* plan, cudaStream_t s) {
   if (H != kH) return 1;
   static int smem_cap = 0, clusters_hint = 0;
-  constexpr int info = 0;
   if (smem_cap == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
@@ -656,8 +675,8 @@ int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float
   const bool small = B <= 4 * clusters_hint;
   const int fixed = static_cast<int>(small ? sizeof(Smem<1>) : sizeof(Smem<2>)) + ((cls_per + 3) & ~3) * 4;
   const bool glob = (smem_cap - fixed) / (kWoPitch * 4) < cls_per;   // some class rows have to stay in L2
-  if (small) return glob ? launch_nh<1, true>(p, B, V1, smem_cap, info != 0, s) : launch_nh<1, false>(p, B, V1, smem_cap, info != 0, s);
-  return glob ? launch_nh<2, true>(p, B, V1, smem_cap, info != 0, s) : launch_nh<2, false>(p, B, V1, smem_cap, info != 0, s);
+  if (small) return glob ? launch_nh<1, true>(p, B, V1, smem_cap, plan, s) : launch_nh<1, false>(p, B, V1, smem_cap, plan, s);
+  return glob ? launch_nh<2, true>(p, B, V1, smem_cap, plan, s) : launch_nh<2, false>(p, B, V1, smem_cap, plan, s);
 }
 
 }  // namespace gam

@@ -309,6 +309,14 @@ int gam_test_frames_split(gam_handle* h, const float* wav, int32_t B, int64_t n_
  * bins [mel_lo[m], mel_hi[m]) only (device i32 [n_mels]) */
 int gam_test_mel_log(gam_handle* h, const float* P, const int32_t* fexp, int32_t B, int32_t M, int32_t nbins, const float* fb,
                      const int32_t* mel_lo, const int32_t* mel_hi, int32_t n_mels, float* mel, void* stream);
+/* gam_rnnt_greedy's cluster kernel on caller weights (H = 320, blank = V1 - 1): encproj f32 [B, T, 320] (joint.enc applied),
+ * len i32 [B], emb_gates f32 [V1, 1280] (embed W_ih^T + b_ih + b_hh), whhT f32 [320, 1280], wpT f32 [320, 320], bp [320],
+ * wo f32 [V1, 320], bo [V1] -> ids / frames i32 [B, max_out], counts i32 [B].  plan (host i32 [7], or NULL) receives the
+ * launch chosen: NH, GLOB, class rows per CTA in shared memory, classes per CTA, utterances per group, groups, clusters. */
+int gam_test_rnnt_greedy(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,
+                         const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
+                         int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts, int32_t* plan,
+                         void* stream);
 /* qkv: f16 [B*T, 3*d_model]; klen i32 [B] or NULL -> out f16 [B*T, d_model].  T up to the handle's max_encoded_frames */
 int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void* out, int32_t B, int32_t T, void* stream);
 /* rel_pos variant: qkv f16 [B*T, 4*d_model] = [q+u | q+v | k | v]; pos f16 [2*max-1, d_model] laid out like pos_proj

@@ -306,7 +306,8 @@ def rnnt_greedy(enc: Tensor, enc_len: Tensor, sd: SD, max_symbols: int = 10) -> 
         for t in range(L):
             f = F.linear(x[b, t:t + 1], W_e, b_e)
             for _ in range(max_symbols):
-                k = int(F.linear(F.relu(f + pg), W_o, b_o).argmax(dim=-1))
+                # argmax after log_softmax, as gigaam/decoder.py:47 + decoding.py:162: a row with a NaN gives 0
+                k = int(torch.log_softmax(F.linear(F.relu(f + pg), W_o, b_o), dim=-1).argmax(dim=-1))
                 if k == blank:
                     break
                 ids.append(k)
