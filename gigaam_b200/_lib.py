@@ -57,7 +57,10 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_rnnt_joint_workspace_bytes", "gam_rnnt_joint", "gam_rnnt_predict", "gam_test_gemm_conv",
            "gam_test_layernorm", "gam_test_ln_rope", "gam_test_ln_out_ln", "gam_test_unpack_rows", "gam_test_dwconv",
            "gam_test_pack_plan", "gam_test_subsample_conv1", "gam_test_mel_to_tmajor", "gam_emo_workspace_bytes",
-           "gam_emo_head", "gam_test_frames_split", "gam_test_mel_log", "gam_test_rnnt_greedy")
+           "gam_emo_head", "gam_test_frames_split", "gam_test_mel_log", "gam_test_rnnt_greedy",
+           "gam_rnnt_predict_train", "gam_ctc_log_probs_backward_workspace_bytes", "gam_ctc_log_probs_backward",
+           "gam_rnnt_joint_backward_workspace_bytes", "gam_rnnt_joint_backward", "gam_rnnt_predict_backward_workspace_bytes",
+           "gam_rnnt_predict_backward")
 
 
 def lib_path() -> Path:
@@ -117,6 +120,18 @@ def load() -> C.CDLL:
     lib.gam_rnnt_joint.restype = C.c_int
     lib.gam_rnnt_predict.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, c_vp, c_vp, c_vp, c_vp]
     lib.gam_rnnt_predict.restype = C.c_int
+    lib.gam_rnnt_predict_train.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, c_vp, c_vp, c_vp, c_vp, c_vp]
+    lib.gam_ctc_log_probs_backward_workspace_bytes.argtypes = [H, i32, i32]
+    lib.gam_ctc_log_probs_backward.argtypes = [H, c_vp, i32, i32, c_vp, c_vp, c_vp, i64, c_vp, c_vp, c_vp, c_vp]
+    lib.gam_rnnt_joint_backward_workspace_bytes.argtypes = [H, i32, i32, i32]
+    lib.gam_rnnt_joint_backward.argtypes = [H, c_vp, c_vp, i32, i32, i32, c_vp, c_vp, c_vp, i64] + [c_vp] * 9
+    lib.gam_rnnt_predict_backward_workspace_bytes.argtypes = [H, i32, i32]
+    lib.gam_rnnt_predict_backward.argtypes = [H, c_vp, c_vp, c_vp, i32, i32] + [c_vp] * 8 + [c_vp, i64] + [c_vp] * 7
+    for fn in (lib.gam_ctc_log_probs_backward_workspace_bytes, lib.gam_rnnt_joint_backward_workspace_bytes,
+               lib.gam_rnnt_predict_backward_workspace_bytes):
+        fn.restype = i64
+    for fn in (lib.gam_rnnt_predict_train, lib.gam_ctc_log_probs_backward, lib.gam_rnnt_joint_backward, lib.gam_rnnt_predict_backward):
+        fn.restype = C.c_int
     lib.gam_emo_workspace_bytes.argtypes = [H, i32, i32]
     lib.gam_emo_workspace_bytes.restype = i64
     lib.gam_emo_head.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, i64, c_vp, c_vp, c_vp, c_vp]

@@ -134,7 +134,7 @@ struct gam_handle {
 enum ProfClass : int {
   PC_LOGMEL = 0, PC_SUB_CONV1, PC_GEMM_CONV2, PC_GEMM_SUBOUT, PC_GEMM_FFN_UP, PC_GEMM_FFN_DOWN, PC_GEMM_QKV, PC_GEMM_PROJ,
   PC_GEMM_GLU, PC_LAYERNORM, PC_ATTENTION, PC_DWCONV, PC_CTC_ARGMAX, PC_CTC_COLLAPSE, PC_RNNT_ENCPROJ, PC_RNNT_GREEDY,
-  PC_MISC, PC_CTC_LOG_PROBS, PC_RNNT_JOINT, PC_RNNT_PREDICT, PC_EMO_HEAD, PC_COUNT
+  PC_MISC, PC_CTC_LOG_PROBS, PC_RNNT_JOINT, PC_RNNT_PREDICT, PC_EMO_HEAD, PC_HEAD_BACKWARD, PC_COUNT
 };
 
 struct ProfScope {
@@ -732,6 +732,218 @@ int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const flo
   return 0;
 }
 
+int gam_rnnt_predict_train(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g,
+                           float* h1, float* c1, float* c_seq, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 2) return fail(h, -1, "rnnt_predict_train: model has no RNN-T head");
+  if (B <= 0 || U <= 0) return fail(h, -1, "rnnt_predict_train: bad sizes (B=%d, U=%d)", B, U);
+  if (x == nullptr && U != 1) return fail(h, -1, "rnnt_predict_train: without labels the step count U must be 1 (got %d)", U);
+  if (c.pred_hidden > 1024) return fail(h, -1, "rnnt_predict_train: pred_hidden %d exceeds 1024", c.pred_hidden);
+  const int H = c.pred_hidden;
+  const int64_t BH = static_cast<int64_t>(B) * H;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  for (int u = 0; u < U; ++u) {   // gam_rnnt_predict's steps, with the cell of every step kept in c_seq[u]
+    const float* h_in = u == 0 ? h0 : g + static_cast<int64_t>(u - 1) * H;
+    const int64_t pitch = u == 0 ? H : static_cast<int64_t>(U) * H;
+    PROF(PC_RNNT_PREDICT);
+    launch_lstm_step(x, U, u, c.num_classes, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h_in, pitch, u == 0 ? c0 : c_seq + (u - 1) * BH, g,
+                     u == U - 1 ? h1 : nullptr, c_seq + u * BH, B, H, s);
+  }
+  cudaMemcpyAsync(c1, c_seq + static_cast<int64_t>(U - 1) * BH, BH * 4, cudaMemcpyDeviceToDevice, s);
+  GAM_CHECK_LAUNCH(h, "rnnt_predict_train");
+  return 0;
+}
+
+// ---- backward passes of the head calls (csrc/head_grads.cu).  Workspaces are carved in 1 KiB-aligned pieces.
+namespace {
+struct Carve {
+  uint8_t* base;
+  int64_t off = 0;
+  float* take(int64_t floats) {
+    float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
+    off += align_up(floats * 4, 1024);
+    return p;
+  }
+};
+inline int64_t max3(int64_t a, int64_t b, int64_t c) { return a > b ? (a > c ? a : c) : (b > c ? b : c); }
+
+struct CtcBwdWs { float *dl, *part; };
+int64_t ctc_bwd_layout(const gam_config& c, int64_t R, uint8_t* base, CtcBwdWs* w) {
+  Carve cv{base};
+  w->dl = cv.take(R * c.num_classes);
+  w->part = cv.take(outer_sum_workspace_floats(R, c.num_classes, c.d_model, true));
+  return cv.off;
+}
+
+struct JointBwdWs { float *E, *P, *dl, *dhid, *dE, *dP, *part; };
+int64_t joint_bwd_layout(const gam_config& c, int32_t B, int32_t T, int32_t U, uint8_t* base, JointBwdWs* w) {
+  const int64_t J = c.joint_hidden, BT = static_cast<int64_t>(B) * T, BU = static_cast<int64_t>(B) * U, rows = BT * U;
+  Carve cv{base};
+  w->E = cv.take(BT * J);
+  w->P = cv.take(BU * J);
+  w->dl = cv.take(rows * c.num_classes);
+  w->dhid = cv.take(rows * J);
+  w->dE = cv.take(BT * J);
+  w->dP = cv.take(BU * J);
+  w->part = cv.take(max3(outer_sum_workspace_floats(rows, c.num_classes, J, true), outer_sum_workspace_floats(BT, J, c.d_model, true),
+                         outer_sum_workspace_floats(BU, J, c.pred_hidden, true)));
+  return cv.off;
+}
+
+struct PredBwdWs { float *dgates, *dcc, *dcls, *part; };
+int64_t pred_bwd_layout(const gam_config& c, int32_t B, int32_t U, uint8_t* base, PredBwdWs* w) {
+  const int64_t H = c.pred_hidden, BU = static_cast<int64_t>(B) * U;
+  Carve cv{base};
+  w->dgates = cv.take(BU * 4 * H);
+  w->dcc = cv.take(static_cast<int64_t>(B) * H);
+  w->dcls = cv.take(static_cast<int64_t>(c.num_classes) * 4 * H);
+  w->part = cv.take(max3(outer_sum_workspace_floats(BU, 4 * H, H, true), outer_sum_workspace_floats(c.num_classes, 4 * H, H, false), 0));
+  return cv.off;
+}
+}  // namespace
+
+int64_t gam_ctc_log_probs_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t T) {
+  if (!h || h->cfg.head != 1 || B <= 0 || T <= 0) return -1;
+  CtcBwdWs w;
+  return ctc_bwd_layout(h->cfg, static_cast<int64_t>(B) * T, nullptr, &w) + 1024;
+}
+
+int gam_ctc_log_probs_backward(gam_handle* h, const float* enc, int32_t B, int32_t T, const float* log_probs, const float* grad,
+                               void* workspace, int64_t workspace_bytes, float* d_enc, float* dW, float* db, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 1) return fail(h, -1, "ctc_log_probs_backward: model has no CTC head");
+  if (B <= 0 || T <= 0) return fail(h, -1, "ctc_log_probs_backward: bad sizes (B=%d, T=%d)", B, T);
+  if ((dW == nullptr) != (db == nullptr)) return fail(h, -1, "ctc_log_probs_backward: dW and db go together");
+  const int64_t need = gam_ctc_log_probs_backward_workspace_bytes(h, B, T);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "ctc_log_probs_backward: workspace too small: need %lld bytes, got %lld", (long long)need,
+                (long long)workspace_bytes);
+  const int64_t R = static_cast<int64_t>(B) * T;
+  CtcBwdWs w;
+  ctc_bwd_layout(c, R, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  { PROF(PC_HEAD_BACKWARD);
+    launch_softmax_grad(grad, log_probs, w.dl, R, c.num_classes, s); }
+  if (dW != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_outer_sum(w.dl, enc, R, c.num_classes, c.d_model, dW, db, w.part, s); }
+  if (d_enc != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_head_matmul(w.dl, h->w.ctc_w, c.d_model, 1, d_enc, R, c.num_classes, c.d_model, nullptr, nullptr, 1, 1, s); }
+  GAM_CHECK_LAUNCH(h, "ctc_log_probs_backward");
+  return 0;
+}
+
+int64_t gam_rnnt_joint_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || U <= 0) return -1;
+  JointBwdWs w;
+  return joint_bwd_layout(h->cfg, B, T, U, nullptr, &w) + 1024;
+}
+
+int gam_rnnt_joint_backward(gam_handle* h, const float* enc, const float* dec, int32_t B, int32_t T, int32_t U, const float* log_probs,
+                            const float* grad, void* workspace, int64_t workspace_bytes, float* d_enc, float* d_dec, float* dW_enc,
+                            float* db_enc, float* dW_pred, float* db_pred, float* dW_out, float* db_out, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 2) return fail(h, -1, "rnnt_joint_backward: model has no RNN-T head");
+  if (B <= 0 || T <= 0 || U <= 0) return fail(h, -1, "rnnt_joint_backward: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
+  constexpr int64_t kMaxProjRows = 65535LL * 64;
+  if (static_cast<int64_t>(B) * T > kMaxProjRows || static_cast<int64_t>(B) * U > kMaxProjRows)
+    return fail(h, -1, "rnnt_joint_backward: B*T and B*U must be <= %lld", (long long)kMaxProjRows);
+  if (c.pred_hidden % 16 != 0 || c.d_model % 16 != 0)
+    return fail(h, -1, "rnnt_joint_backward: needs pred_hidden %% 16 == 0 and d_model %% 16 == 0");
+  if ((dW_enc == nullptr) != (db_enc == nullptr) || (dW_pred == nullptr) != (db_pred == nullptr) || (dW_out == nullptr) != (db_out == nullptr))
+    return fail(h, -1, "rnnt_joint_backward: each weight gradient goes with its bias gradient");
+  const int64_t need = gam_rnnt_joint_backward_workspace_bytes(h, B, T, U);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "rnnt_joint_backward: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  JointBwdWs w;
+  joint_bwd_layout(c, B, T, U, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  const int J = c.joint_hidden, V1 = c.num_classes;
+  const int64_t BT = static_cast<int64_t>(B) * T, BU = static_cast<int64_t>(B) * U, rows = BT * U;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // the forward's two projections, recomputed with the forward's kernels (same bits)
+  { PROF(PC_HEAD_BACKWARD);
+    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, w.E, B * T, J, c.d_model, s); }
+  { PROF(PC_HEAD_BACKWARD);
+    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, w.P, B * U, J, c.pred_hidden, s); }
+  { PROF(PC_HEAD_BACKWARD);
+    launch_softmax_grad(grad, log_probs, w.dl, rows, V1, s); }
+  if (dW_out != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_outer_sum_joint(w.dl, w.E, w.P, T, U, rows, V1, J, dW_out, db_out, w.part, s); }
+  const bool need_hidden = d_enc || d_dec || dW_enc || dW_pred;
+  if (need_hidden) {
+    { PROF(PC_HEAD_BACKWARD);   // dhid = (dlogit W_o) * [hid > 0]
+      launch_head_matmul(w.dl, h->w.rnnt_wo, J, 1, w.dhid, rows, V1, J, w.E, w.P, T, U, s); }
+    { PROF(PC_HEAD_BACKWARD);   // dE[b, t] = sum_u dhid[b, t, u]
+      launch_segment_sum(w.dhid, w.dE, BT, U, J, 1, U, 0, 1, s); }
+    { PROF(PC_HEAD_BACKWARD);   // dP[b, u] = sum_t dhid[b, t, u]
+      launch_segment_sum(w.dhid, w.dP, BU, T, J, U, static_cast<int64_t>(T) * U, 1, U, s); }
+  }
+  if (dW_enc != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_outer_sum(w.dE, enc, BT, J, c.d_model, dW_enc, db_enc, w.part, s); }
+  if (dW_pred != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_outer_sum(w.dP, dec, BU, J, c.pred_hidden, dW_pred, db_pred, w.part, s); }
+  if (d_enc != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_e [J, d]
+    launch_head_matmul(w.dE, h->w.rnnt_enc_w, c.d_model, 1, d_enc, BT, J, c.d_model, nullptr, nullptr, 1, 1, s); }
+  if (d_dec != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_p [J, H] = rnnt_wp_t^T
+    launch_head_matmul(w.dP, h->w.rnnt_wp_t, 1, J, d_dec, BU, J, c.pred_hidden, nullptr, nullptr, 1, 1, s); }
+  GAM_CHECK_LAUNCH(h, "rnnt_joint_backward");
+  return 0;
+}
+
+int64_t gam_rnnt_predict_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t U) {
+  if (!h || h->cfg.head != 2 || B <= 0 || U <= 0) return -1;
+  PredBwdWs w;
+  return pred_bwd_layout(h->cfg, B, U, nullptr, &w) + 1024;
+}
+
+int gam_rnnt_predict_backward(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, const float* g,
+                              const float* c_seq, const float* grad_g, const float* grad_h1, const float* grad_c1, const float* embed,
+                              const float* w_ih, const float* w_hh, void* workspace, int64_t workspace_bytes, float* d_h0, float* d_c0,
+                              float* d_embed, float* dW_ih, float* dW_hh, float* d_bias, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 2) return fail(h, -1, "rnnt_predict_backward: model has no RNN-T head");
+  if (B <= 0 || U <= 0) return fail(h, -1, "rnnt_predict_backward: bad sizes (B=%d, U=%d)", B, U);
+  if (x == nullptr && U != 1) return fail(h, -1, "rnnt_predict_backward: without labels the step count U must be 1 (got %d)", U);
+  const int H = c.pred_hidden, V1 = c.num_classes;
+  if (H > lstm_bwd_max_hidden()) return fail(h, -1, "rnnt_predict_backward: pred_hidden %d exceeds %d", H, lstm_bwd_max_hidden());
+  if (!g || !c_seq || !grad_g || !w_hh) return fail(h, -1, "rnnt_predict_backward: g, c_seq, grad_g and w_hh are required");
+  if ((dW_hh == nullptr) != (d_bias == nullptr)) return fail(h, -1, "rnnt_predict_backward: dW_hh and d_bias go together");
+  if ((dW_ih || d_embed) && (!embed || !w_ih)) return fail(h, -1, "rnnt_predict_backward: embed and w_ih are required for their grads");
+  const int64_t need = gam_rnnt_predict_backward_workspace_bytes(h, B, U);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "rnnt_predict_backward: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  PredBwdWs w;
+  pred_bwd_layout(c, B, U, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  const int64_t BH = static_cast<int64_t>(B) * H, BU = static_cast<int64_t>(B) * U;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (grad_c1 != nullptr)
+    cudaMemcpyAsync(w.dcc, grad_c1, BH * 4, cudaMemcpyDeviceToDevice, s);
+  else
+    cudaMemsetAsync(w.dcc, 0, BH * 4, s);
+  for (int u = U - 1; u >= -1; --u) {
+    PROF(PC_HEAD_BACKWARD);
+    launch_lstm_bwd_step(x, U, u, V1, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, w_hh, h0, c0, g, c_seq, grad_g, grad_h1, w.dgates, w.dcc,
+                         d_h0, d_c0, B, H, s);
+  }
+  if (dW_hh != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_outer_sum_shift(w.dgates, g, h0, U, BU, 4 * H, H, dW_hh, d_bias, w.part, s); }
+  if (dW_ih != nullptr || d_embed != nullptr) {
+    if (x == nullptr) {   // every step read the zero embedding
+      if (dW_ih) cudaMemsetAsync(dW_ih, 0, static_cast<int64_t>(4) * H * H * 4, s);
+      if (d_embed) cudaMemsetAsync(d_embed, 0, static_cast<int64_t>(V1) * H * 4, s);
+    } else {
+      { PROF(PC_HEAD_BACKWARD);
+        if (launch_class_gate_sum(x, BU, w.dgates, 4 * H, V1, V1 - 1, w.dcls, s) != 0)
+          return fail(h, -1, "rnnt_predict_backward: pred_hidden %d too large for the class sums", H); }
+      if (dW_ih != nullptr) { PROF(PC_HEAD_BACKWARD);
+        launch_outer_sum(w.dcls, embed, V1, 4 * H, H, dW_ih, nullptr, w.part, s); }
+      if (d_embed != nullptr) { PROF(PC_HEAD_BACKWARD);
+        launch_head_matmul(w.dcls, w_ih, H, 1, d_embed, V1, 4 * H, H, nullptr, nullptr, 1, 1, s); }
+    }
+  }
+  GAM_CHECK_LAUNCH(h, "rnnt_predict_backward");
+  return 0;
+}
+
 int64_t gam_emo_workspace_bytes(const gam_handle* h, int32_t B, int32_t T) {
   if (!h || h->cfg.head != 3 || B < 1 || T < 1 || T > 65535 * kPoolChunk) return -1;
   return static_cast<int64_t>(B) * pool_chunk_count(T) * h->cfg.d_model * 4;
@@ -826,7 +1038,7 @@ const char* gam_profile_class_name(int32_t cls) {
   static const char* names[PC_COUNT] = {"logmel", "subsample_conv1", "gemm_conv2_implicit", "gemm_subsample_out", "gemm_ffn_up_silu",
                                         "gemm_ffn_down_res", "gemm_qkv", "gemm_proj_res", "gemm_pw1_glu", "layernorm", "attention",
                                         "dwconv_bn_silu", "ctc_head_argmax", "ctc_collapse", "rnnt_enc_proj", "rnnt_greedy", "misc",
-                                        "ctc_log_probs", "rnnt_joint", "rnnt_predict", "emo_head"};
+                                        "ctc_log_probs", "rnnt_joint", "rnnt_predict", "emo_head", "head_backward"};
   return (cls >= 0 && cls < PC_COUNT) ? names[cls] : "?";
 }
 

@@ -90,6 +90,32 @@ int launch_rnnt_joint(const float* E, const float* P, const float* Wo, const flo
 void launch_lstm_step(const int64_t* x, int U, int u, int V1, const float* emb_gates, const float* whh_t, const float* h_in,
                       int64_t h_pitch, const float* c_in, float* g, float* h_out, float* c_out, int B, int H, cudaStream_t s);
 
+// head_grads.cu: backward passes of the heads (fp32, deterministic, no atomics).  Rows are 64-bit.
+// dl = G - exp(logp) * rowsum(G), rows of V1
+void launch_softmax_grad(const float* G, const float* logp, float* dl, int64_t rows, int V1, cudaStream_t s);
+// dW[N, K] = sum_r A[r, n] X(r, k) and, when db != null, db[n] = sum_r A[r, n]; ws: outer_sum_workspace_floats() floats.
+// X(r, k): X[r, k] (plain); shift: X[r-1, k] for r % U != 0, else X0[r / U, k] (X0 null: 0); joint: relu(E[r/U] + P[bu]),
+// bu = (r / U) / T * U + r % U (NaN kept)
+int64_t outer_sum_workspace_floats(int64_t rows, int N, int K, bool with_bias);
+void launch_outer_sum(const float* A, const float* X, int64_t rows, int N, int K, float* dW, float* db, float* ws, cudaStream_t s);
+void launch_outer_sum_shift(const float* A, const float* X, const float* X0, int U, int64_t rows, int N, int K, float* dW, float* db,
+                            float* ws, cudaStream_t s);
+void launch_outer_sum_joint(const float* A, const float* E, const float* P, int T, int U, int64_t rows, int N, int K, float* dW,
+                            float* db, float* ws, cudaStream_t s);
+// out[r, k] = sum_n A[r, n] W[n * sn + k * sk], times [relu(E + P)(r, k) > 0] when mask_E != null (joint row map as above)
+void launch_head_matmul(const float* A, const float* W, int64_t sn, int64_t sk, float* out, int64_t rows, int N, int K,
+                        const float* mask_E, const float* mask_P, int T, int U, cudaStream_t s);
+// out[g, k] = sum_{i < count} X[(g / gi) * so + (g % gi) * si + i * step, k]
+void launch_segment_sum(const float* X, float* out, int64_t groups, int count, int K, int64_t gi, int64_t so, int64_t si, int64_t step,
+                        cudaStream_t s);
+// one BPTT step u of lstm_step_kernel (u = -1: dh0 / dc0); see lstm_bwd_step_kernel.  H <= lstm_bwd_max_hidden()
+int lstm_bwd_max_hidden();
+void launch_lstm_bwd_step(const int64_t* x, int U, int u, int V1, const float* emb_gates, const float* whh_t, const float* whh,
+                          const float* h0, const float* c0, const float* g, const float* c_seq, const float* dG, const float* dh1,
+                          float* dgates, float* dc_carry, float* dh0, float* dc0, int B, int H, cudaStream_t s);
+// out [V1, H4]: per-class sums of dgates rows (blank row zero); returns 1 if H4 is too large
+int launch_class_gate_sum(const int64_t* x, int64_t rows, const float* dgates, int H4, int V1, int blank, float* out, cudaStream_t s);
+
 // rnnt_cluster.cu: returns 0 ok, 1 = 16-CTA clusters unavailable / unsupported shape, <0 error.  plan: host int[7] that
 // receives the chosen launch (NH, GLOB, rows_smem, cls_per, nu, groups, clusters), or NULL
 int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float* emb_gates, const float* whhT, const float* wpT,

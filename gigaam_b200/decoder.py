@@ -20,6 +20,98 @@ def _zeros(entries):
     return [(k, torch.zeros(shape, dtype=torch.float32)) for k, shape, kind, _ in entries]
 
 
+def _trains(module, *inputs) -> bool:
+    """The autograd path engages only when grad mode is on and a parameter of the head module or an input tensor requires
+    grad; otherwise the forward-only path runs (same kernels, same bits, nothing saved)."""
+    if not torch.is_grad_enabled():
+        return False
+    return any(p.requires_grad for p in module.parameters()) or any(t is not None and t.requires_grad for t in inputs)
+
+
+def _param_versions(module) -> Tuple:
+    return tuple(p._version for p in module.parameters())
+
+
+def _check_versions(ctx) -> None:
+    if _param_versions(ctx.module) != ctx.versions:
+        raise RuntimeError(f"{type(ctx.module).__name__}: a head parameter was modified between forward and backward")
+
+
+def _f32(t: Optional[Tensor]) -> Optional[Tensor]:
+    return None if t is None else t.detach().float().contiguous()
+
+
+class _CTCLogProbs(torch.autograd.Function):
+    """CTCHead.forward with gam_ctc_log_probs_backward behind it (dL/d encoder output, decoder_layers.0.weight / bias)."""
+
+    @staticmethod
+    def forward(ctx, module, enc, weight, bias):
+        eng = module._engine()
+        out = eng.ctc_log_probs(enc.detach())
+        ctx.module, ctx.versions = module, _param_versions(module)
+        ctx.save_for_backward(enc, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        _check_versions(ctx)
+        enc, out = ctx.saved_tensors
+        eng = ctx.module._engine()
+        need_w = ctx.needs_input_grad[2] or ctx.needs_input_grad[3]
+        d_enc, dW, db = eng.ctc_log_probs_backward(enc.detach(), out, _f32(grad), ctx.needs_input_grad[1], need_w)
+        w = ctx.module.decoder_layers._modules["0"].weight
+        return (None, d_enc, None if dW is None else dW.view(w.shape).to(w.dtype),
+                None if db is None else db.to(w.dtype))
+
+
+class _RNNTJointFn(torch.autograd.Function):
+    """RNNTJoint.joint with gam_rnnt_joint_backward behind it (enc / dec inputs, joint.enc, joint.pred, joint_net.1)."""
+
+    @staticmethod
+    def forward(ctx, module, enc, dec, *params):
+        eng = module._engine()
+        out = eng.rnnt_joint(enc.detach(), dec.detach())
+        ctx.module, ctx.versions = module, _param_versions(module)
+        ctx.save_for_backward(enc, dec, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        _check_versions(ctx)
+        enc, dec, out = ctx.saved_tensors
+        eng = ctx.module._engine()
+        need_w = any(ctx.needs_input_grad[3:])
+        d_enc, d_dec, *dw = eng.rnnt_joint_backward(enc.detach(), dec.detach(), out, _f32(grad), ctx.needs_input_grad[1],
+                                                    ctx.needs_input_grad[2], need_w)
+        return (None, d_enc, d_dec, *dw)
+
+
+class _RNNTPredictFn(torch.autograd.Function):
+    """RNNTDecoder.predict with gam_rnnt_predict_backward behind it (h0 / c0, embed, lstm weights and biases)."""
+
+    @staticmethod
+    def forward(ctx, module, x, h, c, batch_size, embed, w_ih, w_hh, b_ih, b_hh):
+        eng = module._engine()
+        h_d, c_d = _f32(h), _f32(c)
+        g, h1, c1, c_seq = eng.rnnt_predict_train(x, h_d, c_d, batch_size)
+        ctx.module, ctx.versions = module, _param_versions(module)
+        ctx.save_for_backward(x, h_d, c_d, g, c_seq)
+        return g, h1, c1
+
+    @staticmethod
+    def backward(ctx, grad_g, grad_h1, grad_c1):
+        _check_versions(ctx)
+        x, h, c, g, c_seq = ctx.saved_tensors
+        eng = ctx.module._engine()
+        lstm = ctx.module.lstm
+        need_state = ctx.needs_input_grad[2] or ctx.needs_input_grad[3]
+        need_w = any(ctx.needs_input_grad[5:])
+        d_h, d_c, d_emb, dW_ih, dW_hh, d_b = eng.rnnt_predict_backward(
+            x, h, c, g, c_seq, _f32(grad_g), _f32(grad_h1), _f32(grad_c1), _f32(ctx.module.embed.weight),
+            _f32(lstm.weight_ih_l0), _f32(lstm.weight_hh_l0), need_state, need_w)
+        return None, None, d_h, d_c, None, d_emb, dW_ih, dW_hh, d_b, None if d_b is None else d_b.clone()
+
+
 def _on_device(t: Tensor, eng, dtype: torch.dtype) -> Tensor:
     if not t.is_cuda:
         raise RuntimeError("gigaam_b200 has no CPU path: pass CUDA tensors to the head (the model runs on "
@@ -39,7 +131,11 @@ class CTCHead(Bound):
         """[B, feat_in, T] -> log-probs [B, T, num_classes] (gigaam/decoder.py:18-21).  The encoder's output is a
         transposed view of a [B, T, d] buffer, which the kernel reads as it is."""
         eng = self._engine()
-        return eng.ctc_log_probs(_as_btd(_on_device(encoder_output, eng, torch.float32)))
+        enc = _as_btd(_on_device(encoder_output, eng, torch.float32))
+        if _trains(self, enc):
+            layer = self.decoder_layers._modules["0"]
+            return _CTCLogProbs.apply(self, enc, layer.weight, layer.bias)
+        return eng.ctc_log_probs(enc)
 
 
 class RNNTJoint(Bound):
@@ -55,6 +151,10 @@ class RNNTJoint(Bound):
         eng = self._engine()
         enc = _on_device(encoder_out, eng, torch.float32).contiguous()
         dec = _on_device(decoder_out, eng, torch.float32).contiguous()
+        if _trains(self, enc, dec):
+            out = self.joint_net._modules["1"]
+            return _RNNTJointFn.apply(self, enc, dec, self.enc.weight, self.enc.bias, self.pred.weight, self.pred.bias,
+                                      out.weight, out.bias)
         return eng.rnnt_joint(enc, dec)
 
     def forward(self, enc: Tensor, dec: Tensor) -> Tensor:
@@ -85,7 +185,12 @@ class RNNTDecoder(Bound):
                 raise ValueError(f"predict: state must be two [1, B, {self.pred_hidden}] tensors (one LSTM layer), got "
                                  f"{tuple(h.shape)} and {tuple(c.shape)}")
             h, c = h[0].contiguous(), c[0].contiguous()
-        g, h1, c1 = eng.rnnt_predict(x, h, c, batch_size)
+        if _trains(self, h, c):
+            lstm = self.lstm
+            g, h1, c1 = _RNNTPredictFn.apply(self, x, h, c, batch_size, self.embed.weight, lstm.weight_ih_l0, lstm.weight_hh_l0,
+                                             lstm.bias_ih_l0, lstm.bias_hh_l0)
+        else:
+            g, h1, c1 = eng.rnnt_predict(x, h, c, batch_size)
         return g, (h1.unsqueeze(0), c1.unsqueeze(0))
 
     def forward(self, x: Tensor, h: Tensor, c: Tensor) -> Tuple[Tensor, Tensor, Tensor]:

@@ -67,7 +67,11 @@ class ConformerEncoder(Bound):
         self.pre_encode._bind(owner)
 
     def forward(self, audio_signal: Tensor, length: Tensor) -> Tuple[Tensor, Tensor]:
-        """[B, F, M] log-mel, [B] lengths -> ([B, d_model, T'], [B] int32)  (gigaam/encoder.py:605-647)"""
+        """[B, F, M] log-mel, [B] lengths -> ([B, d_model, T'], [B] int32)  (gigaam/encoder.py:605-647).  Inference-only:
+        with grad enabled and a parameter of this encoder requiring grad this raises NotImplementedError."""
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise NotImplementedError("the encoder is inference-only; freeze it (requires_grad_(False)) and train the head on "
+                                      "its output")
         eng = self._engine()
         mel = audio_signal.to(device=eng.device, dtype=torch.float32)
         enc, enc_len = eng.encode(mel, length)

@@ -120,6 +120,24 @@ def rotary_half_tables(dk: int, base: float, max_len: int):
     return freqs.cos(), freqs.sin()
 
 
+RNNT_HEAD_FIELDS = ("rnnt_emb_gates", "rnnt_whh_t", "rnnt_wp_t", "rnnt_bp", "rnnt_enc_w", "rnnt_enc_b", "rnnt_wo", "rnnt_bo")
+
+
+def rnnt_head_packing(sd: Dict[str, Tensor]) -> Dict[str, Tensor]:
+    """The RNN-T head's device layout (gam_weights fields), fp32, computed on the tensors' device: the embedding table is
+    folded through the LSTM's input weights and both biases, W_hh and W_p are transposed."""
+    emb = sd["head.decoder.embed.weight"].double().clone()
+    # predict(None, None) starts from an all-zero embedding (gigaam/decoder.py:92-95) and nn.Embedding's padding_idx
+    # row is zero by construction but not enforced by load_state_dict: the table's blank row carries the biases only
+    emb[emb.shape[0] - 1].zero_()
+    w_ih, w_hh = sd["head.decoder.lstm.weight_ih_l0"].double(), sd["head.decoder.lstm.weight_hh_l0"].float()
+    bias = sd["head.decoder.lstm.bias_ih_l0"].double() + sd["head.decoder.lstm.bias_hh_l0"].double()
+    return {"rnnt_emb_gates": (emb @ w_ih.t() + bias).float(), "rnnt_whh_t": w_hh.t(),
+            "rnnt_wp_t": sd["head.joint.pred.weight"].float().t(), "rnnt_bp": sd["head.joint.pred.bias"].float(),
+            "rnnt_enc_w": sd["head.joint.enc.weight"].float(), "rnnt_enc_b": sd["head.joint.enc.bias"].float(),
+            "rnnt_wo": sd["head.joint.joint_net.1.weight"].float(), "rnnt_bo": sd["head.joint.joint_net.1.bias"].float()}
+
+
 class _WorkspaceCache:
     """Bounded LRU of scratch tensors of ONE kind (encode / log-mel / decode).  Eviction only drops this cache's
     reference: a CUDA graph that baked a workspace pointer keeps the tensor alive through `Engine.held_workspaces`."""
@@ -154,14 +172,16 @@ class Engine:
 
     WS_CACHE = 4      # workspaces kept per kind (distinct batch shapes)
 
-    PACK_FORMAT = 3   # bump when the packing order / layouts below change
+    PACK_FORMAT = 4   # bump when the packing order / layouts below change (4: the head is no longer cached)
 
     def __init__(self, cfg: Dict, state_dict: Dict[str, Tensor], device: torch.device, pack_cache: Optional[str] = None, *,
                  max_encoded_frames: Optional[int] = None):
         """`pack_cache`: path of an on-disk cache of the re-laid-out weights (SURVEY 8f-4).  When it exists and matches
         this cfg the load-time re-layout (BN folding, concatenations, permutations, fp16 casts, tables) is skipped and the
         packed tensors are uploaded as stored; otherwise it is written after packing.  Callers key the path by the
-        checkpoint's md5 (load_model does).
+        checkpoint's md5 (load_model does).  The cache holds the front end and the encoder only: the head is packed from
+        `state_dict` on every build, because head weights are trainable (a model's head may no longer be its checkpoint's)
+        and re-laying it out costs one small matmul.
 
         `max_encoded_frames`: longest T' (encoder frames, 40 ms each) this engine encodes; None = _lib.REL_POS_MAX_T (768,
         30.7 s), at most the encoder's pos_emb_max_len (5000 for the shipped checkpoints, just under 200 s).  A rel_pos
@@ -211,6 +231,8 @@ class Engine:
         self._pos_emb = rel_pos_embedding(self.max_encoded_frames, self.d_model).to(device) if self.rel_pos else None
         self.head_type = 0
         self.num_classes = 0
+        self._head_bufs: Dict[str, Tensor] = {}     # packed head tensors the handle points at, by gam_weights field
+        self.head_signature = None                  # set by the owning model: the head parameters this pack reflects
         self.max_symbols = 10
         gc = _lib.GamConfig()
         gc.sample_rate, gc.n_mels, gc.n_fft, gc.win_length, gc.hop_length, gc.center = sr, self.n_mels, self.n_fft, self.win, self.hop, int(self.center)
@@ -234,13 +256,13 @@ class Engine:
         if head is not None:
             if head["type"] == "ctc":
                 self.head_type, self.num_classes = 1, head["num_classes"]
-                gw.ctc_w = self._dev(sd["head.decoder_layers.0.weight"].reshape(self.num_classes, -1).float())
-                gw.ctc_b = self._dev(sd["head.decoder_layers.0.bias"].float())
+                gw.ctc_w = self._dev_head("ctc_w", sd["head.decoder_layers.0.weight"].reshape(self.num_classes, -1))
+                gw.ctc_b = self._dev_head("ctc_b", sd["head.decoder_layers.0.bias"])
             elif head["type"] == "emo":
                 # Linear(d, C) over the mean of the encoder frames (gigaam/model.py:272-293), fp32 like the reference's head
                 self.head_type, self.num_classes = 3, head["out_features"]
-                gw.emo_w = self._dev(sd["head.weight"].float())
-                gw.emo_b = self._dev(sd["head.bias"].float())
+                gw.emo_w = self._dev_head("emo_w", sd["head.weight"])
+                gw.emo_b = self._dev_head("emo_b", sd["head.bias"])
             else:
                 self._pack_rnnt(gw, gc, sd, head)
                 self.max_symbols = int(_cfg_get(cfg.get("decoding", {}), "max_symbols_per_step", 10))
@@ -268,6 +290,13 @@ class Engine:
                 self._pack_out.append(t.cpu().contiguous())
         t = t.to(self.device).contiguous()
         self._keep.append(t)
+        return t.data_ptr()
+
+    def _dev_head(self, name: str, t: Tensor) -> int:
+        """Upload one packed head tensor (fp32) outside the pack cache: it is neither replayed from nor written to it.
+        repack_head() later rewrites it in place."""
+        t = t.detach().to(device=self.device, dtype=torch.float32).contiguous()
+        self._head_bufs[name] = t
         return t.data_ptr()
 
     def _read_pack_cache(self, path: str) -> Optional[List[Tensor]]:
@@ -400,20 +429,25 @@ class Engine:
         self.head_type, self.num_classes = 2, jt["num_classes"]
         self.pred_hidden = dc["pred_hidden"]
         gc.pred_hidden, gc.joint_hidden = dc["pred_hidden"], jt["joint_hidden"]
-        emb = sd["head.decoder.embed.weight"].double().clone()
-        # predict(None, None) starts from an all-zero embedding (gigaam/decoder.py:92-95) and nn.Embedding's padding_idx
-        # row is zero by construction but not enforced by load_state_dict: the table's blank row carries the biases only
-        emb[jt["num_classes"] - 1].zero_()
-        w_ih, w_hh = sd["head.decoder.lstm.weight_ih_l0"].double(), sd["head.decoder.lstm.weight_hh_l0"].float()
-        bias = sd["head.decoder.lstm.bias_ih_l0"].double() + sd["head.decoder.lstm.bias_hh_l0"].double()
-        gw.rnnt_emb_gates = self._dev((emb @ w_ih.t() + bias).float())
-        gw.rnnt_whh_t = self._dev(w_hh.t())
-        gw.rnnt_wp_t = self._dev(sd["head.joint.pred.weight"].float().t())
-        gw.rnnt_bp = self._dev(sd["head.joint.pred.bias"].float())
-        gw.rnnt_enc_w = self._dev(sd["head.joint.enc.weight"].float())
-        gw.rnnt_enc_b = self._dev(sd["head.joint.enc.bias"].float())
-        gw.rnnt_wo = self._dev(sd["head.joint.joint_net.1.weight"].float())
-        gw.rnnt_bo = self._dev(sd["head.joint.joint_net.1.bias"].float())
+        packed = rnnt_head_packing(sd)
+        for name in RNNT_HEAD_FIELDS:
+            setattr(gw, name, self._dev_head(name, packed[name]))
+
+    def repack_head(self, sd: Dict[str, Tensor]) -> None:
+        """Re-lay the head weights out from `sd` (the model's current head parameters, key "head.*") into the device
+        buffers the handle already points at, on the current stream.  The encoder is untouched, the handle and any captured
+        CUDA graph stay valid, and nothing is written to the pack cache."""
+        if self.head_type == 1:
+            packed = {"ctc_w": sd["head.decoder_layers.0.weight"].reshape(self.num_classes, -1), "ctc_b": sd["head.decoder_layers.0.bias"]}
+        elif self.head_type == 2:
+            packed = rnnt_head_packing({k: v.to(self.device) for k, v in sd.items()})
+        elif self.head_type == 3:
+            packed = {"emo_w": sd["head.weight"], "emo_b": sd["head.bias"]}
+        else:
+            return
+        with torch.no_grad(), torch.cuda.device(self.device):
+            for name, t in packed.items():
+                self._head_bufs[name].copy_(t.detach().reshape(self._head_bufs[name].shape))
 
     # ------------------------------------------------------------------ calls
     def _stream(self) -> C.c_void_p:
@@ -568,6 +602,93 @@ class Engine:
                                            self._stream())
         _lib.check(self.lib, self.handle, rc, "gam_rnnt_predict")
         return g, h1, c1
+
+    # ------------------------------------------------------------------ backward passes of the head calls (head_grads.cu)
+    def _empty(self, *shape) -> Tensor:
+        return torch.empty(shape, dtype=torch.float32, device=self.device)
+
+    def _scratch(self, nbytes: int, what: str) -> Tensor:
+        if nbytes < 0:
+            raise ValueError(f"{what}: bad sizes")
+        return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
+
+    def rnnt_predict_train(self, x: Optional[Tensor], h: Optional[Tensor], c: Optional[Tensor], batch_size: int = 1
+                           ) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+        """rnnt_predict (same bits) that also returns the cell state of every step, c_seq [U, B, H]."""
+        if self.head_type != 2:
+            raise RuntimeError("model has no RNN-T head")
+        if x is not None:
+            assert x.is_cuda and x.dtype == torch.int64 and x.is_contiguous() and x.dim() == 2
+        B, U = (x.shape[0], x.shape[1]) if x is not None else (int(batch_size), 1)
+        H = self.pred_hidden
+        for name, t in (("h", h), ("c", c)):
+            if t is not None and (tuple(t.shape) != (B, H) or not t.is_contiguous()):
+                raise ValueError(f"predict: state {name} has shape {tuple(t.shape)}, expected ({B}, {H})")
+        g, h1, c1, c_seq = self._empty(B, U, H), self._empty(B, H), self._empty(B, H), self._empty(U, B, H)
+
+        def ptr(t):
+            return None if t is None else t.data_ptr()
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_rnnt_predict_train(self.handle, ptr(x), ptr(h), ptr(c), B, U, g.data_ptr(), h1.data_ptr(), c1.data_ptr(),
+                                                 c_seq.data_ptr(), self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_rnnt_predict_train")
+        return g, h1, c1, c_seq
+
+    def ctc_log_probs_backward(self, enc: Tensor, log_probs: Tensor, grad: Tensor, need_enc: bool, need_weights: bool):
+        """-> (d_enc [B, T, d] or None, dW [V+1, d] or None, db [V+1] or None); every tensor f32 contiguous on the device."""
+        B, T, d = enc.shape
+        d_enc = self._empty(B, T, d) if need_enc else None
+        dW, db = (self._empty(self.num_classes, d), self._empty(self.num_classes)) if need_weights else (None, None)
+        ws = self._scratch(int(self.lib.gam_ctc_log_probs_backward_workspace_bytes(self.handle, B, T)), "ctc backward")
+
+        def ptr(t):
+            return None if t is None else t.data_ptr()
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_ctc_log_probs_backward(self.handle, enc.data_ptr(), B, T, log_probs.data_ptr(), grad.data_ptr(),
+                                                     ws.data_ptr(), ws.numel(), ptr(d_enc), ptr(dW), ptr(db), self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_ctc_log_probs_backward")
+        return d_enc, dW, db
+
+    def rnnt_joint_backward(self, enc: Tensor, dec: Tensor, log_probs: Tensor, grad: Tensor, need_enc: bool, need_dec: bool,
+                            need_weights: bool):
+        """-> (d_enc [B, T, d], d_dec [B, U, H], dW_enc, db_enc, dW_pred, db_pred, dW_out, db_out); None where not needed."""
+        B, T, d = enc.shape
+        U, H = dec.shape[1], dec.shape[2]
+        J, V1 = self.gam_config.joint_hidden, self.num_classes
+        outs = [self._empty(B, T, d) if need_enc else None, self._empty(B, U, H) if need_dec else None]
+        if need_weights:
+            outs += [self._empty(J, d), self._empty(J), self._empty(J, H), self._empty(J), self._empty(V1, J), self._empty(V1)]
+        else:
+            outs += [None] * 6
+        ws = self._scratch(int(self.lib.gam_rnnt_joint_backward_workspace_bytes(self.handle, B, T, U)), "joint backward")
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_rnnt_joint_backward(self.handle, enc.data_ptr(), dec.data_ptr(), B, T, U, log_probs.data_ptr(),
+                                                  grad.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                  *[None if t is None else t.data_ptr() for t in outs], self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_rnnt_joint_backward")
+        return tuple(outs)
+
+    def rnnt_predict_backward(self, x: Optional[Tensor], h: Optional[Tensor], c: Optional[Tensor], g: Tensor, c_seq: Tensor,
+                              grad_g: Tensor, grad_h1: Optional[Tensor], grad_c1: Optional[Tensor], embed: Tensor, w_ih: Tensor,
+                              w_hh: Tensor, need_state: bool, need_weights: bool):
+        """BPTT through rnnt_predict_train -> (d_h0, d_c0 [B, H], d_embed [V+1, H], dW_ih, dW_hh [4H, H], d_bias [4H]); None
+        where not needed.  embed / w_ih / w_hh: the module's weights, f32 contiguous on the device."""
+        B, U, H = g.shape
+        V1 = self.num_classes
+        outs = [self._empty(B, H), self._empty(B, H)] if need_state else [None, None]
+        outs += ([self._empty(V1, H), self._empty(4 * H, H), self._empty(4 * H, H), self._empty(4 * H)] if need_weights
+                 else [None] * 4)
+        ws = self._scratch(int(self.lib.gam_rnnt_predict_backward_workspace_bytes(self.handle, B, U)), "predict backward")
+
+        def ptr(t):
+            return None if t is None else t.data_ptr()
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_rnnt_predict_backward(self.handle, ptr(x), ptr(h), ptr(c), B, U, g.data_ptr(), c_seq.data_ptr(),
+                                                    grad_g.data_ptr(), ptr(grad_h1), ptr(grad_c1), embed.data_ptr(), w_ih.data_ptr(),
+                                                    w_hh.data_ptr(), ws.data_ptr(), ws.numel(), *[ptr(t) for t in outs],
+                                                    self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_rnnt_predict_backward")
+        return tuple(outs)
 
     def emo_head(self, enc_btd: Tensor, enc_len: Optional[Tensor]) -> Tuple[Tensor, Tensor, Tensor]:
         """enc [B, T, d] f32 contiguous, len [B] or None (all T frames) -> (pooled [B, d], logits [B, C], probs [B, C]) f32

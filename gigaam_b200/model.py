@@ -118,8 +118,24 @@ class GigaAM(nn.Module):
             sd = {k: v for k, v in self.state_dict().items()}
             eng = Engine(self._engine_cfg(), sd, dev, pack_cache=self._pack_cache_path(),
                          max_encoded_frames=self.__dict__.get("_max_encoded_frames"))
+            eng.head_signature = self._head_signature()
             self.__dict__["_engine_obj"] = eng
+        elif eng.head_signature is not None:
+            sig = self._head_signature()
+            if sig != eng.head_signature:      # an optimizer step or copy_ changed a head weight: repack it in place
+                eng.repack_head({f"head.{k}": v for k, v in self.head.state_dict().items()})
+                eng.head_signature = sig
         return eng
+
+    def _head_signature(self):
+        """(storage, version counter) of every head parameter: changes with optimizer.step(), copy_() and friends."""
+        head = self._modules.get("head")
+        return None if head is None else tuple((p.data_ptr(), p._version) for p in head.parameters())
+
+    def _check_frozen_encoder(self, *modules: nn.Module) -> None:
+        if torch.is_grad_enabled() and any(p.requires_grad for m in modules for p in m.parameters()):
+            raise NotImplementedError("the encoder is inference-only; freeze it (requires_grad_(False) on the encoder and "
+                                      "preprocessor) and train the head on its output")
 
     def _pack_cache_path(self) -> Optional[str]:
         """On-disk cache of the packed weights, set by load_model for checkpoints read from a file: keyed by the
@@ -139,6 +155,9 @@ class GigaAM(nn.Module):
 
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
         res = super().load_state_dict(state_dict, strict=strict, assign=assign)
+        # the weights may no longer be the checkpoint's: the next engine packs this state_dict instead of replaying the
+        # checkpoint's pack cache (load_model sets the cache key again after loading the checkpoint itself)
+        self.__dict__.pop("_pack_cache_base", None)
         self._invalidate_engine()
         return res
 
@@ -149,7 +168,9 @@ class GigaAM(nn.Module):
 
     # ---- reference surface
     def forward(self, features: Tensor, feature_lengths: Tensor) -> Tuple[Tensor, Tensor]:
-        """wav [B, N], lengths [B] -> (encoded [B, d_model, T'], encoded_len [B] int32)  (gigaam/model.py:27-37)"""
+        """wav [B, N], lengths [B] -> (encoded [B, d_model, T'], encoded_len [B] int32)  (gigaam/model.py:27-37).  The
+        encoder is inference-only: with grad enabled and an encoder or preprocessor parameter requiring grad this raises."""
+        self._check_frozen_encoder(self.preprocessor, self.encoder)
         features, feature_lengths = self.preprocessor(features, feature_lengths)
         return self.encoder(features, feature_lengths)
 

@@ -205,6 +205,40 @@ int gam_rnnt_joint(gam_handle* h, const float* enc, const float* dec, int32_t B,
  * succeeds.  One launch per step. */
 int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g, float* h1,
                      float* c1, void* stream);
+/* gam_rnnt_predict (same bits) that also keeps the cell state of every step: c_seq device f32 [U, B, pred_hidden], the
+ * operand gam_rnnt_predict_backward needs. */
+int gam_rnnt_predict_train(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g,
+                           float* h1, float* c1, float* c_seq, void* stream);
+
+/* ---- backward passes of the three head calls above, for training the heads on a frozen encoder.  fp32, stream-ordered, no
+ * host synchronisation and no atomics: every sum runs in an order fixed by the sizes, so two calls on the same inputs give
+ * bit-identical gradients.  They use the handle's current head weights.  Every output pointer may be NULL (not computed),
+ * except that a weight gradient and its bias gradient go together.  Each needs a workspace of *_workspace_bytes().
+ *
+ * CTC: grad = dL/dlog_probs [B, T, V+1], log_probs = gam_ctc_log_probs's output.  dlogit = grad - exp(log_probs) * rowsum(grad);
+ *   d_enc [B, T, d_model] = dlogit W, dW [V+1, d_model] = sum over frames of dlogit^T enc, db [V+1] = sum of dlogit. */
+int64_t gam_ctc_log_probs_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t T);
+int gam_ctc_log_probs_backward(gam_handle* h, const float* enc, int32_t B, int32_t T, const float* log_probs, const float* grad,
+                               void* workspace, int64_t workspace_bytes, float* d_enc, float* dW, float* db, void* stream);
+/* Joint: grad [B, T, U, V+1], log_probs = gam_rnnt_joint's output.  The hidden rows relu(E[b,t] + P[b,u]) are rebuilt from the
+ * two projections, never stored; their gradient dhid [B, T, U, joint_hidden] is kept in the workspace.  Outputs: d_enc
+ * [B, T, d_model], d_dec [B, U, pred_hidden], and the gradients of joint.enc (dW_enc [J, d_model], db_enc [J]), joint.pred
+ * (dW_pred [J, pred_hidden], db_pred [J]) and joint.joint_net.1 (dW_out [V+1, J], db_out [V+1]).  64-bit offsets. */
+int64_t gam_rnnt_joint_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_rnnt_joint_backward(gam_handle* h, const float* enc, const float* dec, int32_t B, int32_t T, int32_t U, const float* log_probs,
+                            const float* grad, void* workspace, int64_t workspace_bytes, float* d_enc, float* d_dec, float* dW_enc,
+                            float* db_enc, float* dW_pred, float* db_pred, float* dW_out, float* db_out, void* stream);
+/* Prediction LSTM: BPTT over the U steps of gam_rnnt_predict_train (x, h0, c0 as given to it; g and c_seq its outputs), one
+ * launch per step.  grad_g [B, U, H] is required, grad_h1 / grad_c1 [B, H] may be NULL (zero).  embed [V+1, H], w_ih [4H, H],
+ * w_hh [4H, H] are the module's lstm / embed weights (w_hh must match the packed one).  Outputs: d_h0, d_c0 [B, H]; d_embed
+ * [V+1, H] with a zero blank row (nn.Embedding's padding_idx); dW_ih, dW_hh [4H, H]; d_bias [4H], the gradient of both
+ * bias_ih_l0 and bias_hh_l0.  An utterance with an id outside [0, V] gets NaN in its d_h0 / d_c0 (and the weight gradients it
+ * feeds).  pred_hidden <= 614. */
+int64_t gam_rnnt_predict_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t U);
+int gam_rnnt_predict_backward(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, const float* g,
+                              const float* c_seq, const float* grad_g, const float* grad_h1, const float* grad_c1, const float* embed,
+                              const float* w_ih, const float* w_hh, void* workspace, int64_t workspace_bytes, float* d_h0, float* d_c0,
+                              float* d_embed, float* dW_ih, float* dW_hh, float* d_bias, void* stream);
 
 /* Emotion head  <- gigaam/model.py:272-293 (GigaAMEmo.get_probs / forward_for_export): the mean of utterance b's encoder
  * frames, logits = W mean + b, probs = softmax(logits), fp32.
