@@ -60,7 +60,7 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_emo_head", "gam_test_frames_split", "gam_test_mel_log", "gam_test_rnnt_greedy",
            "gam_rnnt_predict_train", "gam_ctc_log_probs_backward_workspace_bytes", "gam_ctc_log_probs_backward",
            "gam_rnnt_joint_backward_workspace_bytes", "gam_rnnt_joint_backward", "gam_rnnt_predict_backward_workspace_bytes",
-           "gam_rnnt_predict_backward")
+           "gam_rnnt_predict_backward", "gam_test_gemm_used_slots")
 
 
 def lib_path() -> Path:
@@ -138,6 +138,8 @@ def load() -> C.CDLL:
     lib.gam_emo_head.restype = C.c_int
     lib.gam_test_gemm.argtypes = [H, i32, c_vp, c_vp, i32, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, i32, C.c_float, i32, c_vp,
                                   c_vp]
+    lib.gam_test_gemm_used_slots.argtypes = [H]
+    lib.gam_test_gemm_used_slots.restype = C.c_int
     lib.gam_test_gemm_conv.argtypes = [H, i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, i32, i32, i32, i32, c_vp]
     lib.gam_test_layernorm.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, c_vp, i32, c_vp]
     lib.gam_test_ln_rope.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, c_vp, c_vp, i32, i32, c_vp]

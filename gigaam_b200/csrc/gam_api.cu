@@ -33,18 +33,33 @@ static int init_encode() {
   return 0;
 }
 
-// 2-D fp16 row-major tensor [rows, cols] with row pitch ld_elems; box = [box_rows, box_cols], SWIZZLE_128B
-int make_tmap_2d_f16(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
-                     uint32_t box_cols) {
+// 2-D row-major tensor [rows, cols] of `esz`-byte elements with row pitch ld_elems; box = [box_rows, box_cols], SWIZZLE_128B
+static int make_tmap_2d(CUtensorMap* m, CUtensorMapDataType type, uint64_t esz, const void* base, uint64_t rows, uint64_t cols,
+                        uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols) {
   if (init_encode() != 0) return -1;
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld_elems * 2};
+  cuuint64_t strides[1] = {ld_elems * esz};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = g_encode(m, type, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : -static_cast<int>(r) - 1000;
+}
+int make_tmap_2d_f16(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
+                     uint32_t box_cols) {
+  return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, rows, cols, ld_elems, box_rows, box_cols);
+}
+static int make_tmap_2d_f32(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
+                            uint32_t box_cols) {
+  return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, rows, cols, ld_elems, box_rows, box_cols);
+}
+
+// GEMM output columns [rows, cols] at `base`, pitch ld_elems, in boxes of one store slot of the GEMM
+// (64 rows x 128 bytes: 64 fp16 or 32 fp32 columns).  Nonzero when TMA cannot address it (base or pitch not 16-byte
+// aligned): the launch then stores every tile directly.
+static int make_tmap_out(CUtensorMap* m, const void* base, bool f32, uint64_t rows, uint64_t cols, uint64_t ld_elems) {
+  if (reinterpret_cast<uintptr_t>(base) % 16 != 0 || (ld_elems * (f32 ? 4 : 2)) % 16 != 0) return -1;
+  return f32 ? make_tmap_2d_f32(m, base, rows, cols, ld_elems, 64, 32) : make_tmap_2d_f16(m, base, rows, cols, ld_elems, 64, 64);
 }
 
 // 4-D channels-last activation [B, T1, F1, C] fp16 for the stride-2 3x3 conv: box = 8 time x 16 freq x 64 ch,
@@ -101,6 +116,9 @@ struct Plan {
   float* x = nullptr;
   int64_t bytes = 0;
   CUtensorMap m_s1, m_s2, m_a16, m_r16, m_hid, m_qkv, m_qkv4, m_o16;
+  // GEMM outputs (make_tmap_out): big16 at d_ff / 3d / 4d columns, its q|k and v column ranges of the unmerged projection, g16,
+  // and x (fp32, the sub_out GEMM)
+  CUtensorMap o_hid, o_qkv, o_qkv4, o_qk, o_v, o_g16, o_x;
 };
 
 }  // namespace gam
@@ -120,6 +138,7 @@ struct gam_handle {
   int gemm_clusters = 0;   // co-resident clusters of the GEMM kernel (gemm_init)
   int max_t = GAM_REL_POS_MAX_T;   // longest T' (cfg.max_encoded_frames, 0 = default); rel_pos tables have 2*max_t-1 rows
   int64_t launches = 0;
+  int test_gemm_slots = 0;   // the last gam_test_gemm launch could store through the shared-memory slots
   void* comm = nullptr;      // ncclComm_t of gam_comm_init
   int comm_rank = 0, comm_nranks = 1;
   std::string err;
@@ -257,6 +276,13 @@ Plan* get_plan(gam_handle* h, int B, int64_t M, void* ws, int64_t ws_bytes) {
   rc |= make_tmap_2d_f16(&p->m_qkv, p->big16, R, 3 * d, 3 * d, 128, 64);
   rc |= make_tmap_2d_f16(&p->m_qkv4, p->big16, R, 4 * d, 4 * d, 128, 64);
   rc |= make_tmap_2d_f16(&p->m_o16, p->o16, R, d, d, 128, 64);
+  rc |= make_tmap_out(&p->o_hid, p->big16, false, R, c.d_ff, c.d_ff);
+  rc |= make_tmap_out(&p->o_qkv, p->big16, false, R, 3 * d, 3 * d);
+  rc |= make_tmap_out(&p->o_qkv4, p->big16, false, R, 4 * d, 4 * d);
+  rc |= make_tmap_out(&p->o_qk, p->big16, false, R, 2 * d, 3 * d);
+  rc |= make_tmap_out(&p->o_v, p->big16 + 2 * d, false, R, d, 3 * d);
+  rc |= make_tmap_out(&p->o_g16, p->g16, false, R, d, d);
+  rc |= make_tmap_out(&p->o_x, p->x, true, R, d, d);
   if (rc != 0) {
     fail(h, -2, "cuTensorMapEncodeTiled failed for activation maps (rc=%d)", rc);
     delete p;
@@ -515,7 +541,8 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
     if (rc) return fail(h, -4, "subsampling launch rejected (rc=%d)", rc);
     {
       PROF(PC_GEMM_SUBOUT);
-      rc |= launch_gemm(GEMM_BIAS_F32, &p->m_s2, &h->m_sub_out_w, R, d, p->F2 * d, h->w.sub_out_b, nullptr, p->x, d, 1.f, ncl, s, 0, rdev);
+      rc |= launch_gemm(GEMM_BIAS_F32, &p->m_s2, &h->m_sub_out_w, R, d, p->F2 * d, h->w.sub_out_b, nullptr, p->x, d, 1.f, ncl, s, 0, rdev,
+                        &p->o_x);
     }
   } else {
     // conv1d subsampling (gigaam/encoder.py:59-70 with Conv1d): two k-tap / stride-2 implicit GEMMs over time-major data
@@ -554,7 +581,8 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
     const LayerMaps& m = h->lmaps[l];
     // x += 0.5 * FF1(LN(x))                                     (encoder.py:480-483)
     { PROF(PC_GEMM_FFN_UP);
-      rc |= launch_gemm(GEMM_BIAS_SILU_F16, &p->m_a16, &m.ff1_w1, R, c.d_ff, d, w.ff1_b1, nullptr, p->big16, c.d_ff, 1.f, ncl, s, 0, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_SILU_F16, &p->m_a16, &m.ff1_w1, R, c.d_ff, d, w.ff1_b1, nullptr, p->big16, c.d_ff, 1.f, ncl, s, 0, rdev,
+                        &p->o_hid); }
     { PROF(PC_GEMM_FFN_DOWN);
       rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_hid, &m.ff1_w2, R, d, c.d_ff, w.ff1_b2, p->x, p->x, d, 0.5f, ncl, s, zz, rdev); }
     // x += W_o attn(q = W_q rope(u), k = W_k rope(u), v = W_v u), u = LN(x)   (encoder.py:485-487, 236-277)
@@ -565,13 +593,16 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
       bool merged = false;
       if (m.qkv_merged) {
         PROF(PC_GEMM_QKV);
-        merged = launch_gemm_dual_a(&p->m_r16, &p->m_a16, 2 * d, &m.w_qkv, R, 3 * d, d, w.b_qk, p->big16, 3 * d, ncl, s, zz, rdev) == 0;
+        merged = launch_gemm_dual_a(&p->m_r16, &p->m_a16, 2 * d, &m.w_qkv, R, 3 * d, d, w.b_qk, p->big16, 3 * d, ncl, s, zz, rdev,
+                                    &p->o_qkv) == 0;
       }
       if (!merged) {
         { PROF(PC_GEMM_QKV);
-          rc |= launch_gemm(GEMM_BIAS_F16, &p->m_r16, &m.w_qk, R, 2 * d, d, w.b_qk, nullptr, p->big16, 3 * d, 1.f, ncl, s, zz, rdev); }
+          rc |= launch_gemm(GEMM_BIAS_F16, &p->m_r16, &m.w_qk, R, 2 * d, d, w.b_qk, nullptr, p->big16, 3 * d, 1.f, ncl, s, zz, rdev,
+                            &p->o_qk); }
         { PROF(PC_GEMM_QKV);
-          rc |= launch_gemm(GEMM_BIAS_F16, &p->m_a16, &m.w_v, R, d, d, w.b_v, nullptr, p->big16 + 2 * d, 3 * d, 1.f, ncl, s, zz, rdev); }
+          rc |= launch_gemm(GEMM_BIAS_F16, &p->m_a16, &m.w_v, R, d, d, w.b_v, nullptr, p->big16 + 2 * d, 3 * d, 1.f, ncl, s, zz, rdev,
+                            &p->o_v); }
       }
       { PROF(PC_ATTENTION);
         rc |= launch_attention(&p->m_qkv, p->plen, p->cu, p->o16, B, p->T2, c.n_heads, dk, d, s); }
@@ -580,7 +611,8 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
       { PROF(PC_LAYERNORM);
         launch_ln_f16(p->x, w.ln_att_g, w.ln_att_b, p->a16, R, rdev, 0, s); }
       { PROF(PC_GEMM_QKV);
-        rc |= launch_gemm(GEMM_BIAS_F16, &p->m_a16, &m.w_qkv_rel, R, 4 * d, d, w.b_qkv_rel, nullptr, p->big16, 4 * d, 1.f, ncl, s, zz, rdev); }
+        rc |= launch_gemm(GEMM_BIAS_F16, &p->m_a16, &m.w_qkv_rel, R, 4 * d, d, w.b_qkv_rel, nullptr, p->big16, 4 * d, 1.f, ncl, s, zz, rdev,
+                          &p->o_qkv4); }
       { PROF(PC_ATTENTION);
         rc |= launch_attention_relpos(&p->m_qkv4, &m.pos_proj, h->max_t, p->plen, p->cu, p->o16, B, p->T2, c.n_heads, dk, d, s); }
     }
@@ -590,7 +622,7 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
     { PROF(PC_LAYERNORM);
       launch_ln_f16(p->x, w.ln_conv_g, w.ln_conv_b, p->a16, R, rdev, 0, s); }
     { PROF(PC_GEMM_GLU);
-      rc |= launch_gemm(GEMM_BIAS_GLU_F16, &p->m_a16, &m.pw1, R, 2 * d, d, w.pw1_b, nullptr, p->g16, d, 1.f, ncl, s, zz, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_GLU_F16, &p->m_a16, &m.pw1, R, 2 * d, d, w.pw1_b, nullptr, p->g16, d, 1.f, ncl, s, zz, rdev, &p->o_g16); }
     { PROF(PC_DWCONV);
       if (c.conv_norm == 0)
         rc |= launch_dwconv_bn_silu(p->g16, w.dw_w, w.dw_b, p->len2, p->cu, p->plen, p->o16, B, p->T2, c.conv_kernel_size, s);
@@ -603,7 +635,8 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
     { PROF(PC_LAYERNORM);
       launch_ln_f16(p->x, w.ln_ff2_g, w.ln_ff2_b, p->a16, R, rdev, 0, s); }
     { PROF(PC_GEMM_FFN_UP);
-      rc |= launch_gemm(GEMM_BIAS_SILU_F16, &p->m_a16, &m.ff2_w1, R, c.d_ff, d, w.ff2_b1, nullptr, p->big16, c.d_ff, 1.f, ncl, s, zz, rdev); }
+      rc |= launch_gemm(GEMM_BIAS_SILU_F16, &p->m_a16, &m.ff2_w1, R, c.d_ff, d, w.ff2_b1, nullptr, p->big16, c.d_ff, 1.f, ncl, s, zz, rdev,
+                        &p->o_hid); }
     { PROF(PC_GEMM_FFN_DOWN);
       rc |= launch_gemm(GEMM_BIAS_RES_F32, &p->m_hid, &m.ff2_w2, R, d, c.d_ff, w.ff2_b2, p->x, p->x, d, 0.5f, ncl, s, 0, rdev); }
     // x = LN_out(x) (+ next layer's first LN fused)                (encoder.py:497)
@@ -1064,20 +1097,26 @@ int gam_test_gemm(gam_handle* h, int32_t kind, const void* A, const void* A2, in
   const size_t esz = (kind == GEMM_BIAS_RES_F32 || kind == GEMM_BIAS_F32 || kind == kTestGemmPower) ? 4 : 2;
   void* o = static_cast<char*>(out) + col0 * esz;
   const float* r = res ? reinterpret_cast<const float*>(reinterpret_cast<const char*>(res) + col0 * esz) : nullptr;
+  // output map of the shared-memory store path; a column range TMA cannot address is stored directly
+  CUtensorMap to;
+  const bool has_to = kind != kTestGemmPower && kind != GEMM_BIAS_RES_F32 && make_tmap_out(&to, o, esz == 4, M, ncol, ldo) == 0;
+  h->test_gemm_slots = has_to ? 1 : 0;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   {
     PROF(PC_MISC);
     if (kind == kTestGemmPower)
       rc = launch_gemm_power(&ta, &tw, M, N, K, static_cast<float*>(o), ldo, h->gemm_clusters, s);
     else if (A2)
-      rc = launch_gemm_dual_a(&ta, &ta2, n1, &tw, M, N, K, bias, o, ldo, h->gemm_clusters, s, reverse, m_dev);
+      rc = launch_gemm_dual_a(&ta, &ta2, n1, &tw, M, N, K, bias, o, ldo, h->gemm_clusters, s, reverse, m_dev, has_to ? &to : nullptr);
     else
-      rc = launch_gemm(kind, &ta, &tw, M, N, K, bias, r, o, ldo, scale, h->gemm_clusters, s, reverse, m_dev);
+      rc = launch_gemm(kind, &ta, &tw, M, N, K, bias, r, o, ldo, scale, h->gemm_clusters, s, reverse, m_dev, has_to ? &to : nullptr);
   }
   if (rc) return fail(h, -4, "gemm launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "test_gemm");
   return 0;
 }
+
+int gam_test_gemm_used_slots(gam_handle* h) { return h->test_gemm_slots; }
 
 int gam_test_gemm_conv(gam_handle* h, int32_t conv1d, const void* A, const void* W, const float* bias, const int32_t* len_out,
                        const int32_t* cu, const int32_t* plen, void* out, int32_t out_frames, int32_t B, int32_t T_in, int32_t F1,

@@ -13,14 +13,18 @@ constexpr int kBN = kG2BN;
 
 // p.num_m_tiles counts 128-row blocks; the grid is one cluster of kG2Cluster CTAs per co-resident pair of m-blocks
 // (max_clusters: gemm_init's count), each walking the list of tile pairs
+// to: output map of the shared-memory store path (gemm_sm90.cuh); without it (null) every tile stores straight from the
+// fragment
 template <int EPI, int AMODE>
 int launch_v2(const CUtensorMap* ta, const CUtensorMap* tw, GemmParams p, int max_clusters, cudaStream_t s,
-              const CUtensorMap* ta2 = nullptr) {
+              const CUtensorMap* ta2 = nullptr, const CUtensorMap* to = nullptr) {
   auto kern = gemm_f16_tn_kernel<EPI, AMODE>;
   const int pairs = (p.num_m_tiles + kG2Cluster - 1) / kG2Cluster * p.num_n_tiles;
   const int nclusters = pairs < max_clusters ? pairs : max_clusters;
   if (nclusters <= 0) return 0;
-  return launch_k(kern, dim3(nclusters * kG2Cluster), dim3(kG2Threads), kG2Smem, s, *ta, ta2 ? *ta2 : *ta, *tw, p) == cudaSuccess
+  p.tma_out = gemm_tma_store<EPI, AMODE>() && to != nullptr;
+  return launch_k(kern, dim3(nclusters * kG2Cluster), dim3(kG2Threads), gemm_smem_bytes<EPI, AMODE>(), s, *ta, ta2 ? *ta2 : *ta, *tw, to ? *to : *ta,
+                  p) == cudaSuccess
              ? 0
              : -2;
 }
@@ -30,11 +34,12 @@ int launch_v2(const CUtensorMap* ta, const CUtensorMap* tw, GemmParams p, int ma
 template <int EPI, int AMODE>
 int init_one(int* clusters) {
   auto kern = gemm_f16_tn_kernel<EPI, AMODE>;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kG2Smem) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem_bytes<EPI, AMODE>()) != cudaSuccess)
+    return -1;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(kG2Cluster);
   cfg.blockDim = dim3(kG2Threads);
-  cfg.dynamicSmemBytes = kG2Smem;
+  cfg.dynamicSmemBytes = gemm_smem_bytes<EPI, AMODE>();
   int n = 0;
   if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) return -1;
   if (n < *clusters) *clusters = n;
@@ -59,7 +64,8 @@ int gemm_init(int* max_clusters) {
 }
 
 int launch_gemm(int kind, const CUtensorMap* ta, const CUtensorMap* tw, int M, int N, int K, const float* bias,
-                const float* res, void* out, int ldo, float scale, int max_clusters, cudaStream_t s, int reverse, const int* m_dev) {
+                const float* res, void* out, int ldo, float scale, int max_clusters, cudaStream_t s, int reverse, const int* m_dev,
+                const CUtensorMap* to) {
   if (N % kBN != 0 || K % kGemmBK != 0 || M <= 0) return -1;
   GemmParams p{};
   p.M = M;
@@ -75,11 +81,11 @@ int launch_gemm(int kind, const CUtensorMap* ta, const CUtensorMap* tw, int M, i
   p.scale = scale;
   p.reverse = reverse;
   switch (kind) {
-    case GEMM_BIAS_F16: return launch_v2<EPI_BIAS_F16, A_2D>(ta, tw, p, max_clusters, s);
-    case GEMM_BIAS_SILU_F16: return launch_v2<EPI_BIAS_SILU_F16, A_2D>(ta, tw, p, max_clusters, s);
-    case GEMM_BIAS_GLU_F16: return launch_v2<EPI_BIAS_GLU_F16, A_2D>(ta, tw, p, max_clusters, s);
+    case GEMM_BIAS_F16: return launch_v2<EPI_BIAS_F16, A_2D>(ta, tw, p, max_clusters, s, nullptr, to);
+    case GEMM_BIAS_SILU_F16: return launch_v2<EPI_BIAS_SILU_F16, A_2D>(ta, tw, p, max_clusters, s, nullptr, to);
+    case GEMM_BIAS_GLU_F16: return launch_v2<EPI_BIAS_GLU_F16, A_2D>(ta, tw, p, max_clusters, s, nullptr, to);
     case GEMM_BIAS_RES_F32: return launch_v2<EPI_BIAS_RES_F32, A_2D>(ta, tw, p, max_clusters, s);
-    case GEMM_BIAS_F32: return launch_v2<EPI_BIAS_F32, A_2D>(ta, tw, p, max_clusters, s);
+    case GEMM_BIAS_F32: return launch_v2<EPI_BIAS_F32, A_2D>(ta, tw, p, max_clusters, s, nullptr, to);
     default: return -1;
   }
 }
@@ -87,7 +93,8 @@ int launch_gemm(int kind, const CUtensorMap* ta, const CUtensorMap* tw, int M, i
 // D[:, :n1] = A1 W[:n1]^T + b, D[:, n1:] = A2 W[n1:]^T + b  (fp16 out) in ONE launch of the persistent kernel: more tiles
 // per launch = less wave quantisation and one launch less.
 int launch_gemm_dual_a(const CUtensorMap* ta1, const CUtensorMap* ta2, int n1, const CUtensorMap* tw, int M, int N, int K,
-                       const float* bias, void* out, int ldo, int max_clusters, cudaStream_t s, int reverse, const int* m_dev) {
+                       const float* bias, void* out, int ldo, int max_clusters, cudaStream_t s, int reverse, const int* m_dev,
+                       const CUtensorMap* to) {
   if (N % kBN != 0 || n1 % kBN != 0 || n1 <= 0 || n1 >= N || K % kGemmBK != 0 || M <= 0) return -1;
   GemmParams p{};
   p.M = M;
@@ -102,7 +109,7 @@ int launch_gemm_dual_a(const CUtensorMap* ta1, const CUtensorMap* ta2, int n1, c
   p.scale = 1.f;
   p.a1_nblks = n1 / kBN;
   p.reverse = reverse;
-  return launch_v2<EPI_BIAS_F16, A_2D>(ta1, tw, p, max_clusters, s, ta2);
+  return launch_v2<EPI_BIAS_F16, A_2D>(ta1, tw, p, max_clusters, s, ta2, to);
 }
 
 int launch_gemm_conv(const CUtensorMap* ta4, const CUtensorMap* tw, int B, int T2, int C, int N, const float* bias,

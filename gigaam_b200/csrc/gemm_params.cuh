@@ -62,6 +62,10 @@ struct GemmParams {
   // read in the producer's own order, a buffer that does not fit is evicted just ahead of the reader (LRU) and every
   // byte comes from DRAM.
   int reverse;
+  // A_2D epilogues but EPI_BIAS_RES_F32 and EPI_POWER_F32: tiles whose 128 rows all lie below the live row count leave
+  // through shared memory and TMA bulk stores (tmap_out); 0 = every tile stores directly from the fragment (the output
+  // could not be described by a tensor map)
+  int tma_out;
 };
 
 constexpr int kGemmBM = 128;

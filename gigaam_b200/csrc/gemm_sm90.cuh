@@ -11,6 +11,20 @@
 // straight from the wgmma fragment (a thread holds two adjacent columns of two rows per 8-column block; four threads
 // cover 32 contiguous bytes of a row, so every access fills whole 32-byte sectors).
 //
+// How a finished tile leaves the SM (A_2D epilogues but the residual and the DFT power): a tile whose 128 rows all lie
+// below the live row count goes out through shared memory.  Each consumer warpgroup owns two 8 KB slots of 64 rows x 128
+// bytes (64 fp16 or 32 fp32 columns, laid out as a SWIZZLE_128B TMA box, so the fragment writes are free of bank
+// conflicts) and stores its 64 rows chunk by chunk, alternating slots: the leader waits until the bulk store issued from
+// the slot two chunks ago has read it (wait_group.read 1), the warpgroup writes the chunk, fences it to the async proxy
+// and the leader issues the bulk store.  The warpgroup goes on to the next tile without waiting for the stores, so the
+// HBM traffic of the epilogue runs under the next main loop instead of stalling the tensor cores.  The tile that straddles the live row count, the
+// phantom / dead half of a pair and the conv modes store straight from the fragment: no row at or past the live count is
+// ever written.  EPI_BIAS_RES_F32 stores directly too: its residual loads stay on the epilogue's critical path, and
+// loaded one chunk at a time for the slots they made more round trips than the direct path's batches (measured slower on
+// an H100, with and without an L2 prefetch of the residual; DESIGN.md §7).  Only the instantiations that use the slots reserve them
+// (gemm_smem_bytes): the others keep the shared memory, and so the L1 share of the unified L1 / shared memory, they had
+// without them.
+//
 // Clusters of two CTAs share the weight tile.  The persistent grid walks pairs of tiles, m-blocks 2i and 2i + 1 of one
 // n-block; the CTA of cluster rank r computes m-block 2i + r and loads W rows 128 r .. 128 r + 127 of the n-block with a
 // TMA multicast into the same stage of both CTAs.  Each CTA so fetches 16 KB of A and 16 KB of W per k-block instead of
@@ -35,8 +49,20 @@ constexpr int kG2BN = 256;
 constexpr int kG2ABytes = 128 * 64 * 2;       // 16 KB: 128 rows of A
 constexpr int kG2BBytes = 256 * 64 * 2;       // 32 KB: 256 rows of W
 constexpr int kG2StageBytes = kG2ABytes + kG2BBytes;
+constexpr int kG2SlotBytes = 64 * 128;          // 8 KB store slot: 64 rows x 128 bytes
+constexpr int kG2StoreBytes = 2 * 2 * kG2SlotBytes;   // two slots per consumer warpgroup
 constexpr int kG2BarBytes = 256;
-constexpr int kG2Smem = kG2Stages * kG2StageBytes + kG2BarBytes + 1024;
+
+template <int EPI, int AMODE>
+constexpr bool gemm_tma_store() {
+  return AMODE == A_2D && EPI != EPI_POWER_F32 && EPI != EPI_BIAS_RES_F32;
+}
+// dynamic shared memory: stages | store slots (only where used) | barriers, + 1 KB to align the base to 1024 bytes.
+// 230 656 B with the slots (of the 232 448 B opt-in), 197 888 B without
+template <int EPI, int AMODE>
+constexpr int gemm_smem_bytes() {
+  return kG2Stages * kG2StageBytes + (gemm_tma_store<EPI, AMODE>() ? kG2StoreBytes : 0) + kG2BarBytes + 1024;
+}
 
 // output row of local row `lr` (0..127) of 128-row block m_blk: whether it exists (is stored) and whether it lies
 // inside the utterance's valid length (conv modes: ReLU value, else 0)
@@ -69,15 +95,85 @@ __device__ __forceinline__ GemmRow gemm_row(const GemmParams& p, int m_rows, int
   return g;
 }
 
+// The epilogue arithmetic of fragment block i (columns 8 i + cq, + 1 of the tile) of row half h, shared by both store paths.
+// bias (+ scale * residual) (+ SiLU); res is read only by EPI_BIAS_RES_F32
+template <int EPI>
+__device__ __forceinline__ float2 bias_act_pair(const float (&acc)[128], const float* bsrc, int i, int h, int cq, const float2& res,
+                                                float scale) {
+  const float2 bv = __ldg(reinterpret_cast<const float2*>(bsrc + 8 * i + cq));
+  float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
+  if constexpr (EPI == EPI_BIAS_RES_F32) {
+    x0 = fmaf(scale, x0, res.x);
+    x1 = fmaf(scale, x1, res.y);
+  }
+  if constexpr (EPI == EPI_BIAS_SILU_F16) { x0 = silu_f(x0); x1 = silu_f(x1); }
+  return make_float2(x0, x1);
+}
+// GLU, i < 16: value columns [0,128) of the tile, gate columns [128,256)
+__device__ __forceinline__ uint32_t glu_pair(const float (&acc)[128], const float* bsrc, int i, int h, int cq) {
+  const int c = 8 * i + cq;
+  const float2 ba = __ldg(reinterpret_cast<const float2*>(bsrc + c));
+  const float2 bb = __ldg(reinterpret_cast<const float2*>(bsrc + 128 + c));
+  const float g0 = (acc[4 * i + 2 * h] + ba.x) * sigmoid_f(acc[4 * (i + 16) + 2 * h] + bb.x);
+  const float g1 = (acc[4 * i + 2 * h + 1] + ba.y) * sigmoid_f(acc[4 * (i + 16) + 2 * h + 1] + bb.y);
+  return pack_half2(g0, g1);
+}
+
+// One consumer warpgroup's 64 rows (row0 ..) of a tile whose rows are all live, out through the warpgroup's two store slots
+// (see the header).  rw: the thread's first row inside the 64 (the second is rw + 8).  Each chunk is 64 rows x 128 bytes:
+// 8 fragment blocks of fp16 or 4 of fp32.  The chunk count per tile is even, so chunk c always uses slot c & 1 and the slot
+// written now is the one whose bulk store was committed two groups ago: wait_group.read 1 frees it.
+template <int EPI>
+__device__ __forceinline__ void store_tile_tma(const GemmParams& p, const CUtensorMap& tmap_out, const float (&acc)[128],
+                                               uint8_t* slots, int row0, int n_blk, int rw, int cq, int wg, bool leader) {
+  constexpr bool kF32 = EPI == EPI_BIAS_F32;
+  constexpr int kChunkBlocks = kF32 ? 4 : 8;
+  constexpr int kOutCols = EPI == EPI_BIAS_GLU_F16 ? kG2BN / 2 : kG2BN;
+  constexpr int kChunks = kOutCols / (8 * kChunkBlocks);   // 8 (fp32), 4 (fp16) or 2 (GLU)
+  static_assert(kChunks % 2 == 0, "chunk c must map to slot c & 1 in every tile");
+  const float* bsrc = p.bias + n_blk * kG2BN;
+#pragma unroll
+  for (int c = 0; c < kChunks; ++c) {
+    uint8_t* slot = slots + (c & 1) * kG2SlotBytes;
+    if (leader) ptx::tma_store_wait_read<1>();
+    ptx::named_bar_sync<128>(1 + wg);   // the slot is free for every thread of the warpgroup
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = rw + 8 * h;
+#pragma unroll
+      for (int j = 0; j < kChunkBlocks; ++j) {
+        const int i = c * kChunkBlocks + j;
+        if constexpr (EPI == EPI_BIAS_GLU_F16) {
+          *reinterpret_cast<uint32_t*>(slot + ptx::sw128_off(r, 8 * j + cq) + 2 * cq) = glu_pair(acc, bsrc, i, h, cq);
+        } else {
+          const float2 x = bias_act_pair<EPI>(acc, bsrc, i, h, cq, make_float2(0.f, 0.f), p.scale);
+          if constexpr (kF32)
+            *reinterpret_cast<float2*>(slot + ptx::sw128_off_f32(r, 8 * j + cq) + 4 * (cq & 3)) = x;
+          else
+            *reinterpret_cast<uint32_t*>(slot + ptx::sw128_off(r, 8 * j + cq) + 2 * cq) = pack_half2(x.x, x.y);
+        }
+      }
+    }
+    ptx::fence_proxy_async_smem();      // this thread's slot writes are visible to the bulk store ...
+    ptx::named_bar_sync<128>(1 + wg);   // ... and so are every other thread's
+    if (leader) {
+      ptx::tma_store_2d(&tmap_out, slot, n_blk * kOutCols + c * 8 * kChunkBlocks, row0);
+      ptx::tma_store_commit();
+    }
+  }
+}
+
 template <int EPI, int AMODE>
 __global__ void __cluster_dims__(kG2Cluster, 1, 1) __launch_bounds__(kG2Threads, 1)
 gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
-                   const __grid_constant__ CUtensorMap tmap_w, const GemmParams p) {
+                   const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_out,
+                   const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kG2Stages * kG2ABytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kG2Stages * kG2StageBytes);
+  uint8_t* smem_store = smem + kG2Stages * kG2StageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_store + (gemm_tma_store<EPI, AMODE>() ? kG2StoreBytes : 0));
   uint64_t* empty_bar = full_bar + kG2Stages;
 
   const int warp_idx = threadIdx.x >> 5;
@@ -108,11 +204,19 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     }
   };
   auto pair_dead = [&](int m_pair) -> bool { return conv_tile_dead(2 * m_pair) && conv_tile_dead(2 * m_pair + 1); };
+  // every row of the block is live: the tile leaves through the store slots (see the header)
+  auto tma_tile = [&](int m_blk) -> bool {
+    if constexpr (gemm_tma_store<EPI, AMODE>()) return p.tma_out != 0 && (m_blk + 1) * 128 <= m_rows;
+    return false;
+  };
 
   if (warp_idx == 0 && ptx::elect_one()) {
     ptx::prefetch_tmap(&tmap_a);
     ptx::prefetch_tmap(&tmap_a2);
     ptx::prefetch_tmap(&tmap_w);
+    if constexpr (gemm_tma_store<EPI, AMODE>()) {
+      if (p.tma_out) ptx::prefetch_tmap(&tmap_out);
+    }
     for (int s = 0; s < kG2Stages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
       ptx::mbar_init(&empty_bar[s], 2 * kG2Cluster);   // one arrival per consumer warpgroup of every CTA in the cluster
@@ -213,6 +317,13 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(acc[i])::"memory");
       if (prev >= 0) release(prev);
 
+      if constexpr (gemm_tma_store<EPI, AMODE>()) {
+        if (tma_tile(m_blk)) {
+          store_tile_tma<EPI>(p, tmap_out, acc, smem_store + wg * 2 * kG2SlotBytes, m_blk * 128 + wg * 64, n_blk,
+                              (warp_idx & 3) * 16 + (lane >> 2), cq, wg, wg_leader);
+          continue;
+        }
+      }
       // ---- epilogue straight from the fragment
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -235,14 +346,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           const float* bsrc = p.bias + n_blk * kG2BN;
           __half* outp = reinterpret_cast<__half*>(p.out) + static_cast<size_t>(gr.row) * p.ldo + n_blk * 128;
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int c = 8 * i + cq;
-            const float2 ba = __ldg(reinterpret_cast<const float2*>(bsrc + c));
-            const float2 bb = __ldg(reinterpret_cast<const float2*>(bsrc + 128 + c));
-            const float g0 = (acc[4 * i + 2 * h] + ba.x) * sigmoid_f(acc[4 * (i + 16) + 2 * h] + bb.x);
-            const float g1 = (acc[4 * i + 2 * h + 1] + ba.y) * sigmoid_f(acc[4 * (i + 16) + 2 * h + 1] + bb.y);
-            *reinterpret_cast<uint32_t*>(outp + c) = pack_half2(g0, g1);
-          }
+          for (int i = 0; i < 16; ++i) *reinterpret_cast<uint32_t*>(outp + 8 * i + cq) = glu_pair(acc, bsrc, i, h, cq);
         } else {
           const float* bsrc = p.bias + n_blk * kG2BN;
           const size_t base = static_cast<size_t>(gr.row) * p.ldo + static_cast<size_t>(n_blk) * kG2BN;
@@ -260,13 +364,8 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 #pragma unroll
             for (int i = i0; i < i0 + kBatch; ++i) {
               const int c = 8 * i + cq;
-              const float2 bv = __ldg(reinterpret_cast<const float2*>(bsrc + c));
-              float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
-              if constexpr (EPI == EPI_BIAS_RES_F32) {
-                x0 = fmaf(p.scale, x0, res[i - i0].x);
-                x1 = fmaf(p.scale, x1, res[i - i0].y);
-              }
-              if constexpr (EPI == EPI_BIAS_SILU_F16) { x0 = silu_f(x0); x1 = silu_f(x1); }
+              const float2 x = bias_act_pair<EPI>(acc, bsrc, i, h, cq, res[i - i0], p.scale);
+              float x0 = x.x, x1 = x.y;
               if constexpr (EPI == EPI_CONV_RELU_MASK_F16 || EPI == EPI_CONV_RELU_MASK_F32) {
                 x0 = gr.live ? fmaxf(x0, 0.f) : 0.f;
                 x1 = gr.live ? fmaxf(x1, 0.f) : 0.f;
@@ -281,6 +380,8 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         }
       }
     }
+    // the slots are not reused any more, but the kernel ends only once its stores have landed
+    if (gemm_tma_store<EPI, AMODE>() && wg_leader) ptx::tma_store_wait<0>();
   }
   __syncwarp();
   ptx::cluster_sync();   // the peer may still multicast into this CTA's stages and arrive on its barriers until here

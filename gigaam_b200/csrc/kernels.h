@@ -133,14 +133,17 @@ enum GemmKind : int {
   GEMM_CONV_RELU_MASK_F16 = 5,
 };
 // 2-D operand GEMM  D[M,N] = A[M,K] W[N,K]^T with fused epilogue `kind`; N % 256 == 0, K % 64 == 0.
+// m_dev: row count on the device (<= M), see GemmParams::m_dev.  tmap_out: the output's [M, ncol] columns (ncol = N, N/2 for
+// GLU) at `out`, row pitch ldo (gam_api.cu: make_tmap_out).  With it, tiles whose rows are all live leave through shared
+// memory and TMA bulk stores; without (null), and always for GEMM_BIAS_RES_F32, every tile is stored directly.
 int launch_gemm(int kind, const CUtensorMap* tmap_a, const CUtensorMap* tmap_w, int M, int N, int K, const float* bias,
                 const float* res, void* out, int ldo, float scale, int max_clusters, cudaStream_t s, int reverse = 0,
-                const int* m_dev = nullptr);   // m_dev: row count on the device (<= M), see GemmParams::m_dev
+                const int* m_dev = nullptr, const CUtensorMap* tmap_out = nullptr);
 // one launch for two GEMMs that share M, K, W's row space and the output buffer but read different A operands:
 // columns [0, n1) from tmap_a1, [n1, N) from tmap_a2 (bias -> fp16).  
 int launch_gemm_dual_a(const CUtensorMap* tmap_a1, const CUtensorMap* tmap_a2, int n1, const CUtensorMap* tmap_w, int M, int N,
                        int K, const float* bias, void* out, int ldo, int max_clusters, cudaStream_t s, int reverse = 0,
-                       const int* m_dev = nullptr);
+                       const int* m_dev = nullptr, const CUtensorMap* tmap_out = nullptr);
 // implicit-GEMM 3x3/s2 conv over channels-last [B,T1,F1,C] (tmap_a 4-D strided), output [rows*16, N] fp16.
 // cu / plen (both or neither): packed output rows, frame (b, t < plen[b]) -> row cu[b] + t; null: row b*T2 + t, all frames
 int launch_gemm_conv(const CUtensorMap* tmap_a4d, const CUtensorMap* tmap_w, int B, int T2, int C, int N, const float* bias,

@@ -126,6 +126,12 @@ __device__ __forceinline__ void tma_store_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
+// named barrier `id` (1..15; 0 is __syncthreads) over `n` threads, a multiple of 32
+template <int N>
+__device__ __forceinline__ void named_bar_sync(int id) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(N) : "memory");
+}
+
 // Per-warpgroup register budget (all four warps of a warpgroup execute it): the data-movement warpgroup gives registers
 // back to the CTA's pool, the math warpgroups take them.  ptxas allocates the code behind each to the stated limit.
 template <int kRegs>
@@ -225,6 +231,10 @@ __device__ __forceinline__ void mma_16816(float* d, const uint32_t* a, uint32_t 
 // SWIZZLE_128B TMA box (1024-byte aligned)
 __device__ __forceinline__ uint32_t sw128_off(int row, int col) {
   return static_cast<uint32_t>(row * 128 + ((((col >> 3) ^ row) & 7) << 4));
+}
+// the same for a tile of 32-column fp32 rows: the 16-byte chunk holding (row, col .. col + 3)
+__device__ __forceinline__ uint32_t sw128_off_f32(int row, int col) {
+  return static_cast<uint32_t>(row * 128 + ((((col >> 2) ^ row) & 7) << 4));
 }
 
 }  // namespace ptx

@@ -289,6 +289,10 @@ int gam_group_words(gam_handle* h, const int32_t* ids, const int32_t* frames, co
 int gam_test_gemm(gam_handle* h, int32_t kind, const void* A, const void* A2, int32_t n1, const void* W, const float* bias,
                   const float* res, void* out, int32_t M, int32_t N, int32_t K, int32_t ldo, int32_t col0, float scale,
                   int32_t reverse, const int32_t* m_dev, void* stream);
+/* 1 when the last gam_test_gemm launch stored its full tiles (every row live) through shared memory and TMA bulk stores,
+ * 0 when every tile was stored straight from the registers (residual and power kinds, or an output column range TMA
+ * cannot address: base or row pitch not 16-byte aligned). */
+int gam_test_gemm_used_slots(gam_handle* h);
 /* Implicit-GEMM stride-2 convolutions of the subsampling, out[frame, N] = relu(conv + bias) for frames t < len_out[b], 0 for the
  * others (fp16, or fp32 when f32_out):
  *   conv1d == 0: 3x3 / pad 1 over channels-last A f16 [B, T_in, F1 = 32, C], W = [N, (kt, kf, c)] f16; frame row = 16 rows
