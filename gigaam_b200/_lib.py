@@ -60,7 +60,8 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_emo_head", "gam_test_frames_split", "gam_test_mel_log", "gam_test_rnnt_greedy",
            "gam_rnnt_predict_train", "gam_ctc_log_probs_backward_workspace_bytes", "gam_ctc_log_probs_backward",
            "gam_rnnt_joint_backward_workspace_bytes", "gam_rnnt_joint_backward", "gam_rnnt_predict_backward_workspace_bytes",
-           "gam_rnnt_predict_backward", "gam_test_gemm_used_slots")
+           "gam_rnnt_predict_backward", "gam_test_gemm_used_slots", "gam_decode_scored_workspace_bytes",
+           "gam_ctc_greedy_scored", "gam_rnnt_greedy_scored", "gam_test_rnnt_greedy_scored")
 
 
 def lib_path() -> Path:
@@ -96,6 +97,8 @@ def load() -> C.CDLL:
     lib.gam_workspace_bytes.restype = i64
     lib.gam_decode_workspace_bytes.argtypes = [H, i32, i32]
     lib.gam_decode_workspace_bytes.restype = i64
+    lib.gam_decode_scored_workspace_bytes.argtypes = [H, i32, i32]
+    lib.gam_decode_scored_workspace_bytes.restype = i64
     lib.gam_comm_unique_id.argtypes = [c_vp]
     lib.gam_comm_unique_id.restype = C.c_int
     lib.gam_comm_init.argtypes = [H, c_vp, i32, i32]
@@ -111,6 +114,9 @@ def load() -> C.CDLL:
     lib.gam_encode.restype = C.c_int
     for fn in (lib.gam_ctc_greedy, lib.gam_rnnt_greedy):
         fn.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, i64, c_vp, c_vp, c_vp, i32, c_vp]
+        fn.restype = C.c_int
+    for fn in (lib.gam_ctc_greedy_scored, lib.gam_rnnt_greedy_scored):
+        fn.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, i64, c_vp, c_vp, c_vp, i32, c_vp, c_vp, c_vp, c_vp]
         fn.restype = C.c_int
     lib.gam_ctc_log_probs.argtypes = [H, c_vp, i32, i32, c_vp, c_vp]
     lib.gam_ctc_log_probs.restype = C.c_int
@@ -154,6 +160,9 @@ def load() -> C.CDLL:
     lib.gam_test_mel_log.argtypes = [H, c_vp, c_vp, i32, i32, i32, c_vp, c_vp, c_vp, i32, c_vp, c_vp]
     lib.gam_test_rnnt_greedy.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, i32, c_vp, c_vp, c_vp,
                                          c_vp, c_vp]
+    lib.gam_test_rnnt_greedy_scored.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, i32, i32, c_vp, c_vp,
+                                                c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    lib.gam_test_rnnt_greedy_scored.restype = C.c_int
     for fn in (lib.gam_test_gemm, lib.gam_test_gemm_conv, lib.gam_test_layernorm, lib.gam_test_ln_rope, lib.gam_test_ln_out_ln,
                lib.gam_test_unpack_rows, lib.gam_test_dwconv, lib.gam_test_pack_plan, lib.gam_test_subsample_conv1,
                lib.gam_test_mel_to_tmajor, lib.gam_test_frames_split, lib.gam_test_mel_log, lib.gam_test_rnnt_greedy):

@@ -6,6 +6,12 @@
 //   (2) collapse: keep (l != blank) && (t == 0 || l != l_{t-1}) && (t < len); one warp per utterance,
 //       ballot + popc prefix compaction, results resident on device:
 //       ids[B,T], frames[B,T], counts[B] (int32).
+//   Scored variants (gam_ctc_greedy_scored): the argmax also keeps, per class group, the running sum of exp(z_c - best)
+//   beside its (best value, index), rescaled whenever the best moves; the groups merge in the same shared-memory merge and
+//   the frame's l = log_softmax(row)[label] = -log sum_c exp(z_c - z_max) goes to scratch (NaN on a row whose label is
+//   0 by the non-finite rule).  The logits are the same fp32 sums in the same k order, so the labels are the unscored
+//   kernel's.  The scored collapse gathers l at the emitted frames and sums it over t < len in fp64, in an order fixed by
+//   t alone (lane-strided partial sums, then a fixed xor tree), so an utterance's scores do not depend on its batch.
 #include "kernels.h"
 
 namespace gam {
@@ -21,17 +27,21 @@ constexpr int kCT = kGroups * kCG;   // class tile (36)
 // Block = 32 frames x 4 class groups (one warp per group: its W reads are broadcasts, its enc reads conflict-free):
 // 502 blocks at the benchmark shape instead of 126 single-warp-per-SM blocks.
 // Every (frame, class) sum still runs over k in ascending order, so the logits -- and the argmax -- are bit-identical.
+// SCORED: also lp[R] = l of every row (the unscored instantiation computes and stores nothing more).
+template <bool SCORED>
 __global__ void __launch_bounds__(kRows * kGroups) ctc_argmax_kernel(const float* __restrict__ enc, const float* __restrict__ W,
                                                                      const float* __restrict__ bias, int* __restrict__ labels,
-                                                                     int R, int D, int V1) {
+                                                                     int R, int D, int V1, float* __restrict__ lp) {
   __shared__ float e_s[kKC][kRows + 1];
   __shared__ float w_s[kCT][kKC];
   __shared__ float best_v[kGroups][kRows];
   __shared__ int best_c[kGroups][kRows];
+  __shared__ float best_s[SCORED ? kGroups : 1][kRows];
   const int r = threadIdx.x & 31, cg = threadIdx.x >> 5;
   const int row0 = blockIdx.x * kRows;
   float best = -INFINITY;
   int best_i = 0;
+  [[maybe_unused]] float sum = 0.f;   // SCORED: sum of exp(v - best) over this group's finite logits so far
   for (int c0 = 0; c0 < V1; c0 += kCT) {
     float acc[kCG];
 #pragma unroll
@@ -69,8 +79,13 @@ __global__ void __launch_bounds__(kRows * kGroups) ctc_argmax_kernel(const float
         // "non-finite seen" mark that no later logit replaces and that wins the merge below
         if (!(v <= best)) {
           const bool bad = !(v < INFINITY);
+          if constexpr (SCORED) {
+            if (!bad) sum = sum * expf(best - v) + 1.f;   // best = -inf at the start: 0 * 0 + 1
+          }
           best = bad ? INFINITY : v;
           best_i = bad ? -1 : cls;
+        } else if constexpr (SCORED) {
+          if (v > -INFINITY) sum += expf(v - best);
         }
       }
     }
@@ -79,6 +94,7 @@ __global__ void __launch_bounds__(kRows * kGroups) ctc_argmax_kernel(const float
   // among equal values, decided explicitly
   best_v[cg][r] = best;
   best_c[cg][r] = best_i;
+  if constexpr (SCORED) best_s[cg][r] = sum;
   __syncthreads();
   if (cg == 0 && row0 + r < R) {
 #pragma unroll
@@ -88,18 +104,39 @@ __global__ void __launch_bounds__(kRows * kGroups) ctc_argmax_kernel(const float
       if (v > best || (v == best && i < best_i)) { best = v; best_i = i; }
     }
     labels[row0 + r] = best_i < 0 ? 0 : best_i;   // NaN or +inf in any group -> 0
+    if constexpr (SCORED) {
+      // the row's maximum is `best` whatever the merge order; the groups' sums are rescaled to it in group order.  A
+      // row with a NaN / +inf logit (best_i < 0) or with no logit above -inf has l = NaN, as torch's log_softmax gives.
+      float l = __int_as_float(0x7fffffff);
+      if (best_i >= 0 && best > -INFINITY) {
+        float s = 0.f;
+#pragma unroll
+        for (int g = 0; g < kGroups; ++g) {
+          const float v = best_v[g][r];
+          if (v > -INFINITY) s += best_s[g][r] * expf(v - best);
+        }
+        l = -logf(s);
+      }
+      lp[row0 + r] = l;
+    }
   }
 }
 
+// SCORED: token_logp[b, pos] = lp of the kept frame, path_logp[b] = sum of lp over t < len (fp64, fixed order),
+// path_rows[b] = len
+template <bool SCORED>
 __global__ void __launch_bounds__(128) ctc_collapse_kernel(const int* __restrict__ labels, const int* __restrict__ len, int B,
                                                            int T, int blank, int* __restrict__ ids, int* __restrict__ frames,
-                                                           int* __restrict__ counts) {
+                                                           int* __restrict__ counts, const float* __restrict__ lp,
+                                                           float* __restrict__ token_logp, float* __restrict__ path_logp,
+                                                           int* __restrict__ path_rows) {
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (b >= B) return;
   const int L = min(max(len[b], 0), T);
   const int* lab = labels + static_cast<size_t>(b) * T;
   int base = 0;
+  [[maybe_unused]] double path = 0.0;
   for (int t0 = 0; t0 < T; t0 += 32) {
     const int t = t0 + lane;
     int l = blank, prev = -1;
@@ -113,21 +150,45 @@ __global__ void __launch_bounds__(128) ctc_collapse_kernel(const int* __restrict
       const int pos = base + __popc(mask & ((1u << lane) - 1u));
       ids[static_cast<size_t>(b) * T + pos] = l;
       frames[static_cast<size_t>(b) * T + pos] = t;
+      if constexpr (SCORED) token_logp[static_cast<size_t>(b) * T + pos] = lp[static_cast<size_t>(b) * T + t];
+    }
+    if constexpr (SCORED) {
+      if (t < L) path += static_cast<double>(lp[static_cast<size_t>(b) * T + t]);
     }
     base += __popc(mask);
   }
-  if (lane == 0) counts[b] = base;
+  if constexpr (SCORED) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) path += __shfl_xor_sync(0xffffffffu, path, o);
+  }
+  if (lane == 0) {
+    counts[b] = base;
+    if constexpr (SCORED) {
+      path_logp[b] = static_cast<float>(path);
+      path_rows[b] = L;
+    }
+  }
 }
 
 }  // namespace
 
 void launch_ctc_argmax(const float* enc, const float* W, const float* bias, int* labels, int R, int D, int V1,
                        cudaStream_t s) {
-  ctc_argmax_kernel<<<(R + kRows - 1) / kRows, kRows * kGroups, 0, s>>>(enc, W, bias, labels, R, D, V1);
+  ctc_argmax_kernel<false><<<(R + kRows - 1) / kRows, kRows * kGroups, 0, s>>>(enc, W, bias, labels, R, D, V1, nullptr);
 }
 void launch_ctc_collapse(const int* labels, const int* len, int B, int T, int blank, int* ids, int* frames, int* counts,
                          cudaStream_t s) {
-  ctc_collapse_kernel<<<(B + 3) / 4, 128, 0, s>>>(labels, len, B, T, blank, ids, frames, counts);
+  ctc_collapse_kernel<false><<<(B + 3) / 4, 128, 0, s>>>(labels, len, B, T, blank, ids, frames, counts, nullptr, nullptr, nullptr,
+                                                         nullptr);
+}
+void launch_ctc_argmax_scored(const float* enc, const float* W, const float* bias, int* labels, float* lp, int R, int D, int V1,
+                              cudaStream_t s) {
+  ctc_argmax_kernel<true><<<(R + kRows - 1) / kRows, kRows * kGroups, 0, s>>>(enc, W, bias, labels, R, D, V1, lp);
+}
+void launch_ctc_collapse_scored(const int* labels, const float* lp, const int* len, int B, int T, int blank, int* ids, int* frames,
+                                int* counts, float* token_logp, float* path_logp, int* path_rows, cudaStream_t s) {
+  ctc_collapse_kernel<true><<<(B + 3) / 4, 128, 0, s>>>(labels, len, B, T, blank, ids, frames, counts, lp, token_logp, path_logp,
+                                                        path_rows);
 }
 
 }  // namespace gam

@@ -428,6 +428,12 @@ int64_t gam_encoded_frames(const gam_handle* h, int64_t M) {
 
 int64_t gam_decode_workspace_bytes(const gam_handle* h, int32_t B, int32_t T) { return decode_ws_bytes(h, B, T) + 1024; }
 
+// the scored decoders also keep the CTC per-frame l [B*T] f32 after the labels
+static int64_t scored_extra_bytes(int32_t B, int32_t T) { return align_up(static_cast<int64_t>(B) * T * 4, 1024); }
+int64_t gam_decode_scored_workspace_bytes(const gam_handle* h, int32_t B, int32_t T) {
+  return decode_ws_bytes(h, B, T) + scored_extra_bytes(B, T) + 1024;
+}
+
 int64_t gam_workspace_bytes(const gam_handle* h, int32_t B, int64_t M) {
   Plan p;
   plan_geometry(h, B, M, &p);
@@ -670,8 +676,50 @@ int gam_ctc_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int3
   return 0;
 }
 
+int gam_ctc_greedy_scored(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
+                          int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
+                          float* token_logp, float* path_logp, int32_t* path_rows, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 1) return fail(h, -1, "model has no CTC head");
+  if (max_out < T) return fail(h, -1, "max_out (%d) must be >= T (%d)", max_out, T);
+  if (max_out != T) return fail(h, -1, "ids/frames row pitch must equal T for the CTC path");
+  if (!token_logp || !path_logp || !path_rows) return fail(h, -1, "ctc_greedy_scored: token_logp, path_logp and path_rows are required");
+  const int64_t R = static_cast<int64_t>(B) * T;
+  const int64_t lp_off = align_up(R * 4, 1024);
+  if (workspace_bytes < lp_off + R * 4) return fail(h, -1, "workspace too small for CTC labels and scores");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int* labels = static_cast<int*>(workspace);
+  float* lp = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + lp_off);
+  { PROF(PC_CTC_ARGMAX);
+    launch_ctc_argmax_scored(enc, h->w.ctc_w, h->w.ctc_b, labels, lp, static_cast<int>(R), c.d_model, c.num_classes, s); }
+  { PROF(PC_CTC_COLLAPSE);
+    launch_ctc_collapse_scored(labels, lp, enc_len, B, T, c.num_classes - 1, ids, frames, counts, token_logp, path_logp, path_rows,
+                               s); }
+  GAM_CHECK_LAUNCH(h, "ctc_greedy_scored");
+  return 0;
+}
+
+static int rnnt_greedy_impl(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
+                            int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
+                            float* token_logp, float* path_logp, int32_t* path_rows, void* stream);
+
+int gam_rnnt_greedy_scored(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
+                           int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
+                           float* token_logp, float* path_logp, int32_t* path_rows, void* stream) {
+  if (!token_logp || !path_logp || !path_rows) return fail(h, -1, "rnnt_greedy_scored: token_logp, path_logp and path_rows are required");
+  return rnnt_greedy_impl(h, enc, enc_len, B, T, workspace, workspace_bytes, ids, frames, counts, max_out, token_logp, path_logp,
+                          path_rows, stream);
+}
+
 int gam_rnnt_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
                     int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out, void* stream) {
+  return rnnt_greedy_impl(h, enc, enc_len, B, T, workspace, workspace_bytes, ids, frames, counts, max_out, nullptr, nullptr, nullptr,
+                          stream);
+}
+
+static int rnnt_greedy_impl(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
+                            int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
+                            float* token_logp, float* path_logp, int32_t* path_rows, void* stream) {
   const gam_config& c = h->cfg;
   if (c.head != 2) return fail(h, -1, "model has no RNN-T head");
   if (c.pred_hidden != c.joint_hidden) return fail(h, -1, "pred_hidden != joint_hidden is not supported");
@@ -684,7 +732,7 @@ int gam_rnnt_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int
   PROF(PC_RNNT_GREEDY);
   const int rc = launch_rnnt_greedy_cluster(encproj, enc_len, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h->w.rnnt_wp_t, h->w.rnnt_bp,
                                             h->w.rnnt_wo, h->w.rnnt_bo, B, T, c.pred_hidden, c.num_classes, c.num_classes - 1,
-                                            c.max_symbols, max_out, ids, frames, counts, nullptr, s);
+                                            c.max_symbols, max_out, ids, frames, counts, token_logp, path_logp, path_rows, nullptr, s);
   if (rc > 0)
     return fail(h, -1, "rnnt: the greedy kernel is specialised for pred_hidden = joint_hidden = 320 and needs 16-CTA clusters "
                 "(pred_hidden %d)", c.pred_hidden);
@@ -1347,6 +1395,27 @@ int gam_test_mel_log(gam_handle* h, const float* P, const int32_t* fexp, int32_t
   return 0;
 }
 
+int gam_test_rnnt_greedy_scored(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,
+                                const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
+                                int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts,
+                                float* token_logp, float* path_logp, int32_t* path_rows, int32_t* plan, void* stream) {
+  if (!encproj || !len || !emb_gates || !whhT || !wpT || !bp || !wo || !bo || !ids || !frames || !counts || !token_logp || !path_logp ||
+      !path_rows)
+    return fail(h, -1, "test_rnnt_greedy_scored: every operand is required");
+  if (B <= 0 || T <= 0 || V1 < 2 || max_symbols <= 0 || max_out <= 0)
+    return fail(h, -1, "test_rnnt_greedy_scored: bad sizes (B=%d, T=%d, V1=%d, max_symbols=%d, max_out=%d)", B, T, V1, max_symbols,
+                max_out);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  { PROF(PC_RNNT_GREEDY);
+    rc = launch_rnnt_greedy_cluster(encproj, len, emb_gates, whhT, wpT, bp, wo, bo, B, T, 320, V1, V1 - 1, max_symbols, max_out, ids,
+                                    frames, counts, token_logp, path_logp, path_rows, plan, s); }
+  if (rc > 0) return fail(h, -1, "test_rnnt_greedy_scored: 16-CTA clusters cannot be scheduled on this device");
+  if (rc < 0) return fail(h, -4, "test_rnnt_greedy_scored: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, "test_rnnt_greedy_scored");
+  return 0;
+}
+
 int gam_test_rnnt_greedy(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,
                          const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
                          int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts, int32_t* plan,
@@ -1359,7 +1428,7 @@ int gam_test_rnnt_greedy(gam_handle* h, const float* encproj, const int32_t* len
   int rc;
   { PROF(PC_RNNT_GREEDY);
     rc = launch_rnnt_greedy_cluster(encproj, len, emb_gates, whhT, wpT, bp, wo, bo, B, T, 320, V1, V1 - 1, max_symbols, max_out, ids,
-                                    frames, counts, plan, s); }
+                                    frames, counts, nullptr, nullptr, nullptr, plan, s); }
   if (rc > 0) return fail(h, -1, "test_rnnt_greedy: 16-CTA clusters cannot be scheduled on this device");
   if (rc < 0) return fail(h, -4, "test_rnnt_greedy: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "test_rnnt_greedy");

@@ -55,6 +55,12 @@ void launch_ctc_argmax(const float* enc, const float* W, const float* bias, int*
                        cudaStream_t s);
 void launch_ctc_collapse(const int* labels, const int* len, int B, int T, int blank, int* ids, int* frames, int* counts,
                          cudaStream_t s);
+// scored twins (gam_ctc_greedy_scored): lp [R] f32 scratch of per-frame log_softmax(row)[label]; token_logp [B, T],
+// path_logp [B], path_rows [B]
+void launch_ctc_argmax_scored(const float* enc, const float* W, const float* bias, int* labels, float* lp, int R, int D, int V1,
+                              cudaStream_t s);
+void launch_ctc_collapse_scored(const int* labels, const float* lp, const int* len, int B, int T, int blank, int* ids, int* frames,
+                                int* counts, float* token_logp, float* path_logp, int* path_rows, cudaStream_t s);
 
 // words.cu: (token id, frame) pairs -> word records (first frame, last frame + 1, first token, tokens) per utterance
 void launch_group_words(const int* ids, const int* frames, const int* counts, const unsigned char* flags, int B, int V, int max_out,
@@ -117,10 +123,12 @@ void launch_lstm_bwd_step(const int64_t* x, int U, int u, int V1, const float* e
 int launch_class_gate_sum(const int64_t* x, int64_t rows, const float* dgates, int H4, int V1, int blank, float* out, cudaStream_t s);
 
 // rnnt_cluster.cu: returns 0 ok, 1 = 16-CTA clusters unavailable / unsupported shape, <0 error.  plan: host int[7] that
-// receives the chosen launch (NH, GLOB, rows_smem, cls_per, nu, groups, clusters), or NULL
+// receives the chosen launch (NH, GLOB, rows_smem, cls_per, nu, groups, clusters), or NULL.  token_logp [B, max_out],
+// path_logp [B], path_rows [B]: all NULL for the unscored kernel, all set for the scored one
 int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float* emb_gates, const float* whhT, const float* wpT,
                                const float* bp, const float* wo, const float* bo, int B, int T, int H, int V1, int blank,
-                               int max_symbols, int max_out, int* ids, int* frames, int* counts, int* plan, cudaStream_t s);
+                               int max_symbols, int max_out, int* ids, int* frames, int* counts, float* token_logp,
+                               float* path_logp, int* path_rows, int* plan, cudaStream_t s);
 
 // gemm.cu
 struct GemmParams;

@@ -31,9 +31,19 @@
 // is therefore always in [0, V1).  A NaN or +inf logit enters the argmax as (+inf, index -1), which wins every later
 // compare and every merge (equal values: lower index); warp 0 maps index -1 ("non-finite seen") and the empty index
 // 0x7fffffff ("no winner") to 0.  hid keeps NaN as relu(NaN) = NaN does.
+//
+// Scored instantiation (SCORED, gam_rnnt_greedy_scored): every decision row also yields l = log_softmax(row)[label] =
+// -log sum_c exp(z_c - z_max) (NaN where the label is 0 by the non-finite rule).  Each warp keeps, beside its running
+// (max, argmax), the sum of exp(z - max) over its classes, rescaled when the max moves; warp 0 folds the 16 warp partials
+// and, after the best-value exchange (which then carries that sum as a third float per utterance-half), the 16 CTA
+// partials.  Both folds run in an order fixed by the warp / CTA index alone (4 runs of 4 in index order, then
+// (0 + 1) + (2 + 3)), whatever the group width, so an utterance's scores do not depend on the batch it is decoded in.
+// Warp 0 writes l on emission and sums it (fp64) over the utterance's decision rows.  The unscored instantiation
+// compiles none of this.
 #include <cooperative_groups.h>
 
 #include <cstdlib>
+#include <type_traits>
 
 #include "kernels.h"
 #include "ptx.cuh"
@@ -71,6 +81,14 @@ struct RnntClParams {
   int* frames;
   int* counts;
 };
+// the scored instantiation's parameters (the unscored kernel keeps RnntClParams, so its code does not move)
+struct RnntClScoredParams : RnntClParams {
+  float* token_logp;       // [B, max_out]
+  float* path_logp;        // [B]
+  int* path_rows;          // [B]
+};
+template <bool SCORED>
+using ClParams = std::conditional_t<SCORED, RnntClScoredParams, RnntClParams>;
 
 // per-utterance decoding state (gigaam/decoding.py:150-205), owned by warp 0 of every CTA (identical in all of them)
 struct Ctl {
@@ -96,8 +114,34 @@ struct Smem {
   int4 my_i[NH];
   Ctl ctl;
   uint64_t bar_h[2], bar_pg[2], bar_best[2];   // arrival of the three all-to-all exchanges (alternating pairs)
-  // followed by: float bo[cls_pad]; float wo[rows_smem][kWoPitch];
+  // followed by: [ScoreSmem<NH> if SCORED]; float bo[cls_pad]; float wo[rows_smem][kWoPitch];
 };
+
+// what the scored instantiation adds after Smem
+template <int NH>
+struct ScoreSmem {
+  float4 best_s[2][kCl][NH];      // per-CTA partial sum of exp(z - CTA max), exchanged beside best_v / best_i
+  float wbest_s[kWarps][4 * NH];
+  float4 my_s[NH];
+  double path[kMaxU];             // sum of l over the decision rows so far (warp 0, lane u)
+  int rows[kMaxU];
+};
+
+// Bytes one CTA receives per best-value exchange: one 16-byte store per utterance-half from each CTA of the cluster for
+// every field of the payload (best_v, best_i and, when scored, best_s).  The expect-tx count of bar_best is this value,
+// and the receive buffers of one parity are sized from the same constant, so the two cannot disagree.
+template <int NH, bool SCORED>
+constexpr uint32_t best_exchange_bytes() { return kCl * NH * (SCORED ? 3 : 2) * 16; }
+static_assert(sizeof(Smem<1>::best_v[0]) + sizeof(Smem<1>::best_i[0]) == best_exchange_bytes<1, false>(), "best exchange payload");
+static_assert(sizeof(Smem<2>::best_v[0]) + sizeof(Smem<2>::best_i[0]) == best_exchange_bytes<2, false>(), "best exchange payload");
+static_assert(sizeof(Smem<1>::best_v[0]) + sizeof(Smem<1>::best_i[0]) + sizeof(ScoreSmem<1>::best_s[0]) ==
+              best_exchange_bytes<1, true>(), "scored best exchange payload");
+static_assert(sizeof(Smem<2>::best_v[0]) + sizeof(Smem<2>::best_i[0]) + sizeof(ScoreSmem<2>::best_s[0]) ==
+              best_exchange_bytes<2, true>(), "scored best exchange payload");
+static_assert(sizeof(float4) == 16 && sizeof(int4) == 16, "push16 moves one float4 / int4");
+
+template <int NH, bool SCORED>
+constexpr int fixed_smem_bytes() { return static_cast<int>(sizeof(Smem<NH>) + (SCORED ? sizeof(ScoreSmem<NH>) : 0)); }
 
 __device__ __forceinline__ float sigm(float x) { return 1.0f / (1.0f + expf(-x)); }
 __device__ __forceinline__ float comp(const float4& v, int u) { return u == 0 ? v.x : (u == 1 ? v.y : (u == 2 ? v.z : v.w)); }
@@ -133,6 +177,44 @@ __device__ __forceinline__ void arg_update(float a, int cls, float& bv, int& bi)
   }
 }
 
+// arg_update plus, when scored, the running sum of exp(a - bv) over the finite logits (rescaled when bv moves; bv = -inf
+// at the start gives 0 * 0 + 1).  After a NaN / +inf logit the sum is meaningless and l becomes NaN.
+template <bool SCORED>
+__device__ __forceinline__ void arg_update_s(float a, int cls, float& bv, int& bi, float& bs) {
+  if constexpr (SCORED) {
+    if (!(a <= bv)) {
+      const bool bad = !(a < INFINITY);
+      if (!bad) bs = bs * expf(bv - a) + 1.f;
+      bv = bad ? INFINITY : a;
+      bi = bad ? -1 : cls;
+    } else if (a > -INFINITY) {
+      bs += expf(a - bv);
+    }
+  } else {
+    arg_update(a, cls, bv, bi);
+  }
+}
+
+// scored fold of 16 partials (value v_k, sum s_k relative to v_k) to the sum relative to the maximum m: lane `lane` of
+// utterance u = lane % nu folds partials 4 sub .. 4 sub + 3 (sub = lane / nu < 4), then (0 + 1) + (2 + 3) across subs.
+// The order depends on the partial index alone, not on nu (4 or 8); the result is in the lanes of sub 0.
+template <typename VS>
+__device__ __forceinline__ float fold16(VS vs, float m, int nu, int lane) {
+  const int sub = lane / nu;
+  float acc = 0.f;
+  if (sub < 4) {
+#pragma unroll
+    for (int k = 4 * sub; k < 4 * sub + 4; ++k) {
+      float v, sk;
+      vs(k, v, sk);
+      if (v > -INFINITY) acc += sk * expf(v - m);
+    }
+  }
+  acc += __shfl_xor_sync(0xffffffffu, acc, nu);
+  acc += __shfl_xor_sync(0xffffffffu, acc, 2 * nu);
+  return acc;
+}
+
 __device__ __forceinline__ void fma4(float4& a, float w, const float4& h) {
   a.x = fmaf(w, h.x, a.x); a.y = fmaf(w, h.y, a.y); a.z = fmaf(w, h.z, a.z); a.w = fmaf(w, h.w, a.w);
 }
@@ -156,13 +238,14 @@ __device__ long long g_rnnt_dbg[16];
 
 // NH: float4 halves of utterances per group (4 or 8 utterances).  GLOB: some class rows stay in L2 (large vocabularies);
 // compiled out otherwise (the round loop is executed once per step by every warp; 16 KB less code).
-template <int NH, bool GLOB>
-__global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClParams p) {
+template <int NH, bool GLOB, bool SCORED>
+__global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const ClParams<SCORED> p) {
   constexpr int NU = 4 * NH;
   using SM = Smem<NH>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   SM& s = *reinterpret_cast<SM*>(smem_raw);
-  float* s_bo = reinterpret_cast<float*>(smem_raw + sizeof(SM));
+  [[maybe_unused]] ScoreSmem<NH>& sc = *reinterpret_cast<ScoreSmem<NH>*>(smem_raw + sizeof(SM));
+  float* s_bo = reinterpret_cast<float*>(smem_raw + fixed_smem_bytes<NH, SCORED>());
   float* s_wo = s_bo + p.cls_pad;
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = static_cast<int>(cluster.block_rank());
@@ -211,7 +294,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
   __syncthreads();
   uint32_t n_h = 0, n_pg = 0, n_b = 0;   // exchanges done so far (barrier = n & 1, phase parity = (n >> 1) & 1)
   constexpr uint32_t kStateBytes = kCl * kHS * NH * 16;
-  constexpr uint32_t kBestBytes = kCl * NH * 32;
+  constexpr uint32_t kBestBytes = best_exchange_bytes<NH, SCORED>();
 
   for (int group = cluster_id; group < p.num_groups; group += num_clusters) {
     // ---- control state (warp 0: lane u = utterance u)
@@ -222,6 +305,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         Lu = (lane < p.nu && lane < NU && ug < p.B) ? min(max(p.len[ug], 0), p.T) : 0;
         s.ctl.t[lane] = 0; s.ctl.nsym[lane] = 0; s.ctl.cnt[lane] = 0; s.ctl.label[lane] = p.blank;
         s.ctl.L[lane] = Lu; s.ctl.need[lane] = Lu > 0;
+        if constexpr (SCORED) { sc.path[lane] = 0.0; sc.rows[lane] = 0; }
       }
       const unsigned am = __ballot_sync(0xffffffffu, Lu > 0);
       if (lane == 0) { s.ctl.act_m = static_cast<int>(am); s.ctl.run_m = static_cast<int>(am); s.ctl.moved_m = 0; s.ctl.emit_m = 0; }
@@ -384,8 +468,9 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
       const int myu = (lane >> 3) & 3;       // the utterance (within a half) whose logits this lane ends up holding
       float bv[NH];
       int bi[NH];
+      [[maybe_unused]] float bs[NH];
 #pragma unroll
-      for (int hh = 0; hh < NH; ++hh) { bv[hh] = -INFINITY; bi[hh] = 0x7fffffff; }
+      for (int hh = 0; hh < NH; ++hh) { bv[hh] = -INFINITY; bi[hh] = 0x7fffffff; bs[hh] = 0.f; }
       // shared-memory rows: local rows warp, warp+16, ... (ascending, so the first maximum wins as in torch.argmax)
       for (int lr0 = warp; lr0 < nsm; lr0 += kWarps * kCB) {
         float4 acc[kCB][NH];
@@ -413,7 +498,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
           if (lr < nsm) {
 #pragma unroll
             for (int hh = 0; hh < NH; ++hh) {
-              arg_update(reduce4(acc[c][hh], lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh]);
+              arg_update_s<SCORED>(reduce4(acc[c][hh], lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh], bs[hh]);
             }
           }
         }
@@ -428,7 +513,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int kk = 0; kk < kH / 32; ++kk) fma4(acc, wg[gi][kk], s.hid4[hh][lane + 32 * kk]);
-            arg_update(reduce4(acc, lane) + s_bo[gcls[gi]], cls0 + gcls[gi], bv[hh], bi[hh]);
+            arg_update_s<SCORED>(reduce4(acc, lane) + s_bo[gcls[gi]], cls0 + gcls[gi], bv[hh], bi[hh], bs[hh]);
           }
         }
       }
@@ -438,7 +523,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         for (int hh = 0; hh < NH; ++hh) {
           float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
           for (int kk = 0; kk < kH / 32; ++kk) fma4(acc, __ldg(w + lane + 32 * kk), s.hid4[hh][lane + 32 * kk]);
-          arg_update(reduce4(acc, lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh]);
+          arg_update_s<SCORED>(reduce4(acc, lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh], bs[hh]);
         }
       }
       }
@@ -446,6 +531,10 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
       if ((lane & 7) == 0) {
 #pragma unroll
         for (int hh = 0; hh < NH; ++hh) { s.wbest_v[warp][4 * hh + myu] = bv[hh]; s.wbest_i[warp][4 * hh + myu] = bi[hh]; }
+        if constexpr (SCORED) {
+#pragma unroll
+          for (int hh = 0; hh < NH; ++hh) sc.wbest_s[warp][4 * hh + myu] = bs[hh];
+        }
       }
       __syncthreads();
       DBG_T(15);
@@ -469,14 +558,19 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
           if (v > v0 || (v == v0 && i < i0)) { v0 = v; i0 = i; }
         }
         if (lane < NU) { reinterpret_cast<float*>(s.my_v)[u] = v0; reinterpret_cast<int*>(s.my_i)[u] = i0; }
+        if constexpr (SCORED) {   // the CTA's sum relative to its maximum v0 (every lane of utterance u holds v0)
+          const float cs = fold16([&](int w, float& v, float& sk) { v = s.wbest_v[w][u]; sk = sc.wbest_s[w][u]; }, v0, NU, lane);
+          if (lane < NU) reinterpret_cast<float*>(sc.my_s)[u] = cs;
+        }
         __syncwarp();
-        if (lane < kCl) {   // lane = destination CTA
+        if (lane < kCl) {   // lane = destination CTA; one 16-byte store per field and half (best_exchange_bytes)
 #pragma unroll
           for (int hh = 0; hh < NH; ++hh) {
             const int4 ii = s.my_i[hh];
             push16(&s.best_v[par][rank][hh], &s.bar_best[par], lane, s.my_v[hh]);
             push16(&s.best_i[par][rank][hh], &s.bar_best[par], lane, static_cast<uint32_t>(ii.x), static_cast<uint32_t>(ii.y),
                    static_cast<uint32_t>(ii.z), static_cast<uint32_t>(ii.w));
+            if constexpr (SCORED) push16(&sc.best_s[par][rank][hh], &s.bar_best[par], lane, sc.my_s[hh]);
           }
         }
         DBG_T(4);
@@ -499,6 +593,14 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         // "non-finite seen" (-1) and "no winner" (0x7fffffff: every logit -inf) give label 0, as torch's argmax of an
         // all-NaN log_softmax row; the label that indexes emb_gates below is in [0, V1) by construction
         const int lab = (i0 < 0 || i0 >= p.V1) ? 0 : i0;
+        [[maybe_unused]] float lp = 0.f;
+        if constexpr (SCORED) {   // l of this row: NaN where the label is 0 by the non-finite rule
+          const float ts = fold16([&](int r, float& v, float& sk) {
+            v = reinterpret_cast<const float*>(&s.best_v[par][r][0])[u];
+            sk = reinterpret_cast<const float*>(&sc.best_s[par][r][0])[u];
+          }, v0, NU, lane);
+          lp = (i0 < 0 || i0 >= p.V1 || !(v0 > -INFINITY)) ? __int_as_float(0x7fffffff) : -logf(ts);
+        }
         // lane u < NU decides for utterance u (gigaam/decoding.py:176-205)
         bool act_new = false, run_new = false, moved = false, emitted = false;
         if (lane < NU) {
@@ -506,6 +608,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
           const int Lu = s.ctl.L[u];
           int need = s.ctl.need[u];
           if (t < Lu) {
+            if constexpr (SCORED) { sc.path[u] += static_cast<double>(lp); sc.rows[u] += 1; }
             if (lab == p.blank) {
               t += 1;
               s.ctl.nsym[u] = 0;
@@ -517,6 +620,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
                 const size_t o = static_cast<size_t>(group * p.nu + u) * p.max_out + cnt;
                 p.ids[o] = lab;
                 p.frames[o] = t;
+                if constexpr (SCORED) p.token_logp[o] = lp;
               }
               s.ctl.cnt[u] = cnt + 1;
               s.ctl.label[u] = lab;
@@ -569,7 +673,10 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
     }
     if (rank == 0 && warp == 0 && lane < NU) {
       const int ug = group * p.nu + lane;
-      if (lane < p.nu && ug < p.B) p.counts[ug] = min(s.ctl.cnt[lane], p.max_out);
+      if (lane < p.nu && ug < p.B) {
+        p.counts[ug] = min(s.ctl.cnt[lane], p.max_out);
+        if constexpr (SCORED) { p.path_logp[ug] = static_cast<float>(sc.path[lane]); p.path_rows[ug] = sc.rows[lane]; }
+      }
     }
     __syncthreads();   // ctl is re-initialised by warp 0 at the top of the next group
   }
@@ -585,15 +692,15 @@ struct LaunchState {
   int smem_set = 0;
 };
 
-template <int NH, bool GLOB>
-int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, int* plan, cudaStream_t s) {
+template <int NH, bool GLOB, bool SCORED>
+int launch_nh(ClParams<SCORED>& p, int B, int V1, int smem_cap, int* plan, cudaStream_t s) {
   static LaunchState per_device[64];   // function attributes and cluster occupancy are per device
   int dev_index = 0;
   cudaGetDevice(&dev_index);
   LaunchState& st = per_device[dev_index & 63];
   const int cls_per = (V1 + kCl - 1) / kCl;
   const int cls_pad = (cls_per + 3) & ~3;
-  const int fixed = static_cast<int>(sizeof(Smem<NH>)) + cls_pad * 4;
+  const int fixed = fixed_smem_bytes<NH, SCORED>() + cls_pad * 4;
   int rows_smem = (smem_cap - fixed) / (kWoPitch * 4);
   if (rows_smem < 0) return 1;
   if (rows_smem > cls_per) rows_smem = cls_per;
@@ -611,15 +718,15 @@ int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, int* plan, cudaStrea
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   if (st.max_clusters < 0 || smem > st.smem_set) {
-    if (cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-        cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
+    if (cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
+        cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
       cudaGetLastError();
       st.max_clusters = 0;
     } else {
       st.smem_set = smem;
       cfg.gridDim = dim3(kCl);
       int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, rnnt_cluster_kernel<NH, GLOB>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+      if (cudaOccupancyMaxActiveClusters(&n, rnnt_cluster_kernel<NH, GLOB, SCORED>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
       st.max_clusters = n;
     }
   }
@@ -637,7 +744,7 @@ int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, int* plan, cudaStrea
     const int v[7] = {NH, GLOB ? 1 : 0, rows_smem, cls_per, nu, p.num_groups, nclusters};
     for (int i = 0; i < 7; ++i) plan[i] = v[i];
   }
-  if (cudaLaunchKernelEx(&cfg, rnnt_cluster_kernel<NH, GLOB>, p) != cudaSuccess) return -2;
+  if (cudaLaunchKernelEx(&cfg, rnnt_cluster_kernel<NH, GLOB, SCORED>, p) != cudaSuccess) return -2;
   return 0;
 }
 
@@ -652,9 +759,11 @@ extern "C" int gam_rnnt_debug_read(long long* out16) {
 // returns 0 on success, 1 if the shape is unsupported (pred_hidden != 320) or a 16-CTA cluster cannot be scheduled on
 // this device, negative on a launch error.  plan (host, 7 ints, or NULL) receives the launch that was chosen:
 // NH, GLOB, class rows per CTA in shared memory, classes per CTA, utterances per group, groups, clusters launched.
+// token_logp (or NULL: the unscored kernel) selects the scored instantiation, which also writes path_logp / path_rows.
 int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float* emb_gates, const float* whhT, const float* wpT,
                                const float* bp, const float* wo, const float* bo, int B, int T, int H, int V1, int blank,
-                               int max_symbols, int max_out, int* ids, int* frames, int* counts, int* plan, cudaStream_t s) {
+                               int max_symbols, int max_out, int* ids, int* frames, int* counts, float* token_logp,
+                               float* path_logp, int* path_rows, int* plan, cudaStream_t s) {
   if (H != kH) return 1;
   static int smem_cap = 0, clusters_hint = 0;
   if (smem_cap == 0) {
@@ -666,17 +775,26 @@ int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float
     clusters_hint = sms / kCl - 2;   // GPCs rarely hold more than one 16-CTA cluster each (a 132-SM H100 has 7 or 8 GPCs)
     if (clusters_hint < 1) clusters_hint = 1;
   }
-  RnntClParams p;
+  RnntClScoredParams p;
   p.encproj = encproj; p.len = len; p.emb_gates = emb_gates; p.whhT = whhT; p.wpT = wpT; p.bp = bp; p.wo = wo; p.bo = bo;
   p.B = B; p.T = T; p.V1 = V1; p.blank = blank; p.max_symbols = max_symbols; p.max_out = max_out;
   p.ids = ids; p.frames = frames; p.counts = counts;
+  p.token_logp = token_logp; p.path_logp = path_logp; p.path_rows = path_rows;
   // groups of up to 4 utterances while every group still gets its own cluster, else groups of up to 8
   const int cls_per = (V1 + kCl - 1) / kCl;
   const bool small = B <= 4 * clusters_hint;
-  const int fixed = static_cast<int>(small ? sizeof(Smem<1>) : sizeof(Smem<2>)) + ((cls_per + 3) & ~3) * 4;
+  const bool scored = token_logp != nullptr;
+  if (scored && (!path_logp || !path_rows)) return -1;
+  const int fixed = (scored ? (small ? fixed_smem_bytes<1, true>() : fixed_smem_bytes<2, true>())
+                            : (small ? fixed_smem_bytes<1, false>() : fixed_smem_bytes<2, false>())) + ((cls_per + 3) & ~3) * 4;
   const bool glob = (smem_cap - fixed) / (kWoPitch * 4) < cls_per;   // some class rows have to stay in L2
-  if (small) return glob ? launch_nh<1, true>(p, B, V1, smem_cap, plan, s) : launch_nh<1, false>(p, B, V1, smem_cap, plan, s);
-  return glob ? launch_nh<2, true>(p, B, V1, smem_cap, plan, s) : launch_nh<2, false>(p, B, V1, smem_cap, plan, s);
+  if (scored) {
+    if (small) return glob ? launch_nh<1, true, true>(p, B, V1, smem_cap, plan, s) : launch_nh<1, false, true>(p, B, V1, smem_cap, plan, s);
+    return glob ? launch_nh<2, true, true>(p, B, V1, smem_cap, plan, s) : launch_nh<2, false, true>(p, B, V1, smem_cap, plan, s);
+  }
+  RnntClParams& up = p;
+  if (small) return glob ? launch_nh<1, true, false>(up, B, V1, smem_cap, plan, s) : launch_nh<1, false, false>(up, B, V1, smem_cap, plan, s);
+  return glob ? launch_nh<2, true, false>(up, B, V1, smem_cap, plan, s) : launch_nh<2, false, false>(up, B, V1, smem_cap, plan, s);
 }
 
 }  // namespace gam

@@ -47,20 +47,27 @@ class _GreedyBase:
         self.tokenizer = Tokenizer(vocabulary, model_path)
         self.blank_id = len(self.tokenizer)
 
-    def decode_device(self, head, encoded: Tensor, lengths: Tensor, packed: Optional[Tensor] = None
-                      ) -> Tuple[Tensor, Tensor, Tensor]:
+    def decode_device(self, head, encoded: Tensor, lengths: Tensor, packed: Optional[Tensor] = None, scores: bool = False
+                      ) -> Tuple[Tensor, ...]:
         """Device-resident result: ids [B, max_out] i32, frames [B, max_out] i32, counts [B] i32 (views of `packed`, an
-        `Engine.packed_hypotheses` buffer, when one is given: the layout the multi-GPU gather ships)."""
+        `Engine.packed_hypotheses` buffer, when one is given: the layout the multi-GPU gather ships).  `scores=True`
+        appends token_logp [B, max_out] f32, path_logp [B] f32 and path_rows [B] i32 (`Engine.greedy`)."""
         eng = head._engine()
         assert eng.num_classes == len(self.tokenizer) + 1, \
             f"Num classes {eng.num_classes} != len(vocab)+1 {len(self.tokenizer) + 1}"
         enc = _as_btd(encoded.to(device=eng.device, dtype=torch.float32))
-        return eng.greedy(enc, lengths, packed)
+        return eng.greedy(enc, lengths, packed, scores=scores)
 
     @torch.inference_mode()
-    def decode(self, head, encoded: Tensor, lengths: Tensor) -> List[Tuple[str, List[int], List[int]]]:
-        ids, frames, counts = self.decode_device(head, encoded, lengths)
-        return self.to_hypotheses(ids.cpu(), frames.cpu(), counts.cpu())
+    def decode(self, head, encoded: Tensor, lengths: Tensor, return_scores: bool = False) -> List[Tuple]:
+        """[(text, token_ids, token_frames)] per utterance; with `return_scores`, (text, token_ids, token_frames,
+        token_logprobs, path_logprob, path_rows): the log-probability of every emitted token, the sum over every decision
+        row of the greedy path and the number of those rows (include/gigaam_b200.h, gam_ctc_greedy_scored)."""
+        if not return_scores:
+            ids, frames, counts = self.decode_device(head, encoded, lengths)
+            return self.to_hypotheses(ids.cpu(), frames.cpu(), counts.cpu())
+        out = [t.cpu() for t in self.decode_device(head, encoded, lengths, scores=True)]
+        return self.to_scored_hypotheses(*out)
 
     def to_hypotheses(self, ids: Tensor, frames: Tensor, counts: Tensor) -> List[Tuple[str, List[int], List[int]]]:
         out = []
@@ -68,6 +75,11 @@ class _GreedyBase:
             tok = ids[b, :n].tolist()
             out.append((self.tokenizer.decode(tok), tok, frames[b, :n].tolist()))
         return out
+
+    def to_scored_hypotheses(self, ids: Tensor, frames: Tensor, counts: Tensor, token_logp: Tensor, path_logp: Tensor,
+                             path_rows: Tensor) -> List[Tuple[str, List[int], List[int], List[float], float, int]]:
+        return [hyp + (token_logp[b, :len(hyp[1])].tolist(), float(path_logp[b]), int(path_rows[b]))
+                for b, hyp in enumerate(self.to_hypotheses(ids, frames, counts))]
 
 
 class CTCGreedyDecoding(_GreedyBase):

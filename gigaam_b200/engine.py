@@ -513,12 +513,16 @@ class Engine:
         w = self.hyp_width(T)
         return torch.zeros(2 * rows * w + rows, dtype=torch.int32, device=self.device)
 
-    def greedy(self, enc_btd: Tensor, enc_len: Tensor, packed: Optional[Tensor] = None) -> Tuple[Tensor, Tensor, Tensor]:
+    def greedy(self, enc_btd: Tensor, enc_len: Tensor, packed: Optional[Tensor] = None, scores: bool = False) -> Tuple[Tensor, ...]:
         """enc [B, T, d] f32 contiguous, len [B] -> (ids [B, max_out] i32, frames, counts [B] i32) on device.
-        `packed` (from packed_hypotheses, rows >= B): the results are written into that buffer and returned as views of it."""
+        `packed` (from packed_hypotheses, rows >= B): the results are written into that buffer and returned as views of it.
+        `scores=True` decodes with gam_*_greedy_scored (the same ids / frames / counts) and also returns token_logp
+        [B, max_out] f32, path_logp [B] f32 and path_rows [B] i32 (include/gigaam_b200.h has the definitions)."""
         assert enc_btd.is_cuda and enc_btd.dtype == torch.float32 and enc_btd.is_contiguous()
         if self.head_type == 0:
             raise RuntimeError("model has no head to decode with")
+        if scores and packed is not None:
+            raise ValueError("scores are not part of the packed hypothesis layout")
         B, T, _ = enc_btd.shape
         enc_len = enc_len.to(device=self.device, dtype=torch.int32).contiguous()
         max_out = self.hyp_width(T)
@@ -532,6 +536,18 @@ class Engine:
             ids = torch.empty((B, max_out), dtype=torch.int32, device=self.device)
             frames = torch.empty((B, max_out), dtype=torch.int32, device=self.device)
             counts = torch.empty((B,), dtype=torch.int32, device=self.device)
+        if scores:
+            token_logp = torch.empty((B, max_out), dtype=torch.float32, device=self.device)
+            path_logp = torch.empty((B,), dtype=torch.float32, device=self.device)
+            path_rows = torch.empty((B,), dtype=torch.int32, device=self.device)
+            ws = self._ws_dec.get((B, T), int(self.lib.gam_decode_scored_workspace_bytes(self.handle, B, T)), self.device)
+            fn = self.lib.gam_ctc_greedy_scored if self.head_type == 1 else self.lib.gam_rnnt_greedy_scored
+            with torch.cuda.device(self.device):
+                rc = fn(self.handle, enc_btd.data_ptr(), enc_len.data_ptr(), B, T, ws.data_ptr(), ws.numel(), ids.data_ptr(),
+                        frames.data_ptr(), counts.data_ptr(), max_out, token_logp.data_ptr(), path_logp.data_ptr(),
+                        path_rows.data_ptr(), self._stream())
+            _lib.check(self.lib, self.handle, rc, "gam_greedy_scored")
+            return ids, frames, counts, token_logp, path_logp, path_rows
         ws = self._ws_dec.get((B, T), int(self.lib.gam_decode_workspace_bytes(self.handle, B, T)), self.device)
         fn = self.lib.gam_ctc_greedy if self.head_type == 1 else self.lib.gam_rnnt_greedy
         with torch.cuda.device(self.device):

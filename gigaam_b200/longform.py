@@ -59,11 +59,12 @@ def split_on_energy(wav: Tensor, sample_rate: int = SAMPLE_RATE, max_duration: f
 
 
 def transcribe_segments(model, segments: Sequence[Tensor], boundaries: Sequence[Tuple[float, float]], word_timestamps: bool = False,
-                        batch_size: int = 16) -> LongformTranscriptionResult:
+                        batch_size: int = 16, confidence: bool = False) -> LongformTranscriptionResult:
     """Batched inference over pre-cut segments, results in the original order (gigaam/model.py:222-259).  The
     length-bucketed batches go through `pipeline.BatchPipeline`: the upload of batch i+1 and the read-back of batch i-1
     overlap the kernels of batch i, recurring shapes replay a CUDA graph, and word grouping stays on the device."""
     from .pipeline import BatchPipeline
+    from .timestamps_utils import path_confidence
     if len(segments) != len(boundaries):
         raise ValueError("segments and boundaries differ in length")
     if not segments:
@@ -84,12 +85,13 @@ def transcribe_segments(model, segments: Sequence[Tensor], boundaries: Sequence[
 
     # a graph per distinct (batch, padded length) only pays off when shapes recur; VAD segments rarely do
     shapes = [(len(b), max(lengths[i] for i in b)) for b in batches]
-    pipe = BatchPipeline(model, use_graph=len(set(shapes)) < len(shapes), with_words=word_timestamps)
+    pipe = BatchPipeline(model, use_graph=len(set(shapes)) < len(shapes), with_words=word_timestamps, with_scores=confidence)
     for batch, host in zip(batches, pipe.run_raw(host_batches())):
         ids, frames, counts, enc_len = host[:4]
+        token_logp, path_logp, path_rows = host[-3:] if confidence else (None, None, None)
         if word_timestamps:
             wav_lens = torch.tensor([lengths[i] for i in batch])
-            results = model._words_from_records(ids, counts, enc_len, wav_lens, list(host[4:]))
+            results = model._words_from_records(ids, counts, enc_len, wav_lens, list(host[4:9]), token_logp)
         else:
             results = [(t, None) for t, _, _ in model.decoding.to_hypotheses(ids, frames, counts)]
         for row, (text, words) in enumerate(results):
@@ -97,6 +99,8 @@ def transcribe_segments(model, segments: Sequence[Tensor], boundaries: Sequence[
             seg_start, seg_end = boundaries[i]
             shifted = None
             if word_timestamps:
-                shifted = [Word(text=w.text, start=round(w.start + seg_start, 3), end=round(w.end + seg_start, 3)) for w in words or []]
-            out[i] = Segment(text=text, start=seg_start, end=seg_end, words=shifted)
+                shifted = [Word(text=w.text, start=round(w.start + seg_start, 3), end=round(w.end + seg_start, 3),
+                                confidence=w.confidence) for w in words or []]
+            conf = path_confidence(path_logp[row], path_rows[row]) if confidence else None
+            out[i] = Segment(text=text, start=seg_start, end=seg_end, words=shifted, confidence=conf)
     return LongformTranscriptionResult(segments=[s for s in out if s is not None])

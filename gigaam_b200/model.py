@@ -209,15 +209,25 @@ class GigaAMASR(GigaAM):
         self.head._bind(self)
         self.decoding = instantiate(dec_cfg, "RNNTGreedyDecoding" if head_cfg.get("type") == "rnnt" else "CTCGreedyDecoding")
 
-    def _decode(self, encoded: Tensor, encoded_len: Tensor, wav_lens: Tensor, word_timestamps: bool = False
-                ) -> List[Tuple[str, Optional[List[Word]]]]:
-        """gigaam/model.py:96-124"""
+    def _decode(self, encoded: Tensor, encoded_len: Tensor, wav_lens: Tensor, word_timestamps: bool = False,
+                confidence: bool = False) -> List[Tuple[str, Optional[List[Word]], Optional[float]]]:
+        """gigaam/model.py:96-124; (text, words, confidence) per utterance (confidence None unless requested)."""
+        from .timestamps_utils import path_confidence
         if not word_timestamps:
-            return [(t, None) for t, _, _ in self.decoding.decode(self.head, encoded, encoded_len)]
+            if not confidence:
+                return [(t, None, None) for t, _, _ in self.decoding.decode(self.head, encoded, encoded_len)]
+            return [(h[0], None, path_confidence(h[4], h[5]))
+                    for h in self.decoding.decode(self.head, encoded, encoded_len, return_scores=True)]
         # tokens are grouped into words on the device (csrc/words.cu); one D2H copy brings ids and word records back
-        ids, frames, counts = self.decoding.decode_device(self.head, encoded, encoded_len)
+        out = self.decoding.decode_device(self.head, encoded, encoded_len, scores=confidence)
+        ids, frames, counts = out[:3]
         rec = self._get_engine().group_words(ids, frames, counts, self._word_flags())
-        return self._words_from_records(ids.cpu(), counts.cpu(), encoded_len.cpu(), wav_lens.cpu(), [t.cpu() for t in rec])
+        scores = [t.cpu() for t in out[3:]] if confidence else None
+        res = self._words_from_records(ids.cpu(), counts.cpu(), encoded_len.cpu(), wav_lens.cpu(), [t.cpu() for t in rec],
+                                       scores[0] if confidence else None)
+        if not confidence:
+            return [(t, w, None) for t, w in res]
+        return [(t, w, path_confidence(scores[1][i], scores[2][i])) for i, (t, w) in enumerate(res)]
 
     def _word_flags(self) -> Tensor:
         """Per-token flag table of the device word grouping (timestamps_utils.token_flag_table), built once."""
@@ -228,9 +238,10 @@ class GigaAMASR(GigaAM):
             self.__dict__["_token_flags"] = flags
         return flags
 
-    def _words_from_records(self, ids: Tensor, counts: Tensor, encoded_len: Tensor, wav_lens: Tensor, rec: List[Tensor]
-                            ) -> List[Tuple[str, Optional[List[Word]]]]:
-        """Host copies of (ids, counts, encoded_len, wav_lens, gam_group_words records) -> [(text, words)] per utterance."""
+    def _words_from_records(self, ids: Tensor, counts: Tensor, encoded_len: Tensor, wav_lens: Tensor, rec: List[Tensor],
+                            token_logp: Optional[Tensor] = None) -> List[Tuple[str, Optional[List[Word]]]]:
+        """Host copies of (ids, counts, encoded_len, wav_lens, gam_group_words records[, token_logp]) -> [(text, words)] per
+        utterance; with token_logp every word carries its confidence."""
         from .timestamps_utils import compute_frame_shift, words_from_device
         tok = self.decoding.tokenizer
         ws, we, wf, wn, nw = rec
@@ -239,7 +250,8 @@ class GigaAMASR(GigaAM):
             row = ids[i, :n].tolist()
             k = int(nw[i])
             shift = compute_frame_shift(int(wav_lens[i]), int(encoded_len[i]))
-            words = words_from_device(tok, row, ws[i, :k].tolist(), we[i, :k].tolist(), wf[i, :k].tolist(), wn[i, :k].tolist(), shift)
+            words = words_from_device(tok, row, ws[i, :k].tolist(), we[i, :k].tolist(), wf[i, :k].tolist(), wn[i, :k].tolist(), shift,
+                                      None if token_logp is None else token_logp[i, :n].tolist())
             out.append((tok.decode(row), words))
         return out
 
@@ -250,30 +262,32 @@ class GigaAMASR(GigaAM):
         return self.head(encoded), encoded_len
 
     @torch.inference_mode()
-    def transcribe(self, wav_file, word_timestamps: bool = False) -> TranscriptionResult:
-        """gigaam/model.py:126-140"""
+    def transcribe(self, wav_file, word_timestamps: bool = False, confidence: bool = False) -> TranscriptionResult:
+        """gigaam/model.py:126-140.  `confidence=True` decodes with the scored kernels (the same text and words) and fills
+        `confidence` of the result, and of every word when word timestamps are on (INTEGRATION.md, "Confidence")."""
         wav, length = self.prepare_wav(wav_file)
         if length.item() > LONGFORM_THRESHOLD:
             raise ValueError("Too long wav file, use 'transcribe_longform' method.")
         encoded, encoded_len = self.forward(wav, length)
-        text, words = self._decode(encoded, encoded_len, length, word_timestamps)[0]
-        return TranscriptionResult(text=text, words=words)
+        text, words, conf = self._decode(encoded, encoded_len, length, word_timestamps, confidence)[0]
+        return TranscriptionResult(text=text, words=words, confidence=conf)
 
     @torch.inference_mode()
     def transcribe_longform(self, wav_file, word_timestamps: bool = False, fr_batch_size: int = 16, fr_num_workers: int = 0,
                             segments: Optional[List[Tensor]] = None, boundaries: Optional[List[Tuple[float, float]]] = None,
-                            **kwargs):
+                            confidence: bool = False, **kwargs):
         """gigaam/model.py:195-259.  Segmentation is pluggable: pass `segments` / `boundaries` from any VAD (the
         reference's pyannote pipeline, gigaam/vad_utils.py, is third party and not vendored); without them the
         recording is cut at low-energy points (`longform.split_on_energy`, kwargs forwarded).  Segments are
-        length-bucketed into batches of `fr_batch_size`; `fr_num_workers` is accepted for signature compatibility."""
+        length-bucketed into batches of `fr_batch_size`; `fr_num_workers` is accepted for signature compatibility.
+        `confidence=True` fills every segment's (and word's) `confidence`, scored inside the same device step."""
         from .longform import split_on_energy, transcribe_segments
         if segments is None:
             wav = load_audio(wav_file) if isinstance(wav_file, str) else torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1)
             segments, boundaries = split_on_energy(wav, SAMPLE_RATE, **kwargs)
         elif boundaries is None:
             raise ValueError("boundaries are required when segments are given")
-        return transcribe_segments(self, segments, boundaries, word_timestamps, fr_batch_size)
+        return transcribe_segments(self, segments, boundaries, word_timestamps, fr_batch_size, confidence)
 
     @torch.inference_mode()
     def transcribe_batch(self, wav: Tensor, lengths: Tensor) -> List[str]:

@@ -16,8 +16,9 @@ Tensor = torch.Tensor
 class _ShapeGraph:
     """The whole device step for one (B, N) input shape, captured once: static inputs -> static outputs."""
 
-    def __init__(self, model, B: int, N: int, dev: torch.device, with_words: bool = False, gather=None):
+    def __init__(self, model, B: int, N: int, dev: torch.device, with_words: bool = False, gather=None, with_scores: bool = False):
         self.with_words = with_words
+        self.with_scores = with_scores
         self.gather = gather
         self.wav = torch.zeros((B, N), dtype=torch.float32, device=dev)
         self.len = torch.full((B,), N, dtype=torch.int64, device=dev)
@@ -36,13 +37,16 @@ class _ShapeGraph:
         self._held = model._get_engine().held_workspaces(B, N)
 
     def _step(self, model):
-        return device_step(model, self.wav, self.len, self.with_words, self.gather)
+        return device_step(model, self.wav, self.len, self.with_words, self.gather, self.with_scores)
 
 
-def device_step(model, wav: Tensor, lengths: Tensor, with_words: bool = False, gather=None):
-    """wav -> device-resident hypotheses (ids, frames, counts, encoded_len[, word records]): the kernels of one batch.
-    With `gather` (dist.HypothesisGather; every rank runs the same number of equally shaped steps) the shard's packed
-    hypotheses are all-gathered inside the step and ids / frames / counts are those of the GLOBAL batch."""
+def device_step(model, wav: Tensor, lengths: Tensor, with_words: bool = False, gather=None, with_scores: bool = False):
+    """wav -> device-resident hypotheses (ids, frames, counts, encoded_len[, word records][, token_logp, path_logp,
+    path_rows]): the kernels of one batch.  With `gather` (dist.HypothesisGather; every rank runs the same number of
+    equally shaped steps) the shard's packed hypotheses are all-gathered inside the step and ids / frames / counts are
+    those of the GLOBAL batch; scores are not part of that layout.  `with_scores` decodes with the scored kernels."""
+    if gather is not None and with_scores:
+        raise ValueError("scores are not gathered across ranks")
     enc, enc_len = model(wav, lengths)
     if gather is not None:
         from .dist import unpack_gathered
@@ -52,19 +56,23 @@ def device_step(model, wav: Tensor, lengths: Tensor, with_words: bool = False, g
         model.decoding.decode_device(model.head, enc, enc_len, packed)
         ids, frames, counts = unpack_gathered(gather.all_gather(packed), B * gather.world, gather.world, B, eng.hyp_width(T))
         return ids, frames, counts, enc_len
-    ids, frames, counts = model.decoding.decode_device(model.head, enc, enc_len)
-    if not with_words:
-        return ids, frames, counts, enc_len
-    return (ids, frames, counts, enc_len) + tuple(model._get_engine().group_words(ids, frames, counts, model._word_flags()))
+    out = model.decoding.decode_device(model.head, enc, enc_len, scores=with_scores)
+    ids, frames, counts = out[:3]
+    words = tuple(model._get_engine().group_words(ids, frames, counts, model._word_flags())) if with_words else ()
+    return (ids, frames, counts, enc_len) + words + tuple(out[3:])
 
 
 class BatchPipeline:
     """`run(host_batches)` yields the hypotheses of every batch.  `with_words=True` also groups tokens into words on the
-    device (csrc/words.cu) and `run_raw` then yields the host copies of the raw records for word timestamps."""
+    device (csrc/words.cu) and `run_raw` then yields the host copies of the raw records for word timestamps.
+    `with_scores=True` decodes with the scored kernels inside the same step (and graph): `run_raw` appends token_logp,
+    path_logp and path_rows."""
 
-    def __init__(self, model, use_graph: bool = True, max_graphs: int = 4, with_words: bool = False, gather=None):
+    def __init__(self, model, use_graph: bool = True, max_graphs: int = 4, with_words: bool = False, gather=None,
+                 with_scores: bool = False):
         self.model = model
         self.with_words = with_words
+        self.with_scores = with_scores
         self.gather = gather          # dist.HypothesisGather: results are then those of all ranks' batches
         self.dev = model._device
         self.copy_stream = torch.cuda.Stream(device=self.dev)
@@ -86,7 +94,7 @@ class BatchPipeline:
         if g is None:
             if len(self._graphs) >= self.max_graphs:
                 self._graphs.pop(next(iter(self._graphs)))
-            g = _ShapeGraph(self.model, B, N, self.dev, self.with_words, self.gather)
+            g = _ShapeGraph(self.model, B, N, self.dev, self.with_words, self.gather, self.with_scores)
             self._graphs[(B, N)] = g
         return g
 
@@ -99,7 +107,8 @@ class BatchPipeline:
     @torch.inference_mode()
     def run_raw(self, host_batches: Iterable[Tuple[Tensor, Tensor]]) -> Iterator[List[Tensor]]:
         """Like `run`, but yields the pinned host copies of the device step's outputs: ids, frames, counts, encoded_len
-        (+ word_start, word_end, word_first, word_ntok, n_words with `with_words`)."""
+        (+ word_start, word_end, word_first, word_ntok, n_words with `with_words`; + token_logp, path_logp, path_rows with
+        `with_scores`)."""
         model = self.model
         compute = torch.cuda.current_stream(self.dev)
         it = iter(host_batches)
@@ -124,7 +133,7 @@ class BatchPipeline:
                 g.graph.replay()
                 outs = g.out
             else:
-                outs = device_step(model, wav_d, len_d, self.with_words, self.gather)
+                outs = device_step(model, wav_d, len_d, self.with_words, self.gather, self.with_scores)
             host = [torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in outs]
             for h, t in zip(host, outs):
                 h.copy_(t, non_blocking=True)           # stream-ordered before the next replay overwrites the outputs

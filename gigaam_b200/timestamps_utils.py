@@ -8,7 +8,8 @@ word's token range.  `frames_to_words` is the reference's host function with the
 and as the checker of the device path in the tests."""
 from __future__ import annotations
 
-from typing import List, Sequence
+import math
+from typing import List, Optional, Sequence
 
 import torch
 
@@ -63,13 +64,27 @@ def token_flag_table(tokenizer) -> torch.Tensor:
     return flags
 
 
+def mean_logp_confidence(logps: Sequence[float]) -> float:
+    """exp(mean of the log-probabilities), summed in order in float64; NaN for an empty sequence or a NaN member."""
+    return math.exp(sum(float(x) for x in logps) / len(logps)) if len(logps) else math.nan
+
+
+def path_confidence(path_logp: float, path_rows: int) -> float:
+    """exp(path_logp / path_rows): the per-decision likelihood of a greedy path, blank decisions included; NaN when the
+    path has no decision rows."""
+    return math.exp(float(path_logp) / int(path_rows)) if int(path_rows) > 0 else math.nan
+
+
 def words_from_device(tokenizer, ids: Sequence[int], word_start: Sequence[int], word_end: Sequence[int],
-                      word_first: Sequence[int], word_ntok: Sequence[int], frame_shift: float) -> List[Word]:
-    """Word records of one utterance (host copies of gam_group_words' outputs) -> List[Word]."""
+                      word_first: Sequence[int], word_ntok: Sequence[int], frame_shift: float,
+                      token_logp: Optional[Sequence[float]] = None) -> List[Word]:
+    """Word records of one utterance (host copies of gam_group_words' outputs) -> List[Word].  With `token_logp` (the
+    scored decoder's per-token log-probabilities) every word gets confidence = exp(mean over its tokens)."""
     out: List[Word] = []
     for s, e, f, n in zip(word_start, word_end, word_first, word_ntok):
         pieces = [tokenizer.id_to_str(t) for t in ids[f:f + n]]
         if pieces and pieces[0].startswith(_SP_SPACE):
             pieces[0] = pieces[0][1:]
-        out.append(Word(text="".join(pieces).strip(), start=s * frame_shift, end=e * frame_shift))
+        conf = None if token_logp is None else mean_logp_confidence(token_logp[f:f + n])
+        out.append(Word(text="".join(pieces).strip(), start=s * frame_shift, end=e * frame_shift, confidence=conf))
     return out

@@ -8,10 +8,12 @@ from typing import Any, Dict, Iterator, List, Optional, Tuple
 
 
 class _Record:
-    """Positional / keyword construction over `_fields`, value equality and a readable repr."""
+    """Positional / keyword construction over `_fields`, value equality and a readable repr.  Fields in `_quiet` are
+    left out of the repr while they hold their default (None), so records without them print as before."""
     __slots__ = ()
     _fields: Tuple[str, ...] = ()
     _defaults: Dict[str, Any] = {}
+    _quiet: Tuple[str, ...] = ()
 
     def __init__(self, *args: Any, **kwargs: Any) -> None:
         if len(args) > len(self._fields):
@@ -35,36 +37,47 @@ class _Record:
         return type(other) is type(self) and all(getattr(self, n) == getattr(other, n) for n in self._fields)
 
     def __repr__(self) -> str:
-        return f"{type(self).__name__}({', '.join(f'{n}={getattr(self, n)!r}' for n in self._fields)})"
+        shown = (n for n in self._fields if n not in self._quiet or getattr(self, n) is not None)
+        return f"{type(self).__name__}({', '.join(f'{n}={getattr(self, n)!r}' for n in shown)})"
 
 
 class Word(_Record):
-    """One word with its start / end time in seconds."""
-    __slots__ = _fields = ("text", "start", "end")
+    """One word with its start / end time in seconds.  `confidence` (transcribe(..., confidence=True)) is
+    exp(mean log-probability of the word's tokens)."""
+    __slots__ = _fields = ("text", "start", "end", "confidence")
+    _defaults = {"confidence": None}
+    _quiet = ("confidence",)
     text: str
     start: float
     end: float
+    confidence: Optional[float]
 
 
 class TranscriptionResult(_Record):
-    """`transcribe()` result: `words` stays None unless word timestamps were requested."""
-    __slots__ = _fields = ("text", "words")
-    _defaults = {"words": None}
+    """`transcribe()` result: `words` stays None unless word timestamps were requested.  `confidence`
+    (confidence=True) is exp(path log-probability / decision rows) of the greedy path, blank decisions included."""
+    __slots__ = _fields = ("text", "words", "confidence")
+    _defaults = {"words": None, "confidence": None}
+    _quiet = ("confidence",)
     text: str
     words: Optional[List[Word]]
+    confidence: Optional[float]
 
     def __str__(self) -> str:
         return self.text
 
 
 class Segment(_Record):
-    """One speech segment of a long recording (times in seconds from the start of the recording)."""
-    __slots__ = _fields = ("text", "start", "end", "words")
-    _defaults = {"words": None}
+    """One speech segment of a long recording (times in seconds from the start of the recording).  `confidence` as
+    in TranscriptionResult, for the segment."""
+    __slots__ = _fields = ("text", "start", "end", "words", "confidence")
+    _defaults = {"words": None, "confidence": None}
+    _quiet = ("confidence",)
     text: str
     start: float
     end: float
     words: Optional[List[Word]]
+    confidence: Optional[float]
 
 
 class LongformTranscriptionResult(_Record):

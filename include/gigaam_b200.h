@@ -149,6 +149,8 @@ int64_t gam_workspace_bytes(const gam_handle* h, int32_t B, int64_t mel_frames);
 
 /* bytes of scratch gam_ctc_greedy / gam_rnnt_greedy need on their own (B utterances of T encoder frames) */
 int64_t gam_decode_workspace_bytes(const gam_handle* h, int32_t B, int32_t T);
+/* ... and the scored twins gam_ctc_greedy_scored / gam_rnnt_greedy_scored (>= gam_decode_workspace_bytes) */
+int64_t gam_decode_scored_workspace_bytes(const gam_handle* h, int32_t B, int32_t T);
 
 /* wav: device f32 [B, n_samples]  ->  mel: device f32 [B, n_mels, M] */
 int gam_logmel(gam_handle* h, const float* wav, int32_t B, int64_t n_samples, float* mel, void* stream);
@@ -179,6 +181,23 @@ int gam_ctc_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int3
 int gam_rnnt_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
                     int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
                     void* stream);
+
+/* Scored greedy decoding: the same ids / frames / counts as gam_*_greedy, bit for bit, plus how sure the model was.
+ * A decision row is one logit row the greedy rule evaluates: CTC, every frame t < enc_len[b]; RNN-T, every joint row of
+ * the loop of gigaam/decoding.py:184-205, emissions and blanks alike (a frame that reaches max_symbols emissions has no
+ * closing blank row).  l(row) = log_softmax(row)[label] for the label the greedy rule picks = -log sum_c exp(z_c - z_max)
+ * on a finite row; NaN on a row with a NaN or +inf logit or with only -inf logits (the label stays 0).
+ *   token_logp device f32 [B, max_out]: l of the row that emitted token i (CTC: the first frame of the token's run).
+ *   path_logp  device f32 [B]: sum of l over all decision rows of utterance b (fp64 accumulation; NaN if any row was).
+ *   path_rows  device i32 [B]: the number of those rows.
+ * An utterance's scores are bit-identical whatever batch it is decoded in.  Stream-ordered, no host sync, capturable in a
+ * CUDA graph; workspace: gam_decode_scored_workspace_bytes. */
+int gam_ctc_greedy_scored(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
+                          int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
+                          float* token_logp, float* path_logp, int32_t* path_rows, void* stream);
+int gam_rnnt_greedy_scored(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
+                           int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
+                           float* token_logp, float* path_logp, int32_t* path_rows, void* stream);
 
 /* ---- the heads' forward passes, for callers that run their own search (LM beam search, N-best rescoring, forced
  * alignment, lattice scoring).  fp32 CUDA-core arithmetic like the reference's heads; no workspace except for the joint.
@@ -355,6 +374,11 @@ int gam_test_rnnt_greedy(gam_handle* h, const float* encproj, const int32_t* len
                          const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
                          int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts, int32_t* plan,
                          void* stream);
+/* the scored twin of gam_test_rnnt_greedy (gam_rnnt_greedy_scored's kernel); plan as there */
+int gam_test_rnnt_greedy_scored(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,
+                                const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
+                                int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts,
+                                float* token_logp, float* path_logp, int32_t* path_rows, int32_t* plan, void* stream);
 /* qkv: f16 [B*T, 3*d_model]; klen i32 [B] or NULL -> out f16 [B*T, d_model].  T up to the handle's max_encoded_frames */
 int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void* out, int32_t B, int32_t T, void* stream);
 /* rel_pos variant: qkv f16 [B*T, 4*d_model] = [q+u | q+v | k | v]; pos f16 [2*max-1, d_model] laid out like pos_proj
