@@ -1,0 +1,286 @@
+// Viterbi and forward (log-sum-exp) alignment of known transcripts over caller-supplied fp32 scores
+// (include/gigaam_b200.h, gam_ctc_align / gam_rnnt_align, has the definitions).  One CTA per utterance, fixed orders and no
+// atomics, so an utterance's results are the same bits in any batch and on every call.
+//   (1) ctc_align_kernel: walks the frames t.  Viterbi and forward values of the S = 2U + 1 states are double-buffered in
+//       shared memory; each frame reads log_probs at the utterance's labels and at blank only.  Backpointers: 2 bits per
+//       (t, s), packed 16 states to a word by shuffles.
+//   (2) rnnt_align_kernel: walks the anti-diagonals d = t + u of the [T, U + 1] lattice; the nodes of one diagonal are
+//       independent.  Every value is one fp32 add of two fp32 numbers, so the walk order does not change the bits.
+//       Backpointers: 1 bit per node, 32 nodes of a diagonal to a word by ballot.
+// Both backtrack with one thread (a serial walk of T or T + U steps) and then gather token_logp with the whole CTA.
+#include <cmath>
+
+#include "kernels.h"
+#include "launch.cuh"
+
+namespace gam {
+namespace {
+
+constexpr int kSkip = 1 << 30;   // ctc lab_s: the state may also be entered from s - 2
+
+__device__ __forceinline__ float lse3(float a, float b, float c) {
+  const float m = fmaxf(fmaxf(a, b), c);
+  if (m == -INFINITY) return -INFINITY;
+  return m + logf(expf(a - m) + expf(b - m) + expf(c - m));
+}
+
+__device__ __forceinline__ float lse2(float a, float b) {
+  const float m = fmaxf(a, b);
+  if (m == -INFINITY) return -INFINITY;
+  return m + log1pf(expf(fminf(a, b) - m));
+}
+
+__device__ __forceinline__ float qnan() { return __int_as_float(0x7fc00000); }
+
+// log_probs [B, T, V1], targets [B, U] (may be null when U == 0), bp: B * T * W words, W = ctc_bp_words(U)
+__global__ void ctc_align_kernel(const float* __restrict__ log_probs, const int* __restrict__ enc_len, const int* __restrict__ targets,
+                                 const int* __restrict__ target_len, int T, int U, int V1, uint32_t* __restrict__ bp, int* __restrict__ frames,
+                                 float* __restrict__ token_logp, float* __restrict__ viterbi_logp, float* __restrict__ log_likelihood,
+                                 int* __restrict__ path_rows) {
+  extern __shared__ float4 smem_f4[];
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x, lane = tid & 31;
+  const int Tb = min(max(enc_len[b], 0), T), Ub = min(max(target_len[b], 0), U);
+  const int S = 2 * Ub + 1, Smax = 2 * U + 1, W = (Smax + 15) / 16;
+  int* lab_s = reinterpret_cast<int*>(smem_f4);   // [Smax]: l'_s | kSkip
+  float* va = reinterpret_cast<float*>(lab_s + Smax);
+  float* vb = va + Smax;
+  float* fa = vb + Smax;
+  float* fb = fa + Smax;
+  __shared__ int final_s;
+  const int blank = V1 - 1;
+  const int* y = targets + static_cast<int64_t>(b) * U;
+  int bad = 0;
+  for (int s = tid; s < S; s += nt) {
+    int l = blank;
+    if (s & 1) {
+      l = y[s >> 1];
+      if (l < 0 || l >= blank) bad = 1;
+      else if (s >= 3 && l != y[(s >> 1) - 1]) l |= kSkip;
+    }
+    lab_s[s] = l;
+  }
+  bad = __syncthreads_or(bad);
+  const float* lp = log_probs + static_cast<int64_t>(b) * T * V1;
+  uint32_t* bpu = bp + static_cast<int64_t>(b) * T * W;
+  float vit = -INFINITY, fwd = -INFINITY;
+  int nan = 0;
+  if (!bad && Tb > 0) {
+    for (int s = tid; s < S; s += nt) {
+      const float x = s < 2 ? lp[lab_s[s] & ~kSkip] : -INFINITY;
+      nan |= isnan(x);
+      va[s] = fa[s] = x;
+    }
+    for (int s = tid; s < S; s += nt) {   // frame 0 reads every state's entry: the NaN rule counts them
+      if (s >= 2) nan |= isnan(lp[lab_s[s] & ~kSkip]);
+    }
+    for (int t = 1; t < Tb; ++t) {
+      __syncthreads();   // frame t - 1 complete
+      const float* row = lp + static_cast<int64_t>(t) * V1;
+      for (int s0 = 0; s0 < S; s0 += nt) {   // uniform trip count: whole warps take part in the shuffles
+        const int s = s0 + tid;
+        uint32_t code = 0;
+        if (s < S) {
+          const int l = lab_s[s];
+          float best = va[s];
+          float fm1 = -INFINITY, fm2 = -INFINITY;
+          if (s >= 1) {
+            const float c = va[s - 1];
+            if (c > best) { best = c; code = 1; }
+            fm1 = fa[s - 1];
+          }
+          if (l & kSkip) {
+            const float c = va[s - 2];
+            if (c > best) { best = c; code = 2; }
+            fm2 = fa[s - 2];
+          }
+          const float x = row[l & ~kSkip];
+          nan |= isnan(x);
+          vb[s] = x + best;
+          fb[s] = x + lse3(fa[s], fm1, fm2);
+        }
+        uint32_t word = code << (2 * (lane & 15));
+#pragma unroll
+        for (int off = 1; off < 16; off <<= 1) word |= __shfl_xor_sync(0xffffffffu, word, off);
+        if ((lane & 15) == 0 && s < S) bpu[static_cast<int64_t>(t) * W + s / 16] = word;
+      }
+      float* tmp = va; va = vb; vb = tmp;
+      tmp = fa; fa = fb; fb = tmp;
+    }
+  }
+  nan = __syncthreads_or(nan);   // also completes the last frame
+  if (tid == 0) {
+    int fs = -1;
+    if (!bad && !nan && Tb > 0) {
+      fs = S - 1;
+      vit = va[S - 1];
+      fwd = fa[S - 1];
+      if (S >= 2) {
+        if (va[S - 2] > vit) { vit = va[S - 2]; fs = S - 2; }
+        fwd = lse2(fa[S - 1], fa[S - 2]);
+      }
+    }
+    if (bad || nan) vit = fwd = qnan();
+    viterbi_logp[b] = vit;
+    log_likelihood[b] = fwd;
+    path_rows[b] = Tb;
+    final_s = (vit == -INFINITY || vit != vit) ? -1 : fs;
+  }
+  __syncthreads();
+  int* fr = frames + static_cast<int64_t>(b) * U;
+  float* tl = token_logp + static_cast<int64_t>(b) * U;
+  const int fs = final_s;
+  for (int i = tid; i < U; i += nt) fr[i] = -1;
+  __syncthreads();
+  if (fs >= 0 && tid == 0) {   // serial backtrack: a token's frame is the first frame of its run
+    int s = fs;
+    for (int t = Tb - 1; t >= 0; --t) {
+      if (s & 1) fr[s >> 1] = t;
+      if (t > 0) s -= (bpu[static_cast<int64_t>(t) * W + s / 16] >> (2 * (s & 15))) & 3u;
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < U; i += nt) {
+    float v = -INFINITY;
+    if (i < Ub) {
+      if (bad || nan) v = qnan();
+      else if (fs >= 0) v = lp[static_cast<int64_t>(fr[i]) * V1 + y[i]];
+    }
+    tl[i] = v;
+  }
+}
+
+// blank / label [B, T, U + 1]; bp: B * (T + U) * W words, W = rnnt_bp_words(U)
+__global__ void rnnt_align_kernel(const float* __restrict__ blank, const float* __restrict__ label, const int* __restrict__ enc_len,
+                                  const int* __restrict__ target_len, int T, int U, uint32_t* __restrict__ bp, int* __restrict__ frames,
+                                  float* __restrict__ token_logp, float* __restrict__ viterbi_logp, float* __restrict__ log_likelihood,
+                                  int* __restrict__ path_rows) {
+  extern __shared__ float4 smem_f4[];
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x, lane = tid & 31;
+  const int U1 = U + 1, W = (U1 + 31) / 32;
+  const int Tb = min(max(enc_len[b], 0), T), Ub = min(max(target_len[b], 0), U);
+  float* va = reinterpret_cast<float*>(smem_f4);   // [U1] per diagonal, indexed by u
+  float* vb = va + U1;
+  float* fa = vb + U1;
+  float* fb = fa + U1;
+  __shared__ int ok_s;
+  const float* bl = blank + static_cast<int64_t>(b) * T * U1;
+  const float* lb = label + static_cast<int64_t>(b) * T * U1;
+  uint32_t* bpu = bp + static_cast<int64_t>(b) * (T + U) * W;
+  int nan = 0;
+  if (Tb > 0) {
+    if (tid == 0) va[0] = fa[0] = 0.f;
+    const int D = Tb - 1 + Ub;
+    for (int d = 1; d <= D; ++d) {
+      __syncthreads();   // diagonal d - 1 complete
+      const int lo = max(0, d - (Tb - 1)), hi = min(Ub, d);
+      for (int u0 = 0; u0 <= hi; u0 += nt) {   // uniform trip count for the ballot
+        const int u = u0 + tid;
+        bool take = false;
+        if (u >= lo && u <= hi) {
+          const int t = d - u;
+          float cb = -INFINITY, cl = -INFINITY, fbk = -INFINITY, flk = -INFINITY;
+          if (t > 0) {
+            const float x = bl[static_cast<int64_t>(t - 1) * U1 + u];
+            nan |= isnan(x);
+            cb = va[u] + x;
+            fbk = fa[u] + x;
+          }
+          if (u > 0) {
+            const float x = lb[static_cast<int64_t>(t) * U1 + u - 1];
+            nan |= isnan(x);
+            cl = va[u - 1] + x;
+            flk = fa[u - 1] + x;
+            take = t == 0 || cl > cb;   // ties: the blank edge
+          }
+          vb[u] = take ? cl : cb;
+          fb[u] = lse2(fbk, flk);
+        }
+        const uint32_t word = __ballot_sync(0xffffffffu, take);
+        if (lane == 0 && u <= hi) bpu[static_cast<int64_t>(d) * W + u / 32] = word;
+      }
+      float* tmp = va; va = vb; vb = tmp;
+      tmp = fa; fa = fb; fb = tmp;
+    }
+  }
+  // the closing blank edge is read before the reduction, so that a NaN there reaches every thread's flag
+  float x_end = 0.f;
+  if (tid == 0 && Tb > 0) {
+    x_end = bl[static_cast<int64_t>(Tb - 1) * U1 + Ub];
+    nan |= isnan(x_end);
+  }
+  nan = __syncthreads_or(nan);
+  if (tid == 0) {
+    float vit = -INFINITY, fwd = -INFINITY;
+    if (Tb > 0) {
+      vit = va[Ub] + x_end;
+      fwd = fa[Ub] + x_end;
+    }
+    if (nan) vit = fwd = qnan();
+    viterbi_logp[b] = vit;
+    log_likelihood[b] = fwd;
+    path_rows[b] = Tb + Ub;
+    ok_s = !(vit == -INFINITY || vit != vit);
+  }
+  __syncthreads();
+  int* fr = frames + static_cast<int64_t>(b) * U;
+  float* tl = token_logp + static_cast<int64_t>(b) * U;
+  const int ok = ok_s;
+  for (int i = tid; i < U; i += nt) fr[i] = -1;
+  __syncthreads();
+  if (ok && tid == 0) {   // serial backtrack from (Tb - 1, Ub): a label edge out of (t, u - 1) emits token u - 1 at frame t
+    int t = Tb - 1, u = Ub;
+    while (t + u > 0) {
+      if ((bpu[static_cast<int64_t>(t + u) * W + u / 32] >> (u & 31)) & 1u) {
+        fr[u - 1] = t;
+        --u;
+      } else {
+        --t;
+      }
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < U; i += nt) {
+    float v = -INFINITY;
+    if (i < Ub) {
+      if (nan) v = qnan();
+      else if (ok) v = lb[static_cast<int64_t>(fr[i]) * U1 + i];
+    }
+    tl[i] = v;
+  }
+}
+
+int align_threads(int n) { return n <= 64 ? 64 : n >= 1024 ? 1024 : (n + 31) / 32 * 32; }
+
+}  // namespace
+
+int64_t ctc_bp_words(int T, int U) { return static_cast<int64_t>(T) * ((2 * U + 1 + 15) / 16); }
+int64_t rnnt_bp_words(int T, int U) { return static_cast<int64_t>(T + U) * ((U + 1 + 31) / 32); }
+
+int launch_ctc_align(const float* log_probs, const int* enc_len, const int* targets, const int* target_len, int B, int T, int U, int V1,
+                     uint32_t* bp, int* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int* path_rows,
+                     cudaStream_t s) {
+  static PerDeviceOnce attr_once;
+  if (U > kAlignMaxTokens) return 1;
+  if (attr_once.first() && cudaFuncSetAttribute(ctc_align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                5 * (2 * kAlignMaxTokens + 1) * 4) != cudaSuccess)
+    return -1;
+  const size_t smem = static_cast<size_t>(5) * (2 * U + 1) * 4;
+  ctc_align_kernel<<<B, align_threads(2 * U + 1), smem, s>>>(log_probs, enc_len, targets, target_len, T, U, V1, bp, frames, token_logp,
+                                                            viterbi_logp, log_likelihood, path_rows);
+  return 0;
+}
+
+int launch_rnnt_align(const float* blank, const float* label, const int* enc_len, const int* target_len, int B, int T, int U, uint32_t* bp,
+                      int* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int* path_rows, cudaStream_t s) {
+  static PerDeviceOnce attr_once;
+  if (U > kAlignMaxTokens) return 1;
+  if (attr_once.first() && cudaFuncSetAttribute(rnnt_align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                4 * (kAlignMaxTokens + 1) * 4) != cudaSuccess)
+    return -1;
+  const size_t smem = static_cast<size_t>(4) * (U + 1) * 4;
+  rnnt_align_kernel<<<B, align_threads(U + 1), smem, s>>>(blank, label, enc_len, target_len, T, U, bp, frames, token_logp, viterbi_logp,
+                                                          log_likelihood, path_rows);
+  return 0;
+}
+
+}  // namespace gam

@@ -153,7 +153,7 @@ struct gam_handle {
 enum ProfClass : int {
   PC_LOGMEL = 0, PC_SUB_CONV1, PC_GEMM_CONV2, PC_GEMM_SUBOUT, PC_GEMM_FFN_UP, PC_GEMM_FFN_DOWN, PC_GEMM_QKV, PC_GEMM_PROJ,
   PC_GEMM_GLU, PC_LAYERNORM, PC_ATTENTION, PC_DWCONV, PC_CTC_ARGMAX, PC_CTC_COLLAPSE, PC_RNNT_ENCPROJ, PC_RNNT_GREEDY,
-  PC_MISC, PC_CTC_LOG_PROBS, PC_RNNT_JOINT, PC_RNNT_PREDICT, PC_EMO_HEAD, PC_HEAD_BACKWARD, PC_COUNT
+  PC_MISC, PC_CTC_LOG_PROBS, PC_RNNT_JOINT, PC_RNNT_PREDICT, PC_EMO_HEAD, PC_HEAD_BACKWARD, PC_ALIGN, PC_COUNT
 };
 
 struct ProfScope {
@@ -791,6 +791,105 @@ int gam_rnnt_joint(gam_handle* h, const float* enc, const float* dec, int32_t B,
   return 0;
 }
 
+// ---- alignment of known transcripts (csrc/align.cu; stage 1 of RNN-T: the gathered joint of heads.cu)
+int64_t gam_ctc_align_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!h || h->cfg.head != 1 || B <= 0 || T <= 0 || T > h->max_t || U < 0 || U > kAlignMaxTokens) return -1;
+  return align_up(static_cast<int64_t>(B) * ctc_bp_words(T, U) * 4, 1024);
+}
+
+int gam_ctc_align(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets, const int32_t* target_len,
+                  int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                  float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 1) return fail(h, -1, "ctc_align: model has no CTC head");
+  if (B <= 0 || T <= 0 || U < 0) return fail(h, -1, "ctc_align: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
+  if (T > h->max_t) return fail(h, -1, "ctc_align: T=%d exceeds the handle's max_encoded_frames %d", T, h->max_t);
+  if (U > kAlignMaxTokens) return fail(h, -1, "ctc_align: U=%d exceeds %d tokens per utterance", U, kAlignMaxTokens);
+  if (!log_probs || !enc_len || !target_len || (U > 0 && (!targets || !frames || !token_logp)) || !viterbi_logp || !log_likelihood ||
+      !path_rows)
+    return fail(h, -1, "ctc_align: a required pointer is NULL");
+  const int64_t need = gam_ctc_align_workspace_bytes(h, B, T, U);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "ctc_align: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  { PROF(PC_ALIGN);
+    rc = launch_ctc_align(log_probs, enc_len, targets, target_len, B, T, U, c.num_classes, static_cast<uint32_t*>(workspace), frames,
+                          token_logp, viterbi_logp, log_likelihood, path_rows, s); }
+  if (rc != 0) return fail(h, -4, "ctc_align: launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, "ctc_align");
+  return 0;
+}
+
+int64_t gam_rnnt_align_scores_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || T > h->max_t || U < 0 || U > kAlignMaxTokens) return -1;
+  return gam_rnnt_joint_workspace_bytes(h, B, T, U + 1);
+}
+
+int gam_rnnt_align_scores(gam_handle* h, const float* enc, const float* dec, const int32_t* targets, int32_t B, int32_t T, int32_t U,
+                          void* workspace, int64_t workspace_bytes, float* blank, float* label, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 2) return fail(h, -1, "rnnt_align_scores: model has no RNN-T head");
+  if (B <= 0 || T <= 0 || U < 0) return fail(h, -1, "rnnt_align_scores: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
+  if (T > h->max_t) return fail(h, -1, "rnnt_align_scores: T=%d exceeds the handle's max_encoded_frames %d", T, h->max_t);
+  if (U > kAlignMaxTokens) return fail(h, -1, "rnnt_align_scores: U=%d exceeds %d tokens per utterance", U, kAlignMaxTokens);
+  const int U1 = U + 1;
+  constexpr int64_t kMaxProjRows = 65535LL * 64;   // grid.y limit of the projection GEMMs (64 rows per block)
+  if (static_cast<int64_t>(B) * T > kMaxProjRows || static_cast<int64_t>(B) * U1 > kMaxProjRows)
+    return fail(h, -1, "rnnt_align_scores: B*T and B*(U+1) must be <= %lld (B=%d, T=%d, U=%d)", (long long)kMaxProjRows, B, T, U);
+  const int J = c.joint_hidden;
+  if (J % 4 != 0 || J > rnnt_joint_max_hidden() || c.pred_hidden % 16 != 0 || c.d_model % 16 != 0)
+    return fail(h, -1, "rnnt_align_scores: needs joint_hidden %% 4 == 0 and <= %d, pred_hidden %% 16 == 0 (joint_hidden %d, pred_hidden %d)",
+                rnnt_joint_max_hidden(), J, c.pred_hidden);
+  if (!enc || !dec || (U > 0 && !targets) || !blank || !label) return fail(h, -1, "rnnt_align_scores: a required pointer is NULL");
+  const int64_t need = gam_rnnt_align_scores_workspace_bytes(h, B, T, U);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "rnnt_align_scores: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  // the projections of gam_rnnt_joint, carved the same way
+  uint8_t* ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
+  float* E = reinterpret_cast<float*>(ws);
+  float* P = reinterpret_cast<float*>(ws + align_up(static_cast<int64_t>(B) * T * J * 4, 1024));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc = 0;
+  { PROF(PC_RNNT_JOINT);
+    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, E, B * T, J, c.d_model, s); }
+  { PROF(PC_RNNT_JOINT);
+    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, P, B * U1, J, c.pred_hidden, s); }
+  { PROF(PC_RNNT_JOINT);
+    rc = launch_rnnt_joint_gather(E, P, h->w.rnnt_wo, h->w.rnnt_bo, targets, blank, label, B, T, U1, J, c.num_classes, s); }
+  if (rc != 0) return fail(h, -4, "rnnt_align_scores: launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, "rnnt_align_scores");
+  return 0;
+}
+
+int64_t gam_rnnt_align_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || T > h->max_t || U < 0 || U > kAlignMaxTokens) return -1;
+  return align_up(static_cast<int64_t>(B) * rnnt_bp_words(T, U) * 4, 1024);
+}
+
+int gam_rnnt_align(gam_handle* h, const float* blank, const float* label, const int32_t* enc_len, const int32_t* target_len, int32_t B,
+                   int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                   float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream) {
+  if (h->cfg.head != 2) return fail(h, -1, "rnnt_align: model has no RNN-T head");
+  if (B <= 0 || T <= 0 || U < 0) return fail(h, -1, "rnnt_align: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
+  if (T > h->max_t) return fail(h, -1, "rnnt_align: T=%d exceeds the handle's max_encoded_frames %d", T, h->max_t);
+  if (U > kAlignMaxTokens) return fail(h, -1, "rnnt_align: U=%d exceeds %d tokens per utterance", U, kAlignMaxTokens);
+  if (!blank || !label || !enc_len || !target_len || (U > 0 && (!frames || !token_logp)) || !viterbi_logp || !log_likelihood ||
+      !path_rows)
+    return fail(h, -1, "rnnt_align: a required pointer is NULL");
+  const int64_t need = gam_rnnt_align_workspace_bytes(h, B, T, U);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "rnnt_align: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  { PROF(PC_ALIGN);
+    rc = launch_rnnt_align(blank, label, enc_len, target_len, B, T, U, static_cast<uint32_t*>(workspace), frames, token_logp,
+                           viterbi_logp, log_likelihood, path_rows, s); }
+  if (rc != 0) return fail(h, -4, "rnnt_align: launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, "rnnt_align");
+  return 0;
+}
+
 int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g, float* h1,
                      float* c1, void* stream) {
   const gam_config& c = h->cfg;
@@ -1119,7 +1218,7 @@ const char* gam_profile_class_name(int32_t cls) {
   static const char* names[PC_COUNT] = {"logmel", "subsample_conv1", "gemm_conv2_implicit", "gemm_subsample_out", "gemm_ffn_up_silu",
                                         "gemm_ffn_down_res", "gemm_qkv", "gemm_proj_res", "gemm_pw1_glu", "layernorm", "attention",
                                         "dwconv_bn_silu", "ctc_head_argmax", "ctc_collapse", "rnnt_enc_proj", "rnnt_greedy", "misc",
-                                        "ctc_log_probs", "rnnt_joint", "rnnt_predict", "emo_head", "head_backward"};
+                                        "ctc_log_probs", "rnnt_joint", "rnnt_predict", "emo_head", "head_backward", "align"};
   return (cls >= 0 && cls < PC_COUNT) ? names[cls] : "?";
 }
 

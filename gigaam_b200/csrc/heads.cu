@@ -118,10 +118,17 @@ __host__ __device__ constexpr int joint_kpad(int J) { return (J + kJBK - 1) / kJ
 __host__ __device__ constexpr size_t joint_smem_bytes(int J) { return (static_cast<size_t>(joint_kpad(J)) + kJBK) * kJLd * 4; }
 
 // E [B*T, J], P [B*U, J] (biases included), W_o [V1, J], b_o [V1] -> out [B, T, U, V1], row (b, t, u) = (b*T + t)*U + u.
+// kGather (gam_rnnt_align_scores): the same rows, tiles and running statistics, but of each row only the blank logit and
+// the logit of the row's next label are kept: U = U_y + 1 lattice columns, targets [B, U_y] i32, and
+//   blank_out[row] = log_softmax(row)[V1 - 1],  label_out[row] = log_softmax(row)[targets[b, u]] for u < U_y
+// (NaN for an id outside [0, V1 - 1), -inf at u = U_y).  Each is the same fp32 subtraction as the lattice's, so it is
+// bit-identical to the matching lattice entry.  out is unused and no [V1] row is stored.
+template <bool kGather>
 __global__ void __launch_bounds__(kJThreads) rnnt_joint_kernel(const float* __restrict__ E, const float* __restrict__ P,
                                                                const float* __restrict__ Wo, const float* __restrict__ bo,
                                                                float* __restrict__ out, int T, int U, int J, int V1,
-                                                               int64_t rows) {
+                                                               int64_t rows, const int* __restrict__ targets,
+                                                               float* __restrict__ blank_out, float* __restrict__ label_out) {
   extern __shared__ float4 smem_f4[];
   float* A_s = reinterpret_cast<float*>(smem_f4);   // [Jp][kJLd]: relu(E + P) of the block's rows, k-major
   const int Jp = joint_kpad(J);
@@ -129,6 +136,21 @@ __global__ void __launch_bounds__(kJThreads) rnnt_joint_kernel(const float* __re
   __shared__ float lse_s[kJBM];
   const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
   const int64_t row0 = static_cast<int64_t>(blockIdx.x) * kJBM;
+  // kGather: the kept raw logits and the label id of each row of the block (-1: none, -2: id out of range), behind W_s
+  float* blank_s = W_s + kJBK * kJLd;
+  float* label_s = blank_s + kJBM;
+  int* y_s = reinterpret_cast<int*>(label_s + kJBM);
+  if constexpr (kGather) {
+    if (tid < kJBM) {
+      const int64_t row = row0 + tid;
+      int y = -1;
+      if (row < rows && row % U < U - 1) {
+        y = targets[row / U / T * (U - 1) + row % U];
+        if (y < 0 || y >= V1 - 1) y = -2;
+      }
+      y_s[tid] = y;   // read after the main loop's barriers
+    }
+  }
 
   const int J4 = J / 4;
   for (int i = tid; i < kJBM * J4; i += kJThreads) {
@@ -189,7 +211,12 @@ __global__ void __launch_bounds__(kJThreads) rnnt_joint_kernel(const float* __re
         if (n < V1) {
           const float v = acc[i][j] + __ldg(bo + n);
           lse_push(rm[i], rs[i], v);
-          if (row < rows) orow[n] = v;
+          if constexpr (kGather) {
+            if (n == V1 - 1) blank_s[ty * 4 + i] = v;
+            if (n == y_s[ty * 4 + i]) label_s[ty * 4 + i] = v;
+          } else {
+            if (row < rows) orow[n] = v;
+          }
         }
       }
     }
@@ -206,6 +233,15 @@ __global__ void __launch_bounds__(kJThreads) rnnt_joint_kernel(const float* __re
     if (tx == 0) lse_s[ty * 4 + i] = rm[i] + logf(rs[i]);
   }
   __syncthreads();
+  if constexpr (kGather) {
+    const int64_t row = row0 + tid;
+    if (tid < kJBM && row < rows) {
+      blank_out[row] = blank_s[tid] - lse_s[tid];
+      const int y = y_s[tid];
+      label_out[row] = y >= 0 ? label_s[tid] - lse_s[tid] : (y == -1 ? -INFINITY : __int_as_float(0x7fc00000));
+    }
+    return;
+  }
   const int64_t left = rows - row0;
   const int n = static_cast<int>(left < kJBM ? left : kJBM) * V1;
   float* base = out + row0 * V1;
@@ -304,12 +340,30 @@ int launch_rnnt_joint(const float* E, const float* P, const float* Wo, const flo
   static PerDeviceOnce attr_once;
   if (J % 4 != 0 || J > rnnt_joint_max_hidden()) return 1;
   if (attr_once.first() &&
-      cudaFuncSetAttribute(rnnt_joint_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kJointMaxSmem)) != cudaSuccess)
+      cudaFuncSetAttribute(rnnt_joint_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kJointMaxSmem)) !=
+          cudaSuccess)
     return -1;
   const int64_t rows = static_cast<int64_t>(B) * T * U;
   const int64_t blocks = (rows + kJBM - 1) / kJBM;
   if (blocks > 0x7fffffff) return 1;
-  rnnt_joint_kernel<<<static_cast<unsigned>(blocks), kJThreads, joint_smem_bytes(J), s>>>(E, P, Wo, bo, out, T, U, J, V1, rows);
+  rnnt_joint_kernel<false><<<static_cast<unsigned>(blocks), kJThreads, joint_smem_bytes(J), s>>>(E, P, Wo, bo, out, T, U, J, V1, rows,
+                                                                                                  nullptr, nullptr, nullptr);
+  return 0;
+}
+
+int launch_rnnt_joint_gather(const float* E, const float* P, const float* Wo, const float* bo, const int* targets, float* blank,
+                             float* label, int B, int T, int U1, int J, int V1, cudaStream_t s) {
+  static PerDeviceOnce attr_once;
+  constexpr size_t kExtra = 3 * kJBM * 4;   // blank_s, label_s, y_s
+  if (J % 4 != 0 || J > rnnt_joint_max_hidden()) return 1;
+  if (attr_once.first() && cudaFuncSetAttribute(rnnt_joint_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                static_cast<int>(kJointMaxSmem + kExtra)) != cudaSuccess)
+    return -1;
+  const int64_t rows = static_cast<int64_t>(B) * T * U1;
+  const int64_t blocks = (rows + kJBM - 1) / kJBM;
+  if (blocks > 0x7fffffff) return 1;
+  rnnt_joint_kernel<true><<<static_cast<unsigned>(blocks), kJThreads, joint_smem_bytes(J) + kExtra, s>>>(
+      E, P, Wo, bo, nullptr, T, U1, J, V1, rows, targets, blank, label);
   return 0;
 }
 

@@ -92,9 +92,23 @@ constexpr size_t kJointMaxSmem = 200 * 1024;
 int rnnt_joint_max_hidden();
 int launch_rnnt_joint(const float* E, const float* P, const float* Wo, const float* bo, float* out, int B, int T, int U, int J,
                       int V1, cudaStream_t s);
+// the same rows, but only blank [B, T, U1] and label [B, T, U1] = the log-probs of blank and of targets[b, u] (targets [B, U1 - 1])
+int launch_rnnt_joint_gather(const float* E, const float* P, const float* Wo, const float* bo, const int* targets, float* blank,
+                             float* label, int B, int T, int U1, int J, int V1, cudaStream_t s);
 // one step u of the 1-layer prediction LSTM (heads.cu: lstm_step_kernel documents the operands); H <= 1024
 void launch_lstm_step(const int64_t* x, int U, int u, int V1, const float* emb_gates, const float* whh_t, const float* h_in,
                       int64_t h_pitch, const float* c_in, float* g, float* h_out, float* c_out, int B, int H, cudaStream_t s);
+
+// align.cu: Viterbi + forward alignment over caller scores, one CTA per utterance (gam_ctc_align / gam_rnnt_align).
+// bp: backpointer scratch of B * ctc_bp_words(T, U) / B * rnnt_bp_words(T, U) words.  Return 1 for U > kAlignMaxTokens.
+constexpr int kAlignMaxTokens = 4096;
+int64_t ctc_bp_words(int T, int U);
+int64_t rnnt_bp_words(int T, int U);
+int launch_ctc_align(const float* log_probs, const int* enc_len, const int* targets, const int* target_len, int B, int T, int U, int V1,
+                     uint32_t* bp, int* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int* path_rows,
+                     cudaStream_t s);
+int launch_rnnt_align(const float* blank, const float* label, const int* enc_len, const int* target_len, int B, int T, int U, uint32_t* bp,
+                      int* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int* path_rows, cudaStream_t s);
 
 // head_grads.cu: backward passes of the heads (fp32, deterministic, no atomics).  Rows are 64-bit.
 // dl = G - exp(logp) * rowsum(G), rows of V1

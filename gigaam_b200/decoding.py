@@ -22,6 +22,24 @@ class Tokenizer:
             self.model = SentencePieceProcessor()
             self.model.load(model_path)
 
+    def normalize(self, text: str) -> str:
+        """The text `encode` tokenises (the reference fine-tuner's rule, gigaam/utils.py:228-239): ё -> е, whitespace runs
+        collapsed to one space and trimmed, lower case; a charwise vocabulary also drops every character it lacks."""
+        text = " ".join(text.replace("ё", "е").replace("Ё", "Е").split()).lower()
+        if self.charwise:
+            vocab = set(self.vocab)
+            text = "".join(c for c in text if c in vocab)
+        return text
+
+    def encode(self, text: str) -> List[int]:
+        """Token ids of `normalize(text)`: one id per character for a charwise vocabulary, SentencePiece's `encode` otherwise
+        (gigaam/utils.py:218-226)."""
+        text = self.normalize(text)
+        if self.charwise:
+            c2i = {c: i for i, c in enumerate(self.vocab)}
+            return [c2i[c] for c in text]
+        return list(self.model.encode(text))
+
     def decode(self, tokens: List[int]) -> str:
         if self.charwise:
             return "".join(self.vocab[tok] for tok in tokens)
@@ -92,3 +110,27 @@ class RNNTGreedyDecoding(_GreedyBase):
     def __init__(self, vocabulary: List[str], model_path: Optional[str] = None, max_symbols_per_step: int = 10):
         super().__init__(vocabulary, model_path)
         self.max_symbols = max_symbols_per_step
+
+
+def align(head, encoded: Tensor, encoded_len: Tensor, targets: Tensor, target_lengths: Tensor) -> Tuple[Tensor, ...]:
+    """Viterbi and forward alignment of known transcripts (include/gigaam_b200.h, gam_ctc_align / gam_rnnt_align).
+    encoded [B, d, T] (the encoder's output), encoded_len [B], targets [B, U] token ids in [0, V) (entries at or past
+    target_lengths[b] are ignored), target_lengths [B] -> device tensors (frames [B, U] i32, token_logp [B, U] f32,
+    viterbi_logp [B] f32, log_likelihood [B] f32, path_rows [B] i32).  CTC: gam_ctc_log_probs, then gam_ctc_align.  RNN-T:
+    the prediction network over cat[blank, y] (one launch per step), the gathered joint scores, then gam_rnnt_align.  No host
+    synchronisation: the call can be captured in a CUDA graph."""
+    eng = head._engine()
+    enc = _as_btd(encoded.to(device=eng.device, dtype=torch.float32))
+    targets = targets.to(device=eng.device)
+    target_lengths = target_lengths.to(device=eng.device)
+    if eng.head_type == 1:
+        return eng.ctc_align(eng.ctc_log_probs(enc), encoded_len, targets, target_lengths)
+    B, U = targets.shape
+    blank = eng.num_classes - 1
+    # the prediction network reads every step of its input: padding becomes blank so that it cannot poison the utterance
+    used = torch.arange(U, device=eng.device)[None, :] < target_lengths.to(torch.int64)[:, None]
+    y = torch.where(used, targets.to(torch.int64), torch.full_like(targets, blank, dtype=torch.int64))
+    x = torch.cat([torch.full((B, 1), blank, dtype=torch.int64, device=eng.device), y], 1).contiguous()
+    dec, _, _ = eng.rnnt_predict(x, None, None)
+    blank_lp, label_lp = eng.rnnt_align_scores(enc, dec, y)
+    return eng.rnnt_align(blank_lp, label_lp, encoded_len, target_lengths)

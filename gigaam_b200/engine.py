@@ -211,6 +211,7 @@ class Engine:
         self._ws_mel = _WorkspaceCache(self.WS_CACHE)
         self._ws_dec = _WorkspaceCache(self.WS_CACHE)
         self._ws_joint = _WorkspaceCache(self.WS_CACHE)
+        self._ws_align = _WorkspaceCache(self.WS_CACHE)
         self._ws_emo = _WorkspaceCache(self.WS_CACHE)
         self.handle = C.c_void_p()
         pre = cfg["preprocessor"]
@@ -618,6 +619,81 @@ class Engine:
                                            self._stream())
         _lib.check(self.lib, self.handle, rc, "gam_rnnt_predict")
         return g, h1, c1
+
+    # ------------------------------------------------------------------ alignment of known transcripts (align.cu)
+    def _align_outputs(self, B: int, U: int) -> Tuple[Tensor, ...]:
+        i32 = dict(dtype=torch.int32, device=self.device)
+        f32 = dict(dtype=torch.float32, device=self.device)
+        return (torch.empty((B, U), **i32), torch.empty((B, U), **f32), torch.empty((B,), **f32), torch.empty((B,), **f32),
+                torch.empty((B,), **i32))
+
+    @staticmethod
+    def _i32(t: Tensor, device) -> Tensor:
+        return t.to(device=device, dtype=torch.int32).contiguous()
+
+    def ctc_align(self, log_probs: Tensor, enc_len: Tensor, targets: Tensor, target_len: Tensor) -> Tuple[Tensor, ...]:
+        """log_probs [B, T, V+1] f32 contiguous (ctc_log_probs), enc_len [B], targets [B, U], target_len [B] -> (frames [B, U] i32,
+        token_logp [B, U] f32, viterbi_logp [B] f32, log_likelihood [B] f32, path_rows [B] i32) on the device (gam_ctc_align)."""
+        assert log_probs.is_cuda and log_probs.dtype == torch.float32 and log_probs.is_contiguous() and log_probs.dim() == 3
+        if self.head_type != 1:
+            raise RuntimeError("model has no CTC head")
+        B, T, _ = log_probs.shape
+        U = targets.shape[1]
+        nbytes = int(self.lib.gam_ctc_align_workspace_bytes(self.handle, B, T, U))
+        if nbytes < 0:
+            raise ValueError(f"ctc_align: bad sizes B={B}, T={T}, U={U}")
+        ws = self._ws_align.get(("ctc", B, T, U), nbytes, self.device)
+        enc_len, targets, target_len = (self._i32(t, self.device) for t in (enc_len, targets, target_len))
+        outs = self._align_outputs(B, U)
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_ctc_align(self.handle, log_probs.data_ptr(), enc_len.data_ptr(), targets.data_ptr(), target_len.data_ptr(),
+                                        B, T, U, ws.data_ptr(), ws.numel(), *[t.data_ptr() for t in outs], self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_ctc_align")
+        return outs
+
+    def rnnt_align_scores(self, enc: Tensor, dec: Tensor, targets: Tensor) -> Tuple[Tensor, Tensor]:
+        """enc [B, T, d], dec [B, U+1, pred_hidden] f32 contiguous, targets [B, U] -> (blank, label) [B, T, U+1] f32: the
+        entries of rnnt_joint's lattice that alignment reads (gam_rnnt_align_scores)."""
+        assert enc.is_cuda and dec.is_cuda and enc.dtype == dec.dtype == torch.float32
+        assert enc.is_contiguous() and dec.is_contiguous() and enc.dim() == dec.dim() == 3
+        if self.head_type != 2:
+            raise RuntimeError("model has no RNN-T head")
+        B, T, _ = enc.shape
+        U = targets.shape[1]
+        if dec.shape[0] != B or dec.shape[1] != U + 1:
+            raise ValueError(f"align scores: dec has shape {tuple(dec.shape)}, expected ({B}, {U + 1}, H)")
+        nbytes = int(self.lib.gam_rnnt_align_scores_workspace_bytes(self.handle, B, T, U))
+        if nbytes < 0:
+            raise ValueError(f"align scores: bad sizes B={B}, T={T}, U={U}")
+        ws = self._ws_joint.get((B, T, U + 1), nbytes, self.device)
+        targets = self._i32(targets, self.device)
+        blank = torch.empty((B, T, U + 1), dtype=torch.float32, device=self.device)
+        label = torch.empty((B, T, U + 1), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_rnnt_align_scores(self.handle, enc.data_ptr(), dec.data_ptr(), targets.data_ptr(), B, T, U, ws.data_ptr(),
+                                                ws.numel(), blank.data_ptr(), label.data_ptr(), self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_rnnt_align_scores")
+        return blank, label
+
+    def rnnt_align(self, blank: Tensor, label: Tensor, enc_len: Tensor, target_len: Tensor) -> Tuple[Tensor, ...]:
+        """blank / label [B, T, U+1] f32 contiguous, enc_len [B], target_len [B] -> the outputs of ctc_align (gam_rnnt_align)."""
+        assert blank.is_cuda and label.is_cuda and blank.dtype == label.dtype == torch.float32
+        assert blank.is_contiguous() and label.is_contiguous() and blank.dim() == 3 and blank.shape == label.shape
+        if self.head_type != 2:
+            raise RuntimeError("model has no RNN-T head")
+        B, T, U1 = blank.shape
+        U = U1 - 1
+        nbytes = int(self.lib.gam_rnnt_align_workspace_bytes(self.handle, B, T, U))
+        if nbytes < 0:
+            raise ValueError(f"rnnt_align: bad sizes B={B}, T={T}, U={U}")
+        ws = self._ws_align.get(("rnnt", B, T, U), nbytes, self.device)
+        enc_len, target_len = self._i32(enc_len, self.device), self._i32(target_len, self.device)
+        outs = self._align_outputs(B, U)
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_rnnt_align(self.handle, blank.data_ptr(), label.data_ptr(), enc_len.data_ptr(), target_len.data_ptr(), B, T,
+                                         U, ws.data_ptr(), ws.numel(), *[t.data_ptr() for t in outs], self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_rnnt_align")
+        return outs
 
     # ------------------------------------------------------------------ backward passes of the head calls (head_grads.cu)
     def _empty(self, *shape) -> Tensor:

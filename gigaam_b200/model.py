@@ -4,7 +4,8 @@ prepare_wav, GigaAMASR.transcribe / _decode, GigaAMEmo.get_probs / forward_for_e
 registry keyed on the same class names."""
 from __future__ import annotations
 
-from typing import Dict, List, Optional, Tuple, Union
+import math
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -15,9 +16,10 @@ from .decoding import CTCGreedyDecoding, RNNTGreedyDecoding, _as_btd
 from .encoder import ConformerEncoder
 from .engine import Engine
 from .preprocess import SAMPLE_RATE, FeatureExtractor, load_audio
-from .types import TranscriptionResult, Word
+from .types import Alignment, TranscriptionResult, Word
 
 LONGFORM_THRESHOLD = 25 * SAMPLE_RATE
+ALIGN_MAX_TOKENS = 4096   # kAlignMaxTokens of csrc/kernels.h
 
 _REGISTRY = {
     "FeatureExtractor": FeatureExtractor, "ConformerEncoder": ConformerEncoder, "CTCHead": CTCHead,
@@ -288,6 +290,65 @@ class GigaAMASR(GigaAM):
         elif boundaries is None:
             raise ValueError("boundaries are required when segments are given")
         return transcribe_segments(self, segments, boundaries, word_timestamps, fr_batch_size, confidence)
+
+    @torch.inference_mode()
+    def align(self, wav_file, text: Union[str, Sequence[int]], word_timestamps: bool = True) -> Alignment:
+        """Align a known transcript to one recording: `text` is a string (normalised and tokenised by
+        `Tokenizer.encode`) or a sequence of token ids.  There is no 25 s limit: any length the loaded model encodes is
+        accepted (INTEGRATION.md §7d)."""
+        wav, length = self.prepare_wav(wav_file)
+        return self.align_batch(wav, length, [text], word_timestamps)[0]
+
+    @torch.inference_mode()
+    def align_batch(self, wav: Tensor, lengths: Tensor, texts: Sequence[Union[str, Sequence[int]]],
+                    word_timestamps: bool = True) -> List[Alignment]:
+        """Align texts[b] to wav[b, :lengths[b]] for every b (Viterbi words, forward log-likelihood, path confidence).
+        Raises ValueError before any device work for an empty batch, len(texts) != B, more than 4096 tokens or an id outside
+        [0, V).  An utterance without an alignment (too few frames for its tokens) gets log_likelihood = -inf and no words."""
+        from .decoding import align
+        from .timestamps_utils import path_confidence
+        B = int(wav.shape[0]) if wav.dim() == 2 else 0
+        if B == 0:
+            raise ValueError("align: empty batch")
+        if len(texts) != B:
+            raise ValueError(f"align: {len(texts)} texts for a batch of {B} recordings")
+        tok = self.decoding.tokenizer
+        V = len(tok)
+        norm, ids = [], []
+        for text in texts:
+            if isinstance(text, str):
+                row = tok.encode(text)
+                norm.append(tok.normalize(text))
+            else:
+                row = [int(i) for i in text]
+                bad = [i for i in row if not 0 <= i < V]
+                if bad:
+                    raise ValueError(f"align: token id {bad[0]} outside [0, {V})")
+                norm.append(tok.decode(row))
+            if len(row) > ALIGN_MAX_TOKENS:
+                raise ValueError(f"align: {len(row)} tokens exceed the limit of {ALIGN_MAX_TOKENS} per utterance")
+            ids.append(row)
+        U = max(len(r) for r in ids)
+        targets = torch.zeros((B, U), dtype=torch.int32)
+        for b, row in enumerate(ids):
+            targets[b, :len(row)] = torch.tensor(row, dtype=torch.int32)
+        target_len = torch.tensor([len(r) for r in ids], dtype=torch.int32)
+        encoded, encoded_len = self.forward(wav, lengths)
+        dev = encoded.device
+        targets_d, target_len_d = targets.to(dev), target_len.to(dev)
+        frames, token_logp, viterbi_logp, log_likelihood, path_rows = align(self.head, encoded, encoded_len, targets_d, target_len_d)
+        words: List[Optional[List[Word]]] = [None] * B
+        if word_timestamps:
+            words = [[] for _ in range(B)]
+            if U > 0:
+                rec = self._get_engine().group_words(targets_d, frames, target_len_d, self._word_flags())
+                found = [w for _, w in self._words_from_records(targets, target_len, encoded_len.cpu(), lengths.cpu(),
+                                                                [t.cpu() for t in rec], token_logp.cpu())]
+                vit = viterbi_logp.cpu().tolist()
+                words = [w if math.isfinite(v) else [] for w, v in zip(found, vit)]
+        ll, vit, rows = log_likelihood.cpu().tolist(), viterbi_logp.cpu().tolist(), path_rows.cpu().tolist()
+        return [Alignment(text=norm[b], words=words[b], log_likelihood=ll[b], confidence=path_confidence(vit[b], rows[b]))
+                for b in range(B)]
 
     @torch.inference_mode()
     def transcribe_batch(self, wav: Tensor, lengths: Tensor) -> List[str]:

@@ -80,6 +80,21 @@ class Segment(_Record):
     confidence: Optional[float]
 
 
+class Alignment(_Record):
+    """`align()` result: `text` is the normalised text that was aligned (characters a charwise vocabulary lacks are gone),
+    `words` its words with times and confidences from the Viterbi path (None without word timestamps), `log_likelihood`
+    the forward score log p(text | audio) summed over all paths, and `confidence` = exp(Viterbi path score / path edges)."""
+    __slots__ = _fields = ("text", "words", "log_likelihood", "confidence")
+    _defaults = {"words": None}
+    text: str
+    words: Optional[List[Word]]
+    log_likelihood: float
+    confidence: float
+
+    def __str__(self) -> str:
+        return self.text
+
+
 class LongformTranscriptionResult(_Record):
     """`transcribe_longform()` result: the segments in recording order."""
     __slots__ = _fields = ("segments",)

@@ -229,6 +229,57 @@ int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const flo
 int gam_rnnt_predict_train(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g,
                            float* h1, float* c1, float* c_seq, void* stream);
 
+/* ---- alignment of known transcripts: where in the audio a given token sequence lies, and how well the audio supports it.
+ * Notation: T_b = enc_len[b] and U_b = target_len[b], each clamped to [0, T] / [0, U]; y_1..y_U_b are utterance b's target ids,
+ * each in [0, V); blank = V (V + 1 = num_classes).  Every score is fp32 and comes from the caller.
+ *
+ * CTC (gam_ctc_align): states l' = (blank, y_1, blank, ..., y_U_b, blank), S = 2 U_b + 1.  State s is entered from s and s - 1,
+ * and from s - 2 when l'_s != blank and l'_s != l'_{s-2}.  Paths start in state 0 or 1 at t = 0 and end in S - 1 or S - 2 at
+ * t = T_b - 1.  Viterbi: v(0, s) = lp[0, l'_s] for s < 2, -inf elsewhere; v(t, s) = lp[t, l'_s] + max over the predecessors,
+ * the max taken in the order s, s - 1, s - 2 with a later candidate replacing the current one only when strictly greater (on
+ * ties, staying wins), then one fp32 add.  The final state is S - 1 unless v(T_b - 1, S - 2) > v(T_b - 1, S - 1) strictly.
+ * Forward: the same recursion with log-sum-exp (-inf, never NaN, for all -inf operands); log_likelihood = logsumexp of the
+ * final states = -F.ctc_loss(..., reduction="none").
+ *
+ * RNN-T (gam_rnnt_align): nodes (t, u), t < T_b, u <= U_b; blank(t, u) = log_softmax(joint(t, u))[V] and label(t, u) =
+ * log_softmax(joint(t, u))[y_{u+1}], u < U_b, with joint(t, u) the row gam_rnnt_joint computes for dec = predict(cat[blank, y]).
+ * Viterbi: v(0, 0) = 0, v(t, u) = max(v(t-1, u) + blank(t-1, u), v(t, u-1) + label(t, u-1)), one fp32 add per candidate, the
+ * blank edge winning ties; no max_symbols cap.  viterbi_logp = v(T_b - 1, U_b) + blank(T_b - 1, U_b).  Forward: the same with
+ * log-sum-exp; log_likelihood = -torchaudio rnnt_loss(..., reduction="none") on the log-prob lattice.
+ *
+ * Outputs per utterance b (frames / token_logp have row pitch U; entries i >= U_b are -1 / -inf):
+ *   frames [B, U] i32: CTC, the first frame of token i's run on the Viterbi path; RNN-T, the frame at which token i is emitted
+ *     (the greedy decoders' convention, so gam_group_words takes them with counts = target_len);
+ *   token_logp [B, U] f32: CTC, lp at that frame; RNN-T, label(t, i) on the emitting edge;
+ *   viterbi_logp [B], log_likelihood [B] f32; path_rows [B] i32: the edges on a path, T_b for CTC and T_b + U_b for RNN-T.
+ * No path (CTC: T_b = 0 or T_b < U_b + adjacent repeats; RNN-T: T_b = 0), or a Viterbi score of -inf: both scores -inf, every
+ * frame -1 and every token_logp -inf.  U_b = 0 is the all-blank path.  A NaN in any score the recursion reads (CTC: lp[t, blank]
+ * and lp[t, y_i], t < T_b; RNN-T: blank(t, u) for t < T_b - 1, u <= U_b, label(t, u) for t < T_b, u < U_b, and
+ * blank(T_b - 1, U_b)), or a CTC target id outside [0, V), makes both scores and every token_logp NaN and every frame -1;
+ * entries that are not read never affect the result.  One CTA per utterance with fixed orders and no atomics: an utterance's
+ * results are bit-identical in any batch and on every call.  Stream-ordered, no host synchronisation, capturable in a CUDA
+ * graph.  Limits: U <= 4096 tokens, T <= the handle's max_encoded_frames; larger sizes are refused.  The workspaces hold the
+ * backpointers (2 bits per CTC (t, s), 1 bit per RNN-T node); *_workspace_bytes return -1 for bad sizes or a handle without
+ * the head.
+ *
+ * gam_ctc_align: log_probs [B, T, V+1] (gam_ctc_log_probs), enc_len [B], targets [B, U], target_len [B], all device. */
+int64_t gam_ctc_align_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_ctc_align(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets, const int32_t* target_len,
+                  int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                  float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream);
+/* RNN-T stage 1: enc [B, T, d_model], dec [B, U+1, pred_hidden] (gam_rnnt_predict over cat[blank, y]), targets [B, U] i32
+ *   -> blank [B, T, U+1], label [B, T, U+1]: bit-identical to the matching entries of gam_rnnt_joint's lattice for the same
+ *   enc / dec, but no [.., V+1] row is ever stored.  label is -inf at u = U and NaN where targets[b, u] is outside [0, V) (so
+ *   that utterance's alignment is NaN).  Workspace: the two projections, as gam_rnnt_joint's. */
+int64_t gam_rnnt_align_scores_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_rnnt_align_scores(gam_handle* h, const float* enc, const float* dec, const int32_t* targets, int32_t B, int32_t T, int32_t U,
+                          void* workspace, int64_t workspace_bytes, float* blank, float* label, void* stream);
+/* RNN-T stage 2: blank / label [B, T, U+1] (stage 1's, or any caller scores), enc_len [B], target_len [B], all device. */
+int64_t gam_rnnt_align_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_rnnt_align(gam_handle* h, const float* blank, const float* label, const int32_t* enc_len, const int32_t* target_len, int32_t B,
+                   int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                   float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream);
+
 /* ---- backward passes of the three head calls above, for training the heads on a frozen encoder.  fp32, stream-ordered, no
  * host synchronisation and no atomics: every sum runs in an order fixed by the sizes, so two calls on the same inputs give
  * bit-identical gradients.  They use the handle's current head weights.  Every output pointer may be NULL (not computed),
