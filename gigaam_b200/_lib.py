@@ -63,7 +63,7 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_rnnt_predict_backward", "gam_test_gemm_used_slots", "gam_decode_scored_workspace_bytes",
            "gam_ctc_greedy_scored", "gam_rnnt_greedy_scored", "gam_test_rnnt_greedy_scored", "gam_ctc_align_workspace_bytes",
            "gam_ctc_align", "gam_rnnt_align_scores_workspace_bytes", "gam_rnnt_align_scores", "gam_rnnt_align_workspace_bytes",
-           "gam_rnnt_align")
+           "gam_rnnt_align", "gam_ctc_align_long_workspace_bytes", "gam_ctc_align_long", "gam_test_ctc_align_long")
 
 
 def lib_path() -> Path:
@@ -140,13 +140,16 @@ def load() -> C.CDLL:
         fn.restype = i64
     for fn in (lib.gam_rnnt_predict_train, lib.gam_ctc_log_probs_backward, lib.gam_rnnt_joint_backward, lib.gam_rnnt_predict_backward):
         fn.restype = C.c_int
-    for fn in (lib.gam_ctc_align_workspace_bytes, lib.gam_rnnt_align_scores_workspace_bytes, lib.gam_rnnt_align_workspace_bytes):
+    for fn in (lib.gam_ctc_align_workspace_bytes, lib.gam_rnnt_align_scores_workspace_bytes, lib.gam_rnnt_align_workspace_bytes,
+               lib.gam_ctc_align_long_workspace_bytes):
         fn.argtypes = [H, i32, i32, i32]
         fn.restype = i64
     lib.gam_ctc_align.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, c_vp, i64] + [c_vp] * 6
     lib.gam_rnnt_align_scores.argtypes = [H, c_vp, c_vp, c_vp, i32, i32, i32, c_vp, i64, c_vp, c_vp, c_vp]
     lib.gam_rnnt_align.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, c_vp, i64] + [c_vp] * 6
-    for fn in (lib.gam_ctc_align, lib.gam_rnnt_align_scores, lib.gam_rnnt_align):
+    lib.gam_ctc_align_long.argtypes = lib.gam_ctc_align.argtypes
+    lib.gam_test_ctc_align_long.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, c_vp, i64] + [c_vp] * 5 + [i32, c_vp, c_vp]
+    for fn in (lib.gam_ctc_align, lib.gam_rnnt_align_scores, lib.gam_rnnt_align, lib.gam_ctc_align_long, lib.gam_test_ctc_align_long):
         fn.restype = C.c_int
     lib.gam_emo_workspace_bytes.argtypes = [H, i32, i32]
     lib.gam_emo_workspace_bytes.restype = i64

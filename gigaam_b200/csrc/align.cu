@@ -7,11 +7,16 @@
 //   (2) rnnt_align_kernel: walks the anti-diagonals d = t + u of the [T, U + 1] lattice; the nodes of one diagonal are
 //       independent.  Every value is one fp32 add of two fp32 numbers, so the walk order does not change the bits.
 //       Backpointers: 1 bit per node, 32 nodes of a diagonal to a word by ballot.
-// Both backtrack with one thread (a serial walk of T or T + U steps) and then gather token_logp with the whole CTA.
+//   (3) ctc_align_long_kernel: (1) for long recordings.  One thread-block cluster of C <= 16 CTAs per utterance; CTA k
+//       owns states [k P, (k + 1) P), P a multiple of 16, and keeps their labels and double-buffered values in its own
+//       shared memory.  Each frame reads the two states left of its range from CTA k - 1 over distributed shared memory,
+//       then one cluster barrier closes the frame.  The per-state arithmetic is (1)'s, so the results are its bits.
+// All backtrack with one thread (a serial walk of T or T + U steps) and then gather token_logp with the whole CTA.
 #include <cmath>
 
 #include "kernels.h"
 #include "launch.cuh"
+#include "ptx.cuh"
 
 namespace gam {
 namespace {
@@ -249,6 +254,163 @@ __global__ void rnnt_align_kernel(const float* __restrict__ blank, const float* 
   }
 }
 
+// ctc_align_kernel over a cluster of C = %cluster_nctarank CTAs per utterance (blockIdx.x / C); bp as there.  CTA k owns
+// states [k P, min((k + 1) P, S)): 20 bytes of shared memory per state (label, two Viterbi and two forward buffers).
+// Frame t reads frame t - 1's buffer, of this CTA and of CTA k - 1 (states s - 1 and s - 2 of the first two states), and
+// writes the other buffer; one cluster barrier (release / acquire) per frame.  CTA k - 1 overwrites the buffer that CTA k
+// reads in frame t only in frame t + 1, after the barrier that CTA k reaches when its frame t is done, so one barrier per
+// frame is enough.  Every CTA checks all target ids itself, so `bad` needs no exchange; the NaN flags and the final states
+// are read by CTA 0, which then backtracks (the last barrier makes every CTA's backpointer stores visible to it) and
+// writes all outputs.
+__global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const int* __restrict__ enc_len,
+                                      const int* __restrict__ targets, const int* __restrict__ target_len, int T, int U, int V1, int P,
+                                      uint32_t* __restrict__ bp, int* __restrict__ frames, float* __restrict__ token_logp,
+                                      float* __restrict__ viterbi_logp, float* __restrict__ log_likelihood, int* __restrict__ path_rows) {
+  extern __shared__ float4 smem_f4[];
+  uint32_t C;
+  asm("mov.u32 %0, %%cluster_nctarank;" : "=r"(C));
+  const int k = static_cast<int>(ptx::cluster_ctarank());
+  const int b = blockIdx.x / C, tid = threadIdx.x, nt = blockDim.x, lane = tid & 31;
+  const int Tb = min(max(enc_len[b], 0), T), Ub = min(max(target_len[b], 0), U);
+  const int S = 2 * Ub + 1, Smax = 2 * U + 1, W = (Smax + 15) / 16;
+  const int s0 = k * P, n = min(P, S - s0);   // this CTA's states of the utterance (none when n <= 0)
+  int* lab_s = reinterpret_cast<int*>(smem_f4);   // [P]: l'_s | kSkip
+  float* vbuf = reinterpret_cast<float*>(lab_s + P);   // [2][P]: frame t in buffer t & 1
+  float* fbuf = vbuf + 2 * P;                          // [2][P]
+  __shared__ int nan_s, poison_s, final_s;
+  const int blank = V1 - 1;
+  const int* y = targets + static_cast<int64_t>(b) * U;
+  int bad = 0;
+  for (int i = tid; i < Ub; i += nt) {
+    const int l = y[i];
+    if (l < 0 || l >= blank) bad = 1;
+  }
+  for (int i = tid; i < n; i += nt) {
+    const int s = s0 + i;
+    int l = blank;
+    if (s & 1) {
+      l = y[s >> 1];
+      if (l >= 0 && l < blank && s >= 3 && l != y[(s >> 1) - 1]) l |= kSkip;
+    }
+    lab_s[i] = l;
+  }
+  bad = __syncthreads_or(bad);
+  const float* lp = log_probs + static_cast<int64_t>(b) * T * V1;
+  uint32_t* bpu = bp + static_cast<int64_t>(b) * T * W;
+  // frame buffers of CTA k - 1, as shared::cluster addresses
+  const uint32_t left_v = k > 0 ? ptx::mapa_u32(ptx::smem_u32(vbuf), k - 1) : 0u;
+  const uint32_t left_f = k > 0 ? ptx::mapa_u32(ptx::smem_u32(fbuf), k - 1) : 0u;
+  int nan = 0;
+  if (!bad && Tb > 0) {   // uniform over the cluster: every barrier below is reached by all of its threads
+    for (int i = tid; i < n; i += nt) {
+      const int s = s0 + i;
+      const float x = lp[lab_s[i] & ~kSkip];   // frame 0 reads every state's entry: the NaN rule counts them
+      nan |= isnan(x);
+      vbuf[i] = fbuf[i] = s < 2 ? x : -INFINITY;
+    }
+    for (int t = 1; t < Tb; ++t) {
+      ptx::cluster_sync();   // frame t - 1 complete in every CTA of the cluster
+      const int p = (t - 1) & 1;
+      const float* va = vbuf + p * P;
+      const float* fa = fbuf + p * P;
+      float* vb = vbuf + (p ^ 1) * P;
+      float* fb = fbuf + (p ^ 1) * P;
+      const uint32_t lv = left_v + 4u * static_cast<uint32_t>(p * P), lf = left_f + 4u * static_cast<uint32_t>(p * P);
+      const float* row = lp + static_cast<int64_t>(t) * V1;
+      for (int i0 = 0; i0 < P; i0 += nt) {   // uniform trip count: whole warps take part in the shuffles
+        const int i = i0 + tid, s = s0 + i;
+        uint32_t code = 0;
+        if (i < n) {
+          const int l = lab_s[i];
+          float best = va[i];
+          float fm1 = -INFINITY, fm2 = -INFINITY;
+          if (s >= 1) {
+            float c;
+            if (i >= 1) {
+              c = va[i - 1];
+              fm1 = fa[i - 1];
+            } else {
+              c = ptx::ld_cluster_f32(lv + 4u * (P - 1));
+              fm1 = ptx::ld_cluster_f32(lf + 4u * (P - 1));
+            }
+            if (c > best) { best = c; code = 1; }
+          }
+          if (l & kSkip) {
+            float c;
+            if (i >= 2) {
+              c = va[i - 2];
+              fm2 = fa[i - 2];
+            } else {
+              c = ptx::ld_cluster_f32(lv + 4u * (P - 2 + i));
+              fm2 = ptx::ld_cluster_f32(lf + 4u * (P - 2 + i));
+            }
+            if (c > best) { best = c; code = 2; }
+          }
+          const float x = row[l & ~kSkip];
+          nan |= isnan(x);
+          vb[i] = x + best;
+          fb[i] = x + lse3(fa[i], fm1, fm2);
+        }
+        uint32_t word = code << (2 * (lane & 15));
+#pragma unroll
+        for (int off = 1; off < 16; off <<= 1) word |= __shfl_xor_sync(0xffffffffu, word, off);
+        if ((lane & 15) == 0 && i < n) bpu[static_cast<int64_t>(t) * W + s / 16] = word;
+      }
+    }
+  }
+  nan = __syncthreads_or(nan);
+  if (tid == 0) nan_s = nan;
+  ptx::cluster_sync();   // the last frame, every CTA's flag and backpointer stores are visible to the whole cluster
+  if (k == 0 && tid == 0) {
+    for (uint32_t r = 1; r < C; ++r) nan |= ptx::ld_cluster_s32(ptx::mapa_u32(ptx::smem_u32(&nan_s), r));
+    int fs = -1;
+    float vit = -INFINITY, fwd = -INFINITY;
+    if (!bad && !nan && Tb > 0) {
+      const int p = (Tb - 1) & 1;
+      auto at = [&](const float* buf, int s) {   // state s of the last frame, in whichever CTA owns it
+        return ptx::ld_cluster_f32(ptx::mapa_u32(ptx::smem_u32(buf + p * P + s % P), s / P));
+      };
+      fs = S - 1;
+      vit = at(vbuf, S - 1);
+      fwd = at(fbuf, S - 1);
+      if (S >= 2) {
+        const float v2 = at(vbuf, S - 2);
+        if (v2 > vit) { vit = v2; fs = S - 2; }
+        fwd = lse2(fwd, at(fbuf, S - 2));
+      }
+    }
+    if (bad || nan) vit = fwd = qnan();
+    viterbi_logp[b] = vit;
+    log_likelihood[b] = fwd;
+    path_rows[b] = Tb;
+    poison_s = bad || nan;
+    final_s = (vit == -INFINITY || vit != vit) ? -1 : fs;
+  }
+  ptx::cluster_sync();   // CTA 0 is done reading the others' shared memory: they may exit
+  if (k != 0) return;
+  int* fr = frames + static_cast<int64_t>(b) * U;
+  float* tl = token_logp + static_cast<int64_t>(b) * U;
+  const int fs = final_s, poison = poison_s;
+  for (int i = tid; i < U; i += nt) fr[i] = -1;
+  __syncthreads();
+  if (fs >= 0 && tid == 0) {   // serial backtrack, as ctc_align_kernel's
+    int s = fs;
+    for (int t = Tb - 1; t >= 0; --t) {
+      if (s & 1) fr[s >> 1] = t;
+      if (t > 0) s -= (bpu[static_cast<int64_t>(t) * W + s / 16] >> (2 * (s & 15))) & 3u;
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < U; i += nt) {
+    float v = -INFINITY;
+    if (i < Ub) {
+      if (poison) v = qnan();
+      else if (fs >= 0) v = lp[static_cast<int64_t>(fr[i]) * V1 + y[i]];
+    }
+    tl[i] = v;
+  }
+}
+
 int align_threads(int n) { return n <= 64 ? 64 : n >= 1024 ? 1024 : (n + 31) / 32 * 32; }
 
 }  // namespace
@@ -267,6 +429,65 @@ int launch_ctc_align(const float* log_probs, const int* enc_len, const int* targ
   const size_t smem = static_cast<size_t>(5) * (2 * U + 1) * 4;
   ctc_align_kernel<<<B, align_threads(2 * U + 1), smem, s>>>(log_probs, enc_len, targets, target_len, T, U, V1, bp, frames, token_logp,
                                                             viterbi_logp, log_likelihood, path_rows);
+  return 0;
+}
+
+int ctc_align_long_plan(int U, int forced_ctas, int* ctas, int* states_per_cta) {
+  if (U < 0 || U > kAlignLongMaxTokens || forced_ctas < 0 || forced_ctas > kAlignLongMaxCtas) return 1;
+  int dev = 0, cap = 0;
+  cudaGetDevice(&dev);
+  if (cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) return -1;
+  const int smax = 2 * U + 1;
+  const int lo = forced_ctas ? forced_ctas : 1, hi = forced_ctas ? forced_ctas : kAlignLongMaxCtas;
+  for (int c = lo; c <= hi; ++c) {
+    const int p = ((smax + c - 1) / c + 15) / 16 * 16;
+    if ((c - 1) * p >= smax) {   // CTA c - 1 would own no state
+      if (forced_ctas) return 2;
+      continue;
+    }
+    if (static_cast<int64_t>(p) * 20 + kAlignLongStaticSmem <= cap) {
+      *ctas = c;
+      *states_per_cta = p;
+      return 0;
+    }
+  }
+  return 1;
+}
+
+int launch_ctc_align_long(const float* log_probs, const int* enc_len, const int* targets, const int* target_len, int B, int T, int U,
+                          int V1, int forced_ctas, uint32_t* bp, int* frames, float* token_logp, float* viterbi_logp,
+                          float* log_likelihood, int* path_rows, int* plan, cudaStream_t s) {
+  static PerDeviceOnce attr_once;
+  int C = 0, P = 0;
+  const int rc = ctc_align_long_plan(U, forced_ctas, &C, &P);
+  if (rc != 0) return rc;
+  if (attr_once.first()) {
+    int dev = 0, cap = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    if (cudaFuncSetAttribute(ctc_align_long_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
+        cudaFuncSetAttribute(ctc_align_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap - kAlignLongStaticSmem) != cudaSuccess)
+      return -1;
+  }
+  if (plan) {
+    plan[0] = C;
+    plan[1] = P;
+  }
+  cudaLaunchConfig_t cfg{};
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = C;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.gridDim = dim3(static_cast<unsigned>(B) * C);
+  cfg.blockDim = dim3(align_threads(P));
+  cfg.dynamicSmemBytes = static_cast<size_t>(P) * 20;
+  cfg.stream = s;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if (cudaLaunchKernelEx(&cfg, ctc_align_long_kernel, log_probs, enc_len, targets, target_len, T, U, V1, P, bp, frames, token_logp,
+                         viterbi_logp, log_likelihood, path_rows) != cudaSuccess)
+    return -2;
   return 0;
 }
 

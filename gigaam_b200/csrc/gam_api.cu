@@ -821,6 +821,55 @@ int gam_ctc_align(gam_handle* h, const float* log_probs, const int32_t* enc_len,
   return 0;
 }
 
+int64_t gam_ctc_align_long_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!h || h->cfg.head != 1 || B <= 0 || T <= 0 || U < 0 || U > kAlignLongMaxTokens) return -1;
+  return align_up(static_cast<int64_t>(B) * ctc_bp_words(T, U) * 4, 1024);
+}
+
+static int ctc_align_long_run(gam_handle* h, const char* what, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                              const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes,
+                              int32_t* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int32_t* path_rows,
+                              int32_t cluster_ctas, int32_t* plan, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 1) return fail(h, -1, "%s: model has no CTC head", what);
+  if (B <= 0 || T <= 0 || U < 0) return fail(h, -1, "%s: bad sizes (B=%d, T=%d, U=%d)", what, B, T, U);
+  if (U > kAlignLongMaxTokens) return fail(h, -1, "%s: U=%d exceeds %d tokens per utterance", what, U, kAlignLongMaxTokens);
+  if (static_cast<int64_t>(B) * kAlignLongMaxCtas > INT32_MAX) return fail(h, -1, "%s: B=%d is too large", what, B);
+  if (!log_probs || !enc_len || !target_len || (U > 0 && (!targets || !frames || !token_logp)) || !viterbi_logp || !log_likelihood ||
+      !path_rows)
+    return fail(h, -1, "%s: a required pointer is NULL", what);
+  const int64_t need = gam_ctc_align_long_workspace_bytes(h, B, T, U);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "%s: workspace too small: need %lld bytes, got %lld", what, (long long)need, (long long)workspace_bytes);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  { PROF(PC_ALIGN);
+    rc = launch_ctc_align_long(log_probs, enc_len, targets, target_len, B, T, U, c.num_classes, cluster_ctas,
+                               static_cast<uint32_t*>(workspace), frames, token_logp, viterbi_logp, log_likelihood, path_rows, plan, s); }
+  if (rc == 2) return fail(h, -1, "%s: %d CTAs leave a CTA without states at U=%d", what, cluster_ctas, U);
+  if (rc == 1) return fail(h, -1, "%s: no cluster of <= %d CTAs holds U=%d (forced %d)", what, kAlignLongMaxCtas, U, cluster_ctas);
+  if (rc != 0) return fail(h, -4, "%s: launch rejected (rc=%d): %s", what, rc, cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, what);
+  return 0;
+}
+
+int gam_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets, const int32_t* target_len,
+                       int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                       float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream) {
+  return ctc_align_long_run(h, "ctc_align_long", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes, frames,
+                            token_logp, viterbi_logp, log_likelihood, path_rows, 0, nullptr, stream);
+}
+
+int gam_test_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                            const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes,
+                            int32_t* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int32_t* path_rows,
+                            int32_t cluster_ctas, int32_t* plan, void* stream) {
+  if (cluster_ctas < 0 || cluster_ctas > kAlignLongMaxCtas)
+    return fail(h, -1, "test_ctc_align_long: cluster_ctas=%d outside [0, %d]", cluster_ctas, kAlignLongMaxCtas);
+  return ctc_align_long_run(h, "test_ctc_align_long", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes,
+                            frames, token_logp, viterbi_logp, log_likelihood, path_rows, cluster_ctas, plan, stream);
+}
+
 int64_t gam_rnnt_align_scores_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
   if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || T > h->max_t || U < 0 || U > kAlignMaxTokens) return -1;
   return gam_rnnt_joint_workspace_bytes(h, B, T, U + 1);

@@ -109,6 +109,17 @@ int launch_ctc_align(const float* log_probs, const int* enc_len, const int* targ
                      cudaStream_t s);
 int launch_rnnt_align(const float* blank, const float* label, const int* enc_len, const int* target_len, int B, int T, int U, uint32_t* bp,
                       int* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int* path_rows, cudaStream_t s);
+// the CTC sweep of launch_ctc_align over a cluster of C <= kAlignLongMaxCtas CTAs per utterance, for U <= kAlignLongMaxTokens
+// and any T (gam_ctc_align_long); bp as there.  The plan is the smallest C whose states per CTA P (a multiple of 16) fit in
+// shared memory at 20 bytes per state, or `forced_ctas` when it is > 0.  Return 0, 1 for a U or C that does not fit, 2 for a
+// forced C that leaves a CTA without states, negative on a launch error.  plan (host, 2 ints, or NULL) receives C and P.
+constexpr int kAlignLongMaxTokens = 65536;
+constexpr int kAlignLongMaxCtas = 16;
+constexpr int kAlignLongStaticSmem = 1024;   // headroom kept for the kernel's static shared memory
+int ctc_align_long_plan(int U, int forced_ctas, int* ctas, int* states_per_cta);
+int launch_ctc_align_long(const float* log_probs, const int* enc_len, const int* targets, const int* target_len, int B, int T, int U,
+                          int V1, int forced_ctas, uint32_t* bp, int* frames, float* token_logp, float* viterbi_logp,
+                          float* log_likelihood, int* path_rows, int* plan, cudaStream_t s);
 
 // head_grads.cu: backward passes of the heads (fp32, deterministic, no atomics).  Rows are 64-bit.
 // dl = G - exp(logp) * rowsum(G), rows of V1

@@ -160,6 +160,17 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// loads from a shared::cluster address (mapa_u32): another CTA's shared memory, or this CTA's own
+__device__ __forceinline__ float ld_cluster_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ int ld_cluster_s32(uint32_t addr) {
+  int v;
+  asm volatile("ld.shared::cluster.s32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
 // arrive on the mbarrier at `bar`'s offset in CTA `cta` of the cluster (this CTA included).  Default (.release.cta)
 // semantics: it releases a stage whose wgmma reads have retired (wgmma.wait_group), which needs no fence; the
 // .release.cluster form would add a MEMBAR.GPU that waits for the epilogue's global stores.

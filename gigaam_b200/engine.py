@@ -651,6 +651,34 @@ class Engine:
         _lib.check(self.lib, self.handle, rc, "gam_ctc_align")
         return outs
 
+    def ctc_align_long(self, log_probs: Tensor, enc_len: Tensor, targets: Tensor, target_len: Tensor,
+                       cluster_ctas: Optional[int] = None) -> Tuple[Tensor, ...]:
+        """ctc_align for recordings of any length and up to 65 536 tokens (gam_ctc_align_long): the same arguments and
+        outputs, and the same bits on every input ctc_align accepts.  `cluster_ctas` forces the number of CTAs per utterance
+        (gam_test_ctc_align_long); the plan used, (CTAs, states per CTA), is then kept in `last_align_long_plan`."""
+        assert log_probs.is_cuda and log_probs.dtype == torch.float32 and log_probs.is_contiguous() and log_probs.dim() == 3
+        if self.head_type != 1:
+            raise RuntimeError("model has no CTC head")
+        B, T, _ = log_probs.shape
+        U = targets.shape[1]
+        nbytes = int(self.lib.gam_ctc_align_long_workspace_bytes(self.handle, B, T, U))
+        if nbytes < 0:
+            raise ValueError(f"ctc_align_long: bad sizes B={B}, T={T}, U={U}")
+        ws = self._ws_align.get(("ctc_long", B, T, U), nbytes, self.device)
+        enc_len, targets, target_len = (self._i32(t, self.device) for t in (enc_len, targets, target_len))
+        outs = self._align_outputs(B, U)
+        ptrs = [log_probs.data_ptr(), enc_len.data_ptr(), targets.data_ptr(), target_len.data_ptr(), B, T, U, ws.data_ptr(), ws.numel(),
+                *[t.data_ptr() for t in outs]]
+        with torch.cuda.device(self.device):
+            if cluster_ctas is None:
+                rc = self.lib.gam_ctc_align_long(self.handle, *ptrs, self._stream())
+            else:
+                plan = (C.c_int32 * 2)()
+                rc = self.lib.gam_test_ctc_align_long(self.handle, *ptrs, int(cluster_ctas), plan, self._stream())
+                self.last_align_long_plan = (int(plan[0]), int(plan[1]))
+        _lib.check(self.lib, self.handle, rc, "gam_ctc_align_long")
+        return outs
+
     def rnnt_align_scores(self, enc: Tensor, dec: Tensor, targets: Tensor) -> Tuple[Tensor, Tensor]:
         """enc [B, T, d], dec [B, U+1, pred_hidden] f32 contiguous, targets [B, U] -> (blank, label) [B, T, U+1] f32: the
         entries of rnnt_joint's lattice that alignment reads (gam_rnnt_align_scores)."""

@@ -8,7 +8,9 @@ before batching, so a batch pads to its own longest member instead of the record
 pure waste on this path: the kernels mask it but still stream it)."""
 from __future__ import annotations
 
-from typing import List, Optional, Sequence, Tuple
+import bisect
+import math
+from typing import Callable, List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 from torch import Tensor
@@ -104,3 +106,115 @@ def transcribe_segments(model, segments: Sequence[Tensor], boundaries: Sequence[
             conf = path_confidence(path_logp[row], path_rows[row]) if confidence else None
             out[i] = Segment(text=text, start=seg_start, end=seg_end, words=shifted, confidence=conf)
     return LongformTranscriptionResult(segments=[s for s in out if s is not None])
+
+
+# ------------------------------------------------------------------------------------------ long-form alignment windows
+FRAME_SAMPLES = 640   # one encoder frame: hop 160 x subsampling 4, for both front ends
+
+
+class Window(NamedTuple):
+    """One encoder window of `plan_windows`: samples [start, end) of the recording; it supplies global frames
+    [keep_start, keep_end), which are its local frames shifted by start / FRAME_SAMPLES."""
+    start: int
+    end: int
+    keep_start: int
+    keep_end: int
+
+
+def _frame_multiple(seconds: float, what: str) -> int:
+    """seconds -> samples, refusing a value that is not a whole number of 40 ms encoder frames."""
+    frames = round(float(seconds) * SAMPLE_RATE / FRAME_SAMPLES)
+    if not math.isclose(frames * FRAME_SAMPLES / SAMPLE_RATE, float(seconds), rel_tol=0.0, abs_tol=1e-9):
+        raise ValueError(f"{what}={seconds} s is not a multiple of {FRAME_SAMPLES / SAMPLE_RATE} s (one encoder frame)")
+    return frames * FRAME_SAMPLES
+
+
+def plan_windows(n_samples: int, window_s: float, overlap_s: float, length_fn: Callable[[int], int],
+                 max_frames: Optional[int] = None) -> Tuple[List[Window], int]:
+    """Overlapping encoder windows over a recording of `n_samples` samples, and its encoder frame count T = length_fn(N).
+
+    W = window samples, H = (window - overlap) samples, O = overlap frames.  n = 1 window if N <= W, else
+    1 + ceil((N - W) / H); window w covers samples [w H, min(w H + W, N)) and keeps global frames [c_w, c_{w+1}) with
+    c_0 = 0, c_w = w H / 640 + floor(O / 2) and c_n = T.  The encoders' length recursions are additive in whole frames
+    (length_fn(N) = o / 640 + length_fn(N - o) for o a multiple of 640), so local frame j of window w is global frame
+    w H / 640 + j, every frame is kept exactly once, and each window keeps frames at least O / 2 from its cut ends.  A window
+    whose kept range is empty (the last one, with no overlap, when it is shorter than a frame) is still listed.
+    Raises ValueError for an empty recording, one that encodes to no frame, a window or overlap that is not a multiple of
+    40 ms, an overlap < 0 or >= the window, or a window of more than `max_frames` encoder frames."""
+    n = int(n_samples)
+    if n <= 0:
+        raise ValueError("align_longform: empty recording")
+    W = _frame_multiple(window_s, "window")
+    V = _frame_multiple(overlap_s, "overlap")
+    if W <= 0:
+        raise ValueError(f"window={window_s} s must be positive")
+    if V < 0 or V >= W:
+        raise ValueError(f"overlap={overlap_s} s must be >= 0 and shorter than the window ({window_s} s)")
+    if max_frames is not None and length_fn(W) > max_frames:
+        raise ValueError(f"window={window_s} s encodes to {length_fn(W)} frames, more than the model's max_encoded_frames "
+                         f"{max_frames}")
+    T = int(length_fn(n))
+    if T <= 0:
+        raise ValueError(f"align_longform: {n} samples encode to no frame")
+    H = W - V
+    count = 1 if n <= W else 1 + -(-(n - W) // H)
+    cuts = [0] + [w * H // FRAME_SAMPLES + V // FRAME_SAMPLES // 2 for w in range(1, count)] + [T]
+    return [Window(w * H, min(w * H + W, n), cuts[w], cuts[w + 1]) for w in range(count)], T
+
+
+def stitch_ctc_log_probs(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16) -> Tensor:
+    """CTC log-probs [1, T, V+1] f32 of a whole recording (wav [N] on the model's device, already in the model's dtype):
+    the windows are encoded through `model.forward` (the varlen path) in batches of up to `batch_size` windows of one
+    length, `model.head` (gam_ctc_log_probs) gives each batch's log-probs, and each window's kept rows are copied into
+    place.  Only one batch of window log-probs is alive at a time."""
+    if batch_size < 1:
+        raise ValueError("batch_size must be >= 1")
+    eng = model._get_engine()
+    out = torch.empty((1, T, eng.num_classes), dtype=torch.float32, device=eng.device)
+    todo = [w for w in windows if w.keep_end > w.keep_start]
+    groups: List[List[Window]] = []
+    for w in todo:   # windows of one length share a batch: no padding, so no row depends on its neighbours
+        if groups and len(groups[-1]) < batch_size and groups[-1][0].end - groups[-1][0].start == w.end - w.start:
+            groups[-1].append(w)
+        else:
+            groups.append([w])
+    for group in groups:
+        length = group[0].end - group[0].start
+        batch = torch.stack([wav[w.start:w.end] for w in group])
+        lens = torch.full((len(group),), length, dtype=torch.int64, device=wav.device)
+        encoded, _ = model.forward(batch, lens)
+        lp = model.head(encoded)
+        for row, w in enumerate(group):
+            first = w.start // FRAME_SAMPLES
+            out[0, w.keep_start:w.keep_end] = lp[row, w.keep_start - first:w.keep_end - first]
+        del lp, encoded
+    return out
+
+
+def line_segments(lines: Sequence[str], ranges: Sequence[Tuple[int, int]], frames: Sequence[int], token_logp: Sequence[float],
+                  frame_shift: float, viterbi_logp: float, words: Optional[Sequence[Word]] = None,
+                  word_first: Optional[Sequence[int]] = None) -> List[Segment]:
+    """One Segment per line of an aligned text.  ranges[i] = line i's token range [a, b) in the aligned sequence, frames /
+    token_logp the alignment's per-token outputs, words (None: no word timestamps) the words of the whole sequence with
+    word_first their first token.  A line spans the frames of its first and last token (its first word's start and its
+    last word's end) and has confidence exp(mean token log-prob); a line without tokens starts and ends where the line
+    before it ended (0.0 first), has no words and confidence NaN.  Without a path (a Viterbi score that is not finite)
+    every line has no words, NaN times and confidence 0.0."""
+    if not math.isfinite(viterbi_logp):
+        return [Segment(text=t, start=math.nan, end=math.nan, words=None if words is None else [], confidence=0.0) for t in lines]
+    from .timestamps_utils import mean_logp_confidence
+    starts = [a for a, _ in ranges]
+    by_line: List[List[Word]] = [[] for _ in lines]
+    for w, f in zip(words or [], word_first or []):
+        by_line[bisect.bisect_right(starts, f) - 1].append(w)
+    out: List[Segment] = []
+    prev_end = 0.0
+    for i, (text, (a, b)) in enumerate(zip(lines, ranges)):
+        seg_words = None if words is None else by_line[i]
+        if a == b:
+            out.append(Segment(text=text, start=prev_end, end=prev_end, words=seg_words, confidence=math.nan))
+            continue
+        start, end = frames[a] * frame_shift, (frames[b - 1] + 1) * frame_shift
+        out.append(Segment(text=text, start=start, end=end, words=seg_words, confidence=mean_logp_confidence(token_logp[a:b])))
+        prev_end = end
+    return out

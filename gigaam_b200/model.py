@@ -11,15 +11,17 @@ import numpy as np
 import torch
 from torch import Tensor, nn
 
+from . import _lib
 from .decoder import CTCHead, Linear, RNNTHead
 from .decoding import CTCGreedyDecoding, RNNTGreedyDecoding, _as_btd
 from .encoder import ConformerEncoder
 from .engine import Engine
 from .preprocess import SAMPLE_RATE, FeatureExtractor, load_audio
-from .types import Alignment, TranscriptionResult, Word
+from .types import Alignment, LongformAlignment, TranscriptionResult, Word
 
 LONGFORM_THRESHOLD = 25 * SAMPLE_RATE
 ALIGN_MAX_TOKENS = 4096   # kAlignMaxTokens of csrc/kernels.h
+ALIGN_LONG_MAX_TOKENS = 65536   # kAlignLongMaxTokens of csrc/kernels.h
 
 _REGISTRY = {
     "FeatureExtractor": FeatureExtractor, "ConformerEncoder": ConformerEncoder, "CTCHead": CTCHead,
@@ -349,6 +351,80 @@ class GigaAMASR(GigaAM):
         ll, vit, rows = log_likelihood.cpu().tolist(), viterbi_logp.cpu().tolist(), path_rows.cpu().tolist()
         return [Alignment(text=norm[b], words=words[b], log_likelihood=ll[b], confidence=path_confidence(vit[b], rows[b]))
                 for b in range(B)]
+
+    def _encoded_length(self, n_samples: int) -> int:
+        """Encoder frames of a recording of n_samples samples (the front end's and the subsampling's length rules), on the
+        host."""
+        mel = self.preprocessor.out_len(torch.tensor([int(n_samples)]))
+        return int(self.encoder.pre_encode.calc_output_length(mel)[0])
+
+    def _line_tokens(self, lines: Sequence[str]) -> Tuple[List[str], List[int], List[Tuple[int, int]]]:
+        """Normalised lines, the token ids of the whole text and each line's token range [a, b).  Lines are joined so that
+        no word spans two of them: a charwise vocabulary puts one space token between non-empty lines; SentencePiece
+        lines start with U+2581, which opens a word by itself.  (A charwise vocabulary without a space token has no word
+        boundaries at all: its lines are joined as they are.)"""
+        tok = self.decoding.tokenizer
+        space = tok.vocab.index(" ") if tok.charwise and " " in tok.vocab else None
+        norm, ids, ranges = [], [], []
+        for line in lines:
+            if not isinstance(line, str):
+                raise TypeError(f"align_longform: lines must be strings, got {type(line).__name__}")
+            row = tok.encode(line)
+            norm.append(tok.normalize(line))
+            if row and ids and space is not None:
+                ids.append(space)
+            ranges.append((len(ids), len(ids) + len(row)))
+            ids.extend(row)
+        return norm, ids, ranges
+
+    @torch.inference_mode()
+    def align_longform(self, wav_file, text: Union[str, Sequence[str]], word_timestamps: bool = True, window: float = 30.0,
+                       overlap: float = 4.0, batch_size: int = 16) -> LongformAlignment:
+        """Align a known text, one string or a sequence of lines, to a recording of any length (INTEGRATION.md §7e).  The
+        encoder runs over overlapping windows (`longform.plan_windows`), the windows' CTC log-probs are stitched into one
+        sequence and gam_ctc_align_long aligns the whole text to it: up to 65 536 tokens, no frame limit.  Returns one
+        Segment per line.  CTC models only: RNN-T raises NotImplementedError.  Raises ValueError before any device work for
+        more than 65 536 tokens and for the window plan's refusals (longform.plan_windows)."""
+        from .longform import line_segments, plan_windows, stitch_ctc_log_probs
+        from .timestamps_utils import compute_frame_shift, path_confidence, words_from_device
+        if self._ncfg["head"].get("type") == "rnnt":
+            raise NotImplementedError("align_longform needs a CTC head: RNN-T alignment walks a [T, U + 1] lattice, about "
+                                      "4.5e9 nodes for an hour of speech, and banding it would no longer give the Viterbi "
+                                      "path; use a *_ctc model, or align() up to max_encoded_frames")
+        lines = [text] if isinstance(text, str) else list(text)
+        norm, ids, ranges = self._line_tokens(lines)
+        if len(ids) > ALIGN_LONG_MAX_TOKENS:
+            raise ValueError(f"align_longform: {len(ids)} tokens exceed the limit of {ALIGN_LONG_MAX_TOKENS}")
+        if isinstance(wav_file, str):
+            wav = load_audio(wav_file)
+        else:
+            wav = torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1)
+        max_frames = self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
+        windows, T = plan_windows(wav.numel(), window, overlap, self._encoded_length, max_frames)
+        if batch_size < 1:
+            raise ValueError("batch_size must be >= 1")
+        wav, length = self.prepare_wav(wav)
+        lp = stitch_ctc_log_probs(self, wav[0], windows, T, batch_size)
+        eng = self._get_engine()
+        U = len(ids)
+        targets = torch.tensor([ids], dtype=torch.int32).reshape(1, U)
+        targets_d = targets.to(eng.device)
+        target_len_d = torch.tensor([U], dtype=torch.int32, device=eng.device)
+        enc_len = torch.tensor([T], dtype=torch.int32, device=eng.device)
+        frames, token_logp, viterbi_logp, log_likelihood, path_rows = eng.ctc_align_long(lp, enc_len, targets_d, target_len_d)
+        del lp
+        vit, ll = float(viterbi_logp[0]), float(log_likelihood[0])
+        shift = compute_frame_shift(int(length[0]), T)
+        fr, logp = frames[0].cpu().tolist(), token_logp[0].cpu().tolist()
+        words, word_first = None, None
+        if word_timestamps:
+            words, word_first = [], []
+            if U > 0 and math.isfinite(vit):
+                ws, we, wf, wn, k = (t[0].cpu().tolist() for t in eng.group_words(targets_d, frames, target_len_d, self._word_flags()))
+                words = words_from_device(self.decoding.tokenizer, ids, ws[:k], we[:k], wf[:k], wn[:k], shift, logp)
+                word_first = wf[:k]
+        segs = line_segments(norm, ranges, fr, logp, shift, vit, words, word_first)
+        return LongformAlignment(segments=segs, log_likelihood=ll, confidence=path_confidence(vit, int(path_rows[0])))
 
     @torch.inference_mode()
     def transcribe_batch(self, wav: Tensor, lengths: Tensor) -> List[str]:

@@ -95,6 +95,34 @@ class Alignment(_Record):
         return self.text
 
 
+class LongformAlignment(_Record):
+    """`align_longform()` result: one `Segment` per input line, in order (its normalised text, the start of its first token's
+    frame and the end of its last, its words, and `confidence` = exp(mean log-probability of its tokens)), plus the
+    whole recording's `log_likelihood` (forward score) and `confidence` = exp(Viterbi path score / frames), as in
+    `Alignment`."""
+    __slots__ = _fields = ("segments", "log_likelihood", "confidence")
+    segments: List[Segment]
+    log_likelihood: float
+    confidence: float
+
+    @property
+    def text(self) -> str:
+        return " ".join(seg.text for seg in self.segments if seg.text)
+
+    @property
+    def words(self) -> List[Word]:
+        return [word for seg in self.segments for word in (seg.words or [])]
+
+    def __str__(self) -> str:
+        return self.text
+
+    def __len__(self) -> int:
+        return len(self.segments)
+
+    def __iter__(self) -> Iterator[Segment]:
+        return iter(self.segments)
+
+
 class LongformTranscriptionResult(_Record):
     """`transcribe_longform()` result: the segments in recording order."""
     __slots__ = _fields = ("segments",)

@@ -267,6 +267,18 @@ int64_t gam_ctc_align_workspace_bytes(const gam_handle* h, int32_t B, int32_t T,
 int gam_ctc_align(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets, const int32_t* target_len,
                   int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
                   float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream);
+/* gam_ctc_align for recordings of any length: the same arguments, definitions, rules and outputs as gam_ctc_align, and on
+ * every input gam_ctc_align accepts the same bits.  Only these differ:
+ *   - limits: U <= 65536 tokens; T is bounded only by int32 and the workspace (not by max_encoded_frames);
+ *   - one thread-block cluster of C <= 16 CTAs per utterance, C the smallest whose share of the 2U + 1 states (a multiple of
+ *     16) fits in shared memory at 20 bytes per state; frame boundaries are exchanged through distributed shared memory;
+ *   - workspace: B * T * ceil((2U + 1) / 16) * 4 bytes of backpointers (2.95 GB for T = 90 000, U = 65 536), rounded up to
+ *     1 KiB; *_workspace_bytes returns -1 for bad sizes, U > 65536 or a handle without a CTC head.
+ * Stream-ordered, no host synchronisation, capturable in a CUDA graph. */
+int64_t gam_ctc_align_long_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets, const int32_t* target_len,
+                       int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                       float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream);
 /* RNN-T stage 1: enc [B, T, d_model], dec [B, U+1, pred_hidden] (gam_rnnt_predict over cat[blank, y]), targets [B, U] i32
  *   -> blank [B, T, U+1], label [B, T, U+1]: bit-identical to the matching entries of gam_rnnt_joint's lattice for the same
  *   enc / dec, but no [.., V+1] row is ever stored.  label is -inf at u = U and NaN where targets[b, u] is outside [0, V) (so
@@ -430,6 +442,13 @@ int gam_test_rnnt_greedy_scored(gam_handle* h, const float* encproj, const int32
                                 const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
                                 int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts,
                                 float* token_logp, float* path_logp, int32_t* path_rows, int32_t* plan, void* stream);
+/* gam_ctc_align_long with the cluster size forced to cluster_ctas (0: the library's choice), so that CTA boundaries can be
+ * placed with few states; a C that leaves a CTA without states is refused.  plan (host i32 [2], or NULL) receives C and the
+ * states per CTA. */
+int gam_test_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                            const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes,
+                            int32_t* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int32_t* path_rows,
+                            int32_t cluster_ctas, int32_t* plan, void* stream);
 /* qkv: f16 [B*T, 3*d_model]; klen i32 [B] or NULL -> out f16 [B*T, d_model].  T up to the handle's max_encoded_frames */
 int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void* out, int32_t B, int32_t T, void* stream);
 /* rel_pos variant: qkv f16 [B*T, 4*d_model] = [q+u | q+v | k | v]; pos f16 [2*max-1, d_model] laid out like pos_proj
