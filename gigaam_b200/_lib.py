@@ -63,7 +63,9 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_rnnt_predict_backward", "gam_test_gemm_used_slots", "gam_decode_scored_workspace_bytes",
            "gam_ctc_greedy_scored", "gam_rnnt_greedy_scored", "gam_test_rnnt_greedy_scored", "gam_ctc_align_workspace_bytes",
            "gam_ctc_align", "gam_rnnt_align_scores_workspace_bytes", "gam_rnnt_align_scores", "gam_rnnt_align_workspace_bytes",
-           "gam_rnnt_align", "gam_ctc_align_long_workspace_bytes", "gam_ctc_align_long", "gam_test_ctc_align_long")
+           "gam_rnnt_align", "gam_ctc_align_long_workspace_bytes", "gam_ctc_align_long", "gam_test_ctc_align_long",
+           "gam_decode_state_bytes", "gam_decode_state_init", "gam_decode_resume_workspace_bytes", "gam_ctc_greedy_resume",
+           "gam_rnnt_greedy_resume")
 
 
 def lib_path() -> Path:
@@ -119,6 +121,15 @@ def load() -> C.CDLL:
         fn.restype = C.c_int
     for fn in (lib.gam_ctc_greedy_scored, lib.gam_rnnt_greedy_scored):
         fn.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, i64, c_vp, c_vp, c_vp, i32, c_vp, c_vp, c_vp, c_vp]
+        fn.restype = C.c_int
+    lib.gam_decode_state_bytes.argtypes = [H]
+    lib.gam_decode_state_bytes.restype = i64
+    lib.gam_decode_state_init.argtypes = [H, c_vp, i32, c_vp]
+    lib.gam_decode_state_init.restype = C.c_int
+    lib.gam_decode_resume_workspace_bytes.argtypes = [H, i32, i32]
+    lib.gam_decode_resume_workspace_bytes.restype = i64
+    for fn in (lib.gam_ctc_greedy_resume, lib.gam_rnnt_greedy_resume):
+        fn.argtypes = [H, c_vp, i32, i32, c_vp, c_vp, c_vp, c_vp, c_vp, i64, c_vp, c_vp, c_vp, i32] + [c_vp] * 5 + [i64, c_vp]
         fn.restype = C.c_int
     lib.gam_ctc_log_probs.argtypes = [H, c_vp, i32, i32, c_vp, c_vp]
     lib.gam_ctc_log_probs.restype = C.c_int

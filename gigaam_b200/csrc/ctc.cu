@@ -170,7 +170,111 @@ __global__ void __launch_bounds__(128) ctc_collapse_kernel(const int* __restrict
   }
 }
 
+// ctc_collapse_kernel continued across calls (gam_ctc_greedy_resume): utterance b collapses labels [lo, hi) of its row with the
+// previous frame's label taken from its DecodeState, appends at counts[b] and emits frames frame_base[b] + t.  Decoding [0, L) in
+// consecutive ranges gives the one-shot kernel's bits: the collapse rule only looks one frame back, and the scored path sum keeps
+// the one-shot partials -- row r of the stream (r = rows before the call + t - lo) goes to partial r % 32, in ascending r, and
+// the 32 partials meet in the same xor tree.  SCORED also writes frame_logp / frame_rows (one decision row per frame).
+template <bool SCORED>
+__global__ void __launch_bounds__(128) ctc_collapse_resume_kernel(const int* __restrict__ labels, const float* __restrict__ lp,
+                                                                  const int* __restrict__ lo, const int* __restrict__ hi,
+                                                                  const int* __restrict__ frame_base, int B, int T, int blank,
+                                                                  uint8_t* __restrict__ state, int64_t stride, int* __restrict__ ids,
+                                                                  int* __restrict__ frames, int* __restrict__ counts, int max_out,
+                                                                  float* __restrict__ token_logp, float* __restrict__ path_logp,
+                                                                  int* __restrict__ path_rows, double* __restrict__ frame_logp,
+                                                                  int* __restrict__ frame_rows, int64_t frame_pitch) {
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (b >= B) return;
+  const int a = min(max(lo[b], 0), T), e = min(max(hi[b], a), T);
+  if (a == e) return;
+  DecodeState* st = reinterpret_cast<DecodeState*>(state + b * stride);
+  const int* lab = labels + static_cast<size_t>(b) * T;
+  const int fb = frame_base[b], prev0 = st->label, rows0 = st->rows;
+  const int pos0 = counts[b];
+  int pos = pos0;
+  [[maybe_unused]] double part = 0.0;
+  [[maybe_unused]] const int rot = rows0 & 31;   // lane k keeps partial k; row t comes from lane (k - rot) mod 32
+  if constexpr (SCORED) part = st->part[lane];
+  for (int t0 = a; t0 < e; t0 += 32) {
+    const int t = t0 + lane;
+    int l = blank, prev = blank;
+    if (t < e) {
+      l = lab[t];
+      prev = t > a ? lab[t - 1] : prev0;
+    }
+    const bool keep = (t < e) && (l != blank) && (l != prev);
+    const unsigned mask = __ballot_sync(0xffffffffu, keep);
+    const int p = pos + __popc(mask & ((1u << lane) - 1u));
+    [[maybe_unused]] float x = 0.f;
+    if constexpr (SCORED) {
+      if (t < e) {
+        x = lp[static_cast<size_t>(b) * T + t];
+        frame_logp[b * frame_pitch + fb + t] = static_cast<double>(x);
+        frame_rows[b * frame_pitch + fb + t] = 1;
+      }
+    }
+    if (keep && p < max_out) {
+      ids[static_cast<size_t>(b) * max_out + p] = l;
+      frames[static_cast<size_t>(b) * max_out + p] = fb + t;
+      if constexpr (SCORED) token_logp[static_cast<size_t>(b) * max_out + p] = x;
+    }
+    if constexpr (SCORED) {
+      const int src = (lane - rot) & 31;
+      const float xs = __shfl_sync(0xffffffffu, x, src);
+      if (t0 + src < e) part += static_cast<double>(xs);
+    }
+    pos += __popc(mask);
+  }
+  if constexpr (SCORED) {
+    st->part[lane] = part;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+  }
+  if (lane == 0) {
+    counts[b] = min(pos, max_out);
+    st->label = lab[e - 1];
+    st->count += pos - pos0;
+    if constexpr (SCORED) {
+      st->rows = rows0 + (e - a);
+      path_logp[b] = static_cast<float>(part);
+      path_rows[b] = rows0 + (e - a);
+    }
+  }
+}
+
+__global__ void decode_state_init_kernel(uint8_t* state, int64_t stride, int n, int blank) {
+  const int b = blockIdx.x;
+  if (b >= n) return;
+  uint32_t* w = reinterpret_cast<uint32_t*>(state + b * stride);
+  for (int i = threadIdx.x; i < static_cast<int>(stride / 4); i += blockDim.x) w[i] = 0u;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    DecodeState* st = reinterpret_cast<DecodeState*>(state + b * stride);
+    st->label = blank;
+    st->pending = 1;
+  }
+}
+
 }  // namespace
+
+void launch_decode_state_init(uint8_t* state, int64_t stride, int n, int blank, cudaStream_t s) {
+  if (n > 0) decode_state_init_kernel<<<n, 256, 0, s>>>(state, stride, n, blank);
+}
+void launch_ctc_collapse_resume(const int* labels, const float* lp, const int* lo, const int* hi, const int* frame_base, int B, int T,
+                                int blank, uint8_t* state, int64_t stride, int* ids, int* frames, int* counts, int max_out,
+                                float* token_logp, float* path_logp, int* path_rows, double* frame_logp, int* frame_rows,
+                                int64_t frame_pitch, cudaStream_t s) {
+  if (token_logp)
+    ctc_collapse_resume_kernel<true><<<(B + 3) / 4, 128, 0, s>>>(labels, lp, lo, hi, frame_base, B, T, blank, state, stride, ids, frames,
+                                                                 counts, max_out, token_logp, path_logp, path_rows, frame_logp,
+                                                                 frame_rows, frame_pitch);
+  else
+    ctc_collapse_resume_kernel<false><<<(B + 3) / 4, 128, 0, s>>>(labels, lp, lo, hi, frame_base, B, T, blank, state, stride, ids,
+                                                                  frames, counts, max_out, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                                  frame_pitch);
+}
 
 void launch_ctc_argmax(const float* enc, const float* W, const float* bias, int* labels, int R, int D, int V1,
                        cudaStream_t s) {

@@ -741,6 +741,95 @@ static int rnnt_greedy_impl(gam_handle* h, const float* enc, const int32_t* enc_
   return 0;
 }
 
+int64_t gam_decode_state_bytes(const gam_handle* h) {
+  if (h->cfg.head == 1) return kCtcDecodeStateBytes;
+  if (h->cfg.head == 2) return kRnntDecodeStateBytes;
+  return -1;
+}
+
+int gam_decode_state_init(gam_handle* h, void* state, int32_t n, void* stream) {
+  const int64_t bytes = gam_decode_state_bytes(h);
+  if (bytes < 0) return fail(h, -1, "decode_state_init: model has no CTC or RNN-T head");
+  if (n < 0 || (n > 0 && state == nullptr)) return fail(h, -1, "decode_state_init: bad state buffer (n=%d)", n);
+  launch_decode_state_init(static_cast<uint8_t*>(state), bytes, n, h->cfg.num_classes - 1, static_cast<cudaStream_t>(stream));
+  GAM_CHECK_LAUNCH(h, "decode_state_init");
+  return 0;
+}
+
+int64_t gam_decode_resume_workspace_bytes(const gam_handle* h, int32_t B, int32_t T) {
+  return gam_decode_scored_workspace_bytes(h, B, T);
+}
+
+// shared argument checks of gam_*_greedy_resume
+static int resume_args(gam_handle* h, const char* what, int head, const float* enc, int32_t B, int32_t T, const int32_t* lo,
+                       const int32_t* hi, const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes,
+                       int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp,
+                       int32_t* path_rows, double* frame_logp, int32_t* frame_rows, int64_t frame_pitch) {
+  if (h->cfg.head != head) return fail(h, -1, "%s: model has no %s head", what, head == 1 ? "CTC" : "RNN-T");
+  if (B < 1 || T < 1 || static_cast<int64_t>(B) * T > INT32_MAX) return fail(h, -1, "%s: bad sizes (B=%d, T=%d)", what, B, T);
+  if (max_out < 1) return fail(h, -1, "%s: max_out (%d) must be >= 1", what, max_out);
+  if (!enc || !lo || !hi || !frame_base || !state || !ids || !frames || !counts)
+    return fail(h, -1, "%s: enc, lo, hi, frame_base, state, ids, frames and counts are required", what);
+  if (token_logp && (!path_logp || !path_rows || !frame_logp || !frame_rows || frame_pitch < 1))
+    return fail(h, -1, "%s: a scored call needs path_logp, path_rows, frame_logp, frame_rows and frame_pitch >= 1", what);
+  const int64_t need = gam_decode_resume_workspace_bytes(h, B, T);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "%s: workspace too small: need %lld bytes, got %lld", what, (long long)need, (long long)workspace_bytes);
+  return 0;
+}
+
+int gam_ctc_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
+                          const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes, int32_t* ids,
+                          int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
+                          double* frame_logp, int32_t* frame_rows, int64_t frame_pitch, void* stream) {
+  if (resume_args(h, "ctc_greedy_resume", 1, enc, B, T, lo, hi, frame_base, state, workspace, workspace_bytes, ids, frames, counts,
+                  max_out, token_logp, path_logp, path_rows, frame_logp, frame_rows, frame_pitch) != 0)
+    return -1;
+  const gam_config& c = h->cfg;
+  const int64_t R = static_cast<int64_t>(B) * T;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // the ranges live on the device, so every row is labelled; each row's label and l do not depend on the others
+  int* labels = static_cast<int*>(workspace);
+  float* lp = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + align_up(R * 4, 1024));
+  { PROF(PC_CTC_ARGMAX);
+    if (token_logp) launch_ctc_argmax_scored(enc, h->w.ctc_w, h->w.ctc_b, labels, lp, static_cast<int>(R), c.d_model, c.num_classes, s);
+    else launch_ctc_argmax(enc, h->w.ctc_w, h->w.ctc_b, labels, static_cast<int>(R), c.d_model, c.num_classes, s); }
+  { PROF(PC_CTC_COLLAPSE);
+    launch_ctc_collapse_resume(labels, lp, lo, hi, frame_base, B, T, c.num_classes - 1, static_cast<uint8_t*>(state),
+                               kCtcDecodeStateBytes, ids, frames, counts, max_out, token_logp, path_logp, path_rows, frame_logp,
+                               frame_rows, frame_pitch, s); }
+  GAM_CHECK_LAUNCH(h, "ctc_greedy_resume");
+  return 0;
+}
+
+int gam_rnnt_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
+                           const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes, int32_t* ids,
+                           int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
+                           double* frame_logp, int32_t* frame_rows, int64_t frame_pitch, void* stream) {
+  if (resume_args(h, "rnnt_greedy_resume", 2, enc, B, T, lo, hi, frame_base, state, workspace, workspace_bytes, ids, frames, counts,
+                  max_out, token_logp, path_logp, path_rows, frame_logp, frame_rows, frame_pitch) != 0)
+    return -1;
+  const gam_config& c = h->cfg;
+  if (c.pred_hidden != c.joint_hidden) return fail(h, -1, "pred_hidden != joint_hidden is not supported");
+  const int64_t R = static_cast<int64_t>(B) * T;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  float* encproj = static_cast<float*>(workspace);
+  { PROF(PC_RNNT_ENCPROJ);   // every row, as gam_rnnt_greedy: a row's projection does not depend on the others
+    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, encproj, static_cast<int>(R), c.joint_hidden, c.d_model, s); }
+  PROF(PC_RNNT_GREEDY);
+  const int rc = launch_rnnt_greedy_resume(encproj, lo, hi, frame_base, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h->w.rnnt_wp_t,
+                                           h->w.rnnt_bp, h->w.rnnt_wo, h->w.rnnt_bo, B, T, c.pred_hidden, c.num_classes,
+                                           c.num_classes - 1, c.max_symbols, max_out, static_cast<uint8_t*>(state),
+                                           kRnntDecodeStateBytes, ids, frames, counts, token_logp, path_logp, path_rows, frame_logp,
+                                           frame_rows, frame_pitch, s);
+  if (rc > 0)
+    return fail(h, -1, "rnnt: the greedy kernel is specialised for pred_hidden = joint_hidden = 320 and needs 16-CTA clusters "
+                "(pred_hidden %d)", c.pred_hidden);
+  if (rc < 0) return fail(h, -4, "rnnt cluster kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, "rnnt_greedy_resume");
+  return 0;
+}
+
 int gam_ctc_log_probs(gam_handle* h, const float* enc, int32_t B, int32_t T, float* log_probs, void* stream) {
   const gam_config& c = h->cfg;
   if (c.head != 1) return fail(h, -1, "ctc_log_probs: model has no CTC head");

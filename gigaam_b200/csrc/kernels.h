@@ -3,6 +3,7 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace gam {
@@ -61,6 +62,29 @@ void launch_ctc_argmax_scored(const float* enc, const float* W, const float* bia
                               cudaStream_t s);
 void launch_ctc_collapse_scored(const int* labels, const float* lp, const int* len, int B, int T, int blank, int* ids, int* frames,
                                 int* counts, float* token_logp, float* path_logp, int* path_rows, cudaStream_t s);
+
+// Resumable greedy decoding (gam_*_greedy_resume): what the greedy loop keeps across a frame boundary, one record per decoding
+// stream.  CTC uses the record up to `h`; RNN-T all of it.  A fresh utterance is label = blank, pending = 1, zeros elsewhere.
+constexpr int kDecodeStateH = 320;
+struct alignas(16) DecodeState {
+  int label;        // CTC: the previous frame's label; RNN-T: the last label fed to the prediction network
+  int pending;      // RNN-T: that label's LSTM step has not run yet
+  int count;        // tokens emitted so far (the true count: not capped by max_out)
+  int rows;         // decision rows so far (scored calls)
+  double path;      // RNN-T: fp64 sum of l over those rows (warp 0's running sum)
+  double pad;       // keeps the CTC record (up to h) a multiple of 16 bytes
+  double part[32];  // CTC: the fp64 partial sums of the scored collapse, partial k over the rows r with r % 32 == k
+  float h[kDecodeStateH], c[kDecodeStateH], pg[kDecodeStateH];   // RNN-T: LSTM state and W_p h + b_p
+};
+constexpr int64_t kCtcDecodeStateBytes = static_cast<int64_t>(offsetof(DecodeState, h));
+constexpr int64_t kRnntDecodeStateBytes = static_cast<int64_t>(sizeof(DecodeState));
+static_assert(kCtcDecodeStateBytes % 16 == 0, "state records stay 16-byte aligned");
+void launch_decode_state_init(uint8_t* state, int64_t stride, int n, int blank, cudaStream_t s);
+// CTC collapse of labels[b, lo[b] .. hi[b]) continuing the stream at state + b * stride (lp / token_logp null: unscored)
+void launch_ctc_collapse_resume(const int* labels, const float* lp, const int* lo, const int* hi, const int* frame_base, int B, int T,
+                                int blank, uint8_t* state, int64_t stride, int* ids, int* frames, int* counts, int max_out,
+                                float* token_logp, float* path_logp, int* path_rows, double* frame_logp, int* frame_rows,
+                                int64_t frame_pitch, cudaStream_t s);
 
 // words.cu: (token id, frame) pairs -> word records (first frame, last frame + 1, first token, tokens) per utterance
 void launch_group_words(const int* ids, const int* frames, const int* counts, const unsigned char* flags, int B, int V, int max_out,
@@ -154,6 +178,14 @@ int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float
                                const float* bp, const float* wo, const float* bo, int B, int T, int H, int V1, int blank,
                                int max_symbols, int max_out, int* ids, int* frames, int* counts, float* token_logp,
                                float* path_logp, int* path_rows, int* plan, cudaStream_t s);
+// the same kernel resuming stream b (DecodeState at state + b * stride) over frames [lo[b], hi[b]) of encproj row b; frames are
+// emitted as frame_base[b] + t and tokens appended at counts[b].  token_logp set: scored, and frame_logp / frame_rows
+// [b * frame_pitch + frame_base[b] + t] receive each frame's sum of l and its decision rows.  Returns as above.
+int launch_rnnt_greedy_resume(const float* encproj, const int* lo, const int* hi, const int* frame_base, const float* emb_gates,
+                              const float* whhT, const float* wpT, const float* bp, const float* wo, const float* bo, int B, int T,
+                              int H, int V1, int blank, int max_symbols, int max_out, uint8_t* state, int64_t stride, int* ids,
+                              int* frames, int* counts, float* token_logp, float* path_logp, int* path_rows, double* frame_logp,
+                              int* frame_rows, int64_t frame_pitch, cudaStream_t s);
 
 // gemm.cu
 struct GemmParams;

@@ -10,13 +10,26 @@ import hashlib
 import json
 import math
 import os
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 
 from . import _lib
 
 Tensor = torch.Tensor
+
+
+class DecodeBuffers(NamedTuple):
+    """Outputs that Engine.greedy_resume appends to across calls (Engine.decode_buffers); the score fields are None for
+    unscored decoding."""
+    ids: Tensor
+    frames: Tensor
+    counts: Tensor
+    token_logp: Optional[Tensor] = None
+    path_logp: Optional[Tensor] = None
+    path_rows: Optional[Tensor] = None
+    frame_logp: Optional[Tensor] = None
+    frame_rows: Optional[Tensor] = None
 
 
 def _cfg_get(section, key, default=None):
@@ -556,6 +569,54 @@ class Engine:
                     frames.data_ptr(), counts.data_ptr(), max_out, self._stream())
         _lib.check(self.lib, self.handle, rc, "gam_greedy")
         return ids, frames, counts
+
+    # ------------------------------------------------------------------ resumable greedy decoding (gam_*_greedy_resume)
+    def decode_state(self, n: int = 1) -> Tensor:
+        """n fresh decoding streams (gam_decode_state_init): uint8 [n, gam_decode_state_bytes] on the device."""
+        nbytes = int(self.lib.gam_decode_state_bytes(self.handle))
+        if nbytes < 0:
+            raise RuntimeError("model has no head to decode with")
+        state = torch.empty((n, nbytes), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_decode_state_init(self.handle, state.data_ptr(), n, self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_decode_state_init")
+        return state
+
+    def decode_buffers(self, B: int, max_out: int, n_frames: int = 0, scores: bool = False) -> "DecodeBuffers":
+        """The outputs greedy_resume appends to, for B streams: ids / frames [B, max_out], counts [B] = 0 and, with `scores`,
+        token_logp [B, max_out], the running path_logp / path_rows [B] and frame_logp (f64) / frame_rows [B, n_frames] = 0."""
+        i32 = dict(dtype=torch.int32, device=self.device)
+        out = DecodeBuffers(torch.empty((B, max_out), **i32), torch.empty((B, max_out), **i32), torch.zeros((B,), **i32))
+        if not scores:
+            return out
+        return out._replace(token_logp=torch.empty((B, max_out), dtype=torch.float32, device=self.device),
+                            path_logp=torch.zeros((B,), dtype=torch.float32, device=self.device), path_rows=torch.zeros((B,), **i32),
+                            frame_logp=torch.zeros((B, n_frames), dtype=torch.float64, device=self.device),
+                            frame_rows=torch.zeros((B, n_frames), **i32))
+
+    def greedy_resume(self, enc_btd: Tensor, lo: Tensor, hi: Tensor, frame_base: Tensor, state: Tensor, out: "DecodeBuffers",
+                      scores: bool = False) -> None:
+        """Decode frames [lo[b], hi[b]) of enc [B, T, d] (f32 contiguous) continuing stream b of `state` (decode_state) and
+        append to `out` (decode_buffers, emitted frames frame_base[b] + t).  lo / hi / frame_base: device int32 [B].  Decoding
+        an utterance in consecutive ranges gives `greedy`'s bits (include/gigaam_b200.h, gam_ctc_greedy_resume)."""
+        assert enc_btd.is_cuda and enc_btd.dtype == torch.float32 and enc_btd.is_contiguous() and enc_btd.dim() == 3
+        B, T, _ = enc_btd.shape
+        for t in (lo, hi, frame_base):
+            assert t.device == self.device and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == B
+        assert state.dtype == torch.uint8 and state.is_contiguous() and state.shape[0] >= B
+        assert state.shape[1] == int(self.lib.gam_decode_state_bytes(self.handle))
+        assert out.ids.shape[0] >= B and out.ids.is_contiguous() and out.frames.is_contiguous()
+        if scores and out.token_logp is None:
+            raise ValueError("greedy_resume: scores need buffers from decode_buffers(..., scores=True)")
+        ws = self._ws_dec.get(("resume", B, T), int(self.lib.gam_decode_resume_workspace_bytes(self.handle, B, T)), self.device)
+        fn = self.lib.gam_ctc_greedy_resume if self.head_type == 1 else self.lib.gam_rnnt_greedy_resume
+        sc = [out.token_logp, out.path_logp, out.path_rows, out.frame_logp, out.frame_rows] if scores else [None] * 5
+        pitch = out.frame_logp.shape[1] if scores else 0
+        with torch.cuda.device(self.device):
+            rc = fn(self.handle, enc_btd.data_ptr(), B, T, lo.data_ptr(), hi.data_ptr(), frame_base.data_ptr(), state.data_ptr(),
+                    ws.data_ptr(), ws.numel(), out.ids.data_ptr(), out.frames.data_ptr(), out.counts.data_ptr(), out.ids.shape[1],
+                    *[None if t is None else t.data_ptr() for t in sc], pitch, self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_greedy_resume")
 
     def ctc_log_probs(self, enc_btd: Tensor) -> Tensor:
         """enc [B, T, d] f32 contiguous -> log_probs [B, T, V+1] f32 (CTCHead.forward, gigaam/decoder.py:18-21)."""

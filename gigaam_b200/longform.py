@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import bisect
 import math
-from typing import Callable, List, NamedTuple, Optional, Sequence, Tuple
+from typing import Callable, Iterator, List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 from torch import Tensor
@@ -143,7 +143,7 @@ def plan_windows(n_samples: int, window_s: float, overlap_s: float, length_fn: C
     40 ms, an overlap < 0 or >= the window, or a window of more than `max_frames` encoder frames."""
     n = int(n_samples)
     if n <= 0:
-        raise ValueError("align_longform: empty recording")
+        raise ValueError("empty recording")
     W = _frame_multiple(window_s, "window")
     V = _frame_multiple(overlap_s, "overlap")
     if W <= 0:
@@ -155,39 +155,123 @@ def plan_windows(n_samples: int, window_s: float, overlap_s: float, length_fn: C
                          f"{max_frames}")
     T = int(length_fn(n))
     if T <= 0:
-        raise ValueError(f"align_longform: {n} samples encode to no frame")
+        raise ValueError(f"{n} samples encode to no frame")
     H = W - V
     count = 1 if n <= W else 1 + -(-(n - W) // H)
     cuts = [0] + [w * H // FRAME_SAMPLES + V // FRAME_SAMPLES // 2 for w in range(1, count)] + [T]
     return [Window(w * H, min(w * H + W, n), cuts[w], cuts[w + 1]) for w in range(count)], T
 
 
-def stitch_ctc_log_probs(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16) -> Tensor:
-    """CTC log-probs [1, T, V+1] f32 of a whole recording (wav [N] on the model's device, already in the model's dtype):
-    the windows are encoded through `model.forward` (the varlen path) in batches of up to `batch_size` windows of one
-    length, `model.head` (gam_ctc_log_probs) gives each batch's log-probs, and each window's kept rows are copied into
-    place.  Only one batch of window log-probs is alive at a time."""
+def window_batches(model, wav: Tensor, windows: Sequence[Window], batch_size: int) -> Iterator[Tuple[List[Window], Tensor]]:
+    """Encode the windows of `wav` ([N], already in the model's dtype, on the model's device or in pinned host memory) in
+    window order through `model.forward` (the varlen path), in batches of up to `batch_size` windows of one length: no
+    padding, so no row depends on its neighbours.  Windows that keep no frame are skipped.  A host waveform is uploaded one
+    batch at a time.  Yields (the batch's windows, encoded [nb, d, T_w])."""
     if batch_size < 1:
         raise ValueError("batch_size must be >= 1")
-    eng = model._get_engine()
-    out = torch.empty((1, T, eng.num_classes), dtype=torch.float32, device=eng.device)
-    todo = [w for w in windows if w.keep_end > w.keep_start]
+    dev = model._device
     groups: List[List[Window]] = []
-    for w in todo:   # windows of one length share a batch: no padding, so no row depends on its neighbours
+    for w in windows:
+        if w.keep_end <= w.keep_start:
+            continue
         if groups and len(groups[-1]) < batch_size and groups[-1][0].end - groups[-1][0].start == w.end - w.start:
             groups[-1].append(w)
         else:
             groups.append([w])
     for group in groups:
         length = group[0].end - group[0].start
-        batch = torch.stack([wav[w.start:w.end] for w in group])
-        lens = torch.full((len(group),), length, dtype=torch.int64, device=wav.device)
+        if wav.device == dev:
+            batch = torch.stack([wav[w.start:w.end] for w in group])
+        else:
+            staged = torch.empty((len(group), length), dtype=wav.dtype, pin_memory=True)
+            torch.stack([wav[w.start:w.end] for w in group], out=staged)
+            batch = staged.to(dev, non_blocking=True)
+        lens = torch.full((len(group),), length, dtype=torch.int64, device=dev)
         encoded, _ = model.forward(batch, lens)
+        yield group, encoded
+
+
+def stitch_ctc_log_probs(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16) -> Tensor:
+    """CTC log-probs [1, T, V+1] f32 of a whole recording (wav [N] on the model's device, already in the model's dtype):
+    the windows are encoded by `window_batches`, `model.head` (gam_ctc_log_probs) gives each batch's log-probs, and each
+    window's kept rows are copied into place.  Only one batch of window log-probs is alive at a time."""
+    eng = model._get_engine()
+    out = torch.empty((1, T, eng.num_classes), dtype=torch.float32, device=eng.device)
+    for group, encoded in window_batches(model, wav, windows, batch_size):
         lp = model.head(encoded)
         for row, w in enumerate(group):
             first = w.start // FRAME_SAMPLES
             out[0, w.keep_start:w.keep_end] = lp[row, w.keep_start - first:w.keep_end - first]
         del lp, encoded
+    return out
+
+
+def decode_windows(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16, scores: bool = False):
+    """Greedy-decode a whole recording of T encoder frames as one utterance: `window_batches` encodes the windows, and each
+    window's kept frames are decoded in window order, resuming the previous window's decoder state on the device
+    (Engine.greedy_resume).  Only one batch of encoder output is alive at a time.  Returns the Engine.DecodeBuffers of the
+    one stream: ids / frames [1, max_out] (global frames), counts [1] and, with `scores`, token_logp, path_logp, path_rows and
+    the per-frame frame_logp / frame_rows [1, T].  max_out = Engine.hyp_width(T), so the buffers never overflow."""
+    from .decoding import _as_btd
+    eng = model._get_engine()
+    index = {w: i for i, w in enumerate(windows)}
+    first = [w.start // FRAME_SAMPLES for w in windows]
+    ranges = torch.tensor([[w.keep_start - f for w, f in zip(windows, first)], [w.keep_end - f for w, f in zip(windows, first)], first],
+                          dtype=torch.int32).to(eng.device)
+    state = eng.decode_state(1)
+    out = eng.decode_buffers(1, eng.hyp_width(T), T, scores=scores)
+    for group, encoded in window_batches(model, wav, windows, batch_size):
+        enc = _as_btd(encoded)
+        for row, w in enumerate(group):
+            i = index[w]
+            eng.greedy_resume(enc[row:row + 1], ranges[0, i:i + 1], ranges[1, i:i + 1], ranges[2, i:i + 1], state, out, scores)
+        del enc, encoded
+    return out
+
+
+def segment_cuts(word_spans: Sequence[Tuple[int, int]], T: int, frame_shift: float, pause: float, max_segment: float) -> List[int]:
+    """Segment boundaries of a transcribed recording of T frames, from its words' frame spans [start, end) in order:
+    [c_0 = 0, c_1, ..., c_n = T], segment k covering frames [c_k, c_{k+1}).  Cuts fall only between consecutive words whose
+    spans do not overlap, at the gap's middle frame (end_prev + start_next) // 2: first at every gap of at least `pause`
+    seconds, then, while a segment lasts more than `max_segment` seconds, at the middle of its longest inner gap (the first
+    of equal ones), until it fits or has no such gap left."""
+    starts = [s for s, _ in word_spans]
+    gaps = [(e, s) for (_, e), (s, _) in zip(word_spans, word_spans[1:])]     # gap i: between word i and word i + 1
+    cuts = [0] + [(e + s) // 2 for e, s in gaps if s >= e and (s - e) * frame_shift >= pause] + [T]
+    out = [0]
+    todo = list(zip(cuts, cuts[1:]))[::-1]
+    while todo:
+        a, b = todo.pop()
+        if (b - a) * frame_shift > max_segment:
+            i0, i1 = bisect.bisect_left(starts, a), bisect.bisect_left(starts, b)     # the words of [a, b)
+            inner = [(gaps[i][1] - gaps[i][0], i) for i in range(i0, i1 - 1) if gaps[i][1] >= gaps[i][0]]
+            if inner:
+                e, s = gaps[max(inner, key=lambda g: g[0])[1]]    # max keeps the first of equal gaps
+                mid = (e + s) // 2                               # a < e <= mid <= s < b
+                todo.extend([(mid, b), (a, mid)])
+                continue
+        out.append(b)
+    return out
+
+
+def windowed_segments(tokenizer, ids: Sequence[int], frames: Sequence[int], cuts: Sequence[int], frame_shift: float, duration: float,
+                      words: Optional[Sequence[Word]], word_starts: Sequence[int], frame_logp=None, frame_rows=None) -> List[Segment]:
+    """One Segment per range [cuts[k], cuts[k+1]) of `segment_cuts`: the tokens whose frames fall inside it (text =
+    tokenizer.decode of them), the words that start inside it (None when `words` is None), start / end = the cut frames
+    times the frame shift (the last segment ends at `duration`) and, when frame_logp / frame_rows (per-frame sums of l and
+    decision rows) are given, confidence = exp(sum of l over its frames / their rows), NaN without rows."""
+    from .timestamps_utils import path_confidence
+    out: List[Segment] = []
+    n = len(cuts) - 1
+    for k in range(n):
+        a, b = cuts[k], cuts[k + 1]
+        t0, t1 = bisect.bisect_left(frames, a), bisect.bisect_left(frames, b)
+        w0, w1 = bisect.bisect_left(word_starts, a), bisect.bisect_left(word_starts, b)
+        conf = None
+        if frame_logp is not None:
+            conf = path_confidence(float(frame_logp[a:b].sum()), int(frame_rows[a:b].sum()))
+        out.append(Segment(text=tokenizer.decode(list(ids[t0:t1])), start=a * frame_shift, end=duration if k == n - 1 else b * frame_shift,
+                           words=None if words is None else list(words[w0:w1]), confidence=conf))
     return out
 
 

@@ -427,6 +427,50 @@ class GigaAMASR(GigaAM):
         return LongformAlignment(segments=segs, log_likelihood=ll, confidence=path_confidence(vit, int(path_rows[0])))
 
     @torch.inference_mode()
+    def transcribe_windowed(self, wav_file, word_timestamps: bool = False, confidence: bool = False, window: float = 30.0,
+                            overlap: float = 4.0, batch_size: int = 16, pause: float = 1.0, max_segment: float = 25.0):
+        """Transcribe a recording of any length without a VAD (INTEGRATION.md §7f).  The encoder runs over overlapping
+        windows (`longform.plan_windows`), and the greedy decoder runs over the windows' kept frames as ONE utterance: each
+        window is decoded as soon as its batch is encoded, resuming the decoder state of the window before it
+        (gam_*_greedy_resume), so no cut falls inside a word and device memory does not grow with the recording.  Segments
+        are cut afterwards between words (`longform.segment_cuts`: at pauses of at least `pause` seconds, then inside
+        segments longer than `max_segment` seconds).  Returns a LongformTranscriptionResult whose segments tile the
+        recording.  Raises ValueError before any device work for the window plan's refusals, batch_size < 1, pause < 0 and
+        max_segment <= 0."""
+        from .longform import decode_windows, plan_windows, segment_cuts, windowed_segments
+        from .timestamps_utils import compute_frame_shift, words_from_device
+        from .types import LongformTranscriptionResult
+        if isinstance(wav_file, str):
+            wav = load_audio(wav_file)
+        else:
+            wav = torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1)
+        if batch_size < 1:
+            raise ValueError("batch_size must be >= 1")
+        if not pause >= 0:
+            raise ValueError(f"pause={pause} s must be >= 0")
+        if not max_segment > 0:
+            raise ValueError(f"max_segment={max_segment} s must be positive")
+        max_frames = self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
+        windows, T = plan_windows(wav.numel(), window, overlap, self._encoded_length, max_frames)
+        N = wav.numel()
+        host = wav.to(self._dtype).pin_memory()          # the rounding of prepare_wav; uploaded one batch at a time
+        eng = self._get_engine()
+        out = decode_windows(self, host, windows, T, batch_size, confidence)
+        rec = eng.group_words(out.ids, out.frames, out.counts, self._word_flags())
+        n = int(out.counts[0])
+        ids, frames = out.ids[0, :n].tolist(), out.frames[0, :n].tolist()
+        ws, we, wf, wn, k = (t[0].cpu().tolist() for t in rec)
+        shift = compute_frame_shift(N, T)
+        logp = out.token_logp[0, :n].tolist() if confidence else None
+        words = words_from_device(self.decoding.tokenizer, ids, ws[:k], we[:k], wf[:k], wn[:k], shift, logp)
+        cuts = segment_cuts(list(zip(ws[:k], we[:k])), T, shift, pause, max_segment)
+        frame_logp = out.frame_logp[0].cpu().numpy() if confidence else None
+        frame_rows = out.frame_rows[0].cpu().numpy() if confidence else None
+        segs = windowed_segments(self.decoding.tokenizer, ids, frames, cuts, shift, N / SAMPLE_RATE,
+                                 words if word_timestamps else None, ws[:k], frame_logp, frame_rows)
+        return LongformTranscriptionResult(segments=segs)
+
+    @torch.inference_mode()
     def transcribe_batch(self, wav: Tensor, lengths: Tensor) -> List[str]:
         """Batched entry (the path eval.py / transcribe_longform drive: model(wav, len) -> decoding.decode)."""
         encoded, encoded_len = self.forward(wav, lengths)

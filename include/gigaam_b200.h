@@ -199,6 +199,42 @@ int gam_rnnt_greedy_scored(gam_handle* h, const float* enc, const int32_t* enc_l
                            int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
                            float* token_logp, float* path_logp, int32_t* path_rows, void* stream);
 
+/* Resumable greedy decoding: decode an utterance in consecutive chunks of frames, with the decoder's state carried in device
+ * memory between calls, so that a recording of any length is decoded as one utterance while only a chunk of encoder output
+ * is alive (GigaAMASR.transcribe_windowed).
+ *
+ * A decoding stream's state is one record of gam_decode_state_bytes(h) bytes: everything the greedy loop keeps across a
+ * frame boundary.  RNN-T: h, c, W_p h + b_p, the last label, whether that label's LSTM step is still pending (a frame that
+ * ended on its max_symbols-th emission), the token count and, when scored, the fp64 path sum and row count.  CTC: the
+ * previous frame's label (a repeat across a chunk edge collapses), the token count, the fp64 partial path sums and the row
+ * count.  gam_decode_state_init writes n fresh records (a new utterance) back to back at `state`.
+ *
+ * One call: row b decodes local frames [lo[b], hi[b]) (clamped to [0, T]) of enc[b] (device f32 [B, T, d_model], gam_encode's
+ * layout), continuing stream b from state + b * gam_decode_state_bytes(h) and leaving the updated record there.  lo, hi and
+ * frame_base are device i32 [B].
+ *   ids / frames  device i32 [B, max_out]: tokens are appended at counts[b] (device i32 [B], read and written); frames are
+ *                 frame_base[b] + t.  Tokens past max_out are dropped, counts[b] stops at max_out and the record keeps the
+ *                 true count, so an overflow can be detected.
+ *   token_logp    device f32 [B, max_out], or NULL for the unscored decoder, which writes none of the outputs below.
+ *   path_logp / path_rows  device f32 / i32 [B]: the stream's running totals (gam_*_greedy_scored's definitions).
+ *   frame_logp / frame_rows  device f64 / i32 [B, frame_pitch]: at frame_base[b] + t, the sum of l over the decision rows of
+ *                 that frame and their number (CTC: one row per frame).
+ * lo[b] == hi[b] leaves row b's record and outputs untouched.  Splitting [0, L) into consecutive ranges and decoding them in
+ * order gives ids, frames, counts, token_logp, path_logp and path_rows bit-identical to one gam_*_greedy(_scored) call over
+ * the same L frames, and frame_rows sums to path_rows.  Every row of enc is labelled / projected (the ranges live on the
+ * device); workspace: gam_decode_resume_workspace_bytes.  Stream-ordered, no host sync, capturable in a CUDA graph. */
+int64_t gam_decode_state_bytes(const gam_handle* h);
+int gam_decode_state_init(gam_handle* h, void* state, int32_t n, void* stream);
+int64_t gam_decode_resume_workspace_bytes(const gam_handle* h, int32_t B, int32_t T);
+int gam_ctc_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
+                          const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes, int32_t* ids,
+                          int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
+                          double* frame_logp, int32_t* frame_rows, int64_t frame_pitch, void* stream);
+int gam_rnnt_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
+                           const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes, int32_t* ids,
+                           int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
+                           double* frame_logp, int32_t* frame_rows, int64_t frame_pitch, void* stream);
+
 /* ---- the heads' forward passes, for callers that run their own search (LM beam search, N-best rescoring, forced
  * alignment, lattice scoring).  fp32 CUDA-core arithmetic like the reference's heads; no workspace except for the joint.
  *
