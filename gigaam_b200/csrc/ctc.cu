@@ -3,10 +3,10 @@
 //       argmax-invariant on finite rows so it is never computed.  The label is torch's log_softmax(row).argmax(-1):
 //       on a row whose maximum is finite the first maximal index (torch.argmax); if any logit is NaN or +inf, or none
 //       exceeds -inf, 0 (log_softmax makes such a row all NaN).  Always in [0, V1).
-//   (2) collapse: keep (l != blank) && (t == 0 || l != l_{t-1}) && (t < len); one warp per utterance,
-//       ballot + popc prefix compaction, results resident on device:
-//       ids[B,T], frames[B,T], counts[B] (int32).
-//   Scored variants (gam_ctc_greedy_scored): the argmax also keeps, per class group, the running sum of exp(z_c - best)
+//   (2) collapse: keep (l != blank) && (l != l_{t-1}) && (t < len); one warp per utterance, ballot + popc prefix
+//       compaction, results resident on device: ids, frames, counts (int32).  One kernel serves the one-shot calls (a
+//       fresh stream) and gam_ctc_greedy_resume (a stream continued from its DecodeState).
+//   Scored (gam_ctc_greedy_scored, scored resume): the argmax also keeps, per class group, the running sum of exp(z_c - best)
 //   beside its (best value, index), rescaled whenever the best moves; the groups merge in the same shared-memory merge and
 //   the frame's l = log_softmax(row)[label] = -log sum_c exp(z_c - z_max) goes to scratch (NaN on a row whose label is
 //   0 by the non-finite rule).  The logits are the same fp32 sums in the same k order, so the labels are the unscored
@@ -122,81 +122,31 @@ __global__ void __launch_bounds__(kRows * kGroups) ctc_argmax_kernel(const float
   }
 }
 
-// SCORED: token_logp[b, pos] = lp of the kept frame, path_logp[b] = sum of lp over t < len (fp64, fixed order),
-// path_rows[b] = len
+// Greedy collapse of one utterance per warp (GreedyIo): keep (l != blank) && (l != prev) over frames [a, e), ballot + popc
+// prefix compaction, appending at pos0.  A fresh call starts at a = 0 with prev = blank, pos0 = 0 and zero partials; a resume
+// call takes prev, the rows so far and the partials from the stream's DecodeState.  The fresh rule keeps the tokens of the
+// one-frame-back rule (t == 0 || l != l_{t-1}): at t = 0 a kept label is not the blank, so it differs from prev = blank.
+// SCORED: token_logp = lp of the kept frame, and the path sum is taken in fp64 in an order fixed by the stream's row index
+// r alone -- row r goes to lane partial r % 32 in ascending r (rot = 0 on a fresh call), and the 32 partials meet in one xor
+// tree -- so decoding [0, L) in consecutive calls gives a fresh call's bits and scores do not depend on the batch.
 template <bool SCORED>
-__global__ void __launch_bounds__(128) ctc_collapse_kernel(const int* __restrict__ labels, const int* __restrict__ len, int B,
-                                                           int T, int blank, int* __restrict__ ids, int* __restrict__ frames,
-                                                           int* __restrict__ counts, const float* __restrict__ lp,
-                                                           float* __restrict__ token_logp, float* __restrict__ path_logp,
-                                                           int* __restrict__ path_rows) {
+__global__ void __launch_bounds__(128) ctc_collapse_kernel(const int* __restrict__ labels, const float* __restrict__ lp, int B, int T,
+                                                           int blank, const GreedyIo io) {
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (b >= B) return;
-  const int L = min(max(len[b], 0), T);
+  DecodeState* st = io.state ? reinterpret_cast<DecodeState*>(io.state + b * io.stride) : nullptr;
+  const int a = st ? min(max(io.lo[b], 0), T) : 0, e = min(max(io.hi[b], a), T);
+  if (st && a == e) return;   // a resume call leaves a stream without frames as it is
   const int* lab = labels + static_cast<size_t>(b) * T;
-  int base = 0;
-  [[maybe_unused]] double path = 0.0;
-  for (int t0 = 0; t0 < T; t0 += 32) {
-    const int t = t0 + lane;
-    int l = blank, prev = -1;
-    if (t < T) {
-      l = lab[t];
-      prev = t > 0 ? lab[t - 1] : -1;
-    }
-    const bool keep = (t < L) && (l != blank) && (t == 0 || l != prev);
-    const unsigned mask = __ballot_sync(0xffffffffu, keep);
-    if (keep) {
-      const int pos = base + __popc(mask & ((1u << lane) - 1u));
-      ids[static_cast<size_t>(b) * T + pos] = l;
-      frames[static_cast<size_t>(b) * T + pos] = t;
-      if constexpr (SCORED) token_logp[static_cast<size_t>(b) * T + pos] = lp[static_cast<size_t>(b) * T + t];
-    }
-    if constexpr (SCORED) {
-      if (t < L) path += static_cast<double>(lp[static_cast<size_t>(b) * T + t]);
-    }
-    base += __popc(mask);
-  }
-  if constexpr (SCORED) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) path += __shfl_xor_sync(0xffffffffu, path, o);
-  }
-  if (lane == 0) {
-    counts[b] = base;
-    if constexpr (SCORED) {
-      path_logp[b] = static_cast<float>(path);
-      path_rows[b] = L;
-    }
-  }
-}
-
-// ctc_collapse_kernel continued across calls (gam_ctc_greedy_resume): utterance b collapses labels [lo, hi) of its row with the
-// previous frame's label taken from its DecodeState, appends at counts[b] and emits frames frame_base[b] + t.  Decoding [0, L) in
-// consecutive ranges gives the one-shot kernel's bits: the collapse rule only looks one frame back, and the scored path sum keeps
-// the one-shot partials -- row r of the stream (r = rows before the call + t - lo) goes to partial r % 32, in ascending r, and
-// the 32 partials meet in the same xor tree.  SCORED also writes frame_logp / frame_rows (one decision row per frame).
-template <bool SCORED>
-__global__ void __launch_bounds__(128) ctc_collapse_resume_kernel(const int* __restrict__ labels, const float* __restrict__ lp,
-                                                                  const int* __restrict__ lo, const int* __restrict__ hi,
-                                                                  const int* __restrict__ frame_base, int B, int T, int blank,
-                                                                  uint8_t* __restrict__ state, int64_t stride, int* __restrict__ ids,
-                                                                  int* __restrict__ frames, int* __restrict__ counts, int max_out,
-                                                                  float* __restrict__ token_logp, float* __restrict__ path_logp,
-                                                                  int* __restrict__ path_rows, double* __restrict__ frame_logp,
-                                                                  int* __restrict__ frame_rows, int64_t frame_pitch) {
-  const int lane = threadIdx.x & 31;
-  const int b = blockIdx.x * 4 + (threadIdx.x >> 5);
-  if (b >= B) return;
-  const int a = min(max(lo[b], 0), T), e = min(max(hi[b], a), T);
-  if (a == e) return;
-  DecodeState* st = reinterpret_cast<DecodeState*>(state + b * stride);
-  const int* lab = labels + static_cast<size_t>(b) * T;
-  const int fb = frame_base[b], prev0 = st->label, rows0 = st->rows;
-  const int pos0 = counts[b];
+  const int fb = st ? io.frame_base[b] : 0, prev0 = st ? st->label : blank, rows0 = st ? st->rows : 0;
+  const int pos0 = st ? io.counts[b] : 0;
   int pos = pos0;
   [[maybe_unused]] double part = 0.0;
   [[maybe_unused]] const int rot = rows0 & 31;   // lane k keeps partial k; row t comes from lane (k - rot) mod 32
-  if constexpr (SCORED) part = st->part[lane];
+  if constexpr (SCORED) {
+    if (st) part = st->part[lane];
+  }
   for (int t0 = a; t0 < e; t0 += 32) {
     const int t = t0 + lane;
     int l = blank, prev = blank;
@@ -211,14 +161,16 @@ __global__ void __launch_bounds__(128) ctc_collapse_resume_kernel(const int* __r
     if constexpr (SCORED) {
       if (t < e) {
         x = lp[static_cast<size_t>(b) * T + t];
-        frame_logp[b * frame_pitch + fb + t] = static_cast<double>(x);
-        frame_rows[b * frame_pitch + fb + t] = 1;
+        if (io.frame_logp) {
+          io.frame_logp[b * io.frame_pitch + fb + t] = static_cast<double>(x);
+          io.frame_rows[b * io.frame_pitch + fb + t] = 1;
+        }
       }
     }
-    if (keep && p < max_out) {
-      ids[static_cast<size_t>(b) * max_out + p] = l;
-      frames[static_cast<size_t>(b) * max_out + p] = fb + t;
-      if constexpr (SCORED) token_logp[static_cast<size_t>(b) * max_out + p] = x;
+    if (keep && p < io.max_out) {
+      io.ids[static_cast<size_t>(b) * io.max_out + p] = l;
+      io.frames[static_cast<size_t>(b) * io.max_out + p] = fb + t;
+      if constexpr (SCORED) io.token_logp[static_cast<size_t>(b) * io.max_out + p] = x;
     }
     if constexpr (SCORED) {
       const int src = (lane - rot) & 31;
@@ -228,18 +180,20 @@ __global__ void __launch_bounds__(128) ctc_collapse_resume_kernel(const int* __r
     pos += __popc(mask);
   }
   if constexpr (SCORED) {
-    st->part[lane] = part;
+    if (st) st->part[lane] = part;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
   }
   if (lane == 0) {
-    counts[b] = min(pos, max_out);
-    st->label = lab[e - 1];
-    st->count += pos - pos0;
+    io.counts[b] = min(pos, io.max_out);
+    if (st) {
+      st->label = lab[e - 1];
+      st->count += pos - pos0;
+      if constexpr (SCORED) st->rows = rows0 + (e - a);
+    }
     if constexpr (SCORED) {
-      st->rows = rows0 + (e - a);
-      path_logp[b] = static_cast<float>(part);
-      path_rows[b] = rows0 + (e - a);
+      io.path_logp[b] = static_cast<float>(part);
+      io.path_rows[b] = rows0 + (e - a);
     }
   }
 }
@@ -262,37 +216,18 @@ __global__ void decode_state_init_kernel(uint8_t* state, int64_t stride, int n, 
 void launch_decode_state_init(uint8_t* state, int64_t stride, int n, int blank, cudaStream_t s) {
   if (n > 0) decode_state_init_kernel<<<n, 256, 0, s>>>(state, stride, n, blank);
 }
-void launch_ctc_collapse_resume(const int* labels, const float* lp, const int* lo, const int* hi, const int* frame_base, int B, int T,
-                                int blank, uint8_t* state, int64_t stride, int* ids, int* frames, int* counts, int max_out,
-                                float* token_logp, float* path_logp, int* path_rows, double* frame_logp, int* frame_rows,
-                                int64_t frame_pitch, cudaStream_t s) {
-  if (token_logp)
-    ctc_collapse_resume_kernel<true><<<(B + 3) / 4, 128, 0, s>>>(labels, lp, lo, hi, frame_base, B, T, blank, state, stride, ids, frames,
-                                                                 counts, max_out, token_logp, path_logp, path_rows, frame_logp,
-                                                                 frame_rows, frame_pitch);
-  else
-    ctc_collapse_resume_kernel<false><<<(B + 3) / 4, 128, 0, s>>>(labels, lp, lo, hi, frame_base, B, T, blank, state, stride, ids,
-                                                                  frames, counts, max_out, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                                                  frame_pitch);
-}
-
-void launch_ctc_argmax(const float* enc, const float* W, const float* bias, int* labels, int R, int D, int V1,
+void launch_ctc_argmax(const float* enc, const float* W, const float* bias, int* labels, float* lp, int R, int D, int V1,
                        cudaStream_t s) {
-  ctc_argmax_kernel<false><<<(R + kRows - 1) / kRows, kRows * kGroups, 0, s>>>(enc, W, bias, labels, R, D, V1, nullptr);
+  if (lp)
+    ctc_argmax_kernel<true><<<(R + kRows - 1) / kRows, kRows * kGroups, 0, s>>>(enc, W, bias, labels, R, D, V1, lp);
+  else
+    ctc_argmax_kernel<false><<<(R + kRows - 1) / kRows, kRows * kGroups, 0, s>>>(enc, W, bias, labels, R, D, V1, nullptr);
 }
-void launch_ctc_collapse(const int* labels, const int* len, int B, int T, int blank, int* ids, int* frames, int* counts,
-                         cudaStream_t s) {
-  ctc_collapse_kernel<false><<<(B + 3) / 4, 128, 0, s>>>(labels, len, B, T, blank, ids, frames, counts, nullptr, nullptr, nullptr,
-                                                         nullptr);
-}
-void launch_ctc_argmax_scored(const float* enc, const float* W, const float* bias, int* labels, float* lp, int R, int D, int V1,
-                              cudaStream_t s) {
-  ctc_argmax_kernel<true><<<(R + kRows - 1) / kRows, kRows * kGroups, 0, s>>>(enc, W, bias, labels, R, D, V1, lp);
-}
-void launch_ctc_collapse_scored(const int* labels, const float* lp, const int* len, int B, int T, int blank, int* ids, int* frames,
-                                int* counts, float* token_logp, float* path_logp, int* path_rows, cudaStream_t s) {
-  ctc_collapse_kernel<true><<<(B + 3) / 4, 128, 0, s>>>(labels, len, B, T, blank, ids, frames, counts, lp, token_logp, path_logp,
-                                                        path_rows);
+void launch_ctc_collapse(const int* labels, const float* lp, int B, int T, int blank, const GreedyIo& io, cudaStream_t s) {
+  if (io.token_logp)
+    ctc_collapse_kernel<true><<<(B + 3) / 4, 128, 0, s>>>(labels, lp, B, T, blank, io);
+  else
+    ctc_collapse_kernel<false><<<(B + 3) / 4, 128, 0, s>>>(labels, lp, B, T, blank, io);
 }
 
 }  // namespace gam

@@ -658,6 +658,53 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
   return 0;
 }
 
+// the greedy decoders' launches, after each entry point's own checks: labels and (scored) l of every row in the workspace,
+// then the collapse (io: a fresh or a resume call, kernels.h)
+static int ctc_greedy_impl(gam_handle* h, const char* what, const float* enc, int32_t B, int32_t T, void* workspace,
+                           const GreedyIo& io, void* stream) {
+  const gam_config& c = h->cfg;
+  const int64_t R = static_cast<int64_t>(B) * T;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int* labels = static_cast<int*>(workspace);
+  float* lp = io.token_logp ? reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + align_up(R * 4, 1024)) : nullptr;
+  { PROF(PC_CTC_ARGMAX);
+    launch_ctc_argmax(enc, h->w.ctc_w, h->w.ctc_b, labels, lp, static_cast<int>(R), c.d_model, c.num_classes, s); }
+  { PROF(PC_CTC_COLLAPSE);
+    launch_ctc_collapse(labels, lp, B, T, c.num_classes - 1, io, s); }
+  GAM_CHECK_LAUNCH(h, what);
+  return 0;
+}
+
+// the encoder projection of every row into the workspace, then the cluster kernel
+static int rnnt_greedy_impl(gam_handle* h, const char* what, const float* enc, int32_t B, int32_t T, void* workspace,
+                            const GreedyIo& io, void* stream) {
+  const gam_config& c = h->cfg;
+  const int64_t R = static_cast<int64_t>(B) * T;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  float* encproj = static_cast<float*>(workspace);
+  { PROF(PC_RNNT_ENCPROJ);   // a row's projection does not depend on the others, so a resume call projects every row too
+    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, encproj, static_cast<int>(R), c.joint_hidden, c.d_model, s); }
+  PROF(PC_RNNT_GREEDY);
+  const int rc = launch_rnnt_greedy(encproj, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h->w.rnnt_wp_t, h->w.rnnt_bp, h->w.rnnt_wo,
+                                    h->w.rnnt_bo, B, T, c.pred_hidden, c.num_classes, c.num_classes - 1, c.max_symbols, io, nullptr, s);
+  if (rc > 0)
+    return fail(h, -1, "rnnt: the greedy kernel is specialised for pred_hidden = joint_hidden = 320 and needs 16-CTA clusters "
+                "(pred_hidden %d)", c.pred_hidden);
+  if (rc < 0) return fail(h, -4, "rnnt cluster kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, what);
+  return 0;
+}
+
+// a one-shot call: every row from a fresh stream over [0, enc_len[b])
+static GreedyIo fresh_io(const int32_t* enc_len, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp,
+                         float* path_logp, int32_t* path_rows) {
+  GreedyIo io{};
+  io.ids = ids; io.frames = frames; io.counts = counts; io.max_out = max_out;
+  io.token_logp = token_logp; io.path_logp = path_logp; io.path_rows = path_rows;
+  io.hi = enc_len;
+  return io;
+}
+
 int gam_ctc_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
                    int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out, void* stream) {
   const gam_config& c = h->cfg;
@@ -666,14 +713,8 @@ int gam_ctc_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int3
   if (max_out != T) return fail(h, -1, "ids/frames row pitch must equal T for the CTC path");
   const int64_t R = static_cast<int64_t>(B) * T;
   if (workspace_bytes < R * 4) return fail(h, -1, "workspace too small for CTC labels");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int* labels = static_cast<int*>(workspace);
-  { PROF(PC_CTC_ARGMAX);
-    launch_ctc_argmax(enc, h->w.ctc_w, h->w.ctc_b, labels, static_cast<int>(R), c.d_model, c.num_classes, s); }
-  { PROF(PC_CTC_COLLAPSE);
-    launch_ctc_collapse(labels, enc_len, B, T, c.num_classes - 1, ids, frames, counts, s); }
-  GAM_CHECK_LAUNCH(h, "ctc_greedy");
-  return 0;
+  return ctc_greedy_impl(h, "ctc_greedy", enc, B, T, workspace,
+                         fresh_io(enc_len, ids, frames, counts, max_out, nullptr, nullptr, nullptr), stream);
 }
 
 int gam_ctc_greedy_scored(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
@@ -685,60 +726,34 @@ int gam_ctc_greedy_scored(gam_handle* h, const float* enc, const int32_t* enc_le
   if (max_out != T) return fail(h, -1, "ids/frames row pitch must equal T for the CTC path");
   if (!token_logp || !path_logp || !path_rows) return fail(h, -1, "ctc_greedy_scored: token_logp, path_logp and path_rows are required");
   const int64_t R = static_cast<int64_t>(B) * T;
-  const int64_t lp_off = align_up(R * 4, 1024);
-  if (workspace_bytes < lp_off + R * 4) return fail(h, -1, "workspace too small for CTC labels and scores");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int* labels = static_cast<int*>(workspace);
-  float* lp = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + lp_off);
-  { PROF(PC_CTC_ARGMAX);
-    launch_ctc_argmax_scored(enc, h->w.ctc_w, h->w.ctc_b, labels, lp, static_cast<int>(R), c.d_model, c.num_classes, s); }
-  { PROF(PC_CTC_COLLAPSE);
-    launch_ctc_collapse_scored(labels, lp, enc_len, B, T, c.num_classes - 1, ids, frames, counts, token_logp, path_logp, path_rows,
-                               s); }
-  GAM_CHECK_LAUNCH(h, "ctc_greedy_scored");
-  return 0;
+  if (workspace_bytes < align_up(R * 4, 1024) + R * 4) return fail(h, -1, "workspace too small for CTC labels and scores");
+  return ctc_greedy_impl(h, "ctc_greedy_scored", enc, B, T, workspace,
+                         fresh_io(enc_len, ids, frames, counts, max_out, token_logp, path_logp, path_rows), stream);
 }
 
-static int rnnt_greedy_impl(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
-                            int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
-                            float* token_logp, float* path_logp, int32_t* path_rows, void* stream);
+static int rnnt_greedy_args(gam_handle* h, int32_t B, int32_t T, int64_t workspace_bytes) {
+  const gam_config& c = h->cfg;
+  if (c.head != 2) return fail(h, -1, "model has no RNN-T head");
+  if (c.pred_hidden != c.joint_hidden) return fail(h, -1, "pred_hidden != joint_hidden is not supported");
+  if (workspace_bytes < static_cast<int64_t>(B) * T * c.joint_hidden * 4)
+    return fail(h, -1, "workspace too small for the RNN-T encoder projection");
+  return 0;
+}
 
 int gam_rnnt_greedy_scored(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
                            int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
                            float* token_logp, float* path_logp, int32_t* path_rows, void* stream) {
   if (!token_logp || !path_logp || !path_rows) return fail(h, -1, "rnnt_greedy_scored: token_logp, path_logp and path_rows are required");
-  return rnnt_greedy_impl(h, enc, enc_len, B, T, workspace, workspace_bytes, ids, frames, counts, max_out, token_logp, path_logp,
-                          path_rows, stream);
+  if (rnnt_greedy_args(h, B, T, workspace_bytes) != 0) return -1;
+  return rnnt_greedy_impl(h, "rnnt_greedy", enc, B, T, workspace,
+                          fresh_io(enc_len, ids, frames, counts, max_out, token_logp, path_logp, path_rows), stream);
 }
 
 int gam_rnnt_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
                     int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out, void* stream) {
-  return rnnt_greedy_impl(h, enc, enc_len, B, T, workspace, workspace_bytes, ids, frames, counts, max_out, nullptr, nullptr, nullptr,
-                          stream);
-}
-
-static int rnnt_greedy_impl(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
-                            int64_t workspace_bytes, int32_t* ids, int32_t* frames, int32_t* counts, int32_t max_out,
-                            float* token_logp, float* path_logp, int32_t* path_rows, void* stream) {
-  const gam_config& c = h->cfg;
-  if (c.head != 2) return fail(h, -1, "model has no RNN-T head");
-  if (c.pred_hidden != c.joint_hidden) return fail(h, -1, "pred_hidden != joint_hidden is not supported");
-  const int64_t R = static_cast<int64_t>(B) * T;
-  if (workspace_bytes < R * c.joint_hidden * 4) return fail(h, -1, "workspace too small for the RNN-T encoder projection");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  float* encproj = static_cast<float*>(workspace);
-  { PROF(PC_RNNT_ENCPROJ);
-    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, encproj, static_cast<int>(R), c.joint_hidden, c.d_model, s); }
-  PROF(PC_RNNT_GREEDY);
-  const int rc = launch_rnnt_greedy_cluster(encproj, enc_len, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h->w.rnnt_wp_t, h->w.rnnt_bp,
-                                            h->w.rnnt_wo, h->w.rnnt_bo, B, T, c.pred_hidden, c.num_classes, c.num_classes - 1,
-                                            c.max_symbols, max_out, ids, frames, counts, token_logp, path_logp, path_rows, nullptr, s);
-  if (rc > 0)
-    return fail(h, -1, "rnnt: the greedy kernel is specialised for pred_hidden = joint_hidden = 320 and needs 16-CTA clusters "
-                "(pred_hidden %d)", c.pred_hidden);
-  if (rc < 0) return fail(h, -4, "rnnt cluster kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-  GAM_CHECK_LAUNCH(h, "rnnt_greedy");
-  return 0;
+  if (rnnt_greedy_args(h, B, T, workspace_bytes) != 0) return -1;
+  return rnnt_greedy_impl(h, "rnnt_greedy", enc, B, T, workspace,
+                          fresh_io(enc_len, ids, frames, counts, max_out, nullptr, nullptr, nullptr), stream);
 }
 
 int64_t gam_decode_state_bytes(const gam_handle* h) {
@@ -778,6 +793,16 @@ static int resume_args(gam_handle* h, const char* what, int head, const float* e
   return 0;
 }
 
+// a resume call: stream b continues from its DecodeState over [lo[b], hi[b])
+static GreedyIo resume_io(const int32_t* lo, const int32_t* hi, const int32_t* frame_base, void* state, int64_t stride, int32_t* ids,
+                          int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
+                          double* frame_logp, int32_t* frame_rows, int64_t frame_pitch) {
+  GreedyIo io = fresh_io(hi, ids, frames, counts, max_out, token_logp, path_logp, path_rows);
+  io.frame_logp = frame_logp; io.frame_rows = frame_rows; io.frame_pitch = frame_pitch;
+  io.lo = lo; io.frame_base = frame_base; io.state = static_cast<uint8_t*>(state); io.stride = stride;
+  return io;
+}
+
 int gam_ctc_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
                           const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes, int32_t* ids,
                           int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
@@ -785,21 +810,10 @@ int gam_ctc_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T,
   if (resume_args(h, "ctc_greedy_resume", 1, enc, B, T, lo, hi, frame_base, state, workspace, workspace_bytes, ids, frames, counts,
                   max_out, token_logp, path_logp, path_rows, frame_logp, frame_rows, frame_pitch) != 0)
     return -1;
-  const gam_config& c = h->cfg;
-  const int64_t R = static_cast<int64_t>(B) * T;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
   // the ranges live on the device, so every row is labelled; each row's label and l do not depend on the others
-  int* labels = static_cast<int*>(workspace);
-  float* lp = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + align_up(R * 4, 1024));
-  { PROF(PC_CTC_ARGMAX);
-    if (token_logp) launch_ctc_argmax_scored(enc, h->w.ctc_w, h->w.ctc_b, labels, lp, static_cast<int>(R), c.d_model, c.num_classes, s);
-    else launch_ctc_argmax(enc, h->w.ctc_w, h->w.ctc_b, labels, static_cast<int>(R), c.d_model, c.num_classes, s); }
-  { PROF(PC_CTC_COLLAPSE);
-    launch_ctc_collapse_resume(labels, lp, lo, hi, frame_base, B, T, c.num_classes - 1, static_cast<uint8_t*>(state),
-                               kCtcDecodeStateBytes, ids, frames, counts, max_out, token_logp, path_logp, path_rows, frame_logp,
-                               frame_rows, frame_pitch, s); }
-  GAM_CHECK_LAUNCH(h, "ctc_greedy_resume");
-  return 0;
+  return ctc_greedy_impl(h, "ctc_greedy_resume", enc, B, T, workspace,
+                         resume_io(lo, hi, frame_base, state, kCtcDecodeStateBytes, ids, frames, counts, max_out, token_logp,
+                                   path_logp, path_rows, frame_logp, frame_rows, frame_pitch), stream);
 }
 
 int gam_rnnt_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
@@ -809,25 +823,10 @@ int gam_rnnt_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T
   if (resume_args(h, "rnnt_greedy_resume", 2, enc, B, T, lo, hi, frame_base, state, workspace, workspace_bytes, ids, frames, counts,
                   max_out, token_logp, path_logp, path_rows, frame_logp, frame_rows, frame_pitch) != 0)
     return -1;
-  const gam_config& c = h->cfg;
-  if (c.pred_hidden != c.joint_hidden) return fail(h, -1, "pred_hidden != joint_hidden is not supported");
-  const int64_t R = static_cast<int64_t>(B) * T;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  float* encproj = static_cast<float*>(workspace);
-  { PROF(PC_RNNT_ENCPROJ);   // every row, as gam_rnnt_greedy: a row's projection does not depend on the others
-    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, encproj, static_cast<int>(R), c.joint_hidden, c.d_model, s); }
-  PROF(PC_RNNT_GREEDY);
-  const int rc = launch_rnnt_greedy_resume(encproj, lo, hi, frame_base, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h->w.rnnt_wp_t,
-                                           h->w.rnnt_bp, h->w.rnnt_wo, h->w.rnnt_bo, B, T, c.pred_hidden, c.num_classes,
-                                           c.num_classes - 1, c.max_symbols, max_out, static_cast<uint8_t*>(state),
-                                           kRnntDecodeStateBytes, ids, frames, counts, token_logp, path_logp, path_rows, frame_logp,
-                                           frame_rows, frame_pitch, s);
-  if (rc > 0)
-    return fail(h, -1, "rnnt: the greedy kernel is specialised for pred_hidden = joint_hidden = 320 and needs 16-CTA clusters "
-                "(pred_hidden %d)", c.pred_hidden);
-  if (rc < 0) return fail(h, -4, "rnnt cluster kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-  GAM_CHECK_LAUNCH(h, "rnnt_greedy_resume");
-  return 0;
+  if (h->cfg.pred_hidden != h->cfg.joint_hidden) return fail(h, -1, "pred_hidden != joint_hidden is not supported");
+  return rnnt_greedy_impl(h, "rnnt_greedy_resume", enc, B, T, workspace,
+                          resume_io(lo, hi, frame_base, state, kRnntDecodeStateBytes, ids, frames, counts, max_out, token_logp,
+                                    path_logp, path_rows, frame_logp, frame_rows, frame_pitch), stream);
 }
 
 int gam_ctc_log_probs(gam_handle* h, const float* enc, int32_t B, int32_t T, float* log_probs, void* stream) {
@@ -1632,6 +1631,21 @@ int gam_test_mel_log(gam_handle* h, const float* P, const int32_t* fexp, int32_t
   return 0;
 }
 
+static int test_rnnt_greedy(gam_handle* h, const char* what, const float* encproj, const int32_t* len, const float* emb_gates,
+                            const float* whhT, const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T,
+                            int32_t V1, int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts,
+                            float* token_logp, float* path_logp, int32_t* path_rows, int32_t* plan, void* stream) {
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  { PROF(PC_RNNT_GREEDY);
+    rc = launch_rnnt_greedy(encproj, emb_gates, whhT, wpT, bp, wo, bo, B, T, 320, V1, V1 - 1, max_symbols,
+                            fresh_io(len, ids, frames, counts, max_out, token_logp, path_logp, path_rows), plan, s); }
+  if (rc > 0) return fail(h, -1, "%s: 16-CTA clusters cannot be scheduled on this device", what);
+  if (rc < 0) return fail(h, -4, "%s: launch failed: %s", what, cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, what);
+  return 0;
+}
+
 int gam_test_rnnt_greedy_scored(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,
                                 const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
                                 int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts,
@@ -1642,15 +1656,8 @@ int gam_test_rnnt_greedy_scored(gam_handle* h, const float* encproj, const int32
   if (B <= 0 || T <= 0 || V1 < 2 || max_symbols <= 0 || max_out <= 0)
     return fail(h, -1, "test_rnnt_greedy_scored: bad sizes (B=%d, T=%d, V1=%d, max_symbols=%d, max_out=%d)", B, T, V1, max_symbols,
                 max_out);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int rc;
-  { PROF(PC_RNNT_GREEDY);
-    rc = launch_rnnt_greedy_cluster(encproj, len, emb_gates, whhT, wpT, bp, wo, bo, B, T, 320, V1, V1 - 1, max_symbols, max_out, ids,
-                                    frames, counts, token_logp, path_logp, path_rows, plan, s); }
-  if (rc > 0) return fail(h, -1, "test_rnnt_greedy_scored: 16-CTA clusters cannot be scheduled on this device");
-  if (rc < 0) return fail(h, -4, "test_rnnt_greedy_scored: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-  GAM_CHECK_LAUNCH(h, "test_rnnt_greedy_scored");
-  return 0;
+  return test_rnnt_greedy(h, "test_rnnt_greedy_scored", encproj, len, emb_gates, whhT, wpT, bp, wo, bo, B, T, V1, max_symbols, max_out,
+                          ids, frames, counts, token_logp, path_logp, path_rows, plan, stream);
 }
 
 int gam_test_rnnt_greedy(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,
@@ -1661,15 +1668,8 @@ int gam_test_rnnt_greedy(gam_handle* h, const float* encproj, const int32_t* len
     return fail(h, -1, "test_rnnt_greedy: every operand is required");
   if (B <= 0 || T <= 0 || V1 < 2 || max_symbols <= 0 || max_out <= 0)
     return fail(h, -1, "test_rnnt_greedy: bad sizes (B=%d, T=%d, V1=%d, max_symbols=%d, max_out=%d)", B, T, V1, max_symbols, max_out);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int rc;
-  { PROF(PC_RNNT_GREEDY);
-    rc = launch_rnnt_greedy_cluster(encproj, len, emb_gates, whhT, wpT, bp, wo, bo, B, T, 320, V1, V1 - 1, max_symbols, max_out, ids,
-                                    frames, counts, nullptr, nullptr, nullptr, plan, s); }
-  if (rc > 0) return fail(h, -1, "test_rnnt_greedy: 16-CTA clusters cannot be scheduled on this device");
-  if (rc < 0) return fail(h, -4, "test_rnnt_greedy: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-  GAM_CHECK_LAUNCH(h, "test_rnnt_greedy");
-  return 0;
+  return test_rnnt_greedy(h, "test_rnnt_greedy", encproj, len, emb_gates, whhT, wpT, bp, wo, bo, B, T, V1, max_symbols, max_out, ids,
+                          frames, counts, nullptr, nullptr, nullptr, plan, stream);
 }
 
 int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void* out, int32_t B, int32_t T, void* stream) {

@@ -51,17 +51,9 @@ int launch_attention(const CUtensorMap* tmap_qkv, const int* klen, const int* cu
 int launch_attention_relpos(const CUtensorMap* tmap_qkv, const CUtensorMap* tmap_pos, int max_t, const int* klen, const int* cu,
                             __half* out, int B, int T, int H, int dk, int d_model, cudaStream_t s);
 
-// ctc.cu
-void launch_ctc_argmax(const float* enc, const float* W, const float* bias, int* labels, int R, int D, int V1,
+// ctc.cu: labels [R] of every row; lp (or NULL: unscored) [R] f32 scratch of each row's log_softmax(row)[label]
+void launch_ctc_argmax(const float* enc, const float* W, const float* bias, int* labels, float* lp, int R, int D, int V1,
                        cudaStream_t s);
-void launch_ctc_collapse(const int* labels, const int* len, int B, int T, int blank, int* ids, int* frames, int* counts,
-                         cudaStream_t s);
-// scored twins (gam_ctc_greedy_scored): lp [R] f32 scratch of per-frame log_softmax(row)[label]; token_logp [B, T],
-// path_logp [B], path_rows [B]
-void launch_ctc_argmax_scored(const float* enc, const float* W, const float* bias, int* labels, float* lp, int R, int D, int V1,
-                              cudaStream_t s);
-void launch_ctc_collapse_scored(const int* labels, const float* lp, const int* len, int B, int T, int blank, int* ids, int* frames,
-                                int* counts, float* token_logp, float* path_logp, int* path_rows, cudaStream_t s);
 
 // Resumable greedy decoding (gam_*_greedy_resume): what the greedy loop keeps across a frame boundary, one record per decoding
 // stream.  CTC uses the record up to `h`; RNN-T all of it.  A fresh utterance is label = blank, pending = 1, zeros elsewhere.
@@ -80,11 +72,32 @@ constexpr int64_t kCtcDecodeStateBytes = static_cast<int64_t>(offsetof(DecodeSta
 constexpr int64_t kRnntDecodeStateBytes = static_cast<int64_t>(sizeof(DecodeState));
 static_assert(kCtcDecodeStateBytes % 16 == 0, "state records stay 16-byte aligned");
 void launch_decode_state_init(uint8_t* state, int64_t stride, int n, int blank, cudaStream_t s);
-// CTC collapse of labels[b, lo[b] .. hi[b]) continuing the stream at state + b * stride (lp / token_logp null: unscored)
-void launch_ctc_collapse_resume(const int* labels, const float* lp, const int* lo, const int* hi, const int* frame_base, int B, int T,
-                                int blank, uint8_t* state, int64_t stride, int* ids, int* frames, int* counts, int max_out,
-                                float* token_logp, float* path_logp, int* path_rows, double* frame_logp, int* frame_rows,
-                                int64_t frame_pitch, cudaStream_t s);
+
+// What a greedy decode of B streams writes, and which frames of each stream it decodes (launch_ctc_collapse,
+// launch_rnnt_greedy).  A fresh call (state NULL) decodes frames [0, hi[b]) of row b from a fresh stream, emits frames t and
+// writes counts (and, scored, path_logp / path_rows) for every row; lo and frame_base are not read.  A resume call continues
+// the DecodeState at state + b * stride over frames [lo[b], hi[b]), appends at counts[b], emits frames frame_base[b] + t and
+// stores the record back; a row with lo[b] == hi[b] keeps its record and outputs.  Either way decoding [0, L) of a stream in
+// consecutive calls gives a fresh call's bits.
+struct GreedyIo {
+  int* ids;              // [B, max_out]
+  int* frames;           // [B, max_out]
+  int* counts;           // [B]: tokens stored (at most max_out)
+  int max_out;
+  float* token_logp;     // [B, max_out]; NULL: unscored, and the three score outputs are not written
+  float* path_logp;      // [B] sum of l over the decision rows (scored)
+  int* path_rows;        // [B] their number (scored)
+  double* frame_logp;    // [b * frame_pitch + frame] sum of l over the frame's decision rows (scored), or NULL
+  int* frame_rows;       // [b * frame_pitch + frame] their number (set with frame_logp)
+  int64_t frame_pitch;
+  const int* lo;         // [B] (resume)
+  const int* hi;         // [B] one past the last frame: the lengths for a fresh call
+  const int* frame_base; // [B] (resume)
+  uint8_t* state;        // DecodeState records, or NULL: a fresh call
+  int64_t stride;
+};
+// CTC collapse of labels [B, T] (lp [B, T] from launch_ctc_argmax when scored)
+void launch_ctc_collapse(const int* labels, const float* lp, int B, int T, int blank, const GreedyIo& io, cudaStream_t s);
 
 // words.cu: (token id, frame) pairs -> word records (first frame, last frame + 1, first token, tokens) per utterance
 void launch_group_words(const int* ids, const int* frames, const int* counts, const unsigned char* flags, int B, int V, int max_out,
@@ -171,21 +184,12 @@ void launch_lstm_bwd_step(const int64_t* x, int U, int u, int V1, const float* e
 // out [V1, H4]: per-class sums of dgates rows (blank row zero); returns 1 if H4 is too large
 int launch_class_gate_sum(const int64_t* x, int64_t rows, const float* dgates, int H4, int V1, int blank, float* out, cudaStream_t s);
 
-// rnnt_cluster.cu: returns 0 ok, 1 = 16-CTA clusters unavailable / unsupported shape, <0 error.  plan: host int[7] that
-// receives the chosen launch (NH, GLOB, rows_smem, cls_per, nu, groups, clusters), or NULL.  token_logp [B, max_out],
-// path_logp [B], path_rows [B]: all NULL for the unscored kernel, all set for the scored one
-int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float* emb_gates, const float* whhT, const float* wpT,
-                               const float* bp, const float* wo, const float* bo, int B, int T, int H, int V1, int blank,
-                               int max_symbols, int max_out, int* ids, int* frames, int* counts, float* token_logp,
-                               float* path_logp, int* path_rows, int* plan, cudaStream_t s);
-// the same kernel resuming stream b (DecodeState at state + b * stride) over frames [lo[b], hi[b]) of encproj row b; frames are
-// emitted as frame_base[b] + t and tokens appended at counts[b].  token_logp set: scored, and frame_logp / frame_rows
-// [b * frame_pitch + frame_base[b] + t] receive each frame's sum of l and its decision rows.  Returns as above.
-int launch_rnnt_greedy_resume(const float* encproj, const int* lo, const int* hi, const int* frame_base, const float* emb_gates,
-                              const float* whhT, const float* wpT, const float* bp, const float* wo, const float* bo, int B, int T,
-                              int H, int V1, int blank, int max_symbols, int max_out, uint8_t* state, int64_t stride, int* ids,
-                              int* frames, int* counts, float* token_logp, float* path_logp, int* path_rows, double* frame_logp,
-                              int* frame_rows, int64_t frame_pitch, cudaStream_t s);
+// rnnt_cluster.cu: greedy decode of encproj [B, T, H] (see GreedyIo).  Returns 0 ok, 1 = 16-CTA clusters unavailable /
+// unsupported shape, <0 error.  plan: host int[7] that receives the chosen launch (NH, GLOB, rows_smem, cls_per, nu, groups,
+// clusters), or NULL.
+int launch_rnnt_greedy(const float* encproj, const float* emb_gates, const float* whhT, const float* wpT, const float* bp,
+                       const float* wo, const float* bo, int B, int T, int H, int V1, int blank, int max_symbols, const GreedyIo& io,
+                       int* plan, cudaStream_t s);
 
 // gemm.cu
 struct GemmParams;

@@ -43,7 +43,6 @@
 #include <cooperative_groups.h>
 
 #include <cstdlib>
-#include <type_traits>
 
 #include "kernels.h"
 #include "ptx.cuh"
@@ -67,39 +66,17 @@ constexpr int kGP = 2;            // L2-resident class rows a warp prefetches in
 
 struct RnntClParams {
   const float* encproj;    // [B*T, H]
-  const int* len;          // [B]
   const float* emb_gates;  // [V1, 4H]
   const float* whhT;       // [H, 4H]  (W_hh^T)
   const float* wpT;        // [H, H]   (W_p^T)
   const float* bp;
   const float* wo;         // [V1, H]
   const float* bo;
-  int B, T, V1, blank, max_symbols, max_out, num_groups, nu;   // nu <= 4 * NH utterances per group
+  int B, T, V1, blank, max_symbols, num_groups, nu;   // nu <= 4 * NH utterances per group
   int rows_smem;           // class rows of W_o resident in shared memory per CTA
   int cls_pad;             // floats reserved for the bias slice
-  int* ids;
-  int* frames;
-  int* counts;
+  GreedyIo io;             // outputs and stream ranges (kernels.h); io.state == NULL: a fresh call
 };
-// the scored instantiation's parameters (the unscored kernel keeps RnntClParams, so its code does not move)
-struct RnntClScoredParams : RnntClParams {
-  float* token_logp;       // [B, max_out]
-  float* path_logp;        // [B]
-  int* path_rows;          // [B]
-};
-// the resumable instantiations' parameters (gam_rnnt_greedy_resume; token_logp null: unscored)
-struct RnntClResumeParams : RnntClScoredParams {
-  const int* lo;           // [B] first frame of row b to decode
-  const int* hi;           // [B] one past the last
-  const int* frame_base;   // [B] emitted frame = frame_base[b] + t
-  uint8_t* state;          // DecodeState of stream b at state + b * stride
-  int64_t stride;
-  double* frame_logp;      // [B, frame_pitch] (scored): sum of l over the decision rows of frame frame_base[b] + t
-  int* frame_rows;         // [B, frame_pitch] (scored): their number
-  int64_t frame_pitch;
-};
-template <bool SCORED, bool RESUME = false>
-using ClParams = std::conditional_t<RESUME, RnntClResumeParams, std::conditional_t<SCORED, RnntClScoredParams, RnntClParams>>;
 
 // per-utterance decoding state (gigaam/decoding.py:150-205), owned by warp 0 of every CTA (identical in all of them)
 struct Ctl {
@@ -239,6 +216,11 @@ __device__ __forceinline__ void push16(const void* local_dst, uint64_t* local_ba
   push16(local_dst, local_bar, cta, __float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w));
 }
 
+// stream b's DecodeState, or NULL on a fresh call
+__device__ __forceinline__ DecodeState* state_of(const RnntClParams& p, int b) {
+  return p.io.state ? reinterpret_cast<DecodeState*>(p.io.state + b * p.io.stride) : nullptr;
+}
+
 #ifdef GAM_RNNT_DBG
 // phase timing of cluster 0 / CTA 0 / thread 0 (tools/rnnt_phase_probe.py; never compiled into the shipped library)
 __device__ long long g_rnnt_dbg[16];
@@ -249,12 +231,13 @@ __device__ long long g_rnnt_dbg[16];
 
 // NH: float4 halves of utterances per group (4 or 8 utterances).  GLOB: some class rows stay in L2 (large vocabularies);
 // compiled out otherwise (the round loop is executed once per step by every warp; 16 KB less code).
-// RESUME (gam_rnnt_greedy_resume): a group starts from the DecodeState records of its utterances instead of a fresh
-// utterance -- control state, label, pending LSTM step, h, c and pg -- decodes frames [lo, hi) of each row and stores the
-// state back.  A chunk edge is a frame edge (nsym = 0), so decoding [0, L) in consecutive chunks runs the same operations on
-// the same values as one pass.  The other instantiations compile none of it.
-template <int NH, bool GLOB, bool SCORED, bool RESUME>
-__global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const ClParams<SCORED, RESUME> p) {
+// A resume call (p.io.state set, gam_rnnt_greedy_resume) starts a group from the DecodeState records of its utterances --
+// control state, label, pending LSTM step, h, c and pg -- decodes frames [lo, hi) of each row and stores the state back.
+// A fresh call starts from the constants of a fresh record (blank label, a pending step, zeros) and decodes [0, hi).  A chunk
+// edge is a frame edge (nsym = 0), so decoding [0, L) in consecutive chunks runs the same operations on the same values as
+// one fresh call.
+template <int NH, bool GLOB, bool SCORED>
+__global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClParams p) {
   constexpr int NU = 4 * NH;
   using SM = Smem<NH>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -312,74 +295,61 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const ClParam
   constexpr uint32_t kBestBytes = best_exchange_bytes<NH, SCORED>();
 
   for (int group = cluster_id; group < p.num_groups; group += num_clusters) {
-    // RESUME, warp 0 lane u: counts[b] when the call started, frame_base[b], and the current frame's sum of l and rows
-    [[maybe_unused]] int r_cnt0 = 0, r_fb = 0, r_frows = 0;
+    // warp 0 lane u: counts[b] when the call started, frame_base[b], and the current frame's sum of l and rows
+    int r_cnt0 = 0, r_fb = 0;
+    [[maybe_unused]] int r_frows = 0;
     [[maybe_unused]] double r_facc = 0.0;
-    // ---- control state (warp 0: lane u = utterance u)
+    // ---- start of the group: control state (warp 0: lane u = utterance u), read from the DecodeState records on a resume
+    // call; lanes without an utterance start inactive
     if (warp == 0) {
-      int Lu = 0, t0 = 0;
-      [[maybe_unused]] int pend = 0;
+      int Lu = 0, t0 = 0, pend = 0;
       if (lane < kMaxU) {
         const int ug = group * p.nu + lane;
-        if constexpr (RESUME) {
-          int lbl = p.blank;
-          if (lane < p.nu && lane < NU && ug < p.B) {
-            const DecodeState* st = reinterpret_cast<const DecodeState*>(p.state + ug * p.stride);
-            t0 = min(max(p.lo[ug], 0), p.T);
-            Lu = min(max(p.hi[ug], t0), p.T);
-            lbl = st->label; pend = st->pending;
-            r_cnt0 = p.counts[ug]; r_fb = p.frame_base[ug];
-            if constexpr (SCORED) { sc.path[lane] = st->path; sc.rows[lane] = st->rows; }
-          } else if constexpr (SCORED) {
-            sc.path[lane] = 0.0; sc.rows[lane] = 0;
+        int lbl = p.blank, rows = 0;
+        double path = 0.0;
+        if (lane < p.nu && lane < NU && ug < p.B) {
+          const DecodeState* st = state_of(p, ug);
+          t0 = st ? min(max(p.io.lo[ug], 0), p.T) : 0;
+          Lu = min(max(p.io.hi[ug], t0), p.T);
+          pend = 1;
+          if (st) {
+            lbl = st->label; pend = st->pending; path = st->path; rows = st->rows;
+            r_cnt0 = p.io.counts[ug]; r_fb = p.io.frame_base[ug];
           }
-          s.ctl.t[lane] = t0; s.ctl.nsym[lane] = 0; s.ctl.cnt[lane] = r_cnt0; s.ctl.label[lane] = lbl;
-          s.ctl.L[lane] = Lu; s.ctl.need[lane] = pend;
-        } else {
-          Lu = (lane < p.nu && lane < NU && ug < p.B) ? min(max(p.len[ug], 0), p.T) : 0;
-          s.ctl.t[lane] = 0; s.ctl.nsym[lane] = 0; s.ctl.cnt[lane] = 0; s.ctl.label[lane] = p.blank;
-          s.ctl.L[lane] = Lu; s.ctl.need[lane] = Lu > 0;
-          if constexpr (SCORED) { sc.path[lane] = 0.0; sc.rows[lane] = 0; }
         }
+        s.ctl.t[lane] = t0; s.ctl.nsym[lane] = 0; s.ctl.cnt[lane] = r_cnt0; s.ctl.label[lane] = lbl;
+        s.ctl.L[lane] = Lu; s.ctl.need[lane] = pend;
+        if constexpr (SCORED) { sc.path[lane] = path; sc.rows[lane] = rows; }
       }
-      const unsigned am = __ballot_sync(0xffffffffu, Lu > t0);
-      if constexpr (RESUME) {   // only the utterances with a pending step run the first LSTM round
-        const unsigned rm = __ballot_sync(0xffffffffu, Lu > t0 && pend != 0);
-        if (lane == 0) { s.ctl.act_m = static_cast<int>(am); s.ctl.run_m = static_cast<int>(rm); s.ctl.moved_m = 0; s.ctl.emit_m = 0; }
-      } else {
-        if (lane == 0) { s.ctl.act_m = static_cast<int>(am); s.ctl.run_m = static_cast<int>(am); s.ctl.moved_m = 0; s.ctl.emit_m = 0; }
-      }
+      // only the utterances with a pending step run the first LSTM round
+      const unsigned am = __ballot_sync(0xffffffffu, Lu > t0), rm = __ballot_sync(0xffffffffu, Lu > t0 && pend != 0);
+      if (lane == 0) { s.ctl.act_m = static_cast<int>(am); s.ctl.run_m = static_cast<int>(rm); s.ctl.moved_m = 0; s.ctl.emit_m = 0; }
     }
-    if constexpr (RESUME) {   // h, pg (all units, utterance-interleaved) and c (own units) from the state records
-      for (int i = tid; i < NH * kH; i += kThreads) {
-        const int hh = i / kH, k = i % kH;
-        float4 hv = make_float4(0.f, 0.f, 0.f, 0.f), gv = hv;
+    // h, pg (all units, utterance-interleaved) and c (own units): from the records, or zero
+    for (int i = tid; i < NH * kH; i += kThreads) {
+      const int hh = i / kH, k = i % kH;
+      float4 hv = make_float4(0.f, 0.f, 0.f, 0.f), gv = hv;
 #pragma unroll
-        for (int cc = 0; cc < 4; ++cc) {
-          const int u = 4 * hh + cc, ug = group * p.nu + u;
-          if (u < p.nu && ug < p.B) {
-            const DecodeState* st = reinterpret_cast<const DecodeState*>(p.state + ug * p.stride);
-            set_comp(hv, cc, st->h[k]);
-            set_comp(gv, cc, st->pg[k]);
-          }
+      for (int cc = 0; cc < 4; ++cc) {
+        const int u = 4 * hh + cc, ug = group * p.nu + u;
+        const DecodeState* st = u < p.nu && ug < p.B ? state_of(p, ug) : nullptr;
+        if (st) {
+          set_comp(hv, cc, st->h[k]);
+          set_comp(gv, cc, st->pg[k]);
         }
-        s.h4[0][hh][k] = hv;
-        s.h4[1][hh][k] = make_float4(0.f, 0.f, 0.f, 0.f);
-        s.pg4[hh][k] = gv;
       }
-      for (int i = tid; i < NU * kHS; i += kThreads) {
-        const int u = i / kHS, j = i % kHS, ug = group * p.nu + u;
-        s.c[0][u][j] = (u < p.nu && ug < p.B) ? reinterpret_cast<const DecodeState*>(p.state + ug * p.stride)->c[rank * kHS + j] : 0.f;
-        s.c[1][u][j] = 0.f;
-      }
-    } else {
-      for (int i = tid; i < 2 * NH * kH; i += kThreads) (&s.h4[0][0][0])[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int i = tid; i < NH * kH; i += kThreads) (&s.pg4[0][0])[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int i = tid; i < 2 * NU * kHS; i += kThreads) (&s.c[0][0][0])[i] = 0.f;
+      s.h4[0][hh][k] = hv;
+      s.h4[1][hh][k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      s.pg4[hh][k] = gv;
+    }
+    for (int i = tid; i < NU * kHS; i += kThreads) {
+      const int u = i / kHS, j = i % kHS, ug = group * p.nu + u;
+      const DecodeState* st = u < p.nu && ug < p.B ? state_of(p, ug) : nullptr;
+      s.c[0][u][j] = st ? st->c[rank * kHS + j] : 0.f;
+      s.c[1][u][j] = 0.f;
     }
     __syncthreads();
-    int act0 = 0;   // RESUME: the utterances this call decodes (the others' records and outputs are left as they are)
-    if constexpr (RESUME) act0 = s.ctl.act_m;
+    const int act0 = s.ctl.act_m;   // the utterances this call decodes (a resume call leaves the others' records and outputs)
     // encoder projection of the current frame (ep) and of the next one (epn): thread k < H keeps all utterances'
     // values in registers; a frame advance promotes epn and requests the frame after it
     float4 ep[NH], epn[NH];
@@ -393,7 +363,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const ClParam
         for (int cc = 0; cc < 4; ++cc) {
           const int u = 4 * hh + cc;
           const int Lu = s.ctl.L[u];
-          const int t0 = RESUME ? s.ctl.t[u] : 0;
+          const int t0 = s.ctl.t[u];
           if (Lu > t0) set_comp(ep[hh], cc, __ldg(ep_base + (static_cast<size_t>(u) * p.T + t0) * kH));
           if (Lu > t0 + 1) set_comp(epn[hh], cc, __ldg(ep_base + (static_cast<size_t>(u) * p.T + t0 + 1) * kH));
         }
@@ -403,8 +373,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const ClParam
     float eg[NH];
 #pragma unroll
     for (int hh = 0; hh < NH; ++hh) {
-      const int lbl = RESUME ? s.ctl.label[4 * hh + lq] : p.blank;
-      eg[hh] = gate_thread ? __ldg(p.emb_gates + static_cast<size_t>(lbl) * G + eg_off) : 0.f;
+      eg[hh] = gate_thread ? __ldg(p.emb_gates + static_cast<size_t>(s.ctl.label[4 * hh + lq]) * G + eg_off) : 0.f;
     }
     int gb = 0;   // parity of the h4 / c buffer that holds the current prediction-network state of all utterances
     cluster.sync();   // every CTA's buffers and barriers are initialised before the first remote store can arrive
@@ -679,7 +648,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const ClParam
           int need = s.ctl.need[u];
           if (t < Lu) {
             if constexpr (SCORED) { sc.path[u] += static_cast<double>(lp); sc.rows[u] += 1; }
-            if constexpr (RESUME && SCORED) { r_facc += static_cast<double>(lp); r_frows += 1; }
+            if constexpr (SCORED) { r_facc += static_cast<double>(lp); r_frows += 1; }
             if (lab == p.blank) {
               t += 1;
               s.ctl.nsym[u] = 0;
@@ -687,11 +656,11 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const ClParam
               moved = true;
             } else {
               const int cnt = s.ctl.cnt[u];
-              if (rank == 0 && cnt < p.max_out) {
-                const size_t o = static_cast<size_t>(group * p.nu + u) * p.max_out + cnt;
-                p.ids[o] = lab;
-                p.frames[o] = RESUME ? r_fb + t : t;
-                if constexpr (SCORED) p.token_logp[o] = lp;
+              if (rank == 0 && cnt < p.io.max_out) {
+                const size_t o = static_cast<size_t>(group * p.nu + u) * p.io.max_out + cnt;
+                p.io.ids[o] = lab;
+                p.io.frames[o] = r_fb + t;
+                if constexpr (SCORED) p.io.token_logp[o] = lp;
               }
               s.ctl.cnt[u] = cnt + 1;
               s.ctl.label[u] = lab;
@@ -703,12 +672,12 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const ClParam
             }
             s.ctl.t[u] = t;
             s.ctl.need[u] = need;
-            if constexpr (RESUME && SCORED) {   // a frame is complete when the decoder leaves it
+            if constexpr (SCORED) {   // a frame is complete when the decoder leaves it
               if (moved) {
-                if (rank == 0) {
-                  const int64_t o = static_cast<int64_t>(group * p.nu + u) * p.frame_pitch + r_fb + t - 1;
-                  p.frame_logp[o] = r_facc;
-                  p.frame_rows[o] = r_frows;
+                if (rank == 0 && p.io.frame_logp) {
+                  const int64_t o = static_cast<int64_t>(group * p.nu + u) * p.io.frame_pitch + r_fb + t - 1;
+                  p.io.frame_logp[o] = r_facc;
+                  p.io.frame_rows[o] = r_frows;
                 }
                 r_facc = 0.0;
                 r_frows = 0;
@@ -753,37 +722,28 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const ClParam
       }
       DBG_T(12);
     }
-    if constexpr (RESUME) {
-      if (rank == 0 && warp == 0 && lane < NU && ((act0 >> lane) & 1)) {
-        const int ug = group * p.nu + lane;
-        DecodeState* st = reinterpret_cast<DecodeState*>(p.state + ug * p.stride);
-        p.counts[ug] = min(s.ctl.cnt[lane], p.max_out);
-        st->label = s.ctl.label[lane];
-        st->pending = s.ctl.need[lane];
-        st->count += s.ctl.cnt[lane] - r_cnt0;
-        if constexpr (SCORED) {
-          st->path = sc.path[lane];
-          st->rows = sc.rows[lane];
-          p.path_logp[ug] = static_cast<float>(sc.path[lane]);
-          p.path_rows[ug] = sc.rows[lane];
+    // ---- end of the group: a fresh call writes the outputs of every row, a resume call those of the streams it advanced and
+    // their records
+    if (rank == 0 && warp == 0 && lane < NU) {
+      const int ug = group * p.nu + lane;
+      if (p.io.state ? ((act0 >> lane) & 1) != 0 : (lane < p.nu && ug < p.B)) {
+        p.io.counts[ug] = min(s.ctl.cnt[lane], p.io.max_out);
+        if constexpr (SCORED) { p.io.path_logp[ug] = static_cast<float>(sc.path[lane]); p.io.path_rows[ug] = sc.rows[lane]; }
+        if (DecodeState* st = state_of(p, ug)) {
+          st->label = s.ctl.label[lane];
+          st->pending = s.ctl.need[lane];
+          st->count += s.ctl.cnt[lane] - r_cnt0;
+          if constexpr (SCORED) { st->path = sc.path[lane]; st->rows = sc.rows[lane]; }
         }
       }
-      if (tid < NU * kHS) {   // every CTA stores its own units of h, c and pg
-        const int u = tid / kHS, j = tid % kHS, k = rank * kHS + j;
-        if ((act0 >> u) & 1) {
-          DecodeState* st = reinterpret_cast<DecodeState*>(p.state + (group * p.nu + u) * p.stride);
-          st->h[k] = comp(s.h4[gb][u >> 2][k], u & 3);
-          st->c[k] = s.c[gb][u][j];
-          st->pg[k] = comp(s.pg4[u >> 2][k], u & 3);
-        }
-      }
-    } else {
-      if (rank == 0 && warp == 0 && lane < NU) {
-        const int ug = group * p.nu + lane;
-        if (lane < p.nu && ug < p.B) {
-          p.counts[ug] = min(s.ctl.cnt[lane], p.max_out);
-          if constexpr (SCORED) { p.path_logp[ug] = static_cast<float>(sc.path[lane]); p.path_rows[ug] = sc.rows[lane]; }
-        }
+    }
+    if (p.io.state && tid < NU * kHS) {   // every CTA stores its own units of h, c and pg
+      const int u = tid / kHS, j = tid % kHS, k = rank * kHS + j;
+      if ((act0 >> u) & 1) {
+        DecodeState* st = state_of(p, group * p.nu + u);
+        st->h[k] = comp(s.h4[gb][u >> 2][k], u & 3);
+        st->c[k] = s.c[gb][u][j];
+        st->pg[k] = comp(s.pg4[u >> 2][k], u & 3);
       }
     }
     __syncthreads();   // ctl is re-initialised by warp 0 at the top of the next group
@@ -800,8 +760,8 @@ struct LaunchState {
   int smem_set = 0;
 };
 
-template <int NH, bool GLOB, bool SCORED, bool RESUME = false>
-int launch_nh(ClParams<SCORED, RESUME>& p, int B, int V1, int smem_cap, int* plan, cudaStream_t s) {
+template <int NH, bool GLOB, bool SCORED>
+int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, int* plan, cudaStream_t s) {
   static LaunchState per_device[64];   // function attributes and cluster occupancy are per device
   int dev_index = 0;
   cudaGetDevice(&dev_index);
@@ -826,15 +786,15 @@ int launch_nh(ClParams<SCORED, RESUME>& p, int B, int V1, int smem_cap, int* pla
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   if (st.max_clusters < 0 || smem > st.smem_set) {
-    if (cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED, RESUME>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-        cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED, RESUME>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
+    if (cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
+        cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
       cudaGetLastError();
       st.max_clusters = 0;
     } else {
       st.smem_set = smem;
       cfg.gridDim = dim3(kCl);
       int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, rnnt_cluster_kernel<NH, GLOB, SCORED, RESUME>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+      if (cudaOccupancyMaxActiveClusters(&n, rnnt_cluster_kernel<NH, GLOB, SCORED>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
       st.max_clusters = n;
     }
   }
@@ -852,7 +812,7 @@ int launch_nh(ClParams<SCORED, RESUME>& p, int B, int V1, int smem_cap, int* pla
     const int v[7] = {NH, GLOB ? 1 : 0, rows_smem, cls_per, nu, p.num_groups, nclusters};
     for (int i = 0; i < 7; ++i) plan[i] = v[i];
   }
-  if (cudaLaunchKernelEx(&cfg, rnnt_cluster_kernel<NH, GLOB, SCORED, RESUME>, p) != cudaSuccess) return -2;
+  if (cudaLaunchKernelEx(&cfg, rnnt_cluster_kernel<NH, GLOB, SCORED>, p) != cudaSuccess) return -2;
   return 0;
 }
 
@@ -867,72 +827,44 @@ extern "C" int gam_rnnt_debug_read(long long* out16) {
 // returns 0 on success, 1 if the shape is unsupported (pred_hidden != 320) or a 16-CTA cluster cannot be scheduled on
 // this device, negative on a launch error.  plan (host, 7 ints, or NULL) receives the launch that was chosen:
 // NH, GLOB, class rows per CTA in shared memory, classes per CTA, utterances per group, groups, clusters launched.
-// token_logp (or NULL: the unscored kernel) selects the scored instantiation, which also writes path_logp / path_rows.
-int launch_rnnt_greedy_cluster(const float* encproj, const int* len, const float* emb_gates, const float* whhT, const float* wpT,
-                               const float* bp, const float* wo, const float* bo, int B, int T, int H, int V1, int blank,
-                               int max_symbols, int max_out, int* ids, int* frames, int* counts, float* token_logp,
-                               float* path_logp, int* path_rows, int* plan, cudaStream_t s) {
+// io.token_logp (or NULL: the unscored kernel) selects the scored instantiation.
+int launch_rnnt_greedy(const float* encproj, const float* emb_gates, const float* whhT, const float* wpT, const float* bp,
+                       const float* wo, const float* bo, int B, int T, int H, int V1, int blank, int max_symbols, const GreedyIo& io,
+                       int* plan, cudaStream_t s) {
   if (H != kH) return 1;
-  static int smem_cap = 0, clusters_hint = 0;
-  if (smem_cap == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&smem_cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  struct DeviceLimits {
+    int smem_cap = 0, clusters_hint = 0;
+  };
+  static DeviceLimits per_device[64];
+  int dev = 0;
+  cudaGetDevice(&dev);
+  DeviceLimits& lim = per_device[dev & 63];
+  if (lim.smem_cap == 0) {
+    cudaDeviceGetAttribute(&lim.smem_cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     int sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    clusters_hint = sms / kCl - 2;   // GPCs rarely hold more than one 16-CTA cluster each (a 132-SM H100 has 7 or 8 GPCs)
-    if (clusters_hint < 1) clusters_hint = 1;
+    // GPCs rarely hold more than one 16-CTA cluster each (a 132-SM H100 has 7 or 8 GPCs)
+    lim.clusters_hint = sms / kCl - 2 < 1 ? 1 : sms / kCl - 2;
   }
-  RnntClScoredParams p;
-  p.encproj = encproj; p.len = len; p.emb_gates = emb_gates; p.whhT = whhT; p.wpT = wpT; p.bp = bp; p.wo = wo; p.bo = bo;
-  p.B = B; p.T = T; p.V1 = V1; p.blank = blank; p.max_symbols = max_symbols; p.max_out = max_out;
-  p.ids = ids; p.frames = frames; p.counts = counts;
-  p.token_logp = token_logp; p.path_logp = path_logp; p.path_rows = path_rows;
+  const bool scored = io.token_logp != nullptr;
+  if (scored && (!io.path_logp || !io.path_rows)) return -1;
+  RnntClParams p;
+  p.encproj = encproj; p.emb_gates = emb_gates; p.whhT = whhT; p.wpT = wpT; p.bp = bp; p.wo = wo; p.bo = bo;
+  p.B = B; p.T = T; p.V1 = V1; p.blank = blank; p.max_symbols = max_symbols;
+  p.io = io;
   // groups of up to 4 utterances while every group still gets its own cluster, else groups of up to 8
   const int cls_per = (V1 + kCl - 1) / kCl;
-  const bool small = B <= 4 * clusters_hint;
-  const bool scored = token_logp != nullptr;
-  if (scored && (!path_logp || !path_rows)) return -1;
+  const bool small = B <= 4 * lim.clusters_hint;
   const int fixed = (scored ? (small ? fixed_smem_bytes<1, true>() : fixed_smem_bytes<2, true>())
                             : (small ? fixed_smem_bytes<1, false>() : fixed_smem_bytes<2, false>())) + ((cls_per + 3) & ~3) * 4;
-  const bool glob = (smem_cap - fixed) / (kWoPitch * 4) < cls_per;   // some class rows have to stay in L2
+  const bool glob = (lim.smem_cap - fixed) / (kWoPitch * 4) < cls_per;   // some class rows have to stay in L2
+  const int cap = lim.smem_cap;
   if (scored) {
-    if (small) return glob ? launch_nh<1, true, true>(p, B, V1, smem_cap, plan, s) : launch_nh<1, false, true>(p, B, V1, smem_cap, plan, s);
-    return glob ? launch_nh<2, true, true>(p, B, V1, smem_cap, plan, s) : launch_nh<2, false, true>(p, B, V1, smem_cap, plan, s);
+    if (small) return glob ? launch_nh<1, true, true>(p, B, V1, cap, plan, s) : launch_nh<1, false, true>(p, B, V1, cap, plan, s);
+    return glob ? launch_nh<2, true, true>(p, B, V1, cap, plan, s) : launch_nh<2, false, true>(p, B, V1, cap, plan, s);
   }
-  RnntClParams& up = p;
-  if (small) return glob ? launch_nh<1, true, false>(up, B, V1, smem_cap, plan, s) : launch_nh<1, false, false>(up, B, V1, smem_cap, plan, s);
-  return glob ? launch_nh<2, true, false>(up, B, V1, smem_cap, plan, s) : launch_nh<2, false, false>(up, B, V1, smem_cap, plan, s);
-}
-
-// launch_rnnt_greedy_cluster resuming DecodeState records (kernels.h).  Groups of up to 4 utterances (NH = 1): a call decodes
-// a chunk of each stream, usually of one recording.
-int launch_rnnt_greedy_resume(const float* encproj, const int* lo, const int* hi, const int* frame_base, const float* emb_gates,
-                              const float* whhT, const float* wpT, const float* bp, const float* wo, const float* bo, int B, int T,
-                              int H, int V1, int blank, int max_symbols, int max_out, uint8_t* state, int64_t stride, int* ids,
-                              int* frames, int* counts, float* token_logp, float* path_logp, int* path_rows, double* frame_logp,
-                              int* frame_rows, int64_t frame_pitch, cudaStream_t s) {
-  if (H != kH) return 1;
-  static int smem_cap = 0;
-  if (smem_cap == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&smem_cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  }
-  RnntClResumeParams p;
-  p.encproj = encproj; p.len = nullptr; p.emb_gates = emb_gates; p.whhT = whhT; p.wpT = wpT; p.bp = bp; p.wo = wo; p.bo = bo;
-  p.B = B; p.T = T; p.V1 = V1; p.blank = blank; p.max_symbols = max_symbols; p.max_out = max_out;
-  p.ids = ids; p.frames = frames; p.counts = counts;
-  p.token_logp = token_logp; p.path_logp = path_logp; p.path_rows = path_rows;
-  p.lo = lo; p.hi = hi; p.frame_base = frame_base; p.state = state; p.stride = stride;
-  p.frame_logp = frame_logp; p.frame_rows = frame_rows; p.frame_pitch = frame_pitch;
-  const bool scored = token_logp != nullptr;
-  if (scored && (!path_logp || !path_rows || !frame_logp || !frame_rows)) return -1;
-  const int cls_per = (V1 + kCl - 1) / kCl;
-  const int fixed = (scored ? fixed_smem_bytes<1, true>() : fixed_smem_bytes<1, false>()) + ((cls_per + 3) & ~3) * 4;
-  const bool glob = (smem_cap - fixed) / (kWoPitch * 4) < cls_per;
-  if (scored) return glob ? launch_nh<1, true, true, true>(p, B, V1, smem_cap, nullptr, s) : launch_nh<1, false, true, true>(p, B, V1, smem_cap, nullptr, s);
-  return glob ? launch_nh<1, true, false, true>(p, B, V1, smem_cap, nullptr, s) : launch_nh<1, false, false, true>(p, B, V1, smem_cap, nullptr, s);
+  if (small) return glob ? launch_nh<1, true, false>(p, B, V1, cap, plan, s) : launch_nh<1, false, false>(p, B, V1, cap, plan, s);
+  return glob ? launch_nh<2, true, false>(p, B, V1, cap, plan, s) : launch_nh<2, false, false>(p, B, V1, cap, plan, s);
 }
 
 }  // namespace gam

@@ -5,9 +5,10 @@ gam_rnnt_greedy_resume, include/gigaam_b200.h), `longform.decode_windows`, the s
 The point of the resumable decoders is one invariant: an utterance decoded in consecutive ranges of frames, with the state
 carried on the device, gives one gam_*_greedy(_scored) call's ids, frames, counts, token log-probs and path scores bit for
 bit.  CPU: the segmentation rules, the refusals and the exported symbols.  GPU: the invariant for both heads (with chunk edges
-on pending RNN-T steps and on CTC repeats), truncation, the stitched encoder output, one window == transcribe, and flat
+on pending RNN-T steps and on CTC repeats, and for 32 RNN-T streams decoded in groups of 8), truncation, the stitched encoder output, one window == transcribe, and flat
 device memory.
 """
+import ctypes
 import math
 import random
 
@@ -223,6 +224,33 @@ def test_rnnt_resume_is_bit_identical(name, blank_shift):
             assert torch.equal(state.view(torch.int32)[:, 2].cpu(), want[2].cpu())          # the true count
     if blank_shift < -100:
         assert saw_pending, "no chunk edge fell on a pending LSTM step"
+
+
+@pytest.mark.gpu
+def test_rnnt_resume_of_many_streams_is_bit_identical():
+    """32 streams decode in groups of 8 (NH = 2), the width a one-shot call of that batch takes too; the folds do not depend
+    on the group width, so resuming them in random chunks still gives the one-shot bits."""
+    eng = _model("v3_e2e_rnnt", -4.0)._get_engine()
+    B, T, H, V1 = 32, 120, 320, eng.num_classes
+    # the launch plan of this batch, read with all lengths 0: NH (plan[0]) = 2
+    f32 = [torch.zeros(shape, device=_dev()) for shape in ((B, 1, H), (V1, 4 * H), (H, 4 * H), (H, H), (H,), (V1, H), (V1,))]
+    i32 = [torch.zeros(shape, dtype=torch.int32, device=_dev()) for shape in ((B,), (B, 1), (B, 1), (B,))]
+    plan = (ctypes.c_int32 * 7)()
+    rc = eng.lib.gam_test_rnnt_greedy(eng.handle, f32[0].data_ptr(), i32[0].data_ptr(), *[t.data_ptr() for t in f32[1:]], B, 1, V1, 1, 1,
+                                      *[t.data_ptr() for t in i32[1:]], ctypes.cast(plan, ctypes.c_void_p), eng._stream())
+    _lib.check(eng.lib, eng.handle, rc, "gam_test_rnnt_greedy")
+    assert plan[0] == 2, list(plan)
+    g = torch.Generator().manual_seed(32)
+    enc = (torch.randn(B, T, eng.d_model, generator=g) * 0.5).to(_dev())
+    rng = random.Random(32)
+    lens = [rng.randint(1, T) for _ in range(B)]
+    lens_d = torch.tensor(lens, dtype=torch.int32)
+    for scores in (False, True):
+        want = eng.greedy(enc, lens_d, scores=scores)
+        bounds = [_splits(rng, L, rng.choice([1, 2, 7, "random"])) for L in lens]
+        out, state, _ = _resume_all(eng, enc, lens, bounds, eng.hyp_width(T), scores)
+        _check_same(out, want, scores)
+        assert torch.equal(state.view(torch.int32)[:, 2].cpu(), want[2].cpu())
 
 
 @pytest.mark.gpu
