@@ -2,6 +2,7 @@
 // and the kernel sequence of the path.  No compute lives here and nothing here falls back to a CPU
 // or library implementation: every stage is one of the hand-written kernels in this directory.
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -956,6 +957,47 @@ int gam_test_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t
     return fail(h, -1, "test_ctc_align_long: cluster_ctas=%d outside [0, %d]", cluster_ctas, kAlignLongMaxCtas);
   return ctc_align_long_run(h, "test_ctc_align_long", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes,
                             frames, token_logp, viterbi_logp, log_likelihood, path_rows, cluster_ctas, plan, stream);
+}
+
+// ---- keyword spotting (csrc/spot.cu)
+static int ctc_spot_run(gam_handle* h, const char* what, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T,
+                        const int32_t* keywords, const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det,
+                        int32_t* det_start, int32_t* det_end, float* det_score, int32_t* det_count, int32_t warps, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 1) return fail(h, -1, "%s: model has no CTC head", what);
+  if (B <= 0 || B > 65535 || T <= 0) return fail(h, -1, "%s: bad sizes (B=%d, T=%d; B <= 65535)", what, B, T);
+  if (K < 1) return fail(h, -1, "%s: K=%d: at least one keyword is needed", what, K);
+  if (Umax < 1 || Umax > kSpotMaxTokens) return fail(h, -1, "%s: Umax=%d outside [1, %d] tokens per keyword", what, Umax, kSpotMaxTokens);
+  if (!(threshold > 0.f && threshold <= 1.f)) return fail(h, -1, "%s: threshold %g outside (0, 1]", what, static_cast<double>(threshold));
+  if (max_det < 1) return fail(h, -1, "%s: max_det=%d must be >= 1", what, max_det);
+  if (!log_probs || !enc_len || !keywords || !keyword_len || !det_start || !det_end || !det_score || !det_count)
+    return fail(h, -1, "%s: a required pointer is NULL", what);
+  const float log_theta = static_cast<float>(std::log(static_cast<double>(threshold)));   // correctly rounded to fp32
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  { PROF(PC_ALIGN);
+    rc = launch_ctc_spot(log_probs, enc_len, keywords, keyword_len, B, T, c.num_classes, K, Umax, log_theta, max_det, warps, det_start,
+                         det_end, det_score, det_count, s); }
+  if (rc == 1) return fail(h, -1, "%s: a frame of %d classes does not fit in shared memory", what, c.num_classes);
+  if (rc != 0) return fail(h, -4, "%s: launch rejected (rc=%d): %s", what, rc, cudaGetErrorString(cudaGetLastError()));
+  GAM_CHECK_LAUNCH(h, what);
+  return 0;
+}
+
+int gam_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
+                 const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det, int32_t* det_start,
+                 int32_t* det_end, float* det_score, int32_t* det_count, void* stream) {
+  return ctc_spot_run(h, "ctc_spot", log_probs, enc_len, B, T, keywords, keyword_len, K, Umax, threshold, max_det, det_start, det_end,
+                      det_score, det_count, 0, stream);
+}
+
+int gam_test_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
+                      const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det, int32_t* det_start,
+                      int32_t* det_end, float* det_score, int32_t* det_count, int32_t warps_per_cta, void* stream) {
+  if (warps_per_cta < 0 || warps_per_cta > kSpotMaxWarps)
+    return fail(h, -1, "test_ctc_spot: warps_per_cta=%d outside [0, %d]", warps_per_cta, kSpotMaxWarps);
+  return ctc_spot_run(h, "test_ctc_spot", log_probs, enc_len, B, T, keywords, keyword_len, K, Umax, threshold, max_det, det_start,
+                      det_end, det_score, det_count, warps_per_cta, stream);
 }
 
 int64_t gam_rnnt_align_scores_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {

@@ -158,6 +158,19 @@ int launch_ctc_align_long(const float* log_probs, const int* enc_len, const int*
                           int V1, int forced_ctas, uint32_t* bp, int* frames, float* token_logp, float* viterbi_logp,
                           float* log_likelihood, int* path_rows, int* plan, cudaStream_t s);
 
+// spot.cu: CTC keyword spotting (gam_ctc_spot), grid (ceil(K / warps), B), one warp per keyword of <= kSpotMaxTokens tokens.
+// keywords [K, Umax], keyword_len [K]; det_* [B, K, max_det], det_count [B, K].  log_theta = fp32 log of the threshold.
+// warps: keyword warps per CTA, 1..kSpotMaxWarps, or 0 for min(kSpotWarps, K).  The plan: frames per tile (rows) and the
+// dynamic shared memory of the ring.  Return 0, 1 when one tile of V1 classes does not fit in shared memory, negative on an
+// attribute error.
+constexpr int kSpotMaxTokens = 64;
+constexpr int kSpotWarps = 8;
+constexpr int kSpotMaxWarps = 32;
+int ctc_spot_plan(int V1, int* rows, int* smem_bytes);
+int launch_ctc_spot(const float* log_probs, const int* enc_len, const int* keywords, const int* keyword_len, int B, int T, int V1, int K,
+                    int Umax, float log_theta, int max_det, int warps, int* det_start, int* det_end, float* det_score, int* det_count,
+                    cudaStream_t s);
+
 // head_grads.cu: backward passes of the heads (fp32, deterministic, no atomics).  Rows are 64-bit.
 // dl = G - exp(logp) * rowsum(G), rows of V1
 void launch_softmax_grad(const float* G, const float* logp, float* dl, int64_t rows, int V1, cudaStream_t s);

@@ -134,3 +134,18 @@ def align(head, encoded: Tensor, encoded_len: Tensor, targets: Tensor, target_le
     dec, _, _ = eng.rnnt_predict(x, None, None)
     blank_lp, label_lp = eng.rnnt_align_scores(enc, dec, y)
     return eng.rnnt_align(blank_lp, label_lp, encoded_len, target_lengths)
+
+
+def spot(head, encoded: Tensor, encoded_len: Tensor, keywords: Tensor, keyword_len: Tensor, threshold: float, max_det: int
+         ) -> Tuple[Tensor, ...]:
+    """CTC keyword spotting (include/gigaam_b200.h, gam_ctc_spot).  encoded [B, d, T] (the encoder's output), encoded_len [B],
+    keywords [K, Umax] token ids in [0, V) (entries at or past keyword_len[k] are ignored), keyword_len [K] in [1, 64],
+    threshold in (0, 1] -> device tensors (start [B, K, max_det] i32, end [B, K, max_det] i32, score [B, K, max_det] f32,
+    count [B, K] i32): gam_ctc_log_probs, then gam_ctc_spot.  No host synchronisation: the call can be captured in a CUDA
+    graph.  RNN-T heads raise NotImplementedError: they have no frame posteriors without a lattice."""
+    eng = head._engine()
+    if eng.head_type != 1:
+        raise NotImplementedError("keyword spotting needs a CTC head: an RNN-T model has no per-frame posteriors without its "
+                                  "[T, U + 1] lattice; use a *_ctc model")
+    enc = _as_btd(encoded.to(device=eng.device, dtype=torch.float32))
+    return eng.ctc_spot(eng.ctc_log_probs(enc), encoded_len, keywords, keyword_len, threshold, max_det)

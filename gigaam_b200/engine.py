@@ -740,6 +740,30 @@ class Engine:
         _lib.check(self.lib, self.handle, rc, "gam_ctc_align_long")
         return outs
 
+    def ctc_spot(self, log_probs: Tensor, enc_len: Tensor, keywords: Tensor, keyword_len: Tensor, threshold: float, max_det: int,
+                 warps_per_cta: Optional[int] = None) -> Tuple[Tensor, ...]:
+        """log_probs [B, T, V+1] f32 contiguous (ctc_log_probs, or stitched windows), enc_len [B], keywords [K, Umax] token ids,
+        keyword_len [K] -> (start [B, K, max_det] i32, end [B, K, max_det] i32, score [B, K, max_det] f32, count [B, K] i32) on
+        the device (gam_ctc_spot).  `warps_per_cta` forces the keyword warps per CTA (gam_test_ctc_spot)."""
+        assert log_probs.is_cuda and log_probs.dtype == torch.float32 and log_probs.is_contiguous() and log_probs.dim() == 3
+        if self.head_type != 1:
+            raise RuntimeError("model has no CTC head")
+        B, T, _ = log_probs.shape
+        K, Umax = keywords.shape
+        enc_len, keywords, keyword_len = (self._i32(t, self.device) for t in (enc_len, keywords, keyword_len))
+        i32 = dict(dtype=torch.int32, device=self.device)
+        outs = (torch.empty((B, K, max_det), **i32), torch.empty((B, K, max_det), **i32),
+                torch.empty((B, K, max_det), dtype=torch.float32, device=self.device), torch.empty((B, K), **i32))
+        args = [log_probs.data_ptr(), enc_len.data_ptr(), B, T, keywords.data_ptr(), keyword_len.data_ptr(), K, Umax, float(threshold),
+                int(max_det), *[t.data_ptr() for t in outs]]
+        with torch.cuda.device(self.device):
+            if warps_per_cta is None:
+                rc = self.lib.gam_ctc_spot(self.handle, *args, self._stream())
+            else:
+                rc = self.lib.gam_test_ctc_spot(self.handle, *args, int(warps_per_cta), self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_ctc_spot")
+        return outs
+
     def rnnt_align_scores(self, enc: Tensor, dec: Tensor, targets: Tensor) -> Tuple[Tensor, Tensor]:
         """enc [B, T, d], dec [B, U+1, pred_hidden] f32 contiguous, targets [B, U] -> (blank, label) [B, T, U+1] f32: the
         entries of rnnt_joint's lattice that alignment reads (gam_rnnt_align_scores)."""

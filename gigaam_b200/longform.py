@@ -192,7 +192,8 @@ def window_batches(model, wav: Tensor, windows: Sequence[Window], batch_size: in
 
 
 def stitch_ctc_log_probs(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16) -> Tensor:
-    """CTC log-probs [1, T, V+1] f32 of a whole recording (wav [N] on the model's device, already in the model's dtype):
+    """CTC log-probs [1, T, V+1] f32 of a whole recording (wav [N] on the model's device or in pinned host memory, already in
+    the model's dtype):
     the windows are encoded by `window_batches`, `model.head` (gam_ctc_log_probs) gives each batch's log-probs, and each
     window's kept rows are copied into place.  Only one batch of window log-probs is alive at a time."""
     eng = model._get_engine()

@@ -17,11 +17,13 @@ from .decoding import CTCGreedyDecoding, RNNTGreedyDecoding, _as_btd
 from .encoder import ConformerEncoder
 from .engine import Engine
 from .preprocess import SAMPLE_RATE, FeatureExtractor, load_audio
-from .types import Alignment, LongformAlignment, TranscriptionResult, Word
+from .types import Alignment, Detection, LongformAlignment, TranscriptionResult, Word
 
 LONGFORM_THRESHOLD = 25 * SAMPLE_RATE
 ALIGN_MAX_TOKENS = 4096   # kAlignMaxTokens of csrc/kernels.h
 ALIGN_LONG_MAX_TOKENS = 65536   # kAlignLongMaxTokens of csrc/kernels.h
+SPOT_MAX_TOKENS = 64   # kSpotMaxTokens of csrc/kernels.h
+SPOT_FIRST_MAX_DET = 256   # spot(): detections kept per keyword by the first launch; a second one keeps them all
 
 _REGISTRY = {
     "FeatureExtractor": FeatureExtractor, "ConformerEncoder": ConformerEncoder, "CTCHead": CTCHead,
@@ -469,6 +471,126 @@ class GigaAMASR(GigaAM):
         segs = windowed_segments(self.decoding.tokenizer, ids, frames, cuts, shift, N / SAMPLE_RATE,
                                  words if word_timestamps else None, ws[:k], frame_logp, frame_rows)
         return LongformTranscriptionResult(segments=segs)
+
+    # ---- keyword spotting (INTEGRATION.md §7g)
+    def _refuse_rnnt_spot(self, what: str) -> None:
+        if self._ncfg["head"].get("type") == "rnnt":
+            raise NotImplementedError(f"{what} needs a CTC head: an RNN-T model has no per-frame posteriors without its "
+                                      "[T, U + 1] lattice, so there is nothing to search; use a *_ctc model")
+
+    def _keyword_ids(self, keywords: Sequence[Union[str, Sequence[int]]], threshold: float) -> Tuple[List[str], List[List[int]]]:
+        """Each keyword's text and token ids, checked before any device work: a string is normalised and tokenised by
+        `Tokenizer.encode` (as `align` does), a sequence of ids is taken as it is.  Raises ValueError for an empty list, a
+        keyword without tokens, more than 64 tokens, an id outside [0, V) and a threshold outside (0, 1] (in fp32)."""
+        tok = self.decoding.tokenizer
+        V = len(tok)
+        kws = [keywords] if isinstance(keywords, str) else list(keywords)
+        if not kws:
+            raise ValueError("spot: no keywords")
+        names, ids = [], []
+        for kw in kws:
+            if isinstance(kw, str):
+                row = tok.encode(kw)
+                if not row:
+                    raise ValueError(f"spot: keyword {kw!r} normalises to no tokens")
+                names.append(tok.normalize(kw))
+            else:
+                row = [int(i) for i in kw]
+                bad = [i for i in row if not 0 <= i < V]
+                if bad:
+                    raise ValueError(f"spot: token id {bad[0]} outside [0, {V})")
+                if not row:
+                    raise ValueError("spot: a keyword without tokens")
+                names.append(tok.decode(row))
+            if len(row) > SPOT_MAX_TOKENS:
+                raise ValueError(f"spot: keyword {names[-1]!r} has {len(row)} tokens, more than {SPOT_MAX_TOKENS}")
+            ids.append(row)
+        if not 0.0 < float(np.float32(threshold)) <= 1.0:
+            raise ValueError(f"spot: threshold={threshold} outside (0, 1]")
+        return names, ids
+
+    @staticmethod
+    def _keyword_tensors(ids: List[List[int]], device) -> Tuple[Tensor, Tensor]:
+        keywords = torch.zeros((len(ids), max(len(r) for r in ids)), dtype=torch.int32)
+        for k, row in enumerate(ids):
+            keywords[k, :len(row)] = torch.tensor(row, dtype=torch.int32)
+        return keywords.to(device), torch.tensor([len(r) for r in ids], dtype=torch.int32, device=device)
+
+    @staticmethod
+    def _detections(names: List[str], ids: List[List[int]], start: Tensor, end: Tensor, score: Tensor, count: Tensor,
+                    frame_shift: float) -> List[Detection]:
+        """Host copies of one recording's gam_ctc_spot outputs -> its stored detections, sorted by start, then keyword."""
+        out = []
+        n = count.clamp(max=start.shape[1]).tolist()
+        for k, name in enumerate(names):
+            U = len(ids[k])
+            for s, e, sc in zip(start[k, :n[k]].tolist(), end[k, :n[k]].tolist(), score[k, :n[k]].tolist()):
+                out.append((s, k, Detection(keyword=name, keyword_index=k, start=s * frame_shift, end=e * frame_shift, score=sc,
+                                            confidence=math.exp(sc / U))))
+        out.sort(key=lambda d: d[:2])
+        return [d for _, _, d in out]
+
+    @torch.inference_mode()
+    def spot_batch(self, wav: Tensor, lengths: Tensor, keywords: Sequence[Union[str, Sequence[int]]], threshold: float = 0.5,
+                   max_det: int = 64) -> List[List[Detection]]:
+        """Spot every keyword in every recording wav[b, :lengths[b]] of a batch the model encodes in one pass (up to
+        max_encoded_frames).  Returns one list per recording, sorted by start, then keyword index; at most `max_det`
+        detections of each keyword are kept (the first ones in time).  Keywords are strings (normalised and tokenised as
+        `align` does) or sequences of token ids, up to 64 tokens; `threshold` in (0, 1] is the lowest per-token likelihood
+        ratio to greedy decoding that is reported (INTEGRATION.md §7g).  RNN-T models raise NotImplementedError; the keyword,
+        threshold and batch checks raise ValueError, all before any device work."""
+        from .decoding import spot
+        from .timestamps_utils import compute_frame_shift
+        self._refuse_rnnt_spot("spot_batch")
+        names, ids = self._keyword_ids(keywords, threshold)
+        if max_det < 1:
+            raise ValueError(f"spot_batch: max_det={max_det} must be >= 1")
+        B = int(wav.shape[0]) if wav.dim() == 2 else 0
+        if B == 0:
+            raise ValueError("spot_batch: empty batch")
+        encoded, encoded_len = self.forward(wav, lengths)
+        kw, kw_len = self._keyword_tensors(ids, encoded.device)
+        start, end, score, count = (t.cpu() for t in spot(self.head, encoded, encoded_len, kw, kw_len, threshold, max_det))
+        enc_len, wav_len = encoded_len.cpu().tolist(), lengths.cpu().tolist()
+        return [self._detections(names, ids, start[b], end[b], score[b], count[b],
+                                 compute_frame_shift(int(wav_len[b]), int(enc_len[b])) if enc_len[b] > 0 else 0.0)
+                for b in range(B)]
+
+    @torch.inference_mode()
+    def spot(self, wav_file, keywords: Sequence[Union[str, Sequence[int]]], threshold: float = 0.5, window: float = 30.0,
+             overlap: float = 4.0, batch_size: int = 16) -> List[Detection]:
+        """Spot keywords in a recording of any length (INTEGRATION.md §7g): the CTC log-probs of the overlapping windows of
+        `align_longform` are stitched into one sequence and gam_ctc_spot searches it for every keyword at once.  Returns
+        every detection, sorted by start, then keyword index.  Keywords and threshold as in `spot_batch`.  CTC models only:
+        RNN-T raises NotImplementedError.  Raises ValueError before any device work for the keyword and threshold checks,
+        batch_size < 1 and the window plan's refusals (longform.plan_windows)."""
+        from .longform import plan_windows, stitch_ctc_log_probs
+        from .timestamps_utils import compute_frame_shift
+        self._refuse_rnnt_spot("spot")
+        names, ids = self._keyword_ids(keywords, threshold)
+        if isinstance(wav_file, str):
+            wav = load_audio(wav_file)
+        else:
+            wav = torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1)
+        max_frames = self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
+        windows, T = plan_windows(wav.numel(), window, overlap, self._encoded_length, max_frames)
+        if batch_size < 1:
+            raise ValueError("batch_size must be >= 1")
+        N = wav.numel()
+        host = wav.to(self._dtype).pin_memory()          # the rounding of prepare_wav; uploaded one batch at a time
+        lp = stitch_ctc_log_probs(self, host, windows, T, batch_size)
+        eng = self._get_engine()
+        kw, kw_len = self._keyword_tensors(ids, eng.device)
+        enc_len = torch.tensor([T], dtype=torch.int32, device=eng.device)
+        # detections of one keyword do not overlap and span >= U frames each: T // U bounds the count
+        max_det = max(1, min(T // min(len(r) for r in ids), SPOT_FIRST_MAX_DET))
+        out = eng.ctc_spot(lp, enc_len, kw, kw_len, threshold, max_det)
+        most = int(out[3].max())
+        if most > max_det:
+            out = eng.ctc_spot(lp, enc_len, kw, kw_len, threshold, most)
+        del lp
+        start, end, score, count = (t[0].cpu() for t in out)
+        return self._detections(names, ids, start, end, score, count, compute_frame_shift(N, T))
 
     @torch.inference_mode()
     def transcribe_batch(self, wav: Tensor, lengths: Tensor) -> List[str]:

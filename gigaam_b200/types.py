@@ -95,6 +95,20 @@ class Alignment(_Record):
         return self.text
 
 
+class Detection(_Record):
+    """One keyword detection of `spot()` / `spot_batch()`: `keyword` (its normalised text, or the decoded ids) and its index in
+    the list asked for, start / end in seconds (end exclusive: one frame after the first frame of the keyword's last token),
+    `score` = log p(keyword path) - log p(greedy path) over the same frames (<= 0) and `confidence` = exp(score / tokens), the
+    per-token likelihood ratio to the greedy decoder, 1.0 exactly where greedy decoding writes the keyword."""
+    __slots__ = _fields = ("keyword", "keyword_index", "start", "end", "score", "confidence")
+    keyword: str
+    keyword_index: int
+    start: float
+    end: float
+    score: float
+    confidence: float
+
+
 class LongformAlignment(_Record):
     """`align_longform()` result: one `Segment` per input line, in order (its normalised text, the start of its first token's
     frame and the end of its last, its words, and `confidence` = exp(mean log-probability of its tokens)), plus the

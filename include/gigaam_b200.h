@@ -315,6 +315,48 @@ int64_t gam_ctc_align_long_workspace_bytes(const gam_handle* h, int32_t B, int32
 int gam_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets, const int32_t* target_len,
                        int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
                        float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream);
+/* ---- CTC keyword spotting: where in a recording each of K keywords was said, and how sure that is.  One exact Viterbi
+ * per (recording, keyword) over the caller's fp32 log-probs; no hypothesis search.
+ *
+ * Recording b has lp[t, c] = log_probs[b, t, c], t < T_b = clamp(enc_len[b], 0, T); blank = V (V + 1 = num_classes).
+ * Keyword k has tokens y_1..y_U, U = keyword_len[k], 1 <= U <= Umax <= 64, ids in [0, V) (keywords [k, i - 1] = y_i).
+ *   States: y_1, blank, y_2, blank, ..., y_U, so S = 2U - 1; even s is token y_{s/2+1}, odd s the blank between two tokens,
+ *     l_s its label.  There is no leading or trailing blank: a keyword starts on its first token and ends on its last.
+ *   Transitions: state s is entered from s and from s - 1; an even s >= 2 also from s - 2 when y_{s/2+1} != y_{s/2} (a
+ *     repeated token needs the blank between its two copies, so U = 1 and repeats have no skip).
+ *   Cost: m[t] = max_c lp[t, c], exact (a zero max is +0); c(t, s) = lp[t, l_s] - m[t], one fp32 subtraction, <= 0, and 0 on
+ *     the state whose label the greedy decoder picks at t.
+ *   Recursion, fp32, one add per value, v(-1, s) = -inf:
+ *     v(t, 0) = c(t, 0) + max(v(t-1, 0), 0): the path continues, or a fresh one starts at t (only when 0 > v(t-1, 0)
+ *       strictly: on a tie the path continues, which keeps the earlier start);
+ *     v(t, s > 0) = c(t, s) + the max over the predecessors, taken in the order s, s - 1, s - 2 with a later candidate
+ *       replacing the current one only when strictly greater.
+ *     Every state carries the start frame of its best path (the frame its fresh start was taken).
+ *   NaN frames: a frame whose row lp[t, 0..V] holds a NaN is a barrier: v(t, s) = -inf for every s, so no path crosses it.
+ *     (Infinite entries are not special: the arithmetic above applies as written.)
+ *   End score: E(t) = v(t, S - 1), the best path that ends on y_U at t, with start frame a(t).  E(t) = log p(keyword path) -
+ *     log p(best unconstrained path) over frames [a(t), t]; exp(E / U) is the per-token likelihood ratio to greedy, 1.0
+ *     exactly where the greedy decoder writes the keyword.
+ *   Detections: tau = fp32(U) * fp32(log threshold) (the log rounded once to fp32, computed on the host); frames t < T_b are
+ *     scanned in order, and each with E(t) >= tau (so never a NaN or -inf one) is a candidate [a(t), t + 1) with score E(t).
+ *     A candidate that overlaps the pending detection (a(t) < its end) replaces it only when its score is strictly greater,
+ *     so ties keep the earlier end; a candidate that does not overlap emits the pending detection and becomes pending; the
+ *     last pending detection is emitted after frame T_b - 1.  A greedy word thus spans [first frame of its first token's run,
+ *     first frame of its last token's run + 1), the gam_group_words convention.
+ *   T_b = 0, or a keyword longer than the frames that can hold it, gives no detection.
+ * Outputs, per (b, k) at row (b K + k) of pitch max_det, in time order: det_start / det_end [B, K, max_det] i32 (frames,
+ *   end exclusive), det_score [B, K, max_det] f32 (E), det_count [B, K] i32.  det_count is the true count even when it exceeds
+ *   max_det; only the first max_det detections are stored, and entries past the stored ones are -1 / -1 / -inf.  A keyword
+ *   with an id outside [0, V) or a length outside [1, Umax] gets count 0 and -1 / -1 / NaN in every entry; the call succeeds.
+ * Refused (gam_last_error): a handle without a CTC head, B outside [1, 65535], T < 1, K < 1, Umax outside [1, 64], a
+ *   threshold outside (0, 1] or NaN, max_det < 1, and a num_classes whose frame does not fit in shared memory.
+ * All pointers are device memory; log_probs [B, T, V+1] (gam_ctc_log_probs, or stitched windows), enc_len [B], keywords
+ * [K, Umax] i32, keyword_len [K] i32.  Fixed orders, no atomics: a (recording, keyword) pair's outputs are bit-identical
+ * whatever else is in the batch and in whatever order the keywords come.  No workspace, no host synchronisation,
+ * capturable in a CUDA graph.  T is bounded only by int32 (not by max_encoded_frames). */
+int gam_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
+                 const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det, int32_t* det_start,
+                 int32_t* det_end, float* det_score, int32_t* det_count, void* stream);
 /* RNN-T stage 1: enc [B, T, d_model], dec [B, U+1, pred_hidden] (gam_rnnt_predict over cat[blank, y]), targets [B, U] i32
  *   -> blank [B, T, U+1], label [B, T, U+1]: bit-identical to the matching entries of gam_rnnt_joint's lattice for the same
  *   enc / dec, but no [.., V+1] row is ever stored.  label is -inf at u = U and NaN where targets[b, u] is outside [0, V) (so
@@ -485,6 +527,11 @@ int gam_test_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t
                             const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes,
                             int32_t* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int32_t* path_rows,
                             int32_t cluster_ctas, int32_t* plan, void* stream);
+/* gam_ctc_spot with the keyword warps per CTA forced to warps_per_cta in [1, 32] (0: the library's choice); the outputs do
+ * not depend on it. */
+int gam_test_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
+                      const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det, int32_t* det_start,
+                      int32_t* det_end, float* det_score, int32_t* det_count, int32_t warps_per_cta, void* stream);
 /* qkv: f16 [B*T, 3*d_model]; klen i32 [B] or NULL -> out f16 [B*T, d_model].  T up to the handle's max_encoded_frames */
 int gam_test_attention(gam_handle* h, const void* qkv, const int32_t* klen, void* out, int32_t B, int32_t T, void* stream);
 /* rel_pos variant: qkv f16 [B*T, 4*d_model] = [q+u | q+v | k | v]; pos f16 [2*max-1, d_model] laid out like pos_proj
