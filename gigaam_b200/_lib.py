@@ -65,7 +65,7 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_ctc_align", "gam_rnnt_align_scores_workspace_bytes", "gam_rnnt_align_scores", "gam_rnnt_align_workspace_bytes",
            "gam_rnnt_align", "gam_ctc_align_long_workspace_bytes", "gam_ctc_align_long", "gam_test_ctc_align_long",
            "gam_decode_state_bytes", "gam_decode_state_init", "gam_decode_resume_workspace_bytes", "gam_ctc_greedy_resume",
-           "gam_rnnt_greedy_resume", "gam_ctc_spot", "gam_test_ctc_spot")
+           "gam_rnnt_greedy_resume", "gam_ctc_spot", "gam_test_ctc_spot", "gam_ctc_bias_workspace_bytes", "gam_ctc_bias")
 
 
 def lib_path() -> Path:
@@ -166,6 +166,11 @@ def load() -> C.CDLL:
     lib.gam_test_ctc_spot.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32, C.c_float, i32] + [c_vp] * 4 + [i32, c_vp]
     for fn in (lib.gam_ctc_spot, lib.gam_test_ctc_spot):
         fn.restype = C.c_int
+    lib.gam_ctc_bias_workspace_bytes.argtypes = [H, i32, i32, i32, i32]
+    lib.gam_ctc_bias_workspace_bytes.restype = i64
+    lib.gam_ctc_bias.argtypes = ([H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32] + [c_vp] * 4 + [i32, C.c_float, c_vp, i32] + [c_vp] * 3
+                                 + [i32] + [c_vp] * 3 + [i64, c_vp, i64] + [c_vp] * 7)
+    lib.gam_ctc_bias.restype = C.c_int
     lib.gam_emo_workspace_bytes.argtypes = [H, i32, i32]
     lib.gam_emo_workspace_bytes.restype = i64
     lib.gam_emo_head.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, i64, c_vp, c_vp, c_vp, c_vp]

@@ -1000,6 +1000,84 @@ int gam_test_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_
                       det_end, det_score, det_count, warps_per_cta, stream);
 }
 
+// ---- hotwords (csrc/bias.cu)
+int64_t gam_ctc_bias_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t K, int32_t max_det) {
+  if (!h || h->cfg.head != 1 || B <= 0 || B > 65535 || T <= 0 || K < 1 || max_det < 1) return -1;
+  const int64_t words = ctc_bias_workspace_words(T, K, max_det);
+  if (words < 0 || words > (int64_t(1) << 40) / B) return -1;
+  return align_up(static_cast<int64_t>(B) * words * 4, 1024);
+}
+
+int gam_ctc_bias(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
+                 const int32_t* keyword_len, int32_t K, int32_t Umax, const int32_t* det_start, const int32_t* det_end,
+                 const float* det_score, const int32_t* det_count, int32_t max_det, float threshold, const uint8_t* token_flags,
+                 int32_t V, const int32_t* ids, const int32_t* frames, const int32_t* counts, int32_t max_out, const float* token_logp,
+                 const float* path_logp, double* frame_logp, int64_t frame_pitch, void* workspace, int64_t workspace_bytes,
+                 int32_t* out_ids, int32_t* out_frames, int32_t* out_counts, int32_t* out_source, float* out_token_logp,
+                 float* out_path_logp, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 1) return fail(h, -1, "ctc_bias: model has no CTC head");
+  if (B <= 0 || B > 65535 || T <= 0) return fail(h, -1, "ctc_bias: bad sizes (B=%d, T=%d; B <= 65535)", B, T);
+  if (K < 1) return fail(h, -1, "ctc_bias: K=%d: at least one keyword is needed", K);
+  if (Umax < 1 || Umax > kSpotMaxTokens) return fail(h, -1, "ctc_bias: Umax=%d outside [1, %d] tokens per keyword", Umax, kSpotMaxTokens);
+  if (!(threshold > 0.f && threshold <= 1.f)) return fail(h, -1, "ctc_bias: threshold %g outside (0, 1]", static_cast<double>(threshold));
+  if (max_det < 1) return fail(h, -1, "ctc_bias: max_det=%d must be >= 1", max_det);
+  if (max_out < T) return fail(h, -1, "ctc_bias: max_out=%d is less than T=%d", max_out, T);
+  if (!token_flags || V != c.num_classes - 1)
+    return fail(h, -1, "ctc_bias: the token flag table is missing or has %d entries, not %d", V, c.num_classes - 1);
+  if (!log_probs || !enc_len || !keywords || !keyword_len || !det_start || !det_end || !det_score || !det_count || !ids || !frames ||
+      !counts || !out_ids || !out_frames || !out_counts || !out_source)
+    return fail(h, -1, "ctc_bias: a required pointer is NULL");
+  if (!token_logp != !out_token_logp || !path_logp != !out_path_logp)
+    return fail(h, -1, "ctc_bias: token_logp / path_logp and their outputs go together");
+  if (frame_logp && frame_pitch < T) return fail(h, -1, "ctc_bias: frame_pitch=%lld is less than T=%d", (long long)frame_pitch, T);
+  int rows = 0, smem = 0;
+  if (ctc_spot_plan(c.num_classes, &rows, &smem) == 1)
+    return fail(h, -1, "ctc_bias: a frame of %d classes does not fit in shared memory", c.num_classes);
+  const int64_t need = gam_ctc_bias_workspace_bytes(h, B, T, K, max_det);
+  if (need < 0) return fail(h, -1, "ctc_bias: K=%d x max_det=%d candidates are too many", K, max_det);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "ctc_bias: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  BiasArgs a{};
+  a.log_probs = log_probs;
+  a.enc_len = enc_len;
+  a.keywords = keywords;
+  a.keyword_len = keyword_len;
+  a.det_start = det_start;
+  a.det_end = det_end;
+  a.det_score = det_score;
+  a.det_count = det_count;
+  a.flags = token_flags;
+  a.ids = ids;
+  a.frames = frames;
+  a.counts = counts;
+  a.token_logp = token_logp;
+  a.path_logp = path_logp;
+  a.frame_logp = frame_logp;
+  a.frame_pitch = frame_pitch;
+  a.B = B;
+  a.T = T;
+  a.V1 = c.num_classes;
+  a.K = K;
+  a.Umax = Umax;
+  a.max_det = max_det;
+  a.max_out = max_out;
+  a.log_theta = static_cast<float>(std::log(static_cast<double>(threshold)));   // spot's rounding
+  a.out_ids = out_ids;
+  a.out_frames = out_frames;
+  a.out_counts = out_counts;
+  a.out_source = out_source;
+  a.out_token_logp = out_token_logp;
+  a.out_path_logp = out_path_logp;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  for (int stage = 0; stage < 3; ++stage) {
+    PROF(PC_ALIGN);
+    launch_ctc_bias(a, static_cast<int32_t*>(workspace), stage, s);
+  }
+  GAM_CHECK_LAUNCH(h, "ctc_bias");
+  return 0;
+}
+
 int64_t gam_rnnt_align_scores_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
   if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || T > h->max_t || U < 0 || U > kAlignMaxTokens) return -1;
   return gam_rnnt_joint_workspace_bytes(h, B, T, U + 1);

@@ -171,6 +171,39 @@ int launch_ctc_spot(const float* log_probs, const int* enc_len, const int* keywo
                     int Umax, float log_theta, int max_det, int warps, int* det_start, int* det_end, float* det_score, int* det_count,
                     cudaStream_t s);
 
+// bias.cu: hotwords spliced into CTC greedy output (gam_ctc_bias), three launches in stage order 0, 1, 2: select (one CTA per
+// recording), trace (kBiasTraceCtas x 4 warps per recording) and compact (one CTA per recording).  ctc_bias_workspace_words is the workspace of
+// one recording in 32-bit words (a multiple of 4), or -1 when it does not fit in int64.
+struct BiasArgs {
+  const float* log_probs;
+  const int* enc_len;
+  const int* keywords;
+  const int* keyword_len;
+  const int* det_start;
+  const int* det_end;
+  const float* det_score;
+  const int* det_count;
+  const unsigned char* flags;
+  const int* ids;
+  const int* frames;
+  const int* counts;
+  const float* token_logp;   // nullable, with out_token_logp
+  const float* path_logp;    // nullable, with out_path_logp
+  double* frame_logp;        // nullable, adjusted in place, row pitch frame_pitch
+  int64_t frame_pitch;
+  int B, T, V1, K, Umax, max_det, max_out;
+  float log_theta;
+  int* out_ids;
+  int* out_frames;
+  int* out_counts;
+  int* out_source;
+  float* out_token_logp;
+  float* out_path_logp;
+};
+constexpr int kBiasTraceCtas = 32;
+int64_t ctc_bias_workspace_words(int T, int K, int max_det);
+void launch_ctc_bias(const BiasArgs& a, int32_t* workspace, int stage, cudaStream_t s);
+
 // head_grads.cu: backward passes of the heads (fp32, deterministic, no atomics).  Rows are 64-bit.
 // dl = G - exp(logp) * rowsum(G), rows of V1
 void launch_softmax_grad(const float* G, const float* logp, float* dl, int64_t rows, int V1, cudaStream_t s);

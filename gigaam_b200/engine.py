@@ -764,6 +764,52 @@ class Engine:
         _lib.check(self.lib, self.handle, rc, "gam_ctc_spot")
         return outs
 
+    def ctc_bias(self, log_probs: Tensor, enc_len: Tensor, keywords: Tensor, keyword_len: Tensor, spotted: Tuple[Tensor, ...],
+                 threshold: float, token_flags: Tensor, ids: Tensor, frames: Tensor, counts: Tensor,
+                 token_logp: Optional[Tensor] = None, path_logp: Optional[Tensor] = None, frame_logp: Optional[Tensor] = None
+                 ) -> Tuple[Tensor, ...]:
+        """Hotwords (gam_ctc_bias): the detections `spotted` = ctc_spot(log_probs, enc_len, keywords, keyword_len, threshold,
+        max_det) replace the greedy words they outscore in ids / frames [B, max_out], counts [B] (greedy).  -> (ids, frames
+        [B, max_out] i32, counts [B] i32, source [B, max_out] i32, token_logp [B, max_out] f32 or None, path_logp [B] f32 or
+        None); the scores are returned when token_logp / path_logp are given.  frame_logp (f64 [B, pitch], greedy_resume's
+        per-frame sums) is adjusted in place."""
+        assert log_probs.is_cuda and log_probs.dtype == torch.float32 and log_probs.is_contiguous() and log_probs.dim() == 3
+        if self.head_type != 1:
+            raise RuntimeError("model has no CTC head")
+        B, T, _ = log_probs.shape
+        K, Umax = keywords.shape
+        max_out = ids.shape[1]
+        max_det = spotted[0].shape[2]
+        nbytes = int(self.lib.gam_ctc_bias_workspace_bytes(self.handle, B, T, K, max_det))
+        if nbytes < 0:
+            raise ValueError(f"ctc_bias: bad sizes B={B}, T={T}, K={K}, max_det={max_det}")
+        ws = self._ws_align.get(("bias", B, T, K, max_det), nbytes, self.device)
+        enc_len, keywords, keyword_len, ids, frames, counts = (self._i32(t, self.device)
+                                                               for t in (enc_len, keywords, keyword_len, ids, frames, counts))
+        flags = token_flags.to(device=self.device, dtype=torch.uint8).contiguous()
+        for t in spotted:
+            assert t.is_cuda and t.is_contiguous()
+        for t in (token_logp, path_logp):
+            assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous())
+        assert frame_logp is None or (frame_logp.dtype == torch.float64 and frame_logp.is_contiguous() and frame_logp.dim() == 2)
+        i32 = dict(dtype=torch.int32, device=self.device)
+        out = [torch.empty((B, max_out), **i32), torch.empty((B, max_out), **i32), torch.empty((B,), **i32),
+               torch.empty((B, max_out), **i32),
+               None if token_logp is None else torch.empty((B, max_out), dtype=torch.float32, device=self.device),
+               None if path_logp is None else torch.empty((B,), dtype=torch.float32, device=self.device)]
+
+        def ptr(t):
+            return None if t is None else t.data_ptr()
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_ctc_bias(self.handle, log_probs.data_ptr(), enc_len.data_ptr(), B, T, keywords.data_ptr(),
+                                       keyword_len.data_ptr(), K, Umax, *[t.data_ptr() for t in spotted], max_det, float(threshold),
+                                       flags.data_ptr(), flags.numel(), ids.data_ptr(), frames.data_ptr(), counts.data_ptr(), max_out,
+                                       ptr(token_logp), ptr(path_logp), ptr(frame_logp),
+                                       0 if frame_logp is None else frame_logp.shape[1], ws.data_ptr(), ws.numel(),
+                                       *[ptr(t) for t in out], self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_ctc_bias")
+        return tuple(out)
+
     def rnnt_align_scores(self, enc: Tensor, dec: Tensor, targets: Tensor) -> Tuple[Tensor, Tensor]:
         """enc [B, T, d], dec [B, U+1, pred_hidden] f32 contiguous, targets [B, U] -> (blank, label) [B, T, U+1] f32: the
         entries of rnnt_joint's lattice that alignment reads (gam_rnnt_align_scores)."""

@@ -207,12 +207,15 @@ def stitch_ctc_log_probs(model, wav: Tensor, windows: Sequence[Window], T: int, 
     return out
 
 
-def decode_windows(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16, scores: bool = False):
+def decode_windows(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16, scores: bool = False,
+                   log_probs: Optional[Tensor] = None):
     """Greedy-decode a whole recording of T encoder frames as one utterance: `window_batches` encodes the windows, and each
     window's kept frames are decoded in window order, resuming the previous window's decoder state on the device
     (Engine.greedy_resume).  Only one batch of encoder output is alive at a time.  Returns the Engine.DecodeBuffers of the
     one stream: ids / frames [1, max_out] (global frames), counts [1] and, with `scores`, token_logp, path_logp, path_rows and
-    the per-frame frame_logp / frame_rows [1, T].  max_out = Engine.hyp_width(T), so the buffers never overflow."""
+    the per-frame frame_logp / frame_rows [1, T].  max_out = Engine.hyp_width(T), so the buffers never overflow.
+    `log_probs` (CTC, f32 [1, T, V+1] on the device): also filled with the stitched log-probs of `stitch_ctc_log_probs`,
+    from the same encoder pass."""
     from .decoding import _as_btd
     eng = model._get_engine()
     index = {w: i for i, w in enumerate(windows)}
@@ -226,6 +229,11 @@ def decode_windows(model, wav: Tensor, windows: Sequence[Window], T: int, batch_
         for row, w in enumerate(group):
             i = index[w]
             eng.greedy_resume(enc[row:row + 1], ranges[0, i:i + 1], ranges[1, i:i + 1], ranges[2, i:i + 1], state, out, scores)
+        if log_probs is not None:
+            lp = model.head(encoded)
+            for row, w in enumerate(group):
+                log_probs[0, w.keep_start:w.keep_end] = lp[row, w.keep_start - first[index[w]]:w.keep_end - first[index[w]]]
+            del lp
         del enc, encoded
     return out
 

@@ -268,9 +268,15 @@ class GigaAMASR(GigaAM):
         return self.head(encoded), encoded_len
 
     @torch.inference_mode()
-    def transcribe(self, wav_file, word_timestamps: bool = False, confidence: bool = False) -> TranscriptionResult:
+    def transcribe(self, wav_file, word_timestamps: bool = False, confidence: bool = False,
+                   hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None, hotword_threshold: float = 0.5
+                   ) -> TranscriptionResult:
         """gigaam/model.py:126-140.  `confidence=True` decodes with the scored kernels (the same text and words) and fills
-        `confidence` of the result, and of every word when word timestamps are on (INTEGRATION.md, "Confidence")."""
+        `confidence` of the result, and of every word when word timestamps are on (INTEGRATION.md, "Confidence").
+        `hotwords` (CTC models only): names or terms that replace the greedy words they outscore by `hotword_threshold`
+        (INTEGRATION.md §7h); None decodes exactly as without them."""
+        if hotwords is not None:
+            return self._transcribe_hotwords(wav_file, word_timestamps, confidence, hotwords, hotword_threshold)
         wav, length = self.prepare_wav(wav_file)
         if length.item() > LONGFORM_THRESHOLD:
             raise ValueError("Too long wav file, use 'transcribe_longform' method.")
@@ -430,7 +436,8 @@ class GigaAMASR(GigaAM):
 
     @torch.inference_mode()
     def transcribe_windowed(self, wav_file, word_timestamps: bool = False, confidence: bool = False, window: float = 30.0,
-                            overlap: float = 4.0, batch_size: int = 16, pause: float = 1.0, max_segment: float = 25.0):
+                            overlap: float = 4.0, batch_size: int = 16, pause: float = 1.0, max_segment: float = 25.0,
+                            hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None, hotword_threshold: float = 0.5):
         """Transcribe a recording of any length without a VAD (INTEGRATION.md §7f).  The encoder runs over overlapping
         windows (`longform.plan_windows`), and the greedy decoder runs over the windows' kept frames as ONE utterance: each
         window is decoded as soon as its batch is encoded, resuming the decoder state of the window before it
@@ -438,10 +445,13 @@ class GigaAMASR(GigaAM):
         are cut afterwards between words (`longform.segment_cuts`: at pauses of at least `pause` seconds, then inside
         segments longer than `max_segment` seconds).  Returns a LongformTranscriptionResult whose segments tile the
         recording.  Raises ValueError before any device work for the window plan's refusals, batch_size < 1, pause < 0 and
-        max_segment <= 0."""
+        max_segment <= 0.  `hotwords` as in `transcribe` (CTC models only): the windows' log-probs are also stitched into one
+        [T, V+1] sequence from the same encoder pass, and the hotwords are applied to the whole recording before it is cut into
+        segments."""
         from .longform import decode_windows, plan_windows, segment_cuts, windowed_segments
         from .timestamps_utils import compute_frame_shift, words_from_device
         from .types import LongformTranscriptionResult
+        kw_ids = None if hotwords is None else self._hotword_ids(hotwords, hotword_threshold, "transcribe_windowed")
         if isinstance(wav_file, str):
             wav = load_audio(wav_file)
         else:
@@ -457,7 +467,17 @@ class GigaAMASR(GigaAM):
         N = wav.numel()
         host = wav.to(self._dtype).pin_memory()          # the rounding of prepare_wav; uploaded one batch at a time
         eng = self._get_engine()
-        out = decode_windows(self, host, windows, T, batch_size, confidence)
+        if kw_ids is None:
+            out = decode_windows(self, host, windows, T, batch_size, confidence)
+        else:
+            lp = torch.empty((1, T, eng.num_classes), dtype=torch.float32, device=eng.device)
+            out = decode_windows(self, host, windows, T, batch_size, confidence, log_probs=lp)
+            enc_len = torch.tensor([T], dtype=torch.int32, device=eng.device)
+            b_ids, b_frames, b_counts, _, b_logp, b_path = self._apply_hotwords(
+                lp, enc_len, kw_ids, hotword_threshold, out.ids, out.frames, out.counts, out.token_logp, out.path_logp,
+                out.frame_logp)
+            del lp
+            out = out._replace(ids=b_ids, frames=b_frames, counts=b_counts, token_logp=b_logp, path_logp=b_path)
         rec = eng.group_words(out.ids, out.frames, out.counts, self._word_flags())
         n = int(out.counts[0])
         ids, frames = out.ids[0, :n].tolist(), out.frames[0, :n].tolist()
@@ -582,15 +602,72 @@ class GigaAMASR(GigaAM):
         eng = self._get_engine()
         kw, kw_len = self._keyword_tensors(ids, eng.device)
         enc_len = torch.tensor([T], dtype=torch.int32, device=eng.device)
+        out = self._spot_all(lp, enc_len, kw, kw_len, ids, threshold)
+        del lp
+        start, end, score, count = (t[0].cpu() for t in out)
+        return self._detections(names, ids, start, end, score, count, compute_frame_shift(N, T))
+
+    def _spot_all(self, lp: Tensor, enc_len: Tensor, kw: Tensor, kw_len: Tensor, ids: List[List[int]], threshold: float
+                  ) -> Tuple[Tensor, ...]:
+        """gam_ctc_spot over log-probs [B, T, V+1] keeping every detection: a first launch keeps up to SPOT_FIRST_MAX_DET per
+        keyword, and one more with the largest count runs only when a count exceeds that."""
+        eng = self._get_engine()
         # detections of one keyword do not overlap and span >= U frames each: T // U bounds the count
-        max_det = max(1, min(T // min(len(r) for r in ids), SPOT_FIRST_MAX_DET))
+        max_det = max(1, min(lp.shape[1] // min(len(r) for r in ids), SPOT_FIRST_MAX_DET))
         out = eng.ctc_spot(lp, enc_len, kw, kw_len, threshold, max_det)
         most = int(out[3].max())
         if most > max_det:
             out = eng.ctc_spot(lp, enc_len, kw, kw_len, threshold, most)
+        return out
+
+    # ---- hotwords (INTEGRATION.md §7h)
+    def _hotword_ids(self, hotwords: Sequence[Union[str, Sequence[int]]], threshold: float, what: str) -> List[List[int]]:
+        """Token ids of the hotwords, checked before any device work: RNN-T models raise NotImplementedError, the keyword and
+        threshold checks of `spot` raise ValueError, and so does a hotword that starts or ends with the space token (the
+        splice keeps to word boundaries by itself)."""
+        self._refuse_rnnt_spot(what)
+        _, ids = self._keyword_ids(hotwords, threshold)
+        tok = self.decoding.tokenizer
+        for row in ids:
+            if any(tok.id_to_str(row[i]) == " " for i in (0, -1)):
+                raise ValueError(f"{what}: hotword {tok.decode(row)!r} starts or ends with the space token; hotwords are "
+                                 "spliced at word boundaries only, so pass the word without its spaces")
+        return ids
+
+    def _apply_hotwords(self, lp: Tensor, enc_len: Tensor, ids: List[List[int]], threshold: float, g_ids: Tensor, g_frames: Tensor,
+                        g_counts: Tensor, token_logp: Optional[Tensor] = None, path_logp: Optional[Tensor] = None,
+                        frame_logp: Optional[Tensor] = None) -> Tuple[Tensor, ...]:
+        """Spot the hotwords in lp [B, T, V+1] (every detection kept) and splice them into the greedy output (gam_ctc_bias):
+        -> (ids, frames, counts, source, token_logp or None, path_logp or None); frame_logp is adjusted in place."""
+        eng = self._get_engine()
+        kw, kw_len = self._keyword_tensors(ids, eng.device)
+        spotted = self._spot_all(lp, enc_len, kw, kw_len, ids, threshold)
+        return eng.ctc_bias(lp, enc_len, kw, kw_len, spotted, threshold, self._word_flags(), g_ids, g_frames, g_counts, token_logp,
+                            path_logp, frame_logp)
+
+    def _transcribe_hotwords(self, wav_file, word_timestamps: bool, confidence: bool, hotwords, threshold: float
+                             ) -> TranscriptionResult:
+        """`transcribe` with hotwords: encode, (scored) greedy decoding, log-probs, spot, splice, then the usual formatting."""
+        from .timestamps_utils import path_confidence
+        kw_ids = self._hotword_ids(hotwords, threshold, "transcribe")
+        wav, length = self.prepare_wav(wav_file)
+        if length.item() > LONGFORM_THRESHOLD:
+            raise ValueError("Too long wav file, use 'transcribe_longform' method.")
+        encoded, encoded_len = self.forward(wav, length)
+        g = self.decoding.decode_device(self.head, encoded, encoded_len, scores=confidence)
+        eng = self._get_engine()
+        lp = eng.ctc_log_probs(_as_btd(encoded.to(dtype=torch.float32)))
+        ids, frames, counts, _, token_logp, path_logp = self._apply_hotwords(
+            lp, encoded_len, kw_ids, threshold, *g[:3], *(g[3:5] if confidence else (None, None)))
         del lp
-        start, end, score, count = (t[0].cpu() for t in out)
-        return self._detections(names, ids, start, end, score, count, compute_frame_shift(N, T))
+        conf = path_confidence(float(path_logp[0]), int(g[5][0])) if confidence else None
+        if not word_timestamps:
+            n = int(counts[0])
+            return TranscriptionResult(text=self.decoding.tokenizer.decode(ids[0, :n].tolist()), words=None, confidence=conf)
+        rec = eng.group_words(ids, frames, counts, self._word_flags())
+        text, words = self._words_from_records(ids.cpu(), counts.cpu(), encoded_len.cpu(), length.cpu(), [t.cpu() for t in rec],
+                                               token_logp.cpu() if confidence else None)[0]
+        return TranscriptionResult(text=text, words=words, confidence=conf)
 
     @torch.inference_mode()
     def transcribe_batch(self, wav: Tensor, lengths: Tensor) -> List[str]:

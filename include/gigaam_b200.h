@@ -357,6 +357,61 @@ int gam_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc
 int gam_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
                  const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det, int32_t* det_start,
                  int32_t* det_end, float* det_score, int32_t* det_count, void* stream);
+/* ---- CTC hotwords: the keywords gam_ctc_spot found replace the greedy words they outscore.  No hypothesis search: the greedy
+ * output changes only where a stored detection beats it by the margin the threshold states.
+ *
+ * Recording b's inputs: lp, T_b, blank and the keywords y (U tokens, S = 2U - 1 states) as in gam_ctc_spot; the greedy tokens
+ * (id_i, f_i), i < n = clamp(counts[b], 0, max_out), frames strictly increasing in [0, T); flag(id) = token_flags[id]
+ * (gam_group_words' table: 1 the piece is " ", 2 it starts with U+2581; 0 for an id outside [0, V)); and every stored
+ * detection (k, j < min(det_count[b, k], max_det)) of gam_ctc_spot at the same threshold: span [s, e), score E.
+ *   1. Gain: G = E - tau in fp32, tau = fp32(U) * fp32(log threshold) (spot's tau), so G >= 0.
+ *   2. Replaced range: [i0, i1) = the greedy tokens with f_i in [s, e) (binary searches over the frames); space tokens (flag 1)
+ *      at either end are removed from the range and stay in the output.
+ *   3. Eligible: i1 > i0 (nothing is inserted into silence) and i0 and i1 are word boundaries.  p is a word boundary when
+ *      p = 0 or p = n, token p - 1 is a space, token p is a space, or token p starts a SentencePiece word (flag 2).  So a
+ *      keyword is never spliced into part of a longer word.
+ *   4. Selection: eligible candidates in the order G descending, then s ascending, then the longer keyword, then the
+ *      lexicographically smaller ids, then the smaller k; each is accepted when [s, e) overlaps no accepted span.  Only exact
+ *      duplicate keywords reach the last tie-break, and they splice the same tokens: the output does not depend on the
+ *      keyword order or on the batch.
+ *   5. Identity: an accepted candidate whose ids[i0, i1) already equal y keeps the greedy tokens, frames and scores bit for bit
+ *      (it still blocks the candidates that overlap it).
+ *   6. Splice: otherwise tokens [i0, i1) are replaced by y.  The traced path is the keyword's best path over [s, e) that starts
+ *      on state 0 at s and ends on state S - 1 at e - 1, with spot's costs, recursion and tie rules and no fresh start after
+ *      s; in exact arithmetic it is the detection's own path, in fp32 the two can part only on exact ties.  Token u's frame is
+ *      the first frame of the path's run on state 2u; its token_logp is lp[frame, y_u].
+ *   Edge spaces never fall inside a keyword: the spaces kept at a splice's left edge (greedy tokens in [s, e) before i0) are
+ *   written just before y at frame s, and those at its right edge (in [s, e) from i1 on) whose frame is at or before the
+ *   frame l of y's last token are written just after y at frame l; the other right-edge spaces keep their frames.  Every
+ *   other kept greedy token keeps its frame, and the output is all tokens ordered by (frame, then: greedy tokens placed
+ *   before the frame's keyword token, the keyword token, greedy tokens placed after it, each group in greedy order), so
+ *   frames never decrease.  out_source[i] = k for a spliced or confirmed token, -1 for the others.  Tokens past max_out are
+ *   dropped and out_counts stops at max_out; with max_out >= T (required; gam_*_greedy's width) that needs more tokens than
+ *   frames, which only shared frames allow.
+ *   7. Scores, when the caller passes them: out_path_logp = fp32(fp64(path_logp) + E_1 + E_2 + ...) in fp64, over the accepted
+ *      splices in start order (path_rows does not change); for frame_logp (device f64 [b * frame_pitch + t], the per-frame
+ *      sums of gam_*_greedy_resume), every frame t of an accepted splice gets += fp64(lp[t, l(t)]) - fp64(m[t]), l(t) the
+ *      traced path's label, so segment and path confidences keep their meaning.
+ * Inputs, all device: log_probs [B, T, V+1], enc_len [B], keywords [K, Umax], keyword_len [K] and det_start / det_end /
+ *   det_score / det_count exactly as given to and produced by gam_ctc_spot with the same threshold and max_det; token_flags u8
+ *   [V]; ids / frames [B, max_out], counts [B] (gam_*_greedy); token_logp [B, max_out] and path_logp [B] (scored greedy), or
+ *   NULL together with out_token_logp / out_path_logp; frame_logp, or NULL.  Outputs: out_ids / out_frames / out_source
+ *   [B, max_out] (entries past out_counts[b] are not written), out_counts [B], out_token_logp [B, max_out], out_path_logp [B];
+ *   they must not alias the inputs.
+ * Refused (gam_last_error): what gam_ctc_spot refuses, plus max_out < T, a missing flag table or V != num_classes - 1,
+ *   frame_pitch < T and a workspace smaller than gam_ctc_bias_workspace_bytes(h, B, T, K, max_det) (which returns -1 for bad
+ *   sizes or a handle without a CTC head).  The workspace holds, per recording, the sort keys of K x min(max_det, T)
+ *   candidates rounded up to a power of two (16 bytes each), 72 bytes per frame (the backpointers, 32 bytes per frame, among
+ *   them) and 4 bytes per keyword.  Three launches, fixed orders, no atomics, no host synchronisation: capturable in a CUDA
+ *   graph. */
+int64_t gam_ctc_bias_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t K, int32_t max_det);
+int gam_ctc_bias(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
+                 const int32_t* keyword_len, int32_t K, int32_t Umax, const int32_t* det_start, const int32_t* det_end,
+                 const float* det_score, const int32_t* det_count, int32_t max_det, float threshold, const uint8_t* token_flags,
+                 int32_t V, const int32_t* ids, const int32_t* frames, const int32_t* counts, int32_t max_out, const float* token_logp,
+                 const float* path_logp, double* frame_logp, int64_t frame_pitch, void* workspace, int64_t workspace_bytes,
+                 int32_t* out_ids, int32_t* out_frames, int32_t* out_counts, int32_t* out_source, float* out_token_logp,
+                 float* out_path_logp, void* stream);
 /* RNN-T stage 1: enc [B, T, d_model], dec [B, U+1, pred_hidden] (gam_rnnt_predict over cat[blank, y]), targets [B, U] i32
  *   -> blank [B, T, U+1], label [B, T, U+1]: bit-identical to the matching entries of gam_rnnt_joint's lattice for the same
  *   enc / dec, but no [.., V+1] row is ever stored.  label is -inf at u = U and NaN where targets[b, u] is outside [0, V) (so
