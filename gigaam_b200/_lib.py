@@ -65,7 +65,8 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_ctc_align", "gam_rnnt_align_scores_workspace_bytes", "gam_rnnt_align_scores", "gam_rnnt_align_workspace_bytes",
            "gam_rnnt_align", "gam_ctc_align_long_workspace_bytes", "gam_ctc_align_long", "gam_test_ctc_align_long",
            "gam_decode_state_bytes", "gam_decode_state_init", "gam_decode_resume_workspace_bytes", "gam_ctc_greedy_resume",
-           "gam_rnnt_greedy_resume", "gam_ctc_spot", "gam_test_ctc_spot", "gam_ctc_bias_workspace_bytes", "gam_ctc_bias")
+           "gam_rnnt_greedy_resume", "gam_ctc_spot", "gam_test_ctc_spot", "gam_ctc_bias_workspace_bytes", "gam_ctc_bias",
+           "gam_ctc_align_long_gaps_workspace_bytes", "gam_ctc_align_long_gaps", "gam_test_ctc_align_long_gaps")
 
 
 def lib_path() -> Path:
@@ -152,7 +153,7 @@ def load() -> C.CDLL:
     for fn in (lib.gam_rnnt_predict_train, lib.gam_ctc_log_probs_backward, lib.gam_rnnt_joint_backward, lib.gam_rnnt_predict_backward):
         fn.restype = C.c_int
     for fn in (lib.gam_ctc_align_workspace_bytes, lib.gam_rnnt_align_scores_workspace_bytes, lib.gam_rnnt_align_workspace_bytes,
-               lib.gam_ctc_align_long_workspace_bytes):
+               lib.gam_ctc_align_long_workspace_bytes, lib.gam_ctc_align_long_gaps_workspace_bytes):
         fn.argtypes = [H, i32, i32, i32]
         fn.restype = i64
     lib.gam_ctc_align.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, c_vp, i64] + [c_vp] * 6
@@ -160,7 +161,10 @@ def load() -> C.CDLL:
     lib.gam_rnnt_align.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, c_vp, i64] + [c_vp] * 6
     lib.gam_ctc_align_long.argtypes = lib.gam_ctc_align.argtypes
     lib.gam_test_ctc_align_long.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, c_vp, i64] + [c_vp] * 5 + [i32, c_vp, c_vp]
-    for fn in (lib.gam_ctc_align, lib.gam_rnnt_align_scores, lib.gam_rnnt_align, lib.gam_ctc_align_long, lib.gam_test_ctc_align_long):
+    lib.gam_ctc_align_long_gaps.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, C.c_float, c_vp, i64] + [c_vp] * 9
+    lib.gam_test_ctc_align_long_gaps.argtypes = lib.gam_ctc_align_long_gaps.argtypes[:-1] + [i32, c_vp, c_vp]
+    for fn in (lib.gam_ctc_align, lib.gam_rnnt_align_scores, lib.gam_rnnt_align, lib.gam_ctc_align_long, lib.gam_test_ctc_align_long,
+               lib.gam_ctc_align_long_gaps, lib.gam_test_ctc_align_long_gaps):
         fn.restype = C.c_int
     lib.gam_ctc_spot.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32, C.c_float, i32] + [c_vp] * 5
     lib.gam_test_ctc_spot.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32, C.c_float, i32] + [c_vp] * 4 + [i32, c_vp]

@@ -11,17 +11,29 @@
 //       owns states [k P, (k + 1) P), P a multiple of 16, and keeps their labels and double-buffered values in its own
 //       shared memory.  Each frame reads the two states left of its range from CTA k - 1 over distributed shared memory,
 //       then one cluster barrier closes the frame.  The per-state arithmetic is (1)'s, so the results are its bits.
+//       Gap mode (the GAPS instantiation, after row_max_kernel's pre-pass) lets the blank states at line edges also emit
+//       m[t] + log theta; the instantiation without gaps is the kernel of gam_ctc_align_long.
 // All backtrack with one thread (a serial walk of T or T + U steps) and then gather token_logp with the whole CTA.
+#include <algorithm>
 #include <cmath>
 
 #include "kernels.h"
 #include "launch.cuh"
 #include "ptx.cuh"
+#include "rowmax.cuh"
 
 namespace gam {
 namespace {
 
 constexpr int kSkip = 1 << 30;   // ctc lab_s: the state may also be entered from s - 2
+constexpr int kBound = 1 << 29;  // ctc_align_long lab_s, gap mode: a boundary state
+
+// gap mode: whether the blank state s (even) of a recording with U_b tokens is a boundary state: the first or last state, or
+// the blank before a token that starts a line or after one that ends a line
+__device__ __forceinline__ bool boundary_state(const uint8_t* edges, int Ub, int s) {
+  const int j = s >> 1;   // the blank between tokens j - 1 and j
+  return s == 0 || j == Ub || (edges[j] & 1) || (edges[j - 1] & 2);
+}
 
 __device__ __forceinline__ float lse3(float a, float b, float c) {
   const float m = fmaxf(fmaxf(a, b), c);
@@ -262,10 +274,15 @@ __global__ void rnnt_align_kernel(const float* __restrict__ blank, const float* 
 // frame is enough.  Every CTA checks all target ids itself, so `bad` needs no exchange; the NaN flags and the final states
 // are read by CTA 0, which then backtracks (the last barrier makes every CTA's backpointer stores visible to it) and
 // writes all outputs.
+// GAPS: a boundary state (kBound) emits max(lp[t, blank], m[t] + log theta) in both recursions, every frame t < T_b also reads
+// m[t] (a NaN there poisons the recording), and CTA 0's backtrack flags the unmatched frames; g is not read otherwise.
+template <bool GAPS>
 __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const int* __restrict__ enc_len,
                                       const int* __restrict__ targets, const int* __restrict__ target_len, int T, int U, int V1, int P,
                                       uint32_t* __restrict__ bp, int* __restrict__ frames, float* __restrict__ token_logp,
-                                      float* __restrict__ viterbi_logp, float* __restrict__ log_likelihood, int* __restrict__ path_rows) {
+                                      float* __restrict__ viterbi_logp, float* __restrict__ log_likelihood, int* __restrict__ path_rows,
+                                      AlignGaps g) {
+  constexpr int kLab = GAPS ? ~(kSkip | kBound) : ~kSkip;   // the label of a lab_s entry
   extern __shared__ float4 smem_f4[];
   uint32_t C;
   asm("mov.u32 %0, %%cluster_nctarank;" : "=r"(C));
@@ -280,6 +297,8 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
   __shared__ int nan_s, poison_s, final_s;
   const int blank = V1 - 1;
   const int* y = targets + static_cast<int64_t>(b) * U;
+  const uint8_t* edges = GAPS ? g.line_edges + static_cast<int64_t>(b) * U : nullptr;
+  const float* mb = GAPS ? g.m + static_cast<int64_t>(b) * T : nullptr;
   int bad = 0;
   for (int i = tid; i < Ub; i += nt) {
     const int l = y[i];
@@ -291,6 +310,8 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
     if (s & 1) {
       l = y[s >> 1];
       if (l >= 0 && l < blank && s >= 3 && l != y[(s >> 1) - 1]) l |= kSkip;
+    } else if (GAPS && boundary_state(edges, Ub, s)) {
+      l |= kBound;
     }
     lab_s[i] = l;
   }
@@ -302,14 +323,26 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
   const uint32_t left_f = k > 0 ? ptx::mapa_u32(ptx::smem_u32(fbuf), k - 1) : 0u;
   int nan = 0;
   if (!bad && Tb > 0) {   // uniform over the cluster: every barrier below is reached by all of its threads
+    float gt = 0.f;   // gap mode: m[t] + log theta of the current frame
+    if constexpr (GAPS) {
+      nan |= isnan(mb[0]);
+      gt = mb[0] + g.log_theta;
+    }
     for (int i = tid; i < n; i += nt) {
       const int s = s0 + i;
-      const float x = lp[lab_s[i] & ~kSkip];   // frame 0 reads every state's entry: the NaN rule counts them
+      float x = lp[lab_s[i] & kLab];   // frame 0 reads every state's entry: the NaN rule counts them
       nan |= isnan(x);
+      if (GAPS && (lab_s[i] & kBound)) x = fmaxf(x, gt);
       vbuf[i] = fbuf[i] = s < 2 ? x : -INFINITY;
     }
     for (int t = 1; t < Tb; ++t) {
+      float mt = 0.f;
+      if constexpr (GAPS) mt = mb[t];   // loaded ahead of the barrier
       ptx::cluster_sync();   // frame t - 1 complete in every CTA of the cluster
+      if constexpr (GAPS) {
+        nan |= isnan(mt);
+        gt = mt + g.log_theta;
+      }
       const int p = (t - 1) & 1;
       const float* va = vbuf + p * P;
       const float* fa = fbuf + p * P;
@@ -346,8 +379,9 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
             }
             if (c > best) { best = c; code = 2; }
           }
-          const float x = row[l & ~kSkip];
+          float x = row[l & kLab];
           nan |= isnan(x);
+          if (GAPS && (l & kBound)) x = fmaxf(x, gt);
           vb[i] = x + best;
           fb[i] = x + lse3(fa[i], fm1, fm2);
         }
@@ -391,14 +425,33 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
   int* fr = frames + static_cast<int64_t>(b) * U;
   float* tl = token_logp + static_cast<int64_t>(b) * U;
   const int fs = final_s, poison = poison_s;
+  uint8_t* um = GAPS ? g.unmatched + static_cast<int64_t>(b) * T : nullptr;
   for (int i = tid; i < U; i += nt) fr[i] = -1;
+  if constexpr (GAPS)
+    for (int t = tid; t < T; t += nt) um[t] = 0;
   __syncthreads();
   if (fs >= 0 && tid == 0) {   // serial backtrack, as ctc_align_kernel's
-    int s = fs;
+    int s = fs, rows = 0;
     for (int t = Tb - 1; t >= 0; --t) {
-      if (s & 1) fr[s >> 1] = t;
+      if (s & 1) {
+        fr[s >> 1] = t;
+      } else if (GAPS && boundary_state(edges, Ub, s) && mb[t] + g.log_theta > lp[static_cast<int64_t>(t) * V1 + blank]) {
+        um[t] = 1;   // the sweep's boundary emission took m[t] + log theta here
+        ++rows;
+      }
       if (t > 0) s -= (bpu[static_cast<int64_t>(t) * W + s / 16] >> (2 * (s & 15))) & 3u;
     }
+    if constexpr (GAPS) {
+      float sum = 0.f;
+      for (int t = 0; t < Tb; ++t)
+        if (um[t]) sum += mb[t] + g.log_theta;   // in frame order
+      g.unmatched_rows[b] = rows;
+      g.unmatched_logp[b] = sum;
+    }
+  }
+  if (GAPS && tid == 0 && fs < 0) {   // no path, or poisoned
+    g.unmatched_rows[b] = 0;
+    g.unmatched_logp[b] = poison ? qnan() : 0.f;
   }
   __syncthreads();
   for (int i = tid; i < U; i += nt) {
@@ -409,6 +462,35 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
     }
     tl[i] = v;
   }
+}
+
+// gap mode's pre-pass: m[b, t] = max_c lp[t, c] (warp_row_max) for t < T_b, one warp per frame, strided over t and b
+__global__ void row_max_kernel(const float* __restrict__ log_probs, const int* __restrict__ enc_len, int B, int T, int V1,
+                               float* __restrict__ m) {
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const int Tb = min(max(enc_len[b], 0), T);
+    for (int t = blockIdx.x * wpb + (threadIdx.x >> 5); t < Tb; t += gridDim.x * wpb) {   // whole warps
+      const int64_t r = static_cast<int64_t>(b) * T + t;
+      const float mx = warp_row_max(log_probs + r * V1, V1, lane);
+      if (lane == 0) m[r] = mx;
+    }
+  }
+}
+
+// cluster and shared-memory attributes of one instantiation, once per device
+template <bool GAPS>
+int align_long_attributes() {
+  static PerDeviceOnce attr_once;
+  if (!attr_once.first()) return 0;
+  int dev = 0, cap = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  if (cudaFuncSetAttribute(ctc_align_long_kernel<GAPS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
+      cudaFuncSetAttribute(ctc_align_long_kernel<GAPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap - kAlignLongStaticSmem) !=
+          cudaSuccess)
+    return -1;
+  return 0;
 }
 
 int align_threads(int n) { return n <= 64 ? 64 : n >= 1024 ? 1024 : (n + 31) / 32 * 32; }
@@ -456,19 +538,11 @@ int ctc_align_long_plan(int U, int forced_ctas, int* ctas, int* states_per_cta) 
 
 int launch_ctc_align_long(const float* log_probs, const int* enc_len, const int* targets, const int* target_len, int B, int T, int U,
                           int V1, int forced_ctas, uint32_t* bp, int* frames, float* token_logp, float* viterbi_logp,
-                          float* log_likelihood, int* path_rows, int* plan, cudaStream_t s) {
-  static PerDeviceOnce attr_once;
+                          float* log_likelihood, int* path_rows, int* plan, const AlignGaps* gaps, cudaStream_t s) {
   int C = 0, P = 0;
   const int rc = ctc_align_long_plan(U, forced_ctas, &C, &P);
   if (rc != 0) return rc;
-  if (attr_once.first()) {
-    int dev = 0, cap = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    if (cudaFuncSetAttribute(ctc_align_long_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-        cudaFuncSetAttribute(ctc_align_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap - kAlignLongStaticSmem) != cudaSuccess)
-      return -1;
-  }
+  if ((gaps ? align_long_attributes<true>() : align_long_attributes<false>()) != 0) return -1;
   if (plan) {
     plan[0] = C;
     plan[1] = P;
@@ -485,8 +559,15 @@ int launch_ctc_align_long(const float* log_probs, const int* enc_len, const int*
   cfg.stream = s;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if (cudaLaunchKernelEx(&cfg, ctc_align_long_kernel, log_probs, enc_len, targets, target_len, T, U, V1, P, bp, frames, token_logp,
-                         viterbi_logp, log_likelihood, path_rows) != cudaSuccess)
+  if (!gaps)
+    return cudaLaunchKernelEx(&cfg, ctc_align_long_kernel<false>, log_probs, enc_len, targets, target_len, T, U, V1, P, bp, frames,
+                              token_logp, viterbi_logp, log_likelihood, path_rows, AlignGaps{}) != cudaSuccess
+               ? -2
+               : 0;
+  const dim3 grid(static_cast<unsigned>(std::min<int64_t>((static_cast<int64_t>(T) + 7) / 8, 65535)), std::min(B, 65535));
+  row_max_kernel<<<grid, 256, 0, s>>>(log_probs, enc_len, B, T, V1, gaps->m);
+  if (cudaLaunchKernelEx(&cfg, ctc_align_long_kernel<true>, log_probs, enc_len, targets, target_len, T, U, V1, P, bp, frames, token_logp,
+                         viterbi_logp, log_likelihood, path_rows, *gaps) != cudaSuccess)
     return -2;
   return 0;
 }

@@ -915,10 +915,17 @@ int64_t gam_ctc_align_long_workspace_bytes(const gam_handle* h, int32_t B, int32
   return align_up(static_cast<int64_t>(B) * ctc_bp_words(T, U) * 4, 1024);
 }
 
+int64_t gam_ctc_align_long_gaps_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  const int64_t bp = gam_ctc_align_long_workspace_bytes(h, B, T, U);
+  return bp < 0 ? -1 : bp + align_up(static_cast<int64_t>(B) * T * 4, 1024);
+}
+
+// gaps: NULL for gam_ctc_align_long; otherwise line_edges, log_theta and the three outputs, with m still to be placed in the
+// workspace behind the backpointers
 static int ctc_align_long_run(gam_handle* h, const char* what, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
                               const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes,
                               int32_t* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int32_t* path_rows,
-                              int32_t cluster_ctas, int32_t* plan, void* stream) {
+                              int32_t cluster_ctas, int32_t* plan, AlignGaps* gaps, void* stream) {
   const gam_config& c = h->cfg;
   if (c.head != 1) return fail(h, -1, "%s: model has no CTC head", what);
   if (B <= 0 || T <= 0 || U < 0) return fail(h, -1, "%s: bad sizes (B=%d, T=%d, U=%d)", what, B, T, U);
@@ -927,14 +934,24 @@ static int ctc_align_long_run(gam_handle* h, const char* what, const float* log_
   if (!log_probs || !enc_len || !target_len || (U > 0 && (!targets || !frames || !token_logp)) || !viterbi_logp || !log_likelihood ||
       !path_rows)
     return fail(h, -1, "%s: a required pointer is NULL", what);
-  const int64_t need = gam_ctc_align_long_workspace_bytes(h, B, T, U);
+  if (gaps) {
+    if ((U > 0 && !gaps->line_edges) || !gaps->unmatched || !gaps->unmatched_rows || !gaps->unmatched_logp)
+      return fail(h, -1, "%s: a required pointer is NULL", what);
+    if (std::isnan(gaps->log_theta) || gaps->log_theta > 0.f)
+      return fail(h, -1, "%s: log_theta=%g must be <= 0 (a threshold in (0, 1]) or -inf", what, gaps->log_theta);
+  }
+  const int64_t bp_bytes = gam_ctc_align_long_workspace_bytes(h, B, T, U);
+  const int64_t need = gaps ? gam_ctc_align_long_gaps_workspace_bytes(h, B, T, U) : bp_bytes;
   if (workspace == nullptr || workspace_bytes < need)
     return fail(h, -1, "%s: workspace too small: need %lld bytes, got %lld", what, (long long)need, (long long)workspace_bytes);
+  if (gaps) gaps->m = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + bp_bytes);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc;
   { PROF(PC_ALIGN);
+    if (gaps) h->launches += 1;   // the pre-pass
     rc = launch_ctc_align_long(log_probs, enc_len, targets, target_len, B, T, U, c.num_classes, cluster_ctas,
-                               static_cast<uint32_t*>(workspace), frames, token_logp, viterbi_logp, log_likelihood, path_rows, plan, s); }
+                               static_cast<uint32_t*>(workspace), frames, token_logp, viterbi_logp, log_likelihood, path_rows, plan, gaps,
+                               s); }
   if (rc == 2) return fail(h, -1, "%s: %d CTAs leave a CTA without states at U=%d", what, cluster_ctas, U);
   if (rc == 1) return fail(h, -1, "%s: no cluster of <= %d CTAs holds U=%d (forced %d)", what, kAlignLongMaxCtas, U, cluster_ctas);
   if (rc != 0) return fail(h, -4, "%s: launch rejected (rc=%d): %s", what, rc, cudaGetErrorString(cudaGetLastError()));
@@ -946,7 +963,17 @@ int gam_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc
                        int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
                        float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream) {
   return ctc_align_long_run(h, "ctc_align_long", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes, frames,
-                            token_logp, viterbi_logp, log_likelihood, path_rows, 0, nullptr, stream);
+                            token_logp, viterbi_logp, log_likelihood, path_rows, 0, nullptr, nullptr, stream);
+}
+
+int gam_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                            const int32_t* target_len, const uint8_t* line_edges, int32_t B, int32_t T, int32_t U, float log_theta,
+                            void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp, float* viterbi_logp,
+                            float* log_likelihood, int32_t* path_rows, uint8_t* unmatched, int32_t* unmatched_rows,
+                            float* unmatched_logp, void* stream) {
+  AlignGaps g{line_edges, log_theta, nullptr, unmatched, unmatched_rows, unmatched_logp};
+  return ctc_align_long_run(h, "ctc_align_long_gaps", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes,
+                            frames, token_logp, viterbi_logp, log_likelihood, path_rows, 0, nullptr, &g, stream);
 }
 
 int gam_test_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
@@ -956,7 +983,19 @@ int gam_test_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t
   if (cluster_ctas < 0 || cluster_ctas > kAlignLongMaxCtas)
     return fail(h, -1, "test_ctc_align_long: cluster_ctas=%d outside [0, %d]", cluster_ctas, kAlignLongMaxCtas);
   return ctc_align_long_run(h, "test_ctc_align_long", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes,
-                            frames, token_logp, viterbi_logp, log_likelihood, path_rows, cluster_ctas, plan, stream);
+                            frames, token_logp, viterbi_logp, log_likelihood, path_rows, cluster_ctas, plan, nullptr, stream);
+}
+
+int gam_test_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                                 const int32_t* target_len, const uint8_t* line_edges, int32_t B, int32_t T, int32_t U, float log_theta,
+                                 void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp, float* viterbi_logp,
+                                 float* log_likelihood, int32_t* path_rows, uint8_t* unmatched, int32_t* unmatched_rows,
+                                 float* unmatched_logp, int32_t cluster_ctas, int32_t* plan, void* stream) {
+  if (cluster_ctas < 0 || cluster_ctas > kAlignLongMaxCtas)
+    return fail(h, -1, "test_ctc_align_long_gaps: cluster_ctas=%d outside [0, %d]", cluster_ctas, kAlignLongMaxCtas);
+  AlignGaps g{line_edges, log_theta, nullptr, unmatched, unmatched_rows, unmatched_logp};
+  return ctc_align_long_run(h, "test_ctc_align_long_gaps", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes,
+                            frames, token_logp, viterbi_logp, log_likelihood, path_rows, cluster_ctas, plan, &g, stream);
 }
 
 // ---- keyword spotting (csrc/spot.cu)

@@ -154,9 +154,20 @@ constexpr int kAlignLongMaxTokens = 65536;
 constexpr int kAlignLongMaxCtas = 16;
 constexpr int kAlignLongStaticSmem = 1024;   // headroom kept for the kernel's static shared memory
 int ctc_align_long_plan(int U, int forced_ctas, int* ctas, int* states_per_cta);
+// Gap mode of the sweep (gam_ctc_align_long_gaps): boundary states may also emit m[t] + log_theta.  A pre-pass fills
+// m [B, T] (frames t < T_b only) before the sweep reads it.
+struct AlignGaps {
+  const uint8_t* line_edges;   // [B, U]: bit 0 the token starts a line, bit 1 it ends one
+  float log_theta;
+  float* m;                    // [B, T] workspace
+  uint8_t* unmatched;          // [B, T]
+  int* unmatched_rows;         // [B]
+  float* unmatched_logp;       // [B]
+};
+// gaps: NULL for gam_ctc_align_long's sweep
 int launch_ctc_align_long(const float* log_probs, const int* enc_len, const int* targets, const int* target_len, int B, int T, int U,
                           int V1, int forced_ctas, uint32_t* bp, int* frames, float* token_logp, float* viterbi_logp,
-                          float* log_likelihood, int* path_rows, int* plan, cudaStream_t s);
+                          float* log_likelihood, int* path_rows, int* plan, const AlignGaps* gaps, cudaStream_t s);
 
 // spot.cu: CTC keyword spotting (gam_ctc_spot), grid (ceil(K / warps), B), one warp per keyword of <= kSpotMaxTokens tokens.
 // keywords [K, Umax], keyword_len [K]; det_* [B, K, max_det], det_count [B, K].  log_theta = fp32 log of the threshold.

@@ -15,6 +15,7 @@
 #include "kernels.h"
 #include "launch.cuh"
 #include "ptx.cuh"
+#include "rowmax.cuh"
 
 namespace gam {
 namespace {
@@ -110,18 +111,8 @@ __global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict_
     const float* tile = reinterpret_cast<const float*>(tiles + st * stage_bytes + (tile_src(i) & 15));
     float* m = mrow + st * R;
     for (int r = warp; r < n; r += nw) {   // m[t] once per frame for the whole CTA
-      const float* row = tile + static_cast<int64_t>(r) * V1;
-      float mx = -INFINITY;
-      int nan = 0;
-      for (int c = lane; c < V1; c += 32) {
-        const float x = row[c];
-        mx = fmaxf(mx, x);
-        nan |= isnan(x);
-      }
-#pragma unroll
-      for (int off = 16; off; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(kFull, mx, off));
-      if (__any_sync(kFull, nan)) mx = __int_as_float(0x7fc00000);
-      if (lane == 0) m[r] = mx + 0.f;   // + 0: a zero max is +0 whatever the order of the max
+      const float mx = warp_row_max(tile + static_cast<int64_t>(r) * V1, V1, lane);
+      if (lane == 0) m[r] = mx;
     }
     __syncthreads();   // m of this tile is published; every warp is done with tile i - 1's stage
     if (tid == 0 && i >= 1 && i - 1 + kSpotStages < ntiles) issue(i - 1 + kSpotStages);

@@ -713,31 +713,46 @@ class Engine:
         return outs
 
     def ctc_align_long(self, log_probs: Tensor, enc_len: Tensor, targets: Tensor, target_len: Tensor,
-                       cluster_ctas: Optional[int] = None) -> Tuple[Tensor, ...]:
+                       cluster_ctas: Optional[int] = None, gaps: Optional[Tuple[Tensor, float]] = None) -> Tuple[Tensor, ...]:
         """ctc_align for recordings of any length and up to 65 536 tokens (gam_ctc_align_long): the same arguments and
         outputs, and the same bits on every input ctc_align accepts.  `cluster_ctas` forces the number of CTAs per utterance
-        (gam_test_ctc_align_long); the plan used, (CTAs, states per CTA), is then kept in `last_align_long_plan`."""
+        (gam_test_ctc_align_long*); the plan used, (CTAs, states per CTA), is then kept in `last_align_long_plan`.
+        `gaps` = (line_edges [B, U] u8, log_theta) runs gam_ctc_align_long_gaps instead and appends its three outputs
+        (unmatched [B, T] u8, unmatched_rows [B] i32, unmatched_logp [B] f32)."""
         assert log_probs.is_cuda and log_probs.dtype == torch.float32 and log_probs.is_contiguous() and log_probs.dim() == 3
         if self.head_type != 1:
             raise RuntimeError("model has no CTC head")
         B, T, _ = log_probs.shape
         U = targets.shape[1]
-        nbytes = int(self.lib.gam_ctc_align_long_workspace_bytes(self.handle, B, T, U))
+        size_fn = self.lib.gam_ctc_align_long_workspace_bytes if gaps is None else self.lib.gam_ctc_align_long_gaps_workspace_bytes
+        nbytes = int(size_fn(self.handle, B, T, U))
         if nbytes < 0:
             raise ValueError(f"ctc_align_long: bad sizes B={B}, T={T}, U={U}")
-        ws = self._ws_align.get(("ctc_long", B, T, U), nbytes, self.device)
+        ws = self._ws_align.get(("ctc_long" if gaps is None else "ctc_long_gaps", B, T, U), nbytes, self.device)
         enc_len, targets, target_len = (self._i32(t, self.device) for t in (enc_len, targets, target_len))
         outs = self._align_outputs(B, U)
-        ptrs = [log_probs.data_ptr(), enc_len.data_ptr(), targets.data_ptr(), target_len.data_ptr(), B, T, U, ws.data_ptr(), ws.numel(),
-                *[t.data_ptr() for t in outs]]
+        head = [log_probs.data_ptr(), enc_len.data_ptr(), targets.data_ptr(), target_len.data_ptr()]
+        if gaps is not None:
+            line_edges, log_theta = gaps
+            line_edges = line_edges.to(device=self.device, dtype=torch.uint8).contiguous()
+            if tuple(line_edges.shape) != (B, U):
+                raise ValueError(f"ctc_align_long: line_edges has shape {tuple(line_edges.shape)}, expected ({B}, {U})")
+            outs = outs + (torch.empty((B, T), dtype=torch.uint8, device=self.device),
+                           torch.empty((B,), dtype=torch.int32, device=self.device),
+                           torch.empty((B,), dtype=torch.float32, device=self.device))
+            head += [line_edges.data_ptr()]
+        sizes = [B, T, U] + ([] if gaps is None else [float(log_theta)])
+        ptrs = head + sizes + [ws.data_ptr(), ws.numel(), *[t.data_ptr() for t in outs]]
         with torch.cuda.device(self.device):
             if cluster_ctas is None:
-                rc = self.lib.gam_ctc_align_long(self.handle, *ptrs, self._stream())
+                fn = self.lib.gam_ctc_align_long if gaps is None else self.lib.gam_ctc_align_long_gaps
+                rc = fn(self.handle, *ptrs, self._stream())
             else:
+                fn = self.lib.gam_test_ctc_align_long if gaps is None else self.lib.gam_test_ctc_align_long_gaps
                 plan = (C.c_int32 * 2)()
-                rc = self.lib.gam_test_ctc_align_long(self.handle, *ptrs, int(cluster_ctas), plan, self._stream())
+                rc = fn(self.handle, *ptrs, int(cluster_ctas), plan, self._stream())
                 self.last_align_long_plan = (int(plan[0]), int(plan[1]))
-        _lib.check(self.lib, self.handle, rc, "gam_ctc_align_long")
+        _lib.check(self.lib, self.handle, rc, "gam_ctc_align_long" if gaps is None else "gam_ctc_align_long_gaps")
         return outs
 
     def ctc_spot(self, log_probs: Tensor, enc_len: Tensor, keywords: Tensor, keyword_len: Tensor, threshold: float, max_det: int,

@@ -311,3 +311,23 @@ def line_segments(lines: Sequence[str], ranges: Sequence[Tuple[int, int]], frame
         out.append(Segment(text=text, start=start, end=end, words=seg_words, confidence=mean_logp_confidence(token_logp[a:b])))
         prev_end = end
     return out
+
+
+def line_edges(ranges: Sequence[Tuple[int, int]], U: int) -> List[int]:
+    """gam_ctc_align_long_gaps' line_edges of a text of U tokens whose lines have token ranges [a, b): bit 0 on the first
+    token of every line, bit 1 on its last.  Empty lines have no tokens and set no bits."""
+    edges = [0] * U
+    for a, b in ranges:
+        if b > a:
+            edges[a] |= 1
+            edges[b - 1] |= 2
+    return edges
+
+
+def unmatched_intervals(flags: Tensor, frame_shift: float) -> List[Tuple[float, float]]:
+    """Maximal runs of unmatched frames (flags [T], nonzero = unmatched) -> (start, end) seconds, end exclusive."""
+    f = torch.cat([torch.zeros(1, dtype=torch.int8), (flags.reshape(-1).cpu() != 0).to(torch.int8), torch.zeros(1, dtype=torch.int8)])
+    d = torch.diff(f)
+    starts = torch.nonzero(d == 1).reshape(-1).tolist()
+    ends = torch.nonzero(d == -1).reshape(-1).tolist()
+    return [(a * frame_shift, b * frame_shift) for a, b in zip(starts, ends)]

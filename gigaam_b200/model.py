@@ -387,18 +387,28 @@ class GigaAMASR(GigaAM):
 
     @torch.inference_mode()
     def align_longform(self, wav_file, text: Union[str, Sequence[str]], word_timestamps: bool = True, window: float = 30.0,
-                       overlap: float = 4.0, batch_size: int = 16) -> LongformAlignment:
+                       overlap: float = 4.0, batch_size: int = 16, *, gap_threshold: Optional[float] = None) -> LongformAlignment:
         """Align a known text, one string or a sequence of lines, to a recording of any length (INTEGRATION.md §7e).  The
         encoder runs over overlapping windows (`longform.plan_windows`), the windows' CTC log-probs are stitched into one
         sequence and gam_ctc_align_long aligns the whole text to it: up to 65 536 tokens, no frame limit.  Returns one
         Segment per line.  CTC models only: RNN-T raises NotImplementedError.  Raises ValueError before any device work for
-        more than 65 536 tokens and for the window plan's refusals (longform.plan_windows)."""
-        from .longform import line_segments, plan_windows, stitch_ctc_log_probs
-        from .timestamps_utils import compute_frame_shift, path_confidence, words_from_device
+        more than 65 536 tokens and for the window plan's refusals (longform.plan_windows).
+        `gap_threshold` (theta in (0, 1], INTEGRATION.md §7e) lets audio between lines that the text lacks stay unaligned
+        (gam_ctc_align_long_gaps): a frame at a line's edge is left unmatched where theta times the greedy decoder's
+        probability beats blank, and the result's `unmatched` lists those stretches; ValueError for theta outside (0, 1] as
+        float32, or NaN."""
+        from .longform import line_edges, line_segments, plan_windows, stitch_ctc_log_probs, unmatched_intervals
+        from .timestamps_utils import compute_frame_shift, gap_confidence, path_confidence, words_from_device
         if self._ncfg["head"].get("type") == "rnnt":
             raise NotImplementedError("align_longform needs a CTC head: RNN-T alignment walks a [T, U + 1] lattice, about "
                                       "4.5e9 nodes for an hour of speech, and banding it would no longer give the Viterbi "
                                       "path; use a *_ctc model, or align() up to max_encoded_frames")
+        log_theta = None
+        if gap_threshold is not None:
+            theta = float(np.float32(gap_threshold))
+            if not 0.0 < theta <= 1.0:          # NaN fails too
+                raise ValueError(f"align_longform: gap_threshold must be in (0, 1], got {gap_threshold!r}")
+            log_theta = float(np.float32(math.log(theta)))   # spot's rounding of log theta
         lines = [text] if isinstance(text, str) else list(text)
         norm, ids, ranges = self._line_tokens(lines)
         if len(ids) > ALIGN_LONG_MAX_TOKENS:
@@ -419,7 +429,12 @@ class GigaAMASR(GigaAM):
         targets_d = targets.to(eng.device)
         target_len_d = torch.tensor([U], dtype=torch.int32, device=eng.device)
         enc_len = torch.tensor([T], dtype=torch.int32, device=eng.device)
-        frames, token_logp, viterbi_logp, log_likelihood, path_rows = eng.ctc_align_long(lp, enc_len, targets_d, target_len_d)
+        if log_theta is None:
+            frames, token_logp, viterbi_logp, log_likelihood, path_rows = eng.ctc_align_long(lp, enc_len, targets_d, target_len_d)
+        else:
+            edges = torch.tensor(line_edges(ranges, U), dtype=torch.uint8).reshape(1, U).to(eng.device)
+            frames, token_logp, viterbi_logp, log_likelihood, path_rows, unmatched, u_rows, u_logp = eng.ctc_align_long(
+                lp, enc_len, targets_d, target_len_d, gaps=(edges, log_theta))
         del lp
         vit, ll = float(viterbi_logp[0]), float(log_likelihood[0])
         shift = compute_frame_shift(int(length[0]), T)
@@ -432,7 +447,11 @@ class GigaAMASR(GigaAM):
                 words = words_from_device(self.decoding.tokenizer, ids, ws[:k], we[:k], wf[:k], wn[:k], shift, logp)
                 word_first = wf[:k]
         segs = line_segments(norm, ranges, fr, logp, shift, vit, words, word_first)
-        return LongformAlignment(segments=segs, log_likelihood=ll, confidence=path_confidence(vit, int(path_rows[0])))
+        if log_theta is None:
+            return LongformAlignment(segments=segs, log_likelihood=ll, confidence=path_confidence(vit, int(path_rows[0])))
+        matched = int(path_rows[0]) - int(u_rows[0])
+        conf = gap_confidence(vit, float(u_logp[0]), matched)
+        return LongformAlignment(segments=segs, log_likelihood=ll, confidence=conf, unmatched=unmatched_intervals(unmatched[0], shift))
 
     @torch.inference_mode()
     def transcribe_windowed(self, wav_file, word_timestamps: bool = False, confidence: bool = False, window: float = 30.0,

@@ -113,11 +113,16 @@ class LongformAlignment(_Record):
     """`align_longform()` result: one `Segment` per input line, in order (its normalised text, the start of its first token's
     frame and the end of its last, its words, and `confidence` = exp(mean log-probability of its tokens)), plus the
     whole recording's `log_likelihood` (forward score) and `confidence` = exp(Viterbi path score / frames), as in
-    `Alignment`."""
-    __slots__ = _fields = ("segments", "log_likelihood", "confidence")
+    `Alignment`.  With `gap_threshold`, `unmatched` holds the (start, end) seconds of every maximal run of frames the text
+    left unaligned, `log_likelihood` is the forward score of the graph with gaps and `confidence` = exp((Viterbi score -
+    score of the unmatched frames) / matched frames) (NaN when no frame is matched); without it `unmatched` is None."""
+    __slots__ = _fields = ("segments", "log_likelihood", "confidence", "unmatched")
+    _defaults = {"unmatched": None}
+    _quiet = ("unmatched",)
     segments: List[Segment]
     log_likelihood: float
     confidence: float
+    unmatched: Optional[List[Tuple[float, float]]]
 
     @property
     def text(self) -> str:

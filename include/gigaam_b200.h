@@ -315,6 +315,37 @@ int64_t gam_ctc_align_long_workspace_bytes(const gam_handle* h, int32_t B, int32
 int gam_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets, const int32_t* target_len,
                        int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
                        float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream);
+/* gam_ctc_align_long for a text that only partly matches the recording: audio between lines that the text lacks is left
+ * unaligned and reported.  An exact Viterbi (and forward) over the same states, transitions, tie rules and outputs as
+ * gam_ctc_align_long; only what some blank states emit changes.
+ *   - line_edges [B, U] u8 (device; may be NULL when U == 0): bit 0 = token i starts a line, bit 1 = it ends one.
+ *   - Boundary states: state 0, state 2 U_b, the blank just before every token that starts a line and the blank just after
+ *     every token that ends one.  (Between two charwise lines joined by a space token, those are the blanks on both sides of
+ *     the space; the space itself is still required.)
+ *   - Emission: at frame t a boundary state emits e_t = max(lp[t, blank], m[t] + log_theta) in both recursions, where
+ *     m[t] = max_c lp[t, c] as gam_ctc_spot computes it (exact; a zero max is +0) and m[t] + log_theta is one fp32 add.  Every
+ *     other state emits lp[t, l'_s] as before.
+ *   - log_theta: the fp32 log of a threshold theta in (0, 1], a per-frame likelihood ratio to the greedy decoder as in
+ *     gam_ctc_spot; -inf is accepted and gives gam_ctc_align_long's graph (on NaN-free input its bits, and no frame flagged).
+ *     NaN and values > 0 are refused.
+ *   - NaN rule: a recording reads the whole row lp[t, 0..V] of every frame t < T_b, so a NaN anywhere in those rows poisons it,
+ *     with gam_ctc_align_long's outputs for a poisoned recording.
+ * Outputs, besides gam_ctc_align_long's:
+ *   unmatched [B, T] u8: 1 where the Viterbi path sits in a boundary state at frame t and m[t] + log_theta > lp[t, blank]
+ *     strictly (a tie is matched), else 0; 0 at every t >= T_b and for a recording without a path or poisoned;
+ *   unmatched_rows [B] i32: the number of unmatched frames;
+ *   unmatched_logp [B] f32: the fp32 sum of m[t] + log_theta over the unmatched frames in frame order (0 when there are none,
+ *     NaN for a poisoned recording).
+ * Workspace: gam_ctc_align_long's backpointers plus B * T * 4 bytes of m[t], each rounded up to 1 KiB; *_workspace_bytes
+ * returns -1 where gam_ctc_align_long_workspace_bytes does.  Two launches (the pre-pass that fills m, then the sweep), fixed
+ * orders and no atomics: the same bits at every cluster size and in any batch.  Stream-ordered, no host synchronisation,
+ * capturable in a CUDA graph.  Refuses everything gam_ctc_align_long refuses. */
+int64_t gam_ctc_align_long_gaps_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                            const int32_t* target_len, const uint8_t* line_edges, int32_t B, int32_t T, int32_t U, float log_theta,
+                            void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp, float* viterbi_logp,
+                            float* log_likelihood, int32_t* path_rows, uint8_t* unmatched, int32_t* unmatched_rows,
+                            float* unmatched_logp, void* stream);
 /* ---- CTC keyword spotting: where in a recording each of K keywords was said, and how sure that is.  One exact Viterbi
  * per (recording, keyword) over the caller's fp32 log-probs; no hypothesis search.
  *
@@ -582,6 +613,12 @@ int gam_test_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t
                             const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes,
                             int32_t* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int32_t* path_rows,
                             int32_t cluster_ctas, int32_t* plan, void* stream);
+/* gam_ctc_align_long_gaps with the cluster size forced, as gam_test_ctc_align_long */
+int gam_test_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                                 const int32_t* target_len, const uint8_t* line_edges, int32_t B, int32_t T, int32_t U, float log_theta,
+                                 void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp, float* viterbi_logp,
+                                 float* log_likelihood, int32_t* path_rows, uint8_t* unmatched, int32_t* unmatched_rows,
+                                 float* unmatched_logp, int32_t cluster_ctas, int32_t* plan, void* stream);
 /* gam_ctc_spot with the keyword warps per CTA forced to warps_per_cta in [1, 32] (0: the library's choice); the outputs do
  * not depend on it. */
 int gam_test_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,

@@ -1,15 +1,19 @@
 """Cost of long-form alignment (GigaAMASR.align_longform: window encoding, CTC log-probs, stitching, gam_ctc_align_long and
 word grouping), with CUDA events.
 
-    python tools/align_long_probe.py [--quick]
+    python tools/align_long_probe.py [--quick] [--gaps]
 
 Part 1, the kernel: gam_ctc_align_long on random log-probs [1, 2000, 34] for U = 1k ... 64k tokens at forced cluster sizes
 C = 1, 4 and 16 (where the states fit), as time per frame.  The backtrack's share is the difference to the same call with one
 target class at -inf on every frame: that sweep does the same work, but there is no path to walk back.
 Part 2, the whole call on synthetic 16-layer models (fp16 encoder) over 10 and 60 minutes of synthetic audio, at V + 1 = 34
 (v2_ctc) and 257 (v3_e2e_ctc), with random targets of U = min(T / 2, 65 536) tokens: each stage timed on its own, and the
-peak device memory (torch.cuda.max_memory_allocated) of one whole pass.  The card's name, power limit and SM clocks are read
-in the same run; the last line is one JSON record of everything printed."""
+peak device memory (torch.cuda.max_memory_allocated) of one whole pass.
+Part 3, alignment with gaps: gam_ctc_align_long_gaps (its row-max pre-pass and sweep) against gam_ctc_align_long on the same
+random log-probs at V + 1 = 34 and 257, for T = 2000 frames at U = 1k ... 64k tokens in lines of 500 tokens, and for an hour
+(T = 90 000, U = 65 536), at the library's cluster size; medians of 7 (3 for the hour), the two calls alternating.  --gaps runs
+part 3 alone.
+The card's name, power limit and SM clocks are read in the same run; the last line is one JSON record of everything printed."""
 import json
 import statistics
 import subprocess
@@ -135,14 +139,48 @@ def call_part(name, minutes, batch_size=16):
     return row
 
 
+def gaps_part(quick):
+    rows = []
+    for name in ("v2_ctc", "v3_e2e_ctc"):
+        ck = gigaam.synthetic_checkpoint(name, seed=0, n_layers=1)
+        eng = gigaam.load_model(name, fp16_encoder=False, device=dev, checkpoint=ck)._get_engine()
+        V1 = eng.num_classes
+        g = torch.Generator().manual_seed(V1)
+        sizes = [(2000, 1024), (2000, 65536)] if quick else [(2000, u) for u in (1024, 4096, 16384, 32768, 65536)]
+        for T, U in sizes + [(90000, 65536)]:
+            lp = torch.randn(1, T, V1, generator=g).log_softmax(-1).to(dev)
+            y = torch.randint(0, V1 - 1, (1, U), generator=g, dtype=torch.int32).to(dev)
+            edges = torch.tensor(longform.line_edges([(a, min(a + 500, U)) for a in range(0, U, 500)], U), dtype=torch.uint8)
+            args = (torch.tensor([T]), y, torch.tensor([U]))
+            gaps = (edges[None].to(dev), -0.6931472)
+            reps, warm = (3, 1) if T > 2000 else (7, 2)
+            plain_ms, gap_ms = [], []
+            for _ in range(warm):
+                eng.ctc_align_long(lp, *args)
+                eng.ctc_align_long(lp, *args, gaps=gaps)
+            for _ in range(reps):                 # alternating, so that drift of the clocks hits both
+                plain_ms.append(median_ms(lambda: eng.ctc_align_long(lp, *args), warmup=0, reps=1))
+                gap_ms.append(median_ms(lambda: eng.ctc_align_long(lp, *args, gaps=gaps), warmup=0, reps=1))
+            a, b = statistics.median(plain_ms), statistics.median(gap_ms)
+            rows.append(dict(V1=V1, T=T, U=U, plain_ms=round(a, 3), gaps_ms=round(b, 3), ratio=round(b / a, 3)))
+            print(f"V+1={V1:4d} T={T:6d} U={U:6d}: gam_ctc_align_long {a:9.3f} ms, gaps {b:9.3f} ms ({b / a:.3f}x)", flush=True)
+            del lp
+        del eng
+        torch.cuda.empty_cache()
+    return rows
+
+
 def main():
     quick = "--quick" in sys.argv
     info = card()
     print(info, flush=True)
-    rec = dict(card=info, kernel=kernel_part(quick), calls=[])
-    for name in ("v2_ctc", "v3_e2e_ctc"):
-        for minutes in ((10,) if quick else (10, 60)):
-            rec["calls"].append(call_part(name, minutes))
+    if "--gaps" in sys.argv:
+        rec = dict(card=info, gaps=gaps_part(quick))
+    else:
+        rec = dict(card=info, kernel=kernel_part(quick), calls=[], gaps=gaps_part(quick))
+        for name in ("v2_ctc", "v3_e2e_ctc"):
+            for minutes in ((10,) if quick else (10, 60)):
+                rec["calls"].append(call_part(name, minutes))
     print(json.dumps(rec))
 
 
