@@ -21,11 +21,13 @@ from .engine import max_encoded_frames_config
 from .model import GigaAM, GigaAMASR, GigaAMEmo, check_emo_head
 from .preprocess import load_audio
 from .synthetic import synthetic_audio, synthetic_checkpoint
-from .types import Alignment, Detection, LongformAlignment, LongformTranscriptionResult, Segment, TranscriptionResult, Word
+from .streaming import StreamServer
+from .types import (Alignment, Detection, LongformAlignment, LongformTranscriptionResult, Segment, StreamResult, StreamUpdate,
+                    TranscriptionResult, Word)
 
 __all__ = ["GigaAM", "GigaAMASR", "GigaAMEmo", "load_audio", "load_model", "synthetic_checkpoint", "synthetic_audio",
            "TranscriptionResult", "Word", "Segment", "LongformTranscriptionResult", "Alignment",
-           "LongformAlignment", "Detection"]
+           "LongformAlignment", "Detection", "StreamServer", "StreamUpdate", "StreamResult"]
 
 _CACHE_DIR = os.path.expanduser("~/.cache/gigaam")
 _MODEL_NAMES = ["emo", "v1_ctc", "v1_rnnt", "v1_ssl", "v2_ctc", "v2_rnnt", "v2_ssl", "v3_ctc", "v3_rnnt",

@@ -66,7 +66,8 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_rnnt_align", "gam_ctc_align_long_workspace_bytes", "gam_ctc_align_long", "gam_test_ctc_align_long",
            "gam_decode_state_bytes", "gam_decode_state_init", "gam_decode_resume_workspace_bytes", "gam_ctc_greedy_resume",
            "gam_rnnt_greedy_resume", "gam_ctc_spot", "gam_test_ctc_spot", "gam_ctc_bias_workspace_bytes", "gam_ctc_bias",
-           "gam_ctc_align_long_gaps_workspace_bytes", "gam_ctc_align_long_gaps", "gam_test_ctc_align_long_gaps")
+           "gam_ctc_align_long_gaps_workspace_bytes", "gam_ctc_align_long_gaps", "gam_test_ctc_align_long_gaps",
+           "gam_ctc_spot_state_bytes", "gam_ctc_spot_state_init", "gam_ctc_spot_resume")
 
 
 def lib_path() -> Path:
@@ -168,7 +169,12 @@ def load() -> C.CDLL:
         fn.restype = C.c_int
     lib.gam_ctc_spot.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32, C.c_float, i32] + [c_vp] * 5
     lib.gam_test_ctc_spot.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32, C.c_float, i32] + [c_vp] * 4 + [i32, c_vp]
-    for fn in (lib.gam_ctc_spot, lib.gam_test_ctc_spot):
+    lib.gam_ctc_spot_state_bytes.argtypes = [H, i32]
+    lib.gam_ctc_spot_state_bytes.restype = i64
+    lib.gam_ctc_spot_state_init.argtypes = [H, c_vp, i32, i32, i32, c_vp]
+    lib.gam_ctc_spot_resume.argtypes = ([H, c_vp, i32, i32] + [c_vp] * 6 + [i32, i32, C.c_float, i32, c_vp, i64] + [c_vp] * 7
+                                        + [c_vp])
+    for fn in (lib.gam_ctc_spot, lib.gam_test_ctc_spot, lib.gam_ctc_spot_state_init, lib.gam_ctc_spot_resume):
         fn.restype = C.c_int
     lib.gam_ctc_bias_workspace_bytes.argtypes = [H, i32, i32, i32, i32]
     lib.gam_ctc_bias_workspace_bytes.restype = i64

@@ -999,7 +999,7 @@ int gam_test_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const in
 }
 
 // ---- keyword spotting (csrc/spot.cu)
-static int ctc_spot_run(gam_handle* h, const char* what, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T,
+static int ctc_spot_run(gam_handle* h, const char* what, const float* log_probs, const SpotResume& io, int32_t B, int32_t T,
                         const int32_t* keywords, const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det,
                         int32_t* det_start, int32_t* det_end, float* det_score, int32_t* det_count, int32_t warps, void* stream) {
   const gam_config& c = h->cfg;
@@ -1009,13 +1009,13 @@ static int ctc_spot_run(gam_handle* h, const char* what, const float* log_probs,
   if (Umax < 1 || Umax > kSpotMaxTokens) return fail(h, -1, "%s: Umax=%d outside [1, %d] tokens per keyword", what, Umax, kSpotMaxTokens);
   if (!(threshold > 0.f && threshold <= 1.f)) return fail(h, -1, "%s: threshold %g outside (0, 1]", what, static_cast<double>(threshold));
   if (max_det < 1) return fail(h, -1, "%s: max_det=%d must be >= 1", what, max_det);
-  if (!log_probs || !enc_len || !keywords || !keyword_len || !det_start || !det_end || !det_score || !det_count)
+  if (!log_probs || !io.hi || !keywords || !keyword_len || !det_start || !det_end || !det_score || !det_count)
     return fail(h, -1, "%s: a required pointer is NULL", what);
   const float log_theta = static_cast<float>(std::log(static_cast<double>(threshold)));   // correctly rounded to fp32
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc;
   { PROF(PC_ALIGN);
-    rc = launch_ctc_spot(log_probs, enc_len, keywords, keyword_len, B, T, c.num_classes, K, Umax, log_theta, max_det, warps, det_start,
+    rc = launch_ctc_spot(log_probs, io, keywords, keyword_len, B, T, c.num_classes, K, Umax, log_theta, max_det, warps, det_start,
                          det_end, det_score, det_count, s); }
   if (rc == 1) return fail(h, -1, "%s: a frame of %d classes does not fit in shared memory", what, c.num_classes);
   if (rc != 0) return fail(h, -4, "%s: launch rejected (rc=%d): %s", what, rc, cudaGetErrorString(cudaGetLastError()));
@@ -1023,11 +1023,49 @@ static int ctc_spot_run(gam_handle* h, const char* what, const float* log_probs,
   return 0;
 }
 
+// a one-shot call: fresh records over [0, enc_len[b]), finished
+static SpotResume spot_fresh_io(const int32_t* enc_len) {
+  SpotResume io{};
+  io.hi = enc_len;
+  return io;
+}
+
+int64_t gam_ctc_spot_state_bytes(const gam_handle* h, int32_t Umax) {
+  if (!h || h->cfg.head != 1 || Umax < 1 || Umax > kSpotMaxTokens) return -1;
+  return ctc_spot_record_bytes(Umax);
+}
+
+int gam_ctc_spot_state_init(gam_handle* h, void* state, int32_t n, int32_t K, int32_t Umax, void* stream) {
+  const int64_t bytes = gam_ctc_spot_state_bytes(h, Umax);
+  if (bytes < 0) return fail(h, -1, "ctc_spot_state_init: no CTC head, or Umax=%d outside [1, %d]", Umax, kSpotMaxTokens);
+  if (n < 0 || K < 1 || static_cast<int64_t>(n) * K > INT32_MAX || (n > 0 && state == nullptr))
+    return fail(h, -1, "ctc_spot_state_init: bad state buffer (n=%d, K=%d)", n, K);
+  launch_ctc_spot_state_init(static_cast<uint8_t*>(state), static_cast<int64_t>(n) * K, Umax, static_cast<cudaStream_t>(stream));
+  GAM_CHECK_LAUNCH(h, "ctc_spot_state_init");
+  return 0;
+}
+
+int gam_ctc_spot_resume(gam_handle* h, const float* log_probs, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
+                        const int32_t* frame_base, const int32_t* finish, const int32_t* keywords, const int32_t* keyword_len, int32_t K,
+                        int32_t Umax, float threshold, int32_t max_det, void* state, int64_t record_bytes, int32_t* det_start,
+                        int32_t* det_end, float* det_score, int32_t* det_count, int32_t* pend_start, int32_t* pend_end,
+                        float* pend_score, void* stream) {
+  if (!lo || !hi || !frame_base || !finish || !state) return fail(h, -1, "ctc_spot_resume: lo, hi, frame_base, finish and state are required");
+  if (Umax >= 1 && Umax <= kSpotMaxTokens && record_bytes != ctc_spot_record_bytes(Umax))
+    return fail(h, -1, "ctc_spot_resume: record_bytes=%lld, but Umax=%d needs %lld", (long long)record_bytes, Umax,
+                (long long)ctc_spot_record_bytes(Umax));
+  if (!pend_start != !pend_end || !pend_start != !pend_score)
+    return fail(h, -1, "ctc_spot_resume: pend_start, pend_end and pend_score go together");
+  SpotResume io{lo, hi, frame_base, finish, static_cast<uint8_t*>(state), record_bytes, pend_start, pend_end, pend_score};
+  return ctc_spot_run(h, "ctc_spot_resume", log_probs, io, B, T, keywords, keyword_len, K, Umax, threshold, max_det, det_start, det_end,
+                      det_score, det_count, 0, stream);
+}
+
 int gam_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
                  const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det, int32_t* det_start,
                  int32_t* det_end, float* det_score, int32_t* det_count, void* stream) {
-  return ctc_spot_run(h, "ctc_spot", log_probs, enc_len, B, T, keywords, keyword_len, K, Umax, threshold, max_det, det_start, det_end,
-                      det_score, det_count, 0, stream);
+  return ctc_spot_run(h, "ctc_spot", log_probs, spot_fresh_io(enc_len), B, T, keywords, keyword_len, K, Umax, threshold, max_det,
+                      det_start, det_end, det_score, det_count, 0, stream);
 }
 
 int gam_test_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
@@ -1035,8 +1073,8 @@ int gam_test_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_
                       int32_t* det_end, float* det_score, int32_t* det_count, int32_t warps_per_cta, void* stream) {
   if (warps_per_cta < 0 || warps_per_cta > kSpotMaxWarps)
     return fail(h, -1, "test_ctc_spot: warps_per_cta=%d outside [0, %d]", warps_per_cta, kSpotMaxWarps);
-  return ctc_spot_run(h, "test_ctc_spot", log_probs, enc_len, B, T, keywords, keyword_len, K, Umax, threshold, max_det, det_start,
-                      det_end, det_score, det_count, warps_per_cta, stream);
+  return ctc_spot_run(h, "test_ctc_spot", log_probs, spot_fresh_io(enc_len), B, T, keywords, keyword_len, K, Umax, threshold,
+                      max_det, det_start, det_end, det_score, det_count, warps_per_cta, stream);
 }
 
 // ---- hotwords (csrc/bias.cu)

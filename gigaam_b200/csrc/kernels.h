@@ -178,7 +178,31 @@ constexpr int kSpotMaxTokens = 64;
 constexpr int kSpotWarps = 8;
 constexpr int kSpotMaxWarps = 32;
 int ctc_spot_plan(int V1, int* rows, int* smem_bytes);
-int launch_ctc_spot(const float* log_probs, const int* enc_len, const int* keywords, const int* keyword_len, int B, int T, int V1, int K,
+// The record of one (stream, keyword) between resume calls (gam_ctc_spot_state_bytes): this header, then each record lane's
+// v[4] as f32 [4][lanes] and its start frames a[4] as i32 [4][lanes], lanes = ceil((2 Umax - 1) / 4).
+struct SpotRecord {
+  int has, p_start, p_end, total;   // the pending detection (when has) and the true count of detections emitted
+  float p_score;
+  int pad[3];
+};
+static_assert(sizeof(SpotRecord) == 32, "SpotRecord is one 32-byte header");
+// Row b walks local frames [lo[b], hi[b]) (clamped to [0, T]) as stream frames frame_base[b] + t, from and back to its records at
+// state + (b K + k) record; finish[b] != 0 emits the pending detection at the end.  state == NULL: a fresh call over [0, hi[b])
+// (hi = enc_len; lo, frame_base, finish and pend_* unused).
+struct SpotResume {
+  const int* lo;
+  const int* hi;
+  const int* frame_base;
+  const int* finish;
+  uint8_t* state;
+  int64_t record;
+  int* pend_start;   // [B, K], or NULL
+  int* pend_end;
+  float* pend_score;
+};
+int64_t ctc_spot_record_bytes(int Umax);
+void launch_ctc_spot_state_init(uint8_t* state, int64_t n, int Umax, cudaStream_t s);
+int launch_ctc_spot(const float* log_probs, const SpotResume& io, const int* keywords, const int* keyword_len, int B, int T, int V1, int K,
                     int Umax, float log_theta, int max_det, int warps, int* det_start, int* det_end, float* det_score, int* det_count,
                     cudaStream_t s);
 

@@ -9,6 +9,9 @@
 // (lane 0 stores a detection when it is emitted), so nothing of size T x K is stored.  A warp reads only its own keyword
 // and the per-frame m, whose max is exact in any order: a (recording, keyword) pair gets the same bits in any batch, keyword
 // order or warps-per-CTA choice.  No atomics, no host synchronisation.
+// Resumable (gam_ctc_spot_resume): a row walks its local frames [lo, hi) as stream frames frame_base + t, and each warp loads
+// its (stream, keyword) SpotRecord before the walk and stores it after, so a stream split into consecutive calls gives the
+// one-shot bits.  A one-shot call (gam_ctc_spot) is the same walk from fresh registers over [0, enc_len) with finish.
 #include <algorithm>
 #include <cmath>
 
@@ -26,7 +29,10 @@ constexpr int kSpotMaxRows = 32;        // frames per tile at most
 constexpr int kSpotHeader = 1024;       // mbarriers at 0, m[t] of every stage at 128, tiles from here
 constexpr unsigned kFull = 0xffffffffu;
 
-__global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict__ log_probs, const int* __restrict__ enc_len,
+// lanes of a record: those that own at least one of the 2 Umax - 1 states
+__host__ __device__ constexpr int spot_record_lanes(int Umax) { return (2 * Umax - 1 + 3) / 4; }
+
+__global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict__ log_probs, const SpotResume io,
                                                         const int* __restrict__ keywords, const int* __restrict__ keyword_len, int T,
                                                         int V1, int K, int Umax, float log_theta, int max_det, int R, int stage_bytes,
                                                         int* __restrict__ det_start, int* __restrict__ det_end,
@@ -37,7 +43,10 @@ __global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict_
   unsigned char* tiles = smem + kSpotHeader;            // [kSpotStages][stage_bytes]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
   const int b = blockIdx.y, k = blockIdx.x * nw + warp;
-  const int Tb = min(max(enc_len[b], 0), T);
+  // local frames [f0, Tb) of row b; frame t of the row is frame fb + t of its stream (0 on a fresh call)
+  const bool resume = io.state != nullptr;
+  const int Tb = min(max(io.hi[b], 0), T);
+  const int f0 = resume ? min(max(io.lo[b], 0), Tb) : 0, fb = resume ? io.frame_base[b] : 0;
   const int blank = V1 - 1;
 
   // ---- this warp's keyword: labels of its lane's four states, and which even states may skip the blank before them
@@ -73,8 +82,30 @@ __global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict_
 
   float v[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
   int a[4] = {0, 0, 0, 0};
-  int count = 0, has = 0, p_start = 0, p_end = 0;
+  int has = 0, p_start = 0, p_end = 0, total = 0;
   float p_score = 0.f;
+  // the stream's record: loaded once before the frame walk, stored once after it
+  const int L = spot_record_lanes(Umax);
+  SpotRecord* rec = resume && k < K ? reinterpret_cast<SpotRecord*>(io.state + (static_cast<int64_t>(b) * K + k) * io.record) : nullptr;
+  float* rec_v = rec ? reinterpret_cast<float*>(rec + 1) : nullptr;   // [4][L]
+  int* rec_a = rec ? reinterpret_cast<int*>(rec_v + 4 * L) : nullptr;  // [4][L]
+  if (rec && active) {
+    has = rec->has;
+    p_start = rec->p_start;
+    p_end = rec->p_end;
+    p_score = rec->p_score;
+    total = rec->total;
+    if (lane < L) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        v[j] = rec_v[j * L + lane];
+        a[j] = rec_a[j * L + lane];
+      }
+    }
+  }
+  // detections stored so far: appended after the caller's count on a resume call
+  const int base = resume && k < K ? min(max(det_count[static_cast<int64_t>(b) * K + k], 0), max_det) : 0;
+  int count = base;
   auto emit = [&]() {
     if (lane == 0 && count < max_det) {
       det_start[row0 + count] = p_start;
@@ -90,13 +121,13 @@ __global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict_
     ptx::fence_mbar_init();
   }
   const int any = __syncthreads_or(active);
-  const int ntiles = any ? (Tb + R - 1) / R : 0;
-  const float* lp = log_probs + static_cast<int64_t>(b) * T * V1;
+  const int ntiles = any ? (Tb - f0 + R - 1) / R : 0;
+  const float* lp = log_probs + (static_cast<int64_t>(b) * T + f0) * V1;
   // tile i: frames [i R, i R + n) copied from the 16-byte boundary at or below its first row up to the one at or above its
   // end; its first row lands `skew` bytes into the stage
   auto tile_src = [&](int i) { return reinterpret_cast<uintptr_t>(lp + static_cast<int64_t>(i) * R * V1); };
   auto issue = [&](int i) {
-    const int st = i % kSpotStages, n = min(R, Tb - i * R);
+    const int st = i % kSpotStages, n = min(R, Tb - f0 - i * R);
     const uintptr_t lo = tile_src(i) & ~uintptr_t(15);
     const uintptr_t hi = (tile_src(i) + static_cast<uintptr_t>(n) * V1 * 4 + 15) & ~uintptr_t(15);
     ptx::mbar_arrive_expect_tx(&full[st], static_cast<uint32_t>(hi - lo));
@@ -106,7 +137,7 @@ __global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict_
     for (int i = 0; i < min(kSpotStages, ntiles); ++i) issue(i);
 
   for (int i = 0; i < ntiles; ++i) {
-    const int st = i % kSpotStages, n = min(R, Tb - i * R);
+    const int st = i % kSpotStages, n = min(R, Tb - f0 - i * R);
     ptx::mbar_wait(&full[st], (i / kSpotStages) & 1);
     const float* tile = reinterpret_cast<const float*>(tiles + st * stage_bytes + (tile_src(i) & 15));
     float* m = mrow + st * R;
@@ -118,7 +149,7 @@ __global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict_
     if (tid == 0 && i >= 1 && i - 1 + kSpotStages < ntiles) issue(i - 1 + kSpotStages);
     if (!active) continue;
     for (int r = 0; r < n; ++r) {
-      const int t = i * R + r;
+      const int t = fb + f0 + i * R + r;
       const float* row = tile + static_cast<int64_t>(r) * V1;
       const float mt = m[r];
       // frame t - 1 of lane - 1's last two states: the s - 1 / s - 2 predecessors of this lane's first two
@@ -175,7 +206,45 @@ __global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict_
     }
   }
   if (k >= K) return;
-  if (has) emit();
+  if (has) {
+    // a call without finish emits the pending detection early when no live path (finite score) starts before its end: a
+    // later candidate starts at or after it, so it can no longer be replaced, only follow
+    bool blocked = false;
+    if (resume && io.finish[b] == 0) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) blocked |= v[j] > -INFINITY && a[j] < p_end;
+    }
+    if (!__any_sync(kFull, blocked)) {
+      emit();
+      has = 0;
+    }
+  }
+  if (resume) {
+    if (active) {
+      if (lane < L) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          rec_v[j * L + lane] = v[j];
+          rec_a[j * L + lane] = a[j];
+        }
+      }
+      if (lane == 0) {
+        rec->has = has;
+        rec->p_start = p_start;
+        rec->p_end = p_end;
+        rec->p_score = p_score;
+        rec->total = total + (count - base);
+        det_count[static_cast<int64_t>(b) * K + k] = min(count, max_det);
+      }
+    }
+    if (lane == 0 && io.pend_start) {
+      const int64_t p = static_cast<int64_t>(b) * K + k;
+      io.pend_start[p] = has ? p_start : -1;
+      io.pend_end[p] = has ? p_end : -1;
+      io.pend_score[p] = has ? p_score : active ? -INFINITY : __int_as_float(0x7fc00000);
+    }
+    return;
+  }
   if (lane == 0) det_count[static_cast<int64_t>(b) * K + k] = active ? count : 0;
   const float fill = active ? -INFINITY : __int_as_float(0x7fc00000);
   for (int i = (active ? min(count, max_det) : 0) + lane; i < max_det; i += 32) {
@@ -185,7 +254,28 @@ __global__ void __launch_bounds__(1024) ctc_spot_kernel(const float* __restrict_
   }
 }
 
+__global__ void spot_state_init_kernel(uint8_t* state, int64_t n, int L, int64_t record) {
+  const int64_t r = blockIdx.x;
+  if (r >= n) return;
+  SpotRecord* rec = reinterpret_cast<SpotRecord*>(state + r * record);
+  float* v = reinterpret_cast<float*>(rec + 1);
+  int* a = reinterpret_cast<int*>(v + 4 * L);
+  for (int i = threadIdx.x; i < 4 * L; i += blockDim.x) {
+    v[i] = -INFINITY;
+    a[i] = 0;
+  }
+  if (threadIdx.x == 0) *rec = SpotRecord{0, 0, 0, 0, 0.f, {0, 0, 0}};
+}
+
 }  // namespace
+
+int64_t ctc_spot_record_bytes(int Umax) {
+  return static_cast<int64_t>(sizeof(SpotRecord)) + 8 * 4 * static_cast<int64_t>(spot_record_lanes(Umax));
+}
+
+void launch_ctc_spot_state_init(uint8_t* state, int64_t n, int Umax, cudaStream_t s) {
+  if (n > 0) spot_state_init_kernel<<<static_cast<unsigned>(n), 128, 0, s>>>(state, n, spot_record_lanes(Umax), ctc_spot_record_bytes(Umax));
+}
 
 int ctc_spot_plan(int V1, int* rows, int* smem_bytes) {
   int dev = 0, cap = 0;
@@ -200,7 +290,7 @@ int ctc_spot_plan(int V1, int* rows, int* smem_bytes) {
   return 0;
 }
 
-int launch_ctc_spot(const float* log_probs, const int* enc_len, const int* keywords, const int* keyword_len, int B, int T, int V1, int K,
+int launch_ctc_spot(const float* log_probs, const SpotResume& io, const int* keywords, const int* keyword_len, int B, int T, int V1, int K,
                     int Umax, float log_theta, int max_det, int warps, int* det_start, int* det_end, float* det_score, int* det_count,
                     cudaStream_t s) {
   static PerDeviceOnce attr_once;
@@ -216,7 +306,7 @@ int launch_ctc_spot(const float* log_probs, const int* enc_len, const int* keywo
   if (warps <= 0) warps = std::min(kSpotWarps, K);
   const int stage_bytes = (smem - kSpotHeader) / kSpotStages;
   const dim3 grid((K + warps - 1) / warps, B);
-  ctc_spot_kernel<<<grid, 32 * warps, smem, s>>>(log_probs, enc_len, keywords, keyword_len, T, V1, K, Umax, log_theta, max_det, R,
+  ctc_spot_kernel<<<grid, 32 * warps, smem, s>>>(log_probs, io, keywords, keyword_len, T, V1, K, Umax, log_theta, max_det, R,
                                                  stage_bytes, det_start, det_end, det_score, det_count);
   return 0;
 }

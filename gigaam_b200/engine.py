@@ -779,6 +779,41 @@ class Engine:
         _lib.check(self.lib, self.handle, rc, "gam_ctc_spot")
         return outs
 
+    def spot_state(self, n: int, K: int, Umax: int) -> Tensor:
+        """n x K fresh keyword-spotting records (gam_ctc_spot_state_init): uint8 [n, K, gam_ctc_spot_state_bytes(Umax)] on the
+        device."""
+        nbytes = int(self.lib.gam_ctc_spot_state_bytes(self.handle, int(Umax)))
+        if nbytes < 0:
+            raise ValueError(f"spot_state: no CTC head, or Umax={Umax} outside [1, 64]")
+        state = torch.empty((n, K, nbytes), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_ctc_spot_state_init(self.handle, state.data_ptr(), n, K, int(Umax), self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_ctc_spot_state_init")
+        return state
+
+    def ctc_spot_resume(self, log_probs: Tensor, lo: Tensor, hi: Tensor, frame_base: Tensor, finish: Tensor, keywords: Tensor,
+                        keyword_len: Tensor, threshold: float, state: Tensor, det: Tuple[Tensor, ...],
+                        pending: Optional[Tuple[Tensor, ...]] = None) -> None:
+        """Spot over local frames [lo[b], hi[b]) of log_probs [B, T, V+1] as stream frames frame_base[b] + t, continuing the
+        records state [B, K, bytes] (spot_state) (gam_ctc_spot_resume).  lo / hi / frame_base / finish: device int32 [B].
+        det = (start, end, score [B, K, max_det], count [B, K]) on the device: detections are appended at count.  `pending` =
+        (start, end, score [B, K]) receives the pending detections."""
+        assert log_probs.is_cuda and log_probs.dtype == torch.float32 and log_probs.is_contiguous() and log_probs.dim() == 3
+        B, T, _ = log_probs.shape
+        K, Umax = keywords.shape
+        for t in (lo, hi, frame_base, finish, keywords, keyword_len):
+            assert t.device == self.device and t.dtype == torch.int32 and t.is_contiguous()
+        assert state.dtype == torch.uint8 and state.is_contiguous() and tuple(state.shape[:2]) == (B, K)
+        assert all(t.is_contiguous() and t.shape[:2] == (B, K) for t in det)
+        max_det = det[0].shape[2]
+        pend = [None] * 3 if pending is None else [t.data_ptr() for t in pending]
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_ctc_spot_resume(self.handle, log_probs.data_ptr(), B, T, lo.data_ptr(), hi.data_ptr(), frame_base.data_ptr(),
+                                              finish.data_ptr(), keywords.data_ptr(), keyword_len.data_ptr(), K, Umax, float(threshold),
+                                              int(max_det), state.data_ptr(), state.shape[2], *[t.data_ptr() for t in det], *pend,
+                                              self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_ctc_spot_resume")
+
     def ctc_bias(self, log_probs: Tensor, enc_len: Tensor, keywords: Tensor, keyword_len: Tensor, spotted: Tuple[Tensor, ...],
                  threshold: float, token_flags: Tensor, ids: Tensor, frames: Tensor, counts: Tensor,
                  token_logp: Optional[Tensor] = None, path_logp: Optional[Tensor] = None, frame_logp: Optional[Tensor] = None

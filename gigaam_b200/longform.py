@@ -167,28 +167,44 @@ def window_batches(model, wav: Tensor, windows: Sequence[Window], batch_size: in
     window order through `model.forward` (the varlen path), in batches of up to `batch_size` windows of one length: no
     padding, so no row depends on its neighbours.  Windows that keep no frame are skipped.  A host waveform is uploaded one
     batch at a time.  Yields (the batch's windows, encoded [nb, d, T_w])."""
+    for group in window_groups(windows, batch_size, lambda w: w):
+        yield group, encode_rows(model, [wav[w.start:w.end] for w in group])
+
+
+def window_groups(items: Sequence, batch_size: int, window_of: Callable[[object], Window]) -> List[List]:
+    """`window_batches`' batches: consecutive items whose windows have one length, up to `batch_size` of them; items whose
+    window keeps no frame are left out."""
     if batch_size < 1:
         raise ValueError("batch_size must be >= 1")
-    dev = model._device
-    groups: List[List[Window]] = []
-    for w in windows:
+    groups: List[List] = []
+    length = None
+    for item in items:
+        w = window_of(item)
         if w.keep_end <= w.keep_start:
             continue
-        if groups and len(groups[-1]) < batch_size and groups[-1][0].end - groups[-1][0].start == w.end - w.start:
-            groups[-1].append(w)
+        if groups and len(groups[-1]) < batch_size and length == w.end - w.start:
+            groups[-1].append(item)
         else:
-            groups.append([w])
-    for group in groups:
-        length = group[0].end - group[0].start
-        if wav.device == dev:
-            batch = torch.stack([wav[w.start:w.end] for w in group])
-        else:
-            staged = torch.empty((len(group), length), dtype=wav.dtype, pin_memory=True)
-            torch.stack([wav[w.start:w.end] for w in group], out=staged)
-            batch = staged.to(dev, non_blocking=True)
-        lens = torch.full((len(group),), length, dtype=torch.int64, device=dev)
-        encoded, _ = model.forward(batch, lens)
-        yield group, encoded
+            groups.append([item])
+            length = w.end - w.start
+    return groups
+
+
+def encode_rows(model, rows: Sequence[Tensor]) -> Tensor:
+    """Encode equal-length waveforms (in the model's dtype, all on the model's device or all on the host) as one batch through
+    `model.forward` (the varlen path) -> encoded [len(rows), d, T_w].  Host rows are staged in pinned memory and uploaded
+    without blocking."""
+    dev = model._device
+    length = rows[0].numel()
+    if rows[0].device == dev:
+        batch = torch.stack(list(rows))
+    else:
+        staged = torch.empty((len(rows), length), dtype=rows[0].dtype, pin_memory=True)
+        torch.stack(list(rows), out=staged)
+        batch = staged.to(dev, non_blocking=True)
+    lens = torch.full((len(rows),), length, dtype=torch.int64, device=dev)
+    encoded, _ = model.forward(batch, lens)
+    return encoded
 
 
 def stitch_ctc_log_probs(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16) -> Tensor:

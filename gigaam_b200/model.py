@@ -511,6 +511,15 @@ class GigaAMASR(GigaAM):
                                  words if word_timestamps else None, ws[:k], frame_logp, frame_rows)
         return LongformTranscriptionResult(segments=segs)
 
+    def streaming(self, window: float = 8.0, overlap: float = 4.0, batch_size: int = 64, confidence: bool = False,
+                  keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5):
+        """A `streaming.StreamServer` for live audio (INTEGRATION.md §7i): open streams, push chunks, `step()` for captions
+        and keyword alerts, `close()` for each stream's `transcribe_windowed` / `spot` result.  Raises before any device
+        work: ValueError for the window plan's refusals, batch_size < 1 and `spot`'s keyword and threshold checks;
+        NotImplementedError for keywords on an RNN-T model."""
+        from .streaming import StreamServer
+        return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold)
+
     # ---- keyword spotting (INTEGRATION.md §7g)
     def _refuse_rnnt_spot(self, what: str) -> None:
         if self._ncfg["head"].get("type") == "rnnt":

@@ -1,0 +1,385 @@
+"""Live streams (INTEGRATION.md §7i): many recordings that arrive a chunk at a time, transcribed and searched for keywords
+while they are spoken.
+
+Each stream is cut into `longform.plan_windows`' windows.  Window w of a stream is *ready* once the stream holds more than
+w H + W samples (W the window, H = W - V the hop): it is then never the last window of the plan, whatever length the
+stream reaches, so its samples and kept frames are final.  `StreamServer.step()` encodes every ready window of every
+stream in batches of equal-length windows (`longform.window_groups` / `encode_rows`, no padding) and decodes each batch's
+kept frames by rounds: one `Engine.greedy_resume` launch decodes the r-th window of every stream in the batch, with the
+streams' decoder records gathered from a device pool and scattered back.  CTC log-probs of the same batch feed
+`Engine.ctc_spot_resume` over the same frames.  `close()` encodes what is left, the last window included, and builds the
+result with `transcribe_windowed`'s and `spot`'s code, so a closed stream gets their output bit for bit.
+
+Device memory does not grow with a stream's duration: a stream owns one decoder record and one spot record per keyword, and
+every step's outputs are step-local.  The host keeps each stream's unencoded samples, its token ids, frames, token
+log-probs, per-frame sums and detections for `close`.  One caller drives a server; it is not thread-safe."""
+from __future__ import annotations
+
+import math
+from typing import Dict, List, Optional, Sequence, Tuple, Union
+
+import numpy as np
+import torch
+from torch import Tensor
+
+from . import _lib
+from .decoding import _as_btd
+from .longform import FRAME_SAMPLES, Window, _frame_multiple, encode_rows, plan_windows, segment_cuts, window_groups, windowed_segments
+from .preprocess import SAMPLE_RATE
+from .timestamps_utils import compute_frame_shift, token_flag_table, words_from_device
+from .types import Detection, LongformTranscriptionResult, StreamResult, StreamUpdate
+
+FRAME_SECONDS = FRAME_SAMPLES / SAMPLE_RATE   # the nominal 40 ms frame step of updates
+
+
+def ready_count(n_samples: int, W: int, V: int) -> int:
+    """How many windows of a stream holding n_samples samples are ready: window w is once n_samples > w H + W, H = W - V.
+    For N >= n_samples this is at most len(plan_windows(N)) - 1, so a ready window is never a plan's last one."""
+    return 0 if n_samples <= W else (n_samples - W - 1) // (W - V) + 1
+
+
+def ready_window(w: int, W: int, V: int) -> Window:
+    """Window w of every plan in which it is not the last one (`longform.plan_windows`' rule): samples [w H, w H + W) and kept
+    frames [c_w, c_{w+1}), c_0 = 0 and c_w = w H / 640 + floor(O / 2), O = V / 640."""
+    H, half = W - V, V // FRAME_SAMPLES // 2
+    return Window(w * H, w * H + W, 0 if w == 0 else w * H // FRAME_SAMPLES + half, (w + 1) * H // FRAME_SAMPLES + half)
+
+
+class TextFeed:
+    """A stream's committed text, a step at a time: `push(all_ids, n_new)` returns the text of the n_new ids just appended,
+    so that the concatenated returns equal tokenizer.decode(all_ids).  Only the ids from the last word opener on (a token in
+    `openers`: a space, or a SentencePiece piece starting with U+2581) are decoded again, which needs decoding to append
+    text past a word opener (decode(ids + more) extends decode(ids) when ids starts with one)."""
+
+    def __init__(self, tokenizer, openers):
+        self.tokenizer = tokenizer
+        self.openers = openers
+        self.anchor = 0        # index of the last word opener (0 before the first)
+        self.tail = ""         # decode(ids[anchor:]) as emitted
+
+    def push(self, ids: Sequence[int], n_new: int) -> str:
+        if n_new == 0:
+            return ""
+        text = self.tokenizer.decode(list(ids[self.anchor:]))
+        new = text[len(self.tail):]
+        self.tail = text
+        for i in range(len(ids) - 1, max(self.anchor, len(ids) - n_new) - 1, -1):
+            if ids[i] in self.openers:
+                self.anchor = i
+                self.tail = self.tokenizer.decode(list(ids[i:]))
+                break
+        return new
+
+
+class _Stream:
+    """Host side of one open stream."""
+
+    def __init__(self, sid: int, slot: int, feed: TextFeed, K: int, dtype: torch.dtype):
+        self.id, self.slot, self.feed = sid, slot, feed
+        self.n = 0                       # samples pushed
+        self.chunks: List[Tensor] = []   # pushed since the last consolidation
+        self.buf = torch.zeros(0, dtype=dtype)   # samples [buf_start, n) that a window not yet encoded may need
+        self.buf_start = 0
+        self.windows: List[Window] = []  # the windows handed to the encoder, in order
+        self.committed = 0               # frames decoded for good
+        self.ids: List[int] = []
+        self.frames: List[int] = []
+        self.token_logp: List[float] = []
+        self.frame_logp: List[np.ndarray] = []
+        self.frame_rows: List[np.ndarray] = []
+        self.dets: List[List[Tuple[int, int, float]]] = [[] for _ in range(K)]
+        self.pending: List[Optional[Tuple[int, int, float]]] = [None] * K
+        self.tentative: List[int] = []
+
+    def samples(self, start: int, end: int) -> Tensor:
+        if self.chunks:
+            self.buf = torch.cat([self.buf] + self.chunks)
+            self.chunks = []
+        return self.buf[start - self.buf_start:end - self.buf_start]
+
+    def trim(self, keep_from: int) -> None:
+        """Drop the samples before `keep_from` (the next window's first sample)."""
+        self.samples(keep_from, keep_from)
+        cut = keep_from - self.buf_start
+        if cut > 0:
+            self.buf = self.buf[cut:].clone()
+            self.buf_start = keep_from
+
+
+class StreamServer:
+    """Transcribe live audio streams, and spot keywords in them, with one encoder batch per step across all of them
+    (INTEGRATION.md §7i).  Made by `GigaAMASR.streaming(...)`:
+
+        srv = model.streaming(window=8.0, overlap=4.0, batch_size=64)
+        a = srv.open()
+        srv.push(a, chunk)              # host samples, any length
+        for u in srv.step():            # a StreamUpdate for every stream that changed
+            ...
+        res = srv.close(a, word_timestamps=True)
+
+    A closed stream's result is `transcribe_windowed(recording, word_timestamps, confidence, window, overlap, pause=pause,
+    max_segment=max_segment)` and, with keywords, `spot(recording, keywords, threshold, window, overlap)`, bit for bit."""
+
+    def __init__(self, model, window: float = 8.0, overlap: float = 4.0, batch_size: int = 64, confidence: bool = False,
+                 keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5):
+        max_frames = model.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
+        self.W = _frame_multiple(window, "window")
+        self.V = _frame_multiple(overlap, "overlap")
+        plan_windows(max(self.W, 1), window, overlap, model._encoded_length, max_frames)   # the window plan's refusals
+        if batch_size < 1:
+            raise ValueError("batch_size must be >= 1")
+        self.names: List[str] = []
+        self.kw_ids: List[List[int]] = []
+        if keywords is not None:
+            if model._ncfg["head"].get("type") == "rnnt":
+                raise NotImplementedError("keywords in streams need a CTC head: an RNN-T model has no per-frame posteriors "
+                                          "without its [T, U + 1] lattice; use a *_ctc model")
+            self.names, self.kw_ids = model._keyword_ids(keywords, threshold)
+        self.model, self.window, self.overlap = model, window, overlap
+        self.batch_size, self.confidence, self.threshold = int(batch_size), bool(confidence), threshold
+        self._openers = set(torch.nonzero(token_flag_table(model.decoding.tokenizer) & 3).reshape(-1).tolist())
+        self._streams: Dict[int, _Stream] = {}
+        self._next_id = 0
+        self._free: List[int] = []
+        self._eng = None
+        self._dec_pool: Optional[Tensor] = None    # uint8 [slots, decode record]
+        self._spot_pool: Optional[Tensor] = None   # uint8 [slots, K, spot record]
+
+    # ---- streams
+    def open(self) -> int:
+        """A new stream; returns its id."""
+        if not self._free:
+            self._grow()
+        slot = self._free.pop()
+        self._dec_pool[slot] = self._fresh_dec[0]
+        if self.kw_ids:
+            self._spot_pool[slot] = self._fresh_spot[0]
+        sid = self._next_id
+        self._next_id += 1
+        self._streams[sid] = _Stream(sid, slot, TextFeed(self.model.decoding.tokenizer, self._openers), len(self.kw_ids),
+                                     self.model._dtype)
+        return sid
+
+    def _grow(self) -> None:
+        if self._eng is None:
+            eng = self._eng = self.model._get_engine()
+            self._fresh_dec = eng.decode_state(1)
+            if self.kw_ids:
+                self._kw, self._kw_len = self.model._keyword_tensors(self.kw_ids, eng.device)
+                self._fresh_spot = eng.spot_state(1, len(self.kw_ids), self._kw.shape[1])
+                self._min_u = min(len(r) for r in self.kw_ids)
+        old = 0 if self._dec_pool is None else self._dec_pool.shape[0]
+        new = max(8, 2 * old)
+        dec = self._fresh_dec.expand(new - old, -1)
+        self._dec_pool = dec.clone() if self._dec_pool is None else torch.cat([self._dec_pool, dec])
+        if self.kw_ids:
+            spot = self._fresh_spot.expand(new - old, -1, -1)
+            self._spot_pool = spot.clone() if self._spot_pool is None else torch.cat([self._spot_pool, spot])
+        self._free.extend(range(new - 1, old - 1, -1))
+
+    def _get(self, stream: int, what: str) -> _Stream:
+        s = self._streams.get(stream)
+        if s is None:
+            raise ValueError(f"{what}: stream {stream!r} is not open")
+        return s
+
+    def push(self, stream: int, chunk) -> None:
+        """Append mono 16 kHz samples (any length) to a stream, rounded to the model's dtype as `prepare_wav` does.  Host
+        only: nothing runs on the device until `step` or `close`."""
+        s = self._get(stream, "push")
+        x = torch.as_tensor(chunk, dtype=torch.float32).detach().reshape(-1).cpu().to(self.model._dtype)
+        if x.numel():
+            s.chunks.append(x)
+            s.n += x.numel()
+
+    # ---- steps
+    @torch.inference_mode()
+    def step(self) -> List[StreamUpdate]:
+        """Encode and decode every ready window of every open stream; returns a StreamUpdate for every stream that has new
+        windows, in the order the streams were opened."""
+        news = {s: [ready_window(w, self.W, self.V) for w in range(len(s.windows), ready_count(s.n, self.W, self.V))]
+                for s in self._streams.values()}
+        jobs = [(s, ws[r]) for r in range(max((len(ws) for ws in news.values()), default=0)) for s, ws in news.items() if r < len(ws)]
+        if not jobs:
+            return []
+        before = {s: (len(s.ids), [len(d) for d in s.dets]) for s in news if news[s]}
+        self._run(jobs, tentative=True)
+        out = []
+        for s, (n0, d0) in before.items():
+            s.trim(len(s.windows) * (self.W - self.V))
+            new_ids = s.ids[n0:]
+            dets = [self._detection(k, *d) for k in range(len(self.kw_ids)) for d in s.dets[k][d0[k]:]]
+            pending = [self._detection(k, *p) for k, p in enumerate(s.pending) if p is not None]
+            dets.sort(key=lambda d: (d.start, d.keyword_index))
+            out.append(StreamUpdate(stream=s.id, new_tokens=new_ids, new_text=s.feed.push(s.ids, len(new_ids)),
+                                    tentative_text=self.model.decoding.tokenizer.decode(s.tentative),
+                                    committed_until=s.committed * FRAME_SECONDS, detections=dets, pending=pending))
+        return out
+
+    def _detection(self, k: int, start: int, end: int, score: float) -> Detection:
+        return Detection(keyword=self.names[k], keyword_index=k, start=start * FRAME_SECONDS, end=end * FRAME_SECONDS, score=score,
+                         confidence=math.exp(score / len(self.kw_ids[k])))
+
+    def _run(self, jobs: List[Tuple[_Stream, Window]], tentative: bool) -> None:
+        """Encode, decode (and spot in) the jobs' windows, each stream's in order, then bring the results to the host."""
+        last = {s: i for i, (s, _) in enumerate(jobs)}
+        for s, w in jobs:
+            s.windows.append(w)
+        reads = []
+        for group in window_groups(list(enumerate(jobs)), self.batch_size, lambda item: item[1][1]):
+            encoded = encode_rows(self.model, [s.samples(w.start, w.end) for _, (s, w) in group])
+            enc = _as_btd(encoded)
+            lp = self.model.head(encoded) if self.kw_ids else None
+            rounds: List[List[int]] = []
+            seen: Dict[_Stream, int] = {}
+            for row, (_, (s, _)) in enumerate(group):
+                r = seen[s] = seen.get(s, -1) + 1
+                if r == len(rounds):
+                    rounds.append([])
+                rounds[r].append(row)
+            for rows in rounds:
+                lp_rows = None if lp is None else self._rows(lp, rows)
+                reads.append(self._decode_round([group[r][1] for r in rows], self._rows(enc, rows), lp_rows))
+            if tentative:
+                rows = [row for row, (i, (s, _)) in enumerate(group) if last[s] == i]
+                reads.append(self._tentative([group[r][1] for r in rows], self._rows(enc, rows)))
+            del encoded, enc, lp
+        for read in reads:           # one synchronisation per call, in job order
+            read()
+
+    def _rows(self, x: Tensor, rows: List[int]) -> Tensor:
+        return x if rows == list(range(x.shape[0])) else x.index_select(0, torch.tensor(rows, device=x.device))
+
+    def _decode_round(self, sel: List[Tuple[_Stream, Window]], enc: Tensor, lp: Optional[Tensor]):
+        """One greedy_resume launch over the kept frames of one window of each stream in `sel` (and one spot launch); returns
+        the host read-back."""
+        eng, dev = self._eng, self._eng.device
+        T_w = enc.shape[1]
+        first = [w.start // FRAME_SAMPLES for _, w in sel]
+        lo = [w.keep_start - f for (_, w), f in zip(sel, first)]
+        hi = [w.keep_end - f for (_, w), f in zip(sel, first)]
+        rng = torch.tensor([lo, hi, [0] * len(sel), first, [0] * len(sel)], dtype=torch.int32).to(dev)
+        slots = torch.tensor([s.slot for s, _ in sel], device=dev)
+        state = self._dec_pool.index_select(0, slots)
+        out = eng.decode_buffers(len(sel), eng.hyp_width(T_w), T_w, scores=self.confidence)
+        eng.greedy_resume(enc, rng[0], rng[1], rng[2], state, out, self.confidence)
+        self._dec_pool.index_copy_(0, slots, state)
+        spot = None
+        if lp is not None:
+            spot = self._spot_round(slots, lp, rng[0], rng[1], rng[3], rng[4], max(h - l for l, h in zip(lo, hi)))
+
+        def read():
+            host = [None if t is None else t.cpu() for t in out]
+            ids, frames, counts = host[:3]
+            for k, ((s, w), f) in enumerate(zip(sel, first)):
+                n = int(counts[k])
+                s.ids.extend(ids[k, :n].tolist())
+                s.frames.extend((frames[k, :n] + f).tolist())
+                if self.confidence:
+                    s.token_logp.extend(host[3][k, :n].tolist())
+                    s.frame_logp.append(host[6][k, lo[k]:hi[k]].numpy())
+                    s.frame_rows.append(host[7][k, lo[k]:hi[k]].numpy())
+                s.committed = w.keep_end
+            if spot is not None:
+                self._read_spot([s for s, _ in sel], spot)
+        return read
+
+    def _spot_round(self, slots: Tensor, lp: Tensor, lo: Tensor, hi: Tensor, base: Tensor, finish: Tensor, frames: int):
+        """One ctc_spot_resume launch for the streams at `slots`; returns its device outputs."""
+        eng = self._eng
+        n, K = slots.numel(), len(self.kw_ids)
+        max_det = frames // self._min_u + 2   # a carried pending one, plus disjoint detections of >= U frames each
+        i32 = dict(dtype=torch.int32, device=eng.device)
+        det = (torch.empty((n, K, max_det), **i32), torch.empty((n, K, max_det), **i32),
+               torch.empty((n, K, max_det), dtype=torch.float32, device=eng.device), torch.zeros((n, K), **i32))
+        pend = (torch.empty((n, K), **i32), torch.empty((n, K), **i32), torch.empty((n, K), dtype=torch.float32, device=eng.device))
+        state = self._spot_pool.index_select(0, slots)
+        eng.ctc_spot_resume(lp, lo, hi, base, finish, self._kw, self._kw_len, self.threshold, state, det, pend)
+        self._spot_pool.index_copy_(0, slots, state)
+        return det + pend
+
+    @staticmethod
+    def _read_spot(streams: List[_Stream], spot: Tuple[Tensor, ...]) -> None:
+        start, end, score, count, p_start, p_end, p_score = (t.cpu() for t in spot)
+        counts, pending = count.tolist(), zip(p_start.tolist(), p_end.tolist(), p_score.tolist())
+        for b, (s, (ps, pe, psc)) in enumerate(zip(streams, pending)):
+            for k, c in enumerate(counts[b]):
+                if c:
+                    s.dets[k].extend(zip(start[b, k, :c].tolist(), end[b, k, :c].tolist(), score[b, k, :c].tolist()))
+            s.pending = [None if a < 0 else (a, e, x) for a, e, x in zip(ps, pe, psc)]
+
+    def _tentative(self, sel: List[Tuple[_Stream, Window]], enc: Tensor):
+        """Decode the frames after the kept ones, [keep_end, T_w), of each stream's newest window from a copy of its committed
+        decoder record; the output is only reported."""
+        eng, dev = self._eng, self._eng.device
+        T_w = enc.shape[1]
+        lo = [w.keep_end - w.start // FRAME_SAMPLES for _, w in sel]
+        rng = torch.tensor([lo, [T_w] * len(sel), [0] * len(sel)], dtype=torch.int32).to(dev)
+        state = self._dec_pool.index_select(0, torch.tensor([s.slot for s, _ in sel], device=dev))
+        out = eng.decode_buffers(len(sel), eng.hyp_width(T_w))
+        eng.greedy_resume(enc, rng[0], rng[1], rng[2], state, out)
+
+        def read():
+            ids, counts = out.ids.cpu(), out.counts.cpu()
+            for k, (s, _) in enumerate(sel):
+                s.tentative = ids[k, :int(counts[k])].tolist()
+        return read
+
+    # ---- the end of a stream
+    @torch.inference_mode()
+    def close(self, stream: int, word_timestamps: bool = False, pause: float = 1.0, max_segment: float = 25.0) -> StreamResult:
+        """End a stream: encode its remaining windows, the last one included, and return its StreamResult.  Raises ValueError
+        for a stream that is not open, pause < 0, max_segment <= 0 and, after freeing the stream, for one whose samples
+        encode to no frame (as `transcribe_windowed` does)."""
+        s = self._get(stream, "close")
+        if not pause >= 0:
+            raise ValueError(f"pause={pause} s must be >= 0")
+        if not max_segment > 0:
+            raise ValueError(f"max_segment={max_segment} s must be positive")
+        del self._streams[stream]
+        self._free.append(s.slot)
+        max_frames = self.model.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
+        windows, T = plan_windows(s.n, self.window, self.overlap, self.model._encoded_length, max_frames)
+        N, done = s.n, len(s.windows)
+        assert windows[:done] == s.windows, "a ready window differs from the plan of the whole stream"
+        self._run([(s, w) for w in windows[done:]], tentative=False)
+        eng, tok = self._eng, self.model.decoding.tokenizer
+        detections = None
+        if self.kw_ids:
+            dev = eng.device
+            one = torch.tensor([s.slot], device=dev)
+            flags = torch.tensor([[0], [0], [0], [1]], dtype=torch.int32, device=dev)   # lo = hi = 0, finish
+            lp = torch.zeros((1, 1, eng.num_classes), dtype=torch.float32, device=dev)
+            self._read_spot([s], self._spot_round(one, lp, flags[0], flags[1], flags[2], flags[3], 0))
+            detections = self._stream_detections(s, compute_frame_shift(N, T))
+        n = len(s.ids)
+        ids_d = torch.tensor(s.ids or [0], dtype=torch.int32).reshape(1, -1).to(eng.device)
+        frames_d = torch.tensor(s.frames or [0], dtype=torch.int32).reshape(1, -1).to(eng.device)
+        counts_d = torch.tensor([n], dtype=torch.int32, device=eng.device)
+        ws, we, wf, wn, k = (t[0].cpu().tolist() for t in eng.group_words(ids_d, frames_d, counts_d, self.model._word_flags()))
+        shift = compute_frame_shift(N, T)
+        words = words_from_device(tok, s.ids, ws[:k], we[:k], wf[:k], wn[:k], shift, s.token_logp if self.confidence else None)
+        cuts = segment_cuts(list(zip(ws[:k], we[:k])), T, shift, pause, max_segment)
+        frame_logp = np.concatenate(s.frame_logp) if self.confidence else None
+        frame_rows = np.concatenate(s.frame_rows) if self.confidence else None
+        segs = windowed_segments(tok, s.ids, s.frames, cuts, shift, N / SAMPLE_RATE, words if word_timestamps else None, ws[:k],
+                                 frame_logp, frame_rows)
+        return StreamResult(transcript=LongformTranscriptionResult(segments=segs), detections=detections)
+
+    def _stream_detections(self, s: _Stream, shift: float) -> List[Detection]:
+        """A closed stream's detections through `spot`'s record builder."""
+        K, width = len(s.dets), max(1, max(len(d) for d in s.dets))
+        start = torch.full((K, width), -1, dtype=torch.int32)
+        end, score = start.clone(), torch.full((K, width), float("-inf"))
+        for k, d in enumerate(s.dets):
+            if d:
+                start[k, :len(d)] = torch.tensor([x[0] for x in d], dtype=torch.int32)
+                end[k, :len(d)] = torch.tensor([x[1] for x in d], dtype=torch.int32)
+                score[k, :len(d)] = torch.tensor([x[2] for x in d], dtype=torch.float32)
+        count = torch.tensor([len(d) for d in s.dets], dtype=torch.int32)
+        return self.model._detections(self.names, self.kw_ids, start, end, score, count, shift)
+
+    @property
+    def streams(self) -> List[int]:
+        """The ids of the open streams."""
+        return list(self._streams)

@@ -167,3 +167,31 @@ class LongformTranscriptionResult(_Record):
 
     def __iter__(self) -> Iterator[Segment]:
         return iter(self.segments)
+
+
+class StreamUpdate(_Record):
+    """What one `StreamServer.step()` changed in a live stream.  `new_tokens` are the token ids committed by the step and
+    `new_text` their text: concatenating a stream's `new_text` in order gives the tokenizer's decoding of every committed
+    token.  `tentative_text` decodes the frames after the committed ones in the newest encoded window; it is replaced at the
+    next step.  `committed_until` is the end of the committed frames in seconds at the nominal 0.04 s per frame.
+    `detections` are the keyword detections made final by the step, `pending` the provisional ones (at most one per keyword),
+    which a better overlapping candidate may still replace; their times use the nominal frame step too."""
+    __slots__ = _fields = ("stream", "new_tokens", "new_text", "tentative_text", "committed_until", "detections", "pending")
+    stream: int
+    new_tokens: List[int]
+    new_text: str
+    tentative_text: str
+    committed_until: float
+    detections: List[Detection]
+    pending: List[Detection]
+
+
+class StreamResult(_Record):
+    """`StreamServer.close()` result: the stream's `transcript`, the `LongformTranscriptionResult` that `transcribe_windowed`
+    gives for the same recording and settings, and its keyword `detections` as `spot` gives them (None without keywords)."""
+    __slots__ = _fields = ("transcript", "detections")
+    transcript: LongformTranscriptionResult
+    detections: Optional[List[Detection]]
+
+    def __str__(self) -> str:
+        return str(self.transcript)

@@ -388,6 +388,36 @@ int gam_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const int32_t
 int gam_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
                  const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det, int32_t* det_start,
                  int32_t* det_end, float* det_score, int32_t* det_count, void* stream);
+/* Resumable keyword spotting: gam_ctc_spot over a stream's frames in consecutive calls (live audio), with each (stream,
+ * keyword) pair's search carried in device memory between them.  gam_ctc_spot itself is one such call from fresh records.
+ *
+ * A record is gam_ctc_spot_state_bytes(h, Umax) bytes: the pending detection (whether there is one, its start, end and
+ * score), the true count of detections emitted so far, and every state's score v and start frame.
+ * gam_ctc_spot_state_init writes n x K fresh records ([n, K, record], stream-major) at `state`.
+ *
+ * One call: row b walks local frames [lo[b], hi[b]) (clamped to [0, T]) of log_probs[b] ([B, T, V+1]) as stream frames
+ * frame_base[b] + t, keyword k continuing from state + (b K + k) record_bytes and leaving the updated record there.  lo, hi,
+ * frame_base and finish are device i32 [B].  Start and end frames, in records and outputs, are stream frames.
+ *   det_*         as gam_ctc_spot's; detections emitted by the call are appended at det_count[b, k] (read and written), which
+ *                 stops at max_det; the record keeps the true count.  Nothing else in det_* is written.
+ *   pend_*        device i32 / i32 / f32 [B, K], or all three NULL: the pending detection after the call (start, end, score),
+ *                 or -1 / -1 / -inf when there is none.  A pending detection may still be replaced by a better overlapping one.
+ *   finish[b]     nonzero: the stream ends with this call, and its pending detection is emitted.  Without finish, the pending
+ *                 detection is emitted early when no state with a finite score has a start frame before its end: no later
+ *                 candidate can overlap it, so the detections and their order are exactly gam_ctc_spot's over the whole stream.
+ * Splitting a stream's frames [0, L) into consecutive ranges, the last call with finish, gives gam_ctc_spot's detections over
+ * the L frames bit for bit.  A keyword with a bad id or length gets no detections and a pending -1 / -1 / NaN.
+ * Refused (gam_last_error): what gam_ctc_spot refuses, plus a NULL lo, hi, frame_base, finish or state, a record_bytes other
+ * than gam_ctc_spot_state_bytes(h, Umax), and pend_* that are not all given or all NULL.  gam_ctc_spot_state_bytes returns -1
+ * for a handle without a CTC head or a Umax outside [1, 64].  No workspace, no host synchronisation, capturable in a CUDA
+ * graph. */
+int64_t gam_ctc_spot_state_bytes(const gam_handle* h, int32_t Umax);
+int gam_ctc_spot_state_init(gam_handle* h, void* state, int32_t n, int32_t K, int32_t Umax, void* stream);
+int gam_ctc_spot_resume(gam_handle* h, const float* log_probs, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
+                        const int32_t* frame_base, const int32_t* finish, const int32_t* keywords, const int32_t* keyword_len, int32_t K,
+                        int32_t Umax, float threshold, int32_t max_det, void* state, int64_t record_bytes, int32_t* det_start,
+                        int32_t* det_end, float* det_score, int32_t* det_count, int32_t* pend_start, int32_t* pend_end,
+                        float* pend_score, void* stream);
 /* ---- CTC hotwords: the keywords gam_ctc_spot found replace the greedy words they outscore.  No hypothesis search: the greedy
  * output changes only where a stored detection beats it by the margin the threshold states.
  *
