@@ -67,7 +67,8 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_decode_state_bytes", "gam_decode_state_init", "gam_decode_resume_workspace_bytes", "gam_ctc_greedy_resume",
            "gam_rnnt_greedy_resume", "gam_ctc_spot", "gam_test_ctc_spot", "gam_ctc_bias_workspace_bytes", "gam_ctc_bias",
            "gam_ctc_align_long_gaps_workspace_bytes", "gam_ctc_align_long_gaps", "gam_test_ctc_align_long_gaps",
-           "gam_ctc_spot_state_bytes", "gam_ctc_spot_state_init", "gam_ctc_spot_resume")
+           "gam_ctc_spot_state_bytes", "gam_ctc_spot_state_init", "gam_ctc_spot_resume",
+           "gam_ctc_align_long_skips_workspace_bytes", "gam_ctc_align_long_skips", "gam_test_ctc_align_long_skips")
 
 
 def lib_path() -> Path:
@@ -154,7 +155,8 @@ def load() -> C.CDLL:
     for fn in (lib.gam_rnnt_predict_train, lib.gam_ctc_log_probs_backward, lib.gam_rnnt_joint_backward, lib.gam_rnnt_predict_backward):
         fn.restype = C.c_int
     for fn in (lib.gam_ctc_align_workspace_bytes, lib.gam_rnnt_align_scores_workspace_bytes, lib.gam_rnnt_align_workspace_bytes,
-               lib.gam_ctc_align_long_workspace_bytes, lib.gam_ctc_align_long_gaps_workspace_bytes):
+               lib.gam_ctc_align_long_workspace_bytes, lib.gam_ctc_align_long_gaps_workspace_bytes,
+               lib.gam_ctc_align_long_skips_workspace_bytes):
         fn.argtypes = [H, i32, i32, i32]
         fn.restype = i64
     lib.gam_ctc_align.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, c_vp, i64] + [c_vp] * 6
@@ -164,8 +166,12 @@ def load() -> C.CDLL:
     lib.gam_test_ctc_align_long.argtypes = [H, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, c_vp, i64] + [c_vp] * 5 + [i32, c_vp, c_vp]
     lib.gam_ctc_align_long_gaps.argtypes = [H, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, C.c_float, c_vp, i64] + [c_vp] * 9
     lib.gam_test_ctc_align_long_gaps.argtypes = lib.gam_ctc_align_long_gaps.argtypes[:-1] + [i32, c_vp, c_vp]
+    lib.gam_ctc_align_long_skips.argtypes = ([H, c_vp, c_vp, c_vp, c_vp, c_vp, i32, i32, i32, C.c_float, C.c_float, c_vp, i64]
+                                             + [c_vp] * 11)
+    lib.gam_test_ctc_align_long_skips.argtypes = lib.gam_ctc_align_long_skips.argtypes[:-1] + [i32, c_vp, c_vp]
     for fn in (lib.gam_ctc_align, lib.gam_rnnt_align_scores, lib.gam_rnnt_align, lib.gam_ctc_align_long, lib.gam_test_ctc_align_long,
-               lib.gam_ctc_align_long_gaps, lib.gam_test_ctc_align_long_gaps):
+               lib.gam_ctc_align_long_gaps, lib.gam_test_ctc_align_long_gaps, lib.gam_ctc_align_long_skips,
+               lib.gam_test_ctc_align_long_skips):
         fn.restype = C.c_int
     lib.gam_ctc_spot.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32, C.c_float, i32] + [c_vp] * 5
     lib.gam_test_ctc_spot.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32, C.c_float, i32] + [c_vp] * 4 + [i32, c_vp]

@@ -12,7 +12,9 @@
 //       shared memory.  Each frame reads the two states left of its range from CTA k - 1 over distributed shared memory,
 //       then one cluster barrier closes the frame.  The per-state arithmetic is (1)'s, so the results are its bits.
 //       Gap mode (the GAPS instantiation, after row_max_kernel's pre-pass) lets the blank states at line edges also emit
-//       m[t] + log theta; the instantiation without gaps is the kernel of gam_ctc_align_long.
+//       m[t] + log theta; the instantiation without gaps is the kernel of gam_ctc_align_long.  Skip mode (SKIPS, on top
+//       of gap mode) adds one edge per line, from the exit blank of the line before it to its own exit blank, whose source
+//       may sit in any CTA of the cluster.
 // All backtrack with one thread (a serial walk of T or T + U steps) and then gather token_logp with the whole CTA.
 #include <algorithm>
 #include <cmath>
@@ -25,14 +27,26 @@
 namespace gam {
 namespace {
 
-constexpr int kSkip = 1 << 30;   // ctc lab_s: the state may also be entered from s - 2
+constexpr int kSkip = 1 << 30;   // ctc lab_s: the state may also be entered from s - 2 (skip mode, blank s: from e_i)
 constexpr int kBound = 1 << 29;  // ctc_align_long lab_s, gap mode: a boundary state
+// skip mode: an exit blank's lab_s holds its source as (CTA << kSrcIndexBits) | index, below the flag bits
+constexpr int kSrcIndexBits = 16, kSrcCtaBits = 4;
+static_assert(kAlignLongMaxCtas <= (1 << kSrcCtaBits), "a source CTA rank must fit in its lab_s field");
+static_assert(kSrcIndexBits + kSrcCtaBits <= 29, "the source fields must stay below kBound and kSkip");
 
 // gap mode: whether the blank state s (even) of a recording with U_b tokens is a boundary state: the first or last state, or
 // the blank before a token that starts a line or after one that ends a line
 __device__ __forceinline__ bool boundary_state(const uint8_t* edges, int Ub, int s) {
   const int j = s >> 1;   // the blank between tokens j - 1 and j
   return s == 0 || j == Ub || (edges[j] & 1) || (edges[j - 1] & 2);
+}
+
+// skip mode: the source e_i of the skip edge into the exit blank x_i = s (s >= 2, token s / 2 - 1 ends a line): the exit
+// blank of the line end before it, or state 0.  A backward walk over line_edges, as long as the line.
+__device__ __forceinline__ int skip_source(const uint8_t* edges, int s) {
+  int j = (s >> 1) - 2;
+  while (j >= 0 && !(edges[j] & 2)) --j;
+  return 2 * (j + 1);
 }
 
 __device__ __forceinline__ float lse3(float a, float b, float c) {
@@ -276,13 +290,21 @@ __global__ void rnnt_align_kernel(const float* __restrict__ blank, const float* 
 // writes all outputs.
 // GAPS: a boundary state (kBound) emits max(lp[t, blank], m[t] + log theta) in both recursions, every frame t < T_b also reads
 // m[t] (a NaN there poisons the recording), and CTA 0's backtrack flags the unmatched frames; g is not read otherwise.
-template <bool GAPS>
+// SKIPS (with GAPS): the exit blank x_i of every line also takes the skip edge from (t - 1, e_i), compared after stay and
+// s - 1, with backpointer code 3 (unused on blank states otherwise).  A blank's label is always blank, so its lab_s entry
+// holds kSkip and the source instead: bits 16..19 its CTA j <= k, bits 0..15 its index there.  The source is read from frame
+// t - 1's buffer, over distributed shared memory when j < k.  That is safe for the reason the left neighbour's read is: CTA
+// j rewrites that buffer only in frame t + 1, after the barrier that CTA k reaches once its own frame t is done.  CTA 0's
+// backtrack finds e_i again from line_edges (the other CTAs may have exited), leaves the jumped tokens at frame -1 and
+// sums the penalties of the skip edges taken in frame order.
+template <bool GAPS, bool SKIPS>
 __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const int* __restrict__ enc_len,
                                       const int* __restrict__ targets, const int* __restrict__ target_len, int T, int U, int V1, int P,
                                       uint32_t* __restrict__ bp, int* __restrict__ frames, float* __restrict__ token_logp,
                                       float* __restrict__ viterbi_logp, float* __restrict__ log_likelihood, int* __restrict__ path_rows,
                                       AlignGaps g) {
-  constexpr int kLab = GAPS ? ~(kSkip | kBound) : ~kSkip;   // the label of a lab_s entry
+  static_assert(GAPS || !SKIPS, "skip mode runs on top of gap mode");
+  constexpr int kLab = GAPS ? ~(kSkip | kBound) : ~kSkip;   // the label of a lab_s entry (odd states, in skip mode)
   extern __shared__ float4 smem_f4[];
   uint32_t C;
   asm("mov.u32 %0, %%cluster_nctarank;" : "=r"(C));
@@ -312,6 +334,10 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
       if (l >= 0 && l < blank && s >= 3 && l != y[(s >> 1) - 1]) l |= kSkip;
     } else if (GAPS && boundary_state(edges, Ub, s)) {
       l |= kBound;
+      if (SKIPS && s >= 2 && (edges[(s >> 1) - 1] & 2)) {   // x_i: keeps the source instead of the label
+        const int e = skip_source(edges, s);
+        l = kSkip | kBound | ((e / P) << kSrcIndexBits) | (e % P);
+      }
     }
     lab_s[i] = l;
   }
@@ -330,7 +356,7 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
     }
     for (int i = tid; i < n; i += nt) {
       const int s = s0 + i;
-      float x = lp[lab_s[i] & kLab];   // frame 0 reads every state's entry: the NaN rule counts them
+      float x = lp[SKIPS && !(s & 1) ? blank : lab_s[i] & kLab];   // frame 0 reads every state's entry: the NaN rule counts them
       nan |= isnan(x);
       if (GAPS && (lab_s[i] & kBound)) x = fmaxf(x, gt);
       vbuf[i] = fbuf[i] = s < 2 ? x : -INFINITY;
@@ -368,7 +394,7 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
             }
             if (c > best) { best = c; code = 1; }
           }
-          if (l & kSkip) {
+          if ((l & kSkip) && (!SKIPS || (s & 1))) {
             float c;
             if (i >= 2) {
               c = va[i - 2];
@@ -378,8 +404,23 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
               fm2 = ptx::ld_cluster_f32(lf + 4u * (P - 2 + i));
             }
             if (c > best) { best = c; code = 2; }
+          } else if (SKIPS && (l & kSkip)) {   // x_i: the skip edge from e_i, penalty fp32(n_i) * log psi
+            const int j = (l >> kSrcIndexBits) & ((1 << kSrcCtaBits) - 1), e = l & ((1 << kSrcIndexBits) - 1);
+            float c, fe;
+            if (j == k) {
+              c = va[e];
+              fe = fa[e];
+            } else {
+              const uint32_t off = 4u * static_cast<uint32_t>(p * P + e);
+              c = ptx::ld_cluster_f32(ptx::mapa_u32(ptx::smem_u32(vbuf), j) + off);
+              fe = ptx::ld_cluster_f32(ptx::mapa_u32(ptx::smem_u32(fbuf), j) + off);
+            }
+            const float pen = __fmul_rn(static_cast<float>((s - (j * P + e)) >> 1), g.log_psi);   // rounded: no FMA
+            c = c + pen;
+            fm2 = fe + pen;
+            if (c > best) { best = c; code = 3; }
           }
-          float x = row[l & kLab];
+          float x = row[SKIPS && !(s & 1) ? blank : l & kLab];
           nan |= isnan(x);
           if (GAPS && (l & kBound)) x = fmaxf(x, gt);
           vb[i] = x + best;
@@ -431,7 +472,7 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
     for (int t = tid; t < T; t += nt) um[t] = 0;
   __syncthreads();
   if (fs >= 0 && tid == 0) {   // serial backtrack, as ctc_align_kernel's
-    int s = fs, rows = 0;
+    int s = fs, rows = 0, skips = 0;
     for (int t = Tb - 1; t >= 0; --t) {
       if (s & 1) {
         fr[s >> 1] = t;
@@ -439,7 +480,15 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
         um[t] = 1;   // the sweep's boundary emission took m[t] + log theta here
         ++rows;
       }
-      if (t > 0) s -= (bpu[static_cast<int64_t>(t) * W + s / 16] >> (2 * (s & 15))) & 3u;
+      if (t > 0) {
+        const uint32_t code = (bpu[static_cast<int64_t>(t) * W + s / 16] >> (2 * (s & 15))) & 3u;
+        if (SKIPS && code == 3) {   // the tokens of (e_i, x_i) keep frame -1
+          s = skip_source(edges, s);
+          ++skips;
+        } else {
+          s -= code;
+        }
+      }
     }
     if constexpr (GAPS) {
       float sum = 0.f;
@@ -448,17 +497,32 @@ __global__ void ctc_align_long_kernel(const float* __restrict__ log_probs, const
       g.unmatched_rows[b] = rows;
       g.unmatched_logp[b] = sum;
     }
+    if constexpr (SKIPS) {   // skip edge i is on the path iff line i's last token was jumped; frame order is line order
+      float sum = 0.f;
+      for (int j = 0, e = 0; skips > 0 && j < Ub; ++j) {
+        if (edges[j] & 2) {
+          if (fr[j] < 0) sum += __fmul_rn(static_cast<float>(j + 1 - e / 2), g.log_psi);
+          e = 2 * (j + 1);
+        }
+      }
+      g.skipped_rows[b] = skips;
+      g.skip_logp[b] = sum;
+    }
   }
   if (GAPS && tid == 0 && fs < 0) {   // no path, or poisoned
     g.unmatched_rows[b] = 0;
     g.unmatched_logp[b] = poison ? qnan() : 0.f;
+    if constexpr (SKIPS) {
+      g.skipped_rows[b] = 0;
+      g.skip_logp[b] = poison ? qnan() : 0.f;
+    }
   }
   __syncthreads();
   for (int i = tid; i < U; i += nt) {
     float v = -INFINITY;
     if (i < Ub) {
       if (poison) v = qnan();
-      else if (fs >= 0) v = lp[static_cast<int64_t>(fr[i]) * V1 + y[i]];
+      else if (fs >= 0 && (!SKIPS || fr[i] >= 0)) v = lp[static_cast<int64_t>(fr[i]) * V1 + y[i]];
     }
     tl[i] = v;
   }
@@ -479,16 +543,16 @@ __global__ void row_max_kernel(const float* __restrict__ log_probs, const int* _
 }
 
 // cluster and shared-memory attributes of one instantiation, once per device
-template <bool GAPS>
+template <bool GAPS, bool SKIPS>
 int align_long_attributes() {
   static PerDeviceOnce attr_once;
   if (!attr_once.first()) return 0;
   int dev = 0, cap = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  if (cudaFuncSetAttribute(ctc_align_long_kernel<GAPS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-      cudaFuncSetAttribute(ctc_align_long_kernel<GAPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap - kAlignLongStaticSmem) !=
-          cudaSuccess)
+  if (cudaFuncSetAttribute(ctc_align_long_kernel<GAPS, SKIPS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
+      cudaFuncSetAttribute(ctc_align_long_kernel<GAPS, SKIPS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           cap - kAlignLongStaticSmem) != cudaSuccess)
     return -1;
   return 0;
 }
@@ -542,7 +606,12 @@ int launch_ctc_align_long(const float* log_probs, const int* enc_len, const int*
   int C = 0, P = 0;
   const int rc = ctc_align_long_plan(U, forced_ctas, &C, &P);
   if (rc != 0) return rc;
-  if ((gaps ? align_long_attributes<true>() : align_long_attributes<false>()) != 0) return -1;
+  const bool skips = gaps && gaps->skipped_rows;
+  if (skips && P > (1 << kSrcIndexBits)) return 1;   // a source index would not fit in its lab_s field
+  if ((skips  ? align_long_attributes<true, true>()
+       : gaps ? align_long_attributes<true, false>()
+              : align_long_attributes<false, false>()) != 0)
+    return -1;
   if (plan) {
     plan[0] = C;
     plan[1] = P;
@@ -560,13 +629,13 @@ int launch_ctc_align_long(const float* log_probs, const int* enc_len, const int*
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   if (!gaps)
-    return cudaLaunchKernelEx(&cfg, ctc_align_long_kernel<false>, log_probs, enc_len, targets, target_len, T, U, V1, P, bp, frames,
+    return cudaLaunchKernelEx(&cfg, ctc_align_long_kernel<false, false>, log_probs, enc_len, targets, target_len, T, U, V1, P, bp, frames,
                               token_logp, viterbi_logp, log_likelihood, path_rows, AlignGaps{}) != cudaSuccess
                ? -2
                : 0;
   const dim3 grid(static_cast<unsigned>(std::min<int64_t>((static_cast<int64_t>(T) + 7) / 8, 65535)), std::min(B, 65535));
   row_max_kernel<<<grid, 256, 0, s>>>(log_probs, enc_len, B, T, V1, gaps->m);
-  if (cudaLaunchKernelEx(&cfg, ctc_align_long_kernel<true>, log_probs, enc_len, targets, target_len, T, U, V1, P, bp, frames, token_logp,
+  if (cudaLaunchKernelEx(&cfg, skips ? ctc_align_long_kernel<true, true> : ctc_align_long_kernel<true, false>, log_probs, enc_len, targets, target_len, T, U, V1, P, bp, frames, token_logp,
                          viterbi_logp, log_likelihood, path_rows, *gaps) != cudaSuccess)
     return -2;
   return 0;

@@ -939,6 +939,11 @@ static int ctc_align_long_run(gam_handle* h, const char* what, const float* log_
       return fail(h, -1, "%s: a required pointer is NULL", what);
     if (std::isnan(gaps->log_theta) || gaps->log_theta > 0.f)
       return fail(h, -1, "%s: log_theta=%g must be <= 0 (a threshold in (0, 1]) or -inf", what, gaps->log_theta);
+    if (gaps->skipped_rows) {
+      if (!gaps->skip_logp) return fail(h, -1, "%s: a required pointer is NULL", what);
+      if (std::isnan(gaps->log_psi) || gaps->log_psi > 0.f)
+        return fail(h, -1, "%s: log_psi=%g must be <= 0 (a threshold in (0, 1]) or -inf", what, gaps->log_psi);
+    }
   }
   const int64_t bp_bytes = gam_ctc_align_long_workspace_bytes(h, B, T, U);
   const int64_t need = gaps ? gam_ctc_align_long_gaps_workspace_bytes(h, B, T, U) : bp_bytes;
@@ -976,6 +981,21 @@ int gam_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const int32_t
                             frames, token_logp, viterbi_logp, log_likelihood, path_rows, 0, nullptr, &g, stream);
 }
 
+int64_t gam_ctc_align_long_skips_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  return gam_ctc_align_long_gaps_workspace_bytes(h, B, T, U);
+}
+
+int gam_ctc_align_long_skips(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                             const int32_t* target_len, const uint8_t* line_edges, int32_t B, int32_t T, int32_t U, float log_theta,
+                             float log_psi, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                             float* viterbi_logp, float* log_likelihood, int32_t* path_rows, uint8_t* unmatched,
+                             int32_t* unmatched_rows, float* unmatched_logp, int32_t* skipped_rows, float* skip_logp, void* stream) {
+  if (!skipped_rows) return fail(h, -1, "ctc_align_long_skips: a required pointer is NULL");
+  AlignGaps g{line_edges, log_theta, nullptr, unmatched, unmatched_rows, unmatched_logp, log_psi, skipped_rows, skip_logp};
+  return ctc_align_long_run(h, "ctc_align_long_skips", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes,
+                            frames, token_logp, viterbi_logp, log_likelihood, path_rows, 0, nullptr, &g, stream);
+}
+
 int gam_test_ctc_align_long(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
                             const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes,
                             int32_t* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int32_t* path_rows,
@@ -995,6 +1015,20 @@ int gam_test_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const in
     return fail(h, -1, "test_ctc_align_long_gaps: cluster_ctas=%d outside [0, %d]", cluster_ctas, kAlignLongMaxCtas);
   AlignGaps g{line_edges, log_theta, nullptr, unmatched, unmatched_rows, unmatched_logp};
   return ctc_align_long_run(h, "test_ctc_align_long_gaps", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes,
+                            frames, token_logp, viterbi_logp, log_likelihood, path_rows, cluster_ctas, plan, &g, stream);
+}
+
+int gam_test_ctc_align_long_skips(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                                  const int32_t* target_len, const uint8_t* line_edges, int32_t B, int32_t T, int32_t U, float log_theta,
+                                  float log_psi, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                                  float* viterbi_logp, float* log_likelihood, int32_t* path_rows, uint8_t* unmatched,
+                                  int32_t* unmatched_rows, float* unmatched_logp, int32_t* skipped_rows, float* skip_logp,
+                                  int32_t cluster_ctas, int32_t* plan, void* stream) {
+  if (cluster_ctas < 0 || cluster_ctas > kAlignLongMaxCtas)
+    return fail(h, -1, "test_ctc_align_long_skips: cluster_ctas=%d outside [0, %d]", cluster_ctas, kAlignLongMaxCtas);
+  if (!skipped_rows) return fail(h, -1, "test_ctc_align_long_skips: a required pointer is NULL");
+  AlignGaps g{line_edges, log_theta, nullptr, unmatched, unmatched_rows, unmatched_logp, log_psi, skipped_rows, skip_logp};
+  return ctc_align_long_run(h, "test_ctc_align_long_skips", log_probs, enc_len, targets, target_len, B, T, U, workspace, workspace_bytes,
                             frames, token_logp, viterbi_logp, log_likelihood, path_rows, cluster_ctas, plan, &g, stream);
 }
 

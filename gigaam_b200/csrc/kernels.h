@@ -163,6 +163,11 @@ struct AlignGaps {
   uint8_t* unmatched;          // [B, T]
   int* unmatched_rows;         // [B]
   float* unmatched_logp;       // [B]
+  // skip mode (gam_ctc_align_long_skips): every line's exit blank may also be entered from the line end before it, at
+  // fp32(n_i) * log_psi.  skipped_rows NULL: gap mode only.
+  float log_psi;
+  int* skipped_rows;           // [B]
+  float* skip_logp;            // [B]
 };
 // gaps: NULL for gam_ctc_align_long's sweep
 int launch_ctc_align_long(const float* log_probs, const int* enc_len, const int* targets, const int* target_len, int B, int T, int U,

@@ -713,22 +713,31 @@ class Engine:
         return outs
 
     def ctc_align_long(self, log_probs: Tensor, enc_len: Tensor, targets: Tensor, target_len: Tensor,
-                       cluster_ctas: Optional[int] = None, gaps: Optional[Tuple[Tensor, float]] = None) -> Tuple[Tensor, ...]:
+                       cluster_ctas: Optional[int] = None, gaps: Optional[Tuple[Tensor, float]] = None,
+                       skips: Optional[float] = None) -> Tuple[Tensor, ...]:
         """ctc_align for recordings of any length and up to 65 536 tokens (gam_ctc_align_long): the same arguments and
         outputs, and the same bits on every input ctc_align accepts.  `cluster_ctas` forces the number of CTAs per utterance
         (gam_test_ctc_align_long*); the plan used, (CTAs, states per CTA), is then kept in `last_align_long_plan`.
         `gaps` = (line_edges [B, U] u8, log_theta) runs gam_ctc_align_long_gaps instead and appends its three outputs
-        (unmatched [B, T] u8, unmatched_rows [B] i32, unmatched_logp [B] f32)."""
+        (unmatched [B, T] u8, unmatched_rows [B] i32, unmatched_logp [B] f32).  `skips` = log_psi (with `gaps`; log_theta
+        = -inf for skips without gaps) runs gam_ctc_align_long_skips and appends (skipped_rows [B] i32, skip_logp [B] f32)."""
         assert log_probs.is_cuda and log_probs.dtype == torch.float32 and log_probs.is_contiguous() and log_probs.dim() == 3
         if self.head_type != 1:
             raise RuntimeError("model has no CTC head")
+        if skips is not None and gaps is None:
+            raise ValueError("ctc_align_long: skips needs gaps=(line_edges, log_theta); pass log_theta=-inf for skips alone")
         B, T, _ = log_probs.shape
         U = targets.shape[1]
-        size_fn = self.lib.gam_ctc_align_long_workspace_bytes if gaps is None else self.lib.gam_ctc_align_long_gaps_workspace_bytes
+        if skips is not None:
+            size_fn, kind = self.lib.gam_ctc_align_long_skips_workspace_bytes, "ctc_long_skips"
+        elif gaps is not None:
+            size_fn, kind = self.lib.gam_ctc_align_long_gaps_workspace_bytes, "ctc_long_gaps"
+        else:
+            size_fn, kind = self.lib.gam_ctc_align_long_workspace_bytes, "ctc_long"
         nbytes = int(size_fn(self.handle, B, T, U))
         if nbytes < 0:
             raise ValueError(f"ctc_align_long: bad sizes B={B}, T={T}, U={U}")
-        ws = self._ws_align.get(("ctc_long" if gaps is None else "ctc_long_gaps", B, T, U), nbytes, self.device)
+        ws = self._ws_align.get((kind, B, T, U), nbytes, self.device)
         enc_len, targets, target_len = (self._i32(t, self.device) for t in (enc_len, targets, target_len))
         outs = self._align_outputs(B, U)
         head = [log_probs.data_ptr(), enc_len.data_ptr(), targets.data_ptr(), target_len.data_ptr()]
@@ -741,18 +750,21 @@ class Engine:
                            torch.empty((B,), dtype=torch.int32, device=self.device),
                            torch.empty((B,), dtype=torch.float32, device=self.device))
             head += [line_edges.data_ptr()]
-        sizes = [B, T, U] + ([] if gaps is None else [float(log_theta)])
+        if skips is not None:
+            outs = outs + (torch.empty((B,), dtype=torch.int32, device=self.device),
+                           torch.empty((B,), dtype=torch.float32, device=self.device))
+        sizes = [B, T, U] + ([] if gaps is None else [float(log_theta)]) + ([] if skips is None else [float(skips)])
         ptrs = head + sizes + [ws.data_ptr(), ws.numel(), *[t.data_ptr() for t in outs]]
+        name = {"ctc_long": "gam_ctc_align_long", "ctc_long_gaps": "gam_ctc_align_long_gaps",
+                "ctc_long_skips": "gam_ctc_align_long_skips"}[kind]
         with torch.cuda.device(self.device):
             if cluster_ctas is None:
-                fn = self.lib.gam_ctc_align_long if gaps is None else self.lib.gam_ctc_align_long_gaps
-                rc = fn(self.handle, *ptrs, self._stream())
+                rc = getattr(self.lib, name)(self.handle, *ptrs, self._stream())
             else:
-                fn = self.lib.gam_test_ctc_align_long if gaps is None else self.lib.gam_test_ctc_align_long_gaps
                 plan = (C.c_int32 * 2)()
-                rc = fn(self.handle, *ptrs, int(cluster_ctas), plan, self._stream())
+                rc = getattr(self.lib, name.replace("gam_", "gam_test_", 1))(self.handle, *ptrs, int(cluster_ctas), plan, self._stream())
                 self.last_align_long_plan = (int(plan[0]), int(plan[1]))
-        _lib.check(self.lib, self.handle, rc, "gam_ctc_align_long" if gaps is None else "gam_ctc_align_long_gaps")
+        _lib.check(self.lib, self.handle, rc, name)
         return outs
 
     def ctc_spot(self, log_probs: Tensor, enc_len: Tensor, keywords: Tensor, keyword_len: Tensor, threshold: float, max_det: int,

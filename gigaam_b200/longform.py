@@ -302,13 +302,13 @@ def windowed_segments(tokenizer, ids: Sequence[int], frames: Sequence[int], cuts
 
 def line_segments(lines: Sequence[str], ranges: Sequence[Tuple[int, int]], frames: Sequence[int], token_logp: Sequence[float],
                   frame_shift: float, viterbi_logp: float, words: Optional[Sequence[Word]] = None,
-                  word_first: Optional[Sequence[int]] = None) -> List[Segment]:
+                  word_first: Optional[Sequence[int]] = None, skipped: Sequence[int] = ()) -> List[Segment]:
     """One Segment per line of an aligned text.  ranges[i] = line i's token range [a, b) in the aligned sequence, frames /
     token_logp the alignment's per-token outputs, words (None: no word timestamps) the words of the whole sequence with
     word_first their first token.  A line spans the frames of its first and last token (its first word's start and its
-    last word's end) and has confidence exp(mean token log-prob); a line without tokens starts and ends where the line
-    before it ended (0.0 first), has no words and confidence NaN.  Without a path (a Viterbi score that is not finite)
-    every line has no words, NaN times and confidence 0.0."""
+    last word's end) and has confidence exp(mean token log-prob); a line without tokens, or one of the `skipped` lines,
+    starts and ends where the line before it ended (0.0 first), has no words and confidence NaN.  Without a path (a
+    Viterbi score that is not finite) every line has no words, NaN times and confidence 0.0."""
     if not math.isfinite(viterbi_logp):
         return [Segment(text=t, start=math.nan, end=math.nan, words=None if words is None else [], confidence=0.0) for t in lines]
     from .timestamps_utils import mean_logp_confidence
@@ -318,9 +318,10 @@ def line_segments(lines: Sequence[str], ranges: Sequence[Tuple[int, int]], frame
         by_line[bisect.bisect_right(starts, f) - 1].append(w)
     out: List[Segment] = []
     prev_end = 0.0
+    skipped = set(skipped)
     for i, (text, (a, b)) in enumerate(zip(lines, ranges)):
         seg_words = None if words is None else by_line[i]
-        if a == b:
+        if a == b or i in skipped:
             out.append(Segment(text=text, start=prev_end, end=prev_end, words=seg_words, confidence=math.nan))
             continue
         start, end = frames[a] * frame_shift, (frames[b - 1] + 1) * frame_shift
@@ -347,3 +348,21 @@ def unmatched_intervals(flags: Tensor, frame_shift: float) -> List[Tuple[float, 
     starts = torch.nonzero(d == 1).reshape(-1).tolist()
     ends = torch.nonzero(d == -1).reshape(-1).tolist()
     return [(a * frame_shift, b * frame_shift) for a, b in zip(starts, ends)]
+
+
+def skip_edges(edges: Sequence[int]) -> List[Tuple[int, int]]:
+    """gam_ctc_align_long_skips' skip edges of a text with these line_edges, one per line end in order: (e_i, x_i), x_i the
+    blank just after the i-th token with bit 1 set and e_i = x_{i-1} (0 for the first).  The edge jumps n_i = (x_i - e_i) / 2
+    tokens: the line and any joining token before it."""
+    out, e = [], 0
+    for j, f in enumerate(edges):
+        if f & 2:
+            out.append((e, 2 * (j + 1)))
+            e = 2 * (j + 1)
+    return out
+
+
+def skipped_lines(ranges: Sequence[Tuple[int, int]], frames: Sequence[int]) -> List[int]:
+    """The lines a path with skips jumped, in ascending order: the lines with tokens whose last token has frame -1.  Only
+    meaningful for an alignment that has a path."""
+    return [i for i, (a, b) in enumerate(ranges) if b > a and frames[b - 1] < 0]

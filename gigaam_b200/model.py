@@ -387,7 +387,8 @@ class GigaAMASR(GigaAM):
 
     @torch.inference_mode()
     def align_longform(self, wav_file, text: Union[str, Sequence[str]], word_timestamps: bool = True, window: float = 30.0,
-                       overlap: float = 4.0, batch_size: int = 16, *, gap_threshold: Optional[float] = None) -> LongformAlignment:
+                       overlap: float = 4.0, batch_size: int = 16, *, gap_threshold: Optional[float] = None,
+                       skip_threshold: Optional[float] = None) -> LongformAlignment:
         """Align a known text, one string or a sequence of lines, to a recording of any length (INTEGRATION.md §7e).  The
         encoder runs over overlapping windows (`longform.plan_windows`), the windows' CTC log-probs are stitched into one
         sequence and gam_ctc_align_long aligns the whole text to it: up to 65 536 tokens, no frame limit.  Returns one
@@ -396,19 +397,24 @@ class GigaAMASR(GigaAM):
         `gap_threshold` (theta in (0, 1], INTEGRATION.md §7e) lets audio between lines that the text lacks stay unaligned
         (gam_ctc_align_long_gaps): a frame at a line's edge is left unmatched where theta times the greedy decoder's
         probability beats blank, and the result's `unmatched` lists those stretches; ValueError for theta outside (0, 1] as
-        float32, or NaN."""
-        from .longform import line_edges, line_segments, plan_windows, stitch_ctc_log_probs, unmatched_intervals
+        float32, or NaN.
+        `skip_threshold` (psi in (0, 1], the same checks) lets whole lines the recording lacks be skipped
+        (gam_ctc_align_long_skips): skipping a line and the joining token before it costs psi per token, and the
+        result's `skipped` lists the skipped lines."""
+        from .longform import line_edges, line_segments, plan_windows, skipped_lines, stitch_ctc_log_probs, unmatched_intervals
         from .timestamps_utils import compute_frame_shift, gap_confidence, path_confidence, words_from_device
         if self._ncfg["head"].get("type") == "rnnt":
             raise NotImplementedError("align_longform needs a CTC head: RNN-T alignment walks a [T, U + 1] lattice, about "
                                       "4.5e9 nodes for an hour of speech, and banding it would no longer give the Viterbi "
                                       "path; use a *_ctc model, or align() up to max_encoded_frames")
-        log_theta = None
-        if gap_threshold is not None:
-            theta = float(np.float32(gap_threshold))
-            if not 0.0 < theta <= 1.0:          # NaN fails too
-                raise ValueError(f"align_longform: gap_threshold must be in (0, 1], got {gap_threshold!r}")
-            log_theta = float(np.float32(math.log(theta)))   # spot's rounding of log theta
+
+        def log_threshold(name, value):
+            x = float(np.float32(value))
+            if not 0.0 < x <= 1.0:              # NaN fails too
+                raise ValueError(f"align_longform: {name} must be in (0, 1], got {value!r}")
+            return float(np.float32(math.log(x)))   # spot's rounding of log theta
+        log_theta = None if gap_threshold is None else log_threshold("gap_threshold", gap_threshold)
+        log_psi = None if skip_threshold is None else log_threshold("skip_threshold", skip_threshold)
         lines = [text] if isinstance(text, str) else list(text)
         norm, ids, ranges = self._line_tokens(lines)
         if len(ids) > ALIGN_LONG_MAX_TOKENS:
@@ -429,29 +435,47 @@ class GigaAMASR(GigaAM):
         targets_d = targets.to(eng.device)
         target_len_d = torch.tensor([U], dtype=torch.int32, device=eng.device)
         enc_len = torch.tensor([T], dtype=torch.int32, device=eng.device)
-        if log_theta is None:
+        skip_rows = skip_logp = None
+        if log_theta is None and log_psi is None:
             frames, token_logp, viterbi_logp, log_likelihood, path_rows = eng.ctc_align_long(lp, enc_len, targets_d, target_len_d)
         else:
             edges = torch.tensor(line_edges(ranges, U), dtype=torch.uint8).reshape(1, U).to(eng.device)
-            frames, token_logp, viterbi_logp, log_likelihood, path_rows, unmatched, u_rows, u_logp = eng.ctc_align_long(
-                lp, enc_len, targets_d, target_len_d, gaps=(edges, log_theta))
+            gaps = (edges, -math.inf if log_theta is None else log_theta)
+            if log_psi is None:
+                frames, token_logp, viterbi_logp, log_likelihood, path_rows, unmatched, u_rows, u_logp = eng.ctc_align_long(
+                    lp, enc_len, targets_d, target_len_d, gaps=gaps)
+            else:
+                (frames, token_logp, viterbi_logp, log_likelihood, path_rows, unmatched, u_rows, u_logp, skip_rows,
+                 skip_logp) = eng.ctc_align_long(lp, enc_len, targets_d, target_len_d, gaps=gaps, skips=log_psi)
         del lp
         vit, ll = float(viterbi_logp[0]), float(log_likelihood[0])
         shift = compute_frame_shift(int(length[0]), T)
         fr, logp = frames[0].cpu().tolist(), token_logp[0].cpu().tolist()
+        skipped = None
+        if log_psi is not None:
+            skipped = skipped_lines(ranges, fr) if math.isfinite(vit) else []
         words, word_first = None, None
         if word_timestamps:
             words, word_first = [], []
-            if U > 0 and math.isfinite(vit):
-                ws, we, wf, wn, k = (t[0].cpu().tolist() for t in eng.group_words(targets_d, frames, target_len_d, self._word_flags()))
-                words = words_from_device(self.decoding.tokenizer, ids, ws[:k], we[:k], wf[:k], wn[:k], shift, logp)
-                word_first = wf[:k]
-        segs = line_segments(norm, ranges, fr, logp, shift, vit, words, word_first)
-        if log_theta is None:
+            kept = [i for i, f in enumerate(fr) if f >= 0] if skipped else None
+            if U > 0 and math.isfinite(vit) and kept != []:     # a path that skips every line has no words
+                if skipped:                                     # group the aligned tokens only
+                    k_ids, k_logp = [ids[i] for i in kept], [logp[i] for i in kept]
+                    k_idx = torch.tensor(kept, dtype=torch.int64, device=eng.device)
+                    k_targets, k_frames = targets_d[:, k_idx].contiguous(), frames[:, k_idx].contiguous()
+                    k_len = torch.tensor([len(kept)], dtype=torch.int32, device=eng.device)
+                else:
+                    k_ids, k_logp, k_targets, k_frames, k_len = ids, logp, targets_d, frames, target_len_d
+                ws, we, wf, wn, k = (t[0].cpu().tolist() for t in eng.group_words(k_targets, k_frames, k_len, self._word_flags()))
+                words = words_from_device(self.decoding.tokenizer, k_ids, ws[:k], we[:k], wf[:k], wn[:k], shift, k_logp)
+                word_first = wf[:k] if kept is None else [kept[f] for f in wf[:k]]
+        segs = line_segments(norm, ranges, fr, logp, shift, vit, words, word_first, skipped or ())
+        if log_theta is None and log_psi is None:
             return LongformAlignment(segments=segs, log_likelihood=ll, confidence=path_confidence(vit, int(path_rows[0])))
         matched = int(path_rows[0]) - int(u_rows[0])
-        conf = gap_confidence(vit, float(u_logp[0]), matched)
-        return LongformAlignment(segments=segs, log_likelihood=ll, confidence=conf, unmatched=unmatched_intervals(unmatched[0], shift))
+        conf = gap_confidence(vit, float(u_logp[0]), matched, 0.0 if skip_logp is None else float(skip_logp[0]))
+        gaps_out = None if log_theta is None else unmatched_intervals(unmatched[0], shift)
+        return LongformAlignment(segments=segs, log_likelihood=ll, confidence=conf, unmatched=gaps_out, skipped=skipped)
 
     @torch.inference_mode()
     def transcribe_windowed(self, wav_file, word_timestamps: bool = False, confidence: bool = False, window: float = 30.0,

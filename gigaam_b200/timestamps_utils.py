@@ -75,10 +75,12 @@ def path_confidence(path_logp: float, path_rows: int) -> float:
     return math.exp(float(path_logp) / int(path_rows)) if int(path_rows) > 0 else math.nan
 
 
-def gap_confidence(viterbi_logp: float, unmatched_logp: float, matched_rows: int) -> float:
-    """exp((viterbi_logp - unmatched_logp) / matched_rows): an alignment with gaps' Viterbi score per matched frame, the
-    unmatched frames' scores taken out; NaN when no frame is matched."""
-    return math.exp((float(viterbi_logp) - float(unmatched_logp)) / int(matched_rows)) if int(matched_rows) > 0 else math.nan
+def gap_confidence(viterbi_logp: float, unmatched_logp: float, matched_rows: int, skip_logp: float = 0.0) -> float:
+    """exp((viterbi_logp - unmatched_logp - skip_logp) / matched_rows): an alignment with gaps' Viterbi score per matched
+    frame, the unmatched frames' scores and the skip edges' penalties taken out; NaN when no frame is matched."""
+    if int(matched_rows) <= 0:
+        return math.nan
+    return math.exp((float(viterbi_logp) - float(unmatched_logp) - float(skip_logp)) / int(matched_rows))
 
 
 def words_from_device(tokenizer, ids: Sequence[int], word_start: Sequence[int], word_end: Sequence[int],

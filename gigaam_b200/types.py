@@ -115,14 +115,18 @@ class LongformAlignment(_Record):
     whole recording's `log_likelihood` (forward score) and `confidence` = exp(Viterbi path score / frames), as in
     `Alignment`.  With `gap_threshold`, `unmatched` holds the (start, end) seconds of every maximal run of frames the text
     left unaligned, `log_likelihood` is the forward score of the graph with gaps and `confidence` = exp((Viterbi score -
-    score of the unmatched frames) / matched frames) (NaN when no frame is matched); without it `unmatched` is None."""
-    __slots__ = _fields = ("segments", "log_likelihood", "confidence", "unmatched")
-    _defaults = {"unmatched": None}
-    _quiet = ("unmatched",)
+    score of the unmatched frames) / matched frames) (NaN when no frame is matched); without it `unmatched` is None.
+    With `skip_threshold`, `skipped` holds the ascending indices of the lines the alignment skipped (their segments have
+    no time span and no words), `log_likelihood` is the forward score of the graph with skips and the skip edges' scores
+    are also taken out of `confidence`; without it `skipped` is None."""
+    __slots__ = _fields = ("segments", "log_likelihood", "confidence", "unmatched", "skipped")
+    _defaults = {"unmatched": None, "skipped": None}
+    _quiet = ("unmatched", "skipped")
     segments: List[Segment]
     log_likelihood: float
     confidence: float
     unmatched: Optional[List[Tuple[float, float]]]
+    skipped: Optional[List[int]]
 
     @property
     def text(self) -> str:

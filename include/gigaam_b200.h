@@ -346,6 +346,36 @@ int gam_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const int32_t
                             void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp, float* viterbi_logp,
                             float* log_likelihood, int32_t* path_rows, uint8_t* unmatched, int32_t* unmatched_rows,
                             float* unmatched_logp, void* stream);
+/* gam_ctc_align_long_gaps for a text that contains lines the recording lacks: a whole line may be skipped.  The graph is
+ * gam_ctc_align_long_gaps' (the same states, transitions, emissions with the boundary states, tie rules, NaN rule and
+ * outputs) with one more kind of edge:
+ *   - Lines come from line_edges: a token with bit 1 set ends a line.  The exit state of the i-th such token j_i is the
+ *     blank just after it, x_i = 2 (j_i + 1).  The skip source is e_i = x_{i-1}, or state 0 for the first line, and
+ *     n_i = (x_i - e_i) / 2 is the number of tokens the edge jumps: the line and any joining token before it (such as the
+ *     space between charwise lines).  Skips of consecutive lines chain, since x_i = e_{i+1}.
+ *   - Edge: (t - 1, e_i) -> (t, x_i) with weight pen_i = fp32(n_i) * log_psi, one fp32 multiply.  x_i emits what it emits
+ *     without the edge (the gap emission included).
+ *   - Viterbi at x_i: the candidates are compared in the order stay, s - 1, skip, a later one winning only when strictly
+ *     greater; the skip candidate is the fp32 add v(t - 1, e_i) + pen_i.  Forward: f(t, x_i) = e_t + lse3(f(t - 1, x_i),
+ *     f(t - 1, x_i - 1), f(t - 1, e_i) + pen_i), operands in that order.
+ *   - log_psi: the fp32 log of a threshold psi in (0, 1]; -inf is accepted and gives every output of
+ *     gam_ctc_align_long_gaps bit for bit (on input without +inf scores).  NaN and values > 0 are refused.
+ *   - The initial and final states are unchanged: skipping the first line costs one frame in state 0, and skipping the last
+ *     line lands on 2 U_b.  A text may have a path with skips where it had none without.
+ * Outputs, besides gam_ctc_align_long_gaps':
+ *   tokens jumped by a skip edge on the Viterbi path have frame -1 and token_logp -inf;
+ *   skipped_rows [B] i32: the number of skip edges on the path;
+ *   skip_logp [B] f32: the fp32 sum of their pen_i in frame order (0 without a path, NaN for a poisoned recording).
+ * Workspace: gam_ctc_align_long_gaps' (the sources are found again from line_edges); *_workspace_bytes returns what
+ * gam_ctc_align_long_gaps_workspace_bytes returns.  The same launches, orders and guarantees as gam_ctc_align_long_gaps: the
+ * same bits at every cluster size and in any batch, no host synchronisation, capturable in a CUDA graph.  Refuses a NaN or
+ * positive log_psi, a NULL skipped_rows or skip_logp, and everything gam_ctc_align_long_gaps refuses. */
+int64_t gam_ctc_align_long_skips_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_ctc_align_long_skips(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                             const int32_t* target_len, const uint8_t* line_edges, int32_t B, int32_t T, int32_t U, float log_theta,
+                             float log_psi, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                             float* viterbi_logp, float* log_likelihood, int32_t* path_rows, uint8_t* unmatched,
+                             int32_t* unmatched_rows, float* unmatched_logp, int32_t* skipped_rows, float* skip_logp, void* stream);
 /* ---- CTC keyword spotting: where in a recording each of K keywords was said, and how sure that is.  One exact Viterbi
  * per (recording, keyword) over the caller's fp32 log-probs; no hypothesis search.
  *
@@ -649,6 +679,13 @@ int gam_test_ctc_align_long_gaps(gam_handle* h, const float* log_probs, const in
                                  void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp, float* viterbi_logp,
                                  float* log_likelihood, int32_t* path_rows, uint8_t* unmatched, int32_t* unmatched_rows,
                                  float* unmatched_logp, int32_t cluster_ctas, int32_t* plan, void* stream);
+/* gam_ctc_align_long_skips with the cluster size forced, as gam_test_ctc_align_long */
+int gam_test_ctc_align_long_skips(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets,
+                                  const int32_t* target_len, const uint8_t* line_edges, int32_t B, int32_t T, int32_t U, float log_theta,
+                                  float log_psi, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
+                                  float* viterbi_logp, float* log_likelihood, int32_t* path_rows, uint8_t* unmatched,
+                                  int32_t* unmatched_rows, float* unmatched_logp, int32_t* skipped_rows, float* skip_logp,
+                                  int32_t cluster_ctas, int32_t* plan, void* stream);
 /* gam_ctc_spot with the keyword warps per CTA forced to warps_per_cta in [1, 32] (0: the library's choice); the outputs do
  * not depend on it. */
 int gam_test_ctc_spot(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,

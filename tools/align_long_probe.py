@@ -1,7 +1,7 @@
 """Cost of long-form alignment (GigaAMASR.align_longform: window encoding, CTC log-probs, stitching, gam_ctc_align_long and
 word grouping), with CUDA events.
 
-    python tools/align_long_probe.py [--quick] [--gaps]
+    python tools/align_long_probe.py [--quick] [--gaps] [--skips]
 
 Part 1, the kernel: gam_ctc_align_long on random log-probs [1, 2000, 34] for U = 1k ... 64k tokens at forced cluster sizes
 C = 1, 4 and 16 (where the states fit), as time per frame.  The backtrack's share is the difference to the same call with one
@@ -13,6 +13,10 @@ Part 3, alignment with gaps: gam_ctc_align_long_gaps (its row-max pre-pass and s
 random log-probs at V + 1 = 34 and 257, for T = 2000 frames at U = 1k ... 64k tokens in lines of 500 tokens, and for an hour
 (T = 90 000, U = 65 536), at the library's cluster size; medians of 7 (3 for the hour), the two calls alternating.  --gaps runs
 part 3 alone.
+Part 4, alignment with skipped lines: gam_ctc_align_long_skips against gam_ctc_align_long_gaps at part 3's shapes and theta,
+psi = 0.5, with lines of 500 tokens and of 12 tokens (short lines: many skip edges, an exit blank in most warps), the two
+calls alternating as in part 3.  A skip source is read from another CTA only when its line crosses a CTA boundary, so at
+most C - 1 lines per recording do (none at U <= 4 096, where the library's plan is C = 1).  --skips runs part 4 alone.
 The card's name, power limit and SM clocks are read in the same run; the last line is one JSON record of everything printed."""
 import json
 import statistics
@@ -170,11 +174,47 @@ def gaps_part(quick):
     return rows
 
 
+def skips_part(quick):
+    rows = []
+    for name in ("v2_ctc", "v3_e2e_ctc"):
+        ck = gigaam.synthetic_checkpoint(name, seed=0, n_layers=1)
+        eng = gigaam.load_model(name, fp16_encoder=False, device=dev, checkpoint=ck)._get_engine()
+        V1 = eng.num_classes
+        g = torch.Generator().manual_seed(V1)
+        sizes = [(2000, 1024), (2000, 65536)] if quick else [(2000, u) for u in (1024, 4096, 16384, 32768, 65536)]
+        for T, U in sizes + [(90000, 65536)]:
+            lp = torch.randn(1, T, V1, generator=g).log_softmax(-1).to(dev)
+            y = torch.randint(0, V1 - 1, (1, U), generator=g, dtype=torch.int32).to(dev)
+            args = (torch.tensor([T]), y, torch.tensor([U]))
+            for line in (500, 12):
+                edges = torch.tensor(longform.line_edges([(a, min(a + line, U)) for a in range(0, U, line)], U), dtype=torch.uint8)
+                gaps = (edges[None].to(dev), -0.6931472)
+                reps, warm = (3, 1) if T > 2000 else (7, 2)
+                gap_ms, skip_ms = [], []
+                for _ in range(warm):
+                    eng.ctc_align_long(lp, *args, gaps=gaps)
+                    out = eng.ctc_align_long(lp, *args, gaps=gaps, skips=-0.6931472)
+                for _ in range(reps):             # alternating, so that drift of the clocks hits both
+                    gap_ms.append(median_ms(lambda: eng.ctc_align_long(lp, *args, gaps=gaps), warmup=0, reps=1))
+                    skip_ms.append(median_ms(lambda: eng.ctc_align_long(lp, *args, gaps=gaps, skips=-0.6931472), warmup=0, reps=1))
+                a, b = statistics.median(gap_ms), statistics.median(skip_ms)
+                rows.append(dict(V1=V1, T=T, U=U, line=line, gaps_ms=round(a, 3), skips_ms=round(b, 3), ratio=round(b / a, 3),
+                                 skipped=int(out[8][0])))
+                print(f"V+1={V1:4d} T={T:6d} U={U:6d} lines of {line:3d}: gaps {a:9.3f} ms, skips {b:9.3f} ms ({b / a:.3f}x), "
+                      f"{int(out[8][0])} lines skipped", flush=True)
+            del lp
+        del eng
+        torch.cuda.empty_cache()
+    return rows
+
+
 def main():
     quick = "--quick" in sys.argv
     info = card()
     print(info, flush=True)
-    if "--gaps" in sys.argv:
+    if "--skips" in sys.argv:
+        rec = dict(card=info, skips=skips_part(quick))
+    elif "--gaps" in sys.argv:
         rec = dict(card=info, gaps=gaps_part(quick))
     else:
         rec = dict(card=info, kernel=kernel_part(quick), calls=[], gaps=gaps_part(quick))
