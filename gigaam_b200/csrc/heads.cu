@@ -13,6 +13,11 @@
 // rows it just wrote (contiguous, coalesced, mostly still in L2).  The alternative, computing the logits twice (once for
 // the statistics, once to write), doubles the GEMM, which is the dominant cost: at joint_hidden 320 a logit is 320 FMAs
 // but the extra normalisation pass is one 4-byte read and write.
+//
+// Non-finite logits follow torch.log_softmax, as the greedy and scored paths of ctc.cu / rnnt_cluster.cu do: a -inf logit
+// (a -inf bias bans a class) gives -inf at its class and leaves the rest of the row finite; a NaN or +inf logit, or a
+// row whose logits are all -inf, gives a row of NaN.  The running log-sum-exp below skips -inf and lets NaN and +inf
+// poison the sum; finite rows take the same branches as without the rule, so their bits do not depend on it.
 #include <cmath>
 
 #include "kernels.h"
@@ -21,19 +26,23 @@
 namespace gam {
 namespace {
 
-// running log-sum-exp: (m, s) = (max so far, sum of exp(v - m))
+// running log-sum-exp: (m, s) = (max so far, sum of exp(v - m)).  m is never NaN; s is NaN once a NaN or a second +inf
+// was pushed, and a +inf max turns s into NaN at the merge (exp(inf - inf)).
 __device__ __forceinline__ void lse_push(float& m, float& s, float v) {
   if (v > m) {
     s = s * expf(m - v) + 1.f;
     m = v;
-  } else {
+  } else if (v != -INFINITY) {   // -inf adds exp(-inf) = 0, but exp(-inf - -inf) = NaN while m is still -inf; NaN gets in
     s += expf(v - m);
   }
 }
 
 __device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
   const float M = fmaxf(m, m2);
-  if (M == -INFINITY) return;   // both still empty
+  if (M == -INFINITY) {   // neither side has a logit above -inf: their sums are 0, or NaN if a NaN was pushed
+    s += s2;
+    return;
+  }
   s = s * expf(m - M) + s2 * expf(m2 - M);
   m = M;
 }

@@ -308,10 +308,14 @@ class Engine:
 
     def _dev_head(self, name: str, t: Tensor) -> int:
         """Upload one packed head tensor (fp32) outside the pack cache: it is neither replayed from nor written to it.
-        repack_head() later rewrites it in place."""
-        t = t.detach().to(device=self.device, dtype=torch.float32).contiguous()
-        self._head_bufs[name] = t
-        return t.data_ptr()
+        repack_head() later rewrites it in place.  The buffer is always a copy, never a view of the parameter (a repack
+        would bump the parameter's version counter and so repack again on every later call), and a normal tensor even
+        when the engine is built under torch.inference_mode() (a repack outside it could not write an inference tensor)."""
+        with torch.inference_mode(False):
+            buf = torch.empty(t.shape, dtype=torch.float32, device=self.device)
+            buf.copy_(t.detach())
+        self._head_bufs[name] = buf
+        return buf.data_ptr()
 
     def _read_pack_cache(self, path: str) -> Optional[List[Tensor]]:
         if not os.path.isfile(path):

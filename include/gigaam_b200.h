@@ -240,13 +240,19 @@ int gam_rnnt_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T
  *
  * CTC posteriors: enc: device f32 [B, T, d_model] (gam_encode's layout)
  *   -> log_probs: device f32 [B, T, V+1] = log_softmax(W enc + b) over the last axis.  Every frame is computed; frames at or
- *   past enc_len hold zeros in gam_encode's output and so give log_softmax(b). */
+ *   past enc_len hold zeros in gam_encode's output and so give log_softmax(b).
+ * Non-finite logits follow torch.log_softmax, here and in gam_rnnt_joint / gam_rnnt_align_scores: a -inf logit (e.g. a -inf
+ * bias, which bans a class) gives -inf at its class and finite log-probs elsewhere; a row with a NaN or +inf logit, or with
+ * every logit -inf, is all NaN. */
 int gam_ctc_log_probs(gam_handle* h, const float* enc, int32_t B, int32_t T, float* log_probs, void* stream);
 
 /* RNN-T joint lattice: enc: device f32 [B, T, d_model]; dec: device f32 [B, U, pred_hidden] (prediction-network outputs)
  *   -> out: device f32 [B, T, U, V+1] = log_softmax(W_o relu(W_e enc[b,t] + b_e + W_p dec[b,u] + b_p) + b_o).
  * workspace: device scratch of at least gam_rnnt_joint_workspace_bytes(B, T, U) bytes (the two projections); the
  * [B, T, U, joint_hidden] hidden tensor is never stored.  Offsets are 64-bit: out may exceed 2^31 elements.
+ * Needs joint_hidden % 4 == 0 and <= 736 (the hidden tile lives in shared memory), pred_hidden % 16 == 0.  Non-finite
+ * logits as gam_ctc_log_probs: -inf only at a -inf logit's class, all NaN for a row with a NaN or +inf logit (relu keeps
+ * a NaN of enc or dec, so it reaches every row that reads it).
  * gam_rnnt_joint_workspace_bytes returns -1 for a handle without an RNN-T head or non-positive sizes. */
 int64_t gam_rnnt_joint_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
 int gam_rnnt_joint(gam_handle* h, const float* enc, const float* dec, int32_t B, int32_t T, int32_t U, void* workspace,
