@@ -68,7 +68,9 @@ EXPORTS = ("gam_create", "gam_destroy", "gam_last_error", "gam_version", "gam_lo
            "gam_rnnt_greedy_resume", "gam_ctc_spot", "gam_test_ctc_spot", "gam_ctc_bias_workspace_bytes", "gam_ctc_bias",
            "gam_ctc_align_long_gaps_workspace_bytes", "gam_ctc_align_long_gaps", "gam_test_ctc_align_long_gaps",
            "gam_ctc_spot_state_bytes", "gam_ctc_spot_state_init", "gam_ctc_spot_resume",
-           "gam_ctc_align_long_skips_workspace_bytes", "gam_ctc_align_long_skips", "gam_test_ctc_align_long_skips")
+           "gam_ctc_align_long_skips_workspace_bytes", "gam_ctc_align_long_skips", "gam_test_ctc_align_long_skips",
+           "gam_rnnt_loss_saved_bytes", "gam_rnnt_loss_workspace_bytes", "gam_rnnt_loss", "gam_rnnt_loss_backward_workspace_bytes",
+           "gam_rnnt_loss_backward")
 
 
 def lib_path() -> Path:
@@ -173,6 +175,12 @@ def load() -> C.CDLL:
                lib.gam_ctc_align_long_gaps, lib.gam_test_ctc_align_long_gaps, lib.gam_ctc_align_long_skips,
                lib.gam_test_ctc_align_long_skips):
         fn.restype = C.c_int
+    for fn in (lib.gam_rnnt_loss_saved_bytes, lib.gam_rnnt_loss_workspace_bytes, lib.gam_rnnt_loss_backward_workspace_bytes):
+        fn.argtypes = [H, i32, i32, i32]
+        fn.restype = i64
+    lib.gam_rnnt_loss.argtypes = [H] + [c_vp] * 5 + [i32, i32, i32, c_vp, i64, c_vp, c_vp, c_vp]
+    lib.gam_rnnt_loss_backward.argtypes = [H] + [c_vp] * 5 + [i32, i32, i32, c_vp, c_vp, c_vp, i64] + [c_vp] * 9
+    lib.gam_rnnt_loss.restype = lib.gam_rnnt_loss_backward.restype = C.c_int
     lib.gam_ctc_spot.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32, C.c_float, i32] + [c_vp] * 5
     lib.gam_test_ctc_spot.argtypes = [H, c_vp, c_vp, i32, i32, c_vp, c_vp, i32, i32, C.c_float, i32] + [c_vp] * 4 + [i32, c_vp]
     lib.gam_ctc_spot_state_bytes.argtypes = [H, i32]

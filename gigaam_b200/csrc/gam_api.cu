@@ -1224,7 +1224,7 @@ int gam_rnnt_align_scores(gam_handle* h, const float* enc, const float* dec, con
   { PROF(PC_RNNT_JOINT);
     launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, P, B * U1, J, c.pred_hidden, s); }
   { PROF(PC_RNNT_JOINT);
-    rc = launch_rnnt_joint_gather(E, P, h->w.rnnt_wo, h->w.rnnt_bo, targets, blank, label, B, T, U1, J, c.num_classes, s); }
+    rc = launch_rnnt_joint_gather(E, P, h->w.rnnt_wo, h->w.rnnt_bo, targets, blank, label, nullptr, B, T, U1, J, c.num_classes, s); }
   if (rc != 0) return fail(h, -4, "rnnt_align_scores: launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "rnnt_align_scores");
   return 0;
@@ -1489,6 +1489,152 @@ int gam_rnnt_predict_backward(gam_handle* h, const int64_t* x, const float* h0, 
     }
   }
   GAM_CHECK_LAUNCH(h, "rnnt_predict_backward");
+  return 0;
+}
+
+// ---- fused RNN-T loss (csrc/rnnt_loss.cu; stage 1 is the gathered joint of heads.cu with the row lse kept)
+namespace {
+constexpr int64_t kLossMaxProjRows = 65535LL * 64;   // grid.y limit of the projection GEMMs (64 rows per block)
+
+bool loss_sizes_ok(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || T > h->max_t || U < 0 || U > kAlignMaxTokens) return false;
+  const gam_config& c = h->cfg;
+  const int J = c.joint_hidden;
+  if (J % 4 != 0 || J > rnnt_joint_max_hidden() || J > rnnt_loss_max_hidden() || c.pred_hidden % 16 != 0 || c.d_model % 16 != 0)
+    return false;
+  return static_cast<int64_t>(B) * T <= kLossMaxProjRows && static_cast<int64_t>(B) * (U + 1) <= kLossMaxProjRows;
+}
+
+struct LossFwdWs { float *E, *P, *blank, *label, *alpha; };
+int64_t loss_fwd_layout(const gam_config& c, int32_t B, int32_t T, int32_t U, uint8_t* base, LossFwdWs* w) {
+  const int64_t J = c.joint_hidden, BT = static_cast<int64_t>(B) * T, BU1 = static_cast<int64_t>(B) * (U + 1), N = BT * (U + 1);
+  Carve cv{base};
+  w->E = cv.take(BT * J);
+  w->P = cv.take(BU1 * J);
+  w->blank = cv.take(N);
+  w->label = cv.take(N);
+  w->alpha = cv.take(N);
+  return cv.off;
+}
+
+struct LossBwdWs { float *E, *P, *dE, *dP, *dE_part, *dP_part, *part; };
+int64_t loss_bwd_layout(const gam_config& c, int32_t B, int32_t T, int32_t U, uint8_t* base, LossBwdWs* w) {
+  const RnntLossPlan p = rnnt_loss_plan(B, T, U, c.num_classes);
+  const int64_t J = c.joint_hidden, BT = static_cast<int64_t>(B) * T, BU1 = static_cast<int64_t>(B) * (U + 1);
+  Carve cv{base};
+  w->E = cv.take(BT * J);
+  w->P = cv.take(BU1 * J);
+  w->dE = cv.take(BT * J);
+  w->dP = cv.take(BU1 * J);
+  w->dE_part = cv.take(p.NS * BT * J);
+  w->dP_part = cv.take(p.ST * BU1 * J);
+  w->part = cv.take(max3(p.S > 1 ? static_cast<int64_t>(p.S) * c.num_classes * (J + 1) : 0,
+                         outer_sum_workspace_floats(BT, static_cast<int>(J), c.d_model, true),
+                         outer_sum_workspace_floats(BU1, static_cast<int>(J), c.pred_hidden, true)));
+  return cv.off;
+}
+}  // namespace
+
+int64_t gam_rnnt_loss_saved_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!loss_sizes_ok(h, B, T, U)) return -1;
+  return static_cast<int64_t>(3) * B * T * (U + 1) * 4;
+}
+
+int64_t gam_rnnt_loss_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!loss_sizes_ok(h, B, T, U)) return -1;
+  LossFwdWs w;
+  return loss_fwd_layout(h->cfg, B, T, U, nullptr, &w) + 1024;
+}
+
+int gam_rnnt_loss(gam_handle* h, const float* enc, const float* dec, const int32_t* targets, const int32_t* enc_len,
+                  const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, float* saved,
+                  float* loss, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 2) return fail(h, -1, "rnnt_loss: model has no RNN-T head");
+  if (!loss_sizes_ok(h, B, T, U))
+    return fail(h, -1, "rnnt_loss: unsupported sizes (B=%d, T=%d, U=%d; T <= %d, U <= %d, joint_hidden %d <= %d)", B, T, U, h->max_t,
+                kAlignMaxTokens, c.joint_hidden, rnnt_loss_max_hidden());
+  if (!enc || !dec || (U > 0 && !targets) || !enc_len || !target_len || !saved || !loss)
+    return fail(h, -1, "rnnt_loss: a required pointer is NULL");
+  const int64_t need = gam_rnnt_loss_workspace_bytes(h, B, T, U);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "rnnt_loss: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  LossFwdWs w;
+  loss_fwd_layout(c, B, T, U, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  const int J = c.joint_hidden, U1 = U + 1;
+  const int64_t N = static_cast<int64_t>(B) * T * U1;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc = 0;
+  { PROF(PC_RNNT_JOINT);
+    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, w.E, B * T, J, c.d_model, s); }
+  { PROF(PC_RNNT_JOINT);
+    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, w.P, B * U1, J, c.pred_hidden, s); }
+  { PROF(PC_RNNT_JOINT);
+    rc = launch_rnnt_joint_gather(w.E, w.P, h->w.rnnt_wo, h->w.rnnt_bo, targets, w.blank, w.label, saved, B, T, U1, J, c.num_classes, s); }
+  if (rc != 0) return fail(h, -4, "rnnt_loss: stage 1 launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+  { PROF(PC_ALIGN);
+    launch_rnnt_loss_alpha_beta(w.blank, w.label, enc_len, target_len, B, T, U, w.alpha, saved + N, saved + 2 * N, loss, s); }
+  GAM_CHECK_LAUNCH(h, "rnnt_loss");
+  return 0;
+}
+
+int64_t gam_rnnt_loss_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!loss_sizes_ok(h, B, T, U)) return -1;
+  LossBwdWs w;
+  return loss_bwd_layout(h->cfg, B, T, U, nullptr, &w) + 1024;
+}
+
+int gam_rnnt_loss_backward(gam_handle* h, const float* enc, const float* dec, const int32_t* targets, const int32_t* enc_len,
+                           const int32_t* target_len, int32_t B, int32_t T, int32_t U, const float* saved, const float* grad_loss,
+                           void* workspace, int64_t workspace_bytes, float* d_enc, float* d_dec, float* dW_enc, float* db_enc,
+                           float* dW_pred, float* db_pred, float* dW_out, float* db_out, void* stream) {
+  const gam_config& c = h->cfg;
+  if (c.head != 2) return fail(h, -1, "rnnt_loss_backward: model has no RNN-T head");
+  if (!loss_sizes_ok(h, B, T, U))
+    return fail(h, -1, "rnnt_loss_backward: unsupported sizes (B=%d, T=%d, U=%d; T <= %d, U <= %d, joint_hidden %d <= %d)", B, T, U,
+                h->max_t, kAlignMaxTokens, c.joint_hidden, rnnt_loss_max_hidden());
+  if (!enc || !dec || (U > 0 && !targets) || !enc_len || !target_len || !saved || !grad_loss)
+    return fail(h, -1, "rnnt_loss_backward: a required pointer is NULL");
+  if ((dW_enc == nullptr) != (db_enc == nullptr) || (dW_pred == nullptr) != (db_pred == nullptr) || (dW_out == nullptr) != (db_out == nullptr))
+    return fail(h, -1, "rnnt_loss_backward: each weight gradient goes with its bias gradient");
+  const int64_t need = gam_rnnt_loss_backward_workspace_bytes(h, B, T, U);
+  if (workspace == nullptr || workspace_bytes < need)
+    return fail(h, -1, "rnnt_loss_backward: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  LossBwdWs w;
+  loss_bwd_layout(c, B, T, U, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  const int J = c.joint_hidden, V1 = c.num_classes, U1 = U + 1;
+  const int64_t BT = static_cast<int64_t>(B) * T, BU1 = static_cast<int64_t>(B) * U1, N = BT * U1;
+  const RnntLossPlan plan = rnnt_loss_plan(B, T, U, V1);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // the forward's two projections, recomputed with the forward's kernels (same bits)
+  { PROF(PC_HEAD_BACKWARD);
+    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, w.E, B * T, J, c.d_model, s); }
+  { PROF(PC_HEAD_BACKWARD);
+    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, w.P, B * U1, J, c.pred_hidden, s); }
+  const bool need_hidden = d_enc || d_dec || dW_enc || dW_pred;
+  if (need_hidden || dW_out) {
+    const RnntLossArgs a{w.E, w.P, h->w.rnnt_wo, h->w.rnnt_bo, targets, enc_len, target_len, saved, saved + N, saved + 2 * N, grad_loss,
+                         B, T, U, J, V1};
+    int rc;
+    { PROF(PC_HEAD_BACKWARD);
+      rc = launch_rnnt_loss_grads(a, plan, need_hidden ? w.dE_part : nullptr, w.dP_part, w.part, dW_out, db_out, s); }
+    if (rc != 0) return fail(h, -4, "rnnt_loss_backward: launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+  }
+  if (need_hidden) {
+    { PROF(PC_HEAD_BACKWARD);   // dE[b, t] = sum over the column strips, in strip order
+      launch_segment_sum(w.dE_part, w.dE, BT, plan.NS, J, 1, 1, 0, BT, s); }
+    { PROF(PC_HEAD_BACKWARD);   // dP[b, u] = sum over the frame ranges, in range order
+      launch_segment_sum(w.dP_part, w.dP, BU1, plan.ST, J, 1, 1, 0, BU1, s); }
+  }
+  if (dW_enc != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_outer_sum(w.dE, enc, BT, J, c.d_model, dW_enc, db_enc, w.part, s); }
+  if (dW_pred != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_outer_sum(w.dP, dec, BU1, J, c.pred_hidden, dW_pred, db_pred, w.part, s); }
+  if (d_enc != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_e [J, d]
+    launch_head_matmul(w.dE, h->w.rnnt_enc_w, c.d_model, 1, d_enc, BT, J, c.d_model, nullptr, nullptr, 1, 1, s); }
+  if (d_dec != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_p [J, H] = rnnt_wp_t^T
+    launch_head_matmul(w.dP, h->w.rnnt_wp_t, 1, J, d_dec, BU1, J, c.pred_hidden, nullptr, nullptr, 1, 1, s); }
+  GAM_CHECK_LAUNCH(h, "rnnt_loss_backward");
   return 0;
 }
 

@@ -391,6 +391,11 @@ void launch_outer_sum_joint(const float* A, const float* E, const float* P, int 
   outer_sum(A, XJoint{E, P, K, T, U}, rows, N, K, dW, db, ws, s);
 }
 
+void launch_outer_sum_reduce(const float* part, int S, int N, int K, int Kc, float* dW, float* db, cudaStream_t s) {
+  const int64_t NK = static_cast<int64_t>(N) * Kc;
+  outer_sum_reduce_kernel<<<static_cast<unsigned>((NK + 255) / 256), 256, 0, s>>>(part, S, N, K, Kc, dW, db);
+}
+
 void launch_head_matmul(const float* A, const float* W, int64_t sn, int64_t sk, float* out, int64_t rows, int N, int K,
                         const float* mask_E, const float* mask_P, int T, int U, cudaStream_t s) {
   if (rows <= 0) return;

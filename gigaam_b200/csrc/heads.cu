@@ -131,13 +131,15 @@ __host__ __device__ constexpr size_t joint_smem_bytes(int J) { return (static_ca
 // the logit of the row's next label are kept: U = U_y + 1 lattice columns, targets [B, U_y] i32, and
 //   blank_out[row] = log_softmax(row)[V1 - 1],  label_out[row] = log_softmax(row)[targets[b, u]] for u < U_y
 // (NaN for an id outside [0, V1 - 1), -inf at u = U_y).  Each is the same fp32 subtraction as the lattice's, so it is
-// bit-identical to the matching lattice entry.  out is unused and no [V1] row is stored.
-template <bool kGather>
+// bit-identical to the matching lattice entry.  out is unused and no [V1] row is stored.  kLse (gam_rnnt_loss, gather mode
+// only): lse_out[row] also receives the row's log-sum-exp, the value both gathered entries subtract.
+template <bool kGather, bool kLse = false>
 __global__ void __launch_bounds__(kJThreads) rnnt_joint_kernel(const float* __restrict__ E, const float* __restrict__ P,
                                                                const float* __restrict__ Wo, const float* __restrict__ bo,
                                                                float* __restrict__ out, int T, int U, int J, int V1,
                                                                int64_t rows, const int* __restrict__ targets,
-                                                               float* __restrict__ blank_out, float* __restrict__ label_out) {
+                                                               float* __restrict__ blank_out, float* __restrict__ label_out,
+                                                               float* __restrict__ lse_out) {
   extern __shared__ float4 smem_f4[];
   float* A_s = reinterpret_cast<float*>(smem_f4);   // [Jp][kJLd]: relu(E + P) of the block's rows, k-major
   const int Jp = joint_kpad(J);
@@ -248,6 +250,7 @@ __global__ void __launch_bounds__(kJThreads) rnnt_joint_kernel(const float* __re
       blank_out[row] = blank_s[tid] - lse_s[tid];
       const int y = y_s[tid];
       label_out[row] = y >= 0 ? label_s[tid] - lse_s[tid] : (y == -1 ? -INFINITY : __int_as_float(0x7fc00000));
+      if constexpr (kLse) lse_out[row] = lse_s[tid];
     }
     return;
   }
@@ -356,23 +359,30 @@ int launch_rnnt_joint(const float* E, const float* P, const float* Wo, const flo
   const int64_t blocks = (rows + kJBM - 1) / kJBM;
   if (blocks > 0x7fffffff) return 1;
   rnnt_joint_kernel<false><<<static_cast<unsigned>(blocks), kJThreads, joint_smem_bytes(J), s>>>(E, P, Wo, bo, out, T, U, J, V1, rows,
-                                                                                                  nullptr, nullptr, nullptr);
+                                                                                                  nullptr, nullptr, nullptr, nullptr);
   return 0;
 }
 
 int launch_rnnt_joint_gather(const float* E, const float* P, const float* Wo, const float* bo, const int* targets, float* blank,
-                             float* label, int B, int T, int U1, int J, int V1, cudaStream_t s) {
+                             float* label, float* lse, int B, int T, int U1, int J, int V1, cudaStream_t s) {
   static PerDeviceOnce attr_once;
   constexpr size_t kExtra = 3 * kJBM * 4;   // blank_s, label_s, y_s
   if (J % 4 != 0 || J > rnnt_joint_max_hidden()) return 1;
-  if (attr_once.first() && cudaFuncSetAttribute(rnnt_joint_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                static_cast<int>(kJointMaxSmem + kExtra)) != cudaSuccess)
+  if (attr_once.first() &&
+      (cudaFuncSetAttribute(rnnt_joint_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            static_cast<int>(kJointMaxSmem + kExtra)) != cudaSuccess ||
+       cudaFuncSetAttribute(rnnt_joint_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            static_cast<int>(kJointMaxSmem + kExtra)) != cudaSuccess))
     return -1;
   const int64_t rows = static_cast<int64_t>(B) * T * U1;
   const int64_t blocks = (rows + kJBM - 1) / kJBM;
   if (blocks > 0x7fffffff) return 1;
-  rnnt_joint_kernel<true><<<static_cast<unsigned>(blocks), kJThreads, joint_smem_bytes(J) + kExtra, s>>>(
-      E, P, Wo, bo, nullptr, T, U1, J, V1, rows, targets, blank, label);
+  if (lse != nullptr)
+    rnnt_joint_kernel<true, true><<<static_cast<unsigned>(blocks), kJThreads, joint_smem_bytes(J) + kExtra, s>>>(
+        E, P, Wo, bo, nullptr, T, U1, J, V1, rows, targets, blank, label, lse);
+  else
+    rnnt_joint_kernel<true><<<static_cast<unsigned>(blocks), kJThreads, joint_smem_bytes(J) + kExtra, s>>>(
+        E, P, Wo, bo, nullptr, T, U1, J, V1, rows, targets, blank, label, nullptr);
   return 0;
 }
 

@@ -129,9 +129,10 @@ constexpr size_t kJointMaxSmem = 200 * 1024;
 int rnnt_joint_max_hidden();
 int launch_rnnt_joint(const float* E, const float* P, const float* Wo, const float* bo, float* out, int B, int T, int U, int J,
                       int V1, cudaStream_t s);
-// the same rows, but only blank [B, T, U1] and label [B, T, U1] = the log-probs of blank and of targets[b, u] (targets [B, U1 - 1])
+// the same rows, but only blank [B, T, U1] and label [B, T, U1] = the log-probs of blank and of targets[b, u] (targets [B, U1 - 1]);
+// lse [B, T, U1], when not null, also receives each row's log-sum-exp
 int launch_rnnt_joint_gather(const float* E, const float* P, const float* Wo, const float* bo, const int* targets, float* blank,
-                             float* label, int B, int T, int U1, int J, int V1, cudaStream_t s);
+                             float* label, float* lse, int B, int T, int U1, int J, int V1, cudaStream_t s);
 // one step u of the 1-layer prediction LSTM (heads.cu: lstm_step_kernel documents the operands); H <= 1024
 void launch_lstm_step(const int64_t* x, int U, int u, int V1, const float* emb_gates, const float* whh_t, const float* h_in,
                       int64_t h_pitch, const float* c_in, float* g, float* h_out, float* c_out, int B, int H, cudaStream_t s);
@@ -146,6 +147,27 @@ int launch_ctc_align(const float* log_probs, const int* enc_len, const int* targ
                      cudaStream_t s);
 int launch_rnnt_align(const float* blank, const float* label, const int* enc_len, const int* target_len, int B, int T, int U, uint32_t* bp,
                       int* frames, float* token_logp, float* viterbi_logp, float* log_likelihood, int* path_rows, cudaStream_t s);
+// rnnt_loss.cu: the fused RNN-T loss (gam_rnnt_loss / gam_rnnt_loss_backward).  Node arrays are [B, T, U + 1].
+// alpha: scratch; e_blank / e_label: the edge occupancies the gradient reads; loss [B].  One CTA per utterance.
+int launch_rnnt_loss_alpha_beta(const float* blank, const float* label, const int* enc_len, const int* target_len, int B, int T, int U,
+                                float* alpha, float* e_blank, float* e_label, float* loss, cudaStream_t s);
+// The gradient pass's grid.  Node-major: 64-node tiles of tT frames x tU lattice columns; NS column strips x ST frame ranges
+// per utterance, so dE partials are [NS][B*T][J] and dP partials [ST][B*(U+1)][J].  Class-major: S node slices, partials
+// [S][V1][J + 1] when S > 1.
+struct RnntLossPlan {
+  int tU, tT, NS, ST, S;
+};
+RnntLossPlan rnnt_loss_plan(int B, int T, int U, int V1);
+int rnnt_loss_max_hidden();
+struct RnntLossArgs {
+  const float *E, *P, *Wo, *bo;   // E [B*T, J], P [B*(U+1), J] (biases included), W_o [V1, J], b_o [V1]
+  const int *targets, *enc_len, *target_len;
+  const float *lse, *e_blank, *e_label, *grad;
+  int B, T, U, J, V1;
+};
+// dE_part null: no node-major pass; dW null: no class-major pass.  Returns 1 for an unsupported J, <0 on an attribute error.
+int launch_rnnt_loss_grads(const RnntLossArgs& a, const RnntLossPlan& p, float* dE_part, float* dP_part, float* part, float* dW, float* db,
+                           cudaStream_t s);
 // the CTC sweep of launch_ctc_align over a cluster of C <= kAlignLongMaxCtas CTAs per utterance, for U <= kAlignLongMaxTokens
 // and any T (gam_ctc_align_long); bp as there.  The plan is the smallest C whose states per CTA P (a multiple of 16) fit in
 // shared memory at 20 bytes per state, or `forced_ctas` when it is > 0.  Return 0, 1 for a U or C that does not fit, 2 for a
@@ -259,6 +281,8 @@ void launch_outer_sum_joint(const float* A, const float* E, const float* P, int 
 // out[r, k] = sum_n A[r, n] W[n * sn + k * sk], times [relu(E + P)(r, k) > 0] when mask_E != null (joint row map as above)
 void launch_head_matmul(const float* A, const float* W, int64_t sn, int64_t sk, float* out, int64_t rows, int N, int K,
                         const float* mask_E, const float* mask_P, int T, int U, cudaStream_t s);
+// dW[n, k] (k < K) / db[n] (k = K) = sum over z < S (ascending) of part[z][n][k], part [S][N][Kc]
+void launch_outer_sum_reduce(const float* part, int S, int N, int K, int Kc, float* dW, float* db, cudaStream_t s);
 // out[g, k] = sum_{i < count} X[(g / gi) * so + (g % gi) * si + i * step, k]
 void launch_segment_sum(const float* X, float* out, int64_t groups, int count, int K, int64_t gi, int64_t so, int64_t si, int64_t step,
                         cudaStream_t s);

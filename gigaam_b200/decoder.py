@@ -86,6 +86,29 @@ class _RNNTJointFn(torch.autograd.Function):
         return (None, d_enc, d_dec, *dw)
 
 
+class _RNNTLossFn(torch.autograd.Function):
+    """The fused RNN-T loss (decoding.rnnt_loss) with gam_rnnt_loss_backward behind it (enc / dec inputs, joint.enc, joint.pred,
+    joint_net.1).  Saves the loss call's per-node [3, B, T, U+1] operands, never a lattice."""
+
+    @staticmethod
+    def forward(ctx, module, enc, dec, targets, enc_len, target_len, *params):
+        eng = module._engine()
+        loss, saved = eng.rnnt_loss(enc.detach(), dec.detach(), targets, enc_len, target_len)
+        ctx.module, ctx.versions = module, _param_versions(module)
+        ctx.save_for_backward(enc, dec, targets, enc_len, target_len, saved)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad):
+        _check_versions(ctx)
+        enc, dec, targets, enc_len, target_len, saved = ctx.saved_tensors
+        eng = ctx.module._engine()
+        need_w = any(ctx.needs_input_grad[6:])
+        d_enc, d_dec, *dw = eng.rnnt_loss_backward(enc.detach(), dec.detach(), targets, enc_len, target_len, saved, _f32(grad),
+                                                   ctx.needs_input_grad[1], ctx.needs_input_grad[2], need_w)
+        return (None, d_enc, d_dec, None, None, None, *dw)
+
+
 class _RNNTPredictFn(torch.autograd.Function):
     """RNNTDecoder.predict with gam_rnnt_predict_backward behind it (h0 / c0, embed, lstm weights and biases)."""
 
@@ -160,6 +183,18 @@ class RNNTJoint(Bound):
     def forward(self, enc: Tensor, dec: Tensor) -> Tensor:
         """[B, enc_hidden, T], [B, pred_hidden, U] -> [B, T, U, num_classes] (gigaam/decoder.py:68-69)"""
         return self.joint(enc.transpose(1, 2), dec.transpose(1, 2))
+
+    def _loss(self, enc: Tensor, dec: Tensor, targets: Tensor, enc_len: Tensor, target_len: Tensor) -> Tensor:
+        """enc [B, T, enc_hidden], dec [B, U+1, pred_hidden] f32 on the device, targets [B, U] (blank where unused), enc_len /
+        target_len [B] -> the per-utterance loss [B] (gam_rnnt_loss), differentiable when a joint parameter, enc or dec
+        requires grad.  decoding.rnnt_loss is the public entry point."""
+        eng = self._engine()
+        enc, dec = enc.contiguous(), dec.contiguous()
+        if _trains(self, enc, dec):
+            out = self.joint_net._modules["1"]
+            return _RNNTLossFn.apply(self, enc, dec, targets, enc_len, target_len, self.enc.weight, self.enc.bias, self.pred.weight,
+                                     self.pred.bias, out.weight, out.bias)
+        return eng.rnnt_loss(enc, dec, targets, enc_len, target_len)[0]
 
 
 class RNNTDecoder(Bound):

@@ -125,15 +125,52 @@ def align(head, encoded: Tensor, encoded_len: Tensor, targets: Tensor, target_le
     target_lengths = target_lengths.to(device=eng.device)
     if eng.head_type == 1:
         return eng.ctc_align(eng.ctc_log_probs(enc), encoded_len, targets, target_lengths)
+    y, x = _rnnt_inputs(eng, targets, target_lengths)
+    dec, _, _ = eng.rnnt_predict(x, None, None)
+    blank_lp, label_lp = eng.rnnt_align_scores(enc, dec, y)
+    return eng.rnnt_align(blank_lp, label_lp, encoded_len, target_lengths)
+
+
+def _rnnt_inputs(eng, targets: Tensor, target_lengths: Tensor) -> Tuple[Tensor, Tensor]:
+    """The RNN-T prologue of align and rnnt_loss: device targets [B, U] -> (y [B, U] i64 with every entry at or past
+    target_lengths[b] replaced by blank, x = cat[blank, y] [B, U+1], the prediction network's input)."""
     B, U = targets.shape
     blank = eng.num_classes - 1
     # the prediction network reads every step of its input: padding becomes blank so that it cannot poison the utterance
     used = torch.arange(U, device=eng.device)[None, :] < target_lengths.to(torch.int64)[:, None]
     y = torch.where(used, targets.to(torch.int64), torch.full_like(targets, blank, dtype=torch.int64))
     x = torch.cat([torch.full((B, 1), blank, dtype=torch.int64, device=eng.device), y], 1).contiguous()
-    dec, _, _ = eng.rnnt_predict(x, None, None)
-    blank_lp, label_lp = eng.rnnt_align_scores(enc, dec, y)
-    return eng.rnnt_align(blank_lp, label_lp, encoded_len, target_lengths)
+    return y, x
+
+
+_REDUCTIONS = ("none", "mean", "sum")
+
+
+def rnnt_loss(head, encoded: Tensor, encoded_len: Tensor, targets: Tensor, target_lengths: Tensor, reduction: str = "mean"
+              ) -> Tensor:
+    """The RNN-T loss -log p(y | x), summed over all alignments, without the [B, T, U+1, V+1] lattice (include/gigaam_b200.h,
+    gam_rnnt_loss).  encoded [B, d, T] (the encoder's output), encoded_len [B], targets [B, U] token ids in [0, V) (entries at or
+    past target_lengths[b] are ignored), target_lengths [B] -> loss [B] for reduction="none", else its batch mean or sum: the
+    values of torchaudio.functional.rnnt_loss(..., blank=V, reduction=...) on the lattice of head.joint.joint.  Differentiable:
+    the prediction network runs through head.decoder.predict and the joint through the fused loss, so gradients reach
+    decoder.embed / decoder.lstm, joint.enc / joint.pred / joint.joint_net.1 and `encoded` when it requires grad.  An
+    utterance with encoded_len 0 has loss +inf and no gradient.  No host synchronisation: the call can be captured in a CUDA
+    graph.  CTC heads raise NotImplementedError (use F.ctc_loss on model.head(encoded)); another reduction raises ValueError."""
+    if reduction not in _REDUCTIONS:
+        raise ValueError(f"rnnt_loss: reduction must be one of {_REDUCTIONS}, got {reduction!r}")
+    if getattr(head, "decoder", None) is None or getattr(head, "joint", None) is None:
+        raise NotImplementedError("rnnt_loss needs an RNN-T head; for a CTC model use torch.nn.functional.ctc_loss on the "
+                                  "log-probs of model.head(encoded), transposed to [T, B, V+1]")
+    eng = head._engine()
+    enc = _as_btd(encoded.to(device=eng.device, dtype=torch.float32))
+    targets = targets.to(device=eng.device)
+    target_lengths = target_lengths.to(device=eng.device)
+    y, x = _rnnt_inputs(eng, targets, target_lengths)
+    dec, _ = head.decoder.predict(x, None)
+    loss = head.joint._loss(enc, dec, y, encoded_len.to(device=eng.device), target_lengths)
+    if reduction == "mean":
+        return loss.mean()
+    return loss.sum() if reduction == "sum" else loss
 
 
 def spot(head, encoded: Tensor, encoded_len: Tensor, keywords: Tensor, keyword_len: Tensor, threshold: float, max_det: int

@@ -920,6 +920,59 @@ class Engine:
         _lib.check(self.lib, self.handle, rc, "gam_rnnt_align")
         return outs
 
+    # ------------------------------------------------------------------ fused RNN-T loss (rnnt_loss.cu)
+    def _loss_args(self, enc: Tensor, dec: Tensor, targets: Tensor, enc_len: Tensor, target_len: Tensor, what: str):
+        assert enc.is_cuda and dec.is_cuda and enc.dtype == dec.dtype == torch.float32
+        assert enc.is_contiguous() and dec.is_contiguous() and enc.dim() == dec.dim() == 3
+        if self.head_type != 2:
+            raise RuntimeError("model has no RNN-T head")
+        B, T, _ = enc.shape
+        U = targets.shape[1]
+        if dec.shape[0] != B or dec.shape[1] != U + 1 or targets.shape[0] != B:
+            raise ValueError(f"{what}: dec has shape {tuple(dec.shape)} and targets {tuple(targets.shape)}, expected ({B}, {U + 1}, H) "
+                             f"and ({B}, U)")
+        return B, T, U, self._i32(targets, self.device), self._i32(enc_len, self.device), self._i32(target_len, self.device)
+
+    def rnnt_loss(self, enc: Tensor, dec: Tensor, targets: Tensor, enc_len: Tensor, target_len: Tensor) -> Tuple[Tensor, Tensor]:
+        """enc [B, T, d], dec [B, U+1, pred_hidden] f32 contiguous, targets [B, U], enc_len [B], target_len [B] -> (loss [B] f32,
+        saved [3, B, T, U+1] f32: the per-node lse, e_blank and e_label that rnnt_loss_backward reads) (gam_rnnt_loss)."""
+        B, T, U, targets, enc_len, target_len = self._loss_args(enc, dec, targets, enc_len, target_len, "rnnt_loss")
+        nbytes = int(self.lib.gam_rnnt_loss_workspace_bytes(self.handle, B, T, U))
+        if nbytes < 0:
+            raise ValueError(f"rnnt_loss: unsupported sizes B={B}, T={T}, U={U} (limits: T <= the model's max_encoded_frames, "
+                             f"U <= 4096 tokens, joint_hidden <= 344)")
+        ws = self._scratch(nbytes, "rnnt_loss")
+        saved = self._empty(3, B, T, U + 1)
+        loss = self._empty(B)
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_rnnt_loss(self.handle, enc.data_ptr(), dec.data_ptr(), targets.data_ptr(), enc_len.data_ptr(),
+                                        target_len.data_ptr(), B, T, U, ws.data_ptr(), ws.numel(), saved.data_ptr(), loss.data_ptr(),
+                                        self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_rnnt_loss")
+        return loss, saved
+
+    def rnnt_loss_backward(self, enc: Tensor, dec: Tensor, targets: Tensor, enc_len: Tensor, target_len: Tensor, saved: Tensor,
+                           grad: Tensor, need_enc: bool, need_dec: bool, need_weights: bool):
+        """-> (d_enc [B, T, d], d_dec [B, U+1, H], dW_enc, db_enc, dW_pred, db_pred, dW_out, db_out); None where not needed.
+        grad: dL/dloss [B] f32 (gam_rnnt_loss_backward)."""
+        B, T, U, targets, enc_len, target_len = self._loss_args(enc, dec, targets, enc_len, target_len, "rnnt_loss_backward")
+        assert saved.is_contiguous() and tuple(saved.shape) == (3, B, T, U + 1)
+        grad = grad.to(device=self.device, dtype=torch.float32).contiguous()
+        d, H = enc.shape[2], dec.shape[2]
+        J, V1 = self.gam_config.joint_hidden, self.num_classes
+        outs = [self._empty(B, T, d) if need_enc else None, self._empty(B, U + 1, H) if need_dec else None]
+        if need_weights:
+            outs += [self._empty(J, d), self._empty(J), self._empty(J, H), self._empty(J), self._empty(V1, J), self._empty(V1)]
+        else:
+            outs += [None] * 6
+        ws = self._scratch(int(self.lib.gam_rnnt_loss_backward_workspace_bytes(self.handle, B, T, U)), "rnnt_loss_backward")
+        with torch.cuda.device(self.device):
+            rc = self.lib.gam_rnnt_loss_backward(self.handle, enc.data_ptr(), dec.data_ptr(), targets.data_ptr(), enc_len.data_ptr(),
+                                                 target_len.data_ptr(), B, T, U, saved.data_ptr(), grad.data_ptr(), ws.data_ptr(),
+                                                 ws.numel(), *[None if t is None else t.data_ptr() for t in outs], self._stream())
+        _lib.check(self.lib, self.handle, rc, "gam_rnnt_loss_backward")
+        return tuple(outs)
+
     # ------------------------------------------------------------------ backward passes of the head calls (head_grads.cu)
     def _empty(self, *shape) -> Tensor:
         return torch.empty(shape, dtype=torch.float32, device=self.device)

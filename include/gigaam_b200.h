@@ -552,6 +552,53 @@ int gam_rnnt_predict_backward(gam_handle* h, const int64_t* x, const float* h0, 
                               const float* w_ih, const float* w_hh, void* workspace, int64_t workspace_bytes, float* d_h0, float* d_c0,
                               float* d_embed, float* dW_ih, float* dW_hh, float* d_bias, void* stream);
 
+/* ---- fused RNN-T loss: -log p(y | x) summed over all alignments, and its gradient, without the [B, T, U+1, V+1] lattice.
+ * Notation as for gam_rnnt_align: nodes (t, u), t < T_b, u <= U_b; blank(t, u) and label(t, u) are stage 1's scores
+ * (gam_rnnt_align_scores, bit for bit) and lse(t, u) is the log-sum-exp of row joint(t, u) that both subtract.
+ *   alpha: gam_rnnt_align's forward recursion, the same lse2 operands in the same order; ll = alpha(T_b - 1, U_b) +
+ *     blank(T_b - 1, U_b) and loss[b] = -ll, so loss[b] == -log_likelihood[b] of gam_rnnt_align bit for bit
+ *     (= torchaudio rnnt_loss(..., blank=V, reduction="none") on the lattice).
+ *   beta: beta(T_b - 1, U_b) = blank(T_b - 1, U_b); beta(t, u) = lse2(blank(t, u) + beta(t + 1, u), label(t, u) + beta(t, u + 1)),
+ *     -inf outside the lattice.
+ *   edge occupancies: e_blank(t, u) = exp(alpha + blank + beta(t + 1, u) - ll), with beta(T_b, U_b) := 0 for the closing edge;
+ *     e_label(t, u) = exp(alpha + label + beta(t, u + 1) - ll) for u < U_b, else 0; gamma = e_blank + e_label, defined so (not
+ *     as exp(alpha + beta - ll)) that sum_v dz[v] = 0 holds as closely as fp32 allows.
+ *   per-node logit gradient, upstream g = grad_loss[b]:
+ *     dz[v] = g (exp(z_v - lse) gamma - [v = blank] e_blank - [v = y_{u+1}] e_label), z = W_o h + b_o, h = relu(E[b,t] + P[b,u]).
+ *   back through the joint: dhid = (dz W_o) * [E + P > 0] (relu's gradient at 0 is 0, as torch's); dW_out = sum dz h^T,
+ *     db_out = sum dz; dE[b, t] = sum_u dhid, dP[b, u] = sum_t dhid; then d_enc, d_dec and the projection gradients exactly as
+ *     gam_rnnt_joint_backward forms them from dE / dP.
+ * Edge cases: T_b = 0 gives loss +inf; an utterance whose loss is +inf (T_b = 0, or no path of finite score) contributes no
+ * gradient.  U_b = 0 is the blank-only path.  A NaN in any score the recursion reads (a target id outside [0, V) makes its label
+ * NaN) makes that utterance's loss NaN and puts NaN in every gradient it feeds; the other utterances' losses are untouched.
+ * Nodes outside an utterance's lattice, and target entries at or past target_len[b], are never read into a result.
+ *
+ * Sizes: enc [B, T, d_model], dec [B, U+1, pred_hidden] (gam_rnnt_predict over cat[blank, y]), targets [B, U] i32, enc_len [B],
+ * target_len [B] i32, all device.  Limits are gam_rnnt_align's (U <= 4096, T <= the handle's max_encoded_frames) plus
+ * joint_hidden <= 344 (a multiple of 4); the *_bytes functions return -1 beyond them or for a handle without an RNN-T head.
+ * Memory, N = B T (U+1) nodes, J = joint_hidden, fp32:
+ *   saved (kept between the calls): 12 N bytes = [lse | e_blank | e_label], each [B, T, U+1];
+ *   forward workspace: 12 N bytes (blank, label, alpha) + 4 (B T + B (U+1)) J bytes (the projections), 1 KiB-aligned pieces;
+ *   backward workspace: 4 J (2 B T + 2 B (U+1) + NS B T + ST B (U+1)) bytes + max(4 S V1 (J+1), the projection gradients'
+ *     partials), with NS = ceil((U+1) / 64) column strips, ST <= 64 frame ranges and S <= 64 node slices (rnnt_loss.cu's plan).
+ * No atomics and every sum in a fixed order: repeated calls give bit-identical gradients, and an utterance's loss is the same
+ * bits in any batch.  Stream-ordered, no host synchronisation, capturable in a CUDA graph.
+ *
+ * gam_rnnt_loss: -> saved (gam_rnnt_loss_saved_bytes), loss [B] f32.
+ * gam_rnnt_loss_backward: the forward's enc, dec, targets, lengths and saved, grad_loss [B] f32 -> d_enc [B, T, d_model],
+ *   d_dec [B, U+1, pred_hidden], dW_enc [J, d_model], db_enc [J], dW_pred [J, pred_hidden], db_pred [J], dW_out [V+1, J],
+ *   db_out [V+1].  Every output may be NULL (not computed), except that a weight gradient and its bias gradient go together. */
+int64_t gam_rnnt_loss_saved_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int64_t gam_rnnt_loss_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_rnnt_loss(gam_handle* h, const float* enc, const float* dec, const int32_t* targets, const int32_t* enc_len,
+                  const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, float* saved,
+                  float* loss, void* stream);
+int64_t gam_rnnt_loss_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U);
+int gam_rnnt_loss_backward(gam_handle* h, const float* enc, const float* dec, const int32_t* targets, const int32_t* enc_len,
+                           const int32_t* target_len, int32_t B, int32_t T, int32_t U, const float* saved, const float* grad_loss,
+                           void* workspace, int64_t workspace_bytes, float* d_enc, float* d_dec, float* dW_enc, float* db_enc,
+                           float* dW_pred, float* db_pred, float* dW_out, float* db_out, void* stream);
+
 /* Emotion head  <- gigaam/model.py:272-293 (GigaAMEmo.get_probs / forward_for_export): the mean of utterance b's encoder
  * frames, logits = W mean + b, probs = softmax(logits), fp32.
  *   enc: device f32 [B, T, d_model] (gam_encode's layout); enc_len: device i32 [B], or NULL = all T frames.
