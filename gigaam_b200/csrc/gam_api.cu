@@ -189,6 +189,31 @@ int fail(gam_handle* h, int code, const char* fmt, ...) {
   return code;
 }
 
+// A workspace carved into 1 KiB-aligned pieces; base == nullptr only sizes it.  `off` is the size with every piece rounded
+// up, `end` where the last piece ends.
+struct Carve {
+  uint8_t* base;
+  int64_t off = 0, end = 0;
+  template <typename T = float>
+  T* take(int64_t count) {
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    end = off + count * static_cast<int64_t>(sizeof(T));
+    off = align_up(end, 1024);
+    return p;
+  }
+};
+
+// The caller's workspace for a layout of `need` bytes: its base, rounded up to 1 KiB when `slack` (the layout's size query
+// adds 1 KiB for that); nullptr, with the error set, when it is NULL or smaller than need.
+uint8_t* workspace_base(gam_handle* h, const char* what, void* workspace, int64_t workspace_bytes, int64_t need, bool slack) {
+  if (workspace == nullptr || workspace_bytes < need) {
+    fail(h, -1, "%s: workspace too small: need %lld bytes, got %lld", what, (long long)need, (long long)workspace_bytes);
+    return nullptr;
+  }
+  const uintptr_t p = reinterpret_cast<uintptr_t>(workspace);
+  return reinterpret_cast<uint8_t*>(slack ? (p + 1023) & ~uintptr_t(1023) : p);
+}
+
 int sub_out_len(int len, int k, int pad) {
   // floor((len + 2p - k) / 2 + 1) with float semantics of the reference (encoder.py:86-90)
   float l = static_cast<float>(len);
@@ -659,6 +684,171 @@ int gam_encode(gam_handle* h, const float* mel, const int64_t* mel_len, int32_t 
   return 0;
 }
 
+// ---- the heads.  Each workspace has one layout, which both its size query (for the greedy decoders, the launcher's size
+// check) and its carve follow; and the joint's projections, shared by its forward, alignment, backward and loss entry points.
+namespace {
+// greedy decoding: CTC, the label of every row (and, scored, its l); RNN-T, the encoder projection of every row.  Returns where
+// the last piece ends, the least each launcher accepts; gam_decode_*workspace_bytes size for either head.
+struct DecodeWs { int* labels; float *lp, *encproj; };
+int64_t decode_layout(const gam_config& c, int64_t R, bool scored, uint8_t* base, DecodeWs* w) {
+  Carve cv{base};
+  w->labels = c.head == 1 ? cv.take<int>(R) : nullptr;
+  w->lp = c.head == 1 && scored ? cv.take(R) : nullptr;
+  w->encproj = c.head == 2 ? cv.take(R * c.joint_hidden) : nullptr;
+  return cv.end;
+}
+
+// the checks of gam_ctc_align and gam_rnnt_align(_scores): the head, and T and U within the short-form limits
+int align_args(gam_handle* h, const char* what, int head, int32_t B, int32_t T, int32_t U) {
+  if (h->cfg.head != head) return fail(h, -1, "%s: model has no %s head", what, head == 1 ? "CTC" : "RNN-T");
+  if (B <= 0 || T <= 0 || U < 0) return fail(h, -1, "%s: bad sizes (B=%d, T=%d, U=%d)", what, B, T, U);
+  if (T > h->max_t) return fail(h, -1, "%s: T=%d exceeds the handle's max_encoded_frames %d", what, T, h->max_t);
+  if (U > kAlignMaxTokens) return fail(h, -1, "%s: U=%d exceeds %d tokens per utterance", what, U, kAlignMaxTokens);
+  return 0;
+}
+
+// CTC alignment: the backpointers, and with gaps m[t] of every frame behind them
+struct CtcAlignWs { uint32_t* bp; float* m; };
+int64_t ctc_align_layout(int32_t B, int32_t T, int32_t U, bool gaps, uint8_t* base, CtcAlignWs* w) {
+  Carve cv{base};
+  w->bp = cv.take<uint32_t>(static_cast<int64_t>(B) * ctc_bp_words(T, U));
+  w->m = gaps ? cv.take(static_cast<int64_t>(B) * T) : nullptr;
+  return cv.off;
+}
+
+constexpr int64_t kProjMaxRows = 65535LL * 64;   // grid.y limit of the projection GEMMs (64 rows per block)
+
+// what every joint entry point needs: at most kProjMaxRows rows in each projection, pred_hidden and d_model multiples of 16
+bool proj_shapes_ok(const gam_config& c, int32_t B, int32_t T, int32_t U1) {
+  return static_cast<int64_t>(B) * T <= kProjMaxRows && static_cast<int64_t>(B) * U1 <= kProjMaxRows && c.pred_hidden % 16 == 0 &&
+         c.d_model % 16 == 0;
+}
+
+// ... and, for the forward joint kernels (hidden_tile), the hidden tile in shared memory
+int joint_args(gam_handle* h, const char* what, int32_t B, int32_t T, int32_t U1, bool hidden_tile) {
+  const int J = h->cfg.joint_hidden;
+  if (hidden_tile && (J % 4 != 0 || J > rnnt_joint_max_hidden()))
+    return fail(h, -1, "%s: needs joint_hidden %% 4 == 0 and <= %d (joint_hidden %d)", what, rnnt_joint_max_hidden(), J);
+  if (proj_shapes_ok(h->cfg, B, T, U1)) return 0;
+  return fail(h, -1, "%s: needs B*T and B*U <= %lld, pred_hidden %% 16 == 0 and d_model %% 16 == 0 (B=%d, T=%d, %d decoder rows, "
+              "pred_hidden %d)", what, (long long)kProjMaxRows, B, T, U1, h->cfg.pred_hidden);
+}
+
+// E = enc W_e^T + b_e [B*T, J] and P = dec W_p + b_p [B*U1, J], one launch each
+void rnnt_project(gam_handle* h, const float* enc, const float* dec, int32_t B, int32_t T, int32_t U1, float* E, float* P,
+                  int prof_class, cudaStream_t s) {
+  const gam_config& c = h->cfg;
+  { PROF(prof_class);
+    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, E, B * T, c.joint_hidden, c.d_model, s); }
+  { PROF(prof_class);
+    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, P, B * U1, c.joint_hidden, c.pred_hidden, s); }
+}
+
+// gam_rnnt_joint's and gam_rnnt_align_scores' workspace: the two projections
+struct ProjWs { float *E, *P; };
+int64_t proj_layout(const gam_config& c, int32_t B, int32_t T, int32_t U1, uint8_t* base, ProjWs* w) {
+  Carve cv{base};
+  w->E = cv.take(static_cast<int64_t>(B) * T * c.joint_hidden);
+  w->P = cv.take(static_cast<int64_t>(B) * U1 * c.joint_hidden);
+  return cv.off;
+}
+
+inline int64_t max3(int64_t a, int64_t b, int64_t c) { return a > b ? (a > c ? a : c) : (b > c ? b : c); }
+
+struct CtcBwdWs { float *dl, *part; };
+int64_t ctc_bwd_layout(const gam_config& c, int64_t R, uint8_t* base, CtcBwdWs* w) {
+  Carve cv{base};
+  w->dl = cv.take(R * c.num_classes);
+  w->part = cv.take(outer_sum_workspace_floats(R, c.num_classes, c.d_model, true));
+  return cv.off;
+}
+
+struct JointBwdWs { float *E, *P, *dl, *dhid, *dE, *dP, *part; };
+int64_t joint_bwd_layout(const gam_config& c, int32_t B, int32_t T, int32_t U, uint8_t* base, JointBwdWs* w) {
+  const int64_t J = c.joint_hidden, BT = static_cast<int64_t>(B) * T, BU = static_cast<int64_t>(B) * U, rows = BT * U;
+  Carve cv{base};
+  w->E = cv.take(BT * J);
+  w->P = cv.take(BU * J);
+  w->dl = cv.take(rows * c.num_classes);
+  w->dhid = cv.take(rows * J);
+  w->dE = cv.take(BT * J);
+  w->dP = cv.take(BU * J);
+  w->part = cv.take(max3(outer_sum_workspace_floats(rows, c.num_classes, J, true), outer_sum_workspace_floats(BT, J, c.d_model, true),
+                         outer_sum_workspace_floats(BU, J, c.pred_hidden, true)));
+  return cv.off;
+}
+
+struct PredBwdWs { float *dgates, *dcc, *dcls, *part; };
+int64_t pred_bwd_layout(const gam_config& c, int32_t B, int32_t U, uint8_t* base, PredBwdWs* w) {
+  const int64_t H = c.pred_hidden, BU = static_cast<int64_t>(B) * U;
+  Carve cv{base};
+  w->dgates = cv.take(BU * 4 * H);
+  w->dcc = cv.take(static_cast<int64_t>(B) * H);
+  w->dcls = cv.take(static_cast<int64_t>(c.num_classes) * 4 * H);
+  w->part = cv.take(max3(outer_sum_workspace_floats(BU, 4 * H, H, true), outer_sum_workspace_floats(c.num_classes, 4 * H, H, false), 0));
+  return cv.off;
+}
+
+// the gradients of the joint's inputs from dE [BT, J] and dP [BU, J], each optional (a weight gradient with its bias): dW_enc /
+// db_enc and dW_pred / db_pred (part: the outer sums' partials), d_enc = dE W_e and d_dec = dP W_p
+void joint_input_grads(gam_handle* h, const float* enc, const float* dec, int64_t BT, int64_t BU, const float* dE, const float* dP,
+                       float* part, float* d_enc, float* d_dec, float* dW_enc, float* db_enc, float* dW_pred, float* db_pred,
+                       cudaStream_t s) {
+  const gam_config& c = h->cfg;
+  const int J = c.joint_hidden;
+  if (dW_enc != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_outer_sum(dE, enc, BT, J, c.d_model, dW_enc, db_enc, part, s); }
+  if (dW_pred != nullptr) { PROF(PC_HEAD_BACKWARD);
+    launch_outer_sum(dP, dec, BU, J, c.pred_hidden, dW_pred, db_pred, part, s); }
+  if (d_enc != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_e [J, d]
+    launch_head_matmul(dE, h->w.rnnt_enc_w, c.d_model, 1, d_enc, BT, J, c.d_model, nullptr, nullptr, 1, 1, s); }
+  if (d_dec != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_p [J, H] = rnnt_wp_t^T
+    launch_head_matmul(dP, h->w.rnnt_wp_t, 1, J, d_dec, BU, J, c.pred_hidden, nullptr, nullptr, 1, 1, s); }
+}
+
+bool loss_sizes_ok(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
+  if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || T > h->max_t || U < 0 || U > kAlignMaxTokens) return false;
+  const int J = h->cfg.joint_hidden;
+  return J % 4 == 0 && J <= rnnt_joint_max_hidden() && J <= rnnt_loss_max_hidden() && proj_shapes_ok(h->cfg, B, T, U + 1);
+}
+
+int loss_args(gam_handle* h, const char* what, int32_t B, int32_t T, int32_t U) {
+  if (h->cfg.head != 2) return fail(h, -1, "%s: model has no RNN-T head", what);
+  if (loss_sizes_ok(h, B, T, U)) return 0;
+  return fail(h, -1, "%s: unsupported sizes (B=%d, T=%d, U=%d; T <= %d, U <= %d, joint_hidden %d <= %d)", what, B, T, U, h->max_t,
+              kAlignMaxTokens, h->cfg.joint_hidden, rnnt_loss_max_hidden());
+}
+
+struct LossFwdWs { float *E, *P, *blank, *label, *alpha; };
+int64_t loss_fwd_layout(const gam_config& c, int32_t B, int32_t T, int32_t U, uint8_t* base, LossFwdWs* w) {
+  const int64_t J = c.joint_hidden, BT = static_cast<int64_t>(B) * T, BU1 = static_cast<int64_t>(B) * (U + 1), N = BT * (U + 1);
+  Carve cv{base};
+  w->E = cv.take(BT * J);
+  w->P = cv.take(BU1 * J);
+  w->blank = cv.take(N);
+  w->label = cv.take(N);
+  w->alpha = cv.take(N);
+  return cv.off;
+}
+
+struct LossBwdWs { float *E, *P, *dE, *dP, *dE_part, *dP_part, *part; };
+int64_t loss_bwd_layout(const gam_config& c, int32_t B, int32_t T, int32_t U, uint8_t* base, LossBwdWs* w) {
+  const RnntLossPlan p = rnnt_loss_plan(B, T, U, c.num_classes);
+  const int64_t J = c.joint_hidden, BT = static_cast<int64_t>(B) * T, BU1 = static_cast<int64_t>(B) * (U + 1);
+  Carve cv{base};
+  w->E = cv.take(BT * J);
+  w->P = cv.take(BU1 * J);
+  w->dE = cv.take(BT * J);
+  w->dP = cv.take(BU1 * J);
+  w->dE_part = cv.take(p.NS * BT * J);
+  w->dP_part = cv.take(p.ST * BU1 * J);
+  w->part = cv.take(max3(p.S > 1 ? static_cast<int64_t>(p.S) * c.num_classes * (J + 1) : 0,
+                         outer_sum_workspace_floats(BT, static_cast<int>(J), c.d_model, true),
+                         outer_sum_workspace_floats(BU1, static_cast<int>(J), c.pred_hidden, true)));
+  return cv.off;
+}
+}  // namespace
+
 // the greedy decoders' launches, after each entry point's own checks: labels and (scored) l of every row in the workspace,
 // then the collapse (io: a fresh or a resume call, kernels.h)
 static int ctc_greedy_impl(gam_handle* h, const char* what, const float* enc, int32_t B, int32_t T, void* workspace,
@@ -666,12 +856,12 @@ static int ctc_greedy_impl(gam_handle* h, const char* what, const float* enc, in
   const gam_config& c = h->cfg;
   const int64_t R = static_cast<int64_t>(B) * T;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int* labels = static_cast<int*>(workspace);
-  float* lp = io.token_logp ? reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + align_up(R * 4, 1024)) : nullptr;
+  DecodeWs w;
+  decode_layout(c, R, io.token_logp != nullptr, static_cast<uint8_t*>(workspace), &w);
   { PROF(PC_CTC_ARGMAX);
-    launch_ctc_argmax(enc, h->w.ctc_w, h->w.ctc_b, labels, lp, static_cast<int>(R), c.d_model, c.num_classes, s); }
+    launch_ctc_argmax(enc, h->w.ctc_w, h->w.ctc_b, w.labels, w.lp, static_cast<int>(R), c.d_model, c.num_classes, s); }
   { PROF(PC_CTC_COLLAPSE);
-    launch_ctc_collapse(labels, lp, B, T, c.num_classes - 1, io, s); }
+    launch_ctc_collapse(w.labels, w.lp, B, T, c.num_classes - 1, io, s); }
   GAM_CHECK_LAUNCH(h, what);
   return 0;
 }
@@ -682,11 +872,12 @@ static int rnnt_greedy_impl(gam_handle* h, const char* what, const float* enc, i
   const gam_config& c = h->cfg;
   const int64_t R = static_cast<int64_t>(B) * T;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  float* encproj = static_cast<float*>(workspace);
+  DecodeWs w;
+  decode_layout(c, R, false, static_cast<uint8_t*>(workspace), &w);
   { PROF(PC_RNNT_ENCPROJ);   // a row's projection does not depend on the others, so a resume call projects every row too
-    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, encproj, static_cast<int>(R), c.joint_hidden, c.d_model, s); }
+    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, w.encproj, static_cast<int>(R), c.joint_hidden, c.d_model, s); }
   PROF(PC_RNNT_GREEDY);
-  const int rc = launch_rnnt_greedy(encproj, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h->w.rnnt_wp_t, h->w.rnnt_bp, h->w.rnnt_wo,
+  const int rc = launch_rnnt_greedy(w.encproj, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h->w.rnnt_wp_t, h->w.rnnt_bp, h->w.rnnt_wo,
                                     h->w.rnnt_bo, B, T, c.pred_hidden, c.num_classes, c.num_classes - 1, c.max_symbols, io, nullptr, s);
   if (rc > 0)
     return fail(h, -1, "rnnt: the greedy kernel is specialised for pred_hidden = joint_hidden = 320 and needs 16-CTA clusters "
@@ -712,8 +903,9 @@ int gam_ctc_greedy(gam_handle* h, const float* enc, const int32_t* enc_len, int3
   if (c.head != 1) return fail(h, -1, "model has no CTC head");
   if (max_out < T) return fail(h, -1, "max_out (%d) must be >= T (%d)", max_out, T);
   if (max_out != T) return fail(h, -1, "ids/frames row pitch must equal T for the CTC path");
-  const int64_t R = static_cast<int64_t>(B) * T;
-  if (workspace_bytes < R * 4) return fail(h, -1, "workspace too small for CTC labels");
+  DecodeWs w;
+  if (workspace_bytes < decode_layout(c, static_cast<int64_t>(B) * T, false, nullptr, &w))
+    return fail(h, -1, "workspace too small for CTC labels");
   return ctc_greedy_impl(h, "ctc_greedy", enc, B, T, workspace,
                          fresh_io(enc_len, ids, frames, counts, max_out, nullptr, nullptr, nullptr), stream);
 }
@@ -726,8 +918,9 @@ int gam_ctc_greedy_scored(gam_handle* h, const float* enc, const int32_t* enc_le
   if (max_out < T) return fail(h, -1, "max_out (%d) must be >= T (%d)", max_out, T);
   if (max_out != T) return fail(h, -1, "ids/frames row pitch must equal T for the CTC path");
   if (!token_logp || !path_logp || !path_rows) return fail(h, -1, "ctc_greedy_scored: token_logp, path_logp and path_rows are required");
-  const int64_t R = static_cast<int64_t>(B) * T;
-  if (workspace_bytes < align_up(R * 4, 1024) + R * 4) return fail(h, -1, "workspace too small for CTC labels and scores");
+  DecodeWs w;
+  if (workspace_bytes < decode_layout(c, static_cast<int64_t>(B) * T, true, nullptr, &w))
+    return fail(h, -1, "workspace too small for CTC labels and scores");
   return ctc_greedy_impl(h, "ctc_greedy_scored", enc, B, T, workspace,
                          fresh_io(enc_len, ids, frames, counts, max_out, token_logp, path_logp, path_rows), stream);
 }
@@ -736,7 +929,8 @@ static int rnnt_greedy_args(gam_handle* h, int32_t B, int32_t T, int64_t workspa
   const gam_config& c = h->cfg;
   if (c.head != 2) return fail(h, -1, "model has no RNN-T head");
   if (c.pred_hidden != c.joint_hidden) return fail(h, -1, "pred_hidden != joint_hidden is not supported");
-  if (workspace_bytes < static_cast<int64_t>(B) * T * c.joint_hidden * 4)
+  DecodeWs w;
+  if (workspace_bytes < decode_layout(c, static_cast<int64_t>(B) * T, false, nullptr, &w))
     return fail(h, -1, "workspace too small for the RNN-T encoder projection");
   return 0;
 }
@@ -788,10 +982,7 @@ static int resume_args(gam_handle* h, const char* what, int head, const float* e
     return fail(h, -1, "%s: enc, lo, hi, frame_base, state, ids, frames and counts are required", what);
   if (token_logp && (!path_logp || !path_rows || !frame_logp || !frame_rows || frame_pitch < 1))
     return fail(h, -1, "%s: a scored call needs path_logp, path_rows, frame_logp, frame_rows and frame_pitch >= 1", what);
-  const int64_t need = gam_decode_resume_workspace_bytes(h, B, T);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "%s: workspace too small: need %lld bytes, got %lld", what, (long long)need, (long long)workspace_bytes);
-  return 0;
+  return workspace_base(h, what, workspace, workspace_bytes, gam_decode_resume_workspace_bytes(h, B, T), false) ? 0 : -1;
 }
 
 // a resume call: stream b continues from its DecodeState over [lo[b], hi[b])
@@ -843,10 +1034,11 @@ int gam_ctc_log_probs(gam_handle* h, const float* enc, int32_t B, int32_t T, flo
   return 0;
 }
 
+// ---- the RNN-T joint lattice
 int64_t gam_rnnt_joint_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
   if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || U <= 0) return -1;
-  const int64_t J = h->cfg.joint_hidden;
-  return align_up(static_cast<int64_t>(B) * T * J * 4, 1024) + align_up(static_cast<int64_t>(B) * U * J * 4, 1024) + 1024;
+  ProjWs w;
+  return proj_layout(h->cfg, B, T, U, nullptr, &w) + 1024;
 }
 
 int gam_rnnt_joint(gam_handle* h, const float* enc, const float* dec, int32_t B, int32_t T, int32_t U, void* workspace,
@@ -854,27 +1046,16 @@ int gam_rnnt_joint(gam_handle* h, const float* enc, const float* dec, int32_t B,
   const gam_config& c = h->cfg;
   if (c.head != 2) return fail(h, -1, "rnnt_joint: model has no RNN-T head");
   if (B <= 0 || T <= 0 || U <= 0) return fail(h, -1, "rnnt_joint: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
-  constexpr int64_t kMaxProjRows = 65535LL * 64;   // grid.y limit of the projection GEMMs (64 rows per block)
-  if (static_cast<int64_t>(B) * T > kMaxProjRows || static_cast<int64_t>(B) * U > kMaxProjRows)
-    return fail(h, -1, "rnnt_joint: B*T and B*U must be <= %lld (B=%d, T=%d, U=%d)", (long long)kMaxProjRows, B, T, U);
-  const int J = c.joint_hidden;
-  if (J % 4 != 0 || J > rnnt_joint_max_hidden() || c.pred_hidden % 16 != 0 || c.d_model % 16 != 0)
-    return fail(h, -1, "rnnt_joint: needs joint_hidden %% 4 == 0 and <= %d, pred_hidden %% 16 == 0 (joint_hidden %d, pred_hidden %d)",
-                rnnt_joint_max_hidden(), J, c.pred_hidden);
-  const int64_t need = gam_rnnt_joint_workspace_bytes(h, B, T, U);
-  if (workspace_bytes < need)
-    return fail(h, -1, "rnnt_joint: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
-  uint8_t* ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
-  float* E = reinterpret_cast<float*>(ws);
-  float* P = reinterpret_cast<float*>(ws + align_up(static_cast<int64_t>(B) * T * J * 4, 1024));
+  if (joint_args(h, "rnnt_joint", B, T, U, true) != 0) return -1;
+  uint8_t* ws = workspace_base(h, "rnnt_joint", workspace, workspace_bytes, gam_rnnt_joint_workspace_bytes(h, B, T, U), true);
+  if (!ws) return -1;
+  ProjWs w;
+  proj_layout(c, B, T, U, ws, &w);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int rc = 0;
+  rnnt_project(h, enc, dec, B, T, U, w.E, w.P, PC_RNNT_JOINT, s);
+  int rc;
   { PROF(PC_RNNT_JOINT);
-    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, E, B * T, J, c.d_model, s); }
-  { PROF(PC_RNNT_JOINT);
-    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, P, B * U, J, c.pred_hidden, s); }
-  { PROF(PC_RNNT_JOINT);
-    rc = launch_rnnt_joint(E, P, h->w.rnnt_wo, h->w.rnnt_bo, out, B, T, U, J, c.num_classes, s); }
+    rc = launch_rnnt_joint(w.E, w.P, h->w.rnnt_wo, h->w.rnnt_bo, out, B, T, U, c.joint_hidden, c.num_classes, s); }
   if (rc != 0) return fail(h, -4, "rnnt_joint: lattice launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "rnnt_joint");
   return 0;
@@ -883,28 +1064,27 @@ int gam_rnnt_joint(gam_handle* h, const float* enc, const float* dec, int32_t B,
 // ---- alignment of known transcripts (csrc/align.cu; stage 1 of RNN-T: the gathered joint of heads.cu)
 int64_t gam_ctc_align_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
   if (!h || h->cfg.head != 1 || B <= 0 || T <= 0 || T > h->max_t || U < 0 || U > kAlignMaxTokens) return -1;
-  return align_up(static_cast<int64_t>(B) * ctc_bp_words(T, U) * 4, 1024);
+  CtcAlignWs w;
+  return ctc_align_layout(B, T, U, false, nullptr, &w);
 }
 
 int gam_ctc_align(gam_handle* h, const float* log_probs, const int32_t* enc_len, const int32_t* targets, const int32_t* target_len,
                   int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
                   float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream) {
   const gam_config& c = h->cfg;
-  if (c.head != 1) return fail(h, -1, "ctc_align: model has no CTC head");
-  if (B <= 0 || T <= 0 || U < 0) return fail(h, -1, "ctc_align: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
-  if (T > h->max_t) return fail(h, -1, "ctc_align: T=%d exceeds the handle's max_encoded_frames %d", T, h->max_t);
-  if (U > kAlignMaxTokens) return fail(h, -1, "ctc_align: U=%d exceeds %d tokens per utterance", U, kAlignMaxTokens);
+  if (align_args(h, "ctc_align", 1, B, T, U) != 0) return -1;
   if (!log_probs || !enc_len || !target_len || (U > 0 && (!targets || !frames || !token_logp)) || !viterbi_logp || !log_likelihood ||
       !path_rows)
     return fail(h, -1, "ctc_align: a required pointer is NULL");
-  const int64_t need = gam_ctc_align_workspace_bytes(h, B, T, U);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "ctc_align: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  uint8_t* ws = workspace_base(h, "ctc_align", workspace, workspace_bytes, gam_ctc_align_workspace_bytes(h, B, T, U), false);
+  if (!ws) return -1;
+  CtcAlignWs w;
+  ctc_align_layout(B, T, U, false, ws, &w);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc;
   { PROF(PC_ALIGN);
-    rc = launch_ctc_align(log_probs, enc_len, targets, target_len, B, T, U, c.num_classes, static_cast<uint32_t*>(workspace), frames,
-                          token_logp, viterbi_logp, log_likelihood, path_rows, s); }
+    rc = launch_ctc_align(log_probs, enc_len, targets, target_len, B, T, U, c.num_classes, w.bp, frames, token_logp, viterbi_logp,
+                          log_likelihood, path_rows, s); }
   if (rc != 0) return fail(h, -4, "ctc_align: launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "ctc_align");
   return 0;
@@ -912,12 +1092,14 @@ int gam_ctc_align(gam_handle* h, const float* log_probs, const int32_t* enc_len,
 
 int64_t gam_ctc_align_long_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
   if (!h || h->cfg.head != 1 || B <= 0 || T <= 0 || U < 0 || U > kAlignLongMaxTokens) return -1;
-  return align_up(static_cast<int64_t>(B) * ctc_bp_words(T, U) * 4, 1024);
+  CtcAlignWs w;
+  return ctc_align_layout(B, T, U, false, nullptr, &w);
 }
 
 int64_t gam_ctc_align_long_gaps_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
-  const int64_t bp = gam_ctc_align_long_workspace_bytes(h, B, T, U);
-  return bp < 0 ? -1 : bp + align_up(static_cast<int64_t>(B) * T * 4, 1024);
+  if (gam_ctc_align_long_workspace_bytes(h, B, T, U) < 0) return -1;
+  CtcAlignWs w;
+  return ctc_align_layout(B, T, U, true, nullptr, &w);
 }
 
 // gaps: NULL for gam_ctc_align_long; otherwise line_edges, log_theta and the three outputs, with m still to be placed in the
@@ -945,18 +1127,18 @@ static int ctc_align_long_run(gam_handle* h, const char* what, const float* log_
         return fail(h, -1, "%s: log_psi=%g must be <= 0 (a threshold in (0, 1]) or -inf", what, gaps->log_psi);
     }
   }
-  const int64_t bp_bytes = gam_ctc_align_long_workspace_bytes(h, B, T, U);
-  const int64_t need = gaps ? gam_ctc_align_long_gaps_workspace_bytes(h, B, T, U) : bp_bytes;
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "%s: workspace too small: need %lld bytes, got %lld", what, (long long)need, (long long)workspace_bytes);
-  if (gaps) gaps->m = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + bp_bytes);
+  const int64_t need = gaps ? gam_ctc_align_long_gaps_workspace_bytes(h, B, T, U) : gam_ctc_align_long_workspace_bytes(h, B, T, U);
+  uint8_t* ws = workspace_base(h, what, workspace, workspace_bytes, need, false);
+  if (!ws) return -1;
+  CtcAlignWs w;
+  ctc_align_layout(B, T, U, gaps != nullptr, ws, &w);
+  if (gaps) gaps->m = w.m;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc;
   { PROF(PC_ALIGN);
     if (gaps) h->launches += 1;   // the pre-pass
-    rc = launch_ctc_align_long(log_probs, enc_len, targets, target_len, B, T, U, c.num_classes, cluster_ctas,
-                               static_cast<uint32_t*>(workspace), frames, token_logp, viterbi_logp, log_likelihood, path_rows, plan, gaps,
-                               s); }
+    rc = launch_ctc_align_long(log_probs, enc_len, targets, target_len, B, T, U, c.num_classes, cluster_ctas, w.bp, frames, token_logp,
+                               viterbi_logp, log_likelihood, path_rows, plan, gaps, s); }
   if (rc == 2) return fail(h, -1, "%s: %d CTAs leave a CTA without states at U=%d", what, cluster_ctas, U);
   if (rc == 1) return fail(h, -1, "%s: no cluster of <= %d CTAs holds U=%d (forced %d)", what, kAlignLongMaxCtas, U, cluster_ctas);
   if (rc != 0) return fail(h, -4, "%s: launch rejected (rc=%d): %s", what, rc, cudaGetErrorString(cudaGetLastError()));
@@ -1033,16 +1215,22 @@ int gam_test_ctc_align_long_skips(gam_handle* h, const float* log_probs, const i
 }
 
 // ---- keyword spotting (csrc/spot.cu)
-static int ctc_spot_run(gam_handle* h, const char* what, const float* log_probs, const SpotResume& io, int32_t B, int32_t T,
-                        const int32_t* keywords, const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det,
-                        int32_t* det_start, int32_t* det_end, float* det_score, int32_t* det_count, int32_t warps, void* stream) {
-  const gam_config& c = h->cfg;
-  if (c.head != 1) return fail(h, -1, "%s: model has no CTC head", what);
+// the checks gam_ctc_spot* and gam_ctc_bias share
+static int spot_args(gam_handle* h, const char* what, int32_t B, int32_t T, int32_t K, int32_t Umax, float threshold, int32_t max_det) {
+  if (h->cfg.head != 1) return fail(h, -1, "%s: model has no CTC head", what);
   if (B <= 0 || B > 65535 || T <= 0) return fail(h, -1, "%s: bad sizes (B=%d, T=%d; B <= 65535)", what, B, T);
   if (K < 1) return fail(h, -1, "%s: K=%d: at least one keyword is needed", what, K);
   if (Umax < 1 || Umax > kSpotMaxTokens) return fail(h, -1, "%s: Umax=%d outside [1, %d] tokens per keyword", what, Umax, kSpotMaxTokens);
   if (!(threshold > 0.f && threshold <= 1.f)) return fail(h, -1, "%s: threshold %g outside (0, 1]", what, static_cast<double>(threshold));
   if (max_det < 1) return fail(h, -1, "%s: max_det=%d must be >= 1", what, max_det);
+  return 0;
+}
+
+static int ctc_spot_run(gam_handle* h, const char* what, const float* log_probs, const SpotResume& io, int32_t B, int32_t T,
+                        const int32_t* keywords, const int32_t* keyword_len, int32_t K, int32_t Umax, float threshold, int32_t max_det,
+                        int32_t* det_start, int32_t* det_end, float* det_score, int32_t* det_count, int32_t warps, void* stream) {
+  const gam_config& c = h->cfg;
+  if (spot_args(h, what, B, T, K, Umax, threshold, max_det) != 0) return -1;
   if (!log_probs || !io.hi || !keywords || !keyword_len || !det_start || !det_end || !det_score || !det_count)
     return fail(h, -1, "%s: a required pointer is NULL", what);
   const float log_theta = static_cast<float>(std::log(static_cast<double>(threshold)));   // correctly rounded to fp32
@@ -1127,12 +1315,7 @@ int gam_ctc_bias(gam_handle* h, const float* log_probs, const int32_t* enc_len, 
                  int32_t* out_ids, int32_t* out_frames, int32_t* out_counts, int32_t* out_source, float* out_token_logp,
                  float* out_path_logp, void* stream) {
   const gam_config& c = h->cfg;
-  if (c.head != 1) return fail(h, -1, "ctc_bias: model has no CTC head");
-  if (B <= 0 || B > 65535 || T <= 0) return fail(h, -1, "ctc_bias: bad sizes (B=%d, T=%d; B <= 65535)", B, T);
-  if (K < 1) return fail(h, -1, "ctc_bias: K=%d: at least one keyword is needed", K);
-  if (Umax < 1 || Umax > kSpotMaxTokens) return fail(h, -1, "ctc_bias: Umax=%d outside [1, %d] tokens per keyword", Umax, kSpotMaxTokens);
-  if (!(threshold > 0.f && threshold <= 1.f)) return fail(h, -1, "ctc_bias: threshold %g outside (0, 1]", static_cast<double>(threshold));
-  if (max_det < 1) return fail(h, -1, "ctc_bias: max_det=%d must be >= 1", max_det);
+  if (spot_args(h, "ctc_bias", B, T, K, Umax, threshold, max_det) != 0) return -1;
   if (max_out < T) return fail(h, -1, "ctc_bias: max_out=%d is less than T=%d", max_out, T);
   if (!token_flags || V != c.num_classes - 1)
     return fail(h, -1, "ctc_bias: the token flag table is missing or has %d entries, not %d", V, c.num_classes - 1);
@@ -1147,8 +1330,8 @@ int gam_ctc_bias(gam_handle* h, const float* log_probs, const int32_t* enc_len, 
     return fail(h, -1, "ctc_bias: a frame of %d classes does not fit in shared memory", c.num_classes);
   const int64_t need = gam_ctc_bias_workspace_bytes(h, B, T, K, max_det);
   if (need < 0) return fail(h, -1, "ctc_bias: K=%d x max_det=%d candidates are too many", K, max_det);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "ctc_bias: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  int32_t* ws = reinterpret_cast<int32_t*>(workspace_base(h, "ctc_bias", workspace, workspace_bytes, need, false));
+  if (!ws) return -1;
   BiasArgs a{};
   a.log_probs = log_probs;
   a.enc_len = enc_len;
@@ -1183,7 +1366,7 @@ int gam_ctc_bias(gam_handle* h, const float* log_probs, const int32_t* enc_len, 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   for (int stage = 0; stage < 3; ++stage) {
     PROF(PC_ALIGN);
-    launch_ctc_bias(a, static_cast<int32_t*>(workspace), stage, s);
+    launch_ctc_bias(a, ws, stage, s);
   }
   GAM_CHECK_LAUNCH(h, "ctc_bias");
   return 0;
@@ -1197,34 +1380,21 @@ int64_t gam_rnnt_align_scores_workspace_bytes(const gam_handle* h, int32_t B, in
 int gam_rnnt_align_scores(gam_handle* h, const float* enc, const float* dec, const int32_t* targets, int32_t B, int32_t T, int32_t U,
                           void* workspace, int64_t workspace_bytes, float* blank, float* label, void* stream) {
   const gam_config& c = h->cfg;
-  if (c.head != 2) return fail(h, -1, "rnnt_align_scores: model has no RNN-T head");
-  if (B <= 0 || T <= 0 || U < 0) return fail(h, -1, "rnnt_align_scores: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
-  if (T > h->max_t) return fail(h, -1, "rnnt_align_scores: T=%d exceeds the handle's max_encoded_frames %d", T, h->max_t);
-  if (U > kAlignMaxTokens) return fail(h, -1, "rnnt_align_scores: U=%d exceeds %d tokens per utterance", U, kAlignMaxTokens);
+  if (align_args(h, "rnnt_align_scores", 2, B, T, U) != 0) return -1;
   const int U1 = U + 1;
-  constexpr int64_t kMaxProjRows = 65535LL * 64;   // grid.y limit of the projection GEMMs (64 rows per block)
-  if (static_cast<int64_t>(B) * T > kMaxProjRows || static_cast<int64_t>(B) * U1 > kMaxProjRows)
-    return fail(h, -1, "rnnt_align_scores: B*T and B*(U+1) must be <= %lld (B=%d, T=%d, U=%d)", (long long)kMaxProjRows, B, T, U);
-  const int J = c.joint_hidden;
-  if (J % 4 != 0 || J > rnnt_joint_max_hidden() || c.pred_hidden % 16 != 0 || c.d_model % 16 != 0)
-    return fail(h, -1, "rnnt_align_scores: needs joint_hidden %% 4 == 0 and <= %d, pred_hidden %% 16 == 0 (joint_hidden %d, pred_hidden %d)",
-                rnnt_joint_max_hidden(), J, c.pred_hidden);
+  if (joint_args(h, "rnnt_align_scores", B, T, U1, true) != 0) return -1;
   if (!enc || !dec || (U > 0 && !targets) || !blank || !label) return fail(h, -1, "rnnt_align_scores: a required pointer is NULL");
-  const int64_t need = gam_rnnt_align_scores_workspace_bytes(h, B, T, U);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "rnnt_align_scores: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
-  // the projections of gam_rnnt_joint, carved the same way
-  uint8_t* ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
-  float* E = reinterpret_cast<float*>(ws);
-  float* P = reinterpret_cast<float*>(ws + align_up(static_cast<int64_t>(B) * T * J * 4, 1024));
+  uint8_t* ws = workspace_base(h, "rnnt_align_scores", workspace, workspace_bytes, gam_rnnt_align_scores_workspace_bytes(h, B, T, U),
+                               true);
+  if (!ws) return -1;
+  ProjWs w;
+  proj_layout(c, B, T, U1, ws, &w);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int rc = 0;
+  rnnt_project(h, enc, dec, B, T, U1, w.E, w.P, PC_RNNT_JOINT, s);
+  int rc;
   { PROF(PC_RNNT_JOINT);
-    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, E, B * T, J, c.d_model, s); }
-  { PROF(PC_RNNT_JOINT);
-    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, P, B * U1, J, c.pred_hidden, s); }
-  { PROF(PC_RNNT_JOINT);
-    rc = launch_rnnt_joint_gather(E, P, h->w.rnnt_wo, h->w.rnnt_bo, targets, blank, label, nullptr, B, T, U1, J, c.num_classes, s); }
+    rc = launch_rnnt_joint_gather(w.E, w.P, h->w.rnnt_wo, h->w.rnnt_bo, targets, blank, label, nullptr, B, T, U1, c.joint_hidden,
+                                  c.num_classes, s); }
   if (rc != 0) return fail(h, -4, "rnnt_align_scores: launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "rnnt_align_scores");
   return 0;
@@ -1238,118 +1408,59 @@ int64_t gam_rnnt_align_workspace_bytes(const gam_handle* h, int32_t B, int32_t T
 int gam_rnnt_align(gam_handle* h, const float* blank, const float* label, const int32_t* enc_len, const int32_t* target_len, int32_t B,
                    int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, int32_t* frames, float* token_logp,
                    float* viterbi_logp, float* log_likelihood, int32_t* path_rows, void* stream) {
-  if (h->cfg.head != 2) return fail(h, -1, "rnnt_align: model has no RNN-T head");
-  if (B <= 0 || T <= 0 || U < 0) return fail(h, -1, "rnnt_align: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
-  if (T > h->max_t) return fail(h, -1, "rnnt_align: T=%d exceeds the handle's max_encoded_frames %d", T, h->max_t);
-  if (U > kAlignMaxTokens) return fail(h, -1, "rnnt_align: U=%d exceeds %d tokens per utterance", U, kAlignMaxTokens);
+  if (align_args(h, "rnnt_align", 2, B, T, U) != 0) return -1;
   if (!blank || !label || !enc_len || !target_len || (U > 0 && (!frames || !token_logp)) || !viterbi_logp || !log_likelihood ||
       !path_rows)
     return fail(h, -1, "rnnt_align: a required pointer is NULL");
-  const int64_t need = gam_rnnt_align_workspace_bytes(h, B, T, U);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "rnnt_align: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  uint8_t* ws = workspace_base(h, "rnnt_align", workspace, workspace_bytes, gam_rnnt_align_workspace_bytes(h, B, T, U), false);
+  if (!ws) return -1;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc;
-  { PROF(PC_ALIGN);
-    rc = launch_rnnt_align(blank, label, enc_len, target_len, B, T, U, static_cast<uint32_t*>(workspace), frames, token_logp,
+  { PROF(PC_ALIGN);   // one piece: the backpointers
+    rc = launch_rnnt_align(blank, label, enc_len, target_len, B, T, U, reinterpret_cast<uint32_t*>(ws), frames, token_logp,
                            viterbi_logp, log_likelihood, path_rows, s); }
   if (rc != 0) return fail(h, -4, "rnnt_align: launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, "rnnt_align");
   return 0;
 }
 
-int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g, float* h1,
-                     float* c1, void* stream) {
+// gam_rnnt_predict's U LSTM steps, one launch each.  Step u reads h from g[:, u-1] (steps are separate launches, so every block
+// of step u sees all of step u-1).  c_seq == nullptr: the cell is updated in place in c1; otherwise step u's cell goes to
+// c_seq[u] and the last one is copied to c1.
+static int rnnt_predict_run(gam_handle* h, const char* what, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U,
+                            float* g, float* h1, float* c1, float* c_seq, void* stream) {
   const gam_config& c = h->cfg;
-  if (c.head != 2) return fail(h, -1, "rnnt_predict: model has no RNN-T head");
-  if (B <= 0 || U <= 0) return fail(h, -1, "rnnt_predict: bad sizes (B=%d, U=%d)", B, U);
-  if (x == nullptr && U != 1) return fail(h, -1, "rnnt_predict: without labels the step count U must be 1 (got %d)", U);
-  if (c.pred_hidden > 1024) return fail(h, -1, "rnnt_predict: pred_hidden %d exceeds 1024", c.pred_hidden);
+  if (c.head != 2) return fail(h, -1, "%s: model has no RNN-T head", what);
+  if (B <= 0 || U <= 0) return fail(h, -1, "%s: bad sizes (B=%d, U=%d)", what, B, U);
+  if (x == nullptr && U != 1) return fail(h, -1, "%s: without labels the step count U must be 1 (got %d)", what, U);
+  if (c.pred_hidden > 1024) return fail(h, -1, "%s: pred_hidden %d exceeds 1024", what, c.pred_hidden);
   const int H = c.pred_hidden;
+  const int64_t BH = static_cast<int64_t>(B) * H;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   for (int u = 0; u < U; ++u) {
-    // step u reads h from g[:, u-1] (steps are separate launches, so every block of step u sees all of step u-1) and
-    // updates c1 in place
     const float* h_in = u == 0 ? h0 : g + static_cast<int64_t>(u - 1) * H;
     const int64_t pitch = u == 0 ? H : static_cast<int64_t>(U) * H;
+    const float* c_in = u == 0 ? c0 : c_seq ? c_seq + (u - 1) * BH : c1;
     PROF(PC_RNNT_PREDICT);
-    launch_lstm_step(x, U, u, c.num_classes, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h_in, pitch, u == 0 ? c0 : c1, g,
-                     u == U - 1 ? h1 : nullptr, c1, B, H, s);
+    launch_lstm_step(x, U, u, c.num_classes, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h_in, pitch, c_in, g, u == U - 1 ? h1 : nullptr,
+                     c_seq ? c_seq + u * BH : c1, B, H, s);
   }
-  GAM_CHECK_LAUNCH(h, "rnnt_predict");
+  if (c_seq) cudaMemcpyAsync(c1, c_seq + (U - 1) * BH, BH * 4, cudaMemcpyDeviceToDevice, s);
+  GAM_CHECK_LAUNCH(h, what);
   return 0;
+}
+
+int gam_rnnt_predict(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g, float* h1,
+                     float* c1, void* stream) {
+  return rnnt_predict_run(h, "rnnt_predict", x, h0, c0, B, U, g, h1, c1, nullptr, stream);
 }
 
 int gam_rnnt_predict_train(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, float* g,
                            float* h1, float* c1, float* c_seq, void* stream) {
-  const gam_config& c = h->cfg;
-  if (c.head != 2) return fail(h, -1, "rnnt_predict_train: model has no RNN-T head");
-  if (B <= 0 || U <= 0) return fail(h, -1, "rnnt_predict_train: bad sizes (B=%d, U=%d)", B, U);
-  if (x == nullptr && U != 1) return fail(h, -1, "rnnt_predict_train: without labels the step count U must be 1 (got %d)", U);
-  if (c.pred_hidden > 1024) return fail(h, -1, "rnnt_predict_train: pred_hidden %d exceeds 1024", c.pred_hidden);
-  const int H = c.pred_hidden;
-  const int64_t BH = static_cast<int64_t>(B) * H;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  for (int u = 0; u < U; ++u) {   // gam_rnnt_predict's steps, with the cell of every step kept in c_seq[u]
-    const float* h_in = u == 0 ? h0 : g + static_cast<int64_t>(u - 1) * H;
-    const int64_t pitch = u == 0 ? H : static_cast<int64_t>(U) * H;
-    PROF(PC_RNNT_PREDICT);
-    launch_lstm_step(x, U, u, c.num_classes, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h_in, pitch, u == 0 ? c0 : c_seq + (u - 1) * BH, g,
-                     u == U - 1 ? h1 : nullptr, c_seq + u * BH, B, H, s);
-  }
-  cudaMemcpyAsync(c1, c_seq + static_cast<int64_t>(U - 1) * BH, BH * 4, cudaMemcpyDeviceToDevice, s);
-  GAM_CHECK_LAUNCH(h, "rnnt_predict_train");
-  return 0;
+  return rnnt_predict_run(h, "rnnt_predict_train", x, h0, c0, B, U, g, h1, c1, c_seq, stream);
 }
 
-// ---- backward passes of the head calls (csrc/head_grads.cu).  Workspaces are carved in 1 KiB-aligned pieces.
-namespace {
-struct Carve {
-  uint8_t* base;
-  int64_t off = 0;
-  float* take(int64_t floats) {
-    float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-    off += align_up(floats * 4, 1024);
-    return p;
-  }
-};
-inline int64_t max3(int64_t a, int64_t b, int64_t c) { return a > b ? (a > c ? a : c) : (b > c ? b : c); }
-
-struct CtcBwdWs { float *dl, *part; };
-int64_t ctc_bwd_layout(const gam_config& c, int64_t R, uint8_t* base, CtcBwdWs* w) {
-  Carve cv{base};
-  w->dl = cv.take(R * c.num_classes);
-  w->part = cv.take(outer_sum_workspace_floats(R, c.num_classes, c.d_model, true));
-  return cv.off;
-}
-
-struct JointBwdWs { float *E, *P, *dl, *dhid, *dE, *dP, *part; };
-int64_t joint_bwd_layout(const gam_config& c, int32_t B, int32_t T, int32_t U, uint8_t* base, JointBwdWs* w) {
-  const int64_t J = c.joint_hidden, BT = static_cast<int64_t>(B) * T, BU = static_cast<int64_t>(B) * U, rows = BT * U;
-  Carve cv{base};
-  w->E = cv.take(BT * J);
-  w->P = cv.take(BU * J);
-  w->dl = cv.take(rows * c.num_classes);
-  w->dhid = cv.take(rows * J);
-  w->dE = cv.take(BT * J);
-  w->dP = cv.take(BU * J);
-  w->part = cv.take(max3(outer_sum_workspace_floats(rows, c.num_classes, J, true), outer_sum_workspace_floats(BT, J, c.d_model, true),
-                         outer_sum_workspace_floats(BU, J, c.pred_hidden, true)));
-  return cv.off;
-}
-
-struct PredBwdWs { float *dgates, *dcc, *dcls, *part; };
-int64_t pred_bwd_layout(const gam_config& c, int32_t B, int32_t U, uint8_t* base, PredBwdWs* w) {
-  const int64_t H = c.pred_hidden, BU = static_cast<int64_t>(B) * U;
-  Carve cv{base};
-  w->dgates = cv.take(BU * 4 * H);
-  w->dcc = cv.take(static_cast<int64_t>(B) * H);
-  w->dcls = cv.take(static_cast<int64_t>(c.num_classes) * 4 * H);
-  w->part = cv.take(max3(outer_sum_workspace_floats(BU, 4 * H, H, true), outer_sum_workspace_floats(c.num_classes, 4 * H, H, false), 0));
-  return cv.off;
-}
-}  // namespace
-
+// ---- backward passes of the head calls (csrc/head_grads.cu)
 int64_t gam_ctc_log_probs_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t T) {
   if (!h || h->cfg.head != 1 || B <= 0 || T <= 0) return -1;
   CtcBwdWs w;
@@ -1362,13 +1473,12 @@ int gam_ctc_log_probs_backward(gam_handle* h, const float* enc, int32_t B, int32
   if (c.head != 1) return fail(h, -1, "ctc_log_probs_backward: model has no CTC head");
   if (B <= 0 || T <= 0) return fail(h, -1, "ctc_log_probs_backward: bad sizes (B=%d, T=%d)", B, T);
   if ((dW == nullptr) != (db == nullptr)) return fail(h, -1, "ctc_log_probs_backward: dW and db go together");
-  const int64_t need = gam_ctc_log_probs_backward_workspace_bytes(h, B, T);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "ctc_log_probs_backward: workspace too small: need %lld bytes, got %lld", (long long)need,
-                (long long)workspace_bytes);
+  uint8_t* ws = workspace_base(h, "ctc_log_probs_backward", workspace, workspace_bytes,
+                               gam_ctc_log_probs_backward_workspace_bytes(h, B, T), true);
+  if (!ws) return -1;
   const int64_t R = static_cast<int64_t>(B) * T;
   CtcBwdWs w;
-  ctc_bwd_layout(c, R, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  ctc_bwd_layout(c, R, ws, &w);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   { PROF(PC_HEAD_BACKWARD);
     launch_softmax_grad(grad, log_probs, w.dl, R, c.num_classes, s); }
@@ -1392,26 +1502,18 @@ int gam_rnnt_joint_backward(gam_handle* h, const float* enc, const float* dec, i
   const gam_config& c = h->cfg;
   if (c.head != 2) return fail(h, -1, "rnnt_joint_backward: model has no RNN-T head");
   if (B <= 0 || T <= 0 || U <= 0) return fail(h, -1, "rnnt_joint_backward: bad sizes (B=%d, T=%d, U=%d)", B, T, U);
-  constexpr int64_t kMaxProjRows = 65535LL * 64;
-  if (static_cast<int64_t>(B) * T > kMaxProjRows || static_cast<int64_t>(B) * U > kMaxProjRows)
-    return fail(h, -1, "rnnt_joint_backward: B*T and B*U must be <= %lld", (long long)kMaxProjRows);
-  if (c.pred_hidden % 16 != 0 || c.d_model % 16 != 0)
-    return fail(h, -1, "rnnt_joint_backward: needs pred_hidden %% 16 == 0 and d_model %% 16 == 0");
+  if (joint_args(h, "rnnt_joint_backward", B, T, U, false) != 0) return -1;
   if ((dW_enc == nullptr) != (db_enc == nullptr) || (dW_pred == nullptr) != (db_pred == nullptr) || (dW_out == nullptr) != (db_out == nullptr))
     return fail(h, -1, "rnnt_joint_backward: each weight gradient goes with its bias gradient");
-  const int64_t need = gam_rnnt_joint_backward_workspace_bytes(h, B, T, U);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "rnnt_joint_backward: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  uint8_t* ws = workspace_base(h, "rnnt_joint_backward", workspace, workspace_bytes, gam_rnnt_joint_backward_workspace_bytes(h, B, T, U),
+                               true);
+  if (!ws) return -1;
   JointBwdWs w;
-  joint_bwd_layout(c, B, T, U, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  joint_bwd_layout(c, B, T, U, ws, &w);
   const int J = c.joint_hidden, V1 = c.num_classes;
   const int64_t BT = static_cast<int64_t>(B) * T, BU = static_cast<int64_t>(B) * U, rows = BT * U;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // the forward's two projections, recomputed with the forward's kernels (same bits)
-  { PROF(PC_HEAD_BACKWARD);
-    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, w.E, B * T, J, c.d_model, s); }
-  { PROF(PC_HEAD_BACKWARD);
-    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, w.P, B * U, J, c.pred_hidden, s); }
+  rnnt_project(h, enc, dec, B, T, U, w.E, w.P, PC_HEAD_BACKWARD, s);   // the forward's projections, the same bits
   { PROF(PC_HEAD_BACKWARD);
     launch_softmax_grad(grad, log_probs, w.dl, rows, V1, s); }
   if (dW_out != nullptr) { PROF(PC_HEAD_BACKWARD);
@@ -1425,14 +1527,7 @@ int gam_rnnt_joint_backward(gam_handle* h, const float* enc, const float* dec, i
     { PROF(PC_HEAD_BACKWARD);   // dP[b, u] = sum_t dhid[b, t, u]
       launch_segment_sum(w.dhid, w.dP, BU, T, J, U, static_cast<int64_t>(T) * U, 1, U, s); }
   }
-  if (dW_enc != nullptr) { PROF(PC_HEAD_BACKWARD);
-    launch_outer_sum(w.dE, enc, BT, J, c.d_model, dW_enc, db_enc, w.part, s); }
-  if (dW_pred != nullptr) { PROF(PC_HEAD_BACKWARD);
-    launch_outer_sum(w.dP, dec, BU, J, c.pred_hidden, dW_pred, db_pred, w.part, s); }
-  if (d_enc != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_e [J, d]
-    launch_head_matmul(w.dE, h->w.rnnt_enc_w, c.d_model, 1, d_enc, BT, J, c.d_model, nullptr, nullptr, 1, 1, s); }
-  if (d_dec != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_p [J, H] = rnnt_wp_t^T
-    launch_head_matmul(w.dP, h->w.rnnt_wp_t, 1, J, d_dec, BU, J, c.pred_hidden, nullptr, nullptr, 1, 1, s); }
+  joint_input_grads(h, enc, dec, BT, BU, w.dE, w.dP, w.part, d_enc, d_dec, dW_enc, db_enc, dW_pred, db_pred, s);
   GAM_CHECK_LAUNCH(h, "rnnt_joint_backward");
   return 0;
 }
@@ -1456,11 +1551,11 @@ int gam_rnnt_predict_backward(gam_handle* h, const int64_t* x, const float* h0, 
   if (!g || !c_seq || !grad_g || !w_hh) return fail(h, -1, "rnnt_predict_backward: g, c_seq, grad_g and w_hh are required");
   if ((dW_hh == nullptr) != (d_bias == nullptr)) return fail(h, -1, "rnnt_predict_backward: dW_hh and d_bias go together");
   if ((dW_ih || d_embed) && (!embed || !w_ih)) return fail(h, -1, "rnnt_predict_backward: embed and w_ih are required for their grads");
-  const int64_t need = gam_rnnt_predict_backward_workspace_bytes(h, B, U);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "rnnt_predict_backward: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  uint8_t* ws = workspace_base(h, "rnnt_predict_backward", workspace, workspace_bytes, gam_rnnt_predict_backward_workspace_bytes(h, B, U),
+                               true);
+  if (!ws) return -1;
   PredBwdWs w;
-  pred_bwd_layout(c, B, U, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  pred_bwd_layout(c, B, U, ws, &w);
   const int64_t BH = static_cast<int64_t>(B) * H, BU = static_cast<int64_t>(B) * U;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (grad_c1 != nullptr)
@@ -1493,48 +1588,6 @@ int gam_rnnt_predict_backward(gam_handle* h, const int64_t* x, const float* h0, 
 }
 
 // ---- fused RNN-T loss (csrc/rnnt_loss.cu; stage 1 is the gathered joint of heads.cu with the row lse kept)
-namespace {
-constexpr int64_t kLossMaxProjRows = 65535LL * 64;   // grid.y limit of the projection GEMMs (64 rows per block)
-
-bool loss_sizes_ok(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
-  if (!h || h->cfg.head != 2 || B <= 0 || T <= 0 || T > h->max_t || U < 0 || U > kAlignMaxTokens) return false;
-  const gam_config& c = h->cfg;
-  const int J = c.joint_hidden;
-  if (J % 4 != 0 || J > rnnt_joint_max_hidden() || J > rnnt_loss_max_hidden() || c.pred_hidden % 16 != 0 || c.d_model % 16 != 0)
-    return false;
-  return static_cast<int64_t>(B) * T <= kLossMaxProjRows && static_cast<int64_t>(B) * (U + 1) <= kLossMaxProjRows;
-}
-
-struct LossFwdWs { float *E, *P, *blank, *label, *alpha; };
-int64_t loss_fwd_layout(const gam_config& c, int32_t B, int32_t T, int32_t U, uint8_t* base, LossFwdWs* w) {
-  const int64_t J = c.joint_hidden, BT = static_cast<int64_t>(B) * T, BU1 = static_cast<int64_t>(B) * (U + 1), N = BT * (U + 1);
-  Carve cv{base};
-  w->E = cv.take(BT * J);
-  w->P = cv.take(BU1 * J);
-  w->blank = cv.take(N);
-  w->label = cv.take(N);
-  w->alpha = cv.take(N);
-  return cv.off;
-}
-
-struct LossBwdWs { float *E, *P, *dE, *dP, *dE_part, *dP_part, *part; };
-int64_t loss_bwd_layout(const gam_config& c, int32_t B, int32_t T, int32_t U, uint8_t* base, LossBwdWs* w) {
-  const RnntLossPlan p = rnnt_loss_plan(B, T, U, c.num_classes);
-  const int64_t J = c.joint_hidden, BT = static_cast<int64_t>(B) * T, BU1 = static_cast<int64_t>(B) * (U + 1);
-  Carve cv{base};
-  w->E = cv.take(BT * J);
-  w->P = cv.take(BU1 * J);
-  w->dE = cv.take(BT * J);
-  w->dP = cv.take(BU1 * J);
-  w->dE_part = cv.take(p.NS * BT * J);
-  w->dP_part = cv.take(p.ST * BU1 * J);
-  w->part = cv.take(max3(p.S > 1 ? static_cast<int64_t>(p.S) * c.num_classes * (J + 1) : 0,
-                         outer_sum_workspace_floats(BT, static_cast<int>(J), c.d_model, true),
-                         outer_sum_workspace_floats(BU1, static_cast<int>(J), c.pred_hidden, true)));
-  return cv.off;
-}
-}  // namespace
-
 int64_t gam_rnnt_loss_saved_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {
   if (!loss_sizes_ok(h, B, T, U)) return -1;
   return static_cast<int64_t>(3) * B * T * (U + 1) * 4;
@@ -1550,25 +1603,18 @@ int gam_rnnt_loss(gam_handle* h, const float* enc, const float* dec, const int32
                   const int32_t* target_len, int32_t B, int32_t T, int32_t U, void* workspace, int64_t workspace_bytes, float* saved,
                   float* loss, void* stream) {
   const gam_config& c = h->cfg;
-  if (c.head != 2) return fail(h, -1, "rnnt_loss: model has no RNN-T head");
-  if (!loss_sizes_ok(h, B, T, U))
-    return fail(h, -1, "rnnt_loss: unsupported sizes (B=%d, T=%d, U=%d; T <= %d, U <= %d, joint_hidden %d <= %d)", B, T, U, h->max_t,
-                kAlignMaxTokens, c.joint_hidden, rnnt_loss_max_hidden());
+  if (loss_args(h, "rnnt_loss", B, T, U) != 0) return -1;
   if (!enc || !dec || (U > 0 && !targets) || !enc_len || !target_len || !saved || !loss)
     return fail(h, -1, "rnnt_loss: a required pointer is NULL");
-  const int64_t need = gam_rnnt_loss_workspace_bytes(h, B, T, U);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "rnnt_loss: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  uint8_t* ws = workspace_base(h, "rnnt_loss", workspace, workspace_bytes, gam_rnnt_loss_workspace_bytes(h, B, T, U), true);
+  if (!ws) return -1;
   LossFwdWs w;
-  loss_fwd_layout(c, B, T, U, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  loss_fwd_layout(c, B, T, U, ws, &w);
   const int J = c.joint_hidden, U1 = U + 1;
   const int64_t N = static_cast<int64_t>(B) * T * U1;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int rc = 0;
-  { PROF(PC_RNNT_JOINT);
-    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, w.E, B * T, J, c.d_model, s); }
-  { PROF(PC_RNNT_JOINT);
-    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, w.P, B * U1, J, c.pred_hidden, s); }
+  rnnt_project(h, enc, dec, B, T, U1, w.E, w.P, PC_RNNT_JOINT, s);
+  int rc;
   { PROF(PC_RNNT_JOINT);
     rc = launch_rnnt_joint_gather(w.E, w.P, h->w.rnnt_wo, h->w.rnnt_bo, targets, w.blank, w.label, saved, B, T, U1, J, c.num_classes, s); }
   if (rc != 0) return fail(h, -4, "rnnt_loss: stage 1 launch rejected (rc=%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
@@ -1589,28 +1635,21 @@ int gam_rnnt_loss_backward(gam_handle* h, const float* enc, const float* dec, co
                            void* workspace, int64_t workspace_bytes, float* d_enc, float* d_dec, float* dW_enc, float* db_enc,
                            float* dW_pred, float* db_pred, float* dW_out, float* db_out, void* stream) {
   const gam_config& c = h->cfg;
-  if (c.head != 2) return fail(h, -1, "rnnt_loss_backward: model has no RNN-T head");
-  if (!loss_sizes_ok(h, B, T, U))
-    return fail(h, -1, "rnnt_loss_backward: unsupported sizes (B=%d, T=%d, U=%d; T <= %d, U <= %d, joint_hidden %d <= %d)", B, T, U,
-                h->max_t, kAlignMaxTokens, c.joint_hidden, rnnt_loss_max_hidden());
+  if (loss_args(h, "rnnt_loss_backward", B, T, U) != 0) return -1;
   if (!enc || !dec || (U > 0 && !targets) || !enc_len || !target_len || !saved || !grad_loss)
     return fail(h, -1, "rnnt_loss_backward: a required pointer is NULL");
   if ((dW_enc == nullptr) != (db_enc == nullptr) || (dW_pred == nullptr) != (db_pred == nullptr) || (dW_out == nullptr) != (db_out == nullptr))
     return fail(h, -1, "rnnt_loss_backward: each weight gradient goes with its bias gradient");
-  const int64_t need = gam_rnnt_loss_backward_workspace_bytes(h, B, T, U);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "rnnt_loss_backward: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  uint8_t* ws = workspace_base(h, "rnnt_loss_backward", workspace, workspace_bytes, gam_rnnt_loss_backward_workspace_bytes(h, B, T, U),
+                               true);
+  if (!ws) return -1;
   LossBwdWs w;
-  loss_bwd_layout(c, B, T, U, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023)), &w);
+  loss_bwd_layout(c, B, T, U, ws, &w);
   const int J = c.joint_hidden, V1 = c.num_classes, U1 = U + 1;
   const int64_t BT = static_cast<int64_t>(B) * T, BU1 = static_cast<int64_t>(B) * U1, N = BT * U1;
   const RnntLossPlan plan = rnnt_loss_plan(B, T, U, V1);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // the forward's two projections, recomputed with the forward's kernels (same bits)
-  { PROF(PC_HEAD_BACKWARD);
-    launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, w.E, B * T, J, c.d_model, s); }
-  { PROF(PC_HEAD_BACKWARD);
-    launch_sgemm_nn_bias(dec, h->w.rnnt_wp_t, h->w.rnnt_bp, w.P, B * U1, J, c.pred_hidden, s); }
+  rnnt_project(h, enc, dec, B, T, U1, w.E, w.P, PC_HEAD_BACKWARD, s);   // the forward's projections, the same bits
   const bool need_hidden = d_enc || d_dec || dW_enc || dW_pred;
   if (need_hidden || dW_out) {
     const RnntLossArgs a{w.E, w.P, h->w.rnnt_wo, h->w.rnnt_bo, targets, enc_len, target_len, saved, saved + N, saved + 2 * N, grad_loss,
@@ -1626,14 +1665,7 @@ int gam_rnnt_loss_backward(gam_handle* h, const float* enc, const float* dec, co
     { PROF(PC_HEAD_BACKWARD);   // dP[b, u] = sum over the frame ranges, in range order
       launch_segment_sum(w.dP_part, w.dP, BU1, plan.ST, J, 1, 1, 0, BU1, s); }
   }
-  if (dW_enc != nullptr) { PROF(PC_HEAD_BACKWARD);
-    launch_outer_sum(w.dE, enc, BT, J, c.d_model, dW_enc, db_enc, w.part, s); }
-  if (dW_pred != nullptr) { PROF(PC_HEAD_BACKWARD);
-    launch_outer_sum(w.dP, dec, BU1, J, c.pred_hidden, dW_pred, db_pred, w.part, s); }
-  if (d_enc != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_e [J, d]
-    launch_head_matmul(w.dE, h->w.rnnt_enc_w, c.d_model, 1, d_enc, BT, J, c.d_model, nullptr, nullptr, 1, 1, s); }
-  if (d_dec != nullptr) { PROF(PC_HEAD_BACKWARD);   // W_p [J, H] = rnnt_wp_t^T
-    launch_head_matmul(w.dP, h->w.rnnt_wp_t, 1, J, d_dec, BU1, J, c.pred_hidden, nullptr, nullptr, 1, 1, s); }
+  joint_input_grads(h, enc, dec, BT, BU1, w.dE, w.dP, w.part, d_enc, d_dec, dW_enc, db_enc, dW_pred, db_pred, s);
   GAM_CHECK_LAUNCH(h, "rnnt_loss_backward");
   return 0;
 }
@@ -1649,11 +1681,10 @@ int gam_emo_head(gam_handle* h, const float* enc, const int32_t* enc_len, int32_
   if (c.head != 3) return fail(h, -1, "emo_head: model has no emo head");
   if (B < 1 || T < 1 || T > 65535 * kPoolChunk)
     return fail(h, -1, "emo_head: bad sizes (B=%d, T=%d; 1 <= T <= %d)", B, T, 65535 * kPoolChunk);
-  const int64_t need = gam_emo_workspace_bytes(h, B, T);
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(h, -1, "emo_head: workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+  float* part = reinterpret_cast<float*>(workspace_base(h, "emo_head", workspace, workspace_bytes, gam_emo_workspace_bytes(h, B, T),
+                                                        false));   // one piece: the per-chunk sums
+  if (!part) return -1;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  float* part = static_cast<float*>(workspace);
   { PROF(PC_EMO_HEAD);
     launch_pool_chunks(enc, enc_len, B, T, part, s); }
   { PROF(PC_EMO_HEAD);

@@ -471,6 +471,24 @@ class Engine:
     def _stream(self) -> C.c_void_p:
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
+    def _call(self, name: str, *args) -> None:
+        """Run entry point `name` on this engine's handle and current stream: a tensor passes its data pointer, None passes
+        NULL.  A nonzero return raises GamError with the library's message."""
+        args = [a.data_ptr() if isinstance(a, Tensor) else a for a in args]
+        with torch.cuda.device(self.device):
+            rc = getattr(self.lib, name)(self.handle, *args, self._stream())
+        _lib.check(self.lib, self.handle, rc, name)
+
+    def _ws(self, cache: Optional["_WorkspaceCache"], key, query: str, *sizes, what: str) -> Tensor:
+        """The workspace entry point `query` sizes for `sizes`, from `cache` (None: a fresh one).  A negative size, which the
+        library returns for sizes it refuses, raises ValueError(what)."""
+        nbytes = int(getattr(self.lib, query)(self.handle, *sizes))
+        if nbytes < 0:
+            raise ValueError(what)
+        if cache is None:
+            return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
+        return cache.get(key, nbytes, self.device)
+
     def logmel_frames(self, n: int) -> int:
         return int(self.lib.gam_logmel_frames(self.handle, int(n)))
 
@@ -496,14 +514,11 @@ class Engine:
         B, N = wav.shape
         M = self.logmel_frames(N)
         mel = torch.empty((B, self.n_mels, M), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            if self._logmel_tc and not fused:
-                ws = self._ws_mel.get((B, N), int(self.lib.gam_logmel_workspace_bytes(self.handle, B, N)), self.device)
-                rc = self.lib.gam_logmel_tc(self.handle, wav.data_ptr(), B, N, mel.data_ptr(), ws.data_ptr(), ws.numel(), self._stream())
-                _lib.check(self.lib, self.handle, rc, "gam_logmel_tc")
-                return mel
-            rc = self.lib.gam_logmel(self.handle, wav.data_ptr(), B, N, mel.data_ptr(), self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_logmel")
+        if self._logmel_tc and not fused:
+            ws = self._ws_mel.get((B, N), int(self.lib.gam_logmel_workspace_bytes(self.handle, B, N)), self.device)
+            self._call("gam_logmel_tc", wav, B, N, mel, ws, ws.numel())
+        else:
+            self._call("gam_logmel", wav, B, N, mel)
         return mel
 
     def encode(self, mel: Tensor, mel_len: Tensor, n_layers_run: int = -1) -> Tuple[Tensor, Tensor]:
@@ -516,10 +531,7 @@ class Engine:
         ws = self.workspace(B, M)
         enc = torch.empty((B, T, self.d_model), dtype=torch.float32, device=self.device)
         enc_len = torch.empty((B,), dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_encode(self.handle, mel.data_ptr(), mel_len.data_ptr(), B, M, ws.data_ptr(), ws.numel(),
-                                     enc.data_ptr(), enc_len.data_ptr(), n_layers_run, self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_encode")
+        self._call("gam_encode", mel, mel_len, B, M, ws, ws.numel(), enc, enc_len, n_layers_run)
         return enc, enc_len
 
     def hyp_width(self, T: int) -> int:
@@ -559,19 +571,12 @@ class Engine:
             path_logp = torch.empty((B,), dtype=torch.float32, device=self.device)
             path_rows = torch.empty((B,), dtype=torch.int32, device=self.device)
             ws = self._ws_dec.get((B, T), int(self.lib.gam_decode_scored_workspace_bytes(self.handle, B, T)), self.device)
-            fn = self.lib.gam_ctc_greedy_scored if self.head_type == 1 else self.lib.gam_rnnt_greedy_scored
-            with torch.cuda.device(self.device):
-                rc = fn(self.handle, enc_btd.data_ptr(), enc_len.data_ptr(), B, T, ws.data_ptr(), ws.numel(), ids.data_ptr(),
-                        frames.data_ptr(), counts.data_ptr(), max_out, token_logp.data_ptr(), path_logp.data_ptr(),
-                        path_rows.data_ptr(), self._stream())
-            _lib.check(self.lib, self.handle, rc, "gam_greedy_scored")
+            self._call("gam_ctc_greedy_scored" if self.head_type == 1 else "gam_rnnt_greedy_scored", enc_btd, enc_len, B, T, ws,
+                       ws.numel(), ids, frames, counts, max_out, token_logp, path_logp, path_rows)
             return ids, frames, counts, token_logp, path_logp, path_rows
         ws = self._ws_dec.get((B, T), int(self.lib.gam_decode_workspace_bytes(self.handle, B, T)), self.device)
-        fn = self.lib.gam_ctc_greedy if self.head_type == 1 else self.lib.gam_rnnt_greedy
-        with torch.cuda.device(self.device):
-            rc = fn(self.handle, enc_btd.data_ptr(), enc_len.data_ptr(), B, T, ws.data_ptr(), ws.numel(), ids.data_ptr(),
-                    frames.data_ptr(), counts.data_ptr(), max_out, self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_greedy")
+        self._call("gam_ctc_greedy" if self.head_type == 1 else "gam_rnnt_greedy", enc_btd, enc_len, B, T, ws, ws.numel(), ids, frames,
+                   counts, max_out)
         return ids, frames, counts
 
     # ------------------------------------------------------------------ resumable greedy decoding (gam_*_greedy_resume)
@@ -581,9 +586,7 @@ class Engine:
         if nbytes < 0:
             raise RuntimeError("model has no head to decode with")
         state = torch.empty((n, nbytes), dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_decode_state_init(self.handle, state.data_ptr(), n, self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_decode_state_init")
+        self._call("gam_decode_state_init", state, n)
         return state
 
     def decode_buffers(self, B: int, max_out: int, n_frames: int = 0, scores: bool = False) -> "DecodeBuffers":
@@ -613,14 +616,10 @@ class Engine:
         if scores and out.token_logp is None:
             raise ValueError("greedy_resume: scores need buffers from decode_buffers(..., scores=True)")
         ws = self._ws_dec.get(("resume", B, T), int(self.lib.gam_decode_resume_workspace_bytes(self.handle, B, T)), self.device)
-        fn = self.lib.gam_ctc_greedy_resume if self.head_type == 1 else self.lib.gam_rnnt_greedy_resume
         sc = [out.token_logp, out.path_logp, out.path_rows, out.frame_logp, out.frame_rows] if scores else [None] * 5
         pitch = out.frame_logp.shape[1] if scores else 0
-        with torch.cuda.device(self.device):
-            rc = fn(self.handle, enc_btd.data_ptr(), B, T, lo.data_ptr(), hi.data_ptr(), frame_base.data_ptr(), state.data_ptr(),
-                    ws.data_ptr(), ws.numel(), out.ids.data_ptr(), out.frames.data_ptr(), out.counts.data_ptr(), out.ids.shape[1],
-                    *[None if t is None else t.data_ptr() for t in sc], pitch, self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_greedy_resume")
+        self._call("gam_ctc_greedy_resume" if self.head_type == 1 else "gam_rnnt_greedy_resume", enc_btd, B, T, lo, hi, frame_base, state,
+                   ws, ws.numel(), out.ids, out.frames, out.counts, out.ids.shape[1], *sc, pitch)
 
     def ctc_log_probs(self, enc_btd: Tensor) -> Tensor:
         """enc [B, T, d] f32 contiguous -> log_probs [B, T, V+1] f32 (CTCHead.forward, gigaam/decoder.py:18-21)."""
@@ -629,9 +628,7 @@ class Engine:
             raise RuntimeError("model has no CTC head")
         B, T, _ = enc_btd.shape
         out = torch.empty((B, T, self.num_classes), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_ctc_log_probs(self.handle, enc_btd.data_ptr(), B, T, out.data_ptr(), self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_ctc_log_probs")
+        self._call("gam_ctc_log_probs", enc_btd, B, T, out)
         return out
 
     def rnnt_joint(self, enc: Tensor, dec: Tensor) -> Tensor:
@@ -646,43 +643,31 @@ class Engine:
         if dec.shape[0] != B:
             raise ValueError(f"joint: encoder batch {B} != decoder batch {dec.shape[0]}")
         out = torch.empty((B, T, U, self.num_classes), dtype=torch.float32, device=self.device)
-        nbytes = int(self.lib.gam_rnnt_joint_workspace_bytes(self.handle, B, T, U))
-        if nbytes < 0:
-            raise ValueError(f"joint: bad sizes B={B}, T={T}, U={U}")
-        ws = self._ws_joint.get((B, T, U), nbytes, self.device)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_rnnt_joint(self.handle, enc.data_ptr(), dec.data_ptr(), B, T, U, ws.data_ptr(), ws.numel(),
-                                         out.data_ptr(), self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_rnnt_joint")
+        ws = self._ws(self._ws_joint, (B, T, U), "gam_rnnt_joint_workspace_bytes", B, T, U, what=f"joint: bad sizes B={B}, T={T}, U={U}")
+        self._call("gam_rnnt_joint", enc, dec, B, T, U, ws, ws.numel(), out)
         return out
+
+    def _predict_sizes(self, x: Optional[Tensor], batch_size: int) -> Tuple[int, int, int]:
+        """(B, U, H) of a prediction-network call, after the checks rnnt_predict and rnnt_predict_train share."""
+        if self.head_type != 2:
+            raise RuntimeError("model has no RNN-T head")
+        if x is not None:
+            assert x.is_cuda and x.dtype == torch.int64 and x.is_contiguous() and x.dim() == 2
+        B, U = (x.shape[0], x.shape[1]) if x is not None else (int(batch_size), 1)
+        return B, U, self.pred_hidden
 
     def rnnt_predict(self, x: Optional[Tensor], h: Optional[Tensor], c: Optional[Tensor], batch_size: int = 1
                      ) -> Tuple[Tensor, Tensor, Tensor]:
         """x [B, U] i64 or None (one step from the zero embedding), h / c [B, H] f32 contiguous or None (zeros)
         -> (g [B, U, H], h1 [B, H], c1 [B, H]) (RNNTDecoder.predict, gigaam/decoder.py:85-102)."""
-        if self.head_type != 2:
-            raise RuntimeError("model has no RNN-T head")
-        H = self.pred_hidden
-        if x is not None:
-            assert x.is_cuda and x.dtype == torch.int64 and x.is_contiguous() and x.dim() == 2
-            B, U = x.shape
-        else:
-            B, U = int(batch_size), 1
+        B, U, H = self._predict_sizes(x, batch_size)
         for name, t in (("h", h), ("c", c)):
             if t is not None:
                 assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
                 if tuple(t.shape) != (B, H):
                     raise ValueError(f"predict: state {name} has shape {tuple(t.shape)}, expected ({B}, {H})")
-        g = torch.empty((B, U, H), dtype=torch.float32, device=self.device)
-        h1 = torch.empty((B, H), dtype=torch.float32, device=self.device)
-        c1 = torch.empty((B, H), dtype=torch.float32, device=self.device)
-
-        def ptr(t):
-            return None if t is None else t.data_ptr()
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_rnnt_predict(self.handle, ptr(x), ptr(h), ptr(c), B, U, g.data_ptr(), h1.data_ptr(), c1.data_ptr(),
-                                           self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_rnnt_predict")
+        g, h1, c1 = self._empty(B, U, H), self._empty(B, H), self._empty(B, H)
+        self._call("gam_rnnt_predict", x, h, c, B, U, g, h1, c1)
         return g, h1, c1
 
     # ------------------------------------------------------------------ alignment of known transcripts (align.cu)
@@ -704,16 +689,11 @@ class Engine:
             raise RuntimeError("model has no CTC head")
         B, T, _ = log_probs.shape
         U = targets.shape[1]
-        nbytes = int(self.lib.gam_ctc_align_workspace_bytes(self.handle, B, T, U))
-        if nbytes < 0:
-            raise ValueError(f"ctc_align: bad sizes B={B}, T={T}, U={U}")
-        ws = self._ws_align.get(("ctc", B, T, U), nbytes, self.device)
+        ws = self._ws(self._ws_align, ("ctc", B, T, U), "gam_ctc_align_workspace_bytes", B, T, U,
+                      what=f"ctc_align: bad sizes B={B}, T={T}, U={U}")
         enc_len, targets, target_len = (self._i32(t, self.device) for t in (enc_len, targets, target_len))
         outs = self._align_outputs(B, U)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_ctc_align(self.handle, log_probs.data_ptr(), enc_len.data_ptr(), targets.data_ptr(), target_len.data_ptr(),
-                                        B, T, U, ws.data_ptr(), ws.numel(), *[t.data_ptr() for t in outs], self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_ctc_align")
+        self._call("gam_ctc_align", log_probs, enc_len, targets, target_len, B, T, U, ws, ws.numel(), *outs)
         return outs
 
     def ctc_align_long(self, log_probs: Tensor, enc_len: Tensor, targets: Tensor, target_len: Tensor,
@@ -733,18 +713,16 @@ class Engine:
         B, T, _ = log_probs.shape
         U = targets.shape[1]
         if skips is not None:
-            size_fn, kind = self.lib.gam_ctc_align_long_skips_workspace_bytes, "ctc_long_skips"
+            name, kind = "gam_ctc_align_long_skips", "ctc_long_skips"
         elif gaps is not None:
-            size_fn, kind = self.lib.gam_ctc_align_long_gaps_workspace_bytes, "ctc_long_gaps"
+            name, kind = "gam_ctc_align_long_gaps", "ctc_long_gaps"
         else:
-            size_fn, kind = self.lib.gam_ctc_align_long_workspace_bytes, "ctc_long"
-        nbytes = int(size_fn(self.handle, B, T, U))
-        if nbytes < 0:
-            raise ValueError(f"ctc_align_long: bad sizes B={B}, T={T}, U={U}")
-        ws = self._ws_align.get((kind, B, T, U), nbytes, self.device)
+            name, kind = "gam_ctc_align_long", "ctc_long"
+        ws = self._ws(self._ws_align, (kind, B, T, U), name + "_workspace_bytes", B, T, U,
+                      what=f"ctc_align_long: bad sizes B={B}, T={T}, U={U}")
         enc_len, targets, target_len = (self._i32(t, self.device) for t in (enc_len, targets, target_len))
         outs = self._align_outputs(B, U)
-        head = [log_probs.data_ptr(), enc_len.data_ptr(), targets.data_ptr(), target_len.data_ptr()]
+        head = [log_probs, enc_len, targets, target_len]
         if gaps is not None:
             line_edges, log_theta = gaps
             line_edges = line_edges.to(device=self.device, dtype=torch.uint8).contiguous()
@@ -753,22 +731,20 @@ class Engine:
             outs = outs + (torch.empty((B, T), dtype=torch.uint8, device=self.device),
                            torch.empty((B,), dtype=torch.int32, device=self.device),
                            torch.empty((B,), dtype=torch.float32, device=self.device))
-            head += [line_edges.data_ptr()]
+            head += [line_edges]
         if skips is not None:
             outs = outs + (torch.empty((B,), dtype=torch.int32, device=self.device),
                            torch.empty((B,), dtype=torch.float32, device=self.device))
         sizes = [B, T, U] + ([] if gaps is None else [float(log_theta)]) + ([] if skips is None else [float(skips)])
-        ptrs = head + sizes + [ws.data_ptr(), ws.numel(), *[t.data_ptr() for t in outs]]
-        name = {"ctc_long": "gam_ctc_align_long", "ctc_long_gaps": "gam_ctc_align_long_gaps",
-                "ctc_long_skips": "gam_ctc_align_long_skips"}[kind]
-        with torch.cuda.device(self.device):
-            if cluster_ctas is None:
-                rc = getattr(self.lib, name)(self.handle, *ptrs, self._stream())
-            else:
-                plan = (C.c_int32 * 2)()
-                rc = getattr(self.lib, name.replace("gam_", "gam_test_", 1))(self.handle, *ptrs, int(cluster_ctas), plan, self._stream())
-                self.last_align_long_plan = (int(plan[0]), int(plan[1]))
-        _lib.check(self.lib, self.handle, rc, name)
+        args = head + sizes + [ws, ws.numel(), *outs]
+        if cluster_ctas is None:
+            self._call(name, *args)
+        else:
+            plan = (C.c_int32 * 2)()
+            test_name = {"gam_ctc_align_long": "gam_test_ctc_align_long", "gam_ctc_align_long_gaps": "gam_test_ctc_align_long_gaps",
+                         "gam_ctc_align_long_skips": "gam_test_ctc_align_long_skips"}[name]
+            self._call(test_name, *args, int(cluster_ctas), plan)
+            self.last_align_long_plan = (int(plan[0]), int(plan[1]))
         return outs
 
     def ctc_spot(self, log_probs: Tensor, enc_len: Tensor, keywords: Tensor, keyword_len: Tensor, threshold: float, max_det: int,
@@ -785,14 +761,11 @@ class Engine:
         i32 = dict(dtype=torch.int32, device=self.device)
         outs = (torch.empty((B, K, max_det), **i32), torch.empty((B, K, max_det), **i32),
                 torch.empty((B, K, max_det), dtype=torch.float32, device=self.device), torch.empty((B, K), **i32))
-        args = [log_probs.data_ptr(), enc_len.data_ptr(), B, T, keywords.data_ptr(), keyword_len.data_ptr(), K, Umax, float(threshold),
-                int(max_det), *[t.data_ptr() for t in outs]]
-        with torch.cuda.device(self.device):
-            if warps_per_cta is None:
-                rc = self.lib.gam_ctc_spot(self.handle, *args, self._stream())
-            else:
-                rc = self.lib.gam_test_ctc_spot(self.handle, *args, int(warps_per_cta), self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_ctc_spot")
+        args = [log_probs, enc_len, B, T, keywords, keyword_len, K, Umax, float(threshold), int(max_det), *outs]
+        if warps_per_cta is None:
+            self._call("gam_ctc_spot", *args)
+        else:
+            self._call("gam_test_ctc_spot", *args, int(warps_per_cta))
         return outs
 
     def spot_state(self, n: int, K: int, Umax: int) -> Tensor:
@@ -802,9 +775,7 @@ class Engine:
         if nbytes < 0:
             raise ValueError(f"spot_state: no CTC head, or Umax={Umax} outside [1, 64]")
         state = torch.empty((n, K, nbytes), dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_ctc_spot_state_init(self.handle, state.data_ptr(), n, K, int(Umax), self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_ctc_spot_state_init")
+        self._call("gam_ctc_spot_state_init", state, n, K, int(Umax))
         return state
 
     def ctc_spot_resume(self, log_probs: Tensor, lo: Tensor, hi: Tensor, frame_base: Tensor, finish: Tensor, keywords: Tensor,
@@ -822,13 +793,9 @@ class Engine:
         assert state.dtype == torch.uint8 and state.is_contiguous() and tuple(state.shape[:2]) == (B, K)
         assert all(t.is_contiguous() and t.shape[:2] == (B, K) for t in det)
         max_det = det[0].shape[2]
-        pend = [None] * 3 if pending is None else [t.data_ptr() for t in pending]
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_ctc_spot_resume(self.handle, log_probs.data_ptr(), B, T, lo.data_ptr(), hi.data_ptr(), frame_base.data_ptr(),
-                                              finish.data_ptr(), keywords.data_ptr(), keyword_len.data_ptr(), K, Umax, float(threshold),
-                                              int(max_det), state.data_ptr(), state.shape[2], *[t.data_ptr() for t in det], *pend,
-                                              self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_ctc_spot_resume")
+        pend = [None] * 3 if pending is None else pending
+        self._call("gam_ctc_spot_resume", log_probs, B, T, lo, hi, frame_base, finish, keywords, keyword_len, K, Umax, float(threshold),
+                   int(max_det), state, state.shape[2], *det, *pend)
 
     def ctc_bias(self, log_probs: Tensor, enc_len: Tensor, keywords: Tensor, keyword_len: Tensor, spotted: Tuple[Tensor, ...],
                  threshold: float, token_flags: Tensor, ids: Tensor, frames: Tensor, counts: Tensor,
@@ -846,10 +813,8 @@ class Engine:
         K, Umax = keywords.shape
         max_out = ids.shape[1]
         max_det = spotted[0].shape[2]
-        nbytes = int(self.lib.gam_ctc_bias_workspace_bytes(self.handle, B, T, K, max_det))
-        if nbytes < 0:
-            raise ValueError(f"ctc_bias: bad sizes B={B}, T={T}, K={K}, max_det={max_det}")
-        ws = self._ws_align.get(("bias", B, T, K, max_det), nbytes, self.device)
+        ws = self._ws(self._ws_align, ("bias", B, T, K, max_det), "gam_ctc_bias_workspace_bytes", B, T, K, max_det,
+                      what=f"ctc_bias: bad sizes B={B}, T={T}, K={K}, max_det={max_det}")
         enc_len, keywords, keyword_len, ids, frames, counts = (self._i32(t, self.device)
                                                                for t in (enc_len, keywords, keyword_len, ids, frames, counts))
         flags = token_flags.to(device=self.device, dtype=torch.uint8).contiguous()
@@ -863,17 +828,9 @@ class Engine:
                torch.empty((B, max_out), **i32),
                None if token_logp is None else torch.empty((B, max_out), dtype=torch.float32, device=self.device),
                None if path_logp is None else torch.empty((B,), dtype=torch.float32, device=self.device)]
-
-        def ptr(t):
-            return None if t is None else t.data_ptr()
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_ctc_bias(self.handle, log_probs.data_ptr(), enc_len.data_ptr(), B, T, keywords.data_ptr(),
-                                       keyword_len.data_ptr(), K, Umax, *[t.data_ptr() for t in spotted], max_det, float(threshold),
-                                       flags.data_ptr(), flags.numel(), ids.data_ptr(), frames.data_ptr(), counts.data_ptr(), max_out,
-                                       ptr(token_logp), ptr(path_logp), ptr(frame_logp),
-                                       0 if frame_logp is None else frame_logp.shape[1], ws.data_ptr(), ws.numel(),
-                                       *[ptr(t) for t in out], self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_ctc_bias")
+        self._call("gam_ctc_bias", log_probs, enc_len, B, T, keywords, keyword_len, K, Umax, *spotted, max_det, float(threshold), flags,
+                   flags.numel(), ids, frames, counts, max_out, token_logp, path_logp, frame_logp,
+                   0 if frame_logp is None else frame_logp.shape[1], ws, ws.numel(), *out)
         return tuple(out)
 
     def rnnt_align_scores(self, enc: Tensor, dec: Tensor, targets: Tensor) -> Tuple[Tensor, Tensor]:
@@ -887,17 +844,12 @@ class Engine:
         U = targets.shape[1]
         if dec.shape[0] != B or dec.shape[1] != U + 1:
             raise ValueError(f"align scores: dec has shape {tuple(dec.shape)}, expected ({B}, {U + 1}, H)")
-        nbytes = int(self.lib.gam_rnnt_align_scores_workspace_bytes(self.handle, B, T, U))
-        if nbytes < 0:
-            raise ValueError(f"align scores: bad sizes B={B}, T={T}, U={U}")
-        ws = self._ws_joint.get((B, T, U + 1), nbytes, self.device)
+        ws = self._ws(self._ws_joint, (B, T, U + 1), "gam_rnnt_align_scores_workspace_bytes", B, T, U,
+                      what=f"align scores: bad sizes B={B}, T={T}, U={U}")
         targets = self._i32(targets, self.device)
         blank = torch.empty((B, T, U + 1), dtype=torch.float32, device=self.device)
         label = torch.empty((B, T, U + 1), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_rnnt_align_scores(self.handle, enc.data_ptr(), dec.data_ptr(), targets.data_ptr(), B, T, U, ws.data_ptr(),
-                                                ws.numel(), blank.data_ptr(), label.data_ptr(), self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_rnnt_align_scores")
+        self._call("gam_rnnt_align_scores", enc, dec, targets, B, T, U, ws, ws.numel(), blank, label)
         return blank, label
 
     def rnnt_align(self, blank: Tensor, label: Tensor, enc_len: Tensor, target_len: Tensor) -> Tuple[Tensor, ...]:
@@ -908,16 +860,11 @@ class Engine:
             raise RuntimeError("model has no RNN-T head")
         B, T, U1 = blank.shape
         U = U1 - 1
-        nbytes = int(self.lib.gam_rnnt_align_workspace_bytes(self.handle, B, T, U))
-        if nbytes < 0:
-            raise ValueError(f"rnnt_align: bad sizes B={B}, T={T}, U={U}")
-        ws = self._ws_align.get(("rnnt", B, T, U), nbytes, self.device)
+        ws = self._ws(self._ws_align, ("rnnt", B, T, U), "gam_rnnt_align_workspace_bytes", B, T, U,
+                      what=f"rnnt_align: bad sizes B={B}, T={T}, U={U}")
         enc_len, target_len = self._i32(enc_len, self.device), self._i32(target_len, self.device)
         outs = self._align_outputs(B, U)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_rnnt_align(self.handle, blank.data_ptr(), label.data_ptr(), enc_len.data_ptr(), target_len.data_ptr(), B, T,
-                                         U, ws.data_ptr(), ws.numel(), *[t.data_ptr() for t in outs], self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_rnnt_align")
+        self._call("gam_rnnt_align", blank, label, enc_len, target_len, B, T, U, ws, ws.numel(), *outs)
         return outs
 
     # ------------------------------------------------------------------ fused RNN-T loss (rnnt_loss.cu)
@@ -937,18 +884,12 @@ class Engine:
         """enc [B, T, d], dec [B, U+1, pred_hidden] f32 contiguous, targets [B, U], enc_len [B], target_len [B] -> (loss [B] f32,
         saved [3, B, T, U+1] f32: the per-node lse, e_blank and e_label that rnnt_loss_backward reads) (gam_rnnt_loss)."""
         B, T, U, targets, enc_len, target_len = self._loss_args(enc, dec, targets, enc_len, target_len, "rnnt_loss")
-        nbytes = int(self.lib.gam_rnnt_loss_workspace_bytes(self.handle, B, T, U))
-        if nbytes < 0:
-            raise ValueError(f"rnnt_loss: unsupported sizes B={B}, T={T}, U={U} (limits: T <= the model's max_encoded_frames, "
-                             f"U <= 4096 tokens, joint_hidden <= 344)")
-        ws = self._scratch(nbytes, "rnnt_loss")
+        ws = self._ws(None, None, "gam_rnnt_loss_workspace_bytes", B, T, U,
+                      what=f"rnnt_loss: unsupported sizes B={B}, T={T}, U={U} (limits: T <= the model's max_encoded_frames, "
+                           f"U <= 4096 tokens, joint_hidden <= 344)")
         saved = self._empty(3, B, T, U + 1)
         loss = self._empty(B)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_rnnt_loss(self.handle, enc.data_ptr(), dec.data_ptr(), targets.data_ptr(), enc_len.data_ptr(),
-                                        target_len.data_ptr(), B, T, U, ws.data_ptr(), ws.numel(), saved.data_ptr(), loss.data_ptr(),
-                                        self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_rnnt_loss")
+        self._call("gam_rnnt_loss", enc, dec, targets, enc_len, target_len, B, T, U, ws, ws.numel(), saved, loss)
         return loss, saved
 
     def rnnt_loss_backward(self, enc: Tensor, dec: Tensor, targets: Tensor, enc_len: Tensor, target_len: Tensor, saved: Tensor,
@@ -965,43 +906,23 @@ class Engine:
             outs += [self._empty(J, d), self._empty(J), self._empty(J, H), self._empty(J), self._empty(V1, J), self._empty(V1)]
         else:
             outs += [None] * 6
-        ws = self._scratch(int(self.lib.gam_rnnt_loss_backward_workspace_bytes(self.handle, B, T, U)), "rnnt_loss_backward")
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_rnnt_loss_backward(self.handle, enc.data_ptr(), dec.data_ptr(), targets.data_ptr(), enc_len.data_ptr(),
-                                                 target_len.data_ptr(), B, T, U, saved.data_ptr(), grad.data_ptr(), ws.data_ptr(),
-                                                 ws.numel(), *[None if t is None else t.data_ptr() for t in outs], self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_rnnt_loss_backward")
+        ws = self._ws(None, None, "gam_rnnt_loss_backward_workspace_bytes", B, T, U, what="rnnt_loss_backward: bad sizes")
+        self._call("gam_rnnt_loss_backward", enc, dec, targets, enc_len, target_len, B, T, U, saved, grad, ws, ws.numel(), *outs)
         return tuple(outs)
 
     # ------------------------------------------------------------------ backward passes of the head calls (head_grads.cu)
     def _empty(self, *shape) -> Tensor:
         return torch.empty(shape, dtype=torch.float32, device=self.device)
 
-    def _scratch(self, nbytes: int, what: str) -> Tensor:
-        if nbytes < 0:
-            raise ValueError(f"{what}: bad sizes")
-        return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
-
     def rnnt_predict_train(self, x: Optional[Tensor], h: Optional[Tensor], c: Optional[Tensor], batch_size: int = 1
                            ) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
         """rnnt_predict (same bits) that also returns the cell state of every step, c_seq [U, B, H]."""
-        if self.head_type != 2:
-            raise RuntimeError("model has no RNN-T head")
-        if x is not None:
-            assert x.is_cuda and x.dtype == torch.int64 and x.is_contiguous() and x.dim() == 2
-        B, U = (x.shape[0], x.shape[1]) if x is not None else (int(batch_size), 1)
-        H = self.pred_hidden
+        B, U, H = self._predict_sizes(x, batch_size)
         for name, t in (("h", h), ("c", c)):
             if t is not None and (tuple(t.shape) != (B, H) or not t.is_contiguous()):
                 raise ValueError(f"predict: state {name} has shape {tuple(t.shape)}, expected ({B}, {H})")
         g, h1, c1, c_seq = self._empty(B, U, H), self._empty(B, H), self._empty(B, H), self._empty(U, B, H)
-
-        def ptr(t):
-            return None if t is None else t.data_ptr()
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_rnnt_predict_train(self.handle, ptr(x), ptr(h), ptr(c), B, U, g.data_ptr(), h1.data_ptr(), c1.data_ptr(),
-                                                 c_seq.data_ptr(), self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_rnnt_predict_train")
+        self._call("gam_rnnt_predict_train", x, h, c, B, U, g, h1, c1, c_seq)
         return g, h1, c1, c_seq
 
     def ctc_log_probs_backward(self, enc: Tensor, log_probs: Tensor, grad: Tensor, need_enc: bool, need_weights: bool):
@@ -1009,14 +930,8 @@ class Engine:
         B, T, d = enc.shape
         d_enc = self._empty(B, T, d) if need_enc else None
         dW, db = (self._empty(self.num_classes, d), self._empty(self.num_classes)) if need_weights else (None, None)
-        ws = self._scratch(int(self.lib.gam_ctc_log_probs_backward_workspace_bytes(self.handle, B, T)), "ctc backward")
-
-        def ptr(t):
-            return None if t is None else t.data_ptr()
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_ctc_log_probs_backward(self.handle, enc.data_ptr(), B, T, log_probs.data_ptr(), grad.data_ptr(),
-                                                     ws.data_ptr(), ws.numel(), ptr(d_enc), ptr(dW), ptr(db), self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_ctc_log_probs_backward")
+        ws = self._ws(None, None, "gam_ctc_log_probs_backward_workspace_bytes", B, T, what="ctc backward: bad sizes")
+        self._call("gam_ctc_log_probs_backward", enc, B, T, log_probs, grad, ws, ws.numel(), d_enc, dW, db)
         return d_enc, dW, db
 
     def rnnt_joint_backward(self, enc: Tensor, dec: Tensor, log_probs: Tensor, grad: Tensor, need_enc: bool, need_dec: bool,
@@ -1030,12 +945,8 @@ class Engine:
             outs += [self._empty(J, d), self._empty(J), self._empty(J, H), self._empty(J), self._empty(V1, J), self._empty(V1)]
         else:
             outs += [None] * 6
-        ws = self._scratch(int(self.lib.gam_rnnt_joint_backward_workspace_bytes(self.handle, B, T, U)), "joint backward")
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_rnnt_joint_backward(self.handle, enc.data_ptr(), dec.data_ptr(), B, T, U, log_probs.data_ptr(),
-                                                  grad.data_ptr(), ws.data_ptr(), ws.numel(),
-                                                  *[None if t is None else t.data_ptr() for t in outs], self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_rnnt_joint_backward")
+        ws = self._ws(None, None, "gam_rnnt_joint_backward_workspace_bytes", B, T, U, what="joint backward: bad sizes")
+        self._call("gam_rnnt_joint_backward", enc, dec, B, T, U, log_probs, grad, ws, ws.numel(), *outs)
         return tuple(outs)
 
     def rnnt_predict_backward(self, x: Optional[Tensor], h: Optional[Tensor], c: Optional[Tensor], g: Tensor, c_seq: Tensor,
@@ -1048,16 +959,9 @@ class Engine:
         outs = [self._empty(B, H), self._empty(B, H)] if need_state else [None, None]
         outs += ([self._empty(V1, H), self._empty(4 * H, H), self._empty(4 * H, H), self._empty(4 * H)] if need_weights
                  else [None] * 4)
-        ws = self._scratch(int(self.lib.gam_rnnt_predict_backward_workspace_bytes(self.handle, B, U)), "predict backward")
-
-        def ptr(t):
-            return None if t is None else t.data_ptr()
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_rnnt_predict_backward(self.handle, ptr(x), ptr(h), ptr(c), B, U, g.data_ptr(), c_seq.data_ptr(),
-                                                    grad_g.data_ptr(), ptr(grad_h1), ptr(grad_c1), embed.data_ptr(), w_ih.data_ptr(),
-                                                    w_hh.data_ptr(), ws.data_ptr(), ws.numel(), *[ptr(t) for t in outs],
-                                                    self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_rnnt_predict_backward")
+        ws = self._ws(None, None, "gam_rnnt_predict_backward_workspace_bytes", B, U, what="predict backward: bad sizes")
+        self._call("gam_rnnt_predict_backward", x, h, c, B, U, g, c_seq, grad_g, grad_h1, grad_c1, embed, w_ih, w_hh, ws, ws.numel(),
+                   *outs)
         return tuple(outs)
 
     def emo_head(self, enc_btd: Tensor, enc_len: Optional[Tensor]) -> Tuple[Tensor, Tensor, Tensor]:
@@ -1068,20 +972,13 @@ class Engine:
         if self.head_type != 3:
             raise RuntimeError("model has no emo head")
         B, T, _ = enc_btd.shape
-        nbytes = int(self.lib.gam_emo_workspace_bytes(self.handle, B, T))
-        if nbytes < 0:
-            raise ValueError(f"emo_head: bad sizes B={B}, T={T}")
+        ws = self._ws(self._ws_emo, (B, T), "gam_emo_workspace_bytes", B, T, what=f"emo_head: bad sizes B={B}, T={T}")
         if enc_len is not None:
             enc_len = enc_len.to(device=self.device, dtype=torch.int32).contiguous()
         pooled = torch.empty((B, self.d_model), dtype=torch.float32, device=self.device)
         logits = torch.empty((B, self.num_classes), dtype=torch.float32, device=self.device)
         probs = torch.empty((B, self.num_classes), dtype=torch.float32, device=self.device)
-        ws = self._ws_emo.get((B, T), nbytes, self.device)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_emo_head(self.handle, enc_btd.data_ptr(), None if enc_len is None else enc_len.data_ptr(), B, T,
-                                       ws.data_ptr(), ws.numel(), pooled.data_ptr(), logits.data_ptr(), probs.data_ptr(),
-                                       self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_emo_head")
+        self._call("gam_emo_head", enc_btd, enc_len, B, T, ws, ws.numel(), pooled, logits, probs)
         return pooled, logits, probs
 
     def group_words(self, ids: Tensor, frames: Tensor, counts: Tensor, token_flags: Tensor):
@@ -1090,10 +987,7 @@ class Engine:
         flags = token_flags.to(device=self.device, dtype=torch.uint8).contiguous()
         outs = [torch.empty((B, max_out), dtype=torch.int32, device=self.device) for _ in range(4)]
         n_words = torch.empty((B,), dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            rc = self.lib.gam_group_words(self.handle, ids.data_ptr(), frames.data_ptr(), counts.data_ptr(), B, max_out, flags.data_ptr(),
-                                          flags.numel(), max_out, *[t.data_ptr() for t in outs], n_words.data_ptr(), self._stream())
-        _lib.check(self.lib, self.handle, rc, "gam_group_words")
+        self._call("gam_group_words", ids, frames, counts, B, max_out, flags, flags.numel(), max_out, *outs, n_words)
         return (*outs, n_words)
 
     def profile_begin(self) -> None:

@@ -41,6 +41,29 @@ def test_struct_layouts_match_header():
     assert cfg_names == [n for n, _ in _lib.GamConfig._fields_]
 
 
+def test_prototypes_parsed_from_header():
+    """_lib binds what the header declares: every declared function, with its C types mapped as by hand, and a type the
+    parser has no mapping for raises instead of binding wrong"""
+    header = (ROOT / "include" / "gigaam_b200.h").read_text()
+    protos = _lib.parse_prototypes(header)
+    assert set(protos) == set(re.findall(r"\b(gam_[a-z0-9_]+)\s*\(", header)) == set(_lib.EXPORTS)
+    vp, i32, i64, f32 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float
+    assert protos["gam_encode"] == (i32, [vp, vp, vp, i32, i64, vp, i64, vp, vp, i32, vp])
+    assert protos["gam_last_error"] == (ctypes.c_char_p, [vp])
+    assert protos["gam_destroy"] == (None, [vp])
+    assert protos["gam_version"] == (i32, [])
+    assert protos["gam_ctc_align_long_skips"] == (i32, [vp] * 6 + [i32] * 3 + [f32, f32, vp, i64] + [vp] * 11)
+    assert protos["gam_ctc_bias"] == (i32, [vp, vp, vp, i32, i32, vp, vp, i32, i32] + [vp] * 4 + [i32, f32, vp, i32] + [vp] * 3
+                                      + [i32] + [vp] * 3 + [i64, vp, i64] + [vp] * 7)
+    assert protos["gam_rnnt_loss_backward"] == (i32, [vp] * 6 + [i32] * 3 + [vp, vp, vp, i64] + [vp] * 9)
+    assert protos["gam_gather_hyps"] == (i32, [vp, vp, i64, vp, vp])
+    assert _lib.REL_POS_MAX_T == int(re.search(r"#define GAM_REL_POS_MAX_T (\d+)", header).group(1))
+    assert _lib.parse_prototypes("/* a comment */\nint64_t gam_x(const gam_handle* h,\n    int32_t n);") == {"gam_x": (i64, [vp, i32])}
+    for bad in ("int gam_x(size_t n);", "double gam_x(void);", "int gam_x(int32_t);", "int gam_x(int (*f)(void));"):
+        with pytest.raises(ValueError):
+            _lib.parse_prototypes(bad)
+
+
 def test_no_cpu_fallback():
     ck = gigaam.synthetic_checkpoint("v2_ctc", n_layers=1)
     model = gigaam.load_model("v2_ctc", device="cpu", checkpoint=ck)
