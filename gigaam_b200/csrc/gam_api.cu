@@ -866,9 +866,9 @@ static int ctc_greedy_impl(gam_handle* h, const char* what, const float* enc, in
   return 0;
 }
 
-// the encoder projection of every row into the workspace, then the cluster kernel
+// the encoder projection of every row into the workspace, then the cluster kernel (boosted unless boost is NULL)
 static int rnnt_greedy_impl(gam_handle* h, const char* what, const float* enc, int32_t B, int32_t T, void* workspace,
-                            const GreedyIo& io, void* stream) {
+                            const GreedyIo& io, void* stream, const BoostGraph* boost = nullptr) {
   const gam_config& c = h->cfg;
   const int64_t R = static_cast<int64_t>(B) * T;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -878,7 +878,8 @@ static int rnnt_greedy_impl(gam_handle* h, const char* what, const float* enc, i
     launch_sgemm_tn_bias(enc, h->w.rnnt_enc_w, h->w.rnnt_enc_b, w.encproj, static_cast<int>(R), c.joint_hidden, c.d_model, s); }
   PROF(PC_RNNT_GREEDY);
   const int rc = launch_rnnt_greedy(w.encproj, h->w.rnnt_emb_gates, h->w.rnnt_whh_t, h->w.rnnt_wp_t, h->w.rnnt_bp, h->w.rnnt_wo,
-                                    h->w.rnnt_bo, B, T, c.pred_hidden, c.num_classes, c.num_classes - 1, c.max_symbols, io, nullptr, s);
+                                    h->w.rnnt_bo, B, T, c.pred_hidden, c.num_classes, c.num_classes - 1, c.max_symbols, io, boost,
+                                    nullptr, s);
   if (rc > 0)
     return fail(h, -1, "rnnt: the greedy kernel is specialised for pred_hidden = joint_hidden = 320 and needs 16-CTA clusters "
                 "(pred_hidden %d)", c.pred_hidden);
@@ -1008,17 +1009,48 @@ int gam_ctc_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T,
                                    path_logp, path_rows, frame_logp, frame_rows, frame_pitch), stream);
 }
 
+static int rnnt_resume(gam_handle* h, const char* what, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
+                       const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes, int32_t* ids, int32_t* frames,
+                       int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows, double* frame_logp,
+                       int32_t* frame_rows, int64_t frame_pitch, void* stream, const BoostGraph* boost) {
+  if (resume_args(h, what, 2, enc, B, T, lo, hi, frame_base, state, workspace, workspace_bytes, ids, frames, counts, max_out,
+                  token_logp, path_logp, path_rows, frame_logp, frame_rows, frame_pitch) != 0)
+    return -1;
+  if (h->cfg.pred_hidden != h->cfg.joint_hidden) return fail(h, -1, "pred_hidden != joint_hidden is not supported");
+  return rnnt_greedy_impl(h, what, enc, B, T, workspace,
+                          resume_io(lo, hi, frame_base, state, kRnntDecodeStateBytes, ids, frames, counts, max_out, token_logp,
+                                    path_logp, path_rows, frame_logp, frame_rows, frame_pitch), stream, boost);
+}
+
 int gam_rnnt_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
                            const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes, int32_t* ids,
                            int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
                            double* frame_logp, int32_t* frame_rows, int64_t frame_pitch, void* stream) {
-  if (resume_args(h, "rnnt_greedy_resume", 2, enc, B, T, lo, hi, frame_base, state, workspace, workspace_bytes, ids, frames, counts,
-                  max_out, token_logp, path_logp, path_rows, frame_logp, frame_rows, frame_pitch) != 0)
-    return -1;
-  if (h->cfg.pred_hidden != h->cfg.joint_hidden) return fail(h, -1, "pred_hidden != joint_hidden is not supported");
-  return rnnt_greedy_impl(h, "rnnt_greedy_resume", enc, B, T, workspace,
-                          resume_io(lo, hi, frame_base, state, kRnntDecodeStateBytes, ids, frames, counts, max_out, token_logp,
-                                    path_logp, path_rows, frame_logp, frame_rows, frame_pitch), stream);
+  return rnnt_resume(h, "rnnt_greedy_resume", enc, B, T, lo, hi, frame_base, state, workspace, workspace_bytes, ids, frames, counts,
+                     max_out, token_logp, path_logp, path_rows, frame_logp, frame_rows, frame_pitch, stream, nullptr);
+}
+
+// the boost graph's own checks (gam_rnnt_greedy_boost, gam_test_rnnt_greedy_boost)
+static bool boost_args(gam_handle* h, const char* what, const int32_t* next, const float* bonus, int32_t n_states, BoostGraph* g) {
+  if (!next || !bonus) { fail(h, -1, "%s: boost_next and boost_bonus are required", what); return false; }
+  if (n_states < 1 || n_states > kBoostMaxStates) {
+    fail(h, -1, "%s: n_states (%d) must be in [1, %d]", what, n_states, kBoostMaxStates);
+    return false;
+  }
+  *g = BoostGraph{next, bonus, n_states};
+  return true;
+}
+
+int gam_rnnt_greedy_boost(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
+                          const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes, int32_t* ids,
+                          int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
+                          double* frame_logp, int32_t* frame_rows, int64_t frame_pitch, const int32_t* boost_next,
+                          const float* boost_bonus, int32_t n_states, void* stream) {
+  if (h->cfg.head != 2) return fail(h, -1, "rnnt_greedy_boost: model has no RNN-T head");
+  BoostGraph g;
+  if (!boost_args(h, "rnnt_greedy_boost", boost_next, boost_bonus, n_states, &g)) return -1;
+  return rnnt_resume(h, "rnnt_greedy_boost", enc, B, T, lo, hi, frame_base, state, workspace, workspace_bytes, ids, frames, counts,
+                     max_out, token_logp, path_logp, path_rows, frame_logp, frame_rows, frame_pitch, stream, &g);
 }
 
 int gam_ctc_log_probs(gam_handle* h, const float* enc, int32_t B, int32_t T, float* log_probs, void* stream) {
@@ -2042,12 +2074,13 @@ int gam_test_mel_log(gam_handle* h, const float* P, const int32_t* fexp, int32_t
 static int test_rnnt_greedy(gam_handle* h, const char* what, const float* encproj, const int32_t* len, const float* emb_gates,
                             const float* whhT, const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T,
                             int32_t V1, int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts,
-                            float* token_logp, float* path_logp, int32_t* path_rows, int32_t* plan, void* stream) {
+                            float* token_logp, float* path_logp, int32_t* path_rows, int32_t* plan, void* stream,
+                            const BoostGraph* boost = nullptr) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc;
   { PROF(PC_RNNT_GREEDY);
     rc = launch_rnnt_greedy(encproj, emb_gates, whhT, wpT, bp, wo, bo, B, T, 320, V1, V1 - 1, max_symbols,
-                            fresh_io(len, ids, frames, counts, max_out, token_logp, path_logp, path_rows), plan, s); }
+                            fresh_io(len, ids, frames, counts, max_out, token_logp, path_logp, path_rows), boost, plan, s); }
   if (rc > 0) return fail(h, -1, "%s: 16-CTA clusters cannot be scheduled on this device", what);
   if (rc < 0) return fail(h, -4, "%s: launch failed: %s", what, cudaGetErrorString(cudaGetLastError()));
   GAM_CHECK_LAUNCH(h, what);
@@ -2066,6 +2099,23 @@ int gam_test_rnnt_greedy_scored(gam_handle* h, const float* encproj, const int32
                 max_out);
   return test_rnnt_greedy(h, "test_rnnt_greedy_scored", encproj, len, emb_gates, whhT, wpT, bp, wo, bo, B, T, V1, max_symbols, max_out,
                           ids, frames, counts, token_logp, path_logp, path_rows, plan, stream);
+}
+
+int gam_test_rnnt_greedy_boost(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,
+                               const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
+                               int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts, float* token_logp,
+                               float* path_logp, int32_t* path_rows, const int32_t* boost_next, const float* boost_bonus,
+                               int32_t n_states, int32_t* plan, void* stream) {
+  if (!encproj || !len || !emb_gates || !whhT || !wpT || !bp || !wo || !bo || !ids || !frames || !counts ||
+      (token_logp && (!path_logp || !path_rows)))
+    return fail(h, -1, "test_rnnt_greedy_boost: every operand is required (path_logp and path_rows when token_logp is given)");
+  if (B <= 0 || T <= 0 || V1 < 2 || max_symbols <= 0 || max_out <= 0)
+    return fail(h, -1, "test_rnnt_greedy_boost: bad sizes (B=%d, T=%d, V1=%d, max_symbols=%d, max_out=%d)", B, T, V1, max_symbols,
+                max_out);
+  BoostGraph g;
+  if (!boost_args(h, "test_rnnt_greedy_boost", boost_next, boost_bonus, n_states, &g)) return -1;
+  return test_rnnt_greedy(h, "test_rnnt_greedy_boost", encproj, len, emb_gates, whhT, wpT, bp, wo, bo, B, T, V1, max_symbols, max_out,
+                          ids, frames, counts, token_logp, path_logp, path_rows, plan, stream, &g);
 }
 
 int gam_test_rnnt_greedy(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,

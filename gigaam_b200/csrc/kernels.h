@@ -65,12 +65,17 @@ struct alignas(16) DecodeState {
   int rows;         // decision rows so far (scored calls)
   double path;      // RNN-T: fp64 sum of l over those rows (warp 0's running sum)
   double pad;       // keeps the CTC record (up to h) a multiple of 16 bytes
-  double part[32];  // CTC: the fp64 partial sums of the scored collapse, partial k over the rows r with r % 32 == k
+  union {
+    double part[32];  // CTC: the fp64 partial sums of the scored collapse, partial k over the rows r with r % 32 == k
+    int boost_state;  // RNN-T: the boost graph's state (gam_rnnt_greedy_boost); 0, the initial state, in a fresh record
+  };
   float h[kDecodeStateH], c[kDecodeStateH], pg[kDecodeStateH];   // RNN-T: LSTM state and W_p h + b_p
 };
 constexpr int64_t kCtcDecodeStateBytes = static_cast<int64_t>(offsetof(DecodeState, h));
 constexpr int64_t kRnntDecodeStateBytes = static_cast<int64_t>(sizeof(DecodeState));
 static_assert(kCtcDecodeStateBytes % 16 == 0, "state records stay 16-byte aligned");
+static_assert(sizeof(DecodeState) == 4128 && offsetof(DecodeState, boost_state) == 32,
+              "the boost state shares the CTC partial sums' bytes; the RNN-T record keeps its size");
 void launch_decode_state_init(uint8_t* state, int64_t stride, int n, int blank, cudaStream_t s);
 
 // What a greedy decode of B streams writes, and which frames of each stream it decodes (launch_ctc_collapse,
@@ -294,12 +299,20 @@ void launch_lstm_bwd_step(const int64_t* x, int U, int u, int V1, const float* e
 // out [V1, H4]: per-class sums of dgates rows (blank row zero); returns 1 if H4 is too large
 int launch_class_gate_sum(const int64_t* x, int64_t rows, const float* dgates, int H4, int V1, int blank, float* out, cudaStream_t s);
 
-// rnnt_cluster.cu: greedy decode of encproj [B, T, H] (see GreedyIo).  Returns 0 ok, 1 = 16-CTA clusters unavailable /
-// unsupported shape, <0 error.  plan: host int[7] that receives the chosen launch (NH, GLOB, rows_smem, cls_per, nu, groups,
-// clusters), or NULL.
+// A boost graph (gam_rnnt_greedy_boost): next [S, V1] and bonus [S, V1], state 0 initial, S <= kBoostMaxStates
+constexpr int kBoostMaxStates = 65536;
+struct BoostGraph {
+  const int* next;
+  const float* bonus;
+  int n_states;
+};
+
+// rnnt_cluster.cu: greedy decode of encproj [B, T, H] (see GreedyIo), boosted by `boost` unless it is NULL.  Returns 0 ok,
+// 1 = 16-CTA clusters unavailable / unsupported shape, <0 error.  plan: host int[7] that receives the chosen launch (NH, GLOB,
+// rows_smem, cls_per, nu, groups, clusters), or NULL.
 int launch_rnnt_greedy(const float* encproj, const float* emb_gates, const float* whhT, const float* wpT, const float* bp,
                        const float* wo, const float* bo, int B, int T, int H, int V1, int blank, int max_symbols, const GreedyIo& io,
-                       int* plan, cudaStream_t s);
+                       const BoostGraph* boost, int* plan, cudaStream_t s);
 
 // gemm.cu
 struct GemmParams;

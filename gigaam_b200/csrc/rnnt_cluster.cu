@@ -40,6 +40,16 @@
 // (0 + 1) + (2 + 3)), whatever the group width, so an utterance's scores do not depend on the batch it is decoded in.
 // Warp 0 writes l on emission and sums it (fp64) over the utterance's decision rows.  The unscored instantiation
 // compiles none of this.
+//
+// Boosted instantiation (BOOST, gam_rnnt_greedy_boost): utterance u is in state q_u of a boost graph, and the argmax runs
+// over fp32(z_c + bonus[q_u, c]) (blank: + 0) with the same first-index and non-finite rules.  Each CTA keeps its own class
+// slice of bonus[q_u] for every utterance of the group in shared memory (taken out of the W_o rows).  After an emission
+// warp kStage0 moves q_u along next[q_u, label] (an entry outside [0, S): state 0) and warps kStage0.. restage the slices of
+// the utterances that emitted; those warps have no work in the LSTM and prediction phases that every emission triggers, so
+// the table loads run beside them.  When scored, l stays the model's own log_softmax(z)[label]: the lanes keep the
+// log-sum-exp of z on its own running maximum, the argmax carries the winner's unboosted z, and the best-value exchange
+// carries both, so l = -(log sum_c exp(z_c - z_max) - (z_label - z_max)), which is -log sum bit for bit with zero bonuses.
+// q_u is stored in the record's boost_state.
 #include <cooperative_groups.h>
 
 #include <cstdlib>
@@ -76,6 +86,7 @@ struct RnntClParams {
   int rows_smem;           // class rows of W_o resident in shared memory per CTA
   int cls_pad;             // floats reserved for the bias slice
   GreedyIo io;             // outputs and stream ranges (kernels.h); io.state == NULL: a fresh call
+  BoostGraph boost;        // read by the boosted instantiation only
 };
 
 // per-utterance decoding state (gigaam/decoding.py:150-205), owned by warp 0 of every CTA (identical in all of them)
@@ -102,7 +113,8 @@ struct Smem {
   int4 my_i[NH];
   Ctl ctl;
   uint64_t bar_h[2], bar_pg[2], bar_best[2];   // arrival of the three all-to-all exchanges (alternating pairs)
-  // followed by: [ScoreSmem<NH> if SCORED]; float bo[cls_pad]; float wo[rows_smem][kWoPitch];
+  // followed by: [ScoreSmem<NH> if SCORED]; [BoostSmem<NH> if BOOST]; [BoostScoreSmem<NH> if BOOST and SCORED];
+  // float bo[cls_pad]; [float bonus[4 NH][cls_pad] if BOOST]; float wo[rows_smem][kWoPitch];
 };
 
 // what the scored instantiation adds after Smem
@@ -115,21 +127,46 @@ struct ScoreSmem {
   int rows[kMaxU];
 };
 
+// what the boosted instantiation adds
+template <int NH>
+struct BoostSmem {
+  int q[kMaxU];                   // boost graph state per utterance (warp kStage0, lane u)
+};
+// ... and, when also scored: the maximum of the unboosted z and the winner's unboosted z beside the boosted argmax
+template <int NH>
+struct BoostScoreSmem {
+  float4 best_m[2][kCl][NH], best_z[2][kCl][NH];
+  float wbest_m[kWarps][4 * NH], wbest_z[kWarps][4 * NH];
+  float4 my_m[NH], my_z[NH];
+};
+
 // Bytes one CTA receives per best-value exchange: one 16-byte store per utterance-half from each CTA of the cluster for
-// every field of the payload (best_v, best_i and, when scored, best_s).  The expect-tx count of bar_best is this value,
-// and the receive buffers of one parity are sized from the same constant, so the two cannot disagree.
-template <int NH, bool SCORED>
-constexpr uint32_t best_exchange_bytes() { return kCl * NH * (SCORED ? 3 : 2) * 16; }
+// every field of the payload (best_v, best_i and, when scored, best_s; boosted and scored, also best_m and best_z).  The
+// expect-tx count of bar_best is this value, and the receive buffers of one parity are sized from the same constant, so the
+// two cannot disagree.
+template <int NH, bool SCORED, bool BOOST = false>
+constexpr uint32_t best_exchange_bytes() { return kCl * NH * (SCORED ? (BOOST ? 5 : 3) : 2) * 16; }
 static_assert(sizeof(Smem<1>::best_v[0]) + sizeof(Smem<1>::best_i[0]) == best_exchange_bytes<1, false>(), "best exchange payload");
 static_assert(sizeof(Smem<2>::best_v[0]) + sizeof(Smem<2>::best_i[0]) == best_exchange_bytes<2, false>(), "best exchange payload");
 static_assert(sizeof(Smem<1>::best_v[0]) + sizeof(Smem<1>::best_i[0]) + sizeof(ScoreSmem<1>::best_s[0]) ==
               best_exchange_bytes<1, true>(), "scored best exchange payload");
 static_assert(sizeof(Smem<2>::best_v[0]) + sizeof(Smem<2>::best_i[0]) + sizeof(ScoreSmem<2>::best_s[0]) ==
               best_exchange_bytes<2, true>(), "scored best exchange payload");
+static_assert(sizeof(Smem<2>::best_v[0]) + sizeof(Smem<2>::best_i[0]) + sizeof(ScoreSmem<2>::best_s[0]) +
+              sizeof(BoostScoreSmem<2>::best_m[0]) + sizeof(BoostScoreSmem<2>::best_z[0]) == best_exchange_bytes<2, true, true>(),
+              "boosted scored best exchange payload");
 static_assert(sizeof(float4) == 16 && sizeof(int4) == 16, "push16 moves one float4 / int4");
 
-template <int NH, bool SCORED>
-constexpr int fixed_smem_bytes() { return static_cast<int>(sizeof(Smem<NH>) + (SCORED ? sizeof(ScoreSmem<NH>) : 0)); }
+template <int NH, bool SCORED, bool BOOST = false>
+constexpr int fixed_smem_bytes() {
+  return static_cast<int>(sizeof(Smem<NH>) + (SCORED ? sizeof(ScoreSmem<NH>) : 0) + (BOOST ? sizeof(BoostSmem<NH>) : 0) +
+                          (BOOST && SCORED ? sizeof(BoostScoreSmem<NH>) : 0));
+}
+static_assert(sizeof(ScoreSmem<1>) % 16 == 0 && sizeof(ScoreSmem<2>) % 16 == 0 && sizeof(BoostSmem<2>) % 16 == 0,
+              "the shared-memory parts stay 16-byte aligned");
+// every byte of shared memory in front of the W_o rows: the fixed parts, the bias slice and (boosted) the bonus slices
+template <int NH, bool SCORED, bool BOOST>
+constexpr int smem_before_rows(int cls_pad) { return fixed_smem_bytes<NH, SCORED, BOOST>() + cls_pad * 4 * (1 + (BOOST ? 4 * NH : 0)); }
 
 __device__ __forceinline__ float sigm(float x) { return 1.0f / (1.0f + expf(-x)); }
 __device__ __forceinline__ float comp(const float4& v, int u) { return u == 0 ? v.x : (u == 1 ? v.y : (u == 2 ? v.z : v.w)); }
@@ -162,6 +199,28 @@ __device__ __forceinline__ void arg_update(float a, int cls, float& bv, int& bi)
     const bool bad = !(a < INFINITY);
     bv = bad ? INFINITY : a;
     bi = bad ? -1 : cls;
+  }
+}
+
+// boosted argmax update: the argmax of arg_update over a = z + b, carrying the winner's z (bz); when scored, the sum of
+// exp(z - zm) over the finite z relative to their own running maximum zm, by arg_update_s's rule
+template <bool SCORED>
+__device__ __forceinline__ void arg_update_b(float z, float b, int cls, float& bv, int& bi, float& bz, float& zm, float& bs) {
+  const float a = z + b;
+  if (!(a <= bv)) {
+    const bool bad = !(a < INFINITY);
+    bv = bad ? INFINITY : a;
+    bi = bad ? -1 : cls;
+    bz = z;
+  }
+  if constexpr (SCORED) {
+    if (!(z <= zm)) {
+      const bool bad = !(z < INFINITY);
+      if (!bad) bs = bs * expf(zm - z) + 1.f;
+      zm = bad ? INFINITY : z;
+    } else if (z > -INFINITY) {
+      bs += expf(z - zm);
+    }
   }
 }
 
@@ -236,15 +295,27 @@ __device__ long long g_rnnt_dbg[16];
 // A fresh call starts from the constants of a fresh record (blank label, a pending step, zeros) and decodes [0, hi).  A chunk
 // edge is a frame edge (nsym = 0), so decoding [0, L) in consecutive chunks runs the same operations on the same values as
 // one fresh call.
-template <int NH, bool GLOB, bool SCORED>
+template <int NH, bool GLOB, bool SCORED, bool BOOST>
 __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClParams p) {
   constexpr int NU = 4 * NH;
   using SM = Smem<NH>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   SM& s = *reinterpret_cast<SM*>(smem_raw);
   [[maybe_unused]] ScoreSmem<NH>& sc = *reinterpret_cast<ScoreSmem<NH>*>(smem_raw + sizeof(SM));
-  float* s_bo = reinterpret_cast<float*>(smem_raw + fixed_smem_bytes<NH, SCORED>());
+  float* s_bo = reinterpret_cast<float*>(smem_raw + fixed_smem_bytes<NH, SCORED, BOOST>());
   float* s_wo = s_bo + p.cls_pad;
+  // boosted: q per utterance, the scored exchange fields and bonus[q_u] over the own classes ([u][cls_pad])
+  [[maybe_unused]] int* s_q = nullptr;
+  [[maybe_unused]] BoostScoreSmem<NH>* bss = nullptr;
+  [[maybe_unused]] float* s_bon = nullptr;
+  constexpr bool BS = BOOST && SCORED;
+  if constexpr (BOOST) {
+    constexpr int off = sizeof(SM) + (SCORED ? sizeof(ScoreSmem<NH>) : 0);
+    s_q = reinterpret_cast<BoostSmem<NH>*>(smem_raw + off)->q;
+    bss = reinterpret_cast<BoostScoreSmem<NH>*>(smem_raw + off + sizeof(BoostSmem<NH>));
+    s_bon = s_wo;
+    s_wo += NU * p.cls_pad;
+  }
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = static_cast<int>(cluster.block_rank());
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -281,6 +352,19 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
   const int pq = lane & 15, pj = warp * 2 + (lane >> 4);
   const bool pred_thread = warp < kHS / 2;
   const float my_bp = pred_thread ? __ldg(p.bp + rank * kHS + pj) : 0.f;
+  // boosted: warps kStage0.. (no LSTM or prediction role) keep the bonus slices; stage(m) loads bonus[q_u] over the own
+  // classes for the utterances of mask m (blank: 0)
+  constexpr int kStage0 = 4 * kHS / 8, kStageThreads = kThreads - 32 * kStage0;
+  static_assert(kHS / 2 <= kStage0 && kStageThreads % 32 == 0, "the staging warps have no LSTM or prediction role");
+  [[maybe_unused]] auto stage = [&](unsigned m) {
+    for (int i = tid - 32 * kStage0; i < NU * ncls; i += kStageThreads) {
+      const int u = i / ncls, c = i - u * ncls;
+      if ((m >> u) & 1) {
+        const int cls = cls0 + c;
+        s_bon[u * p.cls_pad + c] = cls == p.blank ? 0.f : __ldg(p.boost.bonus + static_cast<size_t>(s_q[u]) * p.V1 + cls);
+      }
+    }
+  };
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
       ptx::mbar_init(&s.bar_h[i], 1);
@@ -292,7 +376,7 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
   __syncthreads();
   uint32_t n_h = 0, n_pg = 0, n_b = 0;   // exchanges done so far (barrier = n & 1, phase parity = (n >> 1) & 1)
   constexpr uint32_t kStateBytes = kCl * kHS * NH * 16;
-  constexpr uint32_t kBestBytes = best_exchange_bytes<NH, SCORED>();
+  constexpr uint32_t kBestBytes = best_exchange_bytes<NH, SCORED, BOOST>();
 
   for (int group = cluster_id; group < p.num_groups; group += num_clusters) {
     // warp 0 lane u: counts[b] when the call started, frame_base[b], and the current frame's sum of l and rows
@@ -347,6 +431,18 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
       const DecodeState* st = u < p.nu && ug < p.B ? state_of(p, ug) : nullptr;
       s.c[0][u][j] = st ? st->c[rank * kHS + j] : 0.f;
       s.c[1][u][j] = 0.f;
+    }
+    if constexpr (BOOST) {   // q from the records (a fresh record holds 0), then every utterance's bonus slice
+      if (warp >= kStage0) {
+        if (warp == kStage0 && lane < kMaxU) {
+          const int ug = group * p.nu + lane;
+          const DecodeState* st = lane < p.nu && lane < NU && ug < p.B ? state_of(p, ug) : nullptr;
+          const int q = st ? st->boost_state : 0;
+          s_q[lane] = q >= 0 && q < p.boost.n_states ? q : 0;
+        }
+        ptx::named_bar_sync<kStageThreads>(1);
+        stage(0xffffffffu);
+      }
     }
     __syncthreads();
     const int act0 = s.ctl.act_m;   // the utterances this call decodes (a resume call leaves the others' records and outputs)
@@ -508,8 +604,14 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
       float bv[NH];
       int bi[NH];
       [[maybe_unused]] float bs[NH];
+      [[maybe_unused]] float bz[NH], zm[NH];   // boosted: the winner's unboosted z; when scored, the running max of z
 #pragma unroll
       for (int hh = 0; hh < NH; ++hh) { bv[hh] = -INFINITY; bi[hh] = 0x7fffffff; bs[hh] = 0.f; }
+      if constexpr (BOOST) {
+#pragma unroll
+        for (int hh = 0; hh < NH; ++hh) { bz[hh] = 0.f; zm[hh] = -INFINITY; }
+      }
+      [[maybe_unused]] const float* bon = s_bon + myu * p.cls_pad;   // bonus of utterance 4 hh + myu at bon[4 hh cls_pad + lr]
       // shared-memory rows: local rows warp, warp+16, ... (ascending, so the first maximum wins as in torch.argmax)
       for (int lr0 = warp; lr0 < nsm; lr0 += kWarps * kCB) {
         float4 acc[kCB][NH];
@@ -537,7 +639,11 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
           if (lr < nsm) {
 #pragma unroll
             for (int hh = 0; hh < NH; ++hh) {
-              arg_update_s<SCORED>(reduce4(acc[c][hh], lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh], bs[hh]);
+              if constexpr (BOOST)
+                arg_update_b<SCORED>(reduce4(acc[c][hh], lane) + s_bo[lr], bon[4 * hh * p.cls_pad + lr], cls0 + lr, bv[hh], bi[hh],
+                                     bz[hh], zm[hh], bs[hh]);
+              else
+                arg_update_s<SCORED>(reduce4(acc[c][hh], lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh], bs[hh]);
             }
           }
         }
@@ -552,7 +658,11 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int kk = 0; kk < kH / 32; ++kk) fma4(acc, wg[gi][kk], s.hid4[hh][lane + 32 * kk]);
-            arg_update_s<SCORED>(reduce4(acc, lane) + s_bo[gcls[gi]], cls0 + gcls[gi], bv[hh], bi[hh], bs[hh]);
+            if constexpr (BOOST)
+              arg_update_b<SCORED>(reduce4(acc, lane) + s_bo[gcls[gi]], bon[4 * hh * p.cls_pad + gcls[gi]], cls0 + gcls[gi], bv[hh],
+                                   bi[hh], bz[hh], zm[hh], bs[hh]);
+            else
+              arg_update_s<SCORED>(reduce4(acc, lane) + s_bo[gcls[gi]], cls0 + gcls[gi], bv[hh], bi[hh], bs[hh]);
           }
         }
       }
@@ -562,7 +672,11 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         for (int hh = 0; hh < NH; ++hh) {
           float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
           for (int kk = 0; kk < kH / 32; ++kk) fma4(acc, __ldg(w + lane + 32 * kk), s.hid4[hh][lane + 32 * kk]);
-          arg_update_s<SCORED>(reduce4(acc, lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh], bs[hh]);
+          if constexpr (BOOST)
+            arg_update_b<SCORED>(reduce4(acc, lane) + s_bo[lr], bon[4 * hh * p.cls_pad + lr], cls0 + lr, bv[hh], bi[hh], bz[hh], zm[hh],
+                                 bs[hh]);
+          else
+            arg_update_s<SCORED>(reduce4(acc, lane) + s_bo[lr], cls0 + lr, bv[hh], bi[hh], bs[hh]);
         }
       }
       }
@@ -573,6 +687,10 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         if constexpr (SCORED) {
 #pragma unroll
           for (int hh = 0; hh < NH; ++hh) sc.wbest_s[warp][4 * hh + myu] = bs[hh];
+        }
+        if constexpr (BS) {
+#pragma unroll
+          for (int hh = 0; hh < NH; ++hh) { bss->wbest_m[warp][4 * hh + myu] = zm[hh]; bss->wbest_z[warp][4 * hh + myu] = bz[hh]; }
         }
       }
       __syncthreads();
@@ -585,19 +703,36 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         const int par = n_b & 1;
         float v0 = -INFINITY;
         int i0 = 0x7fffffff;
+        [[maybe_unused]] float z0 = 0.f, zmax = -INFINITY;   // boosted and scored: the winner's z and the maximum of z
         for (int w = sub; w < kWarps; w += kSub) {
           const float v = s.wbest_v[w][u];
           const int i = s.wbest_i[w][u];
-          if (v > v0 || (v == v0 && i < i0)) { v0 = v; i0 = i; }
+          if (v > v0 || (v == v0 && i < i0)) {
+            v0 = v; i0 = i;
+            if constexpr (BS) z0 = bss->wbest_z[w][u];
+          }
+          if constexpr (BS) { const float m = bss->wbest_m[w][u]; if (m > zmax) zmax = m; }
         }
 #pragma unroll
         for (int o = NU; o < 32; o <<= 1) {
           const float v = __shfl_xor_sync(0xffffffffu, v0, o);
           const int i = __shfl_xor_sync(0xffffffffu, i0, o);
+          if constexpr (BS) {
+            const float z = __shfl_xor_sync(0xffffffffu, z0, o), m = __shfl_xor_sync(0xffffffffu, zmax, o);
+            if (v > v0 || (v == v0 && i < i0)) z0 = z;
+            if (m > zmax) zmax = m;
+          }
           if (v > v0 || (v == v0 && i < i0)) { v0 = v; i0 = i; }
         }
         if (lane < NU) { reinterpret_cast<float*>(s.my_v)[u] = v0; reinterpret_cast<int*>(s.my_i)[u] = i0; }
-        if constexpr (SCORED) {   // the CTA's sum relative to its maximum v0 (every lane of utterance u holds v0)
+        if constexpr (BS) {   // the sum relative to the maximum of the unboosted z
+          const float cs = fold16([&](int w, float& v, float& sk) { v = bss->wbest_m[w][u]; sk = sc.wbest_s[w][u]; }, zmax, NU, lane);
+          if (lane < NU) {
+            reinterpret_cast<float*>(sc.my_s)[u] = cs;
+            reinterpret_cast<float*>(bss->my_m)[u] = zmax;
+            reinterpret_cast<float*>(bss->my_z)[u] = z0;
+          }
+        } else if constexpr (SCORED) {   // the CTA's sum relative to its maximum v0 (every lane of utterance u holds v0)
           const float cs = fold16([&](int w, float& v, float& sk) { v = s.wbest_v[w][u]; sk = sc.wbest_s[w][u]; }, v0, NU, lane);
           if (lane < NU) reinterpret_cast<float*>(sc.my_s)[u] = cs;
         }
@@ -610,6 +745,10 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
             push16(&s.best_i[par][rank][hh], &s.bar_best[par], lane, static_cast<uint32_t>(ii.x), static_cast<uint32_t>(ii.y),
                    static_cast<uint32_t>(ii.z), static_cast<uint32_t>(ii.w));
             if constexpr (SCORED) push16(&sc.best_s[par][rank][hh], &s.bar_best[par], lane, sc.my_s[hh]);
+            if constexpr (BS) {
+              push16(&bss->best_m[par][rank][hh], &s.bar_best[par], lane, bss->my_m[hh]);
+              push16(&bss->best_z[par][rank][hh], &s.bar_best[par], lane, bss->my_z[hh]);
+            }
           }
         }
         DBG_T(4);
@@ -617,15 +756,25 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         DBG_T(5);
         v0 = -INFINITY;
         i0 = 0x7fffffff;
+        if constexpr (BS) { z0 = 0.f; zmax = -INFINITY; }
         for (int r = sub; r < kCl; r += kSub) {   // source CTAs ascend with the class index
           const float v = reinterpret_cast<const float*>(&s.best_v[par][r][0])[u];
           const int i = reinterpret_cast<const int*>(&s.best_i[par][r][0])[u];
-          if (v > v0 || (v == v0 && i < i0)) { v0 = v; i0 = i; }
+          if (v > v0 || (v == v0 && i < i0)) {
+            v0 = v; i0 = i;
+            if constexpr (BS) z0 = reinterpret_cast<const float*>(&bss->best_z[par][r][0])[u];
+          }
+          if constexpr (BS) { const float m = reinterpret_cast<const float*>(&bss->best_m[par][r][0])[u]; if (m > zmax) zmax = m; }
         }
 #pragma unroll
         for (int o = NU; o < 32; o <<= 1) {
           const float v = __shfl_xor_sync(0xffffffffu, v0, o);
           const int i = __shfl_xor_sync(0xffffffffu, i0, o);
+          if constexpr (BS) {
+            const float z = __shfl_xor_sync(0xffffffffu, z0, o), m = __shfl_xor_sync(0xffffffffu, zmax, o);
+            if (v > v0 || (v == v0 && i < i0)) z0 = z;
+            if (m > zmax) zmax = m;
+          }
           if (v > v0 || (v == v0 && i < i0)) { v0 = v; i0 = i; }
         }
         DBG_T(10);
@@ -633,7 +782,13 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
         // all-NaN log_softmax row; the label that indexes emb_gates below is in [0, V1) by construction
         const int lab = (i0 < 0 || i0 >= p.V1) ? 0 : i0;
         [[maybe_unused]] float lp = 0.f;
-        if constexpr (SCORED) {   // l of this row: NaN where the label is 0 by the non-finite rule
+        if constexpr (BS) {   // l of the unboosted row; -(log ts - 0) is -log ts bit for bit when the winner is the maximum
+          const float ts = fold16([&](int r, float& v, float& sk) {
+            v = reinterpret_cast<const float*>(&bss->best_m[par][r][0])[u];
+            sk = reinterpret_cast<const float*>(&sc.best_s[par][r][0])[u];
+          }, zmax, NU, lane);
+          lp = (i0 < 0 || i0 >= p.V1 || !(v0 > -INFINITY)) ? __int_as_float(0x7fffffff) : -(logf(ts) - (z0 - zmax));
+        } else if constexpr (SCORED) {   // l of this row: NaN where the label is 0 by the non-finite rule
           const float ts = fold16([&](int r, float& v, float& sk) {
             v = reinterpret_cast<const float*>(&s.best_v[par][r][0])[u];
             sk = reinterpret_cast<const float*>(&sc.best_s[par][r][0])[u];
@@ -720,6 +875,16 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
           if ((emit_m >> u) & 1) eg[hh] = __ldg(p.emb_gates + static_cast<size_t>(s.ctl.label[u]) * G + eg_off);
         }
       }
+      if constexpr (BOOST) {   // the next joint reads the new slices after the __syncthreads that follows the hid4 build
+        if (warp >= kStage0 && emit_m != 0) {
+          if (warp == kStage0 && lane < NU && ((emit_m >> lane) & 1)) {
+            const int q = __ldg(p.boost.next + static_cast<size_t>(s_q[lane]) * p.V1 + s.ctl.label[lane]);
+            s_q[lane] = q >= 0 && q < p.boost.n_states ? q : 0;
+          }
+          ptx::named_bar_sync<kStageThreads>(1);
+          stage(static_cast<unsigned>(emit_m));
+        }
+      }
       DBG_T(12);
     }
     // ---- end of the group: a fresh call writes the outputs of every row, a resume call those of the streams it advanced and
@@ -736,6 +901,9 @@ __global__ void __launch_bounds__(kThreads, 1) rnnt_cluster_kernel(const RnntClP
           if constexpr (SCORED) { st->path = sc.path[lane]; st->rows = sc.rows[lane]; }
         }
       }
+    }
+    if constexpr (BOOST) {   // warp kStage0 is the last writer of q
+      if (p.io.state && rank == 0 && warp == kStage0 && lane < NU && ((act0 >> lane) & 1)) state_of(p, group * p.nu + lane)->boost_state = s_q[lane];
     }
     if (p.io.state && tid < NU * kHS) {   // every CTA stores its own units of h, c and pg
       const int u = tid / kHS, j = tid % kHS, k = rank * kHS + j;
@@ -760,7 +928,7 @@ struct LaunchState {
   int smem_set = 0;
 };
 
-template <int NH, bool GLOB, bool SCORED>
+template <int NH, bool GLOB, bool SCORED, bool BOOST>
 int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, int* plan, cudaStream_t s) {
   static LaunchState per_device[64];   // function attributes and cluster occupancy are per device
   int dev_index = 0;
@@ -768,7 +936,7 @@ int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, int* plan, cudaStrea
   LaunchState& st = per_device[dev_index & 63];
   const int cls_per = (V1 + kCl - 1) / kCl;
   const int cls_pad = (cls_per + 3) & ~3;
-  const int fixed = fixed_smem_bytes<NH, SCORED>() + cls_pad * 4;
+  const int fixed = smem_before_rows<NH, SCORED, BOOST>(cls_pad);
   int rows_smem = (smem_cap - fixed) / (kWoPitch * 4);
   if (rows_smem < 0) return 1;
   if (rows_smem > cls_per) rows_smem = cls_per;
@@ -786,15 +954,15 @@ int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, int* plan, cudaStrea
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   if (st.max_clusters < 0 || smem > st.smem_set) {
-    if (cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-        cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
+    if (cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED, BOOST>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
+        cudaFuncSetAttribute(rnnt_cluster_kernel<NH, GLOB, SCORED, BOOST>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
       cudaGetLastError();
       st.max_clusters = 0;
     } else {
       st.smem_set = smem;
       cfg.gridDim = dim3(kCl);
       int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, rnnt_cluster_kernel<NH, GLOB, SCORED>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+      if (cudaOccupancyMaxActiveClusters(&n, rnnt_cluster_kernel<NH, GLOB, SCORED, BOOST>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
       st.max_clusters = n;
     }
   }
@@ -812,7 +980,7 @@ int launch_nh(RnntClParams& p, int B, int V1, int smem_cap, int* plan, cudaStrea
     const int v[7] = {NH, GLOB ? 1 : 0, rows_smem, cls_per, nu, p.num_groups, nclusters};
     for (int i = 0; i < 7; ++i) plan[i] = v[i];
   }
-  if (cudaLaunchKernelEx(&cfg, rnnt_cluster_kernel<NH, GLOB, SCORED>, p) != cudaSuccess) return -2;
+  if (cudaLaunchKernelEx(&cfg, rnnt_cluster_kernel<NH, GLOB, SCORED, BOOST>, p) != cudaSuccess) return -2;
   return 0;
 }
 
@@ -827,10 +995,22 @@ extern "C" int gam_rnnt_debug_read(long long* out16) {
 // returns 0 on success, 1 if the shape is unsupported (pred_hidden != 320) or a 16-CTA cluster cannot be scheduled on
 // this device, negative on a launch error.  plan (host, 7 ints, or NULL) receives the launch that was chosen:
 // NH, GLOB, class rows per CTA in shared memory, classes per CTA, utterances per group, groups, clusters launched.
-// io.token_logp (or NULL: the unscored kernel) selects the scored instantiation.
+// groups of up to 4 utterances (NH = 1) or 8, and whether some class rows have to stay in L2 (GLOB)
+template <bool SCORED, bool BOOST>
+int launch_sb(RnntClParams& p, bool small, int B, int V1, int cap, int* plan, cudaStream_t s) {
+  const int cls_per = (V1 + kCl - 1) / kCl, cls_pad = (cls_per + 3) & ~3;
+  if (small) {
+    const bool glob = (cap - smem_before_rows<1, SCORED, BOOST>(cls_pad)) / (kWoPitch * 4) < cls_per;
+    return glob ? launch_nh<1, true, SCORED, BOOST>(p, B, V1, cap, plan, s) : launch_nh<1, false, SCORED, BOOST>(p, B, V1, cap, plan, s);
+  }
+  const bool glob = (cap - smem_before_rows<2, SCORED, BOOST>(cls_pad)) / (kWoPitch * 4) < cls_per;
+  return glob ? launch_nh<2, true, SCORED, BOOST>(p, B, V1, cap, plan, s) : launch_nh<2, false, SCORED, BOOST>(p, B, V1, cap, plan, s);
+}
+
+// io.token_logp (or NULL: the unscored kernel) selects the scored instantiation, boost (or NULL) the boosted one.
 int launch_rnnt_greedy(const float* encproj, const float* emb_gates, const float* whhT, const float* wpT, const float* bp,
                        const float* wo, const float* bo, int B, int T, int H, int V1, int blank, int max_symbols, const GreedyIo& io,
-                       int* plan, cudaStream_t s) {
+                       const BoostGraph* boost, int* plan, cudaStream_t s) {
   if (H != kH) return 1;
   struct DeviceLimits {
     int smem_cap = 0, clusters_hint = 0;
@@ -852,19 +1032,12 @@ int launch_rnnt_greedy(const float* encproj, const float* emb_gates, const float
   p.encproj = encproj; p.emb_gates = emb_gates; p.whhT = whhT; p.wpT = wpT; p.bp = bp; p.wo = wo; p.bo = bo;
   p.B = B; p.T = T; p.V1 = V1; p.blank = blank; p.max_symbols = max_symbols;
   p.io = io;
+  p.boost = boost ? *boost : BoostGraph{};
   // groups of up to 4 utterances while every group still gets its own cluster, else groups of up to 8
-  const int cls_per = (V1 + kCl - 1) / kCl;
   const bool small = B <= 4 * lim.clusters_hint;
-  const int fixed = (scored ? (small ? fixed_smem_bytes<1, true>() : fixed_smem_bytes<2, true>())
-                            : (small ? fixed_smem_bytes<1, false>() : fixed_smem_bytes<2, false>())) + ((cls_per + 3) & ~3) * 4;
-  const bool glob = (lim.smem_cap - fixed) / (kWoPitch * 4) < cls_per;   // some class rows have to stay in L2
   const int cap = lim.smem_cap;
-  if (scored) {
-    if (small) return glob ? launch_nh<1, true, true>(p, B, V1, cap, plan, s) : launch_nh<1, false, true>(p, B, V1, cap, plan, s);
-    return glob ? launch_nh<2, true, true>(p, B, V1, cap, plan, s) : launch_nh<2, false, true>(p, B, V1, cap, plan, s);
-  }
-  if (small) return glob ? launch_nh<1, true, false>(p, B, V1, cap, plan, s) : launch_nh<1, false, false>(p, B, V1, cap, plan, s);
-  return glob ? launch_nh<2, true, false>(p, B, V1, cap, plan, s) : launch_nh<2, false, false>(p, B, V1, cap, plan, s);
+  if (boost) return scored ? launch_sb<true, true>(p, small, B, V1, cap, plan, s) : launch_sb<false, true>(p, small, B, V1, cap, plan, s);
+  return scored ? launch_sb<true, false>(p, small, B, V1, cap, plan, s) : launch_sb<false, false>(p, small, B, V1, cap, plan, s);
 }
 
 }  // namespace gam

@@ -4,8 +4,9 @@ RNN-T prediction/joint loop run on the device, then one D2H copy brings ids / fr
 host-side detokenisation (which the reference also does on the host, decoding.py:93-96,207)."""
 from __future__ import annotations
 
-from typing import List, Optional, Tuple
+from typing import List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 from torch import Tensor
 
@@ -171,6 +172,64 @@ def rnnt_loss(head, encoded: Tensor, encoded_len: Tensor, targets: Tensor, targe
     if reduction == "mean":
         return loss.mean()
     return loss.sum() if reduction == "sum" else loss
+
+
+BOOST_MAX_STATES = 65536   # kBoostMaxStates of csrc/kernels.h
+
+
+def boost_graph(phrases: Sequence[Sequence[int]], weight: float, anchor: Optional[int], V1: int, blank: int
+                ) -> Tuple[Tensor, Tensor]:
+    """The boost graph of `phrases` (token-id sequences) for gam_rnnt_greedy_boost: (next int32 [S, V1], bonus float32 [S, V1])
+    on the host, state 0 initial (include/gigaam_b200.h and INTEGRATION.md §7j have the definition).
+
+    Each phrase is a pattern; with `anchor` (the space token of a charwise vocabulary, else None) it is prefixed by the
+    anchor, so that a match can only start at a word start.  The states are all prefixes of all patterns, the empty one
+    included; state 0 is the anchor's (the start of a transcript is a word start), or the empty prefix without an anchor.
+    next(s, v) is the longest suffix of s.v that is a state (Aho-Corasick), and bonus(s, v) = fp32(weight) when next(s, v)
+    ends in a phrase token (it is neither empty nor the bare anchor), else 0.  Blank gets no bonus and does not move the
+    state.  Duplicate phrases are merged.
+
+    There is deliberately no penalty for abandoning a partial match, as some beam-search boosters take back the bonus of a
+    failed match: greedy decisions never compare accumulated totals, so such a penalty would only make the decoder hold on to
+    a wrong partial match, and that costs deletions.
+
+    Raises ValueError for a weight that is not finite and > 0 in fp32, and for a graph of more than 65 536 states."""
+    with np.errstate(over="ignore"):
+        w = np.float32(weight)
+    if not (np.isfinite(w) and w > 0):
+        raise ValueError(f"boost: weight={weight} must be finite and > 0 (in fp32)")
+    pats = {tuple(([] if anchor is None else [int(anchor)]) + [int(t) for t in p]) for p in phrases}
+    prefixes = {p[:k] for p in pats for k in range(len(p) + 1)}
+    if len(prefixes) > BOOST_MAX_STATES:
+        raise ValueError(f"boost: the phrases make a graph of {len(prefixes)} states, more than {BOOST_MAX_STATES}")
+    start = () if anchor is None else (int(anchor),)
+    # states by length (the initial one first): a state's suffix link is shorter, so its row is complete when it is copied
+    order = sorted(prefixes - {start}, key=lambda t: (len(t), t))
+    order.insert(0, start)
+    idx = {t: i for i, t in enumerate(order)}
+    children: dict = {}
+    for t in order:
+        if t:
+            children.setdefault(t[:-1], []).append(t)
+    S = len(order)
+    nxt = np.zeros((S, V1), dtype=np.int32)
+    link = {}
+    root = idx[()]
+    for t in sorted(order, key=len):        # Aho-Corasick: the row of t is its suffix link's row, with t's children over it
+        i = idx[t]
+        if len(t) == 0:
+            nxt[i] = i
+        else:
+            link[t] = root if len(t) == 1 else int(nxt[link[t[:-1]], t[-1]])
+            nxt[i] = nxt[link[t]]
+        for c in children.get(t, ()):
+            nxt[i, c[-1]] = idx[c]
+    # a bonus where the next state ends in a phrase token: neither the empty prefix nor the bare anchor
+    ends_in_phrase = np.array([len(t) > len(start) or (anchor is None and len(t) > 0) for t in order], dtype=bool)
+    bonus = np.where(ends_in_phrase[nxt], w, np.float32(0)).astype(np.float32)
+    bonus[:, blank] = 0
+    nxt[:, blank] = np.arange(S, dtype=np.int32)
+    return torch.from_numpy(nxt), torch.from_numpy(bonus)
 
 
 def spot(head, encoded: Tensor, encoded_len: Tensor, keywords: Tensor, keyword_len: Tensor, threshold: float, max_det: int

@@ -602,10 +602,12 @@ class Engine:
                             frame_rows=torch.zeros((B, n_frames), **i32))
 
     def greedy_resume(self, enc_btd: Tensor, lo: Tensor, hi: Tensor, frame_base: Tensor, state: Tensor, out: "DecodeBuffers",
-                      scores: bool = False) -> None:
+                      scores: bool = False, boost: Optional[Tuple[Tensor, Tensor]] = None) -> None:
         """Decode frames [lo[b], hi[b]) of enc [B, T, d] (f32 contiguous) continuing stream b of `state` (decode_state) and
         append to `out` (decode_buffers, emitted frames frame_base[b] + t).  lo / hi / frame_base: device int32 [B].  Decoding
-        an utterance in consecutive ranges gives `greedy`'s bits (include/gigaam_b200.h, gam_ctc_greedy_resume)."""
+        an utterance in consecutive ranges gives `greedy`'s bits (include/gigaam_b200.h, gam_ctc_greedy_resume).  `boost`:
+        a boost graph's device tables (next int32 [S, V+1], bonus f32 [S, V+1], decoding.boost_graph) steer an RNN-T decoder
+        (gam_rnnt_greedy_boost); None runs gam_*_greedy_resume."""
         assert enc_btd.is_cuda and enc_btd.dtype == torch.float32 and enc_btd.is_contiguous() and enc_btd.dim() == 3
         B, T, _ = enc_btd.shape
         for t in (lo, hi, frame_base):
@@ -618,8 +620,15 @@ class Engine:
         ws = self._ws_dec.get(("resume", B, T), int(self.lib.gam_decode_resume_workspace_bytes(self.handle, B, T)), self.device)
         sc = [out.token_logp, out.path_logp, out.path_rows, out.frame_logp, out.frame_rows] if scores else [None] * 5
         pitch = out.frame_logp.shape[1] if scores else 0
-        self._call("gam_ctc_greedy_resume" if self.head_type == 1 else "gam_rnnt_greedy_resume", enc_btd, B, T, lo, hi, frame_base, state,
-                   ws, ws.numel(), out.ids, out.frames, out.counts, out.ids.shape[1], *sc, pitch)
+        args = (enc_btd, B, T, lo, hi, frame_base, state, ws, ws.numel(), out.ids, out.frames, out.counts, out.ids.shape[1], *sc, pitch)
+        if boost is not None:
+            nxt, bonus = boost
+            assert nxt.shape == bonus.shape and nxt.dim() == 2 and nxt.shape[1] == self.num_classes
+            assert nxt.dtype == torch.int32 and bonus.dtype == torch.float32 and nxt.is_contiguous() and bonus.is_contiguous()
+            assert nxt.device == bonus.device == self.device
+            self._call("gam_rnnt_greedy_boost", *args, nxt, bonus, nxt.shape[0])
+            return
+        self._call("gam_ctc_greedy_resume" if self.head_type == 1 else "gam_rnnt_greedy_resume", *args)
 
     def ctc_log_probs(self, enc_btd: Tensor) -> Tensor:
         """enc [B, T, d] f32 contiguous -> log_probs [B, T, V+1] f32 (CTCHead.forward, gigaam/decoder.py:18-21)."""

@@ -224,14 +224,15 @@ def stitch_ctc_log_probs(model, wav: Tensor, windows: Sequence[Window], T: int, 
 
 
 def decode_windows(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16, scores: bool = False,
-                   log_probs: Optional[Tensor] = None):
+                   log_probs: Optional[Tensor] = None, boost: Optional[Tuple[Tensor, Tensor]] = None):
     """Greedy-decode a whole recording of T encoder frames as one utterance: `window_batches` encodes the windows, and each
     window's kept frames are decoded in window order, resuming the previous window's decoder state on the device
     (Engine.greedy_resume).  Only one batch of encoder output is alive at a time.  Returns the Engine.DecodeBuffers of the
     one stream: ids / frames [1, max_out] (global frames), counts [1] and, with `scores`, token_logp, path_logp, path_rows and
     the per-frame frame_logp / frame_rows [1, T].  max_out = Engine.hyp_width(T), so the buffers never overflow.
     `log_probs` (CTC, f32 [1, T, V+1] on the device): also filled with the stitched log-probs of `stitch_ctc_log_probs`,
-    from the same encoder pass."""
+    from the same encoder pass.  `boost` (RNN-T, device tables of decoding.boost_graph) steers every window's decoding, the
+    graph state carried in the decoder record."""
     from .decoding import _as_btd
     eng = model._get_engine()
     index = {w: i for i, w in enumerate(windows)}
@@ -244,7 +245,7 @@ def decode_windows(model, wav: Tensor, windows: Sequence[Window], T: int, batch_
         enc = _as_btd(encoded)
         for row, w in enumerate(group):
             i = index[w]
-            eng.greedy_resume(enc[row:row + 1], ranges[0, i:i + 1], ranges[1, i:i + 1], ranges[2, i:i + 1], state, out, scores)
+            eng.greedy_resume(enc[row:row + 1], ranges[0, i:i + 1], ranges[1, i:i + 1], ranges[2, i:i + 1], state, out, scores, boost)
         if log_probs is not None:
             lp = model.head(encoded)
             for row, w in enumerate(group):

@@ -269,14 +269,19 @@ class GigaAMASR(GigaAM):
 
     @torch.inference_mode()
     def transcribe(self, wav_file, word_timestamps: bool = False, confidence: bool = False,
-                   hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None, hotword_threshold: float = 0.5
+                   hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None, hotword_threshold: float = 0.5,
+                   boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0
                    ) -> TranscriptionResult:
         """gigaam/model.py:126-140.  `confidence=True` decodes with the scored kernels (the same text and words) and fills
         `confidence` of the result, and of every word when word timestamps are on (INTEGRATION.md, "Confidence").
         `hotwords` (CTC models only): names or terms that replace the greedy words they outscore by `hotword_threshold`
-        (INTEGRATION.md §7h); None decodes exactly as without them."""
+        (INTEGRATION.md §7h); None decodes exactly as without them.  `boost` (RNN-T models only): names or terms whose
+        tokens get `boost_weight` nats added to their logits while the greedy decoder follows them (INTEGRATION.md §7j);
+        scores stay the model's own.  None decodes exactly as without it."""
         if hotwords is not None:
             return self._transcribe_hotwords(wav_file, word_timestamps, confidence, hotwords, hotword_threshold)
+        if boost is not None:
+            return self._transcribe_boost(wav_file, word_timestamps, confidence, boost, boost_weight)
         wav, length = self.prepare_wav(wav_file)
         if length.item() > LONGFORM_THRESHOLD:
             raise ValueError("Too long wav file, use 'transcribe_longform' method.")
@@ -480,7 +485,8 @@ class GigaAMASR(GigaAM):
     @torch.inference_mode()
     def transcribe_windowed(self, wav_file, word_timestamps: bool = False, confidence: bool = False, window: float = 30.0,
                             overlap: float = 4.0, batch_size: int = 16, pause: float = 1.0, max_segment: float = 25.0,
-                            hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None, hotword_threshold: float = 0.5):
+                            hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None, hotword_threshold: float = 0.5,
+                            boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0):
         """Transcribe a recording of any length without a VAD (INTEGRATION.md §7f).  The encoder runs over overlapping
         windows (`longform.plan_windows`), and the greedy decoder runs over the windows' kept frames as ONE utterance: each
         window is decoded as soon as its batch is encoded, resuming the decoder state of the window before it
@@ -490,11 +496,13 @@ class GigaAMASR(GigaAM):
         recording.  Raises ValueError before any device work for the window plan's refusals, batch_size < 1, pause < 0 and
         max_segment <= 0.  `hotwords` as in `transcribe` (CTC models only): the windows' log-probs are also stitched into one
         [T, V+1] sequence from the same encoder pass, and the hotwords are applied to the whole recording before it is cut into
-        segments."""
+        segments.  `boost` and `boost_weight` as in `transcribe` (RNN-T models only): every window's decoding is boosted, the
+        graph state carried across windows with the decoder's."""
         from .longform import decode_windows, plan_windows, segment_cuts, windowed_segments
         from .timestamps_utils import compute_frame_shift, words_from_device
         from .types import LongformTranscriptionResult
         kw_ids = None if hotwords is None else self._hotword_ids(hotwords, hotword_threshold, "transcribe_windowed")
+        tables = None if boost is None else self._boost_tables(boost, boost_weight, "transcribe_windowed")
         if isinstance(wav_file, str):
             wav = load_audio(wav_file)
         else:
@@ -510,7 +518,9 @@ class GigaAMASR(GigaAM):
         N = wav.numel()
         host = wav.to(self._dtype).pin_memory()          # the rounding of prepare_wav; uploaded one batch at a time
         eng = self._get_engine()
-        if kw_ids is None:
+        if tables is not None:
+            out = decode_windows(self, host, windows, T, batch_size, confidence, boost=tuple(t.to(eng.device) for t in tables))
+        elif kw_ids is None:
             out = decode_windows(self, host, windows, T, batch_size, confidence)
         else:
             lp = torch.empty((1, T, eng.num_classes), dtype=torch.float32, device=eng.device)
@@ -536,13 +546,16 @@ class GigaAMASR(GigaAM):
         return LongformTranscriptionResult(segments=segs)
 
     def streaming(self, window: float = 8.0, overlap: float = 4.0, batch_size: int = 64, confidence: bool = False,
-                  keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5):
+                  keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5,
+                  boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0):
         """A `streaming.StreamServer` for live audio (INTEGRATION.md §7i): open streams, push chunks, `step()` for captions
-        and keyword alerts, `close()` for each stream's `transcribe_windowed` / `spot` result.  Raises before any device
-        work: ValueError for the window plan's refusals, batch_size < 1 and `spot`'s keyword and threshold checks;
-        NotImplementedError for keywords on an RNN-T model."""
+        and keyword alerts, `close()` for each stream's `transcribe_windowed` / `spot` result.  `boost` and `boost_weight` as
+        in `transcribe` (RNN-T models only), for every stream of the server.  Raises before any device work: ValueError for
+        the window plan's refusals, batch_size < 1, `spot`'s keyword and threshold checks and `boost`'s checks;
+        NotImplementedError for keywords on an RNN-T model and for boost on a CTC model."""
         from .streaming import StreamServer
-        return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold)
+        tables = None if boost is None else self._boost_tables(boost, boost_weight, "streaming")
+        return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold, boost=tables)
 
     # ---- keyword spotting (INTEGRATION.md §7g)
     def _refuse_rnnt_spot(self, what: str) -> None:
@@ -551,34 +564,41 @@ class GigaAMASR(GigaAM):
                                       "[T, U + 1] lattice, so there is nothing to search; use a *_ctc model")
 
     def _keyword_ids(self, keywords: Sequence[Union[str, Sequence[int]]], threshold: float) -> Tuple[List[str], List[List[int]]]:
-        """Each keyword's text and token ids, checked before any device work: a string is normalised and tokenised by
+        """Each keyword's text and token ids (`_phrase_ids`), then the threshold, checked before any device work: ValueError
+        also for a threshold outside (0, 1] (in fp32)."""
+        names, ids = self._phrase_ids(keywords, "spot", "keyword")
+        if not 0.0 < float(np.float32(threshold)) <= 1.0:
+            raise ValueError(f"spot: threshold={threshold} outside (0, 1]")
+        return names, ids
+
+    def _phrase_ids(self, phrases: Sequence[Union[str, Sequence[int]]], what: str, noun: str) -> Tuple[List[str], List[List[int]]]:
+        """Each phrase's text and token ids, checked before any device work: a string is normalised and tokenised by
         `Tokenizer.encode` (as `align` does), a sequence of ids is taken as it is.  Raises ValueError for an empty list, a
-        keyword without tokens, more than 64 tokens, an id outside [0, V) and a threshold outside (0, 1] (in fp32)."""
+        phrase without tokens, more than 64 tokens and an id outside [0, V); messages start with `what` and name the phrase
+        a `noun`."""
         tok = self.decoding.tokenizer
         V = len(tok)
-        kws = [keywords] if isinstance(keywords, str) else list(keywords)
+        kws = [phrases] if isinstance(phrases, str) else list(phrases)
         if not kws:
-            raise ValueError("spot: no keywords")
+            raise ValueError(f"{what}: no {noun}s")
         names, ids = [], []
         for kw in kws:
             if isinstance(kw, str):
                 row = tok.encode(kw)
                 if not row:
-                    raise ValueError(f"spot: keyword {kw!r} normalises to no tokens")
+                    raise ValueError(f"{what}: {noun} {kw!r} normalises to no tokens")
                 names.append(tok.normalize(kw))
             else:
                 row = [int(i) for i in kw]
                 bad = [i for i in row if not 0 <= i < V]
                 if bad:
-                    raise ValueError(f"spot: token id {bad[0]} outside [0, {V})")
+                    raise ValueError(f"{what}: token id {bad[0]} outside [0, {V})")
                 if not row:
-                    raise ValueError("spot: a keyword without tokens")
+                    raise ValueError(f"{what}: a {noun} without tokens")
                 names.append(tok.decode(row))
             if len(row) > SPOT_MAX_TOKENS:
-                raise ValueError(f"spot: keyword {names[-1]!r} has {len(row)} tokens, more than {SPOT_MAX_TOKENS}")
+                raise ValueError(f"{what}: {noun} {names[-1]!r} has {len(row)} tokens, more than {SPOT_MAX_TOKENS}")
             ids.append(row)
-        if not 0.0 < float(np.float32(threshold)) <= 1.0:
-            raise ValueError(f"spot: threshold={threshold} outside (0, 1]")
         return names, ids
 
     @staticmethod
@@ -685,6 +705,50 @@ class GigaAMASR(GigaAM):
                 raise ValueError(f"{what}: hotword {tok.decode(row)!r} starts or ends with the space token; hotwords are "
                                  "spliced at word boundaries only, so pass the word without its spaces")
         return ids
+
+    # ---- phrase boosting (INTEGRATION.md §7j)
+    def _boost_tables(self, phrases: Sequence[Union[str, Sequence[int]]], weight: float, what: str) -> Tuple[Tensor, Tensor]:
+        """The host tables of the boost graph of `phrases` (decoding.boost_graph), checked before any device work: CTC
+        models raise NotImplementedError; `spot`'s phrase checks, a phrase that starts or ends with the space token, a weight
+        that is not finite and > 0 and a graph of more than 65 536 states raise ValueError.  A charwise vocabulary anchors
+        every phrase at a word start (its space token); SentencePiece pieces open their words themselves."""
+        from .decoding import boost_graph
+        if self._ncfg["head"].get("type") != "rnnt":
+            raise NotImplementedError(f"{what}: boost steers the RNN-T greedy decoder; for a CTC model use hotwords=, which "
+                                      "splices spotted phrases into the transcript")
+        _, ids = self._phrase_ids(phrases, what, "phrase")
+        tok = self.decoding.tokenizer
+        for row in ids:
+            if any(tok.id_to_str(row[i]) == " " for i in (0, -1)):
+                raise ValueError(f"{what}: phrase {tok.decode(row)!r} starts or ends with the space token; a phrase is "
+                                 "anchored at a word start by itself, so pass the words without edge spaces")
+        anchor = tok.vocab.index(" ") if tok.charwise and " " in tok.vocab else None
+        return boost_graph(ids, weight, anchor, len(tok) + 1, len(tok))
+
+    def _transcribe_boost(self, wav_file, word_timestamps: bool, confidence: bool, boost, weight: float) -> TranscriptionResult:
+        """`transcribe` with phrase boosting: encode, then one boosted decoding call from a fresh record, then the usual
+        formatting."""
+        from .timestamps_utils import path_confidence
+        tables = self._boost_tables(boost, weight, "transcribe")
+        wav, length = self.prepare_wav(wav_file)
+        if length.item() > LONGFORM_THRESHOLD:
+            raise ValueError("Too long wav file, use 'transcribe_longform' method.")
+        encoded, encoded_len = self.forward(wav, length)
+        eng = self._get_engine()
+        enc = _as_btd(encoded.to(dtype=torch.float32))
+        T = enc.shape[1]
+        zero = torch.zeros(1, dtype=torch.int32, device=eng.device)
+        out = eng.decode_buffers(1, eng.hyp_width(T), T, scores=confidence)
+        eng.greedy_resume(enc, zero, encoded_len.to(device=eng.device, dtype=torch.int32), zero, eng.decode_state(1), out, confidence,
+                          tuple(t.to(eng.device) for t in tables))
+        conf = path_confidence(float(out.path_logp[0]), int(out.path_rows[0])) if confidence else None
+        if not word_timestamps:
+            n = int(out.counts[0])
+            return TranscriptionResult(text=self.decoding.tokenizer.decode(out.ids[0, :n].tolist()), words=None, confidence=conf)
+        rec = eng.group_words(out.ids, out.frames, out.counts, self._word_flags())
+        text, words = self._words_from_records(out.ids.cpu(), out.counts.cpu(), encoded_len.cpu(), length.cpu(),
+                                               [t.cpu() for t in rec], out.token_logp.cpu() if confidence else None)[0]
+        return TranscriptionResult(text=text, words=words, confidence=conf)
 
     def _apply_hotwords(self, lp: Tensor, enc_len: Tensor, ids: List[List[int]], threshold: float, g_ids: Tensor, g_frames: Tensor,
                         g_counts: Tensor, token_logp: Optional[Tensor] = None, path_logp: Optional[Tensor] = None,

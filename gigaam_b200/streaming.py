@@ -118,10 +118,13 @@ class StreamServer:
         res = srv.close(a, word_timestamps=True)
 
     A closed stream's result is `transcribe_windowed(recording, word_timestamps, confidence, window, overlap, pause=pause,
-    max_segment=max_segment)` and, with keywords, `spot(recording, keywords, threshold, window, overlap)`, bit for bit."""
+    max_segment=max_segment)` (with the server's `boost` and `boost_weight`) and, with keywords, `spot(recording, keywords,
+    threshold, window, overlap)`, bit for bit.  `boost`: the tables of a boost graph (GigaAMASR._boost_tables, moved to the
+    device with the first stream) that steer every stream's decoding, committed and tentative."""
 
     def __init__(self, model, window: float = 8.0, overlap: float = 4.0, batch_size: int = 64, confidence: bool = False,
-                 keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5):
+                 keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5,
+                 boost: Optional[Tuple[Tensor, Tensor]] = None):
         max_frames = model.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
         self.W = _frame_multiple(window, "window")
         self.V = _frame_multiple(overlap, "overlap")
@@ -137,6 +140,7 @@ class StreamServer:
             self.names, self.kw_ids = model._keyword_ids(keywords, threshold)
         self.model, self.window, self.overlap = model, window, overlap
         self.batch_size, self.confidence, self.threshold = int(batch_size), bool(confidence), threshold
+        self.boost = boost
         self._openers = set(torch.nonzero(token_flag_table(model.decoding.tokenizer) & 3).reshape(-1).tolist())
         self._streams: Dict[int, _Stream] = {}
         self._next_id = 0
@@ -164,6 +168,8 @@ class StreamServer:
         if self._eng is None:
             eng = self._eng = self.model._get_engine()
             self._fresh_dec = eng.decode_state(1)
+            if self.boost is not None:
+                self.boost = tuple(t.to(eng.device) for t in self.boost)
             if self.kw_ids:
                 self._kw, self._kw_len = self.model._keyword_tensors(self.kw_ids, eng.device)
                 self._fresh_spot = eng.spot_state(1, len(self.kw_ids), self._kw.shape[1])
@@ -262,7 +268,7 @@ class StreamServer:
         slots = torch.tensor([s.slot for s, _ in sel], device=dev)
         state = self._dec_pool.index_select(0, slots)
         out = eng.decode_buffers(len(sel), eng.hyp_width(T_w), T_w, scores=self.confidence)
-        eng.greedy_resume(enc, rng[0], rng[1], rng[2], state, out, self.confidence)
+        eng.greedy_resume(enc, rng[0], rng[1], rng[2], state, out, self.confidence, self.boost)
         self._dec_pool.index_copy_(0, slots, state)
         spot = None
         if lp is not None:
@@ -317,7 +323,7 @@ class StreamServer:
         rng = torch.tensor([lo, [T_w] * len(sel), [0] * len(sel)], dtype=torch.int32).to(dev)
         state = self._dec_pool.index_select(0, torch.tensor([s.slot for s, _ in sel], device=dev))
         out = eng.decode_buffers(len(sel), eng.hyp_width(T_w))
-        eng.greedy_resume(enc, rng[0], rng[1], rng[2], state, out)
+        eng.greedy_resume(enc, rng[0], rng[1], rng[2], state, out, boost=self.boost)
 
         def read():
             ids, counts = out.ids.cpu(), out.counts.cpu()

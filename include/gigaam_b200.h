@@ -235,6 +235,29 @@ int gam_rnnt_greedy_resume(gam_handle* h, const float* enc, int32_t B, int32_t T
                            int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
                            double* frame_logp, int32_t* frame_rows, int64_t frame_pitch, void* stream);
 
+/* Phrase boosting for RNN-T greedy decoding: gam_rnnt_greedy_resume steered by a boost graph (GigaAMASR.transcribe(boost=)).
+ *
+ * A boost graph is a dense automaton over the vocabulary: S states (1 <= S <= 65 536), boost_next device i32 [S, V1] and
+ * boost_bonus device f32 [S, V1] (V1 = V + 1 columns, blank included); state 0 is the initial state.  Stream b is in one
+ * state q, kept in its decoding record (bytes the RNN-T decoder does not otherwise use; gam_decode_state_init's zeros are
+ * state 0, so the record keeps its size).
+ *   - At every decision row in state q the label is the greedy rule (first maximal index; label 0 on a row with a NaN or +inf
+ *     value or only -inf values) applied to fp32(z_v + bonus[q, v]) instead of z_v.  The blank column is ignored: blank gets
+ *     no bonus, and emitting blank does not change q.
+ *   - On emitting token v, q becomes boost_next[q, v]; an entry outside [0, S) sends the stream to state 0.
+ *   - Scores stay the model's own: token_logp, path_logp / path_rows and frame_logp / frame_rows are log_softmax(z)[label] of
+ *     the unboosted row (NaN by the unboosted rule where the label is 0 by the non-finite rule).  With finite bonuses a row with
+ *     a non-finite logit decides as it does without boosting.
+ *   - With every bonus 0, every output and the record outside q are bit-identical to gam_rnnt_greedy_resume's.
+ * Arguments, scoring (token_logp non-NULL), workspace and the chunking rule are gam_rnnt_greedy_resume's; q is carried across
+ * chunks in the record.  Refused: a model without an RNN-T head, NULL tables, S outside [1, 65 536], and everything the resume
+ * call refuses.  The tables take S * V1 * 8 bytes; each CTA keeps its class slice of bonus[q] per utterance in shared memory. */
+int gam_rnnt_greedy_boost(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi,
+                          const int32_t* frame_base, void* state, void* workspace, int64_t workspace_bytes, int32_t* ids,
+                          int32_t* frames, int32_t* counts, int32_t max_out, float* token_logp, float* path_logp, int32_t* path_rows,
+                          double* frame_logp, int32_t* frame_rows, int64_t frame_pitch, const int32_t* boost_next,
+                          const float* boost_bonus, int32_t n_states, void* stream);
+
 /* ---- the heads' forward passes, for callers that run their own search (LM beam search, N-best rescoring, forced
  * alignment, lattice scoring).  fp32 CUDA-core arithmetic like the reference's heads; no workspace except for the joint.
  *
@@ -719,6 +742,14 @@ int gam_test_rnnt_greedy_scored(gam_handle* h, const float* encproj, const int32
                                 const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
                                 int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts,
                                 float* token_logp, float* path_logp, int32_t* path_rows, int32_t* plan, void* stream);
+/* gam_rnnt_greedy_boost's kernel on caller weights, a fresh call over [0, len[b]) as gam_test_rnnt_greedy (scored when
+ * token_logp is non-NULL, which then needs path_logp and path_rows); plan as there, its class rows per CTA in shared memory
+ * already net of the bonus slices */
+int gam_test_rnnt_greedy_boost(gam_handle* h, const float* encproj, const int32_t* len, const float* emb_gates, const float* whhT,
+                               const float* wpT, const float* bp, const float* wo, const float* bo, int32_t B, int32_t T, int32_t V1,
+                               int32_t max_symbols, int32_t max_out, int32_t* ids, int32_t* frames, int32_t* counts, float* token_logp,
+                               float* path_logp, int32_t* path_rows, const int32_t* boost_next, const float* boost_bonus,
+                               int32_t n_states, int32_t* plan, void* stream);
 /* gam_ctc_align_long with the cluster size forced to cluster_ctas (0: the library's choice), so that CTA boundaries can be
  * placed with few states; a C that leaves a CTA without states is refused.  plan (host i32 [2], or NULL) receives C and the
  * states per CTA. */
