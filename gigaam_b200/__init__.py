@@ -19,13 +19,13 @@ import torch
 
 from .engine import max_encoded_frames_config
 from .model import GigaAM, GigaAMASR, GigaAMEmo, check_emo_head
-from .preprocess import load_audio
+from .preprocess import load_audio, read_audio
 from .synthetic import synthetic_audio, synthetic_checkpoint
 from .streaming import StreamServer
 from .types import (Alignment, Detection, LongformAlignment, LongformTranscriptionResult, Segment, StreamResult, StreamUpdate,
                     TranscriptionResult, Word)
 
-__all__ = ["GigaAM", "GigaAMASR", "GigaAMEmo", "load_audio", "load_model", "synthetic_checkpoint", "synthetic_audio",
+__all__ = ["GigaAM", "GigaAMASR", "GigaAMEmo", "load_audio", "read_audio", "load_model", "synthetic_checkpoint", "synthetic_audio",
            "TranscriptionResult", "Word", "Segment", "LongformTranscriptionResult", "Alignment",
            "LongformAlignment", "Detection", "StreamServer", "StreamUpdate", "StreamResult"]
 

@@ -1737,6 +1737,27 @@ int gam_group_words(gam_handle* h, const int32_t* ids, const int32_t* frames, co
   return 0;
 }
 
+int gam_resample(gam_handle* h, const float* x, int64_t x_pitch, int32_t B, const int64_t* spans, const float* table,
+                 int32_t table_rows, int32_t table_cols, int32_t o, int32_t n, float* y, int64_t y_pitch, void* stream) {
+  if (!h) return -1;
+  if (!x || !spans || !table || !y) return fail(h, -1, "resample: NULL pointer");
+  if (B < 1 || B > 65535) return fail(h, -1, "resample: B=%d outside [1, 65535]", B);
+  if (x_pitch < 0 || y_pitch < 0 || (y_pitch + 255) / 256 > INT32_MAX)
+    return fail(h, -1, "resample: bad row pitch (x %lld, y %lld)", (long long)x_pitch, (long long)y_pitch);
+  // w: torchaudio's ceil(lowpass_filter_width * orig / (min(orig, new) * rolloff)), in the same double operations
+  const int32_t w = (o < 1 || n < 1) ? -1 : static_cast<int32_t>(std::ceil(6.0 * o / (std::min(o, n) * 0.99)));
+  const int32_t taps = table_rows;
+  if (w < 0 || table_cols != n || taps != 2 * static_cast<int64_t>(w) + o || static_cast<int64_t>(taps) * n > (int64_t(1) << 20))
+    return fail(h, -1, "resample: a table of %d x %d does not match o=%d, n=%d (2 w + o = %lld taps x n phases, w = %d, at most 2^20 "
+                "entries)", table_rows, table_cols, o, n, 2 * static_cast<long long>(w) + o, n, w);
+  if (y_pitch == 0) return 0;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  { PROF(PC_MISC);
+    launch_resample(x, x_pitch, table, n, o, w, taps, spans, B, y, y_pitch, s); }
+  GAM_CHECK_LAUNCH(h, "resample");
+  return 0;
+}
+
 int gam_comm_unique_id(uint8_t* out128) { return comm_unique_id(out128); }
 
 int gam_comm_init(gam_handle* h, const uint8_t* id128, int32_t rank, int32_t nranks) {

@@ -108,6 +108,12 @@ void launch_ctc_collapse(const int* labels, const float* lp, int B, int T, int b
 void launch_group_words(const int* ids, const int* frames, const int* counts, const unsigned char* flags, int B, int V, int max_out,
                         int max_words, int* w_start, int* w_end, int* w_first, int* w_ntok, int* n_words, cudaStream_t s);
 
+// resample.cu: gam_resample's polyphase resampler.  table f32 [K, n] (k-major), spans i64 [4, B] = in_begin, in_end,
+// out_begin, out_end; row b of x holds samples [in_begin, in_end) and row b of y gets outputs [out_begin, out_end), both
+// from column 0.  B <= 65535.
+void launch_resample(const float* x, int64_t x_pitch, const float* table, int n, int o, int w, int K, const int64_t* spans, int B,
+                     float* y, int64_t y_pitch, cudaStream_t s);
+
 // rnnt.cu
 // C[M,N] = A[M,K] W[N,K]^T + bias (bias may be null); K % 16 == 0
 void launch_sgemm_tn_bias(const float* A, const float* W, const float* bias, float* C, int M, int N, int K, cudaStream_t s);

@@ -226,6 +226,7 @@ class Engine:
         self._ws_joint = _WorkspaceCache(self.WS_CACHE)
         self._ws_align = _WorkspaceCache(self.WS_CACHE)
         self._ws_emo = _WorkspaceCache(self.WS_CACHE)
+        self._resample_plans: Dict[int, Tuple[Tensor, int, int, int]] = {}
         self.handle = C.c_void_p()
         pre = cfg["preprocessor"]
         head = cfg.get("head") if isinstance(cfg, dict) else None
@@ -520,6 +521,67 @@ class Engine:
         else:
             self._call("gam_logmel", wav, B, N, mel)
         return mel
+
+    # ------------------------------------------------------------------ resampling to 16 kHz (INTEGRATION.md §7k)
+    def resample_plan(self, sample_rate: int) -> Tuple[Tensor, int, int, int]:
+        """(table, o, n, w) of gam_resample from `sample_rate`: the device table is preprocess.resample_table transposed to
+        [2 w + o, n], built once per rate.  ValueError for the rates preprocess.resample_ratio refuses and for 16 kHz, which
+        is not resampled."""
+        from .preprocess import SAMPLE_RATE, resample_ratio, resample_table
+        if sample_rate == SAMPLE_RATE:
+            raise ValueError("16 kHz audio is not resampled")
+        plan = self._resample_plans.get(sample_rate)
+        if plan is None:
+            o, n, w = resample_ratio(sample_rate)
+            plan = (resample_table(sample_rate).t().contiguous().to(self.device), o, n, w)
+            self._resample_plans[int(sample_rate)] = plan
+        return plan
+
+    def resample_spans(self, x: Tensor, spans: Tensor, sample_rate: int, out: Tensor) -> Tensor:
+        """gam_resample, the span form: row b of x (device f32 [B, P]) holds samples [in_begin[b], in_end[b]) of its signal,
+        and row b of out (device f32 [B, C]) gets its outputs [out_begin[b], out_end[b]) from column 0; spans = int64
+        [in_begin, in_end, out_begin, out_end] x [B].  Other columns of out are not written.  Host spans are checked first
+        (ValueError for an inverted range, a negative out_begin, or more samples or outputs than the rows hold); device spans
+        are passed as they are (a CUDA graph can capture the call)."""
+        table, o, n, w = self.resample_plan(sample_rate)
+        assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and out.is_cuda and out.dtype == torch.float32
+        B = x.shape[0]
+        if spans.shape != (4, B) or out.shape[0] != B:
+            raise ValueError(f"resample: spans of shape {tuple(spans.shape)} and {out.shape[0]} output rows for {B} input rows")
+        if spans.device.type == "cpu":
+            in_lo, in_hi, out_lo, out_hi = spans.tolist()
+            for b in range(B):
+                if in_hi[b] < in_lo[b] or out_hi[b] < out_lo[b] or out_lo[b] < 0:
+                    raise ValueError(f"resample: row {b} has an inverted span (in [{in_lo[b]}, {in_hi[b]}), out "
+                                     f"[{out_lo[b]}, {out_hi[b]}))")
+                if in_hi[b] - in_lo[b] > x.shape[1] or out_hi[b] - out_lo[b] > out.shape[1]:
+                    raise ValueError(f"resample: row {b} spans more samples or outputs than its row holds")
+            spans = spans.to(device=self.device, dtype=torch.int64)
+        if not out.is_contiguous():
+            raise ValueError("resample: out must be contiguous")
+        if out.shape[1] == 0:
+            return out
+        x = x.contiguous()
+        if x.shape[1] == 0:
+            x = torch.zeros((B, 1), dtype=torch.float32, device=self.device)
+        self._call("gam_resample", x, x.shape[1], B, spans.contiguous(), table, table.shape[0], table.shape[1], o, n, out, out.shape[1])
+        return out
+
+    def resample(self, x: Tensor, lengths: Tensor, sample_rate: int) -> Tuple[Tensor, Tensor]:
+        """Resample the batch x [B, L] (row b: lengths[b] samples at `sample_rate`) to 16 kHz in one launch: -> (y device f32
+        [B, max length], zero past each row's length; int64 lengths ceil(n lengths / o) on lengths' device).  16 kHz input is returned as it is, with no launch."""
+        from .preprocess import SAMPLE_RATE, resampled_length
+        if sample_rate == SAMPLE_RATE:
+            return x, lengths
+        self.resample_plan(sample_rate)
+        lens = [int(v) for v in lengths.reshape(-1).tolist()]
+        if x.dim() != 2 or len(lens) != x.shape[0] or any(not 0 <= v <= x.shape[1] for v in lens):
+            raise ValueError(f"resample: lengths {lens} do not fit a batch of shape {tuple(x.shape)}")
+        out_len = [resampled_length(v, sample_rate) for v in lens]
+        spans = torch.tensor([[0] * len(lens), lens, [0] * len(lens), out_len], dtype=torch.int64)
+        y = torch.zeros((len(lens), max(out_len, default=0)), dtype=torch.float32, device=self.device)
+        self.resample_spans(x.to(device=self.device, dtype=torch.float32), spans, sample_rate, y)
+        return y, torch.tensor(out_len, dtype=torch.int64, device=lengths.device)
 
     def encode(self, mel: Tensor, mel_len: Tensor, n_layers_run: int = -1) -> Tuple[Tensor, Tensor]:
         """[B, F, M] f32, [B] i64 -> ([B, T', d] f32 row-major, [B] i32)"""

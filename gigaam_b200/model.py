@@ -16,7 +16,7 @@ from .decoder import CTCHead, Linear, RNNTHead
 from .decoding import CTCGreedyDecoding, RNNTGreedyDecoding, _as_btd
 from .encoder import ConformerEncoder
 from .engine import Engine
-from .preprocess import SAMPLE_RATE, FeatureExtractor, load_audio
+from .preprocess import SAMPLE_RATE, FeatureExtractor, read_audio, resample_ratio, resampled_length
 from .types import Alignment, Detection, LongformAlignment, TranscriptionResult, Word
 
 LONGFORM_THRESHOLD = 25 * SAMPLE_RATE
@@ -24,6 +24,8 @@ ALIGN_MAX_TOKENS = 4096   # kAlignMaxTokens of csrc/kernels.h
 ALIGN_LONG_MAX_TOKENS = 65536   # kAlignLongMaxTokens of csrc/kernels.h
 SPOT_MAX_TOKENS = 64   # kSpotMaxTokens of csrc/kernels.h
 SPOT_FIRST_MAX_DET = 256   # spot(): detections kept per keyword by the first launch; a second one keeps them all
+RESAMPLE_SPAN = 30 * SAMPLE_RATE   # outputs per row when a long recording is resampled in bounded spans
+RESAMPLE_ROWS = 4                  # rows (spans) per gam_resample launch of those: 2 minutes of output
 
 _REGISTRY = {
     "FeatureExtractor": FeatureExtractor, "ConformerEncoder": ConformerEncoder, "CTCHead": CTCHead,
@@ -188,19 +190,62 @@ class GigaAM(nn.Module):
     def _dtype(self) -> torch.dtype:
         return next(self.parameters()).dtype
 
-    def prepare_wav(self, wav_file: Union[str, Tensor, np.ndarray]) -> Tuple[Tensor, Tensor]:
-        """gigaam/model.py:47-55; additionally accepts an in-memory mono waveform (tensor / ndarray)."""
+    # ---- audio at any sample rate (INTEGRATION.md §7k)
+    def _native(self, wav_file, sample_rate: int) -> Tuple[Tensor, int]:
+        """(mono float32 waveform, its sample rate) of a path (`preprocess.read_audio`: the file's own rate) or of an
+        in-memory waveform at `sample_rate`.  A rate gam_resample cannot take raises ValueError here, before any device work."""
         if isinstance(wav_file, str):
-            wav = load_audio(wav_file)
+            wav, sr = read_audio(wav_file)
         else:
-            wav = torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1)
+            wav, sr = torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1), sample_rate
+        if sr != SAMPLE_RATE:
+            resample_ratio(sr)
+        return wav, sr
+
+    def _resample_host(self, wav: Tensor, sample_rate: int) -> Tensor:
+        """A 1-D waveform at `sample_rate` -> its 16 kHz samples, a host float32 tensor.  The output is cut into spans of
+        RESAMPLE_SPAN samples, RESAMPLE_ROWS of them per gam_resample launch (the span form: each row uploads only the input
+        its outputs need), so device memory does not grow with the recording; every output is the one-shot call's."""
+        eng = self._get_engine()
+        _, o, n, w = eng.resample_plan(sample_rate)
+        L, K = wav.numel(), 2 * w + o
+        N = resampled_length(L, sample_rate)
+        out = torch.empty(N, dtype=torch.float32)
+        starts = list(range(0, N, RESAMPLE_SPAN))
+        for g in range(0, len(starts), RESAMPLE_ROWS):
+            spans = [(max(0, a // n * o - w), min(L, (min(a + RESAMPLE_SPAN, N) - 1) // n * o - w + K), a,
+                      min(a + RESAMPLE_SPAN, N)) for a in starts[g:g + RESAMPLE_ROWS]]
+            x = torch.zeros((len(spans), max(max(hi - lo for lo, hi, _, _ in spans), 1)), dtype=torch.float32)
+            for r, (lo, hi, _, _) in enumerate(spans):
+                x[r, :hi - lo] = wav[lo:hi]
+            y = torch.empty((len(spans), RESAMPLE_SPAN), dtype=torch.float32, device=eng.device)
+            y = eng.resample_spans(x.to(eng.device), torch.tensor(spans, dtype=torch.int64).t(), sample_rate, y).cpu()
+            for r, (_, _, a, b) in enumerate(spans):
+                out[a:b] = y[r, :b - a]
+        return out
+
+    def _resample_batch(self, wav: Tensor, lengths: Tensor, sample_rate: int) -> Tuple[Tensor, Tensor]:
+        """A batch at `sample_rate` -> the 16 kHz batch (Engine.resample, rounded to the model's dtype as prepare_wav does) and
+        its lengths; 16 kHz input is returned as it is."""
+        if sample_rate == SAMPLE_RATE:
+            return wav, lengths
+        y, y_len = self._get_engine().resample(wav, lengths, sample_rate)
+        return y.to(self._dtype), y_len
+
+    def prepare_wav(self, wav_file: Union[str, Tensor, np.ndarray], sample_rate: int = SAMPLE_RATE) -> Tuple[Tensor, Tensor]:
+        """gigaam/model.py:47-55; additionally accepts an in-memory mono waveform (tensor / ndarray) at `sample_rate` Hz,
+        resampled to 16 kHz on the GPU (a file is read at its own rate, `preprocess.read_audio`).  The 16 kHz samples are
+        rounded to the model's dtype."""
+        wav, sr = self._native(wav_file, sample_rate)
+        if sr != SAMPLE_RATE:
+            wav = self._get_engine().resample(wav[None], torch.tensor([wav.numel()]), sr)[0][0]
         wav = wav.to(self._device).to(self._dtype).unsqueeze(0)
         length = torch.full([1], wav.shape[-1], device=self._device)
         return wav, length
 
-    def embed_audio(self, wav_file) -> Tuple[Tensor, Tensor]:
-        """gigaam/model.py:57-63"""
-        wav, length = self.prepare_wav(wav_file)
+    def embed_audio(self, wav_file, sample_rate: int = SAMPLE_RATE) -> Tuple[Tensor, Tensor]:
+        """gigaam/model.py:57-63; `sample_rate` as in `prepare_wav`."""
+        wav, length = self.prepare_wav(wav_file, sample_rate)
         return self.forward(wav, length)
 
 
@@ -270,19 +315,20 @@ class GigaAMASR(GigaAM):
     @torch.inference_mode()
     def transcribe(self, wav_file, word_timestamps: bool = False, confidence: bool = False,
                    hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None, hotword_threshold: float = 0.5,
-                   boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0
-                   ) -> TranscriptionResult:
+                   boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0,
+                   sample_rate: int = SAMPLE_RATE) -> TranscriptionResult:
         """gigaam/model.py:126-140.  `confidence=True` decodes with the scored kernels (the same text and words) and fills
         `confidence` of the result, and of every word when word timestamps are on (INTEGRATION.md, "Confidence").
         `hotwords` (CTC models only): names or terms that replace the greedy words they outscore by `hotword_threshold`
         (INTEGRATION.md §7h); None decodes exactly as without them.  `boost` (RNN-T models only): names or terms whose
         tokens get `boost_weight` nats added to their logits while the greedy decoder follows them (INTEGRATION.md §7j);
-        scores stay the model's own.  None decodes exactly as without it."""
+        scores stay the model's own.  None decodes exactly as without it.  `sample_rate`: the rate of in-memory audio, resampled
+        to 16 kHz on the GPU before the 25 s check (INTEGRATION.md §7k); times stay seconds of the recording."""
         if hotwords is not None:
-            return self._transcribe_hotwords(wav_file, word_timestamps, confidence, hotwords, hotword_threshold)
+            return self._transcribe_hotwords(wav_file, word_timestamps, confidence, hotwords, hotword_threshold, sample_rate)
         if boost is not None:
-            return self._transcribe_boost(wav_file, word_timestamps, confidence, boost, boost_weight)
-        wav, length = self.prepare_wav(wav_file)
+            return self._transcribe_boost(wav_file, word_timestamps, confidence, boost, boost_weight, sample_rate)
+        wav, length = self.prepare_wav(wav_file, sample_rate)
         if length.item() > LONGFORM_THRESHOLD:
             raise ValueError("Too long wav file, use 'transcribe_longform' method.")
         encoded, encoded_len = self.forward(wav, length)
@@ -292,34 +338,41 @@ class GigaAMASR(GigaAM):
     @torch.inference_mode()
     def transcribe_longform(self, wav_file, word_timestamps: bool = False, fr_batch_size: int = 16, fr_num_workers: int = 0,
                             segments: Optional[List[Tensor]] = None, boundaries: Optional[List[Tuple[float, float]]] = None,
-                            confidence: bool = False, **kwargs):
+                            confidence: bool = False, sample_rate: int = SAMPLE_RATE, **kwargs):
         """gigaam/model.py:195-259.  Segmentation is pluggable: pass `segments` / `boundaries` from any VAD (the
         reference's pyannote pipeline, gigaam/vad_utils.py, is third party and not vendored); without them the
         recording is cut at low-energy points (`longform.split_on_energy`, kwargs forwarded).  Segments are
         length-bucketed into batches of `fr_batch_size`; `fr_num_workers` is accepted for signature compatibility.
-        `confidence=True` fills every segment's (and word's) `confidence`, scored inside the same device step."""
+        `confidence=True` fills every segment's (and word's) `confidence`, scored inside the same device step.  `sample_rate`:
+        the rate of an in-memory `wav_file`, resampled to 16 kHz first; `segments` are 16 kHz."""
         from .longform import split_on_energy, transcribe_segments
         if segments is None:
-            wav = load_audio(wav_file) if isinstance(wav_file, str) else torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1)
+            wav, sr = self._native(wav_file, sample_rate)
+            if sr != SAMPLE_RATE:
+                wav = self._resample_host(wav, sr)
             segments, boundaries = split_on_energy(wav, SAMPLE_RATE, **kwargs)
         elif boundaries is None:
             raise ValueError("boundaries are required when segments are given")
         return transcribe_segments(self, segments, boundaries, word_timestamps, fr_batch_size, confidence)
 
     @torch.inference_mode()
-    def align(self, wav_file, text: Union[str, Sequence[int]], word_timestamps: bool = True) -> Alignment:
+    def align(self, wav_file, text: Union[str, Sequence[int]], word_timestamps: bool = True, sample_rate: int = SAMPLE_RATE
+              ) -> Alignment:
         """Align a known transcript to one recording: `text` is a string (normalised and tokenised by
         `Tokenizer.encode`) or a sequence of token ids.  There is no 25 s limit: any length the loaded model encodes is
-        accepted (INTEGRATION.md §7d)."""
-        wav, length = self.prepare_wav(wav_file)
+        accepted (INTEGRATION.md §7d).  `sample_rate` as in `prepare_wav`."""
+        wav, length = self.prepare_wav(wav_file, sample_rate)
         return self.align_batch(wav, length, [text], word_timestamps)[0]
 
     @torch.inference_mode()
     def align_batch(self, wav: Tensor, lengths: Tensor, texts: Sequence[Union[str, Sequence[int]]],
-                    word_timestamps: bool = True) -> List[Alignment]:
+                    word_timestamps: bool = True, sample_rate: int = SAMPLE_RATE) -> List[Alignment]:
         """Align texts[b] to wav[b, :lengths[b]] for every b (Viterbi words, forward log-likelihood, path confidence).
         Raises ValueError before any device work for an empty batch, len(texts) != B, more than 4096 tokens or an id outside
-        [0, V).  An utterance without an alignment (too few frames for its tokens) gets log_likelihood = -inf and no words."""
+        [0, V) and for a `sample_rate` that cannot be resampled.  An utterance without an alignment (too few frames for its
+        tokens) gets log_likelihood = -inf and no words.  `sample_rate`: the batch's rate, resampled to 16 kHz first."""
+        if sample_rate != SAMPLE_RATE:
+            resample_ratio(sample_rate)
         from .decoding import align
         from .timestamps_utils import path_confidence
         B = int(wav.shape[0]) if wav.dim() == 2 else 0
@@ -348,6 +401,7 @@ class GigaAMASR(GigaAM):
         for b, row in enumerate(ids):
             targets[b, :len(row)] = torch.tensor(row, dtype=torch.int32)
         target_len = torch.tensor([len(r) for r in ids], dtype=torch.int32)
+        wav, lengths = self._resample_batch(wav, lengths, sample_rate)
         encoded, encoded_len = self.forward(wav, lengths)
         dev = encoded.device
         targets_d, target_len_d = targets.to(dev), target_len.to(dev)
@@ -393,7 +447,7 @@ class GigaAMASR(GigaAM):
     @torch.inference_mode()
     def align_longform(self, wav_file, text: Union[str, Sequence[str]], word_timestamps: bool = True, window: float = 30.0,
                        overlap: float = 4.0, batch_size: int = 16, *, gap_threshold: Optional[float] = None,
-                       skip_threshold: Optional[float] = None) -> LongformAlignment:
+                       skip_threshold: Optional[float] = None, sample_rate: int = SAMPLE_RATE) -> LongformAlignment:
         """Align a known text, one string or a sequence of lines, to a recording of any length (INTEGRATION.md §7e).  The
         encoder runs over overlapping windows (`longform.plan_windows`), the windows' CTC log-probs are stitched into one
         sequence and gam_ctc_align_long aligns the whole text to it: up to 65 536 tokens, no frame limit.  Returns one
@@ -405,7 +459,8 @@ class GigaAMASR(GigaAM):
         float32, or NaN.
         `skip_threshold` (psi in (0, 1], the same checks) lets whole lines the recording lacks be skipped
         (gam_ctc_align_long_skips): skipping a line and the joining token before it costs psi per token, and the
-        result's `skipped` lists the skipped lines."""
+        result's `skipped` lists the skipped lines.
+        `sample_rate`: the rate of an in-memory `wav_file`, resampled to 16 kHz in bounded spans before the window plan."""
         from .longform import line_edges, line_segments, plan_windows, skipped_lines, stitch_ctc_log_probs, unmatched_intervals
         from .timestamps_utils import compute_frame_shift, gap_confidence, path_confidence, words_from_device
         if self._ncfg["head"].get("type") == "rnnt":
@@ -424,14 +479,14 @@ class GigaAMASR(GigaAM):
         norm, ids, ranges = self._line_tokens(lines)
         if len(ids) > ALIGN_LONG_MAX_TOKENS:
             raise ValueError(f"align_longform: {len(ids)} tokens exceed the limit of {ALIGN_LONG_MAX_TOKENS}")
-        if isinstance(wav_file, str):
-            wav = load_audio(wav_file)
-        else:
-            wav = torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1)
+        wav, sr = self._native(wav_file, sample_rate)
         max_frames = self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
-        windows, T = plan_windows(wav.numel(), window, overlap, self._encoded_length, max_frames)
+        windows, T = plan_windows(wav.numel() if sr == SAMPLE_RATE else resampled_length(wav.numel(), sr), window, overlap,
+                                  self._encoded_length, max_frames)
         if batch_size < 1:
             raise ValueError("batch_size must be >= 1")
+        if sr != SAMPLE_RATE:
+            wav = self._resample_host(wav, sr)
         wav, length = self.prepare_wav(wav)
         lp = stitch_ctc_log_probs(self, wav[0], windows, T, batch_size)
         eng = self._get_engine()
@@ -486,7 +541,8 @@ class GigaAMASR(GigaAM):
     def transcribe_windowed(self, wav_file, word_timestamps: bool = False, confidence: bool = False, window: float = 30.0,
                             overlap: float = 4.0, batch_size: int = 16, pause: float = 1.0, max_segment: float = 25.0,
                             hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None, hotword_threshold: float = 0.5,
-                            boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0):
+                            boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0,
+                            sample_rate: int = SAMPLE_RATE):
         """Transcribe a recording of any length without a VAD (INTEGRATION.md §7f).  The encoder runs over overlapping
         windows (`longform.plan_windows`), and the greedy decoder runs over the windows' kept frames as ONE utterance: each
         window is decoded as soon as its batch is encoded, resuming the decoder state of the window before it
@@ -497,16 +553,14 @@ class GigaAMASR(GigaAM):
         max_segment <= 0.  `hotwords` as in `transcribe` (CTC models only): the windows' log-probs are also stitched into one
         [T, V+1] sequence from the same encoder pass, and the hotwords are applied to the whole recording before it is cut into
         segments.  `boost` and `boost_weight` as in `transcribe` (RNN-T models only): every window's decoding is boosted, the
-        graph state carried across windows with the decoder's."""
+        graph state carried across windows with the decoder's.  `sample_rate`: the rate of an in-memory `wav_file`, resampled to
+        16 kHz in bounded spans into host memory before the window plan (INTEGRATION.md §7k)."""
         from .longform import decode_windows, plan_windows, segment_cuts, windowed_segments
         from .timestamps_utils import compute_frame_shift, words_from_device
         from .types import LongformTranscriptionResult
         kw_ids = None if hotwords is None else self._hotword_ids(hotwords, hotword_threshold, "transcribe_windowed")
         tables = None if boost is None else self._boost_tables(boost, boost_weight, "transcribe_windowed")
-        if isinstance(wav_file, str):
-            wav = load_audio(wav_file)
-        else:
-            wav = torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1)
+        wav, sr = self._native(wav_file, sample_rate)
         if batch_size < 1:
             raise ValueError("batch_size must be >= 1")
         if not pause >= 0:
@@ -514,7 +568,10 @@ class GigaAMASR(GigaAM):
         if not max_segment > 0:
             raise ValueError(f"max_segment={max_segment} s must be positive")
         max_frames = self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
-        windows, T = plan_windows(wav.numel(), window, overlap, self._encoded_length, max_frames)
+        windows, T = plan_windows(wav.numel() if sr == SAMPLE_RATE else resampled_length(wav.numel(), sr), window, overlap,
+                                  self._encoded_length, max_frames)
+        if sr != SAMPLE_RATE:
+            wav = self._resample_host(wav, sr)
         N = wav.numel()
         host = wav.to(self._dtype).pin_memory()          # the rounding of prepare_wav; uploaded one batch at a time
         eng = self._get_engine()
@@ -547,15 +604,19 @@ class GigaAMASR(GigaAM):
 
     def streaming(self, window: float = 8.0, overlap: float = 4.0, batch_size: int = 64, confidence: bool = False,
                   keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5,
-                  boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0):
+                  boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0,
+                  sample_rate: int = SAMPLE_RATE):
         """A `streaming.StreamServer` for live audio (INTEGRATION.md §7i): open streams, push chunks, `step()` for captions
         and keyword alerts, `close()` for each stream's `transcribe_windowed` / `spot` result.  `boost` and `boost_weight` as
         in `transcribe` (RNN-T models only), for every stream of the server.  Raises before any device work: ValueError for
         the window plan's refusals, batch_size < 1, `spot`'s keyword and threshold checks and `boost`'s checks;
-        NotImplementedError for keywords on an RNN-T model and for boost on a CTC model."""
+        NotImplementedError for keywords on an RNN-T model and for boost on a CTC model.  `sample_rate`: the rate of the pushed
+        samples, resampled to 16 kHz as they arrive (INTEGRATION.md §7k); ValueError for a rate gam_resample cannot take."""
         from .streaming import StreamServer
         tables = None if boost is None else self._boost_tables(boost, boost_weight, "streaming")
-        return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold, boost=tables)
+        if sample_rate == SAMPLE_RATE:
+            return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold, boost=tables)
+        return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold, boost=tables, sample_rate=sample_rate)
 
     # ---- keyword spotting (INTEGRATION.md §7g)
     def _refuse_rnnt_spot(self, what: str) -> None:
@@ -624,13 +685,14 @@ class GigaAMASR(GigaAM):
 
     @torch.inference_mode()
     def spot_batch(self, wav: Tensor, lengths: Tensor, keywords: Sequence[Union[str, Sequence[int]]], threshold: float = 0.5,
-                   max_det: int = 64) -> List[List[Detection]]:
+                   max_det: int = 64, sample_rate: int = SAMPLE_RATE) -> List[List[Detection]]:
         """Spot every keyword in every recording wav[b, :lengths[b]] of a batch the model encodes in one pass (up to
         max_encoded_frames).  Returns one list per recording, sorted by start, then keyword index; at most `max_det`
         detections of each keyword are kept (the first ones in time).  Keywords are strings (normalised and tokenised as
         `align` does) or sequences of token ids, up to 64 tokens; `threshold` in (0, 1] is the lowest per-token likelihood
         ratio to greedy decoding that is reported (INTEGRATION.md §7g).  RNN-T models raise NotImplementedError; the keyword,
-        threshold and batch checks raise ValueError, all before any device work."""
+        threshold, batch and `sample_rate` checks raise ValueError, all before any device work.  `sample_rate`: the batch's rate,
+        resampled to 16 kHz first."""
         from .decoding import spot
         from .timestamps_utils import compute_frame_shift
         self._refuse_rnnt_spot("spot_batch")
@@ -640,6 +702,9 @@ class GigaAMASR(GigaAM):
         B = int(wav.shape[0]) if wav.dim() == 2 else 0
         if B == 0:
             raise ValueError("spot_batch: empty batch")
+        if sample_rate != SAMPLE_RATE:
+            resample_ratio(sample_rate)
+        wav, lengths = self._resample_batch(wav, lengths, sample_rate)
         encoded, encoded_len = self.forward(wav, lengths)
         kw, kw_len = self._keyword_tensors(ids, encoded.device)
         start, end, score, count = (t.cpu() for t in spot(self.head, encoded, encoded_len, kw, kw_len, threshold, max_det))
@@ -650,24 +715,25 @@ class GigaAMASR(GigaAM):
 
     @torch.inference_mode()
     def spot(self, wav_file, keywords: Sequence[Union[str, Sequence[int]]], threshold: float = 0.5, window: float = 30.0,
-             overlap: float = 4.0, batch_size: int = 16) -> List[Detection]:
+             overlap: float = 4.0, batch_size: int = 16, sample_rate: int = SAMPLE_RATE) -> List[Detection]:
         """Spot keywords in a recording of any length (INTEGRATION.md §7g): the CTC log-probs of the overlapping windows of
         `align_longform` are stitched into one sequence and gam_ctc_spot searches it for every keyword at once.  Returns
         every detection, sorted by start, then keyword index.  Keywords and threshold as in `spot_batch`.  CTC models only:
         RNN-T raises NotImplementedError.  Raises ValueError before any device work for the keyword and threshold checks,
-        batch_size < 1 and the window plan's refusals (longform.plan_windows)."""
+        batch_size < 1 and the window plan's refusals (longform.plan_windows).  `sample_rate`: the rate of an in-memory
+        `wav_file`, resampled to 16 kHz in bounded spans into host memory before the window plan."""
         from .longform import plan_windows, stitch_ctc_log_probs
         from .timestamps_utils import compute_frame_shift
         self._refuse_rnnt_spot("spot")
         names, ids = self._keyword_ids(keywords, threshold)
-        if isinstance(wav_file, str):
-            wav = load_audio(wav_file)
-        else:
-            wav = torch.as_tensor(wav_file, dtype=torch.float32).reshape(-1)
+        wav, sr = self._native(wav_file, sample_rate)
         max_frames = self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
-        windows, T = plan_windows(wav.numel(), window, overlap, self._encoded_length, max_frames)
+        windows, T = plan_windows(wav.numel() if sr == SAMPLE_RATE else resampled_length(wav.numel(), sr), window, overlap,
+                                  self._encoded_length, max_frames)
         if batch_size < 1:
             raise ValueError("batch_size must be >= 1")
+        if sr != SAMPLE_RATE:
+            wav = self._resample_host(wav, sr)
         N = wav.numel()
         host = wav.to(self._dtype).pin_memory()          # the rounding of prepare_wav; uploaded one batch at a time
         lp = stitch_ctc_log_probs(self, host, windows, T, batch_size)
@@ -725,12 +791,13 @@ class GigaAMASR(GigaAM):
         anchor = tok.vocab.index(" ") if tok.charwise and " " in tok.vocab else None
         return boost_graph(ids, weight, anchor, len(tok) + 1, len(tok))
 
-    def _transcribe_boost(self, wav_file, word_timestamps: bool, confidence: bool, boost, weight: float) -> TranscriptionResult:
+    def _transcribe_boost(self, wav_file, word_timestamps: bool, confidence: bool, boost, weight: float,
+                          sample_rate: int = SAMPLE_RATE) -> TranscriptionResult:
         """`transcribe` with phrase boosting: encode, then one boosted decoding call from a fresh record, then the usual
         formatting."""
         from .timestamps_utils import path_confidence
         tables = self._boost_tables(boost, weight, "transcribe")
-        wav, length = self.prepare_wav(wav_file)
+        wav, length = self.prepare_wav(wav_file, sample_rate)
         if length.item() > LONGFORM_THRESHOLD:
             raise ValueError("Too long wav file, use 'transcribe_longform' method.")
         encoded, encoded_len = self.forward(wav, length)
@@ -761,12 +828,12 @@ class GigaAMASR(GigaAM):
         return eng.ctc_bias(lp, enc_len, kw, kw_len, spotted, threshold, self._word_flags(), g_ids, g_frames, g_counts, token_logp,
                             path_logp, frame_logp)
 
-    def _transcribe_hotwords(self, wav_file, word_timestamps: bool, confidence: bool, hotwords, threshold: float
-                             ) -> TranscriptionResult:
+    def _transcribe_hotwords(self, wav_file, word_timestamps: bool, confidence: bool, hotwords, threshold: float,
+                             sample_rate: int = SAMPLE_RATE) -> TranscriptionResult:
         """`transcribe` with hotwords: encode, (scored) greedy decoding, log-probs, spot, splice, then the usual formatting."""
         from .timestamps_utils import path_confidence
         kw_ids = self._hotword_ids(hotwords, threshold, "transcribe")
-        wav, length = self.prepare_wav(wav_file)
+        wav, length = self.prepare_wav(wav_file, sample_rate)
         if length.item() > LONGFORM_THRESHOLD:
             raise ValueError("Too long wav file, use 'transcribe_longform' method.")
         encoded, encoded_len = self.forward(wav, length)
@@ -786,8 +853,12 @@ class GigaAMASR(GigaAM):
         return TranscriptionResult(text=text, words=words, confidence=conf)
 
     @torch.inference_mode()
-    def transcribe_batch(self, wav: Tensor, lengths: Tensor) -> List[str]:
-        """Batched entry (the path eval.py / transcribe_longform drive: model(wav, len) -> decoding.decode)."""
+    def transcribe_batch(self, wav: Tensor, lengths: Tensor, sample_rate: int = SAMPLE_RATE) -> List[str]:
+        """Batched entry (the path eval.py / transcribe_longform drive: model(wav, len) -> decoding.decode).  `sample_rate`:
+        the batch's rate, resampled to 16 kHz first (ValueError, before any device work, for a rate that cannot be)."""
+        if sample_rate != SAMPLE_RATE:
+            resample_ratio(sample_rate)
+        wav, lengths = self._resample_batch(wav, lengths, sample_rate)
         encoded, encoded_len = self.forward(wav, lengths)
         return [t for t, _, _ in self.decoding.decode(self.head, encoded, encoded_len)]
 
@@ -814,9 +885,10 @@ class GigaAMEmo(GigaAM):
         return probs
 
     @torch.inference_mode()
-    def get_probs(self, wav_file) -> Dict[str, float]:
-        """gigaam/model.py:272-285: {class name: probability} of one recording (a path or an in-memory waveform)."""
-        wav, length = self.prepare_wav(wav_file)
+    def get_probs(self, wav_file, sample_rate: int = SAMPLE_RATE) -> Dict[str, float]:
+        """gigaam/model.py:272-285: {class name: probability} of one recording (a path or an in-memory waveform at
+        `sample_rate`, as in `prepare_wav`)."""
+        wav, length = self.prepare_wav(wav_file, sample_rate)
         encoded, encoded_len = self.forward(wav, length)
         probs = self._pooled_probs(encoded, encoded_len)[0].tolist()
         return {self.id2name[i]: probs[i] for i in range(len(self.id2name))}

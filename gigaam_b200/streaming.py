@@ -10,6 +10,12 @@ streams' decoder records gathered from a device pool and scattered back.  CTC lo
 `Engine.ctc_spot_resume` over the same frames.  `close()` encodes what is left, the last window included, and builds the
 result with `transcribe_windowed`'s and `spot`'s code, so a closed stream gets their output bit for bit.
 
+A server made with another `sample_rate` takes pushes at that rate.  Each step first resamples, in one `gam_resample`
+launch for all streams (the span form, include/gigaam_b200.h), every 16 kHz output whose taps have all been pushed
+(`resample_ready`), and appends it to the stream's 16 kHz samples; `close()` adds the tail with the end's zero padding.
+Every 16 kHz sample is thus the one-shot resampler's, and the windows see the samples `transcribe_windowed(recording,
+sample_rate=...)` sees.  The host keeps the raw samples that the outputs still pending can need.
+
 Device memory does not grow with a stream's duration: a stream owns one decoder record and one spot record per keyword, and
 every step's outputs are step-local.  The host keeps each stream's unencoded samples, its token ids, frames, token
 log-probs, per-frame sums and detections for `close`.  One caller drives a server; it is not thread-safe."""
@@ -25,7 +31,7 @@ from torch import Tensor
 from . import _lib
 from .decoding import _as_btd
 from .longform import FRAME_SAMPLES, Window, _frame_multiple, encode_rows, plan_windows, segment_cuts, window_groups, windowed_segments
-from .preprocess import SAMPLE_RATE
+from .preprocess import SAMPLE_RATE, resample_ratio, resampled_length
 from .timestamps_utils import compute_frame_shift, token_flag_table, words_from_device
 from .types import Detection, LongformTranscriptionResult, StreamResult, StreamUpdate
 
@@ -36,6 +42,13 @@ def ready_count(n_samples: int, W: int, V: int) -> int:
     """How many windows of a stream holding n_samples samples are ready: window w is once n_samples > w H + W, H = W - V.
     For N >= n_samples this is at most len(plan_windows(N)) - 1, so a ready window is never a plan's last one."""
     return 0 if n_samples <= W else (n_samples - W - 1) // (W - V) + 1
+
+
+def resample_ready(n_raw: int, o: int, n: int, w: int) -> int:
+    """How many 16 kHz outputs of a stream holding n_raw samples at the ratio o / n are final: output j n + p needs input
+    samples up to j o + o + w - 1, so the outputs of every j < (n_raw - w) / o are.  They never exceed ceil(n N / o) for
+    N >= n_raw, the length of any recording the stream can become."""
+    return n * max(0, (n_raw - w) // o)
 
 
 def ready_window(w: int, W: int, V: int) -> Window:
@@ -90,6 +103,10 @@ class _Stream:
         self.dets: List[List[Tuple[int, int, float]]] = [[] for _ in range(K)]
         self.pending: List[Optional[Tuple[int, int, float]]] = [None] * K
         self.tentative: List[int] = []
+        # resampling streams: raw samples [raw_start, raw_n) that pending 16 kHz outputs can need, and the outputs made so far
+        self.raw = torch.zeros(0, dtype=torch.float32)
+        self.raw_chunks: List[Tensor] = []
+        self.raw_start = self.raw_n = self.out_n = 0
 
     def samples(self, start: int, end: int) -> Tensor:
         if self.chunks:
@@ -120,11 +137,14 @@ class StreamServer:
     A closed stream's result is `transcribe_windowed(recording, word_timestamps, confidence, window, overlap, pause=pause,
     max_segment=max_segment)` (with the server's `boost` and `boost_weight`) and, with keywords, `spot(recording, keywords,
     threshold, window, overlap)`, bit for bit.  `boost`: the tables of a boost graph (GigaAMASR._boost_tables, moved to the
-    device with the first stream) that steer every stream's decoding, committed and tentative."""
+    device with the first stream) that steer every stream's decoding, committed and tentative.  `sample_rate`: the rate of the
+    pushed samples; a closed stream's result is then `transcribe_windowed(recording, sample_rate=sample_rate, ...)`'s."""
 
     def __init__(self, model, window: float = 8.0, overlap: float = 4.0, batch_size: int = 64, confidence: bool = False,
                  keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5,
-                 boost: Optional[Tuple[Tensor, Tensor]] = None):
+                 boost: Optional[Tuple[Tensor, Tensor]] = None, sample_rate: int = SAMPLE_RATE):
+        self.sample_rate = sample_rate
+        self._ratio = None if sample_rate == SAMPLE_RATE else resample_ratio(sample_rate)
         max_frames = model.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
         self.W = _frame_multiple(window, "window")
         self.V = _frame_multiple(overlap, "overlap")
@@ -190,10 +210,17 @@ class StreamServer:
         return s
 
     def push(self, stream: int, chunk) -> None:
-        """Append mono 16 kHz samples (any length) to a stream, rounded to the model's dtype as `prepare_wav` does.  Host
-        only: nothing runs on the device until `step` or `close`."""
+        """Append mono samples at the server's sample rate (any length) to a stream.  16 kHz samples are rounded to the model's
+        dtype as `prepare_wav` does; samples at another rate are kept as float32 and rounded once resampled.  Host only:
+        nothing runs on the device until `step` or `close`."""
         s = self._get(stream, "push")
-        x = torch.as_tensor(chunk, dtype=torch.float32).detach().reshape(-1).cpu().to(self.model._dtype)
+        x = torch.as_tensor(chunk, dtype=torch.float32).detach().reshape(-1).cpu()
+        if self._ratio is not None:
+            if x.numel():
+                s.raw_chunks.append(x)
+                s.raw_n += x.numel()
+            return
+        x = x.to(self.model._dtype)
         if x.numel():
             s.chunks.append(x)
             s.n += x.numel()
@@ -203,6 +230,8 @@ class StreamServer:
     def step(self) -> List[StreamUpdate]:
         """Encode and decode every ready window of every open stream; returns a StreamUpdate for every stream that has new
         windows, in the order the streams were opened."""
+        if self._ratio is not None:
+            self._resample(list(self._streams.values()), final=False)
         news = {s: [ready_window(w, self.W, self.V) for w in range(len(s.windows), ready_count(s.n, self.W, self.V))]
                 for s in self._streams.values()}
         jobs = [(s, ws[r]) for r in range(max((len(ws) for ws in news.values()), default=0)) for s, ws in news.items() if r < len(ws)]
@@ -221,6 +250,37 @@ class StreamServer:
                                     tentative_text=self.model.decoding.tokenizer.decode(s.tentative),
                                     committed_until=s.committed * FRAME_SECONDS, detections=dets, pending=pending))
         return out
+
+    def _resample(self, streams: List[_Stream], final: bool) -> None:
+        """Resample, in one launch, each stream's 16 kHz outputs that are final (all of them when `final`: the end of the
+        recording is known), append them to its 16 kHz samples and drop the raw samples no pending output needs."""
+        o, n, w = self._ratio
+        rows = []
+        for s in streams:
+            target = resampled_length(s.raw_n, self.sample_rate) if final else resample_ready(s.raw_n, o, n, w)
+            if target > s.out_n:
+                if s.raw_chunks:
+                    s.raw = torch.cat([s.raw] + s.raw_chunks)
+                    s.raw_chunks = []
+                rows.append((s, target))
+        if not rows:
+            return
+        eng = self._eng
+        x = torch.zeros((len(rows), max(1, max(s.raw.numel() for s, _ in rows))), dtype=torch.float32)
+        for r, (s, _) in enumerate(rows):
+            x[r, :s.raw.numel()] = s.raw
+        spans = torch.tensor([[s.raw_start for s, _ in rows], [s.raw_n for s, _ in rows], [s.out_n for s, _ in rows],
+                              [t for _, t in rows]], dtype=torch.int64)
+        y = torch.empty((len(rows), max(t - s.out_n for s, t in rows)), dtype=torch.float32, device=eng.device)
+        y = eng.resample_spans(x.to(eng.device), spans, self.sample_rate, y).cpu()
+        for r, (s, target) in enumerate(rows):
+            cnt = target - s.out_n
+            s.chunks.append(y[r, :cnt].to(self.model._dtype))
+            s.n += cnt
+            s.out_n = target
+            keep = min(max(s.raw_start, target // n * o - w), s.raw_n)   # the first tap of the next pending output
+            s.raw = s.raw[keep - s.raw_start:].clone()
+            s.raw_start = keep
 
     def _detection(self, k: int, start: int, end: int, score: float) -> Detection:
         return Detection(keyword=self.names[k], keyword_index=k, start=start * FRAME_SECONDS, end=end * FRAME_SECONDS, score=score,
@@ -344,6 +404,8 @@ class StreamServer:
             raise ValueError(f"max_segment={max_segment} s must be positive")
         del self._streams[stream]
         self._free.append(s.slot)
+        if self._ratio is not None:
+            self._resample([s], final=True)
         max_frames = self.model.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
         windows, T = plan_windows(s.n, self.window, self.overlap, self.model._encoded_length, max_frames)
         N, done = s.n, len(s.windows)

@@ -636,6 +636,28 @@ int64_t gam_emo_workspace_bytes(const gam_handle* h, int32_t B, int32_t T);
 int gam_emo_head(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
                  int64_t workspace_bytes, float* pooled, float* logits, float* probs, void* stream);
 
+/* Resampling to 16 kHz  <- the reference resamples with ffmpeg (-ar 16000, gigaam/preprocess.py:12-40); this is torchaudio's
+ * default resample(x, orig, 16000) (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99), restated:
+ *   g = gcd(orig, 16000), o = orig / g, n = 16000 / g, base = min(o, n) * 0.99, w = ceil(6 o / base) (double arithmetic),
+ *   K = 2 w + o taps.  h[p, k], p in [0, n), k in [0, K): torchaudio's _get_sinc_resample_kernel evaluated in float64 and
+ *   rounded once to fp32 (built on the host: preprocess.resample_table).
+ *   y[j n + p] = sum_k h[p, k] x[j o + k - w], samples outside the signal 0; the sum runs over k in increasing order as one
+ *   chain of fp32 FMAs from +0 (skipping taps whose sample is outside the signal gives the same bits), so every output is a
+ *   function of its own taps only.  A signal of len samples gives ceil(n len / o) outputs (integer arithmetic).
+ *   orig = 16000 is not resampled: callers make no launch and build no table.
+ *
+ * gam_resample: a ragged batch of B rows.  spans: device i64 [4, B] = in_begin, in_end, out_begin, out_end; row b of x
+ *   (device f32, row pitch x_pitch) holds the samples [in_begin[b], in_end[b]) of its signal from column 0 (at most x_pitch of
+ *   them are read), every other sample counts as 0; row b of y (device f32, row pitch y_pitch) gets outputs
+ *   [out_begin[b], out_end[b]) from column 0, at most y_pitch of them.  Nothing else of y is written: a row whose out range is
+ *   empty or inverted writes nothing, and an inverted in range reads nothing (Engine.resample refuses both on the host).  The
+ *   one-shot case is in = [0, len), out = [0, ceil(n len / o)); chunks and streams pass the spans of their pieces.
+ *   table: device f32 [table_rows, table_cols] = [2 w + o, n], h transposed (k-major).  One launch, no atomics, no host synchronisation, capturable in a
+ *   CUDA graph.  Refused (gam_last_error): a NULL pointer, B outside [1, 65535], a negative pitch, n or o < 1, table dimensions
+ *   other than [2 w + o, n] for (o, n), and tables of more than 2^20 entries. */
+int gam_resample(gam_handle* h, const float* x, int64_t x_pitch, int32_t B, const int64_t* spans, const float* table,
+                 int32_t table_rows, int32_t table_cols, int32_t o, int32_t n, float* y, int64_t y_pitch, void* stream);
+
 /* ---- the one multi-GPU exchange of the path (SURVEY 8e): utterances are sharded over ranks, one process per GPU, and the
  * device-resident hypotheses are all-gathered ONCE over NCCL (NVLink / NVSwitch) when the batch was actually split.
  * gam_comm_unique_id: rank 0 fills 128 bytes, the host ships them to every rank by any channel (torch.distributed, MPI,
