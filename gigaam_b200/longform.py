@@ -66,7 +66,6 @@ def transcribe_segments(model, segments: Sequence[Tensor], boundaries: Sequence[
     length-bucketed batches go through `pipeline.BatchPipeline`: the upload of batch i+1 and the read-back of batch i-1
     overlap the kernels of batch i, recurring shapes replay a CUDA graph, and word grouping stays on the device."""
     from .pipeline import BatchPipeline
-    from .timestamps_utils import path_confidence
     if len(segments) != len(boundaries):
         raise ValueError("segments and boundaries differ in length")
     if not segments:
@@ -89,21 +88,16 @@ def transcribe_segments(model, segments: Sequence[Tensor], boundaries: Sequence[
     shapes = [(len(b), max(lengths[i] for i in b)) for b in batches]
     pipe = BatchPipeline(model, use_graph=len(set(shapes)) < len(shapes), with_words=word_timestamps, with_scores=confidence)
     for batch, host in zip(batches, pipe.run_raw(host_batches())):
-        ids, frames, counts, enc_len = host[:4]
-        token_logp, path_logp, path_rows = host[-3:] if confidence else (None, None, None)
-        if word_timestamps:
-            wav_lens = torch.tensor([lengths[i] for i in batch])
-            results = model._words_from_records(ids, counts, enc_len, wav_lens, list(host[4:9]), token_logp)
-        else:
-            results = [(t, None) for t, _, _ in model.decoding.to_hypotheses(ids, frames, counts)]
-        for row, (text, words) in enumerate(results):
+        decoded = list(host[:3]) + (list(host[-3:]) if confidence else [])
+        results = model._results(decoded, host[3], torch.tensor([lengths[i] for i in batch]), word_timestamps,
+                                 host[4:9] if word_timestamps else None)
+        for row, (text, words, conf) in enumerate(results):
             i = batch[row]
             seg_start, seg_end = boundaries[i]
             shifted = None
             if word_timestamps:
                 shifted = [Word(text=w.text, start=round(w.start + seg_start, 3), end=round(w.end + seg_start, 3),
                                 confidence=w.confidence) for w in words or []]
-            conf = path_confidence(path_logp[row], path_rows[row]) if confidence else None
             out[i] = Segment(text=text, start=seg_start, end=seg_end, words=shifted, confidence=conf)
     return LongformTranscriptionResult(segments=[s for s in out if s is not None])
 
@@ -299,6 +293,33 @@ def windowed_segments(tokenizer, ids: Sequence[int], frames: Sequence[int], cuts
         out.append(Segment(text=tokenizer.decode(list(ids[t0:t1])), start=a * frame_shift, end=duration if k == n - 1 else b * frame_shift,
                            words=None if words is None else list(words[w0:w1]), confidence=conf))
     return out
+
+
+def check_segmenting(pause: float, max_segment: float) -> None:
+    """`segment_cuts`' settings: ValueError for pause < 0 and max_segment <= 0 (NaN fails both)."""
+    if not pause >= 0:
+        raise ValueError(f"pause={pause} s must be >= 0")
+    if not max_segment > 0:
+        raise ValueError(f"max_segment={max_segment} s must be positive")
+
+
+def windowed_result(model, ids: List[int], frames: List[int], token_logp: Optional[List[float]], frame_logp, frame_rows, N: int,
+                    T: int, word_timestamps: bool, pause: float, max_segment: float) -> LongformTranscriptionResult:
+    """The result of a recording of N samples and T frames decoded as one utterance: its token ids and global frames, and
+    with scores the tokens' log-probs and the per-frame sums of `decode_windows` (None without them).  Words are grouped
+    on the device, segments cut by `segment_cuts` and built by `windowed_segments`.  `transcribe_windowed` and a closed
+    stream both end here, so the same decoding gives them the same result."""
+    from .timestamps_utils import compute_frame_shift, words_from_device
+    eng, tok = model._get_engine(), model.decoding.tokenizer
+    rows = torch.tensor([ids or [0], frames or [0]], dtype=torch.int32).pin_memory().to(eng.device, non_blocking=True)
+    count = torch.full((1,), len(ids), dtype=torch.int32, device=eng.device)
+    ws, we, wf, wn, k = (t[0].cpu().tolist() for t in eng.group_words(rows[:1], rows[1:], count, model._word_flags()))
+    shift = compute_frame_shift(N, T)
+    words = words_from_device(tok, ids, ws[:k], we[:k], wf[:k], wn[:k], shift, token_logp)
+    cuts = segment_cuts(list(zip(ws[:k], we[:k])), T, shift, pause, max_segment)
+    return LongformTranscriptionResult(segments=windowed_segments(tok, ids, frames, cuts, shift, N / SAMPLE_RATE,
+                                                                   words if word_timestamps else None, ws[:k], frame_logp,
+                                                                   frame_rows))
 
 
 def line_segments(lines: Sequence[str], ranges: Sequence[Tuple[int, int]], frames: Sequence[int], token_logp: Sequence[float],

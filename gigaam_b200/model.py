@@ -35,6 +35,9 @@ _REGISTRY = {
 
 EMO_MAX_CLASSES = 256   # kPoolMaxClasses of csrc/kernels.h: one class per thread of the softmax
 
+_NO_POSTERIORS = ("{} needs a CTC head: an RNN-T model has no per-frame posteriors without its [T, U + 1] lattice, so there "
+                  "is nothing to search; use a *_ctc model")
+
 
 def _plain(obj):
     """OmegaConf-like containers -> plain dict / list."""
@@ -226,9 +229,11 @@ class GigaAM(nn.Module):
 
     def _resample_batch(self, wav: Tensor, lengths: Tensor, sample_rate: int) -> Tuple[Tensor, Tensor]:
         """A batch at `sample_rate` -> the 16 kHz batch (Engine.resample, rounded to the model's dtype as prepare_wav does) and
-        its lengths; 16 kHz input is returned as it is."""
+        its lengths; 16 kHz input is returned as it is.  A rate gam_resample cannot take raises ValueError before any device
+        work."""
         if sample_rate == SAMPLE_RATE:
             return wav, lengths
+        resample_ratio(sample_rate)
         y, y_len = self._get_engine().resample(wav, lengths, sample_rate)
         return y.to(self._dtype), y_len
 
@@ -256,29 +261,57 @@ class GigaAMASR(GigaAM):
         super().__init__(cfg)
         head_cfg = self._ncfg["head"]
         dec_cfg = {k: v for k, v in self._ncfg["decoding"].items() if k != "type"}
-        self.head = instantiate(head_cfg, "RNNTHead" if head_cfg.get("type") == "rnnt" else "CTCHead")
+        self._rnnt = head_cfg.get("type") == "rnnt"
+        self.head = instantiate(head_cfg, "RNNTHead" if self._rnnt else "CTCHead")
         self.head._bind(self)
-        self.decoding = instantiate(dec_cfg, "RNNTGreedyDecoding" if head_cfg.get("type") == "rnnt" else "CTCGreedyDecoding")
+        self.decoding = instantiate(dec_cfg, "RNNTGreedyDecoding" if self._rnnt else "CTCGreedyDecoding")
+
+    def _needs_head(self, rnnt: bool, message: str) -> None:
+        """Raise NotImplementedError(message) unless the model has the head a call needs: RNN-T if `rnnt`, else CTC."""
+        if self._rnnt != rnnt:
+            raise NotImplementedError(message)
+
+    @property
+    def _max_frames(self) -> int:
+        """The most encoder frames one window may have: the model's max_encoded_frames, else the position table's length."""
+        return self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
 
     def _decode(self, encoded: Tensor, encoded_len: Tensor, wav_lens: Tensor, word_timestamps: bool = False,
                 confidence: bool = False) -> List[Tuple[str, Optional[List[Word]], Optional[float]]]:
         """gigaam/model.py:96-124; (text, words, confidence) per utterance (confidence None unless requested)."""
-        from .timestamps_utils import path_confidence
-        if not word_timestamps:
-            if not confidence:
-                return [(t, None, None) for t, _, _ in self.decoding.decode(self.head, encoded, encoded_len)]
-            return [(h[0], None, path_confidence(h[4], h[5]))
-                    for h in self.decoding.decode(self.head, encoded, encoded_len, return_scores=True)]
-        # tokens are grouped into words on the device (csrc/words.cu); one D2H copy brings ids and word records back
         out = self.decoding.decode_device(self.head, encoded, encoded_len, scores=confidence)
-        ids, frames, counts = out[:3]
-        rec = self._get_engine().group_words(ids, frames, counts, self._word_flags())
-        scores = [t.cpu() for t in out[3:]] if confidence else None
-        res = self._words_from_records(ids.cpu(), counts.cpu(), encoded_len.cpu(), wav_lens.cpu(), [t.cpu() for t in rec],
-                                       scores[0] if confidence else None)
-        if not confidence:
-            return [(t, w, None) for t, w in res]
-        return [(t, w, path_confidence(scores[1][i], scores[2][i])) for i, (t, w) in enumerate(res)]
+        return self._results(out, encoded_len, wav_lens, word_timestamps)
+
+    def _results(self, out: Sequence[Optional[Tensor]], encoded_len: Tensor, wav_lens: Tensor, word_timestamps: bool,
+                 rec: Optional[Sequence[Tensor]] = None) -> List[Tuple[str, Optional[List[Word]], Optional[float]]]:
+        """Greedy or aligned tokens (ids, frames, counts[, token_logp[, path_logp, path_rows]]), on the device or already on the
+        host, -> (text, words, confidence) per utterance.  Words are None unless `word_timestamps`; they are grouped on the
+        device (csrc/words.cu) unless `rec` holds host copies of gam_group_words' records.  token_logp, when given, gives every
+        word its confidence; path_logp / path_rows give the utterance's (None without them)."""
+        from .timestamps_utils import compute_frame_shift, path_confidence, words_from_device
+        tok = self.decoding.tokenizer
+
+        def host(i: int) -> Optional[Tensor]:
+            return out[i].cpu() if len(out) > i and out[i] is not None else None
+        token_logp = host(3) if word_timestamps else None
+        path_logp, path_rows = host(4), host(5)
+        res = []
+        if word_timestamps:
+            if rec is None:
+                rec = self._get_engine().group_words(out[0], out[1], out[2], self._word_flags())
+            ws, we, wf, wn, nw = (t.cpu() for t in rec)
+            enc_len, wav_len = encoded_len.cpu(), wav_lens.cpu()
+        ids = out[0].cpu()
+        for i, n in enumerate(out[2].cpu().tolist()):
+            row = ids[i, :n].tolist()
+            words = None
+            if word_timestamps:
+                k = int(nw[i])
+                words = words_from_device(tok, row, ws[i, :k].tolist(), we[i, :k].tolist(), wf[i, :k].tolist(), wn[i, :k].tolist(),
+                                          compute_frame_shift(int(wav_len[i]), int(enc_len[i])),
+                                          None if token_logp is None else token_logp[i, :n].tolist())
+            res.append((tok.decode(row), words, None if path_logp is None else path_confidence(path_logp[i], path_rows[i])))
+        return res
 
     def _word_flags(self) -> Tensor:
         """Per-token flag table of the device word grouping (timestamps_utils.token_flag_table), built once."""
@@ -288,23 +321,6 @@ class GigaAMASR(GigaAM):
             flags = token_flag_table(self.decoding.tokenizer).to(self._device)
             self.__dict__["_token_flags"] = flags
         return flags
-
-    def _words_from_records(self, ids: Tensor, counts: Tensor, encoded_len: Tensor, wav_lens: Tensor, rec: List[Tensor],
-                            token_logp: Optional[Tensor] = None) -> List[Tuple[str, Optional[List[Word]]]]:
-        """Host copies of (ids, counts, encoded_len, wav_lens, gam_group_words records[, token_logp]) -> [(text, words)] per
-        utterance; with token_logp every word carries its confidence."""
-        from .timestamps_utils import compute_frame_shift, words_from_device
-        tok = self.decoding.tokenizer
-        ws, we, wf, wn, nw = rec
-        out: List[Tuple[str, Optional[List[Word]]]] = []
-        for i, n in enumerate(counts.tolist()):
-            row = ids[i, :n].tolist()
-            k = int(nw[i])
-            shift = compute_frame_shift(int(wav_lens[i]), int(encoded_len[i]))
-            words = words_from_device(tok, row, ws[i, :k].tolist(), we[i, :k].tolist(), wf[i, :k].tolist(), wn[i, :k].tolist(), shift,
-                                      None if token_logp is None else token_logp[i, :n].tolist())
-            out.append((tok.decode(row), words))
-        return out
 
     def forward_for_export(self, features: Tensor, feature_lengths: Tensor) -> Tuple[Tensor, Tensor]:
         """log-mel [B, F, M], lengths [B] -> (head(encoded), encoded_len) (gigaam/model.py:142-149): CTC log-probs
@@ -324,15 +340,33 @@ class GigaAMASR(GigaAM):
         tokens get `boost_weight` nats added to their logits while the greedy decoder follows them (INTEGRATION.md §7j);
         scores stay the model's own.  None decodes exactly as without it.  `sample_rate`: the rate of in-memory audio, resampled
         to 16 kHz on the GPU before the 25 s check (INTEGRATION.md §7k); times stay seconds of the recording."""
-        if hotwords is not None:
-            return self._transcribe_hotwords(wav_file, word_timestamps, confidence, hotwords, hotword_threshold, sample_rate)
-        if boost is not None:
-            return self._transcribe_boost(wav_file, word_timestamps, confidence, boost, boost_weight, sample_rate)
+        kw_ids = tables = None
+        if hotwords is not None:              # boost is not looked at then
+            kw_ids = self._hotword_ids(hotwords, hotword_threshold, "transcribe")
+        elif boost is not None:
+            tables = self._boost_tables(boost, boost_weight, "transcribe")
         wav, length = self.prepare_wav(wav_file, sample_rate)
         if length.item() > LONGFORM_THRESHOLD:
             raise ValueError("Too long wav file, use 'transcribe_longform' method.")
         encoded, encoded_len = self.forward(wav, length)
-        text, words, conf = self._decode(encoded, encoded_len, length, word_timestamps, confidence)[0]
+        if kw_ids is None and tables is None:
+            text, words, conf = self._decode(encoded, encoded_len, length, word_timestamps, confidence)[0]
+            return TranscriptionResult(text=text, words=words, confidence=conf)
+        eng = self._get_engine()
+        enc = _as_btd(encoded.to(dtype=torch.float32))
+        if tables is not None:                # one boosted decoding call from a fresh record
+            T = enc.shape[1]
+            zero = torch.zeros(1, dtype=torch.int32, device=eng.device)
+            out = eng.decode_buffers(1, eng.hyp_width(T), T, scores=confidence)
+            eng.greedy_resume(enc, zero, encoded_len.to(device=eng.device, dtype=torch.int32), zero, eng.decode_state(1), out,
+                              confidence, tuple(t.to(eng.device) for t in tables))
+        else:                                 # greedy decoding, then the spotted hotwords spliced in
+            g = self.decoding.decode_device(self.head, encoded, encoded_len, scores=confidence)
+            lp = eng.ctc_log_probs(enc)
+            ids, frames, counts, _, token_logp, path_logp = self._apply_hotwords(lp, encoded_len, kw_ids, hotword_threshold, *g[:5])
+            del lp
+            out = (ids, frames, counts, token_logp, path_logp, *g[5:])
+        text, words, conf = self._results(out, encoded_len, length, word_timestamps)[0]
         return TranscriptionResult(text=text, words=words, confidence=conf)
 
     @torch.inference_mode()
@@ -371,30 +405,17 @@ class GigaAMASR(GigaAM):
         Raises ValueError before any device work for an empty batch, len(texts) != B, more than 4096 tokens or an id outside
         [0, V) and for a `sample_rate` that cannot be resampled.  An utterance without an alignment (too few frames for its
         tokens) gets log_likelihood = -inf and no words.  `sample_rate`: the batch's rate, resampled to 16 kHz first."""
-        if sample_rate != SAMPLE_RATE:
-            resample_ratio(sample_rate)
         from .decoding import align
         from .timestamps_utils import path_confidence
-        B = int(wav.shape[0]) if wav.dim() == 2 else 0
-        if B == 0:
-            raise ValueError("align: empty batch")
+        B = self._batch_rows(wav, "align")
         if len(texts) != B:
             raise ValueError(f"align: {len(texts)} texts for a batch of {B} recordings")
-        tok = self.decoding.tokenizer
-        V = len(tok)
         norm, ids = [], []
         for text in texts:
-            if isinstance(text, str):
-                row = tok.encode(text)
-                norm.append(tok.normalize(text))
-            else:
-                row = [int(i) for i in text]
-                bad = [i for i in row if not 0 <= i < V]
-                if bad:
-                    raise ValueError(f"align: token id {bad[0]} outside [0, {V})")
-                norm.append(tok.decode(row))
+            name, row = self._text_ids(text, "align")
             if len(row) > ALIGN_MAX_TOKENS:
                 raise ValueError(f"align: {len(row)} tokens exceed the limit of {ALIGN_MAX_TOKENS} per utterance")
+            norm.append(name)
             ids.append(row)
         U = max(len(r) for r in ids)
         targets = torch.zeros((B, U), dtype=torch.int32)
@@ -406,16 +427,14 @@ class GigaAMASR(GigaAM):
         dev = encoded.device
         targets_d, target_len_d = targets.to(dev), target_len.to(dev)
         frames, token_logp, viterbi_logp, log_likelihood, path_rows = align(self.head, encoded, encoded_len, targets_d, target_len_d)
+        ll, vit = torch.stack([log_likelihood, viterbi_logp]).cpu().tolist()
         words: List[Optional[List[Word]]] = [None] * B
         if word_timestamps:
             words = [[] for _ in range(B)]
             if U > 0:
-                rec = self._get_engine().group_words(targets_d, frames, target_len_d, self._word_flags())
-                found = [w for _, w in self._words_from_records(targets, target_len, encoded_len.cpu(), lengths.cpu(),
-                                                                [t.cpu() for t in rec], token_logp.cpu())]
-                vit = viterbi_logp.cpu().tolist()
-                words = [w if math.isfinite(v) else [] for w, v in zip(found, vit)]
-        ll, vit, rows = log_likelihood.cpu().tolist(), viterbi_logp.cpu().tolist(), path_rows.cpu().tolist()
+                found = self._results((targets_d, frames, target_len_d, token_logp), encoded_len, lengths, True)
+                words = [w if math.isfinite(v) else [] for (_, w, _), v in zip(found, vit)]
+        rows = path_rows.cpu().tolist()
         return [Alignment(text=norm[b], words=words[b], log_likelihood=ll[b], confidence=path_confidence(vit[b], rows[b]))
                 for b in range(B)]
 
@@ -424,6 +443,44 @@ class GigaAMASR(GigaAM):
         host."""
         mel = self.preprocessor.out_len(torch.tensor([int(n_samples)]))
         return int(self.encoder.pre_encode.calc_output_length(mel)[0])
+
+    def _intake(self, wav_file, sample_rate: int, window: float, overlap: float, batch_size: int
+                ) -> Tuple[Tensor, int, list, int]:
+        """One recording for the windowed entry points -> (its 16 kHz samples in the model's dtype in pinned host memory,
+        uploaded one batch of windows at a time; N samples; `longform.plan_windows`' windows over them; T encoder frames).
+        The file is read or the waveform taken, the rate checked, the windows planned on the resampled length and batch_size
+        checked before any device work: ValueError for each refusal.  Then the recording is resampled in bounded spans
+        (`_resample_host`) and rounded to the model's dtype, as prepare_wav rounds it; it is pinned when the model is on a GPU."""
+        from .longform import plan_windows
+        wav, sr = self._native(wav_file, sample_rate)
+        N = wav.numel() if sr == SAMPLE_RATE else resampled_length(wav.numel(), sr)
+        windows, T = plan_windows(N, window, overlap, self._encoded_length, self._max_frames)
+        if batch_size < 1:
+            raise ValueError("batch_size must be >= 1")
+        if sr != SAMPLE_RATE:
+            wav = self._resample_host(wav, sr)
+        host = wav.to(self._dtype)
+        return (host.pin_memory() if self._device.type == "cuda" else host), N, windows, T   # a CPU model uploads nothing
+
+    def _text_ids(self, text: Union[str, Sequence[int]], what: str) -> Tuple[str, List[int]]:
+        """(normalised text, token ids) of a string (`Tokenizer.encode`) or of a sequence of token ids, taken as it is:
+        ValueError `what: token id ... outside [0, V)` for an id the vocabulary lacks."""
+        tok = self.decoding.tokenizer
+        if isinstance(text, str):
+            row = tok.encode(text)
+            return tok.normalize(text), row
+        row = [int(i) for i in text]
+        bad = [i for i in row if not 0 <= i < len(tok)]
+        if bad:
+            raise ValueError(f"{what}: token id {bad[0]} outside [0, {len(tok)})")
+        return tok.decode(row), row
+
+    def _refuse_edge_spaces(self, ids: List[List[int]], what: str, noun: str, why: str) -> None:
+        """ValueError for a phrase whose first or last token is the space token; `why` tells what to pass instead."""
+        tok = self.decoding.tokenizer
+        for row in ids:
+            if any(tok.id_to_str(row[i]) == " " for i in (0, -1)):
+                raise ValueError(f"{what}: {noun} {tok.decode(row)!r} starts or ends with the space token; {why}")
 
     def _line_tokens(self, lines: Sequence[str]) -> Tuple[List[str], List[int], List[Tuple[int, int]]]:
         """Normalised lines, the token ids of the whole text and each line's token range [a, b).  Lines are joined so that
@@ -436,8 +493,8 @@ class GigaAMASR(GigaAM):
         for line in lines:
             if not isinstance(line, str):
                 raise TypeError(f"align_longform: lines must be strings, got {type(line).__name__}")
-            row = tok.encode(line)
-            norm.append(tok.normalize(line))
+            name, row = self._text_ids(line, "align_longform")
+            norm.append(name)
             if row and ids and space is not None:
                 ids.append(space)
             ranges.append((len(ids), len(ids) + len(row)))
@@ -461,12 +518,11 @@ class GigaAMASR(GigaAM):
         (gam_ctc_align_long_skips): skipping a line and the joining token before it costs psi per token, and the
         result's `skipped` lists the skipped lines.
         `sample_rate`: the rate of an in-memory `wav_file`, resampled to 16 kHz in bounded spans before the window plan."""
-        from .longform import line_edges, line_segments, plan_windows, skipped_lines, stitch_ctc_log_probs, unmatched_intervals
+        from .longform import line_edges, line_segments, skipped_lines, stitch_ctc_log_probs, unmatched_intervals
         from .timestamps_utils import compute_frame_shift, gap_confidence, path_confidence, words_from_device
-        if self._ncfg["head"].get("type") == "rnnt":
-            raise NotImplementedError("align_longform needs a CTC head: RNN-T alignment walks a [T, U + 1] lattice, about "
-                                      "4.5e9 nodes for an hour of speech, and banding it would no longer give the Viterbi "
-                                      "path; use a *_ctc model, or align() up to max_encoded_frames")
+        self._needs_head(False, "align_longform needs a CTC head: RNN-T alignment walks a [T, U + 1] lattice, about 4.5e9 nodes "
+                                "for an hour of speech, and banding it would no longer give the Viterbi path; use a *_ctc model, "
+                                "or align() up to max_encoded_frames")
 
         def log_threshold(name, value):
             x = float(np.float32(value))
@@ -479,16 +535,8 @@ class GigaAMASR(GigaAM):
         norm, ids, ranges = self._line_tokens(lines)
         if len(ids) > ALIGN_LONG_MAX_TOKENS:
             raise ValueError(f"align_longform: {len(ids)} tokens exceed the limit of {ALIGN_LONG_MAX_TOKENS}")
-        wav, sr = self._native(wav_file, sample_rate)
-        max_frames = self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
-        windows, T = plan_windows(wav.numel() if sr == SAMPLE_RATE else resampled_length(wav.numel(), sr), window, overlap,
-                                  self._encoded_length, max_frames)
-        if batch_size < 1:
-            raise ValueError("batch_size must be >= 1")
-        if sr != SAMPLE_RATE:
-            wav = self._resample_host(wav, sr)
-        wav, length = self.prepare_wav(wav)
-        lp = stitch_ctc_log_probs(self, wav[0], windows, T, batch_size)
+        host, N, windows, T = self._intake(wav_file, sample_rate, window, overlap, batch_size)
+        lp = stitch_ctc_log_probs(self, host, windows, T, batch_size)
         eng = self._get_engine()
         U = len(ids)
         targets = torch.tensor([ids], dtype=torch.int32).reshape(1, U)
@@ -509,7 +557,7 @@ class GigaAMASR(GigaAM):
                  skip_logp) = eng.ctc_align_long(lp, enc_len, targets_d, target_len_d, gaps=gaps, skips=log_psi)
         del lp
         vit, ll = float(viterbi_logp[0]), float(log_likelihood[0])
-        shift = compute_frame_shift(int(length[0]), T)
+        shift = compute_frame_shift(N, T)
         fr, logp = frames[0].cpu().tolist(), token_logp[0].cpu().tolist()
         skipped = None
         if log_psi is not None:
@@ -555,25 +603,11 @@ class GigaAMASR(GigaAM):
         segments.  `boost` and `boost_weight` as in `transcribe` (RNN-T models only): every window's decoding is boosted, the
         graph state carried across windows with the decoder's.  `sample_rate`: the rate of an in-memory `wav_file`, resampled to
         16 kHz in bounded spans into host memory before the window plan (INTEGRATION.md §7k)."""
-        from .longform import decode_windows, plan_windows, segment_cuts, windowed_segments
-        from .timestamps_utils import compute_frame_shift, words_from_device
-        from .types import LongformTranscriptionResult
+        from .longform import check_segmenting, decode_windows, windowed_result
         kw_ids = None if hotwords is None else self._hotword_ids(hotwords, hotword_threshold, "transcribe_windowed")
         tables = None if boost is None else self._boost_tables(boost, boost_weight, "transcribe_windowed")
-        wav, sr = self._native(wav_file, sample_rate)
-        if batch_size < 1:
-            raise ValueError("batch_size must be >= 1")
-        if not pause >= 0:
-            raise ValueError(f"pause={pause} s must be >= 0")
-        if not max_segment > 0:
-            raise ValueError(f"max_segment={max_segment} s must be positive")
-        max_frames = self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
-        windows, T = plan_windows(wav.numel() if sr == SAMPLE_RATE else resampled_length(wav.numel(), sr), window, overlap,
-                                  self._encoded_length, max_frames)
-        if sr != SAMPLE_RATE:
-            wav = self._resample_host(wav, sr)
-        N = wav.numel()
-        host = wav.to(self._dtype).pin_memory()          # the rounding of prepare_wav; uploaded one batch at a time
+        check_segmenting(pause, max_segment)
+        host, N, windows, T = self._intake(wav_file, sample_rate, window, overlap, batch_size)
         eng = self._get_engine()
         if tables is not None:
             out = decode_windows(self, host, windows, T, batch_size, confidence, boost=tuple(t.to(eng.device) for t in tables))
@@ -588,19 +622,11 @@ class GigaAMASR(GigaAM):
                 out.frame_logp)
             del lp
             out = out._replace(ids=b_ids, frames=b_frames, counts=b_counts, token_logp=b_logp, path_logp=b_path)
-        rec = eng.group_words(out.ids, out.frames, out.counts, self._word_flags())
         n = int(out.counts[0])
-        ids, frames = out.ids[0, :n].tolist(), out.frames[0, :n].tolist()
-        ws, we, wf, wn, k = (t[0].cpu().tolist() for t in rec)
-        shift = compute_frame_shift(N, T)
-        logp = out.token_logp[0, :n].tolist() if confidence else None
-        words = words_from_device(self.decoding.tokenizer, ids, ws[:k], we[:k], wf[:k], wn[:k], shift, logp)
-        cuts = segment_cuts(list(zip(ws[:k], we[:k])), T, shift, pause, max_segment)
-        frame_logp = out.frame_logp[0].cpu().numpy() if confidence else None
-        frame_rows = out.frame_rows[0].cpu().numpy() if confidence else None
-        segs = windowed_segments(self.decoding.tokenizer, ids, frames, cuts, shift, N / SAMPLE_RATE,
-                                 words if word_timestamps else None, ws[:k], frame_logp, frame_rows)
-        return LongformTranscriptionResult(segments=segs)
+        return windowed_result(self, out.ids[0, :n].tolist(), out.frames[0, :n].tolist(),
+                               out.token_logp[0, :n].tolist() if confidence else None,
+                               out.frame_logp[0].cpu().numpy() if confidence else None,
+                               out.frame_rows[0].cpu().numpy() if confidence else None, N, T, word_timestamps, pause, max_segment)
 
     def streaming(self, window: float = 8.0, overlap: float = 4.0, batch_size: int = 64, confidence: bool = False,
                   keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5,
@@ -614,16 +640,9 @@ class GigaAMASR(GigaAM):
         samples, resampled to 16 kHz as they arrive (INTEGRATION.md §7k); ValueError for a rate gam_resample cannot take."""
         from .streaming import StreamServer
         tables = None if boost is None else self._boost_tables(boost, boost_weight, "streaming")
-        if sample_rate == SAMPLE_RATE:
-            return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold, boost=tables)
         return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold, boost=tables, sample_rate=sample_rate)
 
     # ---- keyword spotting (INTEGRATION.md §7g)
-    def _refuse_rnnt_spot(self, what: str) -> None:
-        if self._ncfg["head"].get("type") == "rnnt":
-            raise NotImplementedError(f"{what} needs a CTC head: an RNN-T model has no per-frame posteriors without its "
-                                      "[T, U + 1] lattice, so there is nothing to search; use a *_ctc model")
-
     def _keyword_ids(self, keywords: Sequence[Union[str, Sequence[int]]], threshold: float) -> Tuple[List[str], List[List[int]]]:
         """Each keyword's text and token ids (`_phrase_ids`), then the threshold, checked before any device work: ValueError
         also for a threshold outside (0, 1] (in fp32)."""
@@ -637,28 +656,18 @@ class GigaAMASR(GigaAM):
         `Tokenizer.encode` (as `align` does), a sequence of ids is taken as it is.  Raises ValueError for an empty list, a
         phrase without tokens, more than 64 tokens and an id outside [0, V); messages start with `what` and name the phrase
         a `noun`."""
-        tok = self.decoding.tokenizer
-        V = len(tok)
         kws = [phrases] if isinstance(phrases, str) else list(phrases)
         if not kws:
             raise ValueError(f"{what}: no {noun}s")
         names, ids = [], []
         for kw in kws:
-            if isinstance(kw, str):
-                row = tok.encode(kw)
-                if not row:
-                    raise ValueError(f"{what}: {noun} {kw!r} normalises to no tokens")
-                names.append(tok.normalize(kw))
-            else:
-                row = [int(i) for i in kw]
-                bad = [i for i in row if not 0 <= i < V]
-                if bad:
-                    raise ValueError(f"{what}: token id {bad[0]} outside [0, {V})")
-                if not row:
-                    raise ValueError(f"{what}: a {noun} without tokens")
-                names.append(tok.decode(row))
+            name, row = self._text_ids(kw, what)
+            if not row:
+                raise ValueError(f"{what}: {noun} {kw!r} normalises to no tokens" if isinstance(kw, str)
+                                 else f"{what}: a {noun} without tokens")
             if len(row) > SPOT_MAX_TOKENS:
-                raise ValueError(f"{what}: {noun} {names[-1]!r} has {len(row)} tokens, more than {SPOT_MAX_TOKENS}")
+                raise ValueError(f"{what}: {noun} {name!r} has {len(row)} tokens, more than {SPOT_MAX_TOKENS}")
+            names.append(name)
             ids.append(row)
         return names, ids
 
@@ -670,18 +679,21 @@ class GigaAMASR(GigaAM):
         return keywords.to(device), torch.tensor([len(r) for r in ids], dtype=torch.int32, device=device)
 
     @staticmethod
-    def _detections(names: List[str], ids: List[List[int]], start: Tensor, end: Tensor, score: Tensor, count: Tensor,
+    def _detections(names: List[str], ids: List[List[int]], dets: Sequence[Sequence[Tuple[int, int, float]]],
                     frame_shift: float) -> List[Detection]:
-        """Host copies of one recording's gam_ctc_spot outputs -> its stored detections, sorted by start, then keyword."""
-        out = []
-        n = count.clamp(max=start.shape[1]).tolist()
-        for k, name in enumerate(names):
-            U = len(ids[k])
-            for s, e, sc in zip(start[k, :n[k]].tolist(), end[k, :n[k]].tolist(), score[k, :n[k]].tolist()):
-                out.append((s, k, Detection(keyword=name, keyword_index=k, start=s * frame_shift, end=e * frame_shift, score=sc,
-                                            confidence=math.exp(sc / U))))
+        """Each keyword's (start frame, end frame, score) detections in one recording -> its Detection records, sorted by
+        start, then keyword."""
+        out = [(s, k, Detection(keyword=name, keyword_index=k, start=s * frame_shift, end=e * frame_shift, score=sc,
+                                confidence=math.exp(sc / len(ids[k]))))
+               for k, name in enumerate(names) for s, e, sc in dets[k]]
         out.sort(key=lambda d: d[:2])
         return [d for _, _, d in out]
+
+    @staticmethod
+    def _stored(start: Tensor, end: Tensor, score: Tensor, count: Tensor) -> List[List[Tuple[int, int, float]]]:
+        """Host copies of one recording's gam_ctc_spot outputs ([K, max_det], count [K]) -> each keyword's stored detections."""
+        n = count.clamp(max=start.shape[1]).tolist()
+        return [list(zip(start[k, :c].tolist(), end[k, :c].tolist(), score[k, :c].tolist())) for k, c in enumerate(n)]
 
     @torch.inference_mode()
     def spot_batch(self, wav: Tensor, lengths: Tensor, keywords: Sequence[Union[str, Sequence[int]]], threshold: float = 0.5,
@@ -695,23 +707,27 @@ class GigaAMASR(GigaAM):
         resampled to 16 kHz first."""
         from .decoding import spot
         from .timestamps_utils import compute_frame_shift
-        self._refuse_rnnt_spot("spot_batch")
+        self._needs_head(False, _NO_POSTERIORS.format("spot_batch"))
         names, ids = self._keyword_ids(keywords, threshold)
         if max_det < 1:
             raise ValueError(f"spot_batch: max_det={max_det} must be >= 1")
-        B = int(wav.shape[0]) if wav.dim() == 2 else 0
-        if B == 0:
-            raise ValueError("spot_batch: empty batch")
-        if sample_rate != SAMPLE_RATE:
-            resample_ratio(sample_rate)
+        B = self._batch_rows(wav, "spot_batch")
         wav, lengths = self._resample_batch(wav, lengths, sample_rate)
         encoded, encoded_len = self.forward(wav, lengths)
         kw, kw_len = self._keyword_tensors(ids, encoded.device)
         start, end, score, count = (t.cpu() for t in spot(self.head, encoded, encoded_len, kw, kw_len, threshold, max_det))
         enc_len, wav_len = encoded_len.cpu().tolist(), lengths.cpu().tolist()
-        return [self._detections(names, ids, start[b], end[b], score[b], count[b],
+        return [self._detections(names, ids, self._stored(start[b], end[b], score[b], count[b]),
                                  compute_frame_shift(int(wav_len[b]), int(enc_len[b])) if enc_len[b] > 0 else 0.0)
                 for b in range(B)]
+
+    @staticmethod
+    def _batch_rows(wav: Tensor, what: str) -> int:
+        """The rows of a [B, N] batch; ValueError for an empty batch (or one that is not 2-D)."""
+        B = int(wav.shape[0]) if wav.dim() == 2 else 0
+        if B == 0:
+            raise ValueError(f"{what}: empty batch")
+        return B
 
     @torch.inference_mode()
     def spot(self, wav_file, keywords: Sequence[Union[str, Sequence[int]]], threshold: float = 0.5, window: float = 30.0,
@@ -722,28 +738,18 @@ class GigaAMASR(GigaAM):
         RNN-T raises NotImplementedError.  Raises ValueError before any device work for the keyword and threshold checks,
         batch_size < 1 and the window plan's refusals (longform.plan_windows).  `sample_rate`: the rate of an in-memory
         `wav_file`, resampled to 16 kHz in bounded spans into host memory before the window plan."""
-        from .longform import plan_windows, stitch_ctc_log_probs
+        from .longform import stitch_ctc_log_probs
         from .timestamps_utils import compute_frame_shift
-        self._refuse_rnnt_spot("spot")
+        self._needs_head(False, _NO_POSTERIORS.format("spot"))
         names, ids = self._keyword_ids(keywords, threshold)
-        wav, sr = self._native(wav_file, sample_rate)
-        max_frames = self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
-        windows, T = plan_windows(wav.numel() if sr == SAMPLE_RATE else resampled_length(wav.numel(), sr), window, overlap,
-                                  self._encoded_length, max_frames)
-        if batch_size < 1:
-            raise ValueError("batch_size must be >= 1")
-        if sr != SAMPLE_RATE:
-            wav = self._resample_host(wav, sr)
-        N = wav.numel()
-        host = wav.to(self._dtype).pin_memory()          # the rounding of prepare_wav; uploaded one batch at a time
+        host, N, windows, T = self._intake(wav_file, sample_rate, window, overlap, batch_size)
         lp = stitch_ctc_log_probs(self, host, windows, T, batch_size)
         eng = self._get_engine()
         kw, kw_len = self._keyword_tensors(ids, eng.device)
         enc_len = torch.tensor([T], dtype=torch.int32, device=eng.device)
         out = self._spot_all(lp, enc_len, kw, kw_len, ids, threshold)
         del lp
-        start, end, score, count = (t[0].cpu() for t in out)
-        return self._detections(names, ids, start, end, score, count, compute_frame_shift(N, T))
+        return self._detections(names, ids, self._stored(*(t[0].cpu() for t in out)), compute_frame_shift(N, T))
 
     def _spot_all(self, lp: Tensor, enc_len: Tensor, kw: Tensor, kw_len: Tensor, ids: List[List[int]], threshold: float
                   ) -> Tuple[Tensor, ...]:
@@ -763,13 +769,10 @@ class GigaAMASR(GigaAM):
         """Token ids of the hotwords, checked before any device work: RNN-T models raise NotImplementedError, the keyword and
         threshold checks of `spot` raise ValueError, and so does a hotword that starts or ends with the space token (the
         splice keeps to word boundaries by itself)."""
-        self._refuse_rnnt_spot(what)
+        self._needs_head(False, _NO_POSTERIORS.format(what))
         _, ids = self._keyword_ids(hotwords, threshold)
-        tok = self.decoding.tokenizer
-        for row in ids:
-            if any(tok.id_to_str(row[i]) == " " for i in (0, -1)):
-                raise ValueError(f"{what}: hotword {tok.decode(row)!r} starts or ends with the space token; hotwords are "
-                                 "spliced at word boundaries only, so pass the word without its spaces")
+        self._refuse_edge_spaces(ids, what, "hotword", "hotwords are spliced at word boundaries only, so pass the word without "
+                                 "its spaces")
         return ids
 
     # ---- phrase boosting (INTEGRATION.md §7j)
@@ -779,43 +782,14 @@ class GigaAMASR(GigaAM):
         that is not finite and > 0 and a graph of more than 65 536 states raise ValueError.  A charwise vocabulary anchors
         every phrase at a word start (its space token); SentencePiece pieces open their words themselves."""
         from .decoding import boost_graph
-        if self._ncfg["head"].get("type") != "rnnt":
-            raise NotImplementedError(f"{what}: boost steers the RNN-T greedy decoder; for a CTC model use hotwords=, which "
-                                      "splices spotted phrases into the transcript")
+        self._needs_head(True, f"{what}: boost steers the RNN-T greedy decoder; for a CTC model use hotwords=, which splices "
+                               "spotted phrases into the transcript")
         _, ids = self._phrase_ids(phrases, what, "phrase")
+        self._refuse_edge_spaces(ids, what, "phrase", "a phrase is anchored at a word start by itself, so pass the words "
+                                 "without edge spaces")
         tok = self.decoding.tokenizer
-        for row in ids:
-            if any(tok.id_to_str(row[i]) == " " for i in (0, -1)):
-                raise ValueError(f"{what}: phrase {tok.decode(row)!r} starts or ends with the space token; a phrase is "
-                                 "anchored at a word start by itself, so pass the words without edge spaces")
         anchor = tok.vocab.index(" ") if tok.charwise and " " in tok.vocab else None
         return boost_graph(ids, weight, anchor, len(tok) + 1, len(tok))
-
-    def _transcribe_boost(self, wav_file, word_timestamps: bool, confidence: bool, boost, weight: float,
-                          sample_rate: int = SAMPLE_RATE) -> TranscriptionResult:
-        """`transcribe` with phrase boosting: encode, then one boosted decoding call from a fresh record, then the usual
-        formatting."""
-        from .timestamps_utils import path_confidence
-        tables = self._boost_tables(boost, weight, "transcribe")
-        wav, length = self.prepare_wav(wav_file, sample_rate)
-        if length.item() > LONGFORM_THRESHOLD:
-            raise ValueError("Too long wav file, use 'transcribe_longform' method.")
-        encoded, encoded_len = self.forward(wav, length)
-        eng = self._get_engine()
-        enc = _as_btd(encoded.to(dtype=torch.float32))
-        T = enc.shape[1]
-        zero = torch.zeros(1, dtype=torch.int32, device=eng.device)
-        out = eng.decode_buffers(1, eng.hyp_width(T), T, scores=confidence)
-        eng.greedy_resume(enc, zero, encoded_len.to(device=eng.device, dtype=torch.int32), zero, eng.decode_state(1), out, confidence,
-                          tuple(t.to(eng.device) for t in tables))
-        conf = path_confidence(float(out.path_logp[0]), int(out.path_rows[0])) if confidence else None
-        if not word_timestamps:
-            n = int(out.counts[0])
-            return TranscriptionResult(text=self.decoding.tokenizer.decode(out.ids[0, :n].tolist()), words=None, confidence=conf)
-        rec = eng.group_words(out.ids, out.frames, out.counts, self._word_flags())
-        text, words = self._words_from_records(out.ids.cpu(), out.counts.cpu(), encoded_len.cpu(), length.cpu(),
-                                               [t.cpu() for t in rec], out.token_logp.cpu() if confidence else None)[0]
-        return TranscriptionResult(text=text, words=words, confidence=conf)
 
     def _apply_hotwords(self, lp: Tensor, enc_len: Tensor, ids: List[List[int]], threshold: float, g_ids: Tensor, g_frames: Tensor,
                         g_counts: Tensor, token_logp: Optional[Tensor] = None, path_logp: Optional[Tensor] = None,
@@ -828,36 +802,10 @@ class GigaAMASR(GigaAM):
         return eng.ctc_bias(lp, enc_len, kw, kw_len, spotted, threshold, self._word_flags(), g_ids, g_frames, g_counts, token_logp,
                             path_logp, frame_logp)
 
-    def _transcribe_hotwords(self, wav_file, word_timestamps: bool, confidence: bool, hotwords, threshold: float,
-                             sample_rate: int = SAMPLE_RATE) -> TranscriptionResult:
-        """`transcribe` with hotwords: encode, (scored) greedy decoding, log-probs, spot, splice, then the usual formatting."""
-        from .timestamps_utils import path_confidence
-        kw_ids = self._hotword_ids(hotwords, threshold, "transcribe")
-        wav, length = self.prepare_wav(wav_file, sample_rate)
-        if length.item() > LONGFORM_THRESHOLD:
-            raise ValueError("Too long wav file, use 'transcribe_longform' method.")
-        encoded, encoded_len = self.forward(wav, length)
-        g = self.decoding.decode_device(self.head, encoded, encoded_len, scores=confidence)
-        eng = self._get_engine()
-        lp = eng.ctc_log_probs(_as_btd(encoded.to(dtype=torch.float32)))
-        ids, frames, counts, _, token_logp, path_logp = self._apply_hotwords(
-            lp, encoded_len, kw_ids, threshold, *g[:3], *(g[3:5] if confidence else (None, None)))
-        del lp
-        conf = path_confidence(float(path_logp[0]), int(g[5][0])) if confidence else None
-        if not word_timestamps:
-            n = int(counts[0])
-            return TranscriptionResult(text=self.decoding.tokenizer.decode(ids[0, :n].tolist()), words=None, confidence=conf)
-        rec = eng.group_words(ids, frames, counts, self._word_flags())
-        text, words = self._words_from_records(ids.cpu(), counts.cpu(), encoded_len.cpu(), length.cpu(), [t.cpu() for t in rec],
-                                               token_logp.cpu() if confidence else None)[0]
-        return TranscriptionResult(text=text, words=words, confidence=conf)
-
     @torch.inference_mode()
     def transcribe_batch(self, wav: Tensor, lengths: Tensor, sample_rate: int = SAMPLE_RATE) -> List[str]:
         """Batched entry (the path eval.py / transcribe_longform drive: model(wav, len) -> decoding.decode).  `sample_rate`:
         the batch's rate, resampled to 16 kHz first (ValueError, before any device work, for a rate that cannot be)."""
-        if sample_rate != SAMPLE_RATE:
-            resample_ratio(sample_rate)
         wav, lengths = self._resample_batch(wav, lengths, sample_rate)
         encoded, encoded_len = self.forward(wav, lengths)
         return [t for t, _, _ in self.decoding.decode(self.head, encoded, encoded_len)]

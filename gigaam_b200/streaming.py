@@ -28,12 +28,12 @@ import numpy as np
 import torch
 from torch import Tensor
 
-from . import _lib
 from .decoding import _as_btd
-from .longform import FRAME_SAMPLES, Window, _frame_multiple, encode_rows, plan_windows, segment_cuts, window_groups, windowed_segments
+from .longform import (FRAME_SAMPLES, Window, _frame_multiple, check_segmenting, encode_rows, plan_windows, window_groups,
+                       windowed_result)
 from .preprocess import SAMPLE_RATE, resample_ratio, resampled_length
-from .timestamps_utils import compute_frame_shift, token_flag_table, words_from_device
-from .types import Detection, LongformTranscriptionResult, StreamResult, StreamUpdate
+from .timestamps_utils import compute_frame_shift, token_flag_table
+from .types import Detection, StreamResult, StreamUpdate
 
 FRAME_SECONDS = FRAME_SAMPLES / SAMPLE_RATE   # the nominal 40 ms frame step of updates
 
@@ -145,18 +145,16 @@ class StreamServer:
                  boost: Optional[Tuple[Tensor, Tensor]] = None, sample_rate: int = SAMPLE_RATE):
         self.sample_rate = sample_rate
         self._ratio = None if sample_rate == SAMPLE_RATE else resample_ratio(sample_rate)
-        max_frames = model.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
         self.W = _frame_multiple(window, "window")
         self.V = _frame_multiple(overlap, "overlap")
-        plan_windows(max(self.W, 1), window, overlap, model._encoded_length, max_frames)   # the window plan's refusals
+        plan_windows(max(self.W, 1), window, overlap, model._encoded_length, model._max_frames)   # the window plan's refusals
         if batch_size < 1:
             raise ValueError("batch_size must be >= 1")
         self.names: List[str] = []
         self.kw_ids: List[List[int]] = []
         if keywords is not None:
-            if model._ncfg["head"].get("type") == "rnnt":
-                raise NotImplementedError("keywords in streams need a CTC head: an RNN-T model has no per-frame posteriors "
-                                          "without its [T, U + 1] lattice; use a *_ctc model")
+            model._needs_head(False, "keywords in streams need a CTC head: an RNN-T model has no per-frame posteriors without "
+                                     "its [T, U + 1] lattice; use a *_ctc model")
             self.names, self.kw_ids = model._keyword_ids(keywords, threshold)
         self.model, self.window, self.overlap = model, window, overlap
         self.batch_size, self.confidence, self.threshold = int(batch_size), bool(confidence), threshold
@@ -398,54 +396,28 @@ class StreamServer:
         for a stream that is not open, pause < 0, max_segment <= 0 and, after freeing the stream, for one whose samples
         encode to no frame (as `transcribe_windowed` does)."""
         s = self._get(stream, "close")
-        if not pause >= 0:
-            raise ValueError(f"pause={pause} s must be >= 0")
-        if not max_segment > 0:
-            raise ValueError(f"max_segment={max_segment} s must be positive")
+        check_segmenting(pause, max_segment)
         del self._streams[stream]
         self._free.append(s.slot)
         if self._ratio is not None:
             self._resample([s], final=True)
-        max_frames = self.model.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
-        windows, T = plan_windows(s.n, self.window, self.overlap, self.model._encoded_length, max_frames)
+        windows, T = plan_windows(s.n, self.window, self.overlap, self.model._encoded_length, self.model._max_frames)
         N, done = s.n, len(s.windows)
         assert windows[:done] == s.windows, "a ready window differs from the plan of the whole stream"
         self._run([(s, w) for w in windows[done:]], tentative=False)
-        eng, tok = self._eng, self.model.decoding.tokenizer
         detections = None
         if self.kw_ids:
-            dev = eng.device
+            dev = self._eng.device
             one = torch.tensor([s.slot], device=dev)
             flags = torch.tensor([[0], [0], [0], [1]], dtype=torch.int32, device=dev)   # lo = hi = 0, finish
-            lp = torch.zeros((1, 1, eng.num_classes), dtype=torch.float32, device=dev)
+            lp = torch.zeros((1, 1, self._eng.num_classes), dtype=torch.float32, device=dev)
             self._read_spot([s], self._spot_round(one, lp, flags[0], flags[1], flags[2], flags[3], 0))
-            detections = self._stream_detections(s, compute_frame_shift(N, T))
-        n = len(s.ids)
-        ids_d = torch.tensor(s.ids or [0], dtype=torch.int32).reshape(1, -1).to(eng.device)
-        frames_d = torch.tensor(s.frames or [0], dtype=torch.int32).reshape(1, -1).to(eng.device)
-        counts_d = torch.tensor([n], dtype=torch.int32, device=eng.device)
-        ws, we, wf, wn, k = (t[0].cpu().tolist() for t in eng.group_words(ids_d, frames_d, counts_d, self.model._word_flags()))
-        shift = compute_frame_shift(N, T)
-        words = words_from_device(tok, s.ids, ws[:k], we[:k], wf[:k], wn[:k], shift, s.token_logp if self.confidence else None)
-        cuts = segment_cuts(list(zip(ws[:k], we[:k])), T, shift, pause, max_segment)
-        frame_logp = np.concatenate(s.frame_logp) if self.confidence else None
-        frame_rows = np.concatenate(s.frame_rows) if self.confidence else None
-        segs = windowed_segments(tok, s.ids, s.frames, cuts, shift, N / SAMPLE_RATE, words if word_timestamps else None, ws[:k],
-                                 frame_logp, frame_rows)
-        return StreamResult(transcript=LongformTranscriptionResult(segments=segs), detections=detections)
-
-    def _stream_detections(self, s: _Stream, shift: float) -> List[Detection]:
-        """A closed stream's detections through `spot`'s record builder."""
-        K, width = len(s.dets), max(1, max(len(d) for d in s.dets))
-        start = torch.full((K, width), -1, dtype=torch.int32)
-        end, score = start.clone(), torch.full((K, width), float("-inf"))
-        for k, d in enumerate(s.dets):
-            if d:
-                start[k, :len(d)] = torch.tensor([x[0] for x in d], dtype=torch.int32)
-                end[k, :len(d)] = torch.tensor([x[1] for x in d], dtype=torch.int32)
-                score[k, :len(d)] = torch.tensor([x[2] for x in d], dtype=torch.float32)
-        count = torch.tensor([len(d) for d in s.dets], dtype=torch.int32)
-        return self.model._detections(self.names, self.kw_ids, start, end, score, count, shift)
+            detections = self.model._detections(self.names, self.kw_ids, s.dets, compute_frame_shift(N, T))
+        transcript = windowed_result(self.model, s.ids, s.frames, s.token_logp if self.confidence else None,
+                                     np.concatenate(s.frame_logp) if self.confidence else None,
+                                     np.concatenate(s.frame_rows) if self.confidence else None, N, T, word_timestamps, pause,
+                                     max_segment)
+        return StreamResult(transcript=transcript, detections=detections)
 
     @property
     def streams(self) -> List[int]:

@@ -400,21 +400,20 @@ class _Recorder:
         raise AssertionError(f"unexpected engine call {name}")
 
 
-def test_hotwords_none_calls_what_it_called_before(monkeypatch):
+def test_hotwords_none_runs_the_plain_path(monkeypatch):
     import gigaam_b200.longform as longform
     model = _cpu_model("v2_ctc")
     log = []
     enc = torch.zeros((1, 768, 25))
     monkeypatch.setattr(model, "forward", lambda wav, length: (log.append("forward"), (enc, torch.tensor([25])))[1])
     monkeypatch.setattr(model, "_decode", lambda *a: (log.append(("decode",) + tuple(a[3:])), [("txt", None, None)])[1])
-    monkeypatch.setattr(model, "_transcribe_hotwords", lambda *a: pytest.fail("hotword path taken"))
+    eng = _Recorder()                     # fails on ctc_log_probs, ctc_spot, ctc_bias and any other engine call
+    monkeypatch.setattr(model, "_get_engine", lambda: eng)
     wav = np.zeros(16000, np.float32)
     for kwargs in ({}, {"hotwords": None}):
         log.clear()
         assert model.transcribe(wav, word_timestamps=True, **kwargs).text == "txt"
-        assert log == ["forward", ("decode", True, False)]
-    eng = _Recorder()
-    monkeypatch.setattr(model, "_get_engine", lambda: eng)
+        assert log == ["forward", ("decode", True, False)] and eng.calls == []
     monkeypatch.setattr(torch.Tensor, "pin_memory", lambda self: self)
 
     def fake_decode(m, host, windows, T, batch_size, scores, *extra, **kw):

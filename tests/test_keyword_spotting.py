@@ -505,7 +505,7 @@ def test_every_greedy_word_is_found_where_transcribe_puts_it(name, seconds):
 
 
 @pytest.mark.gpu
-def test_long_recording_equals_the_stitched_log_probs():
+def test_long_recording_equals_spotting_the_stitched_log_probs():
     model = _model("v2_ctc")
     eng = model._get_engine()
     tok = model.decoding.tokenizer
@@ -524,7 +524,9 @@ def test_long_recording_equals_the_stitched_log_probs():
         kw, kw_len = _pad(ids)
         out = eng.ctc_spot(lp, torch.tensor([T]), kw, kw_len, 0.05, T)
     from gigaam_b200.timestamps_utils import compute_frame_shift
-    want = model._detections(names, ids, *(t[0].cpu() for t in out), compute_frame_shift(int(length[0]), T))
+    start, end, score, count = (t[0].cpu() for t in out)
+    stored = [list(zip(start[k, :c].tolist(), end[k, :c].tolist(), score[k, :c].tolist())) for k, c in enumerate(count.tolist())]
+    want = model._detections(names, ids, stored, compute_frame_shift(int(length[0]), T))
     print(f"\n{len(dets)} detections over {T} frames")
     assert dets == want and len(dets) >= 10
     # one window: the same as spot_batch

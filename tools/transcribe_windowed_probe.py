@@ -22,7 +22,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import torch  # noqa: E402
 
 import gigaam_b200 as gigaam  # noqa: E402
-from gigaam_b200 import _lib, longform  # noqa: E402
+from gigaam_b200 import longform  # noqa: E402
 
 dev = torch.device("cuda", 0)
 
@@ -50,7 +50,7 @@ def main():
         model = gigaam.load_model(name, fp16_encoder=True, device=dev, checkpoint=ck)
         for minutes in ((10,) if quick else (10, 60)):
             wav = gigaam.synthetic_audio(1, 60.0 * minutes, seed=minutes)[0][0]
-            max_frames = model.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
+            max_frames = model._max_frames
             windows, T = longform.plan_windows(wav.numel(), 30.0, 4.0, model._encoded_length, max_frames)
             host = wav.to(model._dtype).pin_memory()
 
