@@ -17,7 +17,7 @@ from typing import Dict, Optional, Union
 
 import torch
 
-from .engine import max_encoded_frames_config
+from .engine import check_attention_heads, max_encoded_frames_config
 from .model import GigaAM, GigaAMASR, GigaAMEmo, check_emo_head
 from .preprocess import load_audio, read_audio
 from .synthetic import synthetic_audio, synthetic_checkpoint
@@ -102,6 +102,7 @@ def load_model(model_name: str, fp16_encoder: bool = True, use_flash: Optional[b
     else:
         model = GigaAM(cfg) if "ssl" in model_name else GigaAMASR(cfg)
     max_encoded_frames_config(max_encoded_frames, model.encoder.cfg["pos_emb_max_len"])   # ValueError before any device work
+    check_attention_heads(model.encoder.cfg)                                                 # likewise
     model.load_state_dict(checkpoint["state_dict"])
     model = model.eval()
     model.__dict__["_pack_cache_base"] = pack_cache_base    # packed-weight cache next to the checkpoint (model.py)

@@ -82,6 +82,9 @@ PROTOTYPES = parse_prototypes(_HEADER)
 EXPORTS = tuple(PROTOTYPES)
 # the default longest T' (GamConfig.max_encoded_frames = 0)
 REL_POS_MAX_T = int(re.search(r"#define\s+GAM_REL_POS_MAX_T\s+(\d+)", _HEADER).group(1))
+# the widest head d_k each attention kernel runs (gam_create refuses wider ones)
+ROTARY_MAX_DK = int(re.search(r"#define\s+GAM_ROTARY_MAX_DK\s+(\d+)", _HEADER).group(1))
+REL_POS_MAX_DK = int(re.search(r"#define\s+GAM_REL_POS_MAX_DK\s+(\d+)", _HEADER).group(1))
 
 
 def lib_path() -> Path:

@@ -25,12 +25,15 @@
 // keys j > i + max_t - 1 >= T, which are masked.  Before its start (row < 0: r > max_t-1, which happens in the last query
 // tile when max_t is not a multiple of 128, e.g. 5000 = 39*128 + 8) they only meet queries i > j + max_t - 1 >= T, whose
 // rows are never stored.
+#include "../../include/gigaam_b200.h"
 #include "kernels.h"
 #include "launch.cuh"
 #include "ptx.cuh"
 
 namespace gam {
 namespace {
+
+static_assert(GAM_REL_POS_MAX_DK == 4 * 16, "launch_attention_relpos instantiates KS = 1 .. 4");
 
 constexpr int kThreads = 256;
 constexpr int kTile = 128 * 128;         // bytes of a 128-row x 64-column fp16 tile
@@ -279,7 +282,7 @@ int launch_ks(const CUtensorMap* tmap_qkv, const CUtensorMap* tmap_pos, const Re
 int launch_attention_relpos(const CUtensorMap* tmap_qkv, const CUtensorMap* tmap_pos, int max_t, const int* klen, const int* cu,
                             __half* out, int B, int T, int H, int dk, int d_model, cudaStream_t s) {
   const int nkb = (T + 127) / 128;
-  if (nkb <= 0 || T > max_t || dk % 16 != 0 || dk > 64 || (cu != nullptr && klen == nullptr)) return -1;
+  if (nkb <= 0 || T > max_t || dk % 16 != 0 || dk > GAM_REL_POS_MAX_DK || (cu != nullptr && klen == nullptr)) return -1;
   RelParams p;
   p.T = T;
   p.klen = klen;

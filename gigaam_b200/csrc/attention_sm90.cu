@@ -24,6 +24,7 @@
 //   * LAZY reference point: exact block maximum on the first block; afterwards it moves only when a block maximum exceeds
 //     it by more than 2^8 (P then stays <= 256, far inside fp16).  Moving it rescales O and the row sum;
 //   * the denominator is the fp32 sum of exactly the fp16 P that P.V used.
+#include "../../include/gigaam_b200.h"
 #include "kernels.h"
 #include "launch.cuh"
 #include "ptx.cuh"
@@ -31,7 +32,9 @@
 namespace gam {
 namespace {
 
-constexpr int kMaxKB = 6;              // K / V stages: 768 keys resident (30 s segments of the reference's VAD, gigaam/vad_utils.py:85)
+static_assert(GAM_ROTARY_MAX_DK == 3 * 16, "launch_attention instantiates KS = 1 .. 3");
+
+constexpr int kMaxKB = 6;             // K / V stages: 768 keys resident (30 s segments of the reference's VAD, gigaam/vad_utils.py:85)
 constexpr int kTileBytes = 128 * 128;  // 128 rows x 64 fp16
 constexpr int kThreads = 256;
 constexpr float kLazyLog2 = 8.0f;      // the softmax reference point trails the running maximum by at most 2^8
@@ -242,7 +245,7 @@ int launch_ks(const CUtensorMap* tmap_qkv, const AttnParams& p, int B, int H, cu
 int launch_attention(const CUtensorMap* tmap_qkv, const int* klen, const int* cu, __half* out, int B, int T, int H, int dk,
                      int d_model, cudaStream_t s) {
   const int nkb = (T + 127) / 128;
-  if (nkb <= 0 || dk % 16 != 0 || dk > 48 || (cu != nullptr && klen == nullptr)) return -1;
+  if (nkb <= 0 || dk % 16 != 0 || dk > GAM_ROTARY_MAX_DK || (cu != nullptr && klen == nullptr)) return -1;
   AttnParams p;
   p.T = T;
   p.nkb = nkb;

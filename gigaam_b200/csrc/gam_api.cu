@@ -363,9 +363,15 @@ int gam_create(const gam_config* cfg, const gam_weights* w, int device, gam_hand
   if (c.subsampling == 1 && (c.feat_in % 64 != 0 || (c.subs_kernel_size & 1) == 0))
     return fail(h, -10, "conv1d subsampling needs feat_in %% 64 == 0 and an odd kernel size");
   if (c.self_attention != 0 && c.self_attention != 1) return fail(h, -10, "unknown self_attention type %d", c.self_attention);
-  if (c.d_model != 768 || c.d_model % c.n_heads != 0 || (c.d_model / c.n_heads) % 16 != 0)
+  if (c.d_model != 768 || c.n_heads <= 0 || c.d_model % c.n_heads != 0 || (c.d_model / c.n_heads) % 16 != 0)
     return fail(h, -10, "unsupported d_model/n_heads (%d/%d): kernels are specialised for d_model 768, d_k %% 16 == 0",
                 c.d_model, c.n_heads);
+  {  // refused here, not at the first encode: the attention launchers check the same limits
+    const int dk = c.d_model / c.n_heads, dk_max = c.self_attention == 0 ? GAM_ROTARY_MAX_DK : GAM_REL_POS_MAX_DK;
+    if (dk > dk_max)
+      return fail(h, -10, "%s attention runs heads of d_k <= %d, but d_model %d / n_heads %d gives d_k = %d",
+                  c.self_attention == 0 ? "rotary" : "rel_pos", dk_max, c.d_model, c.n_heads, dk);
+  }
   if (c.d_ff % 256 != 0 || (c.subsampling == 0 && c.subs_kernel_size != 3)) return fail(h, -10, "unsupported d_ff / subs_kernel_size");
   if (c.win_length != c.n_fft) return fail(h, -10, "win_length != n_fft is not supported");
   if (c.n_mels < 1 || c.n_mels > 64) return fail(h, -10, "n_mels %d outside [1, 64]: the log-mel kernels hold 64 mel rows", c.n_mels);

@@ -126,6 +126,20 @@ def max_encoded_frames_config(max_encoded_frames: Optional[int], pos_emb_max_len
     return int(max_encoded_frames)
 
 
+def check_attention_heads(enc: Dict) -> None:
+    """Refuse, before any device work, a head width d_k = d_model / n_heads wider than the attention kernel of this
+    encoder runs (_lib.ROTARY_MAX_DK / REL_POS_MAX_DK, the header's limits, which gam_create also enforces).  The other
+    shape limits (d_model 768, d_k % 16 == 0) are gam_create's."""
+    d, h = enc["d_model"], enc["n_heads"]
+    if h <= 0 or d % h != 0:
+        return
+    kind = enc["self_attention_model"]
+    dk_max = _lib.REL_POS_MAX_DK if kind == "rel_pos" else _lib.ROTARY_MAX_DK
+    if d // h > dk_max:
+        raise ValueError(f"{kind} attention runs heads of d_k <= {dk_max}, but d_model {d} / n_heads {h} gives "
+                         f"d_k = {d // h}")
+
+
 def rotary_half_tables(dk: int, base: float, max_len: int):
     """cos/sin [max_len, dk/2] of t * base^(-2i/dk) (gigaam/encoder.py:342-355; base = pos_emb_max_len)."""
     inv_freq = 1.0 / (base ** (torch.arange(0, dk, 2).float() / dk))
@@ -208,6 +222,7 @@ class Engine:
         self.cfg = cfg
         self._keep: List[Tensor] = []
         enc = cfg["encoder"]
+        check_attention_heads(enc)
         gc_max = max_encoded_frames_config(max_encoded_frames, enc["pos_emb_max_len"])
         self.max_encoded_frames = gc_max or _lib.REL_POS_MAX_T
         # the limit sizes the rel_pos position tables that go through _dev(): a cache written for one limit must not be

@@ -89,6 +89,10 @@ typedef struct gam_layer_weights {
 } gam_layer_weights;
 
 #define GAM_REL_POS_MAX_T 768 /* default longest T' (6 key blocks of 128 = 30.7 s of audio); see max_encoded_frames */
+/* widest head d_k = d_model / n_heads each attention kernel runs (its per-warp Q and O fragments are specialised for
+ * d_k / 16 k16 steps); gam_create refuses a wider one */
+#define GAM_ROTARY_MAX_DK 48
+#define GAM_REL_POS_MAX_DK 64
 
 typedef struct gam_weights {
   /* front end */

@@ -528,6 +528,26 @@ def _rope_tables64(dk, base, dev):
     return inv
 
 
+def rope_ref(y, dy, t, dk, base):
+    """The oracle's rotary formula (x * cos + rotate_half(x) * sin) on float64 tables, applied per head of dk to the rows
+    y (with their error dy) at positions t, and the bound of the kernel's fp32 result with the engine's fp32
+    rotary_half_tables (before the fp16 store)."""
+    n = y.shape[0]
+    inv = _rope_tables64(dk, base, y.device)
+    ang = t.double()[:, None] * torch.cat([inv, inv])[None, :]                     # [n, dk]
+    c, s = torch.cos(ang)[:, None, :], torch.sin(ang)[:, None, :]
+    yh, dyh = y.view(n, D // dk, dk), dy.view(n, D // dk, dk)
+    want = (yh * c + orc._rtt_half(yh) * s).reshape(n, D)
+    # fp32 tables: the rounded exponent 2i/dk moves base^e by ln(5000) e u <= 8.5 u, pow (1 ulp) and the reciprocal add
+    # 3 u, the product t * inv_freq one more; cos / sin of the fp32 angle within 1 ulp + rounding:
+    # |table error| <= 16 u * angle + 3 u
+    dtab = 16 * U * ang.abs()[:, None, :] + 3 * U
+    yp = orc._rtt_half(yh).abs()
+    tol = (dyh * c.abs() + orc._rtt_half(dyh).abs() * s.abs() + (yh.abs() + yp) * dtab
+           + 2 * U * (yh.abs() * c.abs() + yp * s.abs())).reshape(n, D)
+    return want, tol
+
+
 @pytest.mark.parametrize("positions", ["plan", "row_mod_T"])
 @pytest.mark.parametrize("reverse", [0, 1])
 def test_ln_rope(eng, dev, positions, reverse):
@@ -554,18 +574,7 @@ def test_ln_rope(eng, dev, positions, reverse):
           rows_dev, row_t, T, reverse)
     y, dy = _ln_ref(x[:n], gamma, beta)
     _assert_within(ou[:n], y, dy + _f16_store(y), "out_u")
-    inv = _rope_tables64(dk, base, dev)
-    ang = t.double()[:, None] * torch.cat([inv, inv])[None, :]                     # [n, dk]
-    c, s = torch.cos(ang)[:, None, :], torch.sin(ang)[:, None, :]
-    yh, dyh = y.view(n, 16, dk), dy.view(n, 16, dk)
-    want = (yh * c + orc._rtt_half(yh) * s).reshape(n, D)
-    # fp32 tables: the rounded exponent 2i/48 moves base^e by ln(5000) e u <= 8.5 u, pow (1 ulp) and the reciprocal add
-    # 3 u, the product t * inv_freq one more; cos / sin of the fp32 angle within 1 ulp + rounding:
-    # |table error| <= 16 u * angle + 3 u
-    dtab = 16 * U * ang.abs()[:, None, :] + 3 * U
-    yp = orc._rtt_half(yh).abs()
-    tol = (dyh * c.abs() + orc._rtt_half(dyh).abs() * s.abs() + (yh.abs() + yp) * dtab
-           + 2 * U * (yh.abs() * c.abs() + yp * s.abs())).reshape(n, D)
+    want, tol = rope_ref(y, dy, t, dk, base)
     _assert_within(orr[:n], want, tol + _f16_store(want), f"out_r positions={positions}")
     assert bool((ou[n:] == SENT16).all() and (orr[n:] == SENT16).all())
 
