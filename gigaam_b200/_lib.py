@@ -85,6 +85,9 @@ REL_POS_MAX_T = int(re.search(r"#define\s+GAM_REL_POS_MAX_T\s+(\d+)", _HEADER).g
 # the widest head d_k each attention kernel runs (gam_create refuses wider ones)
 ROTARY_MAX_DK = int(re.search(r"#define\s+GAM_ROTARY_MAX_DK\s+(\d+)", _HEADER).group(1))
 REL_POS_MAX_DK = int(re.search(r"#define\s+GAM_REL_POS_MAX_DK\s+(\d+)", _HEADER).group(1))
+# the widest joint_hidden the fused RNN-T loss runs, and the widest pred_hidden the prediction network trains at
+RNNT_LOSS_MAX_JOINT_HIDDEN = int(re.search(r"#define\s+GAM_RNNT_LOSS_MAX_JOINT_HIDDEN\s+(\d+)", _HEADER).group(1))
+PREDICT_BACKWARD_MAX_HIDDEN = int(re.search(r"#define\s+GAM_PREDICT_BACKWARD_MAX_HIDDEN\s+(\d+)", _HEADER).group(1))
 
 
 def lib_path() -> Path:

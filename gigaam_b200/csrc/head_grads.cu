@@ -13,6 +13,7 @@
 //   (6) class_gate_sum_kernel: the gate gradients of all steps whose input was class v, in row order.
 #include <cmath>
 
+#include "../../include/gigaam_b200.h"
 #include "kernels.h"
 
 namespace gam {
@@ -410,7 +411,12 @@ void launch_segment_sum(const float* X, float* out, int64_t groups, int count, i
   segment_sum_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(X, out, groups, count, K, gi, so, si, step);
 }
 
-int lstm_bwd_max_hidden() { return static_cast<int>(48 * 1024 / (kBPB * 5 * 4)); }
+// lstm_bwd_step_kernel's dynamic shared memory: h_{u-1} and dgates of kBPB utterances, 5 H floats each, within the 48 KiB a
+// launch gets without opting in
+constexpr int kLstmBwdMaxHidden = 48 * 1024 / (kBPB * 5 * 4);
+static_assert(kLstmBwdMaxHidden == GAM_PREDICT_BACKWARD_MAX_HIDDEN, "the header's pred_hidden limit of the predict backward");
+
+int lstm_bwd_max_hidden() { return kLstmBwdMaxHidden; }
 
 void launch_lstm_bwd_step(const int64_t* x, int U, int u, int V1, const float* emb_gates, const float* whh_t, const float* whh,
                           const float* h0, const float* c0, const float* g, const float* c_seq, const float* dG, const float* dh1,

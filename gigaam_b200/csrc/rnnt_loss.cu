@@ -16,6 +16,7 @@
 // All fp32 with expf / logf, no atomics, every sum in an order fixed by the sizes: repeated calls give the same bits.
 #include <cmath>
 
+#include "../../include/gigaam_b200.h"
 #include "kernels.h"
 #include "launch.cuh"
 
@@ -428,11 +429,21 @@ __global__ void __launch_bounds__(kLThreads) rnnt_loss_class_grad_kernel(
   }
 }
 
-size_t node_smem_bytes(int J, int tU) {
+constexpr size_t node_smem_bytes(int J, int tU) {
   return (static_cast<size_t>(loss_kpad(J)) * kLLd + kLK * kLLd + kLN * kLLd + kLK * loss_nc(J) * 64 + static_cast<size_t>(tU) * J) * 4;
 }
-size_t class_smem_bytes(int J) { return (static_cast<size_t>(loss_nc(J)) * 64 * kLLd + kLK * kLLd + kLM * kLLd) * 4; }
+constexpr size_t class_smem_bytes(int J) { return (static_cast<size_t>(loss_nc(J)) * 64 * kLLd + kLK * kLLd + kLM * kLLd) * 4; }
 constexpr size_t kLossMaxSmem = 227 * 1024 - sizeof(RowInfo);
+
+// the widest J (a multiple of 4) both gradient kernels hold in registers and shared memory at every strip width
+constexpr int loss_max_hidden() {
+  int J = 4;
+  while (loss_nc(J + 4) <= kLMaxNC && node_smem_bytes(J + 4, kLM) <= kLossMaxSmem && class_smem_bytes(J + 4) <= kLossMaxSmem) J += 4;
+  return J;
+}
+static_assert(loss_max_hidden() == GAM_RNNT_LOSS_MAX_JOINT_HIDDEN, "the header's joint_hidden limit of the fused loss");
+static_assert(node_smem_bytes(GAM_RNNT_LOSS_MAX_JOINT_HIDDEN, kLM) == kLossMaxSmem,
+              "at the widest joint the node kernel uses all of its shared memory (DESIGN.md section 4)");
 
 template <int NC>
 int launch_grads(const RnntLossArgs& a, const RnntLossPlan& p, float* dE_part, float* dP_part, float* part, float* dW, float* db,
@@ -466,11 +477,7 @@ int launch_grads(const RnntLossArgs& a, const RnntLossPlan& p, float* dE_part, f
 
 }  // namespace
 
-int rnnt_loss_max_hidden() {
-  int J = 4;
-  while (loss_nc(J + 4) <= kLMaxNC && node_smem_bytes(J + 4, kLM) <= kLossMaxSmem && class_smem_bytes(J + 4) <= kLossMaxSmem) J += 4;
-  return J;
-}
+int rnnt_loss_max_hidden() { return loss_max_hidden(); }
 
 RnntLossPlan rnnt_loss_plan(int B, int T, int U, int V1) {
   RnntLossPlan p;

@@ -11,7 +11,7 @@ from typing import Dict, Optional, Tuple
 import torch
 from torch import Tensor
 
-from . import synthetic
+from . import _lib, synthetic
 from ._params import Bound, build_tree
 from .decoding import _as_btd
 
@@ -209,7 +209,9 @@ class RNNTDecoder(Bound):
                 ) -> Tuple[Tensor, Tuple[Tensor, Tensor]]:
         """x [B, U] label ids or None (one step from the zero embedding, `batch_size` rows); state (h, c), each
         [1, B, pred_hidden] (strided views are fine), or None (zeros) -> (g [B, U, pred_hidden], (h, c) [1, B, pred_hidden])
-        (gigaam/decoder.py:85-102).  A row with an id outside [0, num_classes) comes back as NaN."""
+        (gigaam/decoder.py:85-102).  A row with an id outside [0, num_classes) comes back as NaN.  With a gradient to
+        compute, pred_hidden above the backward's limit raises ValueError before any launch."""
+        self._check_trainable(*(state if state is not None else ()))
         eng = self._engine()
         if x is not None:
             x = _on_device(x, eng, torch.int64).contiguous()
@@ -227,6 +229,14 @@ class RNNTDecoder(Bound):
         else:
             g, h1, c1 = eng.rnnt_predict(x, h, c, batch_size)
         return g, (h1.unsqueeze(0), c1.unsqueeze(0))
+
+    def _check_trainable(self, *state: Tensor) -> None:
+        """A call that would need gam_rnnt_predict_backward at a pred_hidden it cannot run is refused here, before its
+        forward launches; without a gradient every width up to the forward's runs."""
+        limit = _lib.PREDICT_BACKWARD_MAX_HIDDEN
+        if self.pred_hidden > limit and _trains(self, *state):
+            raise ValueError(f"predict: pred_hidden {self.pred_hidden} cannot be trained: the prediction network's backward "
+                             f"runs pred_hidden <= {limit}; call it without gradients or freeze head.decoder")
 
     def forward(self, x: Tensor, h: Tensor, c: Tensor) -> Tuple[Tensor, Tensor, Tensor]:
         """ONNX form of predict: (x, h, c) -> (g, h, c) (gigaam/decoder.py:131-137)"""

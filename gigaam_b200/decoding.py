@@ -10,6 +10,8 @@ import numpy as np
 import torch
 from torch import Tensor
 
+from . import _lib
+
 
 class Tokenizer:
     """gigaam/decoding.py:10-44 -- charwise vocabulary or a SentencePiece model."""
@@ -156,12 +158,23 @@ def rnnt_loss(head, encoded: Tensor, encoded_len: Tensor, targets: Tensor, targe
     the prediction network runs through head.decoder.predict and the joint through the fused loss, so gradients reach
     decoder.embed / decoder.lstm, joint.enc / joint.pred / joint.joint_net.1 and `encoded` when it requires grad.  An
     utterance with encoded_len 0 has loss +inf and no gradient.  No host synchronisation: the call can be captured in a CUDA
-    graph.  CTC heads raise NotImplementedError (use F.ctc_loss on model.head(encoded)); another reduction raises ValueError."""
+    graph.  CTC heads raise NotImplementedError (use F.ctc_loss on model.head(encoded)); another reduction, a joint_hidden or
+    pred_hidden the fused loss does not run, and a gradient through a prediction network wider than the predict backward
+    runs raise ValueError before any device work."""
     if reduction not in _REDUCTIONS:
         raise ValueError(f"rnnt_loss: reduction must be one of {_REDUCTIONS}, got {reduction!r}")
     if getattr(head, "decoder", None) is None or getattr(head, "joint", None) is None:
         raise NotImplementedError("rnnt_loss needs an RNN-T head; for a CTC model use torch.nn.functional.ctc_loss on the "
                                   "log-probs of model.head(encoded), transposed to [T, B, V+1]")
+    J = head.joint_cfg["joint_hidden"]
+    if J % 4 != 0 or J > _lib.RNNT_LOSS_MAX_JOINT_HIDDEN:
+        raise ValueError(f"rnnt_loss: joint_hidden {J} is not supported: the fused loss runs joint_hidden <= "
+                         f"{_lib.RNNT_LOSS_MAX_JOINT_HIDDEN}, a multiple of 4")
+    H = head.decoder.pred_hidden
+    if H % 16 != 0:   # the projection GEMM's k-step (gam_api.cu, proj_shapes_ok)
+        raise ValueError(f"rnnt_loss: pred_hidden {H} is not supported: the fused loss projects pred_hidden in steps of 16, "
+                         f"so it must be a multiple of 16")
+    head.decoder._check_trainable()
     eng = head._engine()
     enc = _as_btd(encoded.to(device=eng.device, dtype=torch.float32))
     targets = targets.to(device=eng.device)

@@ -972,7 +972,7 @@ class Engine:
         B, T, U, targets, enc_len, target_len = self._loss_args(enc, dec, targets, enc_len, target_len, "rnnt_loss")
         ws = self._ws(None, None, "gam_rnnt_loss_workspace_bytes", B, T, U,
                       what=f"rnnt_loss: unsupported sizes B={B}, T={T}, U={U} (limits: T <= the model's max_encoded_frames, "
-                           f"U <= 4096 tokens, joint_hidden <= 344)")
+                           f"U <= 4096 tokens, joint_hidden <= {_lib.RNNT_LOSS_MAX_JOINT_HIDDEN})")
         saved = self._empty(3, B, T, U + 1)
         loss = self._empty(B)
         self._call("gam_rnnt_loss", enc, dec, targets, enc_len, target_len, B, T, U, ws, ws.numel(), saved, loss)

@@ -93,6 +93,13 @@ typedef struct gam_layer_weights {
  * d_k / 16 k16 steps); gam_create refuses a wider one */
 #define GAM_ROTARY_MAX_DK 48
 #define GAM_REL_POS_MAX_DK 64
+/* widest joint_hidden the fused RNN-T loss runs (gam_rnnt_loss*): its gradient kernels hold six 64-unit chunks of a hidden row
+ * in registers, and at joint_hidden 344 with a 64-column strip the node kernel's dynamic shared memory is exactly the 227 KiB
+ * per-block limit minus its row table */
+#define GAM_RNNT_LOSS_MAX_JOINT_HIDDEN 344
+/* widest pred_hidden gam_rnnt_predict_backward runs: its BPTT step keeps 5 pred_hidden floats of 4 utterances in the 48 KiB
+ * of shared memory a launch gets by default (49 120 bytes at 614) */
+#define GAM_PREDICT_BACKWARD_MAX_HIDDEN 614
 
 typedef struct gam_weights {
   /* front end */
@@ -572,7 +579,7 @@ int gam_rnnt_joint_backward(gam_handle* h, const float* enc, const float* dec, i
  * w_hh [4H, H] are the module's lstm / embed weights (w_hh must match the packed one).  Outputs: d_h0, d_c0 [B, H]; d_embed
  * [V+1, H] with a zero blank row (nn.Embedding's padding_idx); dW_ih, dW_hh [4H, H]; d_bias [4H], the gradient of both
  * bias_ih_l0 and bias_hh_l0.  An utterance with an id outside [0, V] gets NaN in its d_h0 / d_c0 (and the weight gradients it
- * feeds).  pred_hidden <= 614. */
+ * feeds).  pred_hidden <= GAM_PREDICT_BACKWARD_MAX_HIDDEN. */
 int64_t gam_rnnt_predict_backward_workspace_bytes(const gam_handle* h, int32_t B, int32_t U);
 int gam_rnnt_predict_backward(gam_handle* h, const int64_t* x, const float* h0, const float* c0, int32_t B, int32_t U, const float* g,
                               const float* c_seq, const float* grad_g, const float* grad_h1, const float* grad_c1, const float* embed,
@@ -602,7 +609,7 @@ int gam_rnnt_predict_backward(gam_handle* h, const int64_t* x, const float* h0, 
  *
  * Sizes: enc [B, T, d_model], dec [B, U+1, pred_hidden] (gam_rnnt_predict over cat[blank, y]), targets [B, U] i32, enc_len [B],
  * target_len [B] i32, all device.  Limits are gam_rnnt_align's (U <= 4096, T <= the handle's max_encoded_frames) plus
- * joint_hidden <= 344 (a multiple of 4); the *_bytes functions return -1 beyond them or for a handle without an RNN-T head.
+ * joint_hidden <= GAM_RNNT_LOSS_MAX_JOINT_HIDDEN (a multiple of 4); the *_bytes functions return -1 beyond them or for a handle without an RNN-T head.
  * Memory, N = B T (U+1) nodes, J = joint_hidden, fp32:
  *   saved (kept between the calls): 12 N bytes = [lse | e_blank | e_label], each [B, T, U+1];
  *   forward workspace: 12 N bytes (blank, label, alpha) + 4 (B T + B (U+1)) J bytes (the projections), 1 KiB-aligned pieces;

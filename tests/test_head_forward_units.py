@@ -184,9 +184,9 @@ def dev():
     return torch.device("cuda", 0)
 
 
-def _cfg(name, V1=None, J=None, H=None):
-    """synthetic.model_cfg with one encoder layer, V+1 classes, joint_hidden J and pred_hidden H"""
-    cfg = synthetic.model_cfg(name, n_layers=1)
+def _cfg(name, V1=None, J=None, H=None, n_layers=1):
+    """synthetic.model_cfg with n_layers encoder layers, V+1 classes, joint_hidden J and pred_hidden H"""
+    cfg = synthetic.model_cfg(name, n_layers=n_layers)
     h = cfg["head"]
     if V1 is not None:
         cfg["decoding"]["vocabulary"] = [f"<{i}>" for i in range(V1 - 1)]

@@ -267,21 +267,19 @@ def _dev():
     return torch.device("cuda", 0)
 
 
-def _model(name, V1=None, scale=0.05, seed=0):
-    """A 2-layer synthetic model on the GPU with a head that is not saturated.  V1 overrides the vocabulary size."""
-    cfg = synthetic.model_cfg(name, n_layers=2)
-    if V1 is not None:
-        voc = [f"<{i}>" for i in range(V1 - 1)]
-        cfg["decoding"]["vocabulary"] = voc
-        cfg["decoding"].pop("model_path", None)
-        h = cfg["head"]
-        if h["type"] == "ctc":
-            h["num_classes"] = V1
-        else:
-            h["decoder"]["num_classes"] = h["joint"]["num_classes"] = V1
+def _head_ckpt(name, V1=None, J=None, H=None, scale=0.05, seed=0):
+    """A 2-layer synthetic checkpoint (V+1 classes, joint_hidden J, pred_hidden H) with a head that is not saturated."""
+    from test_head_forward_units import _cfg
+    cfg = _cfg(name, V1=V1, J=J, H=H, n_layers=2)
     sd = synthetic.synthetic_state_dict(cfg, seed=seed)
     ck = {"cfg": cfg, "state_dict": sd}
     sd.update(_head_sd(ck, scale=scale, seed=seed))
+    return ck
+
+
+def _model(name, V1=None, scale=0.05, seed=0, J=None, H=None):
+    """_head_ckpt's model on the GPU."""
+    ck = _head_ckpt(name, V1=V1, J=J, H=H, scale=scale, seed=seed)
     model = gigaam.load_model(name, device=_dev(), checkpoint=ck, fp16_encoder=False)
     return model, ck
 
@@ -321,7 +319,7 @@ def _ctc_bounds(e64, W, lp64, G64):
 
 
 def _predict_bounds(x, h0, c0, sd, gG, gh1, gc1):
-    """Per-element error bounds of the six predict gradients computed in fp32 (BPTT over U steps of H = 320 units)."""
+    """Per-element error bounds of the six predict gradients computed in fp32 (BPTT over U steps of H units)."""
     B, U, H = gG.shape
     mag = predict_grads(x, h0, c0, sd, gG, gh1, gc1, absm=True)
     return [(4 * H + 40 * U + B * U) * U32 * m for m in mag]
@@ -359,18 +357,22 @@ def test_ctc_backward_against_float64(V1, B, T):
 
 
 def _joint_case(model, B, T, U, g, dev):
-    enc = torch.randn(B, T, 768, generator=g, device=dev).requires_grad_(True)
-    dec = (torch.rand(B, U, 320, generator=g, device=dev) * 2 - 1).requires_grad_(True)
+    enc = torch.randn(B, T, model.head.joint.enc_hidden, generator=g, device=dev).requires_grad_(True)
+    dec = (torch.rand(B, U, model.head.joint.pred_hidden, generator=g, device=dev) * 2 - 1).requires_grad_(True)
     lp = model.head.joint.joint(enc, dec)
     return enc, dec, lp
 
 
+JOINT_CASES = [("v2_rnnt", 34, 32, 251, 7, None), ("v2_rnnt", 257, 4, 60, 100, None), ("v3_e2e_rnnt", 1025, 3, 33, 1, None),
+               ("v3_e2e_rnnt", 1025, 2, 19, 100, None), ("v2_rnnt", 34, 3, 21, 5, 4), ("v2_rnnt", 65, 2, 17, 9, 68),
+               ("v3_e2e_rnnt", 257, 2, 13, 40, 344)]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,V1,B,T,U", [("v2_rnnt", 34, 32, 251, 7), ("v2_rnnt", 257, 4, 60, 100), ("v3_e2e_rnnt", 1025, 3, 33, 1),
-                                             ("v3_e2e_rnnt", 1025, 2, 19, 100)])
-def test_joint_backward_against_float64(name, V1, B, T, U):
+@pytest.mark.parametrize("name,V1,B,T,U,J", JOINT_CASES, ids=["-".join(map(str, c[:5])) + (f"-J{c[5]}" if c[5] else "") for c in JOINT_CASES])
+def test_joint_backward_against_float64(name, V1, B, T, U, J):
     dev = _dev()
-    model, ck = _model(name, V1=V1)
+    model, ck = _model(name, V1=V1, J=J)
     model.head.requires_grad_(True)
     g = torch.Generator(device=dev).manual_seed(V1 + T + U)
     enc, dec, lp = _joint_case(model, B, T, U, g, dev)
@@ -389,36 +391,88 @@ def test_joint_backward_against_float64(name, V1, B, T, U):
     worst = 0.0
     for i, (a, w, bd) in enumerate(zip(got, want, bounds)):
         worst = max(worst, _check_bound(f"joint grad {i}", a, w, bd))
-    print(f"joint V1={V1} B={B} T={T} U={U}: min row entropy {_entropy_min(l64):.3f} nats, worst err/bound {worst:.3g}")
+    print(f"joint V1={V1} J={model.head.joint_cfg['joint_hidden']} B={B} T={T} U={U}: min row entropy {_entropy_min(l64):.3f} nats, "
+          f"worst err/bound {worst:.3g}")
+
+
+def hidden_rows(e64, d64, sd):
+    """-> (z, zerr) [B, T, U, J]: the joint's pre-activation E + P in float64 and the bound of its fp32 error.  E and P are
+    sgemm_bias_kernel's sums (one fma chain over ascending k, then the bias: depth d + 1 and H + 1); the add is one more
+    rounding."""
+    We, be = sd["head.joint.enc.weight"], sd["head.joint.enc.bias"]
+    Wp, bp = sd["head.joint.pred.weight"], sd["head.joint.pred.bias"]
+    d, H = We.shape[1], Wp.shape[1]
+    zE, zP = e64 @ We.t() + be, d64 @ Wp.t() + bp
+    mE, mP = e64.abs() @ We.abs().t() + be.abs(), d64.abs() @ Wp.abs().t() + bp.abs()
+    z = zE[:, :, None, :] + zP[:, None, :, :]
+    return z, U32 * ((d + 1) * mE[:, :, None, :] + (H + 1) * mP[:, None, :, :] + z.abs())
+
+
+def outer_splits(rows, N, Kc):
+    """outer_splits of csrc/head_grads.cu: the number of row slices of an outer sum"""
+    tiles = -(-N // 64) * -(-Kc // 64)
+    S = min(max(-(-264 // tiles), 1), 64)
+    return min(S, max(-(-rows // 256), 1))
+
+
+def outer_depth(rows, N, K):
+    """rounding depth of outer_sum_kernel's sums over `rows` (with the bias column): one fma chain over the rows of a slice
+    (chunk rows, a multiple of 16), then outer_sum_reduce_kernel's sum of the S slices in order when S > 1"""
+    S = outer_splits(rows, N, K + 1)
+    chunk = -(-(-(-rows // S)) // 16) * 16
+    return min(chunk, rows) + (S if S > 1 else 0)
+
+
+def dhid_bounds(dl, dl_err, z, zerr, Wo):
+    """dhid = (dl W_o) [z > 0] over V1 classes in one fma chain (depth V1): -> (magnitude, error bound) [..., J].  A hidden
+    entry whose fp32 pre-activation may sit on the other side of 0 than the float64 one (|z| <= zerr) may flip its ReLU
+    mask: its whole |dl| . |W_o| term may be present on one side only."""
+    V1 = Wo.shape[0]
+    full = dl @ Wo.abs()
+    mask, amb = z > 0, z.abs() <= zerr
+    err = ((dl_err + V1 * U32 * dl) @ Wo.abs()) * mask + full * amb
+    print(f"joint: {int(amb.sum())} of {amb.numel()} hidden entries within fp32 rounding of 0")
+    return full * (mask | amb), err
+
+
+def joint_input_bounds(e64, d64, sd, dE, dE_err, dP, dP_err):
+    """Bounds of (d_enc, d_dec, dW_enc, db_enc, dW_pred, db_pred) as joint_input_grads (gam_api.cu) forms them from dE
+    [B, T, J] / dP [B, U, J] given as their float64 sums of |terms| and the bounds of their own errors: d_enc = dE W_e and
+    d_dec = dP W_p are matmul_kernel's J-deep fma chains, the weight gradients outer sums over B T and B U rows."""
+    We, Wp = sd["head.joint.enc.weight"], sd["head.joint.pred.weight"]
+    J, d, H = We.shape[0], We.shape[1], Wp.shape[1]
+    e, x = e64.abs().reshape(-1, d), d64.abs().reshape(-1, H)
+    E, Ee, P, Pe = dE.reshape(-1, J), dE_err.reshape(-1, J), dP.reshape(-1, J), dP_err.reshape(-1, J)
+    kE, kP = outer_depth(E.shape[0], J, d), outer_depth(P.shape[0], J, H)
+    return [dE_err @ We.abs() + J * U32 * (dE @ We.abs()), dP_err @ Wp.abs() + J * U32 * (dP @ Wp.abs()),
+            Ee.t() @ e + kE * U32 * (E.t() @ e), Ee.sum(0) + kE * U32 * E.sum(0),
+            Pe.t() @ x + kP * U32 * (P.t() @ x), Pe.sum(0) + kP * U32 * P.sum(0)]
 
 
 def _joint_bounds(e64, d64, sd, l64, G64):
-    """Per-element error bounds of the eight joint gradients computed in fp32 from (enc, dec, saved log-probs, G)."""
+    """Per-element bounds of the eight joint gradients computed in fp32 from (enc, dec, saved log-probs, G) by
+    gam_rnnt_joint_backward, each a sum evaluated at depth k within k u sum|terms| (test_kernel_units.py's rule):
+      dl = G - exp(logp) sum(G): the warp-strided row sum (depth <= V1), expf (2 ulp = 4 u), the product and the difference;
+      dhid = dl W_o: depth V1 (dhid_bounds, with the ReLU flips);
+      dE = sum over U label positions, dP = sum over T frames: segment_sum_kernel, depth U and T;
+      dW_out / db_out: outer_sum_joint over B T U rows, whose rebuilt hidden entries carry hidden_rows' error;
+      the rest: joint_input_bounds."""
     B, T, U, V1 = l64.shape
-    mag = joint_grads(e64, d64, sd, l64, G64, absm=True)
-    # fp32 errors: the hidden row (768 + 320 + 2 terms), the logits' log-sum-exp, the products and sums of each gradient
-    J = 320
-    c = {0: V1 + J + U + 1200, 1: V1 + J + T + 1200, 2: V1 + J + B * T * U + 1200, 3: V1 + J + B * T * U + 1200,
-         4: V1 + J + B * T * U + 1200, 5: V1 + J + B * T * U + 1200, 6: B * T * U + 1200, 7: B * T * U + 1200}
-    lse = 4 * U32 * (l64.abs().amax(-1, keepdim=True) + 1) * l64.exp() * G64.abs().sum(-1, keepdim=True)
-    lse_mag = joint_grads(e64, d64, sd, l64, lse, absm=True)
-    # a hidden entry whose fp32 pre-activation may sit on the other side of 0 than the float64 one flips its ReLU mask:
-    # its whole |dlogit . W_o| term may be present on one side only
-    We, Wp = sd["head.joint.enc.weight"], sd["head.joint.pred.weight"]
-    zE, zP = e64 @ We.t() + sd["head.joint.enc.bias"], d64 @ Wp.t() + sd["head.joint.pred.bias"]
-    mE = e64.abs() @ We.abs().t() + sd["head.joint.enc.bias"].abs()
-    mP = d64.abs() @ Wp.abs().t() + sd["head.joint.pred.bias"].abs()
-    zerr = 2 * U32 * (800 * mE[:, :, None, :] + 340 * mP[:, None, :, :]) + U32 * (zE[:, :, None, :] + zP[:, None, :, :]).abs()
-    amb = (zE[:, :, None, :] + zP[:, None, :, :]).abs() <= zerr
-    dl_abs = softmax_grad(G64, l64, True)
-    flip = (dl_abs @ sd["head.joint.joint_net.1.weight"].abs()) * amb
-    fE, fP = flip.sum(2), flip.sum(1)
-    # dW_o sums dlogit x hid over the lattice: the rebuilt fp32 hidden entries carry an absolute error up to zerr each
-    hid_err = dl_abs.reshape(-1, V1).t() @ zerr.reshape(-1, J)
-    flips = (fE @ We.abs(), fP @ Wp.abs(), fE.reshape(-1, J).t() @ e64.abs().reshape(-1, 768), fE.sum((0, 1)),
-             fP.reshape(-1, J).t() @ d64.abs().reshape(-1, 320), fP.sum((0, 1)), hid_err, 0.0)
-    print(f"joint: {int(amb.sum())} of {amb.numel()} hidden entries within fp32 rounding of 0")
-    return [2 * c[i] * U32 * mag[i] + lse_mag[i] + flips[i] for i in range(8)]
+    Wo = sd["head.joint.joint_net.1.weight"]
+    J = Wo.shape[1]
+    z, zerr = hidden_rows(e64, d64, sd)
+    dl = softmax_grad(G64, l64, True)
+    dl_err = (V1 + 6) * U32 * dl
+    dh, dh_err = dhid_bounds(dl, dl_err, z, zerr, Wo)
+    dE, dE_err = dh.sum(2), dh_err.sum(2) + U * U32 * dh.sum(2)
+    dP, dP_err = dh.sum(1), dh_err.sum(1) + T * U32 * dh.sum(1)
+    hid = z.clamp_min(0).reshape(-1, J)
+    kO = outer_depth(B * T * U, V1, J)
+    dl2, dle2 = dl.reshape(-1, V1), dl_err.reshape(-1, V1)
+    dWo = dle2.t() @ hid + dl2.t() @ zerr.reshape(-1, J) + kO * U32 * (dl2.t() @ hid)
+    dbo = dle2.sum(0) + kO * U32 * dl2.sum(0)
+    ins = joint_input_bounds(e64, d64, sd, dE, dE_err, dP, dP_err)
+    return ins + [dWo, dbo]
 
 
 @pytest.mark.gpu
@@ -445,16 +499,25 @@ def test_joint_backward_past_2_31_lattice_elements():
     want, mag = joint_grads(*args)[1], joint_grads(*args, absm=True)[1]
     nz = dec.grad.abs().sum(-1) > 0
     assert bool(nz[-1, -1]) and int(nz.sum()) == 1
-    _check("d_dec past 2^31", dec.grad[-1:, -1:], want, mag, c=2 * (V1 + 320 + 1200), extra=4 * U32 * mag.abs().amax())
+    # depths: dl (V1 + 6, as _joint_bounds), dhid (V1), dP over the T frames, d_dec = dP W_p (J)
+    J = model.head.joint_cfg["joint_hidden"]
+    _check("d_dec past 2^31", dec.grad[-1:, -1:], want, mag, c=2 * V1 + 6 + T + J, extra=4 * U32 * mag.abs().amax())
+
+
+PREDICT_CASES = [(1, False, False, 320), (1, True, True, 320), (7, True, True, 320), (100, False, True, 320), (100, True, True, 320),
+                 (9, True, True, 16), (9, True, True, 72), (9, True, True, 614)]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("U,with_state,with_x", [(1, False, False), (1, True, True), (7, True, True), (100, False, True), (100, True, True)])
-def test_predict_backward_against_float64(U, with_state, with_x):
+@pytest.mark.parametrize("U,with_state,with_x,H", PREDICT_CASES,
+                         ids=["-".join(map(str, c[:3])) + (f"-H{c[3]}" if c[3] != 320 else "") for c in PREDICT_CASES])
+def test_predict_backward_against_float64(U, with_state, with_x, H):
+    """H = 72 is one 64-unit block with an 8-unit tail; H = 614 is the widest the backward runs
+    (GAM_PREDICT_BACKWARD_MAX_HIDDEN: 49 120 of the 49 152 bytes of shared memory)."""
     dev = _dev()
-    model, ck = _model("v2_rnnt")
+    model, ck = _model("v2_rnnt", H=None if H == 320 else H)
     model.head.requires_grad_(True)
-    B, V1, H = 13, 34, 320
+    B, V1 = 13, 34
     g = torch.Generator(device=dev).manual_seed(U + 2 * with_state)
     x = torch.randint(0, V1, (B, U), generator=g, device=dev) if with_x else None
     if with_x:
@@ -480,7 +543,7 @@ def test_predict_backward_against_float64(U, with_state, with_x):
     for i, (a, w, bd) in enumerate(zip(got, want, bounds)):
         if a is not None:
             worst = max(worst, _check_bound(f"predict grad {i}", a, w, bd))
-    print(f"predict U={U} state={with_state} x={with_x}: worst err/bound {worst:.3g}")
+    print(f"predict H={H} U={U} state={with_state} x={with_x}: worst err/bound {worst:.3g}")
 
 
 @pytest.mark.gpu
