@@ -15,6 +15,11 @@
 //           the spaces kept at a splice's left edge form the group before frame s (select moves them there), those at its
 //           right edge that do not follow the keyword's last token form the group after that token's frame (trace moves
 //           them there), so a kept space never falls inside a spliced keyword.
+// Resumable (gam_ctc_bias_resume): the rows, greedy tokens and detections cover stream frames [frame_base, frame_base + hi), held
+// by the caller.  Select first finds the horizon h (the earliest start of a spot path that can still become a detection, from
+// the spot records), the first undecided overlap component D (one whose last end is past h or past the last greedy token)
+// and the release frame R = min(h, D); only candidates starting before D take part, compact writes frames < R, and the
+// candidates from D on are carried out.  A one-shot call (gam_ctc_bias) is a finished resume from frame 0.
 // Fixed orders everywhere and no atomics: the outputs are a function of the recording's inputs alone.
 #include <cmath>
 #include <cstdint>
@@ -43,7 +48,7 @@ struct BiasWs {
   float* mrow;           // [T] m[t] of traced frames
   uint32_t* occupied;    // [ceil(T / 32)] bitmap of accepted frames
   int* rank;             // [K] keyword order: longer first, then smaller ids, then index
-  int* scalars;          // [4] eligible count, accepted count
+  int* scalars;          // [4] eligible count, accepted count, release frame R, first undecided start D
   unsigned char* bp;     // [T, 32] backpointers, byte l of frame t = lane l's four states
 };
 
@@ -120,6 +125,18 @@ __device__ inline bool key_less(const int4& a, const int4& b) {
   return a.z < b.z;
 }
 
+// the block's minimum of one int per thread (blockDim.x == kBiasThreads).  Ends synchronised.
+__device__ int block_min(int x) {
+  __shared__ int warp_min[32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  x = __reduce_min_sync(kFull, x);
+  if (lane == 0) warp_min[warp] = x;
+  __syncthreads();
+  x = __reduce_min_sync(kFull, warp_min[lane]);
+  __syncthreads();
+  return x;
+}
+
 // keyword a before keyword b in the last tie-breaks: the longer one, then the lexicographically smaller ids, then the index
 __device__ bool keyword_before(const int* keywords, const int* keyword_len, int Umax, int a, int b) {
   const int ua = min(max(keyword_len[a], 0), Umax), ub = min(max(keyword_len[b], 0), Umax);
@@ -142,14 +159,18 @@ __device__ inline int lower_bound(const int* f, int n, int x) {
 
 __device__ inline unsigned flag_of(const unsigned char* flags, int V, int id) { return id >= 0 && id < V ? flags[id] : 0u; }
 
-// the replaced range [i0, i1) of span [s, e) with its edge spaces removed; false when it is empty or not on word boundaries
-__device__ bool replaced_range(const int* ids, const int* fr, int n, const unsigned char* flags, int V, int s, int e, int* i0p, int* i1p) {
+// the replaced range [i0, i1) of span [s, e) with its edge spaces removed; false when it is empty or not on word boundaries.
+// left / right: whether the first / past-the-last token position is a word boundary (the start and end of a whole recording
+// are; a held range starts on one when the stream does or the last greedy token before it is a space, and ends on one only
+// when the stream finishes)
+__device__ bool replaced_range(const int* ids, const int* fr, int n, const unsigned char* flags, int V, int s, int e, bool left,
+                               bool right, int* i0p, int* i1p) {
   int i0 = lower_bound(fr, n, s), i1 = lower_bound(fr, n, e);
   while (i0 < i1 && (flag_of(flags, V, ids[i0]) & 1u)) ++i0;
   while (i1 > i0 && (flag_of(flags, V, ids[i1 - 1]) & 1u)) --i1;
   if (i1 <= i0) return false;
   auto boundary = [&](int p) {
-    return p == 0 || p == n || (flag_of(flags, V, ids[p - 1]) & 1u) || (flag_of(flags, V, ids[p]) & 3u);
+    return (p == 0 ? left : (flag_of(flags, V, ids[p - 1]) & 1u) != 0) || (p == n ? right : (flag_of(flags, V, ids[p]) & 3u) != 0);
   };
   *i0p = i0;
   *i1p = i1;
@@ -164,9 +185,13 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_select_kernel(BiasArgs 
   const int n = min(max(a.counts[b], 0), a.max_out);
   const int* ids = a.ids + static_cast<int64_t>(b) * a.max_out;
   const int* fr = a.frames + static_cast<int64_t>(b) * a.max_out;
+  // stream frame base + t is local frame t; a one-shot call is a finished stream from frame 0
+  const bool resume = a.frame_base != nullptr;
+  const int base = resume ? a.frame_base[b] : 0;
+  const bool fin = !resume || a.finish[b] != 0, left = !resume || a.left_boundary[b] != 0;
 
   for (int t = tid; t < T; t += kBiasThreads) {
-    w.kg[t] = w.ka[t] = w.kgsrc[t] = w.ins_id[t] = w.ins_k[t] = w.acc_at[t] = -1;
+    w.kg[t] = w.ka[t] = w.kgsrc[t] = w.ins_id[t] = w.ins_k[t] = w.acc_at[t] = w.acc_list[t] = -1;
     w.kg_n[t] = 1;
     w.ka_n[t] = 0;
   }
@@ -178,7 +203,61 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_select_kernel(BiasArgs 
   }
   __syncthreads();
   for (int i = tid; i < n; i += kBiasThreads)
-    if (fr[i] >= 0 && fr[i] < T) w.kg[fr[i]] = i;
+    if (fr[i] - base >= 0 && fr[i] - base < T) w.kg[fr[i] - base] = i;
+
+  // ---- what is decided (local frames).  Finished: everything, R = T_b.  Otherwise the horizon h: spot costs are <= 0, so a
+  // path that will end as a candidate (E >= tau) has v >= tau now, and every detection not yet emitted starts at or after
+  // the start of the pending one or of a state with v >= tau (NaN fails), or at a later frame.  A component of the known
+  // candidates' overlap graph is decided when it ends at or before h and at or before the last greedy token's frame (its
+  // members' right boundaries are known); the decided ones form a prefix in time, and D is the start of the first other one.
+  int D = Tb, R = Tb;
+  if (!fin) {
+    const int L4 = (2 * a.Umax - 1 + 3) / 4, per = 2 * a.Umax - 1;
+    int hmin = Tb;
+    for (int64_t i = tid; i < static_cast<int64_t>(K) * per; i += kBiasThreads) {
+      const int k = static_cast<int>(i / per), st = static_cast<int>(i % per), U = a.keyword_len[k];
+      if (U < 1 || U > a.Umax || st >= 2 * U - 1) continue;
+      const SpotRecord* rec = reinterpret_cast<const SpotRecord*>(a.state + (static_cast<int64_t>(b) * K + k) * a.record);
+      const float* v = reinterpret_cast<const float*>(rec + 1);
+      const int* from = reinterpret_cast<const int*>(v + 4 * L4);
+      const int at = (st & 3) * L4 + (st >> 2);
+      if (v[at] >= static_cast<float>(U) * a.log_theta) hmin = min(hmin, from[at] - base);
+      if (st == 0 && rec->has) hmin = min(hmin, rec->p_start - base);
+    }
+    const int h = max(block_min(hmin), 0);
+    if (tid == 0) {
+      // acc_list[t] holds, until the walk, the latest end of the known candidates starting at local frame t
+      for (int k = 0; k < K; ++k)
+        for (int j = 0; j < min(a.det_count[static_cast<int64_t>(b) * K + k], max_det); ++j) {
+          const int64_t row = (static_cast<int64_t>(b) * K + k) * max_det + j;
+          const int s = a.det_start[row] - base, e = a.det_end[row] - base;
+          if (s >= 0 && s < e && e <= Tb) w.acc_list[s] = max(w.acc_list[s], e);
+        }
+      const int last = min(h, n > 0 ? fr[n - 1] - base : -1);
+      int c0 = 0, c1 = -1;   // the current component [c0, c1)
+      for (int t = 0; t < Tb && D == Tb; ++t) {
+        const int e = w.acc_list[t];
+        if (e < 0) continue;
+        if (t >= c1) {
+          if (c1 > last) D = c0;
+          c0 = t;
+          c1 = e;
+        } else {
+          c1 = max(c1, e);
+        }
+      }
+      if (D == Tb && c1 > last) D = c0;
+      w.scalars[2] = min(h, D);
+      w.scalars[3] = D;
+    }
+    __syncthreads();
+    R = w.scalars[2];
+    D = w.scalars[3];
+    for (int t = tid; t < T; t += kBiasThreads) w.acc_list[t] = -1;
+    __syncthreads();
+  } else if (tid == 0) {
+    w.scalars[2] = R;
+  }
 
   // ---- eligible candidates, compacted in candidate order.  Spot's detections of one keyword are disjoint, so at most
   // min(max_det, T) of them are eligible and the key region holds them all; keys past it (detections that break that
@@ -186,8 +265,8 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_select_kernel(BiasArgs 
   const int64_t N = static_cast<int64_t>(K) * max_det;
   const int cap = static_cast<int>(next_pow2(bias_candidates(T, K, max_det)));
   int n_elig = 0;
-  for (int64_t base = 0; base < N; base += kBiasThreads) {
-    const int64_t c = base + tid;
+  for (int64_t c0 = 0; c0 < N; c0 += kBiasThreads) {
+    const int64_t c = c0 + tid;
     int4 key = make_int4(0, 0, 0, 0);
     int ok = 0;
     if (c < N) {
@@ -195,10 +274,11 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_select_kernel(BiasArgs 
       const int64_t row = (static_cast<int64_t>(b) * K + k) * max_det + j;
       const int U = a.keyword_len[k];
       if (j < min(a.det_count[static_cast<int64_t>(b) * K + k], max_det) && U >= 1 && U <= a.Umax) {
-        const int s = a.det_start[row], e = a.det_end[row];
+        const int s = a.det_start[row] - base, e = a.det_end[row] - base;
         const float G = a.det_score[row] - static_cast<float>(U) * a.log_theta;
         int i0, i1;
-        if (G >= 0.f && s >= 0 && s < e && e <= Tb && replaced_range(ids, fr, n, a.flags, V, s, e, &i0, &i1)) {
+        if (G >= 0.f && s >= 0 && s < e && e <= Tb && s < D &&
+            replaced_range(ids, fr, n, a.flags, V, s + base, e + base, left, fin, &i0, &i1)) {
           ok = 1;
           key = make_int4(static_cast<int>(~__float_as_uint(G + 0.f)), s, w.rank[k], static_cast<int>(c));
         }
@@ -233,7 +313,7 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_select_kernel(BiasArgs 
     for (int i = 0; i < n_elig; ++i) {
       const int c = w.keys[i].w;
       const int64_t row = (static_cast<int64_t>(b) * K + c / max_det) * max_det + c % max_det;
-      const int s = a.det_start[row], e = a.det_end[row];
+      const int s = a.det_start[row] - base, e = a.det_end[row] - base;
       bool free_span = true;
       for (int t = s; t < e && free_span;) {
         const int bits = min(32 - (t & 31), e - t);
@@ -253,8 +333,8 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_select_kernel(BiasArgs 
   __syncthreads();
   // ---- accepted spans in start order; identities keep the greedy tokens, the others strike them
   int n_acc = 0;
-  for (int base = 0; base < T; base += kBiasThreads) {
-    const int t = base + tid;
+  for (int t0 = 0; t0 < T; t0 += kBiasThreads) {
+    const int t = t0 + tid;
     const int c = t < T ? w.acc_at[t] : -1;
     int total;
     const int pos = block_scan(c >= 0, &total);
@@ -262,18 +342,21 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_select_kernel(BiasArgs 
       const int k = c / max_det;
       const int64_t row = (static_cast<int64_t>(b) * K + k) * max_det + c % max_det;
       int i0 = 0, i1 = 0;
-      replaced_range(ids, fr, n, a.flags, V, a.det_start[row], a.det_end[row], &i0, &i1);
+      replaced_range(ids, fr, n, a.flags, V, a.det_start[row], a.det_end[row], left, fin, &i0, &i1);
       const int U = a.keyword_len[k];
       const int* y = a.keywords + static_cast<int64_t>(k) * a.Umax;
       bool same = i1 - i0 == U;
       for (int i = 0; same && i < U; ++i) same = ids[i0 + i] == y[i];
       for (int i = i0; i < i1; ++i) {
-        if (same) w.kgsrc[fr[i]] = k;
-        else w.kg[fr[i]] = -1;
+        const int f = fr[i] - base;
+        if (f < 0 || f >= T) continue;   // a token outside the rows breaks the input contract: never written out of bounds
+        if (same) w.kgsrc[f] = k;
+        else w.kg[f] = -1;
       }
       if (!same) {   // the spaces kept at the left edge are written before the keyword, at its first frame s
-        const int s = a.det_start[row], r0 = lower_bound(fr, n, s);
-        for (int i = r0; i < i0; ++i) w.kg[fr[i]] = -1;
+        const int s = a.det_start[row] - base, r0 = lower_bound(fr, n, s + base);
+        for (int i = r0; i < i0; ++i)
+          if (fr[i] - base >= 0 && fr[i] - base < T) w.kg[fr[i] - base] = -1;
         if (i0 > r0) {
           w.kg[s] = r0;
           w.kg_n[s] = i0 - r0;
@@ -295,6 +378,24 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_select_kernel(BiasArgs 
       }
       a.out_path_logp[b] = static_cast<float>(sum);
     }
+    if (resume) a.released_until[b] = base + R;
+  }
+  // ---- resume: the undecided candidates (those from D on), compacted in their order, for the next call
+  if (resume) {
+    for (int k = tid; k < K; k += kBiasThreads) {
+      const int64_t row0 = (static_cast<int64_t>(b) * K + k) * max_det;
+      int c = 0;
+      for (int j = 0; j < min(a.det_count[static_cast<int64_t>(b) * K + k], max_det); ++j) {
+        const int s = a.det_start[row0 + j] - base, e = a.det_end[row0 + j] - base;
+        if (s >= D && s < e && e <= Tb) {
+          a.carry_start[row0 + c] = a.det_start[row0 + j];
+          a.carry_end[row0 + c] = a.det_end[row0 + j];
+          a.carry_score[row0 + c] = a.det_score[row0 + j];
+          ++c;
+        }
+      }
+      a.carry_count[static_cast<int64_t>(b) * K + k] = c;
+    }
   }
 }
 
@@ -303,13 +404,14 @@ __global__ void __launch_bounds__(32 * kTraceWarps) ctc_bias_trace_kernel(BiasAr
   const int T = a.T, K = a.K, max_det = a.max_det, V1 = a.V1, blank = V1 - 1;
   BiasWs w = bias_ws(workspace + b * ws_words, T, K, max_det);
   const int n_acc = w.scalars[1];
+  const int base = a.frame_base ? a.frame_base[b] : 0;
   const float* lp = a.log_probs + static_cast<int64_t>(b) * T * V1;
   for (int idx = blockIdx.x * kTraceWarps + (threadIdx.x >> 5); idx < n_acc; idx += gridDim.x * kTraceWarps) {
     const int c = w.acc_list[idx];
     if (c < 0) continue;   // an identity: nothing to trace
     const int k = c / max_det;
     const int64_t row = (static_cast<int64_t>(b) * K + k) * max_det + c % max_det;
-    const int s0 = a.det_start[row], e0 = a.det_end[row];
+    const int s0 = a.det_start[row] - base, e0 = a.det_end[row] - base;
     const int U = a.keyword_len[k], S = 2 * U - 1;
     const int* y = a.keywords + static_cast<int64_t>(k) * a.Umax;
     int lab[4];
@@ -387,9 +489,10 @@ __global__ void __launch_bounds__(32 * kTraceWarps) ctc_bias_trace_kernel(BiasAr
       const int* ids = a.ids + static_cast<int64_t>(b) * a.max_out;
       const int* fr = a.frames + static_cast<int64_t>(b) * a.max_out;
       int i0 = 0, i1 = 0;
-      replaced_range(ids, fr, n, a.flags, V1 - 1, s0, e0, &i0, &i1);
+      replaced_range(ids, fr, n, a.flags, V1 - 1, s0 + base, e0 + base, true, true, &i0, &i1);
       int j = i1;
-      for (; j < n && fr[j] < e0 && fr[j] <= last; ++j) w.kg[fr[j]] = -1;
+      for (; j < n && fr[j] - base < e0 && fr[j] - base <= last; ++j)
+        if (fr[j] - base >= 0) w.kg[fr[j] - base] = -1;
       if (j > i1) {
         w.ka[last] = i1;
         w.ka_n[last] = j - i1;
@@ -406,19 +509,22 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_compact_kernel(BiasArgs
   const int64_t o = static_cast<int64_t>(b) * a.max_out;
   const float* lp = a.log_probs + static_cast<int64_t>(b) * T * V1;
   const int* fr = a.frames + o;
+  const int base = a.frame_base ? a.frame_base[b] : 0;
+  const int T_out = a.frame_base ? w.scalars[2] : T;   // a resume call writes the frames before its release frame
   int count = 0;
   // greedy tokens [g, g + gn) written at frame t, from position pos on
   auto put_greedy = [&](int g, int gn, int t, int pos) {
     for (int i = 0; i < gn && pos + i < a.max_out; ++i) {
       a.out_ids[o + pos + i] = a.ids[o + g + i];
-      a.out_frames[o + pos + i] = t;
-      a.out_source[o + pos + i] = w.kgsrc[fr[g + i]];
+      a.out_frames[o + pos + i] = base + t;
+      const int f = fr[g + i] - base;
+      a.out_source[o + pos + i] = f >= 0 && f < T ? w.kgsrc[f] : -1;
       if (a.out_token_logp) a.out_token_logp[o + pos + i] = a.token_logp[o + g + i];
     }
   };
-  for (int base = 0; base < T; base += kBiasThreads) {
-    const int t = base + tid;
-    const int g = t < T ? w.kg[t] : -1, x = t < T ? w.ins_id[t] : -1, ga = t < T ? w.ka[t] : -1;
+  for (int t0 = 0; t0 < T_out; t0 += kBiasThreads) {
+    const int t = t0 + tid;
+    const int g = t < T_out ? w.kg[t] : -1, x = t < T_out ? w.ins_id[t] : -1, ga = t < T_out ? w.ka[t] : -1;
     const int gn = g >= 0 ? w.kg_n[t] : 0, an = ga >= 0 ? w.ka_n[t] : 0;
     int total;
     int pos = count + block_scan(gn + (x >= 0) + an, &total);
@@ -426,7 +532,7 @@ __global__ void __launch_bounds__(kBiasThreads) ctc_bias_compact_kernel(BiasArgs
     pos += gn;
     if (x >= 0 && pos < a.max_out) {
       a.out_ids[o + pos] = x;
-      a.out_frames[o + pos] = t;
+      a.out_frames[o + pos] = base + t;
       a.out_source[o + pos] = w.ins_k[t];
       if (a.out_token_logp) a.out_token_logp[o + pos] = lp[static_cast<int64_t>(t) * V1 + x];
     }

@@ -1345,6 +1345,39 @@ int64_t gam_ctc_bias_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, 
   return align_up(static_cast<int64_t>(B) * words * 4, 1024);
 }
 
+// the checks and launches gam_ctc_bias and gam_ctc_bias_resume share; `a` holds every pointer and size but V1 and log_theta
+static int ctc_bias_run(gam_handle* h, const char* what, BiasArgs& a, float threshold, int32_t V, void* workspace,
+                        int64_t workspace_bytes, void* stream) {
+  const gam_config& c = h->cfg;
+  if (spot_args(h, what, a.B, a.T, a.K, a.Umax, threshold, a.max_det) != 0) return -1;
+  if (a.max_out < a.T) return fail(h, -1, "%s: max_out=%d is less than T=%d", what, a.max_out, a.T);
+  if (!a.flags || V != c.num_classes - 1)
+    return fail(h, -1, "%s: the token flag table is missing or has %d entries, not %d", what, V, c.num_classes - 1);
+  if (!a.log_probs || !a.enc_len || !a.keywords || !a.keyword_len || !a.det_start || !a.det_end || !a.det_score || !a.det_count ||
+      !a.ids || !a.frames || !a.counts || !a.out_ids || !a.out_frames || !a.out_counts || !a.out_source)
+    return fail(h, -1, "%s: a required pointer is NULL", what);
+  if (!a.token_logp != !a.out_token_logp || !a.path_logp != !a.out_path_logp)
+    return fail(h, -1, "%s: token_logp / path_logp and their outputs go together", what);
+  if (a.frame_logp && a.frame_pitch < a.T)
+    return fail(h, -1, "%s: frame_pitch=%lld is less than T=%d", what, (long long)a.frame_pitch, a.T);
+  int rows = 0, smem = 0;
+  if (ctc_spot_plan(c.num_classes, &rows, &smem) == 1)
+    return fail(h, -1, "%s: a frame of %d classes does not fit in shared memory", what, c.num_classes);
+  const int64_t need = gam_ctc_bias_workspace_bytes(h, a.B, a.T, a.K, a.max_det);
+  if (need < 0) return fail(h, -1, "%s: K=%d x max_det=%d candidates are too many", what, a.K, a.max_det);
+  int32_t* ws = reinterpret_cast<int32_t*>(workspace_base(h, what, workspace, workspace_bytes, need, false));
+  if (!ws) return -1;
+  a.V1 = c.num_classes;
+  a.log_theta = static_cast<float>(std::log(static_cast<double>(threshold)));   // spot's rounding
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  for (int stage = 0; stage < 3; ++stage) {
+    PROF(PC_ALIGN);
+    launch_ctc_bias(a, ws, stage, s);
+  }
+  GAM_CHECK_LAUNCH(h, what);
+  return 0;
+}
+
 int gam_ctc_bias(gam_handle* h, const float* log_probs, const int32_t* enc_len, int32_t B, int32_t T, const int32_t* keywords,
                  const int32_t* keyword_len, int32_t K, int32_t Umax, const int32_t* det_start, const int32_t* det_end,
                  const float* det_score, const int32_t* det_count, int32_t max_det, float threshold, const uint8_t* token_flags,
@@ -1352,62 +1385,36 @@ int gam_ctc_bias(gam_handle* h, const float* log_probs, const int32_t* enc_len, 
                  const float* path_logp, double* frame_logp, int64_t frame_pitch, void* workspace, int64_t workspace_bytes,
                  int32_t* out_ids, int32_t* out_frames, int32_t* out_counts, int32_t* out_source, float* out_token_logp,
                  float* out_path_logp, void* stream) {
-  const gam_config& c = h->cfg;
-  if (spot_args(h, "ctc_bias", B, T, K, Umax, threshold, max_det) != 0) return -1;
-  if (max_out < T) return fail(h, -1, "ctc_bias: max_out=%d is less than T=%d", max_out, T);
-  if (!token_flags || V != c.num_classes - 1)
-    return fail(h, -1, "ctc_bias: the token flag table is missing or has %d entries, not %d", V, c.num_classes - 1);
-  if (!log_probs || !enc_len || !keywords || !keyword_len || !det_start || !det_end || !det_score || !det_count || !ids || !frames ||
-      !counts || !out_ids || !out_frames || !out_counts || !out_source)
-    return fail(h, -1, "ctc_bias: a required pointer is NULL");
-  if (!token_logp != !out_token_logp || !path_logp != !out_path_logp)
-    return fail(h, -1, "ctc_bias: token_logp / path_logp and their outputs go together");
-  if (frame_logp && frame_pitch < T) return fail(h, -1, "ctc_bias: frame_pitch=%lld is less than T=%d", (long long)frame_pitch, T);
-  int rows = 0, smem = 0;
-  if (ctc_spot_plan(c.num_classes, &rows, &smem) == 1)
-    return fail(h, -1, "ctc_bias: a frame of %d classes does not fit in shared memory", c.num_classes);
-  const int64_t need = gam_ctc_bias_workspace_bytes(h, B, T, K, max_det);
-  if (need < 0) return fail(h, -1, "ctc_bias: K=%d x max_det=%d candidates are too many", K, max_det);
-  int32_t* ws = reinterpret_cast<int32_t*>(workspace_base(h, "ctc_bias", workspace, workspace_bytes, need, false));
-  if (!ws) return -1;
-  BiasArgs a{};
-  a.log_probs = log_probs;
-  a.enc_len = enc_len;
-  a.keywords = keywords;
-  a.keyword_len = keyword_len;
-  a.det_start = det_start;
-  a.det_end = det_end;
-  a.det_score = det_score;
-  a.det_count = det_count;
-  a.flags = token_flags;
-  a.ids = ids;
-  a.frames = frames;
-  a.counts = counts;
-  a.token_logp = token_logp;
-  a.path_logp = path_logp;
-  a.frame_logp = frame_logp;
-  a.frame_pitch = frame_pitch;
-  a.B = B;
-  a.T = T;
-  a.V1 = c.num_classes;
-  a.K = K;
-  a.Umax = Umax;
-  a.max_det = max_det;
-  a.max_out = max_out;
-  a.log_theta = static_cast<float>(std::log(static_cast<double>(threshold)));   // spot's rounding
-  a.out_ids = out_ids;
-  a.out_frames = out_frames;
-  a.out_counts = out_counts;
-  a.out_source = out_source;
-  a.out_token_logp = out_token_logp;
-  a.out_path_logp = out_path_logp;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  for (int stage = 0; stage < 3; ++stage) {
-    PROF(PC_ALIGN);
-    launch_ctc_bias(a, ws, stage, s);
-  }
-  GAM_CHECK_LAUNCH(h, "ctc_bias");
-  return 0;
+  BiasArgs a{log_probs, enc_len, keywords, keyword_len, det_start, det_end, det_score, det_count, token_flags, ids, frames, counts,
+             token_logp, path_logp, frame_logp, frame_pitch, B, T, 0, K, Umax, max_det, max_out, 0.f, out_ids, out_frames, out_counts,
+             out_source, out_token_logp, out_path_logp};
+  return ctc_bias_run(h, "ctc_bias", a, threshold, V, workspace, workspace_bytes, stream);
+}
+
+int64_t gam_ctc_bias_resume_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t K, int32_t max_det) {
+  return gam_ctc_bias_workspace_bytes(h, B, T, K, max_det);
+}
+
+int gam_ctc_bias_resume(gam_handle* h, const float* log_probs, int32_t B, int32_t T, const int32_t* hi, const int32_t* frame_base,
+                        const int32_t* finish, const int32_t* keywords, const int32_t* keyword_len, int32_t K, int32_t Umax,
+                        const void* state, int64_t record_bytes, const int32_t* det_start, const int32_t* det_end,
+                        const float* det_score, const int32_t* det_count, int32_t max_det, float threshold,
+                        const uint8_t* token_flags, int32_t V, const int32_t* ids, const int32_t* frames, const int32_t* counts,
+                        const int32_t* left_boundary, int32_t max_out, const float* token_logp, double* frame_logp,
+                        int64_t frame_pitch, void* workspace, int64_t workspace_bytes, int32_t* out_ids, int32_t* out_frames,
+                        int32_t* out_counts, int32_t* out_source, float* out_token_logp, int32_t* released_until,
+                        int32_t* carry_start, int32_t* carry_end, float* carry_score, int32_t* carry_count, void* stream) {
+  if (!hi || !frame_base || !finish || !left_boundary || !state || !released_until || !carry_start || !carry_end || !carry_score ||
+      !carry_count)
+    return fail(h, -1, "ctc_bias_resume: hi, frame_base, finish, left_boundary, state, released_until and carry_* are required");
+  if (Umax >= 1 && Umax <= kSpotMaxTokens && record_bytes != ctc_spot_record_bytes(Umax))
+    return fail(h, -1, "ctc_bias_resume: record_bytes=%lld, but Umax=%d needs %lld", (long long)record_bytes, Umax,
+                (long long)ctc_spot_record_bytes(Umax));
+  BiasArgs a{log_probs, hi, keywords, keyword_len, det_start, det_end, det_score, det_count, token_flags, ids, frames, counts,
+             token_logp, nullptr, frame_logp, frame_pitch, B, T, 0, K, Umax, max_det, max_out, 0.f, out_ids, out_frames, out_counts,
+             out_source, out_token_logp, nullptr, frame_base, finish, left_boundary, static_cast<const uint8_t*>(state), record_bytes,
+             released_until, carry_start, carry_end, carry_score, carry_count};
+  return ctc_bias_run(h, "ctc_bias_resume", a, threshold, V, workspace, workspace_bytes, stream);
 }
 
 int64_t gam_rnnt_align_scores_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t U) {

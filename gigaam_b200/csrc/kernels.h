@@ -244,7 +244,7 @@ int launch_ctc_spot(const float* log_probs, const SpotResume& io, const int* key
                     int Umax, float log_theta, int max_det, int warps, int* det_start, int* det_end, float* det_score, int* det_count,
                     cudaStream_t s);
 
-// bias.cu: hotwords spliced into CTC greedy output (gam_ctc_bias), three launches in stage order 0, 1, 2: select (one CTA per
+// bias.cu: hotwords spliced into CTC greedy output (gam_ctc_bias, gam_ctc_bias_resume), three launches in stage order 0, 1, 2: select (one CTA per
 // recording), trace (kBiasTraceCtas x 4 warps per recording) and compact (one CTA per recording).  ctc_bias_workspace_words is the workspace of
 // one recording in 32-bit words (a multiple of 4), or -1 when it does not fit in int64.
 struct BiasArgs {
@@ -272,6 +272,17 @@ struct BiasArgs {
   int* out_source;
   float* out_token_logp;
   float* out_path_logp;
+  // gam_ctc_bias_resume; frame_base == NULL: a one-shot call (frames from 0, finished, starting on a word boundary)
+  const int* frame_base;
+  const int* finish;
+  const int* left_boundary;
+  const uint8_t* state;      // the spot records [B, K, record]
+  int64_t record;
+  int* released_until;
+  int* carry_start;
+  int* carry_end;
+  float* carry_score;
+  int* carry_count;
 };
 constexpr int kBiasTraceCtas = 32;
 int64_t ctc_bias_workspace_words(int T, int K, int max_det);

@@ -919,6 +919,44 @@ class Engine:
                    0 if frame_logp is None else frame_logp.shape[1], ws, ws.numel(), *out)
         return tuple(out)
 
+    def ctc_bias_resume(self, log_probs: Tensor, hi: Tensor, frame_base: Tensor, finish: Tensor, keywords: Tensor,
+                        keyword_len: Tensor, threshold: float, state: Tensor, det: Tuple[Tensor, ...], token_flags: Tensor,
+                        ids: Tensor, frames: Tensor, counts: Tensor, left_boundary: Tensor, token_logp: Optional[Tensor] = None,
+                        frame_logp: Optional[Tensor] = None) -> Tuple[Tensor, ...]:
+        """Resumable hotwords (gam_ctc_bias_resume) over held stream frames frame_base[b] + t, t < hi[b], of log_probs
+        [B, T, V+1]: `state` the spot records [B, K, bytes] after this step's ctc_spot_resume, det = (start, end, score
+        [B, K, max_det], count [B, K]) the undecided detections in stream frames, ids / frames [B, max_out] and counts [B] the
+        held greedy tokens (frames in stream frames).  hi / frame_base / finish / left_boundary: device int32 [B].  -> (ids,
+        frames [B, max_out] i32, counts [B] i32, source [B, max_out] i32, token_logp [B, max_out] f32 or None, released_until
+        [B] i32, carry_start, carry_end [B, K, max_det] i32, carry_score [B, K, max_det] f32, carry_count [B, K] i32);
+        frame_logp (f64 [B, pitch], the held frames' per-frame sums) is adjusted in place."""
+        assert log_probs.is_cuda and log_probs.dtype == torch.float32 and log_probs.is_contiguous() and log_probs.dim() == 3
+        if self.head_type != 1:
+            raise RuntimeError("model has no CTC head")
+        B, T, _ = log_probs.shape
+        K, Umax = keywords.shape
+        max_out = ids.shape[1]
+        max_det = det[0].shape[2]
+        ws = self._ws(self._ws_align, ("bias", B, T, K, max_det), "gam_ctc_bias_resume_workspace_bytes", B, T, K, max_det,
+                      what=f"ctc_bias_resume: bad sizes B={B}, T={T}, K={K}, max_det={max_det}")
+        hi, frame_base, finish, left_boundary, keywords, keyword_len, ids, frames, counts = (
+            self._i32(t, self.device) for t in (hi, frame_base, finish, left_boundary, keywords, keyword_len, ids, frames, counts))
+        flags = token_flags.to(device=self.device, dtype=torch.uint8).contiguous()
+        assert state.dtype == torch.uint8 and state.is_contiguous() and tuple(state.shape[:2]) == (B, K)
+        assert all(t.is_cuda and t.is_contiguous() and t.shape[:2] == (B, K) for t in det)
+        assert token_logp is None or (token_logp.is_cuda and token_logp.dtype == torch.float32 and token_logp.is_contiguous())
+        assert frame_logp is None or (frame_logp.dtype == torch.float64 and frame_logp.is_contiguous() and frame_logp.dim() == 2)
+        i32 = dict(dtype=torch.int32, device=self.device)
+        out = [torch.empty((B, max_out), **i32), torch.empty((B, max_out), **i32), torch.empty((B,), **i32),
+               torch.empty((B, max_out), **i32),
+               None if token_logp is None else torch.empty((B, max_out), dtype=torch.float32, device=self.device),
+               torch.empty((B,), **i32), torch.empty((B, K, max_det), **i32), torch.empty((B, K, max_det), **i32),
+               torch.empty((B, K, max_det), dtype=torch.float32, device=self.device), torch.empty((B, K), **i32)]
+        self._call("gam_ctc_bias_resume", log_probs, B, T, hi, frame_base, finish, keywords, keyword_len, K, Umax, state,
+                   state.shape[2], *det, max_det, float(threshold), flags, flags.numel(), ids, frames, counts, left_boundary,
+                   max_out, token_logp, frame_logp, 0 if frame_logp is None else frame_logp.shape[1], ws, ws.numel(), *out)
+        return tuple(out)
+
     def rnnt_align_scores(self, enc: Tensor, dec: Tensor, targets: Tensor) -> Tuple[Tensor, Tensor]:
         """enc [B, T, d], dec [B, U+1, pred_hidden] f32 contiguous, targets [B, U] -> (blank, label) [B, T, U+1] f32: the
         entries of rnnt_joint's lattice that alignment reads (gam_rnnt_align_scores)."""

@@ -631,16 +631,21 @@ class GigaAMASR(GigaAM):
     def streaming(self, window: float = 8.0, overlap: float = 4.0, batch_size: int = 64, confidence: bool = False,
                   keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5,
                   boost: Optional[Sequence[Union[str, Sequence[int]]]] = None, boost_weight: float = 1.0,
-                  sample_rate: int = SAMPLE_RATE):
+                  sample_rate: int = SAMPLE_RATE, hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None,
+                  hotword_threshold: float = 0.5):
         """A `streaming.StreamServer` for live audio (INTEGRATION.md §7i): open streams, push chunks, `step()` for captions
         and keyword alerts, `close()` for each stream's `transcribe_windowed` / `spot` result.  `boost` and `boost_weight` as
         in `transcribe` (RNN-T models only), for every stream of the server.  Raises before any device work: ValueError for
         the window plan's refusals, batch_size < 1, `spot`'s keyword and threshold checks and `boost`'s checks;
         NotImplementedError for keywords on an RNN-T model and for boost on a CTC model.  `sample_rate`: the rate of the pushed
-        samples, resampled to 16 kHz as they arrive (INTEGRATION.md §7k); ValueError for a rate gam_resample cannot take."""
+        samples, resampled to 16 kHz as they arrive (INTEGRATION.md §7k); ValueError for a rate gam_resample cannot take.
+        `hotwords` and `hotword_threshold` as in `transcribe` (CTC models only, checked the same way before any device work):
+        captions commit text with the hotwords spliced in once no later detection can change it, and a closed stream equals
+        `transcribe_windowed(..., hotwords=hotwords, hotword_threshold=hotword_threshold)`."""
         from .streaming import StreamServer
         tables = None if boost is None else self._boost_tables(boost, boost_weight, "streaming")
-        return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold, boost=tables, sample_rate=sample_rate)
+        return StreamServer(self, window, overlap, batch_size, confidence, keywords, threshold, boost=tables, sample_rate=sample_rate,
+                            hotwords=hotwords, hotword_threshold=hotword_threshold)
 
     # ---- keyword spotting (INTEGRATION.md §7g)
     def _keyword_ids(self, keywords: Sequence[Union[str, Sequence[int]]], threshold: float) -> Tuple[List[str], List[List[int]]]:

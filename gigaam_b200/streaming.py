@@ -16,8 +16,15 @@ launch for all streams (the span form, include/gigaam_b200.h), every 16 kHz outp
 Every 16 kHz sample is thus the one-shot resampler's, and the windows see the samples `transcribe_windowed(recording,
 sample_rate=...)` sees.  The host keeps the raw samples that the outputs still pending can need.
 
-Device memory does not grow with a stream's duration: a stream owns one decoder record and one spot record per keyword, and
-every step's outputs are step-local.  The host keeps each stream's unencoded samples, its token ids, frames, token
+With hotwords (CTC models), each decode round also spots the hotwords in a spot pool of their own and runs one
+`Engine.ctc_bias_resume` launch over the round's streams: it releases the tokens whose hotword decisions are final (frames
+before the release frame R) and the stream holds the rest for the next round: the log-prob rows [R, C) and the undecided
+detections on the device, the greedy tokens and per-frame sums of that span on the host.  `close()` makes the last call with
+finish, so a closed stream equals `transcribe_windowed(..., hotwords=...)`.
+
+Device memory does not grow with a stream's duration: a stream owns one decoder record, one spot record per keyword and
+per hotword, and with hotwords the held rows [R, C), bounded by the oldest live hotword path; every step's outputs are
+step-local.  The host keeps each stream's unencoded samples, its token ids, frames, token
 log-probs, per-frame sums and detections for `close`.  One caller drives a server; it is not thread-safe."""
 from __future__ import annotations
 
@@ -107,6 +114,17 @@ class _Stream:
         self.raw = torch.zeros(0, dtype=torch.float32)
         self.raw_chunks: List[Tensor] = []
         self.raw_start = self.raw_n = self.out_n = 0
+        # hotwords: the span [hw_base, C) not yet released -- its rows and its undecided hotword detections on the device
+        # (hw_det: start, end and score bits as i32 [D, 3, K], and the count per hotword [K]), its greedy tokens and
+        # per-frame sums on the host; hw_left: the span starts on a word boundary
+        self.hw_rows: Optional[Tensor] = None
+        self.hw_det: Optional[Tuple[Tensor, Tensor]] = None
+        self.hw_base = 0
+        self.hw_left = True
+        self.hw_ids = np.zeros(0, np.int32)
+        self.hw_frames = np.zeros(0, np.int32)
+        self.hw_logp = np.zeros(0, np.float32)
+        self.hw_flp = np.zeros(0, np.float64)
 
     def samples(self, start: int, end: int) -> Tensor:
         if self.chunks:
@@ -138,11 +156,15 @@ class StreamServer:
     max_segment=max_segment)` (with the server's `boost` and `boost_weight`) and, with keywords, `spot(recording, keywords,
     threshold, window, overlap)`, bit for bit.  `boost`: the tables of a boost graph (GigaAMASR._boost_tables, moved to the
     device with the first stream) that steer every stream's decoding, committed and tentative.  `sample_rate`: the rate of the
-    pushed samples; a closed stream's result is then `transcribe_windowed(recording, sample_rate=sample_rate, ...)`'s."""
+    pushed samples; a closed stream's result is then `transcribe_windowed(recording, sample_rate=sample_rate, ...)`'s.
+    `hotwords` / `hotword_threshold` (CTC models only): checked as `transcribe` checks them; a closed stream's result is then
+    `transcribe_windowed(recording, hotwords=hotwords, hotword_threshold=hotword_threshold, ...)`'s, and updates commit text
+    with the hotwords spliced in once no later detection can change it (INTEGRATION.md §7i)."""
 
     def __init__(self, model, window: float = 8.0, overlap: float = 4.0, batch_size: int = 64, confidence: bool = False,
                  keywords: Optional[Sequence[Union[str, Sequence[int]]]] = None, threshold: float = 0.5,
-                 boost: Optional[Tuple[Tensor, Tensor]] = None, sample_rate: int = SAMPLE_RATE):
+                 boost: Optional[Tuple[Tensor, Tensor]] = None, sample_rate: int = SAMPLE_RATE,
+                 hotwords: Optional[Sequence[Union[str, Sequence[int]]]] = None, hotword_threshold: float = 0.5):
         self.sample_rate = sample_rate
         self._ratio = None if sample_rate == SAMPLE_RATE else resample_ratio(sample_rate)
         self.W = _frame_multiple(window, "window")
@@ -156,6 +178,8 @@ class StreamServer:
             model._needs_head(False, "keywords in streams need a CTC head: an RNN-T model has no per-frame posteriors without "
                                      "its [T, U + 1] lattice; use a *_ctc model")
             self.names, self.kw_ids = model._keyword_ids(keywords, threshold)
+        self.hw_ids: List[List[int]] = [] if hotwords is None else model._hotword_ids(hotwords, hotword_threshold, "streaming")
+        self.hotword_threshold = hotword_threshold
         self.model, self.window, self.overlap = model, window, overlap
         self.batch_size, self.confidence, self.threshold = int(batch_size), bool(confidence), threshold
         self.boost = boost
@@ -166,6 +190,7 @@ class StreamServer:
         self._eng = None
         self._dec_pool: Optional[Tensor] = None    # uint8 [slots, decode record]
         self._spot_pool: Optional[Tensor] = None   # uint8 [slots, K, spot record]
+        self._hw_pool: Optional[Tensor] = None     # uint8 [slots, hotwords, spot record]
 
     # ---- streams
     def open(self) -> int:
@@ -176,10 +201,16 @@ class StreamServer:
         self._dec_pool[slot] = self._fresh_dec[0]
         if self.kw_ids:
             self._spot_pool[slot] = self._fresh_spot[0]
+        if self.hw_ids:
+            self._hw_pool[slot] = self._fresh_hw[0]
         sid = self._next_id
         self._next_id += 1
         self._streams[sid] = _Stream(sid, slot, TextFeed(self.model.decoding.tokenizer, self._openers), len(self.kw_ids),
                                      self.model._dtype)
+        if self.hw_ids:
+            K = len(self.hw_ids)
+            self._streams[sid].hw_det = (torch.zeros((0, 3, K), dtype=torch.int32, device=self._eng.device),
+                                         torch.zeros(K, dtype=torch.int32, device=self._eng.device))
         return sid
 
     def _grow(self) -> None:
@@ -192,6 +223,12 @@ class StreamServer:
                 self._kw, self._kw_len = self.model._keyword_tensors(self.kw_ids, eng.device)
                 self._fresh_spot = eng.spot_state(1, len(self.kw_ids), self._kw.shape[1])
                 self._min_u = min(len(r) for r in self.kw_ids)
+            if self.hw_ids:
+                self._hw_kw, self._hw_kw_len = self.model._keyword_tensors(self.hw_ids, eng.device)
+                self._fresh_hw = eng.spot_state(1, len(self.hw_ids), self._hw_kw.shape[1])
+                self._hw_min_u = min(len(r) for r in self.hw_ids)
+                self._flags = self.model._word_flags()
+                self._flags_host = self._flags.cpu().tolist()
         old = 0 if self._dec_pool is None else self._dec_pool.shape[0]
         new = max(8, 2 * old)
         dec = self._fresh_dec.expand(new - old, -1)
@@ -199,6 +236,9 @@ class StreamServer:
         if self.kw_ids:
             spot = self._fresh_spot.expand(new - old, -1, -1)
             self._spot_pool = spot.clone() if self._spot_pool is None else torch.cat([self._spot_pool, spot])
+        if self.hw_ids:
+            hw = self._fresh_hw.expand(new - old, -1, -1)
+            self._hw_pool = hw.clone() if self._hw_pool is None else torch.cat([self._hw_pool, hw])
         self._free.extend(range(new - 1, old - 1, -1))
 
     def _get(self, stream: int, what: str) -> _Stream:
@@ -245,7 +285,7 @@ class StreamServer:
             pending = [self._detection(k, *p) for k, p in enumerate(s.pending) if p is not None]
             dets.sort(key=lambda d: (d.start, d.keyword_index))
             out.append(StreamUpdate(stream=s.id, new_tokens=new_ids, new_text=s.feed.push(s.ids, len(new_ids)),
-                                    tentative_text=self.model.decoding.tokenizer.decode(s.tentative),
+                                    tentative_text=self.model.decoding.tokenizer.decode(s.hw_ids.tolist() + s.tentative),
                                     committed_until=s.committed * FRAME_SECONDS, detections=dets, pending=pending))
         return out
 
@@ -293,7 +333,7 @@ class StreamServer:
         for group in window_groups(list(enumerate(jobs)), self.batch_size, lambda item: item[1][1]):
             encoded = encode_rows(self.model, [s.samples(w.start, w.end) for _, (s, w) in group])
             enc = _as_btd(encoded)
-            lp = self.model.head(encoded) if self.kw_ids else None
+            lp = self.model.head(encoded) if self.kw_ids or self.hw_ids else None
             rounds: List[List[int]] = []
             seen: Dict[_Stream, int] = {}
             for row, (_, (s, _)) in enumerate(group):
@@ -306,7 +346,8 @@ class StreamServer:
                 reads.append(self._decode_round([group[r][1] for r in rows], self._rows(enc, rows), lp_rows))
             if tentative:
                 rows = [row for row, (i, (s, _)) in enumerate(group) if last[s] == i]
-                reads.append(self._tentative([group[r][1] for r in rows], self._rows(enc, rows)))
+                if rows:   # a group may hold no stream's newest window
+                    reads.append(self._tentative([group[r][1] for r in rows], self._rows(enc, rows)))
             del encoded, enc, lp
         for read in reads:           # one synchronisation per call, in job order
             read()
@@ -328,39 +369,140 @@ class StreamServer:
         out = eng.decode_buffers(len(sel), eng.hyp_width(T_w), T_w, scores=self.confidence)
         eng.greedy_resume(enc, rng[0], rng[1], rng[2], state, out, self.confidence, self.boost)
         self._dec_pool.index_copy_(0, slots, state)
+        frames_max = max(h - l for l, h in zip(lo, hi))
         spot = None
-        if lp is not None:
-            spot = self._spot_round(slots, lp, rng[0], rng[1], rng[3], rng[4], max(h - l for l, h in zip(lo, hi)))
+        if self.kw_ids:
+            spot = self._spot_round(slots, lp, rng[0], rng[1], rng[3], rng[4], frames_max)
+        hot = None
+        if self.hw_ids:
+            hot = self._spot_round(slots, lp, rng[0], rng[1], rng[3], rng[4], frames_max, hotwords=True)
+            for k, (s, _) in enumerate(sel):   # the round's rows join the held span
+                rows = lp[k, lo[k]:hi[k]]
+                s.hw_rows = rows.clone() if s.hw_rows is None else torch.cat([s.hw_rows, rows])
 
         def read():
             host = [None if t is None else t.cpu() for t in out]
             ids, frames, counts = host[:3]
             for k, ((s, w), f) in enumerate(zip(sel, first)):
                 n = int(counts[k])
-                s.ids.extend(ids[k, :n].tolist())
-                s.frames.extend((frames[k, :n] + f).tolist())
+                if self.hw_ids:   # the round's greedy output joins the held span, released by _release below
+                    s.hw_ids = np.concatenate([s.hw_ids, ids[k, :n].numpy()])
+                    s.hw_frames = np.concatenate([s.hw_frames, (frames[k, :n] + f).numpy().astype(np.int32)])
+                    if self.confidence:
+                        s.hw_logp = np.concatenate([s.hw_logp, host[3][k, :n].numpy()])
+                        s.hw_flp = np.concatenate([s.hw_flp, host[6][k, lo[k]:hi[k]].numpy()])
+                else:
+                    s.ids.extend(ids[k, :n].tolist())
+                    s.frames.extend((frames[k, :n] + f).tolist())
+                    if self.confidence:
+                        s.token_logp.extend(host[3][k, :n].tolist())
+                        s.frame_logp.append(host[6][k, lo[k]:hi[k]].numpy())
                 if self.confidence:
-                    s.token_logp.extend(host[3][k, :n].tolist())
-                    s.frame_logp.append(host[6][k, lo[k]:hi[k]].numpy())
                     s.frame_rows.append(host[7][k, lo[k]:hi[k]].numpy())
                 s.committed = w.keep_end
             if spot is not None:
                 self._read_spot([s for s, _ in sel], spot)
+            if hot is not None:
+                self._release([s for s, _ in sel], [w.keep_end for _, w in sel], hot, finish=False)
         return read
 
-    def _spot_round(self, slots: Tensor, lp: Tensor, lo: Tensor, hi: Tensor, base: Tensor, finish: Tensor, frames: int):
-        """One ctc_spot_resume launch for the streams at `slots`; returns its device outputs."""
+    def _spot_round(self, slots: Tensor, lp: Tensor, lo: Tensor, hi: Tensor, base: Tensor, finish: Tensor, frames: int,
+                    hotwords: bool = False):
+        """One ctc_spot_resume launch for the streams at `slots`, over the keywords (returns the device outputs) or the
+        hotwords (returns the detections and the records after the launch)."""
         eng = self._eng
-        n, K = slots.numel(), len(self.kw_ids)
-        max_det = frames // self._min_u + 2   # a carried pending one, plus disjoint detections of >= U frames each
+        kw_ids = self.hw_ids if hotwords else self.kw_ids
+        n, K = slots.numel(), len(kw_ids)
+        max_det = frames // min(len(r) for r in kw_ids) + 2   # a carried pending one, plus disjoint detections of >= U frames
         i32 = dict(dtype=torch.int32, device=eng.device)
         det = (torch.empty((n, K, max_det), **i32), torch.empty((n, K, max_det), **i32),
                torch.empty((n, K, max_det), dtype=torch.float32, device=eng.device), torch.zeros((n, K), **i32))
+        if hotwords:
+            state = self._hw_pool.index_select(0, slots)
+            eng.ctc_spot_resume(lp, lo, hi, base, finish, self._hw_kw, self._hw_kw_len, self.hotword_threshold, state, det)
+            self._hw_pool.index_copy_(0, slots, state)
+            return det, state
         pend = (torch.empty((n, K), **i32), torch.empty((n, K), **i32), torch.empty((n, K), dtype=torch.float32, device=eng.device))
         state = self._spot_pool.index_select(0, slots)
         eng.ctc_spot_resume(lp, lo, hi, base, finish, self._kw, self._kw_len, self.threshold, state, det, pend)
         self._spot_pool.index_copy_(0, slots, state)
         return det + pend
+
+    def _held_detections(self, streams: List[_Stream], new: Tuple[Tensor, ...]) -> Tuple[Tensor, ...]:
+        """The undecided detections of `streams` (held on the device) followed by the round's new ones `new` = (start, end,
+        score [n, K, md], count [n, K]), on the device: the bias-resume input (start, end, score [n, K, D], count [n, K])."""
+        st, en, sc, cnt = new
+        held = [s.hw_det for s in streams]
+        Dc = max(p.shape[0] for p, _ in held)
+        if Dc == 0:
+            return new
+        n, K, md = st.shape
+        packed = torch.nn.utils.rnn.pad_sequence([p for p, _ in held], batch_first=True).permute(0, 2, 3, 1)   # [n, 3, K, Dc]
+        cc = torch.stack([c for _, c in held])[..., None]
+        j = torch.arange(Dc + md, device=st.device)[None, None, :]
+        old = j < cc
+        jc = j.clamp(max=Dc - 1).expand(n, K, -1)
+        jn = (j - cc).clamp(0, md - 1)
+
+        def merge(a, b):
+            return torch.where(old, a.gather(2, jc), b.gather(2, jn))
+        return (merge(packed[:, 0], st), merge(packed[:, 1], en),
+                merge(packed[:, 2].view(torch.float32), sc), cc[..., 0] + cnt)
+
+    def _release(self, streams: List[_Stream], ends: List[int], hot: Tuple[Tuple[Tensor, ...], Tensor], finish: bool) -> None:
+        """One ctc_bias_resume launch over the held spans [hw_base, ends[b]) of `streams`, padded to the longest: the round's
+        new hotword detections join the undecided ones on the device, the released tokens (and per-frame sums) are
+        committed, and the span is trimmed to the release frame.  One read-back per call."""
+        eng, dev = self._eng, self._eng.device
+        det, state = hot
+        det = self._held_detections(streams, det)
+        n = len(streams)
+        held = [e - s.hw_base for s, e in zip(streams, ends)]
+        T = max(1, max(held))
+        lp = torch.zeros((n, T, eng.num_classes), dtype=torch.float32, device=dev)
+        for b, (s, h) in enumerate(zip(streams, held)):
+            if h:
+                lp[b, :h] = s.hw_rows[:h]
+        max_out = max(T, max(s.hw_ids.size for s in streams))
+        ids = np.zeros((n, max_out), np.int32)
+        frames = np.zeros((n, max_out), np.int32)
+        token_logp = np.zeros((n, max_out), np.float32) if self.confidence else None
+        flp = np.zeros((n, T), np.float64) if self.confidence else None
+        for b, s in enumerate(streams):
+            m = s.hw_ids.size
+            ids[b, :m], frames[b, :m] = s.hw_ids, s.hw_frames
+            if self.confidence:
+                token_logp[b, :m] = s.hw_logp
+                flp[b, :s.hw_flp.size] = s.hw_flp
+        rng = torch.tensor([held, [s.hw_base for s in streams], [int(finish)] * n, [int(s.hw_left) for s in streams],
+                            [s.hw_ids.size for s in streams]], dtype=torch.int32).to(dev)
+        flp_dev = None if flp is None else torch.from_numpy(flp).to(dev)
+        out = eng.ctc_bias_resume(lp, rng[0], rng[1], rng[2], self._hw_kw, self._hw_kw_len, self.hotword_threshold, state, det,
+                                  self._flags, torch.from_numpy(ids).to(dev), torch.from_numpy(frames).to(dev), rng[4], rng[3],
+                                  None if token_logp is None else torch.from_numpy(token_logp).to(dev), flp_dev)
+        o_ids, o_frames, o_counts, _, o_logp, until, c_st, c_en, c_sc, c_cnt = out
+        carried = torch.stack([c_st, c_en, c_sc.view(torch.int32)], 1).permute(0, 3, 1, 2)   # [n, D, 3, K], stays on the device
+        o_ids, o_frames, o_counts, until, c_width = (t.cpu().numpy() for t in (o_ids, o_frames, o_counts, until, c_cnt.amax(1)))
+        o_logp = None if o_logp is None else o_logp.cpu().numpy()
+        flp = None if flp_dev is None else flp_dev.cpu().numpy()
+        for b, s in enumerate(streams):
+            m, R = int(o_counts[b]), int(until[b])
+            cut = R - s.hw_base
+            s.ids.extend(o_ids[b, :m].tolist())
+            s.frames.extend(o_frames[b, :m].tolist())
+            if self.confidence:
+                s.token_logp.extend(o_logp[b, :m].tolist())
+                s.frame_logp.append(flp[b, :cut].copy())
+                s.hw_flp = s.hw_flp[cut:]
+            g = int(np.searchsorted(s.hw_frames, R))   # the held greedy tokens before R are released
+            if g:
+                s.hw_left = bool(self._flags_host[int(s.hw_ids[g - 1])] & 1)
+            s.hw_ids, s.hw_frames, s.hw_logp = s.hw_ids[g:], s.hw_frames[g:], s.hw_logp[g:]
+            s.hw_det = (carried[b, :int(c_width[b])], c_cnt[b])
+            if s.hw_rows is not None:
+                s.hw_rows = s.hw_rows[cut:]
+            s.hw_base = R
+            s.committed = R
 
     @staticmethod
     def _read_spot(streams: List[_Stream], spot: Tuple[Tensor, ...]) -> None:
@@ -413,6 +555,12 @@ class StreamServer:
             lp = torch.zeros((1, 1, self._eng.num_classes), dtype=torch.float32, device=dev)
             self._read_spot([s], self._spot_round(one, lp, flags[0], flags[1], flags[2], flags[3], 0))
             detections = self.model._detections(self.names, self.kw_ids, s.dets, compute_frame_shift(N, T))
+        if self.hw_ids:   # the last hotword call: the pending detections are emitted and everything held is released
+            dev = self._eng.device
+            one = torch.tensor([s.slot], device=dev)
+            flags = torch.tensor([[0], [0], [0], [1]], dtype=torch.int32, device=dev)
+            lp = torch.zeros((1, 1, self._eng.num_classes), dtype=torch.float32, device=dev)
+            self._release([s], [T], self._spot_round(one, lp, flags[0], flags[1], flags[2], flags[3], 0, hotwords=True), finish=True)
         transcript = windowed_result(self.model, s.ids, s.frames, s.token_logp if self.confidence else None,
                                      np.concatenate(s.frame_logp) if self.confidence else None,
                                      np.concatenate(s.frame_rows) if self.confidence else None, N, T, word_timestamps, pause,

@@ -179,7 +179,11 @@ class StreamUpdate(_Record):
     token.  `tentative_text` decodes the frames after the committed ones in the newest encoded window; it is replaced at the
     next step.  `committed_until` is the end of the committed frames in seconds at the nominal 0.04 s per frame.
     `detections` are the keyword detections made final by the step, `pending` the provisional ones (at most one per keyword),
-    which a better overlapping candidate may still replace; their times use the nominal frame step too."""
+    which a better overlapping candidate may still replace; their times use the nominal frame step too.
+    With hotwords, `new_tokens` are the tokens released by the step, the hotwords already spliced in: every token at a frame
+    before the release frame R, where no later detection can change the output.  `committed_until` is R, which never
+    decreases and stops short of the decoded frames while a hotword path may still end there.  `tentative_text` decodes the
+    held greedy tokens (frames from R on, no splices) followed by the newest window's tentative tokens."""
     __slots__ = _fields = ("stream", "new_tokens", "new_text", "tentative_text", "committed_until", "detections", "pending")
     stream: int
     new_tokens: List[int]

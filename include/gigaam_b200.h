@@ -543,6 +543,57 @@ int gam_ctc_bias(gam_handle* h, const float* log_probs, const int32_t* enc_len, 
                  const float* path_logp, double* frame_logp, int64_t frame_pitch, void* workspace, int64_t workspace_bytes,
                  int32_t* out_ids, int32_t* out_frames, int32_t* out_counts, int32_t* out_source, float* out_token_logp,
                  float* out_path_logp, void* stream);
+/* Resumable hotwords (live streams): gam_ctc_bias over a stream whose frames arrive in consecutive calls.  Each call releases
+ * the output tokens no later frame can change and leaves the rest with the caller, who holds it for the next call.  Stateless:
+ * the caller keeps the held rows, greedy tokens and undecided detections between calls.
+ *
+ * Row b holds stream frames frame_base[b] + t, t < T_b = clamp(hi[b], 0, T): log_probs [B, T, V+1] rows, the greedy tokens
+ * (ids / frames / counts, frames in stream frames, strictly increasing, in [frame_base, frame_base + T_b); token_logp or NULL),
+ * and the known final detections not yet decided (det_* [B, K, max_det], stream frames, each keyword's in time order: those
+ * carried out of the call before, then those gam_ctc_spot_resume emitted since).  `state` is the spot records after this
+ * step's gam_ctc_spot_resume over the same frames with the same keywords and threshold.  left_boundary[b] != 0 when the held
+ * range starts on a word boundary: the stream starts there, or the last greedy token before it is a space (a greedy token,
+ * never a spliced one).  C = frame_base + T_b is the stream's decoded frame count.
+ * Three facts make an early decision exact:
+ *   1. Future candidates start at or after the horizon h.  Spot costs are <= 0 (c = lp - m exactly), so a path's score never
+ *      rises, and a path that ends as a candidate (E >= tau) had v >= tau at every frame it crossed.  Every detection not yet
+ *      emitted therefore starts at or after h = min(C, the pending detection's start, the start frame of every state with
+ *      v >= tau in every record); NaN scores fail v >= tau, as they fail E >= tau in spot.
+ *   2. gam_ctc_bias's selection (step 4) accepts a candidate only against the candidates it overlaps, so the components of
+ *      the overlap graph are decided independently.
+ *   3. Eligibility (step 3) reads only greedy tokens: a candidate's right boundary is known once a greedy token exists at a
+ *      frame >= its end, or once the stream has finished.
+ * So a component of the known detections is decided when every member ends at or before h and a greedy token exists at a
+ * frame >= its last end (with finish[b], every component is).  The release frame is R = min(h, the start of every undecided
+ * detection); with finish, R = C.  Every output token at a frame < R is final: splices stay inside their spans, left-edge
+ * spaces move to s and right-edge spaces to the keyword's last frame, before e.
+ * Outputs: out_ids / out_frames (stream frames) / out_source / out_token_logp [B, max_out] and out_counts [B], the released
+ *   tokens (frames < R) exactly as gam_ctc_bias writes them; released_until [B] = R (stream frame); carry_* [B, K, max_det] /
+ *   carry_count [B, K], the detections not decided, in their order, for the next call; frame_logp (f64 [b * frame_pitch + t],
+ *   the held frames' per-frame sums, or NULL) adjusted in place at the released spliced frames as gam_ctc_bias adjusts it
+ *   (fp64(lp) - fp64(m), added in the same order).  The caller keeps the greedy tokens and rows at frames >= R and the carried
+ *   detections.  Outputs must not alias the inputs.
+ * Equality: splitting a stream's frames into consecutive calls, the last one with finish, and concatenating the released
+ *   tokens gives gam_ctc_bias's ids, frames, sources, token_logp and frame_logp adjustments over the whole stream, bit for bit.
+ * Held span: [R, C) is bounded by the oldest live hotword path with v >= tau, not by the stream's length; a partial path can
+ *   survive a long silence, where blank costs 0.
+ * Precondition, as for gam_ctc_bias: the held greedy frames are strictly increasing and lie in [frame_base, frame_base + T_b).
+ *   They are device data, so the call cannot refuse other frames without a host synchronisation; a token outside the held
+ *   range is never used to write outside the workspace or the outputs, but the output is then unspecified.
+ * Refused (gam_last_error): what gam_ctc_bias refuses, plus a NULL hi, frame_base, finish, left_boundary, state,
+ *   released_until or carry_* pointer, and a record_bytes other than gam_ctc_spot_state_bytes(h, Umax).  The workspace is
+ *   gam_ctc_bias's (gam_ctc_bias_resume_workspace_bytes).  Three launches, fixed orders, no atomics, no host
+ *   synchronisation, capturable in a CUDA graph; a stream's outputs do not depend on its batch or the keyword order. */
+int64_t gam_ctc_bias_resume_workspace_bytes(const gam_handle* h, int32_t B, int32_t T, int32_t K, int32_t max_det);
+int gam_ctc_bias_resume(gam_handle* h, const float* log_probs, int32_t B, int32_t T, const int32_t* hi, const int32_t* frame_base,
+                        const int32_t* finish, const int32_t* keywords, const int32_t* keyword_len, int32_t K, int32_t Umax,
+                        const void* state, int64_t record_bytes, const int32_t* det_start, const int32_t* det_end,
+                        const float* det_score, const int32_t* det_count, int32_t max_det, float threshold,
+                        const uint8_t* token_flags, int32_t V, const int32_t* ids, const int32_t* frames, const int32_t* counts,
+                        const int32_t* left_boundary, int32_t max_out, const float* token_logp, double* frame_logp,
+                        int64_t frame_pitch, void* workspace, int64_t workspace_bytes, int32_t* out_ids, int32_t* out_frames,
+                        int32_t* out_counts, int32_t* out_source, float* out_token_logp, int32_t* released_until,
+                        int32_t* carry_start, int32_t* carry_end, float* carry_score, int32_t* carry_count, void* stream);
 /* RNN-T stage 1: enc [B, T, d_model], dec [B, U+1, pred_hidden] (gam_rnnt_predict over cat[blank, y]), targets [B, U] i32
  *   -> blank [B, T, U+1], label [B, T, U+1]: bit-identical to the matching entries of gam_rnnt_joint's lattice for the same
  *   enc / dec, but no [.., V+1] row is ever stored.  label is -inf at u = U and NaN where targets[b, u] is outside [0, V) (so
