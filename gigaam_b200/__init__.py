@@ -21,13 +21,14 @@ from .engine import check_attention_heads, max_encoded_frames_config
 from .model import GigaAM, GigaAMASR, GigaAMEmo, check_emo_head
 from .preprocess import load_audio, read_audio
 from .synthetic import synthetic_audio, synthetic_checkpoint
-from .streaming import StreamServer
-from .types import (Alignment, Detection, LongformAlignment, LongformTranscriptionResult, Segment, StreamResult, StreamUpdate,
-                    TranscriptionResult, Word)
+from .streaming import EmotionStreamServer, StreamServer
+from .types import (Alignment, Detection, EmotionSpan, EmotionStreamUpdate, EmotionTimeline, LongformAlignment,
+                    LongformTranscriptionResult, Segment, StreamResult, StreamUpdate, TranscriptionResult, Word)
 
 __all__ = ["GigaAM", "GigaAMASR", "GigaAMEmo", "load_audio", "read_audio", "load_model", "synthetic_checkpoint", "synthetic_audio",
            "TranscriptionResult", "Word", "Segment", "LongformTranscriptionResult", "Alignment",
-           "LongformAlignment", "Detection", "StreamServer", "StreamUpdate", "StreamResult"]
+           "LongformAlignment", "Detection", "StreamServer", "StreamUpdate", "StreamResult", "EmotionSpan", "EmotionTimeline",
+           "EmotionStreamServer", "EmotionStreamUpdate"]
 
 _CACHE_DIR = os.path.expanduser("~/.cache/gigaam")
 _MODEL_NAMES = ["emo", "v1_ctc", "v1_rnnt", "v1_ssl", "v2_ctc", "v2_rnnt", "v2_ssl", "v3_ctc", "v3_rnnt",

@@ -17,7 +17,7 @@ CSRC = PKG_DIR / "csrc"
 BUILD_DIR = PKG_DIR / "build"
 LIB_PATH = PKG_DIR / "libgigaam_b200.so"
 
-SOURCES = ["gam_api.cu", "gemm.cu", "attention_sm90.cu", "attention_relpos_sm90.cu", "rowops.cu", "frontend.cu", "ctc.cu", "words.cu", "comm.cu", "rnnt.cu", "rnnt_cluster.cu", "heads.cu", "pooled_head.cu", "head_grads.cu", "align.cu", "spot.cu", "bias.cu", "rnnt_loss.cu", "resample.cu"]
+SOURCES = ["gam_api.cu", "gemm.cu", "attention_sm90.cu", "attention_relpos_sm90.cu", "rowops.cu", "frontend.cu", "ctc.cu", "words.cu", "comm.cu", "rnnt.cu", "rnnt_cluster.cu", "heads.cu", "pooled_head.cu", "emo_time.cu", "head_grads.cu", "align.cu", "spot.cu", "bias.cu", "rnnt_loss.cu", "resample.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -154,7 +154,7 @@ struct gam_handle {
 enum ProfClass : int {
   PC_LOGMEL = 0, PC_SUB_CONV1, PC_GEMM_CONV2, PC_GEMM_SUBOUT, PC_GEMM_FFN_UP, PC_GEMM_FFN_DOWN, PC_GEMM_QKV, PC_GEMM_PROJ,
   PC_GEMM_GLU, PC_LAYERNORM, PC_ATTENTION, PC_DWCONV, PC_CTC_ARGMAX, PC_CTC_COLLAPSE, PC_RNNT_ENCPROJ, PC_RNNT_GREEDY,
-  PC_MISC, PC_CTC_LOG_PROBS, PC_RNNT_JOINT, PC_RNNT_PREDICT, PC_EMO_HEAD, PC_HEAD_BACKWARD, PC_ALIGN, PC_COUNT
+  PC_MISC, PC_CTC_LOG_PROBS, PC_RNNT_JOINT, PC_RNNT_PREDICT, PC_EMO_HEAD, PC_HEAD_BACKWARD, PC_ALIGN, PC_EMO_FRAME_LOGITS, PC_EMO_SPANS, PC_COUNT
 };
 
 struct ProfScope {
@@ -1738,6 +1738,34 @@ int gam_emo_head(gam_handle* h, const float* enc, const int32_t* enc_len, int32_
   return 0;
 }
 
+int gam_emo_frame_logits(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi, const int32_t* dst,
+                         float* frame_logits, int32_t n_frames, void* stream) {
+  if (!h) return -1;
+  if (h->cfg.head != 3) return fail(h, -1, "emo_frame_logits: model has no emo head");
+  if (B < 1 || B > 65535) return fail(h, -1, "emo_frame_logits: B=%d outside [1, 65535]", B);
+  if (T < 1 || n_frames < 1) return fail(h, -1, "emo_frame_logits: bad sizes (T=%d, n_frames=%d; both must be >= 1)", T, n_frames);
+  if (!enc || !lo || !hi || !dst || !frame_logits) return fail(h, -1, "emo_frame_logits: NULL pointer");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  { PROF(PC_EMO_FRAME_LOGITS);
+    launch_emo_frame_logits(enc, B, T, lo, hi, dst, h->w.emo_w, h->w.emo_b, h->cfg.num_classes, frame_logits, n_frames, s); }
+  GAM_CHECK_LAUNCH(h, "emo_frame_logits");
+  return 0;
+}
+
+int gam_emo_spans(gam_handle* h, const float* frame_logits, int32_t n_frames, const int32_t* span_start, const int32_t* span_end,
+                  int32_t S, float* logits, float* probs, void* stream) {
+  if (!h) return -1;
+  if (h->cfg.head != 3) return fail(h, -1, "emo_spans: model has no emo head");
+  if (n_frames < 1 || S < 1) return fail(h, -1, "emo_spans: bad sizes (n_frames=%d, S=%d; both must be >= 1)", n_frames, S);
+  if (!frame_logits || !span_start || !span_end) return fail(h, -1, "emo_spans: NULL pointer");
+  if (!logits && !probs) return 0;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  { PROF(PC_EMO_SPANS);
+    launch_emo_spans(frame_logits, n_frames, h->cfg.num_classes, span_start, span_end, S, logits, probs, s); }
+  GAM_CHECK_LAUNCH(h, "emo_spans");
+  return 0;
+}
+
 int gam_group_words(gam_handle* h, const int32_t* ids, const int32_t* frames, const int32_t* counts, int32_t B, int32_t max_out,
                     const uint8_t* token_flags, int32_t V, int32_t max_words, int32_t* word_start, int32_t* word_end,
                     int32_t* word_first_token, int32_t* word_tokens, int32_t* n_words, void* stream) {
@@ -1829,7 +1857,8 @@ const char* gam_profile_class_name(int32_t cls) {
   static const char* names[PC_COUNT] = {"logmel", "subsample_conv1", "gemm_conv2_implicit", "gemm_subsample_out", "gemm_ffn_up_silu",
                                         "gemm_ffn_down_res", "gemm_qkv", "gemm_proj_res", "gemm_pw1_glu", "layernorm", "attention",
                                         "dwconv_bn_silu", "ctc_head_argmax", "ctc_collapse", "rnnt_enc_proj", "rnnt_greedy", "misc",
-                                        "ctc_log_probs", "rnnt_joint", "rnnt_predict", "emo_head", "head_backward", "align"};
+                                        "ctc_log_probs", "rnnt_joint", "rnnt_predict", "emo_head", "head_backward", "align", "emo_frame_logits",
+                                        "emo_spans"};
   return (cls >= 0 && cls < PC_COUNT) ? names[cls] : "?";
 }
 

@@ -132,6 +132,16 @@ void launch_pool_chunks(const float* enc, const int* enc_len, int B, int T, floa
 void launch_pooled_head(const float* part, const int* enc_len, int B, int T, const float* W, const float* bias, int C, float* pooled,
                         float* logits, float* probs, cudaStream_t s);
 
+// emo_time.cu: GigaAMEmo over time.  emo_frame_logits: for each row b of enc f32 [B, T, 768], local frames t in
+// [lo', hi') = [clamp(lo[b], 0, T), clamp(hi[b], 0, T)) -> frame_logits row dst[b] + t - lo' ([n_frames, C]; rows outside [0, n_frames)
+// are dropped) = W enc[b, t] + bias in pooled_head_kernel's order.  emo_spans: spans [a_i, b_i) of frame_logits, clamped to
+// [0, n_frames] -> logits [S, C] (the mean) and probs [S, C] (its softmax), either may be null.  lo / hi / dst / spans are
+// device i32.  1 <= C <= kPoolMaxClasses, 1 <= B <= 65535, 1 <= S.
+void launch_emo_frame_logits(const float* enc, int B, int T, const int* lo, const int* hi, const int* dst, const float* W,
+                             const float* bias, int C, float* frame_logits, int n_frames, cudaStream_t s);
+void launch_emo_spans(const float* frame_logits, int n_frames, int C, const int* span_start, const int* span_end, int S, float* logits,
+                      float* probs, cudaStream_t s);
+
 // heads.cu: the heads' forward passes (fp32).  ctc: enc [R, D] -> log_probs [R, V1]
 void launch_ctc_log_probs(const float* enc, const float* W, const float* bias, float* out, int R, int D, int V1, cudaStream_t s);
 // E [B*T, J], P [B*U, J] -> out [B, T, U, V1] = log_softmax(Wo relu(E[b,t] + P[b,u]) + bo); 64-bit offsets.

@@ -1105,6 +1105,30 @@ class Engine:
         self._call("gam_emo_head", enc_btd, enc_len, B, T, ws, ws.numel(), pooled, logits, probs)
         return pooled, logits, probs
 
+    def emo_frame_logits(self, enc_btd: Tensor, lo: Tensor, hi: Tensor, dst: Tensor, frame_logits: Tensor) -> Tensor:
+        """gam_emo_frame_logits: enc [B, T, d] f32 contiguous; lo / hi / dst device i32 [B] -> row b's local frames [lo, hi)
+        get their logits W f + b written to rows dst[b] + t - lo[b] of frame_logits (f32 [n_frames, C] on the device, filled in
+        place and returned).  Rows outside [0, n_frames) are dropped."""
+        assert enc_btd.is_cuda and enc_btd.dtype == torch.float32 and enc_btd.is_contiguous() and enc_btd.dim() == 3
+        assert frame_logits.dtype == torch.float32 and frame_logits.is_contiguous() and frame_logits.shape[-1] == self.num_classes
+        if self.head_type != 3:
+            raise RuntimeError("model has no emo head")
+        B, T, _ = enc_btd.shape
+        self._call("gam_emo_frame_logits", enc_btd, B, T, lo, hi, dst, frame_logits, frame_logits.shape[0])
+        return frame_logits
+
+    def emo_spans(self, frame_logits: Tensor, start: Tensor, end: Tensor, logits: bool = True) -> Tuple[Optional[Tensor], Tensor]:
+        """gam_emo_spans: frame_logits f32 [n_frames, C]; start / end device i32 [S] -> (logits [S, C], the mean of the frame
+        logits over each span [start, end), or None without `logits`; probs [S, C], its softmax).  An empty span gives NaN."""
+        assert frame_logits.dtype == torch.float32 and frame_logits.is_contiguous() and frame_logits.shape[-1] == self.num_classes
+        if self.head_type != 3:
+            raise RuntimeError("model has no emo head")
+        S = start.numel()
+        out_l = self._empty(S, self.num_classes) if logits else None
+        probs = self._empty(S, self.num_classes)
+        self._call("gam_emo_spans", frame_logits, frame_logits.shape[0], start, end, S, out_l, probs)
+        return out_l, probs
+
     def group_words(self, ids: Tensor, frames: Tensor, counts: Tensor, token_flags: Tensor):
         """Device word grouping (gam_group_words): -> (word_start, word_end, word_first, word_ntok [B, max_out] i32, n_words [B] i32)."""
         B, max_out = ids.shape

@@ -217,6 +217,81 @@ def stitch_ctc_log_probs(model, wav: Tensor, windows: Sequence[Window], T: int, 
     return out
 
 
+def stitch_emo_frame_logits(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16) -> Tensor:
+    """Emotion frame logits [T, C] f32 on the device of a whole recording (wav as for `stitch_ctc_log_probs`): the windows are
+    encoded by `window_batches`, and one gam_emo_frame_logits launch per batch writes each window's kept frames straight into
+    place.  Only one batch of encoder output is alive at a time, and no [B, T_w, C] intermediate is built."""
+    from .decoding import _as_btd
+    eng = model._get_engine()
+    out = torch.empty((T, eng.num_classes), dtype=torch.float32, device=eng.device)
+    for group, encoded in window_batches(model, wav, windows, batch_size):
+        rng = torch.tensor([[w.keep_start - w.start // FRAME_SAMPLES for w in group], [w.keep_end - w.start // FRAME_SAMPLES for w in group],
+                            [w.keep_start for w in group]], dtype=torch.int32).to(eng.device)
+        eng.emo_frame_logits(_as_btd(encoded), rng[0], rng[1], rng[2], out)
+        del encoded
+    return out
+
+
+def emotion_spans(T: int, span: int, hop: int) -> List[Tuple[int, int]]:
+    """The planned spans [a, b) of an emotion timeline over T frames, spans of `span` frames every `hop` frames: one span
+    [0, T) when T <= span; else [k hop, k hop + span) for every k >= 0 with k hop + span <= T, and a tail span [T - span, T)
+    when the last of those does not end at T.  With hop <= span the spans cover [0, T); with hop > span they leave gaps of
+    hop - span frames between them (the tail span may still overlap the last one)."""
+    if span < 1 or hop < 1:
+        raise ValueError(f"span={span} and hop={hop} frames must be >= 1")
+    if T <= span:
+        return [(0, T)]
+    out = [(k * hop, k * hop + span) for k in range((T - span) // hop + 1)]
+    if out[-1][1] != T:
+        out.append((T - span, T))
+    return out
+
+
+def emotion_plan_frames(span: float, hop: float) -> Tuple[int, int]:
+    """(span, hop) seconds -> frames; ValueError for a value that is not a positive multiple of 40 ms."""
+    out = []
+    for name, value in (("span", span), ("hop", hop)):
+        if not (isinstance(value, (int, float)) and math.isfinite(value)):
+            raise ValueError(f"{name}={value!r} s must be a finite number of seconds")
+        frames = _frame_multiple(value, name) // FRAME_SAMPLES
+        if frames < 1:
+            raise ValueError(f"{name}={value} s must be positive")
+        out.append(frames)
+    return out[0], out[1]
+
+
+def check_caller_spans(spans: Sequence[Tuple[float, float]]) -> List[Tuple[float, float]]:
+    """Caller spans (start, end) in seconds, checked: ValueError for no spans, a NaN or negative boundary, or end < start.
+    end = start is an empty span, whose row is NaN."""
+    out = [(float(a), float(b)) for a, b in spans]
+    if not out:
+        raise ValueError("spans: no spans")
+    for a, b in out:
+        if math.isnan(a) or math.isnan(b) or a < 0 or b < 0:
+            raise ValueError(f"spans: ({a}, {b}) has a NaN or negative boundary")
+        if b < a:
+            raise ValueError(f"spans: ({a}, {b}) ends before it starts")
+    return out
+
+
+def caller_span_frames(spans: Sequence[Tuple[float, float]], T: int) -> List[Tuple[int, int]]:
+    """Checked caller spans in seconds -> frames [round(start / 0.04), round(end / 0.04)), each clamped to [0, T]."""
+    step = FRAME_SAMPLES / SAMPLE_RATE
+
+    def frame(s: float) -> int:
+        return T if s >= T * step else min(max(round(s / step), 0), T)
+    return [(frame(a), frame(b)) for a, b in spans]
+
+
+def emotion_result(names: Sequence[str], plan: Sequence[Tuple[int, int]], probs: Tensor, frame_logits: Tensor, frame_shift: float):
+    """An EmotionTimeline from host tensors: spans [a, b) in frames, their probs [S, C] and the frame logits [T, C]; times are
+    the frames times `frame_shift`."""
+    from .types import EmotionSpan, EmotionTimeline
+    rows = probs.tolist()
+    spans = [EmotionSpan(start=a * frame_shift, end=b * frame_shift, probs=dict(zip(names, row))) for (a, b), row in zip(plan, rows)]
+    return EmotionTimeline(names=list(names), spans=spans, probs=probs, frame_logits=frame_logits)
+
+
 def decode_windows(model, wav: Tensor, windows: Sequence[Window], T: int, batch_size: int = 16, scores: bool = False,
                    log_probs: Optional[Tensor] = None, boost: Optional[Tuple[Tensor, Tensor]] = None):
     """Greedy-decode a whole recording of T encoder frames as one utterance: `window_batches` encodes the windows, and each

@@ -17,7 +17,7 @@ from .decoding import CTCGreedyDecoding, RNNTGreedyDecoding, _as_btd
 from .encoder import ConformerEncoder
 from .engine import Engine
 from .preprocess import SAMPLE_RATE, FeatureExtractor, read_audio, resample_ratio, resampled_length
-from .types import Alignment, Detection, LongformAlignment, TranscriptionResult, Word
+from .types import Alignment, Detection, EmotionTimeline, LongformAlignment, TranscriptionResult, Word
 
 LONGFORM_THRESHOLD = 25 * SAMPLE_RATE
 ALIGN_MAX_TOKENS = 4096   # kAlignMaxTokens of csrc/kernels.h
@@ -253,6 +253,36 @@ class GigaAM(nn.Module):
         wav, length = self.prepare_wav(wav_file, sample_rate)
         return self.forward(wav, length)
 
+    # ---- the windowed entry points' recording intake
+    @property
+    def _max_frames(self) -> int:
+        """The most encoder frames one window may have: the model's max_encoded_frames, else the position table's length."""
+        return self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
+
+    def _encoded_length(self, n_samples: int) -> int:
+        """Encoder frames of a recording of n_samples samples (the front end's and the subsampling's length rules), on the
+        host."""
+        mel = self.preprocessor.out_len(torch.tensor([int(n_samples)]))
+        return int(self.encoder.pre_encode.calc_output_length(mel)[0])
+
+    def _intake(self, wav_file, sample_rate: int, window: float, overlap: float, batch_size: int
+                ) -> Tuple[Tensor, int, list, int]:
+        """One recording for the windowed entry points -> (its 16 kHz samples in the model's dtype in pinned host memory,
+        uploaded one batch of windows at a time; N samples; `longform.plan_windows`' windows over them; T encoder frames).
+        The file is read or the waveform taken, the rate checked, the windows planned on the resampled length and batch_size
+        checked before any device work: ValueError for each refusal.  Then the recording is resampled in bounded spans
+        (`_resample_host`) and rounded to the model's dtype, as prepare_wav rounds it; it is pinned when the model is on a GPU."""
+        from .longform import plan_windows
+        wav, sr = self._native(wav_file, sample_rate)
+        N = wav.numel() if sr == SAMPLE_RATE else resampled_length(wav.numel(), sr)
+        windows, T = plan_windows(N, window, overlap, self._encoded_length, self._max_frames)
+        if batch_size < 1:
+            raise ValueError("batch_size must be >= 1")
+        if sr != SAMPLE_RATE:
+            wav = self._resample_host(wav, sr)
+        host = wav.to(self._dtype)
+        return (host.pin_memory() if self._device.type == "cuda" else host), N, windows, T   # a CPU model uploads nothing
+
 
 class GigaAMASR(GigaAM):
     """Giga Acoustic Model for Speech Recognition -- drop-in for gigaam.model.GigaAMASR."""
@@ -270,11 +300,6 @@ class GigaAMASR(GigaAM):
         """Raise NotImplementedError(message) unless the model has the head a call needs: RNN-T if `rnnt`, else CTC."""
         if self._rnnt != rnnt:
             raise NotImplementedError(message)
-
-    @property
-    def _max_frames(self) -> int:
-        """The most encoder frames one window may have: the model's max_encoded_frames, else the position table's length."""
-        return self.__dict__.get("_max_encoded_frames") or _lib.REL_POS_MAX_T
 
     def _decode(self, encoded: Tensor, encoded_len: Tensor, wav_lens: Tensor, word_timestamps: bool = False,
                 confidence: bool = False) -> List[Tuple[str, Optional[List[Word]], Optional[float]]]:
@@ -437,30 +462,6 @@ class GigaAMASR(GigaAM):
         rows = path_rows.cpu().tolist()
         return [Alignment(text=norm[b], words=words[b], log_likelihood=ll[b], confidence=path_confidence(vit[b], rows[b]))
                 for b in range(B)]
-
-    def _encoded_length(self, n_samples: int) -> int:
-        """Encoder frames of a recording of n_samples samples (the front end's and the subsampling's length rules), on the
-        host."""
-        mel = self.preprocessor.out_len(torch.tensor([int(n_samples)]))
-        return int(self.encoder.pre_encode.calc_output_length(mel)[0])
-
-    def _intake(self, wav_file, sample_rate: int, window: float, overlap: float, batch_size: int
-                ) -> Tuple[Tensor, int, list, int]:
-        """One recording for the windowed entry points -> (its 16 kHz samples in the model's dtype in pinned host memory,
-        uploaded one batch of windows at a time; N samples; `longform.plan_windows`' windows over them; T encoder frames).
-        The file is read or the waveform taken, the rate checked, the windows planned on the resampled length and batch_size
-        checked before any device work: ValueError for each refusal.  Then the recording is resampled in bounded spans
-        (`_resample_host`) and rounded to the model's dtype, as prepare_wav rounds it; it is pinned when the model is on a GPU."""
-        from .longform import plan_windows
-        wav, sr = self._native(wav_file, sample_rate)
-        N = wav.numel() if sr == SAMPLE_RATE else resampled_length(wav.numel(), sr)
-        windows, T = plan_windows(N, window, overlap, self._encoded_length, self._max_frames)
-        if batch_size < 1:
-            raise ValueError("batch_size must be >= 1")
-        if sr != SAMPLE_RATE:
-            wav = self._resample_host(wav, sr)
-        host = wav.to(self._dtype)
-        return (host.pin_memory() if self._device.type == "cuda" else host), N, windows, T   # a CPU model uploads nothing
 
     def _text_ids(self, text: Union[str, Sequence[int]], what: str) -> Tuple[str, List[int]]:
         """(normalised text, token ids) of a string (`Tokenizer.encode`) or of a sequence of token ids, taken as it is:
@@ -851,3 +852,42 @@ class GigaAMEmo(GigaAM):
         encoded_len frames (all T' for a batch of one; see the class docstring)."""
         encoded, encoded_len = self.encoder(features, feature_lengths)
         return self._pooled_probs(encoded, encoded_len)
+
+    @torch.inference_mode()
+    def emotion_timeline(self, wav_file, window: float = 30.0, overlap: float = 4.0, span: float = 4.0, hop: float = 1.0,
+                         spans: Optional[Sequence[Tuple[float, float]]] = None, batch_size: int = 16,
+                         sample_rate: int = SAMPLE_RATE) -> EmotionTimeline:
+        """Emotions over a recording of any length (INTEGRATION.md, "Emotions over time").  The encoder runs over the
+        overlapping windows of `transcribe_windowed` (`longform.plan_windows`), the head's logits of every kept frame are
+        stitched into one [T, C] sequence (gam_emo_frame_logits), and every span's probabilities are the softmax of its mean
+        frame logits (gam_emo_spans, one call).  Spans are `span` seconds long every `hop` seconds (`longform.emotion_spans`:
+        one span [0, T) when the recording is shorter, a tail span that ends at T; gaps between spans when hop > span), or the
+        caller's `spans` [(start, end), ...] in seconds, each boundary rounded to a 40 ms frame and clamped to the recording.
+        Times use the recording's frame shift, as `transcribe_windowed` does.  Raises ValueError before any device work for a
+        span or hop that is not a positive multiple of 0.04 s, caller spans that are NaN, negative or inverted, batch_size < 1,
+        the window plan's refusals and a `sample_rate` that cannot be resampled."""
+        from .longform import caller_span_frames, check_caller_spans, emotion_plan_frames, emotion_spans, stitch_emo_frame_logits
+        span_f, hop_f = emotion_plan_frames(span, hop)
+        caller = None if spans is None else check_caller_spans(spans)
+        host, N, windows, T = self._intake(wav_file, sample_rate, window, overlap, batch_size)
+        fl = stitch_emo_frame_logits(self, host, windows, T, batch_size)
+        plan = emotion_spans(T, span_f, hop_f) if caller is None else caller_span_frames(caller, T)
+        return self._timeline(fl, plan, N, T)
+
+    def _timeline(self, frame_logits: Tensor, plan: Sequence[Tuple[int, int]], N: int, T: int) -> EmotionTimeline:
+        """One gam_emo_spans call over the device frame logits [T, C] for the spans `plan` -> the EmotionTimeline."""
+        from .longform import emotion_result
+        from .timestamps_utils import compute_frame_shift
+        eng = self._get_engine()
+        se = torch.tensor(plan, dtype=torch.int32).reshape(-1, 2).t().contiguous().to(eng.device)
+        _, probs = eng.emo_spans(frame_logits, se[0], se[1], logits=False)
+        return emotion_result(self.id2name, plan, probs.cpu(), frame_logits.cpu(), compute_frame_shift(N, T))
+
+    def streaming(self, window: float = 8.0, overlap: float = 4.0, span: float = 4.0, hop: float = 1.0, batch_size: int = 64,
+                  sample_rate: int = SAMPLE_RATE):
+        """A `streaming.EmotionStreamServer` for live audio (INTEGRATION.md, "Emotions over time"): open streams, push chunks,
+        `step()` for the spans that became final, `close()` for each stream's `emotion_timeline` with the same window, overlap,
+        span and hop, bit for bit.  Raises ValueError before any device work for the window plan's refusals, batch_size < 1,
+        a span or hop that is not a positive multiple of 0.04 s and a `sample_rate` that cannot be resampled."""
+        from .streaming import EmotionStreamServer
+        return EmotionStreamServer(self, window, overlap, span, hop, batch_size, sample_rate)

@@ -25,7 +25,11 @@ finish, so a closed stream equals `transcribe_windowed(..., hotwords=...)`.
 Device memory does not grow with a stream's duration: a stream owns one decoder record, one spot record per keyword and
 per hotword, and with hotwords the held rows [R, C), bounded by the oldest live hotword path; every step's outputs are
 step-local.  The host keeps each stream's unencoded samples, its token ids, frames, token
-log-probs, per-frame sums and detections for `close`.  One caller drives a server; it is not thread-safe."""
+log-probs, per-frame sums and detections for `close`.  One caller drives a server; it is not thread-safe.
+
+`EmotionStreamServer` (GigaAM-Emo) shares the windows, the sample buffers (`_Audio`) and the resampling stage
+(`resample_streams`): each step writes the emotion head's logits of the ready windows' kept frames next to each stream's
+held frames and scores the planned spans that became final; `close()` returns `emotion_timeline`'s result bit for bit."""
 from __future__ import annotations
 
 import math
@@ -40,7 +44,7 @@ from .longform import (FRAME_SAMPLES, Window, _frame_multiple, check_segmenting,
                        windowed_result)
 from .preprocess import SAMPLE_RATE, resample_ratio, resampled_length
 from .timestamps_utils import compute_frame_shift, token_flag_table
-from .types import Detection, StreamResult, StreamUpdate
+from .types import Detection, EmotionSpan, EmotionStreamUpdate, EmotionTimeline, StreamResult, StreamUpdate
 
 FRAME_SECONDS = FRAME_SAMPLES / SAMPLE_RATE   # the nominal 40 ms frame step of updates
 
@@ -91,40 +95,33 @@ class TextFeed:
         return new
 
 
-class _Stream:
-    """Host side of one open stream."""
+class _Audio:
+    """The samples of one open stream: its 16 kHz samples that a window not yet encoded may need and, for a server at another
+    rate, the raw samples that pending 16 kHz outputs can need."""
 
-    def __init__(self, sid: int, slot: int, feed: TextFeed, K: int, dtype: torch.dtype):
-        self.id, self.slot, self.feed = sid, slot, feed
+    def __init__(self, dtype: torch.dtype):
         self.n = 0                       # samples pushed
         self.chunks: List[Tensor] = []   # pushed since the last consolidation
         self.buf = torch.zeros(0, dtype=dtype)   # samples [buf_start, n) that a window not yet encoded may need
         self.buf_start = 0
         self.windows: List[Window] = []  # the windows handed to the encoder, in order
-        self.committed = 0               # frames decoded for good
-        self.ids: List[int] = []
-        self.frames: List[int] = []
-        self.token_logp: List[float] = []
-        self.frame_logp: List[np.ndarray] = []
-        self.frame_rows: List[np.ndarray] = []
-        self.dets: List[List[Tuple[int, int, float]]] = [[] for _ in range(K)]
-        self.pending: List[Optional[Tuple[int, int, float]]] = [None] * K
-        self.tentative: List[int] = []
         # resampling streams: raw samples [raw_start, raw_n) that pending 16 kHz outputs can need, and the outputs made so far
         self.raw = torch.zeros(0, dtype=torch.float32)
         self.raw_chunks: List[Tensor] = []
         self.raw_start = self.raw_n = self.out_n = 0
-        # hotwords: the span [hw_base, C) not yet released -- its rows and its undecided hotword detections on the device
-        # (hw_det: start, end and score bits as i32 [D, 3, K], and the count per hotword [K]), its greedy tokens and
-        # per-frame sums on the host; hw_left: the span starts on a word boundary
-        self.hw_rows: Optional[Tensor] = None
-        self.hw_det: Optional[Tuple[Tensor, Tensor]] = None
-        self.hw_base = 0
-        self.hw_left = True
-        self.hw_ids = np.zeros(0, np.int32)
-        self.hw_frames = np.zeros(0, np.int32)
-        self.hw_logp = np.zeros(0, np.float32)
-        self.hw_flp = np.zeros(0, np.float64)
+
+    def append(self, chunk, resampling: bool, dtype: torch.dtype) -> None:
+        """Append pushed samples: kept as float32 raw samples when `resampling`, else rounded to `dtype` as `prepare_wav` does."""
+        x = torch.as_tensor(chunk, dtype=torch.float32).detach().reshape(-1).cpu()
+        if resampling:
+            if x.numel():
+                self.raw_chunks.append(x)
+                self.raw_n += x.numel()
+            return
+        x = x.to(dtype)
+        if x.numel():
+            self.chunks.append(x)
+            self.n += x.numel()
 
     def samples(self, start: int, end: int) -> Tensor:
         if self.chunks:
@@ -139,6 +136,67 @@ class _Stream:
         if cut > 0:
             self.buf = self.buf[cut:].clone()
             self.buf_start = keep_from
+
+
+def resample_streams(eng, sample_rate: int, ratio: Tuple[int, int, int], dtype: torch.dtype, streams: Sequence[_Audio],
+                     final: bool) -> None:
+    """Resample, in one launch, each stream's 16 kHz outputs that are final (all of them when `final`: the end of the
+    recording is known), append them to its 16 kHz samples (rounded to `dtype`) and drop the raw samples no pending output
+    needs.  `ratio` = (o, n, w) of preprocess.resample_ratio(sample_rate)."""
+    o, n, w = ratio
+    rows = []
+    for s in streams:
+        target = resampled_length(s.raw_n, sample_rate) if final else resample_ready(s.raw_n, o, n, w)
+        if target > s.out_n:
+            if s.raw_chunks:
+                s.raw = torch.cat([s.raw] + s.raw_chunks)
+                s.raw_chunks = []
+            rows.append((s, target))
+    if not rows:
+        return
+    x = torch.zeros((len(rows), max(1, max(s.raw.numel() for s, _ in rows))), dtype=torch.float32)
+    for r, (s, _) in enumerate(rows):
+        x[r, :s.raw.numel()] = s.raw
+    spans = torch.tensor([[s.raw_start for s, _ in rows], [s.raw_n for s, _ in rows], [s.out_n for s, _ in rows],
+                          [t for _, t in rows]], dtype=torch.int64)
+    y = torch.empty((len(rows), max(t - s.out_n for s, t in rows)), dtype=torch.float32, device=eng.device)
+    y = eng.resample_spans(x.to(eng.device), spans, sample_rate, y).cpu()
+    for r, (s, target) in enumerate(rows):
+        cnt = target - s.out_n
+        s.chunks.append(y[r, :cnt].to(dtype))
+        s.n += cnt
+        s.out_n = target
+        keep = min(max(s.raw_start, target // n * o - w), s.raw_n)   # the first tap of the next pending output
+        s.raw = s.raw[keep - s.raw_start:].clone()
+        s.raw_start = keep
+
+
+class _Stream(_Audio):
+    """Host side of one open stream."""
+
+    def __init__(self, sid: int, slot: int, feed: TextFeed, K: int, dtype: torch.dtype):
+        super().__init__(dtype)
+        self.id, self.slot, self.feed = sid, slot, feed
+        self.committed = 0               # frames decoded for good
+        self.ids: List[int] = []
+        self.frames: List[int] = []
+        self.token_logp: List[float] = []
+        self.frame_logp: List[np.ndarray] = []
+        self.frame_rows: List[np.ndarray] = []
+        self.dets: List[List[Tuple[int, int, float]]] = [[] for _ in range(K)]
+        self.pending: List[Optional[Tuple[int, int, float]]] = [None] * K
+        self.tentative: List[int] = []
+        # hotwords: the span [hw_base, C) not yet released -- its rows and its undecided hotword detections on the device
+        # (hw_det: start, end and score bits as i32 [D, 3, K], and the count per hotword [K]), its greedy tokens and
+        # per-frame sums on the host; hw_left: the span starts on a word boundary
+        self.hw_rows: Optional[Tensor] = None
+        self.hw_det: Optional[Tuple[Tensor, Tensor]] = None
+        self.hw_base = 0
+        self.hw_left = True
+        self.hw_ids = np.zeros(0, np.int32)
+        self.hw_frames = np.zeros(0, np.int32)
+        self.hw_logp = np.zeros(0, np.float32)
+        self.hw_flp = np.zeros(0, np.float64)
 
 
 class StreamServer:
@@ -251,17 +309,7 @@ class StreamServer:
         """Append mono samples at the server's sample rate (any length) to a stream.  16 kHz samples are rounded to the model's
         dtype as `prepare_wav` does; samples at another rate are kept as float32 and rounded once resampled.  Host only:
         nothing runs on the device until `step` or `close`."""
-        s = self._get(stream, "push")
-        x = torch.as_tensor(chunk, dtype=torch.float32).detach().reshape(-1).cpu()
-        if self._ratio is not None:
-            if x.numel():
-                s.raw_chunks.append(x)
-                s.raw_n += x.numel()
-            return
-        x = x.to(self.model._dtype)
-        if x.numel():
-            s.chunks.append(x)
-            s.n += x.numel()
+        self._get(stream, "push").append(chunk, self._ratio is not None, self.model._dtype)
 
     # ---- steps
     @torch.inference_mode()
@@ -292,33 +340,7 @@ class StreamServer:
     def _resample(self, streams: List[_Stream], final: bool) -> None:
         """Resample, in one launch, each stream's 16 kHz outputs that are final (all of them when `final`: the end of the
         recording is known), append them to its 16 kHz samples and drop the raw samples no pending output needs."""
-        o, n, w = self._ratio
-        rows = []
-        for s in streams:
-            target = resampled_length(s.raw_n, self.sample_rate) if final else resample_ready(s.raw_n, o, n, w)
-            if target > s.out_n:
-                if s.raw_chunks:
-                    s.raw = torch.cat([s.raw] + s.raw_chunks)
-                    s.raw_chunks = []
-                rows.append((s, target))
-        if not rows:
-            return
-        eng = self._eng
-        x = torch.zeros((len(rows), max(1, max(s.raw.numel() for s, _ in rows))), dtype=torch.float32)
-        for r, (s, _) in enumerate(rows):
-            x[r, :s.raw.numel()] = s.raw
-        spans = torch.tensor([[s.raw_start for s, _ in rows], [s.raw_n for s, _ in rows], [s.out_n for s, _ in rows],
-                              [t for _, t in rows]], dtype=torch.int64)
-        y = torch.empty((len(rows), max(t - s.out_n for s, t in rows)), dtype=torch.float32, device=eng.device)
-        y = eng.resample_spans(x.to(eng.device), spans, self.sample_rate, y).cpu()
-        for r, (s, target) in enumerate(rows):
-            cnt = target - s.out_n
-            s.chunks.append(y[r, :cnt].to(self.model._dtype))
-            s.n += cnt
-            s.out_n = target
-            keep = min(max(s.raw_start, target // n * o - w), s.raw_n)   # the first tap of the next pending output
-            s.raw = s.raw[keep - s.raw_start:].clone()
-            s.raw_start = keep
+        resample_streams(self._eng, self.sample_rate, self._ratio, self.model._dtype, streams, final)
 
     def _detection(self, k: int, start: int, end: int, score: float) -> Detection:
         return Detection(keyword=self.names[k], keyword_index=k, start=start * FRAME_SECONDS, end=end * FRAME_SECONDS, score=score,
@@ -566,6 +588,175 @@ class StreamServer:
                                      np.concatenate(s.frame_rows) if self.confidence else None, N, T, word_timestamps, pause,
                                      max_segment)
         return StreamResult(transcript=transcript, detections=detections)
+
+    @property
+    def streams(self) -> List[int]:
+        """The ids of the open streams."""
+        return list(self._streams)
+
+
+class _EmoStream(_Audio):
+    """Host side of one open emotion stream."""
+
+    def __init__(self, sid: int, dtype: torch.dtype):
+        super().__init__(dtype)
+        self.id = sid
+        self.final = 0                   # frames whose logits are final
+        self.k = 0                       # the next planned span [k hop, k hop + span) to emit
+        self.dev_from = 0                # first frame a future span can read: the device holds frames [dev_from, final)
+        self.dev: Optional[Tensor] = None
+        self.logits: List[Tensor] = []   # host frame logits of frames [0, final), in pieces
+        self.spans: List[Tuple[int, int]] = []   # the spans emitted, in frames
+        self.probs: List[Tensor] = []    # their probabilities, in pieces
+
+
+class EmotionStreamServer:
+    """Emotions of live audio streams, with one encoder batch per step across all of them (INTEGRATION.md, "Emotions over
+    time").  Made by `GigaAMEmo.streaming(...)`:
+
+        srv = model.streaming(window=8.0, overlap=4.0, span=4.0, hop=1.0)
+        a = srv.open()
+        srv.push(a, chunk)              # host samples, any length
+        for u in srv.step():            # an EmotionStreamUpdate for every stream that got final frames
+            ...
+        timeline = srv.close(a)
+
+    Windows are `StreamServer`'s: window w is encoded once it is ready (`ready_count`, `ready_window`), and one
+    gam_emo_frame_logits launch per batch writes the kept frames' logits into each stream's frames.  A planned span
+    [k hop, k hop + span) is emitted once its last frame is final, by one gam_emo_spans call per step over every stream's new
+    spans; the tail span of `longform.emotion_spans` comes only at `close`, which returns `emotion_timeline(recording, window,
+    overlap, span, hop)` bit for bit.  The device holds, per stream, only the frames a future span can still read (from the
+    next planned span's start, or span frames before the final frames for a tail span), so device memory does not grow with a
+    stream's duration.  The host keeps each stream's frame logits (4 C bytes per 40 ms, returned by `close`) and the spans
+    already emitted.  One caller drives a server; it is not thread-safe."""
+
+    def __init__(self, model, window: float = 8.0, overlap: float = 4.0, span: float = 4.0, hop: float = 1.0, batch_size: int = 64,
+                 sample_rate: int = SAMPLE_RATE):
+        from .longform import emotion_plan_frames
+        self.sample_rate = sample_rate
+        self._ratio = None if sample_rate == SAMPLE_RATE else resample_ratio(sample_rate)
+        self.W = _frame_multiple(window, "window")
+        self.V = _frame_multiple(overlap, "overlap")
+        plan_windows(max(self.W, 1), window, overlap, model._encoded_length, model._max_frames)   # the window plan's refusals
+        if batch_size < 1:
+            raise ValueError("batch_size must be >= 1")
+        self.span, self.hop = emotion_plan_frames(span, hop)
+        self.model, self.window, self.overlap, self.batch_size = model, window, overlap, int(batch_size)
+        self.names: List[str] = list(model.id2name)
+        self._streams: Dict[int, _EmoStream] = {}
+        self._next_id = 0
+        self._eng = None
+
+    def open(self) -> int:
+        """A new stream; returns its id."""
+        sid = self._next_id
+        self._next_id += 1
+        self._streams[sid] = _EmoStream(sid, self.model._dtype)
+        return sid
+
+    def _get(self, stream: int, what: str) -> _EmoStream:
+        s = self._streams.get(stream)
+        if s is None:
+            raise ValueError(f"{what}: stream {stream!r} is not open")
+        return s
+
+    def push(self, stream: int, chunk) -> None:
+        """Append mono samples at the server's sample rate (any length) to a stream, as `StreamServer.push` does.  Host only."""
+        self._get(stream, "push").append(chunk, self._ratio is not None, self.model._dtype)
+
+    def _engine(self):
+        if self._eng is None:
+            self._eng = self.model._get_engine()
+        return self._eng
+
+    @torch.inference_mode()
+    def step(self) -> List[EmotionStreamUpdate]:
+        """Encode every ready window of every open stream and emit the planned spans that became final; returns an
+        EmotionStreamUpdate for every stream that has new windows, in the order the streams were opened."""
+        streams = list(self._streams.values())
+        if self._ratio is not None and streams:
+            resample_streams(self._engine(), self.sample_rate, self._ratio, self.model._dtype, streams, final=False)
+        news = {s: [ready_window(w, self.W, self.V) for w in range(len(s.windows), ready_count(s.n, self.W, self.V))] for s in streams}
+        news = {s: ws for s, ws in news.items() if ws}
+        if not news:
+            return []
+        jobs = [(s, ws[r]) for r in range(max(len(ws) for ws in news.values())) for s, ws in news.items() if r < len(ws)]
+        ends = {s: ws[-1].keep_end for s, ws in news.items()}
+        spans = {}
+        for s, end in ends.items():
+            last = (end - self.span) // self.hop if end >= self.span else -1    # the last k whose span ends by `end`
+            spans[s] = [(k * self.hop, k * self.hop + self.span) for k in range(s.k, last + 1)]
+            s.k = max(s.k, last + 1)
+        probs = self._run(jobs, ends, spans)
+        out = []
+        for s in news:
+            s.trim(len(s.windows) * (self.W - self.V))
+            new = [EmotionSpan(start=a * FRAME_SECONDS, end=b * FRAME_SECONDS, probs=dict(zip(self.names, row)))
+                   for (a, b), row in zip(spans[s], probs[s].tolist())]
+            out.append(EmotionStreamUpdate(stream=s.id, new_spans=new, final_until=s.final * FRAME_SECONDS))
+        return out
+
+    def _run(self, jobs: List[Tuple[_EmoStream, Window]], ends: Dict[_EmoStream, int],
+             spans: Dict[_EmoStream, List[Tuple[int, int]]]) -> Dict[_EmoStream, Tensor]:
+        """Encode the jobs' windows and write their kept frames' logits next to each stream's held frames in one step buffer
+        (one gam_emo_frame_logits launch per batch), score every stream's `spans` in one gam_emo_spans call, bring the new
+        frame logits and the probabilities to the host and keep on the device only the frames a future span can read.
+        `ends[s]` is stream s's final frame count after the jobs.  Returns each stream's probs [len(spans[s]), C] (host)."""
+        eng = self._engine()
+        base, total = {}, 0
+        for s, end in ends.items():
+            base[s] = total
+            total += end - s.dev_from
+        buf = torch.empty((max(total, 1), eng.num_classes), dtype=torch.float32, device=eng.device)
+        for s in ends:
+            if s.dev is not None and s.dev.shape[0]:
+                buf[base[s]:base[s] + s.dev.shape[0]] = s.dev
+        for s, w in jobs:
+            s.windows.append(w)
+        for group in window_groups(jobs, self.batch_size, lambda job: job[1]):
+            encoded = encode_rows(self.model, [s.samples(w.start, w.end) for s, w in group])
+            first = [w.start // FRAME_SAMPLES for _, w in group]
+            rng = torch.tensor([[w.keep_start - f for (_, w), f in zip(group, first)], [w.keep_end - f for (_, w), f in zip(group, first)],
+                                [base[s] + w.keep_start - s.dev_from for s, w in group]], dtype=torch.int32).to(eng.device)
+            eng.emo_frame_logits(_as_btd(encoded), rng[0], rng[1], rng[2], buf)
+            del encoded
+        plan = [(base[s] + a - s.dev_from, base[s] + b - s.dev_from) for s in ends for a, b in spans[s]]
+        assert all(a >= s.dev_from for s in ends for a, _ in spans[s]), "a span reads a frame the device no longer holds"
+        probs = torch.zeros((0, eng.num_classes), dtype=torch.float32)
+        if plan:
+            se = torch.tensor(plan, dtype=torch.int32).t().contiguous().to(eng.device)
+            probs = eng.emo_spans(buf, se[0], se[1], logits=False)[1].cpu()
+        host = buf.cpu()
+        out, row = {}, 0
+        for s, end in ends.items():
+            out[s] = probs[row:row + len(spans[s])]
+            row += len(spans[s])
+            s.probs.append(out[s])
+            s.spans.extend(spans[s])
+            s.logits.append(host[base[s] + s.final - s.dev_from:base[s] + end - s.dev_from].clone())
+            # a future span starts at the next planned span or, as the tail span, at or after end - span
+            keep = min(max(s.dev_from, min(s.k * self.hop, end - self.span)), end)
+            s.dev = buf[base[s] + keep - s.dev_from:base[s] + end - s.dev_from].clone()
+            s.dev_from, s.final = keep, end
+        return out
+
+    @torch.inference_mode()
+    def close(self, stream: int) -> EmotionTimeline:
+        """End a stream: encode its remaining windows, the last one included, and return its EmotionTimeline, which is
+        `emotion_timeline(recording, window, overlap, span, hop)`'s bit for bit.  Raises ValueError for a stream that is not
+        open and, after freeing the stream, for one whose samples encode to no frame."""
+        from .longform import emotion_result, emotion_spans
+        s = self._get(stream, "close")
+        del self._streams[stream]
+        if self._ratio is not None:
+            resample_streams(self._engine(), self.sample_rate, self._ratio, self.model._dtype, [s], final=True)
+        windows, T = plan_windows(s.n, self.window, self.overlap, self.model._encoded_length, self.model._max_frames)
+        N, done = s.n, len(s.windows)
+        assert windows[:done] == s.windows, "a ready window differs from the plan of the whole stream"
+        plan = emotion_spans(T, self.span, self.hop)
+        assert plan[:len(s.spans)] == s.spans, "an emitted span differs from the plan of the whole stream"
+        self._run([(s, w) for w in windows[done:]], {s: T}, {s: plan[len(s.spans):]})
+        return emotion_result(self.names, s.spans, torch.cat(s.probs), torch.cat(s.logits), compute_frame_shift(N, T))
 
     @property
     def streams(self) -> List[int]:

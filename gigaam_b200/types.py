@@ -6,6 +6,8 @@ from __future__ import annotations
 
 from typing import Any, Dict, Iterator, List, Optional, Tuple
 
+import torch
+
 
 class _Record:
     """Positional / keyword construction over `_fields`, value equality and a readable repr.  Fields in `_quiet` are
@@ -203,3 +205,48 @@ class StreamResult(_Record):
 
     def __str__(self) -> str:
         return str(self.transcript)
+
+
+class EmotionSpan(_Record):
+    """One span of an emotion timeline: `start` / `end` in seconds of the recording (end exclusive) and `probs`, {class name:
+    probability} of the softmax of the span's mean frame logits, which is the head applied to the mean of its frames."""
+    __slots__ = _fields = ("start", "end", "probs")
+    start: float
+    end: float
+    probs: Dict[str, float]
+
+
+class EmotionTimeline(_Record):
+    """`GigaAMEmo.emotion_timeline()` result (INTEGRATION.md, "Emotions over time"): the class `names`, one `EmotionSpan` per
+    span in order, `probs` (host f32 [S, C], the spans' probabilities in class order) and `frame_logits` (host f32 [T, C], the
+    head's logits of every 40 ms encoder frame, W f_t + b).  The softmax of the mean of frame_logits over any range of frames
+    is that range's emotion, so callers can pool spans of their own.  Two timelines are equal when their names and spans are,
+    and their tensors have the same bits."""
+    __slots__ = _fields = ("names", "spans", "probs", "frame_logits")
+    names: List[str]
+    spans: List[EmotionSpan]
+    probs: torch.Tensor
+    frame_logits: torch.Tensor
+
+    def __eq__(self, other: object) -> bool:
+        def bits(t: torch.Tensor) -> torch.Tensor:
+            return t.contiguous().view(torch.int32)
+        return (type(other) is type(self) and self.names == other.names and repr(self.spans) == repr(other.spans)
+                and all(a.shape == b.shape and torch.equal(bits(a), bits(b))
+                        for a, b in ((self.probs, other.probs), (self.frame_logits, other.frame_logits))))
+
+    def __len__(self) -> int:
+        return len(self.spans)
+
+    def __iter__(self) -> Iterator[EmotionSpan]:
+        return iter(self.spans)
+
+
+class EmotionStreamUpdate(_Record):
+    """What one `EmotionStreamServer.step()` added to a live stream: `new_spans`, the planned spans whose last frame became
+    final in this step (times at the nominal 0.04 s per frame), and `final_until`, the end of the final frames in seconds.
+    Concatenating a stream's `new_spans` gives its timeline's spans without the tail span, which only `close` adds."""
+    __slots__ = _fields = ("stream", "new_spans", "final_until")
+    stream: int
+    new_spans: List[EmotionSpan]
+    final_until: float

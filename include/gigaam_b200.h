@@ -14,6 +14,7 @@
  *   gam_rnnt_joint    <- gigaam/decoder.py:41-47      RNNTJoint.joint
  *   gam_rnnt_predict  <- gigaam/decoder.py:85-102     RNNTDecoder.predict (1-layer LSTM)
  *   gam_emo_head      <- gigaam/model.py:272-293      GigaAMEmo pooling + head + softmax
+ *   gam_emo_frame_logits / gam_emo_spans              the same head over spans of a recording of any length
  *
  * Conventions: every pointer marked "device" is a CUDA device pointer on the handle's device; the
  * library never allocates or frees caller memory in the hot calls (the caller passes a workspace of
@@ -697,6 +698,32 @@ int gam_rnnt_loss_backward(gam_handle* h, const float* enc, const float* dec, co
 int64_t gam_emo_workspace_bytes(const gam_handle* h, int32_t B, int32_t T);
 int gam_emo_head(gam_handle* h, const float* enc, const int32_t* enc_len, int32_t B, int32_t T, void* workspace,
                  int64_t workspace_bytes, float* pooled, float* logits, float* probs, void* stream);
+/* ---- Emotions over time.  The head is Linear(d_model, C) on the mean of the frames, so in real arithmetic
+ * softmax(W mean_t f_t + b) = softmax(mean_t l_t) with l_t = W f_t + b: any span's emotion follows from the per-frame logits.
+ *
+ * gam_emo_frame_logits: enc device f32 [B, T, d_model] (gam_encode's layout); lo, hi, dst device i32 [B]; frame_logits device
+ *   f32 [n_frames, C].  Row b's local frames t in [lo'[b], hi'[b]), lo' and hi' being lo[b] and hi[b] clamped to [0, T], get
+ *   their logits written to row dst[b] + t - lo'[b] of frame_logits; a row outside [0, n_frames) is dropped and every other row
+ *   is left as it was.  Frames outside [lo', hi') are never read.  The dot product is gam_emo_head's: per class, lane l of a
+ *   warp sums k = 4 l + 128 i (i ascending) with fp32 FMAs from +0, then the xor tree 16, 8, 4, 2, 1, then + bias.  So a
+ *   frame's logits have the same bits whichever batch row, window or launch produced them, and a recording's windows are
+ *   stitched by one launch per batch of windows, straight into the recording's [T, C] buffer.
+ * gam_emo_spans: frame_logits device f32 [n_frames, C]; span_start, span_end device i32 [S], each span [a, b) clamped to
+ *   [0, n_frames] (b < a is empty) -> logits [S, C] = the mean of l over the span's n frames, probs [S, C] = its softmax; either
+ *   output may be NULL (not written).  The mean sums each run of 32 frames in ascending t from its first frame, adds the run
+ *   sums from +0 in ascending order and divides by n (gam_emo_head's order); the softmax is gam_emo_head's.  The order depends
+ *   only on the span's length, so a span's outputs have the same bits at any position in the list, next to any other spans.
+ *   An empty span gives a NaN row, the mean of an empty set.  A NaN frame logit makes that class's mean NaN in every span
+ *   containing it, and with it the span's whole probs row.
+ * lo, hi, dst and the spans are device data: their ranges are a precondition, not a refusal; values outside them never cause a
+ * read outside enc / frame_logits or a write outside frame_logits / logits / probs.
+ * Refused (gam_last_error): a handle without an emo head, B outside [1, 65535], T < 1 or n_frames < 1, S < 1, and a NULL enc,
+ * lo, hi, dst, frame_logits, span_start or span_end.  One launch each, fixed orders, no atomics, no workspace, no host
+ * synchronisation: capturable in a CUDA graph. */
+int gam_emo_frame_logits(gam_handle* h, const float* enc, int32_t B, int32_t T, const int32_t* lo, const int32_t* hi, const int32_t* dst,
+                         float* frame_logits, int32_t n_frames, void* stream);
+int gam_emo_spans(gam_handle* h, const float* frame_logits, int32_t n_frames, const int32_t* span_start, const int32_t* span_end,
+                  int32_t S, float* logits, float* probs, void* stream);
 
 /* Resampling to 16 kHz  <- the reference resamples with ffmpeg (-ar 16000, gigaam/preprocess.py:12-40); this is torchaudio's
  * default resample(x, orig, 16000) (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99), restated:
